@@ -1261,25 +1261,35 @@ __global__ void __launch_bounds__(256, 4) k_refine_filter(FilterParams p) {
 
 
 // k_refine_filter_w: the same test with ONE WARP per candidate (the default; LINEMOD_B200_FILTER_VARIANT=1 selects the
-// kernel above).  The four 8-lane groups of the warp work on the SAME 16x16 patch and deal the features between them: of
-// every 32 consecutive features group q adds features 8q .. 8q+7 into its own partial counter, so a candidate is a chain
-// of nf / 32 steps instead of nf / 8 (a chain four times shorter: what matters when the candidates are fewer than the
-// machine has lanes, e.g. a 1/8 template shard).  Lane L decodes descriptor L of the step once (word offset and shift
-// packed in one register) and the lanes of group q pick theirs up by shuffle; control flow is warp-uniform.  The partial
-// counters meet (bit-sliced adds across the groups, two butterfly steps) at two check points -- after about half and
-// three quarters of the features -- where cells, lanes and whole candidates that can no longer reach `need` are dropped,
-// and at the end.
-__device__ __forceinline__ void vc_allreduce_groups(uint32_t (&c)[LM_FILTER_BITS]) {
+// kernel above).  Lane k of each half-warp owns patch column k: the 16 columns of one row block are 16 consecutive words
+// of the column-major H-plane, so every load of a half-warp reads ONE 64-byte window and a warp-wide load touches two
+// windows (one per half-warp).  Of every 32 consecutive features half-warp h adds features 16h .. 16h+15, two per
+// register: the 16 rows of the first feature of a pair in the low half-word, of the second in the high half-word (one
+// PRMT), so the 9-bit vertical counters count the same 16 cells twice, in two halves.  A candidate is a chain of nf / 32
+// steps.  Lane L decodes descriptor L of the step once (byte offset and shift packed in one register) and stores it to
+// shared memory; every lane picks up four descriptors of its half-warp with one 128-bit broadcast load.  Control flow
+// is warp-uniform.  Every LM_FILTER_CHECK features, once `need` exceeds the features still to come, the partial
+// counters meet (vc_fold) and cells, lanes and whole candidates that can no longer reach `need` are dropped; the last
+// check is at the end.
+
+// The partial counters of a warp meet: each lane adds its high half-word into its low one (bit-sliced), then the two
+// half-warps add theirs (one butterfly step).  Afterwards the low 16 bits of lanes k and k + 16 both hold the totals of
+// patch column k (bit r = row r); the high 16 bits are meaningless.
+__device__ __forceinline__ void vc_fold(uint32_t (&c)[LM_FILTER_BITS]) {
+  uint32_t carry = 0u;
 #pragma unroll
-  for (int step = 8; step <= 16; step <<= 1) {
-    uint32_t carry = 0u;
+  for (int b = 0; b < LM_FILTER_BITS; ++b) {
+    const uint32_t a = c[b], o = a >> 16;
+    c[b] = a ^ o ^ carry;
+    carry = (a & o) | (carry & (a ^ o));
+  }
+  carry = 0u;
 #pragma unroll
-    for (int b = 0; b < LM_FILTER_BITS; ++b) {
-      const uint32_t o = __shfl_xor_sync(0xffffffffu, c[b], step);
-      const uint32_t a = c[b];
-      c[b] = a ^ o ^ carry;
-      carry = (a & o) | (carry & (a ^ o));
-    }
+  for (int b = 0; b < LM_FILTER_BITS; ++b) {
+    const uint32_t o = __shfl_xor_sync(0xffffffffu, c[b], 16);
+    const uint32_t a = c[b];
+    c[b] = a ^ o ^ carry;
+    carry = (a & o) | (carry & (a ^ o));
   }
 }
 
@@ -1302,11 +1312,20 @@ __device__ __forceinline__ const uint32_t* lm_ptr_add(const char* base, uint32_t
   return reinterpret_cast<const uint32_t*>(r);
 }
 
+// one H-plane word of this lane's column, shifted so that bits 0..15 are the 16 patch rows (v = byte offset << 5 | row
+// shift; the funnel shift takes the low 5 bits of v)
+__device__ __forceinline__ uint32_t lm_plane_rows(const char* col, uint32_t v) {
+  return __funnelshift_r(__ldg(lm_ptr_add(col, v >> 5)), 0u, v);
+}
+
 #ifndef LM_FILTER_MIN_CTAS
 #define LM_FILTER_MIN_CTAS 5
 #endif
 #ifndef LM_FILTER_CHUNK
 #define LM_FILTER_CHUNK 1  // consecutive candidates a warp takes from the queue at a time (2..16 measured: tail imbalance costs more than the L1 reuse buys)
+#endif
+#ifndef LM_FILTER_CHECK
+#define LM_FILTER_CHECK 64  // features between two bound checks, a multiple of 32 (32 measured: the extra merges cost more than the words they save, DESIGN.md §9)
 #endif
 // Layout contract with the host (prepare_bank / prepare_work): every template's descriptors are padded to a multiple of
 // 32 with descriptors that point into an all-zero tail of the plane buffer (so the loop needs no bounds predicate), and
@@ -1314,7 +1333,12 @@ __device__ __forceinline__ const uint32_t* lm_ptr_add(const char* base, uint32_t
 // the host for the call's threshold with the same two IEEE float operations (lm_min_kept_raw).
 __global__ void __launch_bounds__(256, LM_FILTER_MIN_CTAS) k_refine_filter_w(FilterParams p) {
   lm_pdl_wait();
-  const int lane = threadIdx.x & 31, grp = lane >> 3, gl = lane & 7;
+  // per warp: the 32 decoded descriptors of a step, two buffers (consecutive steps alternate, so one __syncwarp per step
+  // orders a buffer's reads before its next write)
+  __shared__ uint4 s_desc[8][2][8];
+  const int lane = threadIdx.x & 31, hw = lane >> 4, ck = lane & 15;
+  uint4 (*const sd)[8] = s_desc[threadIdx.x >> 5];
+  int sb = 0;
   const int total = min(p.off[p.n_work], p.cand_cap);
   const int T = p.ref.T, border = 8 * T;
   const int Wd = p.Wd;
@@ -1365,12 +1389,10 @@ __global__ void __launch_bounds__(256, LM_FILTER_MIN_CTAS) k_refine_filter_w(Fil
         x = max(x, border); y = max(y, border);
         x = min(x, p.ref.cols - (fi.z & 0xFFFF) - border);
         y = min(y, p.ref.rows - (int)((unsigned)fi.z >> 16) - border);
-        const char* __restrict__ col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + gl));  // this lane's first column
+        const char* __restrict__ col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + ck));  // this lane's column
         const int cy = y / T - 8;
         const uint32_t* __restrict__ fd = p.rdesc + fi.x;
         const int nfp = (nf + 31) & ~31;  // descriptors are padded with zero-plane entries
-        // check points: multiples of 32 features nearest to 1/2 and 3/4 of the template
-        const int chk1 = ((nf / 2 + 31) & ~31), chk2 = ((nf * 3 / 4 + 31) & ~31);
         uint32_t ch[LM_FILTER_BITS];
 #pragma unroll
         for (int b = 0; b < LM_FILTER_BITS; ++b) ch[b] = 0u;
@@ -1381,37 +1403,37 @@ __global__ void __launch_bounds__(256, LM_FILTER_MIN_CTAS) k_refine_filter_w(Fil
           const uint32_t d = d_next;
           if (i + 32 < nfp) d_next = __ldg(fd + i + 32 + lane);  // one step ahead
           const int py0 = cy + (int)(d >> 23);
-          const uint32_t v = (((d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd)) << 7) | ((uint32_t)py0 & 15u);
+          reinterpret_cast<uint32_t*>(sd[sb])[lane] = (((d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd)) << 7) | ((uint32_t)py0 & 15u);
+          __syncwarp();
           uint32_t xh[8];
 #pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const uint32_t vu = __shfl_sync(0xffffffffu, v, u, 8);  // lane u of this lane's group
-            const uint32_t* __restrict__ ptr = lm_ptr_add(col, vu >> 5);
-            uint32_t w0 = 0u, w1 = 0u;
+          for (int m = 0; m < 4; ++m) {
+            const uint4 v = sd[sb][hw * 4 + m];  // features i + 16 hw + 4m .. + 3
+            uint32_t r0 = 0u, r1 = 0u, r2 = 0u, r3 = 0u;
             if (lane_alive) {
-              w0 = __ldg(ptr);
-              w1 = __ldg(ptr + 8);
+              r0 = lm_plane_rows(col, v.x);
+              r1 = lm_plane_rows(col, v.y);
+              r2 = lm_plane_rows(col, v.z);
+              r3 = lm_plane_rows(col, v.w);
             }
-            // funnel shift = shift by the low 5 bits of vu (the row offset inside the word)
-            xh[u] = __byte_perm(__funnelshift_r(w0, 0u, vu), __funnelshift_r(w1, 0u, vu), 0x5410);
+            xh[2 * m] = __byte_perm(r0, r1, 0x5410);
+            xh[2 * m + 1] = __byte_perm(r2, r3, 0x5410);
           }
+          sb ^= 1;
           if (lane_alive) words_read += 16;
           vc_add8n<LM_FILTER_BITS>(ch, xh);
+          // cells that can still reach `need`: CH >= need - (features not yet added); warp-uniform
           const int done = i + 32;
-          if ((done == chk1 || done == chk2) && done < nf) {
-            vc_allreduce_groups(ch);  // every group now holds the totals of its 32 cells
-            const uint32_t alive_cells = vc_ge(ch, need - (nf - done));
-            lane_alive = alive_cells != 0u;
+          const int thr = need - max(nf - done, 0);
+          if (thr > 0 && (done >= nf || done % LM_FILTER_CHECK == 0)) {
+            vc_fold(ch);
+            lane_alive = (vc_ge(ch, thr) & 0xFFFFu) != 0u;
             if (!__any_sync(0xffffffffu, lane_alive)) { dead = true; break; }
-            if (grp) {  // the totals live on in group 0; the others start their partial counts again
+            // the totals live on in the low half-words of half-warp 0; the rest starts its partial counts again
+            const uint32_t keep = hw ? 0u : 0xFFFFu;
 #pragma unroll
-              for (int b = 0; b < LM_FILTER_BITS; ++b) ch[b] = 0u;
-            }
+            for (int b = 0; b < LM_FILTER_BITS; ++b) ch[b] &= keep;
           }
-        }
-        if (!dead) {
-          vc_allreduce_groups(ch);
-          dead = !__any_sync(0xffffffffu, vc_ge(ch, need) != 0u);
         }
         if (dead) {
           if (lane == 0) dropped_feats += (unsigned)nf;  // the reference's work for it (algorithmic bytes / 256)
@@ -1779,11 +1801,11 @@ __global__ void __launch_bounds__(256, LM_REFINE_MIN_CTAS) k_refine(RefineParams
 //
 // similarityLocal's response is 4*H + N with H = the feature's label bit in the spread mask and N = (either neighbouring
 // label bit) & ~H (lm_response), so the exact 16x16 sums are raw = 4*CH + CN.  Same warp layout as k_refine_filter_w
-// (four 8-lane groups deal the features of the candidate between them, lane k of a group holds patch columns k and k + 8),
-// but three H-plane windows per feature (labels o - 1, o, o + 1) and two vertical counters.  The partial counters meet
-// once, at the end; the score 4*CH + CN, the best cell (max raw, lowest cell index = first maximum in row-major order,
-// LL.cpp:1910-1927) and the keep test (LL.cpp:1935-1937) are evaluated bit-sliced.  The byte linear memories are never
-// touched.
+// (lane k of each half-warp holds patch column k, the half-warps deal the features of a step between them, two features
+// per register), but three H-plane windows per feature (labels o - 1, o, o + 1) and two vertical counters.  The partial
+// counters meet once, at the end; the score 4*CH + CN, the best cell (max raw, lowest cell index = first maximum in
+// row-major order, LL.cpp:1910-1927) and the keep test (LL.cpp:1935-1937) are evaluated bit-sliced.  The byte linear
+// memories are never touched.
 // --------------------------------------------------------------------------------------------
 struct RefineBitsParams {
   const uint32_t* rp;      // H-planes of level 0 (k_refine_prep), zero tail behind
@@ -1827,8 +1849,11 @@ __device__ __forceinline__ void vc_add(uint32_t (&c)[LM_FILTER_BITS], const uint
 __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
   lm_pdl_wait();
   __shared__ uint32_t s_part[8][2 * LM_FILTER_BITS][32];
-  const int lane = threadIdx.x & 31, gl = lane & 7, warp = threadIdx.x >> 5;
+  __shared__ uint4 s_desc[8][2][3][8];  // per warp: the decoded descriptors of a step (three planes), as k_refine_filter_w
+  const int lane = threadIdx.x & 31, hw = lane >> 4, ck = lane & 15, warp = threadIdx.x >> 5;
   const int quad = warp >> 2, q = warp & 3;
+  uint4 (*const sd)[3][8] = s_desc[warp];
+  int sb = 0;
   const int total = min(p.off[p.n_work], p.cand_cap);
   const int n_items = min(__ldcg(p.queue + 1), total);
   const int T = p.ref.T, border = 8 * T;
@@ -1858,7 +1883,7 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
       x = max(x, border); y = max(y, border);  // LL.cpp:1875-1880 (max first, then min)
       x = min(x, p.ref.cols - (fi.z & 0xFFFF) - border);
       y = min(y, p.ref.rows - (int)((unsigned)fi.z >> 16) - border);
-      const char* __restrict__ col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + gl));
+      const char* __restrict__ col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + ck));
       const int cy = y / T - 8;
       const uint32_t* __restrict__ fd = p.rdesc + fi.x;
       const uint8_t* __restrict__ fl = p.rlab + fi.x;
@@ -1875,26 +1900,30 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
         const uint32_t sft = (uint32_t)py0 & 15u;
         const int dm = o >= 8 ? 0 : (o == 0 ? 7 * p.label_stride : -p.label_stride);
         const int dp = o >= 7 ? (o == 7 ? -7 * p.label_stride : 0) : p.label_stride;
-        const uint32_t v0 = (idx << 7) | sft;  // byte offset : 27 | row shift : 5
-        const uint32_t vm = ((uint32_t)((int)idx + dm) << 7) | sft;
-        const uint32_t vp = ((uint32_t)((int)idx + dp) << 7) | sft;
+        uint32_t* const sw = reinterpret_cast<uint32_t*>(sd[sb]);
+        sw[lane] = (idx << 7) | sft;  // byte offset : 27 | row shift : 5
+        sw[32 + lane] = ((uint32_t)((int)idx + dm) << 7) | sft;
+        sw[64 + lane] = ((uint32_t)((int)idx + dp) << 7) | sft;
+        __syncwarp();
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
           uint32_t xh[4], xn[4];
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int src = half * 4 + u;  // lane `src` of this lane's group
-            const uint32_t a0 = __shfl_sync(0xffffffffu, v0, src, 8);
-            const uint32_t am = __shfl_sync(0xffffffffu, vm, src, 8);
-            const uint32_t ap = __shfl_sync(0xffffffffu, vp, src, 8);
-            const uint32_t* __restrict__ p0 = lm_ptr_add(col, a0 >> 5);
-            const uint32_t* __restrict__ pm = lm_ptr_add(col, am >> 5);
-            const uint32_t* __restrict__ pp = lm_ptr_add(col, ap >> 5);
-            const uint32_t h = __byte_perm(__funnelshift_r(__ldg(p0), 0u, a0), __funnelshift_r(__ldg(p0 + 8), 0u, a0), 0x5410);
-            const uint32_t a = __byte_perm(__funnelshift_r(__ldg(pm), 0u, a0), __funnelshift_r(__ldg(pm + 8), 0u, a0), 0x5410);
-            const uint32_t b = __byte_perm(__funnelshift_r(__ldg(pp), 0u, a0), __funnelshift_r(__ldg(pp + 8), 0u, a0), 0x5410);
-            xh[u] = h;
-            xn[u] = (a | b) & ~h;
+          for (int m = 0; m < 2; ++m) {
+            // features i + 16 hw + 8 half + 4m .. + 3, two per register
+            const uint4 a0 = sd[sb][0][hw * 4 + half * 2 + m];
+            const uint4 am = sd[sb][1][hw * 4 + half * 2 + m];
+            const uint4 ap = sd[sb][2][hw * 4 + half * 2 + m];
+            const uint32_t h0 = __byte_perm(lm_plane_rows(col, a0.x), lm_plane_rows(col, a0.y), 0x5410);
+            const uint32_t n0 = __byte_perm(lm_plane_rows(col, am.x), lm_plane_rows(col, am.y), 0x5410) |
+                                __byte_perm(lm_plane_rows(col, ap.x), lm_plane_rows(col, ap.y), 0x5410);
+            const uint32_t h1 = __byte_perm(lm_plane_rows(col, a0.z), lm_plane_rows(col, a0.w), 0x5410);
+            const uint32_t n1 = __byte_perm(lm_plane_rows(col, am.z), lm_plane_rows(col, am.w), 0x5410) |
+                                __byte_perm(lm_plane_rows(col, ap.z), lm_plane_rows(col, ap.w), 0x5410);
+            xh[2 * m] = h0;
+            xn[2 * m] = n0 & ~h0;
+            xh[2 * m + 1] = h1;
+            xn[2 * m + 1] = n1 & ~h1;
           }
           // four 1-bit planes into each vertical counter
           uint32_t t1a, t1b, t2;
@@ -1909,6 +1938,7 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
 #pragma unroll
           for (int b = 2; b < LM_FILTER_BITS; ++b) { const uint32_t k = cn[b] & t2; cn[b] ^= t2; t2 = k; }
         }
+        sb ^= 1;
         words_read += 48;
       }
     }
@@ -1933,8 +1963,8 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
         vc_add(ch, oh);
         vc_add(cn, on);
       }
-      vc_allreduce_groups(ch);
-      vc_allreduce_groups(cn);
+      vc_fold(ch);  // low 16 bits of lanes k, k + 16: column k
+      vc_fold(cn);
       // raw = 4*CH + CN, 11 bits (4 * 511 < 2048)
       uint32_t sc[11];
       sc[0] = cn[0];
@@ -1948,7 +1978,7 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
         carry = (a & h) | (carry & (a ^ h));
       }
       // best raw score: highest bit first, keep the cells that still tie for the maximum
-      uint32_t cells = 0xffffffffu;
+      uint32_t cells = 0xFFFFu;
       int best_raw = 0;
 #pragma unroll
       for (int b = 10; b >= 0; --b) {
@@ -1958,11 +1988,9 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
           best_raw |= 1 << b;
         }
       }
-      // first maximum in row-major order: lowest row, then lowest column (bits 0..15 = rows of column gl, 16..31 = of
-      // gl + 8)
+      // first maximum in row-major order: lowest row, then lowest column (bit r = row r of column ck)
       int cell = 0x7fffffff;
-      if (cells & 0xFFFFu) cell = (__ffs(cells & 0xFFFFu) - 1) * 16 + gl;
-      if (cells >> 16) cell = min(cell, (__ffs(cells >> 16) - 1) * 16 + gl + 8);
+      if (cells) cell = (__ffs(cells) - 1) * 16 + ck;
       cell = __reduce_min_sync(0xffffffffu, cell);
       int br = -1, bc = -1;
       if (best_raw > 0) {
