@@ -28,6 +28,7 @@ SYMBOLS = [
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
+    "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
 ]
@@ -97,6 +98,9 @@ def load():
     L.lm_launch_count.restype = c_i64
     f32p, f64p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
     u16p = ctypes.POINTER(ctypes.c_uint16)
+    L.lm_set_template_renders.argtypes = [vp, c_i64, c_i64, ctypes.POINTER(u16p), c_int, c_int, f32p, f32p, f32p]
+    L.lm_enqueue_pose.argtypes = [vp, f32p, c_int, c_int]
+    L.lm_complete_pose.argtypes = [vp, vp, f64p, f64p, f32p, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
     L.lm_icp_destroy.restype = None
@@ -364,6 +368,52 @@ class NativeDetector:
         check(self._L.lm_match_top(self._h, ptrs, r, c, ctypes.c_float(threshold), float(iou_threshold), int(top_k),
                                    out.ctypes.data_as(ctypes.c_void_p), out.shape[0], ctypes.byref(n), ctypes.byref(nrec)))
         return out[:n.value].copy(), int(nrec.value)
+
+    # ---- pose stage behind the NMS (include/linemod_b200.h, lm_*_pose) ----
+    def set_template_renders(self, first, depths, K, R, t):
+        """Templates [first, first + len(depths)) of the bank: depths u16 HxW (one size per call), K / R [n,3,3] f32,
+        t [n,3] f32 mm.  The same array may serve several templates."""
+        n = len(depths)
+        ds = [np.ascontiguousarray(d, np.uint16) for d in depths]
+        if any(d.ndim != 2 or d.shape != ds[0].shape for d in ds):
+            raise TypeError("renders must be uint16 HxW images of one size")
+        u16p = ctypes.POINTER(ctypes.c_uint16)
+        f32p = ctypes.POINTER(ctypes.c_float)
+        ptrs = (u16p * max(n, 1))(*[d.ctypes.data_as(u16p) for d in ds])
+        K = np.ascontiguousarray(K, np.float32).reshape(n, 9)
+        R = np.ascontiguousarray(R, np.float32).reshape(n, 9)
+        t = np.ascontiguousarray(t, np.float32).reshape(n, 3)
+        rows, cols = ds[0].shape if n else (0, 0)
+        check(self._L.lm_set_template_renders(self._h, int(first), n, ptrs, int(rows), int(cols), K.ctypes.data_as(f32p),
+                                              R.ctypes.data_as(f32p), t.ctypes.data_as(f32p)))
+
+    def enqueue_pose(self, sceneK, max_iterations=30, use_scene_cloud=False):
+        sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+        check(self._L.lm_enqueue_pose(self._h, sK.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), int(max_iterations),
+                                      1 if use_scene_cloud else 0))
+
+    def complete_pose(self):
+        """Returns (survivors, R [n,3,3] f64, t [n,3] f64 mm, residual [n] f32, records seen by the NMS); rows of an
+        early return (residual -1) keep R / t at NaN."""
+        cap = 1024
+        out = np.empty(cap, MATCH_DTYPE)
+        Ro = np.full((cap, 3, 3), np.nan, np.float64)
+        to = np.full((cap, 3), np.nan, np.float64)
+        res = np.zeros(cap, np.float32)
+        n, nrec = ctypes.c_int64(), ctypes.c_int64()
+        f64p = ctypes.POINTER(ctypes.c_double)
+        check(self._L.lm_complete_pose(self._h, out.ctypes.data_as(ctypes.c_void_p), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
+                                       res.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), cap, ctypes.byref(n), ctypes.byref(nrec)))
+        k = n.value
+        return out[:k].copy(), Ro[:k].copy(), to[:k].copy(), res[:k].copy(), int(nrec.value)
+
+    def match_pose(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30, use_scene_cloud=False):
+        """upload_images + enqueue + enqueue_post + enqueue_pose + complete_pose: one chain on the detector's stream."""
+        self.upload_images(rgb, depth, masks)
+        self.enqueue(threshold)
+        self.enqueue_post(iou_threshold, top_k)
+        self.enqueue_pose(sceneK, max_iterations, use_scene_cloud)
+        return self.complete_pose()
 
     def linear_memories(self, level, modality, shape):
         out = np.zeros(shape, np.uint8)

@@ -56,6 +56,7 @@ int lm_fail(int code, const char* fmt, ...) {
 #include "lm_kernels.cuh"
 #include "lm_frontend.cuh"
 #include "lm_post.cuh"
+#include "lm_pose.h"
 
 // Launch with programmatic stream serialization (see lm_pdl_wait in lm_kernels.cuh).
 template <typename... KArgs, typename... Args>
@@ -191,6 +192,12 @@ struct lm_detector {
   bool post_pending = false, post_retry = false;
   double post_iou = 0.5; int post_top_k = 0;
 
+  // pose stage behind the NMS (lm_pose.h): per-template render crops, refinement of the survivors on the device
+  lm_pose_stage* pose = nullptr;
+  bool frame_depth = false;             // the frame came from lm_upload_images: fe_depth holds its depth
+  bool pose_pending = false;
+  float pose_sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; int pose_max_iter = 30, pose_use_scene = 0;
+
   // multi-GPU exchange fused into k_refine (lm_peer_*)
   uint8_t* px_buf = nullptr;            // this rank's exchange buffer (IPC-exportable cudaMalloc)
   int64_t px_cap = 0;                   // records per block
@@ -311,7 +318,7 @@ static void peer_release(lm_detector* d) {
 
 extern "C" void lm_destroy(lm_detector* d) {
   if (!d) return;
-  if (d->device < 0) { delete d; return; }
+  if (d->device < 0) { pose_stage_destroy(d->pose); delete d; return; }
   cudaSetDevice(d->device);
   if (d->stream) cudaStreamSynchronize(d->stream);
   peer_release(d);
@@ -330,6 +337,7 @@ extern "C" void lm_destroy(lm_detector* d) {
     cudaFree(d->fe[l].mask[0]); cudaFree(d->fe[l].mask[1]);
   }
   cudaFree(d->fe_depth); cudaFree(d->fe_nraw);
+  pose_stage_destroy(d->pose);
   for (cudaEvent_t e : d->tev) cudaEventDestroy(e);
   if (d->copy_stream) { cudaStreamSynchronize(d->copy_stream); cudaStreamDestroy(d->copy_stream); }
   if (d->ev_fork) cudaEventDestroy(d->ev_fork);
@@ -379,6 +387,7 @@ extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_
   d->class_of.clear();
   d->boxes.clear();  // box sizes belong to the bank they were set for
   d->post_dirty = true;
+  if (d->pose) pose_stage_clear(d->pose);  // so do the template renders
   d->feats.assign(feats, feats + (size_t)n_feats * 3);
   d->feat_slot.swap(slot_of);
   cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc4); cudaFree(d->d_k2info);
@@ -896,6 +905,7 @@ static int upload_quantized(lm_detector* d, const uint8_t* const* quantized, con
     if (fork) CU(cudaStreamSynchronize(d->copy_stream));
   }
   d->have_frame = true;
+  d->frame_depth = false;
   d->have_run = false;
   return LM_OK;
 }
@@ -916,6 +926,7 @@ extern "C" int lm_bind_quantized_device(lm_detector* d, const uint8_t* const* d_
   if (d->upper_pending) CU(cudaStreamWaitEvent(d->stream, d->ev_upper, 0));  // an earlier upload nobody consumed
   d->upper_pending = false;
   d->have_frame = true;
+  d->frame_depth = false;
   d->have_run = false;
   return LM_OK;
 }
@@ -1009,6 +1020,7 @@ extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16
   CU(cudaGetLastError());
   d->upper_pending = false;
   d->have_frame = true;
+  d->frame_depth = true;
   d->have_run = false;
   return LM_OK;
 }
@@ -1877,6 +1889,8 @@ extern "C" int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k) 
   return LM_OK;
 }
 
+static int enqueue_pose(lm_detector* d);
+
 extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !n_out) return fail(LM_E_INVALID, "null argument");
@@ -1907,6 +1921,10 @@ extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int6
     if (rc) return rc;
     rc = lm_enqueue_post(d, d->post_iou, d->post_top_k);
     if (rc) return rc;
+    if (d->pose_pending) {  // the pose stage ran on the truncated survivor list: run it again behind the new NMS
+      rc = enqueue_pose(d);
+      if (rc) return rc;
+    }
     d->post_retry = true;
     rc = lm_complete_post(d, out, cap, n_out, n_records);
     d->post_retry = false;
@@ -1931,6 +1949,56 @@ extern "C" int lm_match_top(lm_detector* d, const uint8_t* const* quantized, con
   rc = lm_enqueue_post(d, iou_threshold, top_k);
   if (rc) return rc;
   return lm_complete_post(d, out, cap, n_out, n_records);
+}
+
+// ---- pose stage behind the NMS (lm_pose.h, lm_icp.cu) ---------------------------------------------
+extern "C" int lm_set_template_renders(lm_detector* d, int64_t first, int64_t n, const uint16_t* const* depths, int rows, int cols,
+                                       const float* K, const float* R, const float* t) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (d->S == 0) return fail(LM_E_STATE, "no template bank loaded");
+  if (!d->pose) d->pose = pose_stage_create();
+  return pose_stage_register(d->pose, d->class_begin.data(), d->n_classes, first, n, depths, rows, cols, K, R, t);
+}
+
+static int enqueue_pose(lm_detector* d) {
+  PoseEnqueue e;
+  e.d_surv = d->d_post_out; e.d_counts = d->d_post_counts;
+  e.d_scene = d->fe_depth; e.srows = d->fe[0].rows; e.scols = d->fe[0].cols;
+  memcpy(e.sK, d->pose_sK, sizeof(e.sK));
+  e.bound = d->post_top_k > 0 ? std::min(d->post_top_k, LM_POST_MAX) : LM_POST_MAX;
+  e.use_scene_cloud = d->pose_use_scene;
+  e.max_iterations = d->pose_max_iter;
+  e.stream = d->stream;
+  return pose_stage_enqueue(d->pose, e, &d->launches);
+}
+
+extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iterations, int use_scene_cloud) {
+  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (!d || !sceneK) return fail(LM_E_INVALID, "null argument");
+  if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
+  if (!d->post_pending) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
+  if (!d->frame_depth) return fail(LM_E_STATE, "the frame has no depth image: upload it with lm_upload_images");
+  if (!d->pose || !pose_stage_covers(d->pose, d->sel.data(), (int64_t)d->sel.size()))
+    return fail(LM_E_STATE, "no template renders registered for every selected template of this bank (lm_set_template_renders)");
+  CU(cudaSetDevice(d->device));
+  memcpy(d->pose_sK, sceneK, sizeof(d->pose_sK));
+  d->pose_max_iter = max_iterations;
+  d->pose_use_scene = use_scene_cloud ? 1 : 0;
+  int rc = enqueue_pose(d);
+  if (rc) return rc;
+  d->pose_pending = true;
+  return LM_OK;
+}
+
+extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
+                                int64_t* n_out, int64_t* n_records) {
+  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (!d || !n_out || (cap > 0 && (!R_out || !t_out || !residual))) return fail(LM_E_INVALID, "null argument");
+  if (!d->pose_pending) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
+  int rc = lm_complete_post(d, out, cap, n_out, n_records);  // waits; on the capacity retry it runs the pose stage again
+  d->pose_pending = false;
+  if (rc) return rc;
+  return pose_stage_finish(d->pose, d->stream, d->h_post_out, *n_out, R_out, t_out, residual);
 }
 
 extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,

@@ -13,9 +13,15 @@
 // All arithmetic is double, as in Open3D/Eigen.  The reference's quirks are kept: the ICP target is the
 // down-sampled MODEL cloud (LL.cpp:109), only the z component of the initial translation is converted
 // to metres (LL.cpp:37), `residual` carries the fitness (LL.cpp:148).
+//
+// The pose stage (lm_pose.h, end of this file) does the host's cloud building on the device for the detector's NMS
+// survivors: k_pose_cloud + a CUB segmented sort + k_pose_voxel build the same clouds and initial guesses, bit for
+// bit, and feed the same two ICP kernels.
 
 #include "linemod_b200.h"
+#include "lm_pose.h"
 
+#include <cub/cub.cuh>
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdarg.h>
@@ -416,28 +422,55 @@ struct Cloud {
 // LL.cpp:34-109 for one hypothesis.
 void voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out);
 
-void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* model, int mrows, int mcols, const float* sK,
-                 const float* mK, const float* R, const float* t, int detectX, int detectY, bool want_scene, Cloud& c) {
-  // init_base = [R | t] with only t.z converted to metres (LL.cpp:34-38)
-  for (int i = 0; i < 16; ++i) c.base[i] = 0.f;
+// init_base = [R | t] with only t.z converted to metres (LL.cpp:34-38)
+void init_base(const float* R, const float* t, float* base) {
+  for (int i = 0; i < 16; ++i) base[i] = 0.f;
   for (int r = 0; r < 3; ++r) {
-    for (int k = 0; k < 3; ++k) c.base[4 * r + k] = R[3 * r + k];
-    c.base[4 * r + 3] = t[r];
+    for (int k = 0; k < 3; ++k) base[4 * r + k] = R[3 * r + k];
+    base[4 * r + 3] = t[r];
   }
-  c.base[4 * 2 + 3] /= 1000.0f;
-  c.base[15] = 1.f;
-  // dilate(modelDepth > 0, 9x9) + boundingRect (LL.cpp:43-50): the box of the non-zero pixels grown by 4
+  base[4 * 2 + 3] /= 1000.0f;
+  base[15] = 1.f;
+}
+
+// result = transformation_ * init_base (LL.cpp:146); R_refined, t_refined * 1000 (LL.cpp:153-154)
+void compose(const double* T, const float* base, double* R_out, double* t_out) {
+  double res[16];
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) {
+      double s = 0;
+      for (int k = 0; k < 4; ++k) s += T[4 * r + k] * (double)base[4 * k + c];
+      res[4 * r + c] = s;
+    }
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) R_out[3 * r + c] = res[4 * r + c];
+    t_out[r] = res[4 * r + 3] * 1000.0;
+  }
+}
+
+// dilate(modelDepth > 0, 9x9) + boundingRect (LL.cpp:43-50): the box of the non-zero pixels grown by 4, clipped to the
+// image; an all-zero image gives the empty box
+void model_box(const uint16_t* model, int mrows, int mcols, int* box) {
   const int half = 4;
   int x0 = mcols, x1 = -1, y0 = mrows, y1 = -1;
   for (int r = 0; r < mrows; ++r)
     for (int q = 0; q < mcols; ++q)
       if (model[(size_t)r * mcols + q] > 0) { x0 = std::min(x0, q); x1 = std::max(x1, q); y0 = std::min(y0, r); y1 = std::max(y1, r); }
-  int bx = 0, by = 0, bw = 0, bh = 0;
+  box[0] = box[1] = box[2] = box[3] = 0;
   if (x1 >= 0) {
-    bx = std::max(x0 - half, 0); by = std::max(y0 - half, 0);
-    bw = std::min(x1 + half, mcols - 1) - bx + 1;
-    bh = std::min(y1 + half, mrows - 1) - by + 1;
+    box[0] = std::max(x0 - half, 0); box[1] = std::max(y0 - half, 0);
+    box[2] = std::min(x1 + half, mcols - 1) - box[0] + 1;
+    box[3] = std::min(y1 + half, mrows - 1) - box[1] + 1;
   }
+}
+
+void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* model, int mrows, int mcols, const float* sK,
+                 const float* mK, const float* R, const float* t, int detectX, int detectY, bool want_scene, Cloud& c) {
+  init_base(R, t, c.base);
+  const int half = 4;
+  int box[4];
+  model_box(model, mrows, mcols, box);
+  const int bx = box[0], by = box[1], bw = box[2], bh = box[3];
   c.early = (detectX + bw >= scols) || (detectY + bh >= srows);  // LL.cpp:52-55
   if (c.early) return;
   // clouds (LL.cpp:57-99)
@@ -616,18 +649,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   for (int i = 0; i < n_hyp; ++i) {
     if (job_of[i] < 0) { residual[i] = -1.f; continue; }
     const IcpOut& o = h->h_outs[job_of[i]];
-    // result = transformation_ * init_base (LL.cpp:146); R_refined, t_refined * 1000 (LL.cpp:153-154)
-    double res[16];
-    for (int r = 0; r < 4; ++r)
-      for (int c = 0; c < 4; ++c) {
-        double s = 0;
-        for (int k = 0; k < 4; ++k) s += o.T[4 * r + k] * (double)clouds[i].base[4 * k + c];
-        res[4 * r + c] = s;
-      }
-    for (int r = 0; r < 3; ++r) {
-      for (int c = 0; c < 3; ++c) R_out[9 * i + 3 * r + c] = res[4 * r + c];
-      t_out[3 * i + r] = res[4 * r + 3] * 1000.0;
-    }
+    compose(o.T, clouds[i].base, R_out + 9 * i, t_out + 3 * i);
     residual[i] = (float)o.fitness;
     h->last_points = jobs[job_of[i]].src_count;
     h->last_iterations = o.iterations;
@@ -658,5 +680,472 @@ extern "C" int64_t lm_icp_launch_count(lm_icp* h) { return h ? h->launches : 0; 
 extern "C" int lm_icp_set_use_scene_cloud(lm_icp* h, int on) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
   h->use_scene_cloud = on != 0;
+  return LM_OK;
+}
+
+// --------------------------------------------------------------------------------------------
+// pose stage on the device (lm_pose.h): build_cloud + voxel_down_sample for the NMS survivors
+// --------------------------------------------------------------------------------------------
+// Exactness: every float / double operation that build_cloud and voxel_down_sample do is written with an _rn
+// intrinsic (no FMA contraction), points are compacted with block scans in the host's row-major order, the centroids
+// are summed by one thread each in that order, and the voxel keys are sorted stably, so clouds and initial guesses are
+// bit-identical to the host's.
+#define POSE_THREADS 512
+#define POSE_KEY_BITS 21  // per voxel coordinate: 2^21 voxels of 2.5 mm = 5.2 km of cloud extent
+#define POSE_FIRST_FETCH 16
+
+struct PoseTpl {  // per template of the bank, registered once
+  int32_t bx, by, bw, bh;  // dilated box of the render's non-zero pixels, clipped to the render
+  int64_t crop;            // first pixel of the bw x bh crop in the crop pool
+  float K[9];
+  uint32_t anchor;         // render[rows / 2][cols / 2] (mm), usually outside the box
+};
+
+struct PoseParams {
+  const lm_match* surv;
+  const int32_t* counts;
+  const int32_t* class_begin;
+  int32_t n_classes, n_tpl;
+  const PoseTpl* tpl;
+  const uint16_t* crops;
+  const uint16_t* scene;
+  int32_t srows, scols;
+  float sK[9];
+  int32_t A;          // points per cloud slot (largest crop)
+  int32_t use_scene;
+  double* raw;        // [2B][A][3] back-projected points: slot 2i model cloud, 2i + 1 scene cloud of survivor i
+  double* cpts;       // [B][A][3] scene points that enter the scene centroid
+  unsigned long long* keys;  // [2B][A] voxel keys (a, b, c) packed
+  int32_t* vals;      // [2B][A] point index in the slot
+  int32_t* seg_begin; // [2B]
+  int32_t* seg_end;
+  IcpJob* jobs;       // [B]
+  int32_t* err;       // 1: a cloud spans more than 2^21 voxels along an axis
+};
+
+__device__ __forceinline__ double pose_backproject(int pix, float c, float f, double z) {
+  return __dmul_rn((double)__fdiv_rn(__fsub_rn((float)pix, c), f), z);  // int - float -> float, / float, * double
+}
+
+__device__ __forceinline__ int pose_template(const PoseParams& p, const lm_match& m) {
+  if (m.class_index < 0 || m.class_index >= p.n_classes) return -1;
+  const int g = p.class_begin[m.class_index] + m.template_id;
+  return (g >= 0 && g < p.n_tpl) ? g : -1;
+}
+
+// One CTA per survivor slot (launched for the bound; slots past the survivor count write empty jobs).
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
+  typedef cub::BlockScan<unsigned long long, POSE_THREADS> Scan;
+  typedef cub::BlockReduce<double, POSE_THREADS> Reduce;
+  __shared__ union {
+    typename Scan::TempStorage scan;
+    typename Reduce::TempStorage reduce;
+  } tmp;
+  __shared__ double s_min[6], s_sum[6];
+  const int i = blockIdx.x, tid = threadIdx.x;
+  const size_t A = (size_t)p.A;
+  const size_t sm = 2 * (size_t)i * A, ss = sm + A;  // first point of the model / scene slot
+  IcpJob* job = p.jobs + i;
+  lm_match m = {0, 0, 0.f, 0, 0};
+  PoseTpl T;
+  bool live = i < p.counts[0];
+  if (live) {
+    m = p.surv[i];
+    const int g = pose_template(p, m);
+    live = g >= 0;
+    if (live) {
+      T = p.tpl[g];
+      live = !(m.x + T.bw >= p.scols || m.y + T.bh >= p.srows);  // LL.cpp:52-55
+    }
+  }
+  if (!live) {  // block-uniform
+    if (tid == 0) {
+      job->src_first = job->tgt_first = (int32_t)sm;
+      job->src_count = job->tgt_count = 0;
+      for (int k = 0; k < 16; ++k) job->init[k] = (k % 5 == 0) ? 1.0 : 0.0;
+      p.seg_begin[2 * i] = p.seg_end[2 * i] = (int32_t)sm;
+      p.seg_begin[2 * i + 1] = p.seg_end[2 * i + 1] = (int32_t)ss;
+    }
+    return;
+  }
+  const int bw = T.bw, npix = T.bw * T.bh, half = 4;
+  const uint16_t* __restrict__ C = p.crops + T.crop;
+  const double anchor = __ddiv_rn((double)T.anchor, 1000.0);
+  double* __restrict__ M = p.raw + sm * 3;
+  double* __restrict__ S = p.raw + ss * 3;
+  double* __restrict__ Cs = p.cpts + (size_t)i * A * 3;
+  const unsigned long long F = (1ull << POSE_KEY_BITS) - 1;
+  // clouds (LL.cpp:57-99), row-major over the box: three compactions in one 64-bit scan (counts < 2^21 each)
+  unsigned long long base = 0;
+  for (int t0 = 0; t0 < npix; t0 += POSE_THREADS) {
+    const int k = t0 + tid;
+    bool fm = false, fs = false, fc = false;
+    double mx = 0, my = 0, mz = 0, sx = 0, sy = 0, sz = 0;
+    if (k < npix) {
+      const int r = k / bw, q = k - r * bw;
+      const uint16_t md = C[k];
+      bool in = md > 0;
+      // the dilated mask: every non-zero pixel lies inside the box, so the crop holds the whole 9 x 9 neighbourhood
+      for (int dy = -half; dy <= half && !in; ++dy) {
+        const int rr = r + dy;
+        if (rr < 0 || rr >= T.bh) continue;
+        for (int dx = -half; dx <= half; ++dx) {
+          const int qq = q + dx;
+          if (qq >= 0 && qq < bw && C[rr * bw + qq] > 0) { in = true; break; }
+        }
+      }
+      if (in) {
+        const int mr = r + T.by, mc = q + T.bx;
+        int sr = r + m.y - half; if (sr < 0) sr = 0;
+        int sc = q + m.x - half; if (sc < 0) sc = 0;
+        if (md > 0) {
+          fm = true;
+          mz = __ddiv_rn((double)md, 1000.0);
+          mx = pose_backproject(mc, T.K[2], T.K[0], mz);
+          my = pose_backproject(mr, T.K[5], T.K[4], mz);
+        }
+        const uint16_t sd = p.scene[(size_t)sr * p.scols + sc];
+        if (sd > 0) {
+          sz = __ddiv_rn((double)sd, 1000.0);
+          sx = pose_backproject(sc, p.sK[2], p.sK[0], sz);
+          sy = pose_backproject(sr, p.sK[5], p.sK[4], sz);
+          fs = p.use_scene != 0;
+          fc = md > 0 && fabs(__dsub_rn(sz, anchor)) < 0.4;
+        }
+      }
+    }
+    const unsigned long long mine = (fm ? 1ull : 0ull) | (fs ? 1ull << POSE_KEY_BITS : 0ull) | (fc ? 1ull << (2 * POSE_KEY_BITS) : 0ull);
+    unsigned long long excl, agg;
+    Scan(tmp.scan).ExclusiveSum(mine, excl, agg);
+    const unsigned long long at = base + excl;
+    if (fm) { const size_t o = 3 * (at & F); M[o] = mx; M[o + 1] = my; M[o + 2] = mz; }
+    if (fs) { const size_t o = 3 * ((at >> POSE_KEY_BITS) & F); S[o] = sx; S[o + 1] = sy; S[o + 2] = sz; }
+    if (fc) { const size_t o = 3 * (at >> (2 * POSE_KEY_BITS)); Cs[o] = sx; Cs[o + 1] = sy; Cs[o + 2] = sz; }
+    base += agg;
+    __syncthreads();
+  }
+  const int nm = (int)(base & F), ns = (int)((base >> POSE_KEY_BITS) & F), nc = (int)(base >> (2 * POSE_KEY_BITS));
+  // per-axis minima of both clouds (exact in any order)
+  for (int c = 0; c < 6; ++c) {
+    const double* P = c < 3 ? M : S;
+    const int n = c < 3 ? nm : ns;
+    double v = INFINITY;
+    for (int j = tid; j < n; j += POSE_THREADS) v = fmin(v, P[3 * j + c % 3]);
+    v = Reduce(tmp.reduce).Reduce(v, cub::Min());
+    if (tid == 0) s_min[c] = v;
+    __syncthreads();
+  }
+  if (tid < 6) {
+    // centroids: one thread per sum, in the host's sequential order (LL.cpp:71-104)
+    const double* P = tid < 3 ? M : Cs;
+    const int n = tid < 3 ? nm : nc;
+    double s = 0.0;
+    for (int j = 0; j < n; ++j) s = __dadd_rn(s, P[3 * j + tid % 3]);
+    s_sum[tid] = s;
+  } else if (tid >= 32) {
+    // voxel keys floor((p - (min - v/2)) / v) of PointCloud::VoxelDownSample(0.0025), packed (a, b, c)
+    for (int c2 = 0; c2 < 2; ++c2) {
+      const double* P = c2 ? S : M;
+      const int n = c2 ? ns : nm;
+      const size_t slot = c2 ? ss : sm;
+      double o[3];
+      for (int c = 0; c < 3; ++c) o[c] = __dsub_rn(s_min[3 * c2 + c], 0.00125);
+      for (int j = tid - 32; j < n; j += POSE_THREADS - 32) {
+        unsigned long long key = 0;
+        for (int c = 0; c < 3; ++c) {
+          const double v = floor(__ddiv_rn(__dsub_rn(P[3 * j + c], o[c]), 0.0025));
+          unsigned long long a = (unsigned long long)(long long)v;
+          if (!(v >= 0.0 && v <= (double)F)) { atomicExch(p.err, 1); a = F; }
+          key = (key << POSE_KEY_BITS) | a;
+        }
+        p.keys[slot + j] = key;
+        p.vals[slot + j] = j;
+      }
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int k = 0; k < 16; ++k) job->init[k] = (k % 5 == 0) ? 1.0 : 0.0;
+    for (int c = 0; c < 3; ++c) {
+      const double cm = __ddiv_rn(s_sum[c], (double)nm), cs = __ddiv_rn(s_sum[3 + c], (double)nc);  // 0/0 -> NaN as the host
+      job->init[4 * c + 3] = __dsub_rn(cs, cm);
+    }
+    job->src_first = job->tgt_first = (int32_t)sm;
+    job->src_count = job->tgt_count = 0;  // k_pose_voxel sets the counts
+    p.seg_begin[2 * i] = (int32_t)sm; p.seg_end[2 * i] = (int32_t)sm + nm;
+    p.seg_begin[2 * i + 1] = (int32_t)ss; p.seg_end[2 * i + 1] = (int32_t)ss + ns;
+  }
+}
+
+// One CTA per cloud slot: mean of every occupied voxel, summed in sorted order (voxel_down_sample).
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals,
+                                                             const int32_t* __restrict__ seg_begin, const int32_t* __restrict__ seg_end,
+                                                             const double* __restrict__ raw, double* __restrict__ pts, IcpJob* jobs,
+                                                             int use_scene) {
+  typedef cub::BlockScan<int, POSE_THREADS> Scan;
+  __shared__ typename Scan::TempStorage tmp;
+  const int s = blockIdx.x, tid = threadIdx.x;
+  const int b = seg_begin[s], n = seg_end[s] - b;
+  const unsigned long long* K = keys + b;
+  const int32_t* V = vals + b;
+  const double* P = raw + (size_t)b * 3;
+  double* O = pts + (size_t)b * 3;
+  int nv = 0;
+  for (int t0 = 0; t0 < n; t0 += POSE_THREADS) {
+    const int j = t0 + tid;
+    const bool start = j < n && (j == 0 || K[j] != K[j - 1]);
+    int excl, agg;
+    Scan(tmp).ExclusiveSum(start ? 1 : 0, excl, agg);
+    if (start) {
+      double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+      int e = j;
+      const unsigned long long key = K[j];
+      for (; e < n && K[e] == key; ++e) {
+        const double* q = P + 3 * (size_t)V[e];
+        a0 = __dadd_rn(a0, q[0]); a1 = __dadd_rn(a1, q[1]); a2 = __dadd_rn(a2, q[2]);
+      }
+      const double c = (double)(e - j);
+      double* o = O + 3 * (size_t)(nv + excl);
+      o[0] = __ddiv_rn(a0, c); o[1] = __ddiv_rn(a1, c); o[2] = __ddiv_rn(a2, c);
+    }
+    nv += agg;
+    __syncthreads();
+  }
+  if (tid == 0) {
+    IcpJob* job = jobs + s / 2;
+    if (s % 2 == 0) {
+      job->src_first = b; job->src_count = nv;
+      if (!use_scene) { job->tgt_first = b; job->tgt_count = nv; }  // the reference registers against the model cloud
+    } else if (use_scene) {
+      job->tgt_first = b; job->tgt_count = nv;
+    }
+  }
+}
+
+struct TplHost {
+  bool set = false;
+  int box[4] = {0, 0, 0, 0};
+  uint16_t anchor = 0;
+  float K[9], R[9], t[3];
+  std::vector<uint16_t> crop;
+};
+
+struct lm_pose_stage {
+  std::vector<TplHost> tpl;
+  std::vector<int32_t> class_begin;
+  bool dirty = true;           // the device copy of the renders is stale
+  int64_t area_max = 0;        // largest crop
+  PoseTpl* d_tpl = nullptr; uint16_t* d_crops = nullptr; int32_t* d_class_begin = nullptr;
+  // per-frame buffers, sized for (bound, area_max)
+  int cap_bound = 0; int64_t cap_area = 0;
+  double* d_raw = nullptr; double* d_cpts = nullptr; double* d_pts = nullptr; double* d_nrm = nullptr;
+  unsigned long long* d_keys[2] = {nullptr, nullptr};
+  int32_t* d_vals[2] = {nullptr, nullptr};
+  int32_t* d_seg = nullptr;
+  IcpJob* d_jobs = nullptr; IcpOut* d_outs = nullptr;
+  int32_t* d_err = nullptr;
+  void* d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
+  IcpOut* h_outs = nullptr; int32_t* h_err = nullptr;
+  // the enqueued frame
+  int bound = 0, srows = 0, scols = 0;
+};
+
+static void pose_free_frame(lm_pose_stage* s) {
+  cudaFree(s->d_raw); cudaFree(s->d_cpts); cudaFree(s->d_pts); cudaFree(s->d_nrm);
+  cudaFree(s->d_keys[0]); cudaFree(s->d_keys[1]); cudaFree(s->d_vals[0]); cudaFree(s->d_vals[1]);
+  cudaFree(s->d_seg); cudaFree(s->d_jobs); cudaFree(s->d_outs); cudaFree(s->d_sort_tmp);
+  cudaFreeHost(s->h_outs);
+  s->d_raw = s->d_cpts = s->d_pts = s->d_nrm = nullptr;
+  s->d_keys[0] = s->d_keys[1] = nullptr; s->d_vals[0] = s->d_vals[1] = nullptr;
+  s->d_seg = nullptr; s->d_jobs = nullptr; s->d_outs = nullptr; s->d_sort_tmp = nullptr; s->sort_tmp_bytes = 0;
+  s->h_outs = nullptr;
+  s->cap_bound = 0; s->cap_area = 0;
+}
+
+lm_pose_stage* pose_stage_create() { return new lm_pose_stage(); }
+
+void pose_stage_destroy(lm_pose_stage* s) {
+  if (!s) return;
+  pose_free_frame(s);
+  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_err);
+  cudaFreeHost(s->h_err);
+  delete s;
+}
+
+void pose_stage_clear(lm_pose_stage* s) {
+  s->tpl.clear();
+  s->class_begin.clear();
+  s->area_max = 0;
+  s->dirty = true;
+}
+
+int pose_stage_register(lm_pose_stage* s, const int32_t* class_begin, int n_classes, int64_t first, int64_t n,
+                        const uint16_t* const* depths, int rows, int cols, const float* K, const float* R, const float* t) {
+  const int64_t G = class_begin[n_classes];
+  if (!depths || !K || !R || !t) return lm_fail(LM_E_INVALID, "null argument");
+  if (n < 1 || first < 0 || first + n > G)
+    return lm_fail(LM_E_INVALID, "renders [%lld, %lld) outside the bank's %lld templates", (long long)first, (long long)(first + n), (long long)G);
+  if (rows <= 0 || cols <= 0) return lm_fail(LM_E_INVALID, "empty render size %d x %d", rows, cols);
+  std::vector<TplHost> add((size_t)n);
+  for (int64_t i = 0; i < n; ++i) {
+    const uint16_t* d = depths[i];
+    if (!d) return lm_fail(LM_E_INVALID, "depths[%lld] is null", (long long)i);
+    TplHost& h = add[(size_t)i];
+    model_box(d, rows, cols, h.box);
+    if (h.box[2] == 0) return lm_fail(LM_E_INVALID, "render of template %lld has no non-zero pixel", (long long)(first + i));
+    if ((int64_t)h.box[2] * h.box[3] >= (1ll << POSE_KEY_BITS))
+      return lm_fail(LM_E_INVALID, "render of template %lld: box of %d x %d pixels is too large", (long long)(first + i), h.box[2], h.box[3]);
+    h.anchor = d[(size_t)(rows / 2) * cols + cols / 2];
+    h.crop.resize((size_t)h.box[2] * h.box[3]);
+    for (int r = 0; r < h.box[3]; ++r)
+      memcpy(h.crop.data() + (size_t)r * h.box[2], d + (size_t)(r + h.box[1]) * cols + h.box[0], sizeof(uint16_t) * h.box[2]);
+    memcpy(h.K, K + 9 * i, sizeof(h.K));
+    memcpy(h.R, R + 9 * i, sizeof(h.R));
+    memcpy(h.t, t + 3 * i, sizeof(h.t));
+    h.set = true;
+  }
+  if ((int64_t)s->tpl.size() != G) s->tpl.assign((size_t)G, TplHost());
+  s->class_begin.assign(class_begin, class_begin + n_classes + 1);
+  for (int64_t i = 0; i < n; ++i) s->tpl[(size_t)(first + i)] = std::move(add[(size_t)i]);
+  s->area_max = 0;
+  for (const TplHost& h : s->tpl) s->area_max = std::max<int64_t>(s->area_max, (int64_t)h.crop.size());
+  s->dirty = true;
+  return LM_OK;
+}
+
+bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel) {
+  if (s->tpl.empty()) return false;
+  for (int64_t k = 0; k < n_sel; ++k)
+    if (sel[k] < 0 || sel[k] >= (int64_t)s->tpl.size() || !s->tpl[(size_t)sel[k]].set) return false;
+  return true;
+}
+
+static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
+  std::vector<PoseTpl> tp(s->tpl.size());
+  int64_t pool = 0;
+  for (size_t g = 0; g < s->tpl.size(); ++g) {
+    const TplHost& h = s->tpl[g];
+    PoseTpl& d = tp[g];
+    d.bx = h.box[0]; d.by = h.box[1]; d.bw = h.box[2]; d.bh = h.box[3];
+    d.crop = pool;
+    d.anchor = h.anchor;
+    for (int k = 0; k < 9; ++k) d.K[k] = h.set ? h.K[k] : 0.f;
+    pool += (int64_t)h.crop.size();
+  }
+  std::vector<uint16_t> crops((size_t)std::max<int64_t>(pool, 1));
+  for (size_t g = 0; g < s->tpl.size(); ++g)
+    if (!s->tpl[g].crop.empty()) memcpy(crops.data() + tp[g].crop, s->tpl[g].crop.data(), s->tpl[g].crop.size() * sizeof(uint16_t));
+  CUI(cudaStreamSynchronize(st));  // an earlier frame may still read the old copy
+  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin);
+  s->d_tpl = nullptr; s->d_crops = nullptr; s->d_class_begin = nullptr;
+  CUI(cudaMalloc(&s->d_tpl, sizeof(PoseTpl) * tp.size()));
+  CUI(cudaMalloc(&s->d_crops, sizeof(uint16_t) * crops.size()));
+  CUI(cudaMalloc(&s->d_class_begin, sizeof(int32_t) * s->class_begin.size()));
+  CUI(cudaMemcpy(s->d_tpl, tp.data(), sizeof(PoseTpl) * tp.size(), cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(s->d_crops, crops.data(), sizeof(uint16_t) * crops.size(), cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(s->d_class_begin, s->class_begin.data(), sizeof(int32_t) * s->class_begin.size(), cudaMemcpyHostToDevice));
+  s->dirty = false;
+  return LM_OK;
+}
+
+static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t area) {
+  if (!s->d_err) {
+    CUI(cudaMalloc(&s->d_err, sizeof(int32_t)));
+    CUI(cudaMallocHost(&s->h_err, sizeof(int32_t)));
+  }
+  if (bound <= s->cap_bound && area <= s->cap_area) return LM_OK;
+  CUI(cudaStreamSynchronize(st));
+  const int B = std::max(bound, s->cap_bound);
+  const int64_t A = std::max(area, s->cap_area);
+  const int64_t slots = 2 * (int64_t)B * A;  // points of every cloud slot
+  if (slots > 0x7FFFFFFFll)
+    return lm_fail(LM_E_CAPACITY, "pose stage: %d survivors x %lld-pixel crops exceed 2^31 points: lower top_k", B, (long long)A);
+  pose_free_frame(s);
+  CUI(cudaMalloc(&s->d_raw, sizeof(double) * 3 * slots));
+  CUI(cudaMalloc(&s->d_pts, sizeof(double) * 3 * slots));
+  CUI(cudaMalloc(&s->d_nrm, sizeof(double) * 3 * slots));
+  CUI(cudaMalloc(&s->d_cpts, sizeof(double) * 3 * (slots / 2)));
+  for (int k = 0; k < 2; ++k) {
+    CUI(cudaMalloc(&s->d_keys[k], sizeof(unsigned long long) * slots));
+    CUI(cudaMalloc(&s->d_vals[k], sizeof(int32_t) * slots));
+  }
+  CUI(cudaMalloc(&s->d_seg, sizeof(int32_t) * 4 * B));
+  CUI(cudaMalloc(&s->d_jobs, sizeof(IcpJob) * B));
+  CUI(cudaMalloc(&s->d_outs, sizeof(IcpOut) * B));
+  CUI(cudaMallocHost(&s->h_outs, sizeof(IcpOut) * B));
+  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
+  cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, s->sort_tmp_bytes, dk, dv, (int)slots, 2 * B, s->d_seg, s->d_seg + 2 * B, 0,
+                                               3 * POSE_KEY_BITS, st));
+  CUI(cudaMalloc(&s->d_sort_tmp, std::max<size_t>(s->sort_tmp_bytes, 16)));
+  s->cap_bound = B;
+  s->cap_area = A;
+  return LM_OK;
+}
+
+int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches) {
+  cudaStream_t st = e.stream;
+  if (s->dirty) {
+    int rc = pose_upload(s, st);
+    if (rc) return rc;
+  }
+  int rc = pose_buffers(s, st, e.bound, s->area_max);
+  if (rc) return rc;
+  const int B = e.bound;
+  const int64_t A = s->cap_area;  // slot stride: the buffers' area, which may exceed the current largest crop
+  PoseParams p;
+  p.surv = e.d_surv; p.counts = e.d_counts;
+  p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
+  p.tpl = s->d_tpl; p.crops = s->d_crops;
+  p.scene = e.d_scene; p.srows = e.srows; p.scols = e.scols;
+  memcpy(p.sK, e.sK, sizeof(p.sK));
+  p.A = (int32_t)A; p.use_scene = e.use_scene_cloud ? 1 : 0;
+  p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
+  p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * B;
+  p.jobs = s->d_jobs; p.err = s->d_err;
+  CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
+  k_pose_cloud<<<B, POSE_THREADS, 0, st>>>(p);
+  // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
+  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
+  cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
+  size_t tmp_bytes = s->sort_tmp_bytes;
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * B * A), 2 * B, p.seg_begin, p.seg_end, 0,
+                                               3 * POSE_KEY_BITS, st));
+  k_pose_voxel<<<2 * B, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
+                                               p.use_scene);
+  // unchanged ICP kernels, launched for the bound: empty jobs fall through
+  dim3 g((unsigned)((A + 127) / 128), (unsigned)B);
+  k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm);
+  k_icp_point_to_plane<<<B, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, 0.01 * 0.01, e.max_iterations, 1e-6, 1e-6);
+  CUI(cudaGetLastError());
+  *launches += 5;  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals, k_icp_point_to_plane
+  CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(B, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  s->bound = B; s->srows = e.srows; s->scols = e.scols;
+  return LM_OK;
+}
+
+int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
+                      float* residual) {
+  if (n > s->bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, s->bound);
+  if (n > POSE_FIRST_FETCH) {
+    CUI(cudaMemcpyAsync(s->h_outs + POSE_FIRST_FETCH, s->d_outs + POSE_FIRST_FETCH, sizeof(IcpOut) * (size_t)(n - POSE_FIRST_FETCH),
+                        cudaMemcpyDeviceToHost, st));
+    CUI(cudaStreamSynchronize(st));
+  }
+  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  const int n_classes = (int)s->class_begin.size() - 1;
+  for (int64_t i = 0; i < n; ++i) {
+    const lm_match& m = surv[i];
+    const int64_t g = (m.class_index >= 0 && m.class_index < n_classes) ? (int64_t)s->class_begin[m.class_index] + m.template_id : -1;
+    if (g < 0 || g >= (int64_t)s->tpl.size() || !s->tpl[(size_t)g].set)
+      return lm_fail(LM_E_STATE, "survivor %lld: template without a registered render", (long long)i);
+    const TplHost& h = s->tpl[(size_t)g];
+    if (m.x + h.box[2] >= s->scols || m.y + h.box[3] >= s->srows) { residual[i] = -1.f; continue; }  // LL.cpp:52-55
+    float base[16];
+    init_base(h.R, h.t, base);
+    compose(s->h_outs[i].T, base, R_out + 9 * i, t_out + 3 * i);
+    residual[i] = (float)s->h_outs[i].fitness;
+  }
   return LM_OK;
 }

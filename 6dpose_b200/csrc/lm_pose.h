@@ -1,0 +1,39 @@
+// lm_pose.h -- internal interface between the detector (linemod_b200.cu) and the on-device pose stage (lm_icp.cu).
+//
+// The pose stage refines the NMS survivors of k_post_nms where they lie: per-template render crops registered once
+// (lm_set_template_renders), then per frame k_pose_cloud (box test, back-projection, centroids, voxel keys), a CUB
+// segmented radix sort of the voxel keys, k_pose_voxel (voxel means) and the unchanged k_icp_normals /
+// k_icp_point_to_plane, all on the detector's stream.  The host composes result = T * init_base after the copy.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "linemod_b200.h"
+
+struct lm_pose_stage;
+
+lm_pose_stage* pose_stage_create();
+void pose_stage_destroy(lm_pose_stage* s);
+// The bank changed: every registered render is dropped.
+void pose_stage_clear(lm_pose_stage* s);
+// Templates [first, first + n) of a bank of G templates (class_begin[n_classes + 1]).
+int pose_stage_register(lm_pose_stage* s, const int32_t* class_begin, int n_classes, int64_t first, int64_t n,
+                        const uint16_t* const* depths, int rows, int cols, const float* K, const float* R, const float* t);
+// Every template of the selection has a render.
+bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel);
+
+struct PoseEnqueue {
+  const lm_match* d_surv;     // survivors in pick order (k_post_nms output)
+  const int32_t* d_counts;    // [0] = survivors written
+  const uint16_t* d_scene;    // scene depth, srows x scols u16 mm
+  int srows, scols;
+  float sK[9];
+  int bound;                  // survivors the launches are sized for (top_k, or every survivor k_post_nms may write)
+  int use_scene_cloud;
+  int max_iterations;
+  cudaStream_t stream;
+};
+int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches);
+// After the stream has been synchronised: surv[n] are the survivors (host copy).  Outputs as lm_icp_process_batch.
+int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
+                      float* residual);

@@ -197,6 +197,64 @@ class Detector:
         out, nrec = nat.match_top(quantized, float(threshold), float(iou_threshold), int(top_k))
         return self._to_matches(out), nrec
 
+    # ---- pose stage on the device (the drivers' poseRefine loop over the NMS survivors) ----
+    RENDER_CHUNK = 64
+
+    def setTemplateRenders(self, renders):
+        """Model render and pose per template for match_refine: dict class_id -> (depths, K, R, t), every class of
+        the bank.  depths is a sequence of u16 HxW renders, one per template (the drivers' render(model, im_size, K, R,
+        t) of the template's info entry; it may produce them lazily), K / R [n,3,3], t [n,3] mm.  Renders are
+        registered RENDER_CHUNK at a time: only their crops are kept."""
+        from .pose_refine import poseRefine
+        nat = self._ensure_native()
+        first = 0
+        for cid in self._class_order:
+            depths, K, R, t = renders[cid]
+            n = self.bank.num_templates(cid)
+            K = np.asarray(K, np.float32).reshape(-1, 3, 3)
+            R = np.asarray(R, np.float32).reshape(-1, 3, 3)
+            t = np.asarray(t, np.float32).reshape(-1, 3)
+            if not (K.shape[0] == R.shape[0] == t.shape[0] == n):
+                raise ValueError("class %s: K / R / t for %d templates, the bank has %d" % (cid, K.shape[0], n))
+            chunk, got = [], 0
+            for d in depths:
+                chunk.append(poseRefine._depth(d, "render"))
+                if len(chunk) == self.RENDER_CHUNK:
+                    nat.set_template_renders(first + got, chunk, K[got:got + len(chunk)], R[got:got + len(chunk)], t[got:got + len(chunk)])
+                    got += len(chunk)
+                    chunk = []
+            if chunk:
+                nat.set_template_renders(first + got, chunk, K[got:got + len(chunk)], R[got:got + len(chunk)], t[got:got + len(chunk)])
+                got += len(chunk)
+            if got != n:
+                raise ValueError("class %s: %d renders for %d templates" % (cid, got, n))
+            first += n
+
+    def match_refine(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
+                     use_scene_cloud=False, masks=[]):
+        """match + nms + poseRefine().process for every survivor, as the drivers do (linemod_and_levelup_test.py:
+        324-367), in one chain on the GPU: front-end, match, NMS/top-k, cloud building, normals and ICP.  Needs
+        setTemplateRenders.  Returns [(Match, poseRefine)] in pick order; each poseRefine is in the state
+        refine_matches leaves it in (residual -1, R / t None where the model box does not fit the frame)."""
+        from .pose_refine import poseRefine
+        if len(sources) != 2:
+            raise RuntimeError("sources.size() == modalities.size()")
+        sources = [self._as_source(s, i) for i, s in enumerate(sources)]
+        self._whole_bank_only("match_refine()")
+        sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
+        nat = self._select(list(class_ids))
+        out, R, t, res, _ = nat.match_pose(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold),
+                                           int(top_k), int(max_iterations), bool(use_scene_cloud))
+        pairs = []
+        for i, m in enumerate(self._to_matches(out)):
+            p = poseRefine()
+            p._residual = float(res[i])
+            if res[i] != -1.0:
+                p._R = R[i].copy()
+                p._t = t[i].reshape(3, 1).copy()
+            pairs.append((m, p))
+        return pairs
+
     def _to_matches(self, out):
         # column-wise conversion + map(): building ~1400 objects field by field from numpy scalars costs 10x the
         # GPU match itself

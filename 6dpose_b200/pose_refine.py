@@ -35,6 +35,13 @@ class poseRefine:
             raise RuntimeError("%s must have %s elements" % (name, "x".join(map(str, shape))))
         return np.ascontiguousarray(a).reshape(shape)
 
+    @staticmethod
+    def _depth(a, name):
+        a = np.asarray(a)
+        if a.dtype != np.uint16 or a.ndim != 2:
+            raise TypeError("%s must be a uint16 HxW depth image (mm)" % name)
+        return a
+
     def process(self, sceneDepth, modelDepth, sceneK, modelK, modelR, modelT, detectX, detectY):
         scene = np.asarray(sceneDepth)
         model = np.asarray(modelDepth)

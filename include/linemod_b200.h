@@ -184,6 +184,37 @@ int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out,
 int lm_match_top(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols, float threshold,
                  double iou_threshold, int top_k, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records);
 
+/* Pose stage on the device: poseRefine::process for every NMS survivor, behind lm_enqueue_post on the same stream.
+ * The drivers refine each survivor against render(model, K, R, t) of the matched template's info entry
+ * (linemod_and_levelup_test.py:351-367; linemod_ros/detect.py:113-130) -- a constant of the template, registered once.
+ * Registration keeps what poseRefine derives from the full render: the 9x9-dilated box of its non-zero pixels
+ * (LL.cpp:43-50), the render cropped to that box and the anchor depth render[rows/2][cols/2]; only those, and K, go to
+ * the device.  Per frame the device builds the clouds (scan-compacted in row-major order), the centroids and the
+ * voxel down-sampling (CUB segmented radix sort + voxel means) and runs the ICP kernels; only the survivors and their
+ * poses come back.  Clouds, initial guesses, R, t and residual are bit-identical to lm_icp_process_batch on the same
+ * survivors and renders, NaN patterns included.
+ *   lm_set_template_renders  templates [first, first+n) of the bank (bank order, as lm_set_boxes); depths[i] is
+ *                            rows x cols u16 mm, K + 9i / R + 9i row-major f32, t + 3i f32 mm.  May be called in
+ *                            several ranges.  LM_E_INVALID for a render without a non-zero pixel or a range outside
+ *                            the bank.  Loading another bank drops the renders.
+ *   lm_enqueue_pose          after lm_enqueue_post, same stream, no host synchronisation.  The scene depth is that of
+ *                            the frame lm_upload_images uploaded; sceneK is 9 f32.  LM_E_STATE without renders for
+ *                            every selected template, for a frame from lm_upload_quantized / lm_bind_quantized_device
+ *                            (no depth), or without lm_enqueue_post.  Buffers are sized for top_k survivors (every
+ *                            survivor: 1024) times the largest registered crop.  The first call after a registration
+ *                            or with a larger top_k uploads the crops / grows the buffers and synchronises the stream:
+ *                            with a connected peer exchange, every rank enqueues its match before any rank enqueues
+ *                            the post and pose stages.
+ *   lm_complete_pose         waits.  out[n_out] are the survivors in pick order (as lm_complete_post); R_out + 9i,
+ *                            t_out + 3i, residual[i] are lm_icp_process_batch's outputs for survivor i (residual -1 and
+ *                            R/t untouched on the early return of LL.cpp:52-55).  When the records outgrew the result
+ *                            block, the refinement, the NMS and the pose stage run again before it returns. */
+int lm_set_template_renders(lm_detector* d, int64_t first, int64_t n, const uint16_t* const* depths, int rows, int cols,
+                            const float* K, const float* R, const float* t);
+int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iterations, int use_scene_cloud);
+int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
+                     int64_t* n_out, int64_t* n_records);
+
 /* Convenience = lm_upload_quantized + lm_run + lm_fetch_records + lm_finish (single GPU):
  * Detector::match after quantization. */
 int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,
@@ -216,7 +247,8 @@ int lm_set_timing(lm_detector* d, int slots);
 int lm_stage_times(lm_detector* d, float* out8);
 /* The CUDA stream all work of this handle is issued on (cudaStream_t as void*). */
 void* lm_stream(lm_detector* d);
-/* Number of kernel launches issued by this handle since creation. */
+/* Number of kernel launches issued by this handle since creation (the pose stage's CUB segmented sort counts as one;
+ * a frame's pose stage is 5, whatever its survivor count). */
 int64_t lm_launch_count(lm_detector* d);
 
 /* ---- poseRefine (reference: linemodLevelup/linemodLevelup.h:8-19, linemodLevelup.cpp:27-155) ---- */
