@@ -31,6 +31,7 @@ SYMBOLS = [
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
+    "lm_icp_set_capture", "lm_icp_capture",
 ]
 
 _lib = None
@@ -112,6 +113,8 @@ def load():
     L.lm_icp_set_use_scene_cloud.argtypes = [vp, c_int]
     L.lm_icp_launch_count.argtypes = [vp]
     L.lm_icp_launch_count.restype = c_i64
+    L.lm_icp_set_capture.argtypes = [vp, c_int]
+    L.lm_icp_capture.argtypes = [vp, c_int, c_int, vp, c_i64]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export a declared symbol
     _lib = L
@@ -495,6 +498,28 @@ class NativeIcp:
 
     def set_use_scene_cloud(self, on):
         check(self._L.lm_icp_set_use_scene_cloud(self._h, 1 if on else 0))
+
+    def set_capture(self, on):
+        check(self._L.lm_icp_set_capture(self._h, 1 if on else 0))
+
+    def _capture_item(self, hyp, what, out):
+        check(self._L.lm_icp_capture(self._h, int(hyp), what, out.ctypes.data_as(ctypes.c_void_p), out.nbytes))
+        return out
+
+    def capture(self, hyp):
+        """What the kernels saw and kept for hypothesis `hyp` of the last process_batch with capture on (see
+        lm_icp_capture): source / target [n,3] f64, normals [nt,3] f64, init [4,4] f64, T [4,4] f64, fitness, rmse,
+        iterations, knn [nt,30] int32 (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence)."""
+        n, nt = self._capture_item(hyp, 0, np.zeros(2, np.int32)).tolist()
+        res = self._capture_item(hyp, 5, np.zeros(19, np.float64))
+        return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
+                    target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)),
+                    normals=self._capture_item(hyp, 3, np.zeros((nt, 3), np.float64)),
+                    init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
+                    T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
+                    knn=self._capture_item(hyp, 6, np.zeros((nt, 30), np.int32)),
+                    corr_first=self._capture_item(hyp, 7, np.zeros(n, np.int32)),
+                    corr_last=self._capture_item(hyp, 8, np.zeros(n, np.int32)))
 
     def last_stats(self):
         a = (ctypes.c_double * 4)()

@@ -128,8 +128,9 @@ __device__ __forceinline__ void knn_scan_tile(const double (*s_t)[3], int t0, in
   }
 }
 
+// knn_out (capture only, else null): ICP_KNN indices per target point, in kept order, padded with -1.
 __global__ void __launch_bounds__(128) k_icp_normals(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
-                                                     double* __restrict__ normals) {
+                                                     double* __restrict__ normals, int32_t* __restrict__ knn_out) {
   __shared__ double s_t[ICP_TILE][3];
   const IcpJob job = jobs[blockIdx.y];
   const int n = job.tgt_count;
@@ -177,6 +178,10 @@ __global__ void __launch_bounds__(128) k_icp_normals(const IcpJob* __restrict__ 
     }
   }
   if (!live) return;
+  if (knn_out) {
+    int32_t* ko = knn_out + ((size_t)job.tgt_first + i) * ICP_KNN;
+    for (int k = 0; k < ICP_KNN; ++k) ko[k] = k < have ? bi[k] : -1;
+  }
   double* out = normals + ((size_t)job.tgt_first + i) * 3;
   if (have < 3) { out[0] = 0; out[1] = 0; out[2] = 1; return; }
   // cumulants exactly as Open3D's ComputeNormal: E[x], E[x x^T], covariance = E[x x^T] - E[x] E[x]^T
@@ -231,9 +236,12 @@ __device__ void solve6(double A[6][6], double b[6], double x[6]) {
     for (int i = 0; i < 6; ++i) x[i] = 0.0;
 }
 
+// corr_out (capture only, else null): 2 slots per source point, the correspondence (-1: none) of pass 0 and of the
+// latest later pass.
 __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
                                                                   const double* __restrict__ normals, IcpOut* __restrict__ outs,
-                                                                  double max_d2, int max_iter, double rel_fitness, double rel_rmse) {
+                                                                  double max_d2, int max_iter, double rel_fitness, double rel_rmse,
+                                                                  int32_t* __restrict__ corr_out) {
   __shared__ double s_t[ICP_TILE][3];
   __shared__ double s_red[ICP_THREADS / 32][ICP_NACC];
   __shared__ double s_T[16];
@@ -294,6 +302,7 @@ __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob
           }
         }
       }
+      if (corr_out && live) corr_out[((size_t)job.src_first + i) * 2 + (pass > 0)] = bj;
       if (bj >= 0) {
         const double vx = Q[3 * bj], vy = Q[3 * bj + 1], vz = Q[3 * bj + 2];
         const double nx = Nm[3 * bj], ny = Nm[3 * bj + 1], nz = Nm[3 * bj + 2];
@@ -379,6 +388,16 @@ struct lm_icp {
   double last_rmse = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   float last_kernel_us = 0;
+  // lm_icp_set_capture: the kernels' intermediate results of the last lm_icp_process_batch
+  bool capture = false;
+  int32_t* d_knn = nullptr; int32_t* d_corr = nullptr; size_t cap_capture = 0;
+  struct {
+    std::vector<IcpJob> jobs;
+    std::vector<int> job_of;  // per hypothesis, -1: early return
+    std::vector<IcpOut> outs;
+    std::vector<double> pts, nrm;
+    std::vector<int32_t> knn, corr;
+  } cap;
 };
 
 extern "C" int lm_icp_create(int device, lm_icp** out) {
@@ -403,6 +422,7 @@ extern "C" void lm_icp_destroy(lm_icp* h) {
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream);
   cudaFree(h->d_pts); cudaFree(h->d_nrm); cudaFree(h->d_jobs); cudaFree(h->d_outs);
+  cudaFree(h->d_knn); cudaFree(h->d_corr);
   cudaFreeHost(h->h_outs);
   cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1);
   cudaStreamDestroy(h->stream);
@@ -626,17 +646,26 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
       h->cap_houts = std::max<size_t>(jobs.size() * 2, 16);
       CUI(cudaMallocHost(&h->h_outs, h->cap_houts * sizeof(IcpOut)));
     }
+    if (h->capture && npts > h->cap_capture) {
+      cudaFree(h->d_knn); cudaFree(h->d_corr);
+      h->d_knn = nullptr; h->d_corr = nullptr; h->cap_capture = 0;
+      CUI(cudaMalloc(&h->d_knn, npts * ICP_KNN * sizeof(int32_t)));
+      CUI(cudaMalloc(&h->d_corr, npts * 2 * sizeof(int32_t)));
+      h->cap_capture = npts;
+    }
+    int32_t* knn_out = h->capture ? h->d_knn : nullptr;
+    int32_t* corr_out = h->capture ? h->d_corr : nullptr;
     cudaStream_t st = h->stream;
     if (npts) CUI(cudaMemcpyAsync(h->d_pts, all.data(), npts * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
     CUI(cudaMemcpyAsync(h->d_jobs, jobs.data(), jobs.size() * sizeof(IcpJob), cudaMemcpyHostToDevice, st));
     CUI(cudaEventRecord(h->ev0, st));
     if (max_count > 0) {
       dim3 g((unsigned)((max_count + 127) / 128), (unsigned)jobs.size());
-      k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm);
+      k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, knn_out);
       ++h->launches;
     }
     k_icp_point_to_plane<<<(unsigned)jobs.size(), ICP_THREADS, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, h->d_outs, 0.01 * 0.01,
-                                                                      max_iterations, 1e-6, 1e-6);
+                                                                      max_iterations, 1e-6, 1e-6, corr_out);
     ++h->launches;
     CUI(cudaEventRecord(h->ev1, st));
     CUI(cudaMemcpyAsync(h->h_outs, h->d_outs, jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
@@ -645,6 +674,21 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     float ms = 0;
     CUI(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
     h->last_kernel_us = ms * 1000.f;
+  }
+  if (h->capture) {
+    auto& c = h->cap;
+    c.jobs = jobs;
+    c.job_of = job_of;
+    c.outs.assign(h->h_outs, h->h_outs + (jobs.empty() ? 0 : jobs.size()));
+    c.pts = all;
+    c.nrm.assign(npts * 3, 0.0);
+    c.knn.assign(npts * ICP_KNN, -1);
+    c.corr.assign(npts * 2, -1);
+    if (npts) {
+      CUI(cudaMemcpy(c.nrm.data(), h->d_nrm, npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(c.knn.data(), h->d_knn, npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(c.corr.data(), h->d_corr, npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    }
   }
   for (int i = 0; i < n_hyp; ++i) {
     if (job_of[i] < 0) { residual[i] = -1.f; continue; }
@@ -680,6 +724,68 @@ extern "C" int64_t lm_icp_launch_count(lm_icp* h) { return h ? h->launches : 0; 
 extern "C" int lm_icp_set_use_scene_cloud(lm_icp* h, int on) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
   h->use_scene_cloud = on != 0;
+  return LM_OK;
+}
+
+extern "C" int lm_icp_set_capture(lm_icp* h, int on) {
+  if (!h) return lm_fail(LM_E_INVALID, "null handle");
+  h->capture = on != 0;
+  h->cap.job_of.clear();
+  return LM_OK;
+}
+
+extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t cap) {
+  if (!h || !out) return lm_fail(LM_E_INVALID, "null argument");
+  const auto& c = h->cap;
+  if (hyp < 0 || hyp >= (int)c.job_of.size())
+    return lm_fail(LM_E_INVALID, "hypothesis %d outside the %d of the last captured call", hyp, (int)c.job_of.size());
+  if (c.job_of[hyp] < 0) return lm_fail(LM_E_STATE, "hypothesis %d took the early return: nothing was captured", hyp);
+  const IcpJob& j = c.jobs[(size_t)c.job_of[hyp]];
+  const IcpOut& o = c.outs[(size_t)c.job_of[hyp]];
+  const void* src = nullptr;
+  int64_t bytes = 0;
+  std::vector<int32_t> tmp;
+  double res[19];
+  switch (what) {
+    case LM_ICP_CAPTURE_COUNTS:
+      tmp = {j.src_count, j.tgt_count};
+      src = tmp.data(); bytes = 2 * sizeof(int32_t);
+      break;
+    case LM_ICP_CAPTURE_SOURCE:
+      src = c.pts.data() + (size_t)j.src_first * 3; bytes = (int64_t)j.src_count * 3 * sizeof(double);
+      break;
+    case LM_ICP_CAPTURE_TARGET:
+      src = c.pts.data() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double);
+      break;
+    case LM_ICP_CAPTURE_NORMALS:
+      src = c.nrm.data() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double);
+      break;
+    case LM_ICP_CAPTURE_INIT:
+      src = j.init; bytes = sizeof(j.init);
+      break;
+    case LM_ICP_CAPTURE_RESULT:
+      memcpy(res, o.T, sizeof(o.T));
+      res[16] = o.fitness; res[17] = o.rmse; res[18] = o.iterations;
+      src = res; bytes = sizeof(res);
+      break;
+    case LM_ICP_CAPTURE_KNN:
+      src = c.knn.data() + (size_t)j.tgt_first * ICP_KNN; bytes = (int64_t)j.tgt_count * ICP_KNN * sizeof(int32_t);
+      break;
+    case LM_ICP_CAPTURE_CORR_FIRST:
+    case LM_ICP_CAPTURE_CORR_LAST: {
+      // slot 1 holds the last pass after any update; without one, pass 0 was the last pass
+      const int slot = (what == LM_ICP_CAPTURE_CORR_LAST && o.iterations > 0) ? 1 : 0;
+      tmp.resize((size_t)j.src_count);
+      for (int i = 0; i < j.src_count; ++i) tmp[(size_t)i] = c.corr[((size_t)j.src_first + i) * 2 + slot];
+      src = tmp.data(); bytes = (int64_t)j.src_count * sizeof(int32_t);
+      break;
+    }
+    default:
+      return lm_fail(LM_E_INVALID, "unknown capture item %d", what);
+  }
+  if (cap < bytes) return lm_fail(LM_E_CAPACITY, "capture item %d of hypothesis %d needs %lld bytes, cap is %lld", what, hyp,
+                                  (long long)bytes, (long long)cap);
+  if (bytes) memcpy(out, src, (size_t)bytes);
   return LM_OK;
 }
 
@@ -1115,8 +1221,9 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
                                                p.use_scene);
   // unchanged ICP kernels, launched for the bound: empty jobs fall through
   dim3 g((unsigned)((A + 127) / 128), (unsigned)B);
-  k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm);
-  k_icp_point_to_plane<<<B, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, 0.01 * 0.01, e.max_iterations, 1e-6, 1e-6);
+  k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+  k_icp_point_to_plane<<<B, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, 0.01 * 0.01, e.max_iterations, 1e-6, 1e-6,
+                                                  nullptr);
   CUI(cudaGetLastError());
   *launches += 5;  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals, k_icp_point_to_plane
   CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(B, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));

@@ -283,6 +283,32 @@ int lm_icp_last_stats(lm_icp* h, double* out4);
 int lm_icp_set_use_scene_cloud(lm_icp* h, int on);
 int64_t lm_icp_launch_count(lm_icp* h);
 
+/* ---- introspection of the ICP kernels, used by the stage-by-stage tests ---- */
+/* While capture is on (default off), lm_icp_process_batch keeps, per hypothesis, what its kernels saw and kept in the
+ * last call.  Turning it on or off drops what was kept.  The outputs do not depend on it. */
+int lm_icp_set_capture(lm_icp* h, int on);
+/* Copies item `what` of hypothesis `hyp` of the last call to `out` (cap bytes):
+ *   COUNTS      2 int32: source and target points
+ *   SOURCE      source cloud as uploaded, src x 3 f64;  TARGET the target cloud, tgt x 3 f64
+ *   NORMALS     target normals, tgt x 3 f64
+ *   INIT        initial guess, 16 f64 row-major
+ *   RESULT      19 f64: the final transformation (16, row-major), fitness, rmse, iterations
+ *   KNN         tgt x 30 int32: the neighbours k_icp_normals kept (target indices, kept order, padded with -1)
+ *   CORR_FIRST  src int32: the correspondence (target index, -1: none) of every source point on pass 0
+ *   CORR_LAST   src int32: the same for the last pass the kernel ran (the pass whose fitness and rmse are returned)
+ * LM_E_STATE for a hypothesis that took the early return, LM_E_CAPACITY when cap is too small, LM_E_INVALID for a
+ * hypothesis outside the last captured call. */
+#define LM_ICP_CAPTURE_COUNTS 0
+#define LM_ICP_CAPTURE_SOURCE 1
+#define LM_ICP_CAPTURE_TARGET 2
+#define LM_ICP_CAPTURE_NORMALS 3
+#define LM_ICP_CAPTURE_INIT 4
+#define LM_ICP_CAPTURE_RESULT 5
+#define LM_ICP_CAPTURE_KNN 6
+#define LM_ICP_CAPTURE_CORR_FIRST 7
+#define LM_ICP_CAPTURE_CORR_LAST 8
+int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t cap);
+
 #ifdef __cplusplus
 }
 #endif

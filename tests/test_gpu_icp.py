@@ -80,8 +80,9 @@ def test_icp_against_oracle_on_perturbed_blobs(use_scene):
         assert st["points"] == want["n_points"]
         assert st["iterations"] == want["iterations"], (seed, st, want["iterations"])
         assert abs(float(res[0]) - want["residual"]) <= 1e-6
-        # equidistant neighbours (regular pixel grid) may be ranked differently by the KD-tree and the
-        # brute-force search: a handful of normals move in the last digits, well inside the tolerance
+        # the KD-tree and the kernel's (d^2, index) rule pick different 30th neighbours where neighbours 30 and 31
+        # are nearly tied; tests/test_gpu_icp_stages.py checks that those are the only normals that differ, among the
+        # normals its model can compare (an eigenvalue gap large enough against the covariance's rounding)
         assert abs(st["rmse"] - want["rmse"]) <= 1e-9 + TOL * want["rmse"]
         worst = max(worst, rel(Ro[0], want["R"]), rel(to[0], want["t"]))
     assert worst <= TOL, worst
