@@ -29,6 +29,7 @@ SYMBOLS = [
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
+    "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
     "lm_icp_set_capture", "lm_icp_capture",
@@ -102,6 +103,9 @@ def load():
     L.lm_set_template_renders.argtypes = [vp, c_i64, c_i64, ctypes.POINTER(u16p), c_int, c_int, f32p, f32p, f32p]
     L.lm_enqueue_pose.argtypes = [vp, f32p, c_int, c_int]
     L.lm_complete_pose.argtypes = [vp, vp, f64p, f64p, f32p, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
+    L.lm_enqueue_pose_nms.argtypes = [vp, ctypes.c_double]
+    L.lm_complete_detect.argtypes = [vp, vp, f64p, f64p, f32p, c_i64] + [ctypes.POINTER(c_i64)] * 4
+    L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
     L.lm_icp_destroy.restype = None
@@ -418,6 +422,38 @@ class NativeDetector:
         self.enqueue_pose(sceneK, max_iterations, use_scene_cloud)
         return self.complete_pose()
 
+    # ---- pose NMS behind the pose stage (include/linemod_b200.h, lm_enqueue_pose_nms / lm_complete_detect) ----
+    def enqueue_pose_nms(self, translation_threshold=40.0):
+        check(self._L.lm_enqueue_pose_nms(self._h, float(translation_threshold)))
+
+    def complete_detect(self):
+        """Returns (kept survivors, R [n,3,3] f64, t [n,3] f64 mm, residual [n] f32, counts) in keep order; counts is a
+        dict of survivors (box NMS), posed (survivors with a pose) and records (kept records the box NMS saw)."""
+        cap = 1024
+        out = np.empty(cap, MATCH_DTYPE)
+        Ro = np.empty((cap, 3, 3), np.float64)
+        to = np.empty((cap, 3), np.float64)
+        res = np.empty(cap, np.float32)
+        n, ns, npo, nrec = ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int64()
+        f64p = ctypes.POINTER(ctypes.c_double)
+        check(self._L.lm_complete_detect(self._h, out.ctypes.data_as(ctypes.c_void_p), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
+                                         res.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), cap, ctypes.byref(n), ctypes.byref(ns),
+                                         ctypes.byref(npo), ctypes.byref(nrec)))
+        k = n.value
+        return (out[:k].copy(), Ro[:k].copy(), to[:k].copy(), res[:k].copy(),
+                dict(survivors=int(ns.value), posed=int(npo.value), records=int(nrec.value)))
+
+    def detect(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30, use_scene_cloud=False,
+               translation_threshold=40.0):
+        """upload_images + enqueue + enqueue_post + enqueue_pose + enqueue_pose_nms + complete_detect: RGB-D frame to the
+        object list in one chain on the detector's stream."""
+        self.upload_images(rgb, depth, masks)
+        self.enqueue(threshold)
+        self.enqueue_post(iou_threshold, top_k)
+        self.enqueue_pose(sceneK, max_iterations, use_scene_cloud)
+        self.enqueue_pose_nms(translation_threshold)
+        return self.complete_detect()
+
     def linear_memories(self, level, modality, shape):
         out = np.zeros(shape, np.uint8)
         check(self._L.lm_debug_linear_memories(self._h, level, modality, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)),
@@ -528,3 +564,20 @@ class NativeIcp:
 
     def launch_count(self):
         return int(self._L.lm_icp_launch_count(self._h))
+
+
+def nms_translations(t, score, thr, device=0):
+    """The pose NMS's greedy pass (lm_nms_translations) on caller arrays: t [n,3] f64, score [n] f64, n <= 1024.
+    Returns the kept indices (int64) in keep order."""
+    L = load()
+    t = np.ascontiguousarray(t, np.float64).reshape(-1, 3)
+    score = np.ascontiguousarray(score, np.float64).reshape(-1)
+    if score.shape[0] != t.shape[0]:
+        raise ValueError("%d translations, %d scores" % (t.shape[0], score.shape[0]))
+    n = t.shape[0]
+    keep = np.empty(max(n, 1), np.int32)
+    nk = ctypes.c_int64()
+    f64p = ctypes.POINTER(ctypes.c_double)
+    check(L.lm_nms_translations(int(device), n, t.ctypes.data_as(f64p), score.ctypes.data_as(f64p), float(thr),
+                                keep.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), ctypes.byref(nk)))
+    return keep[:nk.value].astype(np.int64)

@@ -196,6 +196,8 @@ struct lm_detector {
   lm_pose_stage* pose = nullptr;
   bool frame_depth = false;             // the frame came from lm_upload_images: fe_depth holds its depth
   bool pose_pending = false;
+  bool pose_nms_pending = false;        // lm_enqueue_pose_nms: the frame completes through lm_complete_detect
+  double pose_nms_thr = 40.0;
   float pose_sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; int pose_max_iter = 30, pose_use_scene = 0;
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
@@ -1890,8 +1892,10 @@ extern "C" int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k) 
 }
 
 static int enqueue_pose(lm_detector* d);
+static int enqueue_pose_nms(lm_detector* d);
 
-extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records) {
+// fetch = false (lm_complete_detect): wait and retry as usual, but copy no survivor back
+static int complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records, bool fetch) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !n_out) return fail(LM_E_INVALID, "null argument");
   if (!d->post_pending) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
@@ -1900,7 +1904,7 @@ extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int6
   CU(cudaMemcpyAsync(d->h_post_counts, d->d_post_counts, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
   // the common top-k is small: fetch a first window with the counts, the rest only if there is more
   const int first = 16;
-  CU(cudaMemcpyAsync(d->h_post_out, d->d_post_out, sizeof(lm_match) * first, cudaMemcpyDeviceToHost, st));
+  if (fetch) CU(cudaMemcpyAsync(d->h_post_out, d->d_post_out, sizeof(lm_match) * first, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(d->h_counters, d->d_counters, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
@@ -1925,12 +1929,17 @@ extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int6
       rc = enqueue_pose(d);
       if (rc) return rc;
     }
+    if (d->pose_nms_pending) {  // and so did the pose NMS
+      rc = enqueue_pose_nms(d);
+      if (rc) return rc;
+    }
     d->post_retry = true;
-    rc = lm_complete_post(d, out, cap, n_out, n_records);
+    rc = complete_post(d, out, cap, n_out, n_records, fetch);
     d->post_retry = false;
     return rc;
   }
   *n_out = n;
+  if (!fetch) return LM_OK;
   if (n > cap) return fail(LM_E_CAPACITY, "%lld survivors, capacity %lld", (long long)n, (long long)cap);
   if (n > first) {
     CU(cudaMemcpyAsync(d->h_post_out + first, d->d_post_out + first, sizeof(lm_match) * (size_t)(n - first), cudaMemcpyDeviceToHost, st));
@@ -1938,6 +1947,10 @@ extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int6
   }
   if (n > 0 && out) memcpy(out, d->h_post_out, sizeof(lm_match) * (size_t)n);
   return LM_OK;
+}
+
+extern "C" int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records) {
+  return complete_post(d, out, cap, n_out, n_records, true);
 }
 
 extern "C" int lm_match_top(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols, float threshold,
@@ -1984,6 +1997,7 @@ extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iter
   memcpy(d->pose_sK, sceneK, sizeof(d->pose_sK));
   d->pose_max_iter = max_iterations;
   d->pose_use_scene = use_scene_cloud ? 1 : 0;
+  d->pose_nms_pending = false;  // a new pose stage: any pose NMS enqueued before belongs to an abandoned frame
   int rc = enqueue_pose(d);
   if (rc) return rc;
   d->pose_pending = true;
@@ -1995,10 +2009,43 @@ extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, do
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !n_out || (cap > 0 && (!R_out || !t_out || !residual))) return fail(LM_E_INVALID, "null argument");
   if (!d->pose_pending) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
+  if (d->pose_nms_pending) return fail(LM_E_STATE, "lm_enqueue_pose_nms is pending: complete the frame with lm_complete_detect");
   int rc = lm_complete_post(d, out, cap, n_out, n_records);  // waits; on the capacity retry it runs the pose stage again
   d->pose_pending = false;
   if (rc) return rc;
   return pose_stage_finish(d->pose, d->stream, d->h_post_out, *n_out, R_out, t_out, residual);
+}
+
+static int enqueue_pose_nms(lm_detector* d) {
+  return pose_stage_enqueue_nms(d->pose, d->d_post_out, d->d_post_counts, d->pose_nms_thr, d->stream, &d->launches);
+}
+
+extern "C" int lm_enqueue_pose_nms(lm_detector* d, double translation_threshold_mm) {
+  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (!(translation_threshold_mm >= 0.0)) return fail(LM_E_INVALID, "translation threshold must be >= 0 (NaN given or negative)");
+  if (!d->pose_pending) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
+  if (d->pose_nms_pending) return fail(LM_E_STATE, "lm_enqueue_pose_nms was already called for this frame");
+  CU(cudaSetDevice(d->device));
+  d->pose_nms_thr = translation_threshold_mm;
+  int rc = enqueue_pose_nms(d);
+  if (rc) return rc;
+  d->pose_nms_pending = true;
+  return LM_OK;
+}
+
+extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
+                                  int64_t* n_out, int64_t* n_survivors, int64_t* n_posed, int64_t* n_records) {
+  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (!d || !n_out || (cap > 0 && (!out || !R_out || !t_out || !residual))) return fail(LM_E_INVALID, "null argument");
+  if (!d->pose_nms_pending) return fail(LM_E_STATE, "lm_enqueue_pose_nms has not been called");
+  int64_t n_surv = 0;
+  // waits; on the capacity retry it runs the NMS, the pose stage and the pose NMS again
+  int rc = complete_post(d, nullptr, 0, &n_surv, n_records, false);
+  d->pose_pending = false;
+  d->pose_nms_pending = false;
+  if (rc) return rc;
+  return pose_stage_finish_nms(d->pose, d->stream, out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
 }
 
 extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,

@@ -827,6 +827,7 @@ struct PoseParams {
   int32_t* seg_end;
   IcpJob* jobs;       // [B]
   int32_t* err;       // 1: a cloud spans more than 2^21 voxels along an axis
+  uint8_t* posed;     // [B] 1: survivor i has a template and its box fits the frame (no early return of LL.cpp:52-55)
 };
 
 __device__ __forceinline__ double pose_backproject(int pix, float c, float f, double z) {
@@ -864,6 +865,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
       live = !(m.x + T.bw >= p.scols || m.y + T.bh >= p.srows);  // LL.cpp:52-55
     }
   }
+  if (tid == 0) p.posed[i] = live ? 1 : 0;
   if (!live) {  // block-uniform
     if (tid == 0) {
       job->src_first = job->tgt_first = (int32_t)sm;
@@ -1028,6 +1030,163 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long
   }
 }
 
+// --------------------------------------------------------------------------------------------
+// pose NMS (lm_pose.h): the greedy translation NMS of linemod_ros/detect.py:41-50, 130-131 behind the pose stage
+// --------------------------------------------------------------------------------------------
+// One CTA, one entry per thread (n <= NMS_THREADS).  Each round picks the best live entry with a block-wide arg-max
+// (order-preserving 64-bit score key, lower index on ties), keeps it and drops every live entry j with
+// !(d_ij > thr), d_ij = sqrt((dx*dx + dy*dy) + dz*dz) in float64 with every operation correctly rounded: what
+// np.linalg.norm(ts[i] - ts[order[1:]], axis=1) computes for 3-vectors.  A NaN distance suppresses.
+#define NMS_THREADS 1024  // == LM_POST_MAX, the most survivors k_post_nms writes
+
+struct PoseRt {  // per template of the bank: the pose its render was made with (init_base, LL.cpp:34-38)
+  float R[9], t[3];
+};
+
+struct PoseNmsHead {
+  int32_t kept, survivors, posed, pad;
+};
+
+struct PoseNmsOut {  // one kept pose
+  double R[9], t[3];  // as lm_complete_pose returns them (t in mm)
+  lm_match m;
+  float residual;
+};
+
+// Score order: descending, -0.0 == +0.0, NaN before every number (where argsort()[::-1] puts it).
+__device__ __forceinline__ unsigned long long nms_score_key(double s) {
+  if (s != s) return ~0ull;
+  if (s == 0.0) return 1ull << 63;
+  const unsigned long long b = (unsigned long long)__double_as_longlong(s);
+  return (b >> 63) ? ~b : (b | (1ull << 63));
+}
+
+__device__ __forceinline__ void nms_argmax_warp(unsigned long long& k, int& i) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    const unsigned long long ok = __shfl_down_sync(0xffffffffu, k, d);
+    const int oi = __shfl_down_sync(0xffffffffu, i, d);
+    if (oi >= 0 && (i < 0 || ok > k || (ok == k && oi < i))) { k = ok; i = oi; }
+  }
+}
+
+// Thread i holds entry i: whether it takes part, its score key and its translation.  Returns the number kept on every
+// thread; thread 0 writes the kept indices in keep order to keep[] (if not null), and a kept entry's thread gets its
+// position in rank.
+// blockDim.x == NMS_THREADS.
+__device__ int nms_translations_block(bool cand, unsigned long long key, double tx, double ty, double tz, double thr,
+                                      int32_t* keep, int& rank) {
+  __shared__ unsigned long long s_key[NMS_THREADS / 32];
+  __shared__ int s_idx[NMS_THREADS / 32];
+  __shared__ int s_pick;
+  __shared__ double s_t[3];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  bool live = cand;
+  int kept = 0;
+  rank = -1;
+  for (;;) {
+    unsigned long long bk = live ? key : 0ull;
+    int bi = live ? tid : -1;
+    nms_argmax_warp(bk, bi);
+    if (lane == 0) { s_key[wid] = bk; s_idx[wid] = bi; }
+    __syncthreads();
+    if (wid == 0) {
+      bk = s_key[lane]; bi = s_idx[lane];
+      nms_argmax_warp(bk, bi);
+      if (lane == 0) s_pick = bi;
+    }
+    __syncthreads();
+    const int pick = s_pick;
+    if (pick < 0) break;  // nothing live
+    if (tid == pick) { s_t[0] = tx; s_t[1] = ty; s_t[2] = tz; live = false; rank = kept; }
+    if (tid == 0 && keep) keep[kept] = pick;
+    ++kept;
+    __syncthreads();
+    if (live) {
+      const double dx = __dsub_rn(s_t[0], tx), dy = __dsub_rn(s_t[1], ty), dz = __dsub_rn(s_t[2], tz);
+      const double d = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+      if (!(d > thr)) live = false;
+    }
+  }
+  return kept;
+}
+
+// lm_nms_translations: the same pass on caller arrays, every entry a candidate.
+__global__ void __launch_bounds__(NMS_THREADS) k_nms_translations(int n, const double* __restrict__ t, const double* __restrict__ score,
+                                                                  double thr, int32_t* __restrict__ keep, int32_t* __restrict__ n_keep) {
+  const int i = threadIdx.x;
+  const bool cand = i < n;
+  double tx = 0, ty = 0, tz = 0;
+  unsigned long long key = 0;
+  if (cand) { tx = t[3 * i]; ty = t[3 * i + 1]; tz = t[3 * i + 2]; key = nms_score_key(score[i]); }
+  int rank;
+  const int kept = nms_translations_block(cand, key, tx, ty, tz, thr, keep, rank);
+  if (i == 0) *n_keep = kept;
+}
+
+// init_base entry (k, c) of the template's pose (init_base: only t.z in metres)
+__device__ __forceinline__ float pose_base(const PoseRt& q, int k, int c) {
+  if (k == 3) return c == 3 ? 1.f : 0.f;
+  if (c < 3) return q.R[3 * k + c];
+  return k == 2 ? __fdiv_rn(q.t[2], 1000.0f) : q.t[k];
+}
+
+// (transformation_ * init_base)[r][c], summed as compose() does (LL.cpp:146)
+__device__ __forceinline__ double pose_compose(const double* T, const PoseRt& q, int r, int c) {
+  double s = 0.0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) s = __dadd_rn(s, __dmul_rn(T[4 * r + k], (double)pose_base(q, k, c)));
+  return s;
+}
+
+struct PoseNmsParams {
+  const lm_match* surv;
+  const int32_t* counts;    // [0] survivors written by k_post_nms
+  const uint8_t* posed;     // k_pose_cloud's verdict per survivor
+  const IcpOut* outs;
+  const PoseRt* rt;
+  const int32_t* class_begin;
+  double thr;
+  PoseNmsHead* head;
+  PoseNmsOut* out;          // kept poses in keep order
+};
+
+// Behind k_icp_point_to_plane: candidates are the survivors with a pose, score -(double)residual.
+__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
+  const int i = threadIdx.x;
+  const int n = min(p.counts[0], NMS_THREADS);
+  bool cand = false;
+  double t[3] = {0, 0, 0};
+  float res = 0.f;
+  int g = 0;
+  if (i < n && p.posed[i]) {
+    const lm_match m = p.surv[i];
+    g = p.class_begin[m.class_index] + m.template_id;  // k_pose_cloud found it: in range
+    const PoseRt q = p.rt[g];
+    for (int r = 0; r < 3; ++r) t[r] = __dmul_rn(pose_compose(p.outs[i].T, q, r, 3), 1000.0);
+    res = __double2float_rn(p.outs[i].fitness);
+    cand = true;
+  }
+  const int posed = __syncthreads_count(cand);
+  int rank;
+  const int kept = nms_translations_block(cand, nms_score_key(-(double)res), t[0], t[1], t[2], p.thr, nullptr, rank);
+  if (rank >= 0) {
+    PoseNmsOut o;
+    const PoseRt q = p.rt[g];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) o.R[3 * r + c] = pose_compose(p.outs[i].T, q, r, c);
+    for (int r = 0; r < 3; ++r) o.t[r] = t[r];
+    o.m = p.surv[i];
+    o.residual = res;
+    p.out[rank] = o;
+  }
+  if (i == 0) {
+    PoseNmsHead h;
+    h.kept = kept; h.survivors = p.counts[0]; h.posed = posed; h.pad = 0;
+    *p.head = h;
+  }
+}
+
 struct TplHost {
   bool set = false;
   int box[4] = {0, 0, 0, 0};
@@ -1042,6 +1201,7 @@ struct lm_pose_stage {
   bool dirty = true;           // the device copy of the renders is stale
   int64_t area_max = 0;        // largest crop
   PoseTpl* d_tpl = nullptr; uint16_t* d_crops = nullptr; int32_t* d_class_begin = nullptr;
+  PoseRt* d_rt = nullptr;      // per template: R, t of its render (k_pose_nms composes the poses)
   // per-frame buffers, sized for (bound, area_max)
   int cap_bound = 0; int64_t cap_area = 0;
   double* d_raw = nullptr; double* d_cpts = nullptr; double* d_pts = nullptr; double* d_nrm = nullptr;
@@ -1052,6 +1212,9 @@ struct lm_pose_stage {
   int32_t* d_err = nullptr;
   void* d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
   IcpOut* h_outs = nullptr; int32_t* h_err = nullptr;
+  uint8_t* d_posed = nullptr;
+  // pose NMS output block: PoseNmsHead + NMS_THREADS PoseNmsOut (device, pinned copy)
+  uint8_t* d_nms = nullptr; uint8_t* h_nms = nullptr;
   // the enqueued frame
   int bound = 0, srows = 0, scols = 0;
 };
@@ -1059,8 +1222,9 @@ struct lm_pose_stage {
 static void pose_free_frame(lm_pose_stage* s) {
   cudaFree(s->d_raw); cudaFree(s->d_cpts); cudaFree(s->d_pts); cudaFree(s->d_nrm);
   cudaFree(s->d_keys[0]); cudaFree(s->d_keys[1]); cudaFree(s->d_vals[0]); cudaFree(s->d_vals[1]);
-  cudaFree(s->d_seg); cudaFree(s->d_jobs); cudaFree(s->d_outs); cudaFree(s->d_sort_tmp);
+  cudaFree(s->d_seg); cudaFree(s->d_jobs); cudaFree(s->d_outs); cudaFree(s->d_sort_tmp); cudaFree(s->d_posed);
   cudaFreeHost(s->h_outs);
+  s->d_posed = nullptr;
   s->d_raw = s->d_cpts = s->d_pts = s->d_nrm = nullptr;
   s->d_keys[0] = s->d_keys[1] = nullptr; s->d_vals[0] = s->d_vals[1] = nullptr;
   s->d_seg = nullptr; s->d_jobs = nullptr; s->d_outs = nullptr; s->d_sort_tmp = nullptr; s->sort_tmp_bytes = 0;
@@ -1073,8 +1237,8 @@ lm_pose_stage* pose_stage_create() { return new lm_pose_stage(); }
 void pose_stage_destroy(lm_pose_stage* s) {
   if (!s) return;
   pose_free_frame(s);
-  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_err);
-  cudaFreeHost(s->h_err);
+  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_err); cudaFree(s->d_rt); cudaFree(s->d_nms);
+  cudaFreeHost(s->h_err); cudaFreeHost(s->h_nms);
   delete s;
 }
 
@@ -1128,6 +1292,7 @@ bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel
 
 static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
   std::vector<PoseTpl> tp(s->tpl.size());
+  std::vector<PoseRt> rt(s->tpl.size());
   int64_t pool = 0;
   for (size_t g = 0; g < s->tpl.size(); ++g) {
     const TplHost& h = s->tpl[g];
@@ -1136,15 +1301,19 @@ static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
     d.crop = pool;
     d.anchor = h.anchor;
     for (int k = 0; k < 9; ++k) d.K[k] = h.set ? h.K[k] : 0.f;
+    for (int k = 0; k < 9; ++k) rt[g].R[k] = h.set ? h.R[k] : 0.f;
+    for (int k = 0; k < 3; ++k) rt[g].t[k] = h.set ? h.t[k] : 0.f;
     pool += (int64_t)h.crop.size();
   }
   std::vector<uint16_t> crops((size_t)std::max<int64_t>(pool, 1));
   for (size_t g = 0; g < s->tpl.size(); ++g)
     if (!s->tpl[g].crop.empty()) memcpy(crops.data() + tp[g].crop, s->tpl[g].crop.data(), s->tpl[g].crop.size() * sizeof(uint16_t));
   CUI(cudaStreamSynchronize(st));  // an earlier frame may still read the old copy
-  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin);
-  s->d_tpl = nullptr; s->d_crops = nullptr; s->d_class_begin = nullptr;
+  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_rt);
+  s->d_tpl = nullptr; s->d_crops = nullptr; s->d_class_begin = nullptr; s->d_rt = nullptr;
   CUI(cudaMalloc(&s->d_tpl, sizeof(PoseTpl) * tp.size()));
+  CUI(cudaMalloc(&s->d_rt, sizeof(PoseRt) * rt.size()));
+  CUI(cudaMemcpy(s->d_rt, rt.data(), sizeof(PoseRt) * rt.size(), cudaMemcpyHostToDevice));
   CUI(cudaMalloc(&s->d_crops, sizeof(uint16_t) * crops.size()));
   CUI(cudaMalloc(&s->d_class_begin, sizeof(int32_t) * s->class_begin.size()));
   CUI(cudaMemcpy(s->d_tpl, tp.data(), sizeof(PoseTpl) * tp.size(), cudaMemcpyHostToDevice));
@@ -1178,6 +1347,7 @@ static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t ar
   CUI(cudaMalloc(&s->d_seg, sizeof(int32_t) * 4 * B));
   CUI(cudaMalloc(&s->d_jobs, sizeof(IcpJob) * B));
   CUI(cudaMalloc(&s->d_outs, sizeof(IcpOut) * B));
+  CUI(cudaMalloc(&s->d_posed, B));
   CUI(cudaMallocHost(&s->h_outs, sizeof(IcpOut) * B));
   cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
   cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
@@ -1208,7 +1378,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
   p.A = (int32_t)A; p.use_scene = e.use_scene_cloud ? 1 : 0;
   p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
   p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * B;
-  p.jobs = s->d_jobs; p.err = s->d_err;
+  p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_posed;
   CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
   k_pose_cloud<<<B, POSE_THREADS, 0, st>>>(p);
   // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
@@ -1254,5 +1424,93 @@ int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, i
     compose(s->h_outs[i].T, base, R_out + 9 * i, t_out + 3 * i);
     residual[i] = (float)s->h_outs[i].fitness;
   }
+  return LM_OK;
+}
+
+// ---- pose NMS behind the pose stage ----
+#define NMS_FIRST_FETCH 16
+
+static PoseNmsOut* nms_entries(uint8_t* block) { return reinterpret_cast<PoseNmsOut*>(block + sizeof(PoseNmsHead)); }
+
+int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32_t* d_counts, double thr, cudaStream_t st,
+                           int64_t* launches) {
+  if (s->bound > NMS_THREADS) return lm_fail(LM_E_STATE, "pose stage launched for %d survivors, the pose NMS takes %d", s->bound, NMS_THREADS);
+  const size_t bytes = sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_THREADS;
+  if (!s->d_nms) {
+    CUI(cudaMalloc(&s->d_nms, bytes));
+    CUI(cudaMallocHost(&s->h_nms, bytes));
+  }
+  PoseNmsParams p;
+  p.surv = d_surv; p.counts = d_counts; p.posed = s->d_posed; p.outs = s->d_outs;
+  p.rt = s->d_rt; p.class_begin = s->d_class_begin;
+  p.thr = thr;
+  p.head = reinterpret_cast<PoseNmsHead*>(s->d_nms); p.out = nms_entries(s->d_nms);
+  k_pose_nms<<<1, NMS_THREADS, 0, st>>>(p);
+  CUI(cudaGetLastError());
+  ++*launches;
+  // the header and a first window of kept poses; the rest only if there are more
+  CUI(cudaMemcpyAsync(s->h_nms, s->d_nms, sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_FIRST_FETCH, cudaMemcpyDeviceToHost, st));
+  return LM_OK;
+}
+
+int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
+                          int64_t* n_out, int64_t* n_survivors, int64_t* n_posed) {
+  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  const PoseNmsHead h = *reinterpret_cast<const PoseNmsHead*>(s->h_nms);
+  *n_out = h.kept;
+  if (n_survivors) *n_survivors = h.survivors;
+  if (n_posed) *n_posed = h.posed;
+  if (h.kept > cap) return lm_fail(LM_E_CAPACITY, "%d poses kept, capacity %lld", h.kept, (long long)cap);
+  const PoseNmsOut* e = nms_entries(s->h_nms);
+  if (h.kept > NMS_FIRST_FETCH) {
+    CUI(cudaMemcpyAsync(nms_entries(s->h_nms) + NMS_FIRST_FETCH, nms_entries(s->d_nms) + NMS_FIRST_FETCH,
+                        sizeof(PoseNmsOut) * (size_t)(h.kept - NMS_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
+    CUI(cudaStreamSynchronize(st));
+  }
+  for (int k = 0; k < h.kept; ++k) {
+    if (out) out[k] = e[k].m;
+    memcpy(R_out + 9 * k, e[k].R, sizeof(e[k].R));
+    memcpy(t_out + 3 * k, e[k].t, sizeof(e[k].t));
+    residual[k] = e[k].residual;
+  }
+  return LM_OK;
+}
+
+// Steps 3-5 of the pose NMS on caller arrays (lm_nms_translations): the same device routine as k_pose_nms.
+extern "C" int lm_nms_translations(int device, int64_t n, const double* t, const double* score, double thr, int32_t* keep,
+                                   int64_t* n_keep) {
+  if (!n_keep || n < 0 || (n > 0 && (!t || !score || !keep))) return lm_fail(LM_E_INVALID, "null argument or n < 0");
+  if (!(thr >= 0.0)) return lm_fail(LM_E_INVALID, "translation threshold must be >= 0 (NaN given or negative)");
+  if (n > NMS_THREADS) return lm_fail(LM_E_CAPACITY, "%lld translations, at most %d", (long long)n, NMS_THREADS);
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
+  CUI(cudaSetDevice(device));
+  const size_t m = (size_t)std::max<int64_t>(n, 1);
+  // one allocation: t [m][3], score [m], keep [m], n_keep
+  const size_t bytes = sizeof(double) * 4 * m + sizeof(int32_t) * (m + 1);
+  uint8_t* buf = nullptr;
+  CUI(cudaMalloc(&buf, bytes));
+  double* d_t = reinterpret_cast<double*>(buf);
+  double* d_s = d_t + 3 * m;
+  int32_t* d_keep = reinterpret_cast<int32_t*>(d_s + m);
+  int32_t* d_n = d_keep + m;
+  int32_t got = 0;
+  cudaError_t err = cudaSuccess;
+  if (n > 0) {
+    err = cudaMemcpy(d_t, t, sizeof(double) * 3 * n, cudaMemcpyHostToDevice);
+    if (err == cudaSuccess) err = cudaMemcpy(d_s, score, sizeof(double) * n, cudaMemcpyHostToDevice);
+  }
+  if (err == cudaSuccess) {
+    k_nms_translations<<<1, NMS_THREADS>>>((int)n, d_t, d_s, thr, d_keep, d_n);
+    err = cudaGetLastError();
+  }
+  if (err == cudaSuccess) err = cudaMemcpy(&got, d_n, sizeof(int32_t), cudaMemcpyDeviceToHost);
+  if (err == cudaSuccess && got > 0) err = cudaMemcpy(keep, d_keep, sizeof(int32_t) * got, cudaMemcpyDeviceToHost);
+  cudaFree(buf);
+  if (err != cudaSuccess) return lm_fail(LM_E_CUDA, "lm_nms_translations: %s", cudaGetErrorString(err));
+  *n_keep = got;
   return LM_OK;
 }

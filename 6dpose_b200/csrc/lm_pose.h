@@ -4,6 +4,8 @@
 // (lm_set_template_renders), then per frame k_pose_cloud (box test, back-projection, centroids, voxel keys), a CUB
 // segmented radix sort of the voxel keys, k_pose_voxel (voxel means) and the unchanged k_icp_normals /
 // k_icp_point_to_plane, all on the detector's stream.  The host composes result = T * init_base after the copy.
+// The pose NMS (k_pose_nms, one CTA behind k_icp_point_to_plane) composes the poses on the device instead, runs the
+// greedy translation NMS of linemod_ros/detect.py over them and compacts the kept ones into one output block.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,3 +39,11 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
 // After the stream has been synchronised: surv[n] are the survivors (host copy).  Outputs as lm_icp_process_batch.
 int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
                       float* residual);
+
+// Pose NMS behind pose_stage_enqueue on the same stream: d_surv / d_counts as given to it.  Also enqueues the copy of
+// the output block's header and first entries.
+int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32_t* d_counts, double thr, cudaStream_t st,
+                           int64_t* launches);
+// After the stream has been synchronised: the kept poses in keep order (outputs as lm_complete_detect).
+int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
+                          int64_t* n_out, int64_t* n_survivors, int64_t* n_posed);

@@ -255,6 +255,31 @@ class Detector:
             pairs.append((m, p))
         return pairs
 
+    def detect(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
+               max_iterations=30, use_scene_cloud=False, masks=[]):
+        """The whole frame of linemod_ros/detect.py (:91-141): match, box NMS, poseRefine of every survivor (top_k=0)
+        and the greedy translation NMS nms_norms(ts, -residual, translation_threshold) (:41-50, :130-131), in one chain
+        on the GPU; only the kept objects are copied back.  Needs setTemplateRenders.  Returns [(Match, poseRefine)] in
+        keep order, as match_refine(top_k) followed by pose_refine.nms_translations would.  Survivors whose model box
+        does not fit the frame (no pose) are not returned; equal residuals keep box-NMS pick order."""
+        from .pose_refine import poseRefine
+        if len(sources) != 2:
+            raise RuntimeError("sources.size() == modalities.size()")
+        sources = [self._as_source(s, i) for i, s in enumerate(sources)]
+        self._whole_bank_only("detect()")
+        sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
+        nat = self._select(list(class_ids))
+        out, R, t, res, _ = nat.detect(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold), int(top_k),
+                                       int(max_iterations), bool(use_scene_cloud), float(translation_threshold))
+        pairs = []
+        for i, m in enumerate(self._to_matches(out)):
+            p = poseRefine()
+            p._residual = float(res[i])
+            p._R = R[i].copy()
+            p._t = t[i].reshape(3, 1).copy()
+            pairs.append((m, p))
+        return pairs
+
     def _to_matches(self, out):
         # column-wise conversion + map(): building ~1400 objects field by field from numpy scalars costs 10x the
         # GPU match itself

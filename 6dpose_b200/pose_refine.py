@@ -97,3 +97,12 @@ def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, m
             p._R = Ro[i].copy()
             p._t = to[i].reshape(3, 1).copy()
     return out
+
+
+def nms_translations(ts, scores, thr, device=None):
+    """linemod_ros/detect.py's nms_norms(ts, scores, thr) (:41-50) for the poses of refine_matches, on the GPU
+    (lm_nms_translations, the routine behind Detector.detect): ts [n,3] mm, scores [n] (detect.py passes -residual),
+    n <= 1024.  Returns the kept indices in keep order.  Equal scores go in index order, NaN scores first; a distance
+    equal to thr, or NaN, suppresses."""
+    dev = _default_device() if device is None else int(device)
+    return _lib.nms_translations(ts, scores, thr, dev)

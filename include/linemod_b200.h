@@ -215,6 +215,46 @@ int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iterations, int
 int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                      int64_t* n_out, int64_t* n_records);
 
+/* Pose NMS on the device: the end of linemod_ros/detect.py's frame (:91-141), which refines every box-NMS survivor and
+ * then drops duplicate objects in pose space with nms_norms(ts, -residual, 40.0) (:41-50, :130-131).  One CTA behind the
+ * pose stage on the detector's stream; only the kept objects come back.
+ *   1. Candidates: the survivors with a pose.  A survivor that took the early return of LL.cpp:52-55 takes no part and
+ *      is not returned (deviation: detect.py would reuse the previous call's pose of its one global poseRefine, or
+ *      raise on the first call; it also allocates ts one-dimensional, so ts[i,:] raises as written: its evident intent,
+ *      3-vectors in mm, is followed).
+ *   2. Score s_i = -(double)residual_i, residual the float fitness getResidual() returns: the script's sign is kept, so
+ *      the LOWEST fitness ranks first.
+ *   3. Order: s descending; equal scores (-0.0 == +0.0) in box-NMS pick order (the reference leaves them to an
+ *      unstable argsort()[::-1]); NaN scores (lm_nms_translations only: fitness is finite) before every number, among
+ *      themselves by ascending index.
+ *   4. Greedy pass: keep the first remaining pose, drop every remaining j with !(d_ij > thr), d_ij =
+ *      sqrt((dx*dx + dy*dy) + dz*dz) in float64, each operation correctly rounded, no FMA -- np.linalg.norm of a
+ *      3-vector.  So a distance equal to thr suppresses, a NaN distance suppresses, and a kept pose with a NaN
+ *      translation (zero anchor depth) suppresses every pose after it.
+ *   5. Output: the kept poses in keep order; lm_match, R (9 f64) and t (3 f64, mm) bit-identical to what
+ *      lm_complete_pose returns for that survivor, residual (f32).
+ * The poses are composed on the device (T * init_base, then t * 1000) with the host's operations in its order, from the
+ * R and t registered with each template's render.  Pose NMS spans classes, as detect.py's does.
+ *   lm_enqueue_pose_nms  after lm_enqueue_pose, same stream, no host synchronisation; one launch whatever the survivor
+ *                        count.  LM_E_STATE without a pending lm_enqueue_pose (or when already enqueued for it),
+ *                        LM_E_INVALID for a NaN or negative threshold (+inf is accepted: every finite distance lies
+ *                        within it, so only the best candidate is kept; 0 drops exact duplicates only).  The frame must then
+ *                        complete through lm_complete_detect: lm_complete_pose returns LM_E_STATE.  With a connected peer
+ *                        exchange, every rank enqueues its match before any rank enqueues the post, pose and pose NMS
+ *                        stages.
+ *   lm_complete_detect   waits; out[n_out], R_out + 9k, t_out + 3k, residual[k] are the kept poses; n_survivors =
+ *                        box-NMS survivors, n_posed = those with a pose, n_records as lm_complete_post.  When the records
+ *                        outgrew the result block, the refinement, the box NMS, the pose stage and the pose NMS run again
+ *                        before it returns.
+ *   lm_nms_translations  steps 3-5 on caller arrays (t [n][3] f64, score [n] f64), with the same device routine, for the
+ *                        poses of lm_icp_process_batch: keep[n_keep] are indices in keep order.  n <= 1024, else
+ *                        LM_E_CAPACITY; threshold as above. */
+int lm_enqueue_pose_nms(lm_detector* d, double translation_threshold_mm);
+int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
+                       int64_t* n_out, int64_t* n_survivors, int64_t* n_posed, int64_t* n_records);
+int lm_nms_translations(int device, int64_t n, const double* t, const double* score, double thr, int32_t* keep,
+                        int64_t* n_keep);
+
 /* Convenience = lm_upload_quantized + lm_run + lm_fetch_records + lm_finish (single GPU):
  * Detector::match after quantization. */
 int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,
