@@ -53,20 +53,28 @@ def test_linear_memories_bit_exact(synth, oracle, T, W, H, nf):
     ([4, 8], 800, 480, 150, 35, 75.0),   # 47 position words, bit-planes still fit shared memory
     ([4, 8], 960, 640, 150, 35, 75.0),   # 75 position words (3 rounds), bit-planes read from global memory
     ([4, 8], 1280, 960, 150, 20, 80.0),  # BASELINE config 5 frame size: 150 words (5 rounds)
+    ([4, 4], 648, 480, 150, 35, 75.0),   # Wd = 162 at level 0: no filter, k_refine<false>; non-band K1
+    ([4, 8], 640, 2064, 150, 35, 75.0),  # Hd = 516 at level 0: no filter, k_refine<false> with 128-bit row loads
+    ([5, 8], 640, 480, 63, 2000, 70.0),  # 2 x 2000 templates: one warp per coarse-scan task (team size S = 1)
 ])
 def test_match_bit_exact_synthetic(synth, oracle, T, W, H, nf, n, thr):
+    import os
     bank = synth.synth_bank(n, num_features=nf, levels=len(T), seed=21, class_ids=("01_template", "02_template"))
     q, planted = synth.synth_frame(W, H, levels=len(T), seed=9, bank=bank, plant=6, T=T)
     nat, packed = _native(T, bank)
     got = nat.match_quantized(q, thr)
-    want = oracle.match(q, T, packed, thr)
+    want, st = oracle.match(q, T, packed, thr, n_threads=os.cpu_count() or 1, want_stats=True)
     assert len(want) > 0
     _assert_same(got, want)
     c = nat.counters()
-    _, st = oracle.match(q, T, packed, thr, want_stats=True)
     assert c["coarse_candidates"] == int(st["coarse_candidates"])
     assert c["scan_bytes"] == int(st["coarse_byte_adds"])
     assert c["refine_bytes"] == int(st["refine_byte_adds"])
+    lr = len(T) - 2
+    if lr >= 0 and ((W >> lr) // T[lr] % 4 or (H >> lr) // T[lr] > 512):
+        # the filtered level's Wd is not a multiple of 4, or it has more than 512 cell rows: no filter, the byte-wise
+        # k_refine refines every candidate
+        assert c["filter_bytes_read"] == 0 and c["refine_bytes_read"] > 0
 
 
 def test_bench_workload_3115_templates_bit_exact(synth, oracle):
@@ -145,33 +153,6 @@ def test_reference_assertion_is_an_error(synth, oracle):
     nat = lib.NativeDetector(T)
     with pytest.raises(RuntimeError):
         nat.load_bank(packed, 4)
-
-
-@pytest.mark.parametrize("env", [
-    {"LINEMOD_B200_FILTER": "0"},                                   # no filter: byte-wise refinement of every candidate
-    {"LINEMOD_B200_BITS_EXACT": "0"},                               # filter, survivors refined byte-wise by four warps each
-    {"LINEMOD_B200_FILTER_VARIANT": "1"},                           # 8-lanes-per-candidate filter + byte-wise survivors
-    {"LINEMOD_B200_PLANES_DIRECT": "0"},                            # H-planes derived from the byte linear memories
-    {"LINEMOD_B200_K2_SPLIT": "0"},                                 # one warp per coarse task whatever the shard
-    {"LINEMOD_B200_PLANES_DIRECT": "0", "LINEMOD_B200_K2_SPLIT": "0", "LINEMOD_B200_BITS_EXACT": "0"},
-])
-def test_alternative_kernel_paths_bit_exact(synth, oracle, env, monkeypatch):
-    """Every switchable path (the fallbacks the default path replaced, kept for templates / pyramids it does not take and
-    for A/B runs) gives the oracle's result too.  The switches are read when the handle is created."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    for T, W, H, nf, n, thr in (([4, 8], 640, 480, 150, 140, 75.0), ([5, 8], 640, 480, 63, 70, 70.0), ([2, 4, 8], 640, 512, 96, 35, 70.0)):
-        bank = synth.synth_bank(n, num_features=nf, levels=len(T), seed=21, class_ids=("01_template", "02_template"))
-        q, _ = synth.synth_frame(W, H, levels=len(T), seed=9, bank=bank, plant=6, T=T)
-        nat, packed = _native(T, bank)
-        got = nat.match_quantized(q, thr)
-        want, st = oracle.match(q, T, packed, thr, want_stats=True)
-        assert len(want) > 0
-        _assert_same(got, want)
-        c = nat.counters()
-        assert c["coarse_candidates"] == int(st["coarse_candidates"])
-        assert c["refine_bytes"] == int(st["refine_byte_adds"])
-        nat.close()
 
 
 def test_unsafe_templates_take_the_byte_path_next_to_the_bit_sliced_one(synth, oracle):

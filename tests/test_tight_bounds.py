@@ -9,7 +9,8 @@ import pytest
 import tight_frames as tf
 
 
-@pytest.mark.parametrize("T,W,H", [([4, 8], 640, 480), ([5, 8], 640, 480), ([2, 4, 8], 640, 480)])
+@pytest.mark.parametrize("T,W,H", [([4, 8], 640, 480), ([5, 8], 640, 480), ([2, 4, 8], 640, 480), ([4, 4], 648, 480),
+                                   ([4, 8], 640, 2064)])
 def test_mosaic_responses_are_one_or_four(oracle, T, W, H):
     """Every T x T window (T >= 3) of a mosaic level holds a whole 2x2 tile: no label responds 0 outside the last T rows
     and columns, so raw = 3*CH + nf holds at every cell a clamped patch reaches."""
@@ -23,6 +24,47 @@ def test_mosaic_responses_are_one_or_four(oracle, T, W, H):
             assert set(np.unique(tf.reachable_responses(resp[l][m], t)).tolist()) == {1, 4}, (l, m)
             checked += 1
     assert checked >= 4
+
+
+@pytest.mark.parametrize("kind,T,W,H,ok", [
+    ("mosaic", [4, 8], 640, 480, True), ("mosaic", [4, 8], 640, 464, True), ("mosaic", [5, 8], 640, 480, True),
+    ("mosaic", [4, 4], 648, 480, False),   # Wd = 162
+    ("mosaic", [4, 8], 640, 2064, False),  # Hd = 516
+    ("zero", [4, 8], 320, 256, True),
+    ("zero", [4, 4], 328, 256, False),     # Wd = 82
+    ("zero", [4, 8], 320, 2064, False),    # Hd = 516
+])
+def test_filter_takes_the_frames_it_should(oracle, kind, T, W, H, ok):
+    """The filtered level's Wd must be a multiple of 4, with at most 512 cell rows (prepare_bank): the GPU tests reach
+    k_refine<false> through the frames that fail this (the staircase frames have the mosaic frames' sizes)."""
+    if kind == "mosaic":
+        bank, q = tf.mosaic_case(T, W, H)
+        packed = bank.pack(bank.class_ids(), len(T) * 2)
+    else:
+        T, _, q, packed = tf.zero_case(False, T, W, H)
+    assert tf.Model(oracle, q, T, packed).filter_ok() == ok
+
+
+def _stair_packed(nf, k, unsafe=False):
+    bank = tf.stair_bank(nf, k, unsafe)
+    return bank.pack(bank.class_ids(), 4)
+
+
+@pytest.mark.parametrize("T,pct", [([4, 8], (50, 90, 99)), ([2, 4, 8], (50,))])
+def test_mixed_banks_have_unsafe_and_safe_templates(oracle, T, pct):
+    """With every third template unsafe, the safe ones stay eligible for the filter and some unsafe template has coarse
+    candidates at every tight threshold: the filter hands them to k_refine<true> next to the filtered ones.  The
+    staircase bank's unsafe copy is its last template."""
+    s = tf.mosaic_setup(oracle, T, 640, 480, percentiles=pct, unsafe=True)
+    mdl = s["model"]
+    unsafe = [g for g in range(mdl.G) if not mdl.t[g]["safe"]]
+    assert unsafe == list(range(0, mdl.G, 3))
+    assert all(mdl.eligible(g) for g in range(mdl.G) if g not in unsafe)
+    for thr in s["thresholds"]:
+        for t in (thr, tf.ulp_up(thr)):
+            assert any(len(mdl.candidates(g, t)) > 0 for g in unsafe), t
+    mdl = tf.Model(oracle, tf.uniform_frame(640, 480, 2), [4, 8], _stair_packed(65, 2, unsafe=True))
+    assert mdl.eligible(0) and not mdl.t[mdl.G - 1]["safe"]
 
 
 @pytest.mark.parametrize("T,pct", [([4, 8], (50, 90, 99)), ([2, 4, 8], (50,))])

@@ -1,7 +1,7 @@
 """Frames and banks that put the refinement filter and the best-cell arg-max exactly on their bounds, and a numpy model of
 the filter's decision.
 
-The refinement filter (k_refine_filter_w / k_refine_filter) drops a coarse candidate unless some cell of its 16x16 patch
+The refinement filter (k_refine_filter_w) drops a coarse candidate unless some cell of its 16x16 patch
 has CH >= need = ceil((raw_keep - nf) / 3), where CH counts the features whose label bit is set in the spread mask at that
 cell.  The bound is raw <= 3*CH + nf.  The frames here make it an equality:
 
@@ -70,16 +70,23 @@ def zero_score_frame(W, H, levels, seed, bank, T):
     return q
 
 
-def zero_case(unsafe=False):
-    """320x256 two-level frame blanked over the left half of level 0, with a three-template bank.  unsafe=True moves a
-    feature of template 1 below its box: prepare_bank does not call it "safe", so the byte-wise refinement takes it."""
-    T = [4, 8]
+def zero_case(unsafe=False, T=(4, 8), W=320, H=256):
+    """Two-level frame (320x256 by default) blanked over the left half of level 0, with a three-template bank.
+    unsafe=True moves a feature of template 1 below its box: prepare_bank does not call it "safe", so the byte-wise
+    refinement takes it."""
+    T = list(T)
     bank = synth.synth_bank(3, num_features=32, levels=2, seed=5)
     if unsafe:
         tps = bank.classes["01_template"]
         tps[1][0].features[5, 1] = tps[1][0].height + 6  # below the box, still over the blank half
-    q = zero_score_frame(320, 256, 2, 6, bank, T)
+    q = zero_score_frame(W, H, 2, 6, bank, T)
     return T, bank, q, bank.pack(bank.class_ids(), 4)
+
+
+def make_unsafe(tp):
+    """Moves a level-0 feature of template pyramid `tp` beyond its box: prepare_bank does not call the template "safe",
+    so the filter hands its candidates unfiltered to the byte-wise refinement (k_refine<true>)."""
+    tp[0].features[5, 0] = tp[0].width + 6
 
 
 def split_modalities(nf):
@@ -295,11 +302,15 @@ def records(arr):
 MOSAIC_BANK = dict(n=40, nf=150, seed=21, variants=40)
 
 
-def mosaic_case(T, W, H, seed=0):
+def mosaic_case(T, W, H, seed=0, unsafe=False):
     """Synthetic bank and mosaic frame.  With more than two levels the levels below the filtered one (L - 2) carry every
-    label bit at every pixel: every cell there scores 100 %, so the filtered level alone decides what is kept."""
+    label bit at every pixel: every cell there scores 100 %, so the filtered level alone decides what is kept.
+    unsafe=True makes every third template unsafe (make_unsafe)."""
     bank = synth.synth_bank(MOSAIC_BANK["n"], num_features=MOSAIC_BANK["nf"], levels=len(T), seed=MOSAIC_BANK["seed"],
                             variants=MOSAIC_BANK["variants"])
+    if unsafe:
+        for tp in bank.classes["01_template"][::3]:
+            make_unsafe(tp)
     q = mosaic_frame(W, H, len(T), seed)
     for l in range(len(T) - 2):
         q[l] = [np.full_like(a, 0xFF) for a in q[l]]
@@ -317,11 +328,11 @@ def tight_thresholds(oracle, q, T, packed, percentiles=(50, 90, 99), n_threads=1
 _MOSAIC = {}
 
 
-def mosaic_setup(oracle, T, W, H, percentiles=(50, 90, 99), n_threads=1):
+def mosaic_setup(oracle, T, W, H, percentiles=(50, 90, 99), n_threads=1, unsafe=False):
     """Bank, frame, packed bank, model and tight thresholds of a mosaic case (built once per process)."""
-    key = (tuple(T), W, H, tuple(percentiles))
+    key = (tuple(T), W, H, tuple(percentiles), unsafe)
     if key not in _MOSAIC:
-        bank, q = mosaic_case(T, W, H)
+        bank, q = mosaic_case(T, W, H, unsafe=unsafe)
         packed = bank.pack(bank.class_ids(), len(T) * 2)
         model = Model(oracle, q, T, packed)
         if len(T) == 2:
@@ -371,10 +382,14 @@ def stair_cases():
     return out
 
 
-def stair_bank(nf, k):
+def stair_bank(nf, k, unsafe=False):
     """One staircase template; the 511-feature one (255 + 256, all odd) shares its bank with a 512-feature one
-    (256 + 256), which the filter does not take."""
+    (256 + 256), which the filter does not take.  unsafe=True appends an unsafe copy of the staircase template (the
+    last template of the bank)."""
     tps = [staircase_template(nf, k, seed=1000 + nf * 7 + k)]
     if nf == 511:
         tps.append(staircase_template((256, 256), 512, seed=5, odd_all=True))
+    if unsafe:
+        tps.append(staircase_template(nf, k, seed=1000 + nf * 7 + k))
+        make_unsafe(tps[-1])
     return make_bank(tps)

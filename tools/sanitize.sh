@@ -6,7 +6,9 @@
 #   synccheck : barrier / mbarrier misuse (the TMA staging of k_coarse_packed, __syncthreads in divergent code)
 # on (a) __graft_entry__.smoke() -- one full match checked against the oracle -- and (b) the fused multi-GPU exchange
 # with three handles in one process (peer stores, ticket counters, frame flags, the collector's spin wait), and
-# (c) a second match with every alternative path switched on by environment (byte-wise refinement, 8-lane filter).
+# (c) memcheck over the frames and banks that route the refinement to its byte-wise kernels: k_refine<false> on frames
+# the filter does not take, k_refine<true> behind the filter (unsafe templates, three levels), k_refine_prep deriving the
+# H-planes from the byte linear memories.
 # Usage (on a GPU box):  bash tools/sanitize.sh [outdir]      -> <outdir>/summary.txt, one log per tool x case
 set -u
 OUT=${1:-gpurun_out/sanitize}
@@ -27,6 +29,6 @@ for tool in memcheck racecheck synccheck; do
   run "$tool" smoke python -c "import __graft_entry__ as g; g.smoke()"
   run "$tool" exchange3 python -m pytest "tests/test_gpu_dist.py::test_fused_exchange_three_handles_one_process" -x -q -p no:cacheprovider
 done
-LINEMOD_B200_BITS_EXACT=0 LINEMOD_B200_FILTER_VARIANT=1 LINEMOD_B200_PLANES_DIRECT=0 run memcheck smoke_altpaths python -c "import __graft_entry__ as g; g.smoke()"
-LINEMOD_B200_FILTER=0 run memcheck smoke_nofilter python -c "import __graft_entry__ as g; g.smoke()"
+run memcheck refine_routes python -m pytest "tests/test_gpu_refine_bounds.py::test_zero_score_patches" \
+  "tests/test_gpu_match_parity.py::test_match_bit_exact_synthetic[T6-640-512-96-35-70.0]" -x -q -p no:cacheprovider
 echo "done: $(cat "$OUT/summary.txt" | wc -l) runs" | tee -a "$OUT/summary.txt"
