@@ -23,7 +23,7 @@ HEADER_DTYPE = np.dtype([("count", "<i4"), ("coarse_candidates", "<i4"), ("capac
 PEER_HANDLE_BYTES = 64
 
 SYMBOLS = [
-    "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare",
+    "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks",
     "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
@@ -63,6 +63,7 @@ def load():
     L.lm_select.argtypes = [vp, i32p, c_int, c_int, c_int]
     L.lm_select_layout.argtypes = [vp, i32p, c_int, c_int, c_int, c_int]
     L.lm_prepare.argtypes = [vp]
+    L.lm_coarse_tasks.argtypes = [i32p, c_i64, c_int, c_i64, i32p, c_i64] + [ctypes.POINTER(c_i64)] * 3 + [i32p]
     L.lm_shard_range.argtypes = [vp, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     L.lm_upload_quantized.argtypes = [vp, u8pp, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]
     u8p_ = ctypes.POINTER(ctypes.c_uint8)
@@ -123,6 +124,24 @@ def load():
         getattr(L, name)  # AttributeError if the library does not export a declared symbol
     _lib = L
     return L
+
+
+def coarse_tasks(words, sm_count, plane_bytes):
+    """lm_coarse_tasks: the bit-sliced coarse scan's task table for items with `words` position words each, and its launch
+    shape.  Returns (table [n_entries, 2] int32, n_full, n_rem, dict(tasks, split, warps_per_cta, grid)); no device needed."""
+    L = load()
+    words = np.ascontiguousarray(words, np.int32)
+    i32p = ctypes.POINTER(ctypes.c_int32)
+    n_entries, n_full, n_rem = ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int64()
+    shape = np.zeros(4, np.int32)
+    args = (words.ctypes.data_as(i32p), len(words), sm_count, plane_bytes)
+    check(L.lm_coarse_tasks(*args, None, 0, ctypes.byref(n_entries), ctypes.byref(n_full), ctypes.byref(n_rem),
+                            shape.ctypes.data_as(i32p)))
+    table = np.zeros((n_entries.value, 2), np.int32)
+    check(L.lm_coarse_tasks(*args, table.ctypes.data_as(i32p), n_entries.value, ctypes.byref(n_entries), ctypes.byref(n_full),
+                            ctypes.byref(n_rem), None))
+    return table, n_full.value, n_rem.value, dict(tasks=int(shape[0]), split=int(shape[1]), warps_per_cta=int(shape[2]),
+                                                  grid=int(shape[3]))
 
 
 def check(rc):

@@ -154,8 +154,10 @@ struct lm_detector {
   int64_t work_base = 0, work_stride = 1;    // entry w of the shard is sel[work_base + w * work_stride]
   std::vector<int32_t> shard_sel;            // global template ids of this shard, in order
   int32_t* d_work = nullptr;
-  int32_t* d_items_bits = nullptr; int n_items_bits = 0;    // work items per coarse kernel
+  int n_items_bits = 0;                                     // work items per coarse kernel
   int32_t* d_items_bytes = nullptr; int n_items_bytes = 0;
+  int2* d_k2task = nullptr;                                 // k_coarse_packed's task table of the shard (coarse_task_table)
+  int k2_full = 0, k2_rem = 0, k2_tasks = 0;                // full tasks, remainder words, all tasks
   bool work_dirty = true;
 
   // per-run buffers
@@ -303,7 +305,7 @@ extern "C" void lm_destroy(lm_detector* d) {
   peer_release(d);
   for (int l = 0; l < LM_MAX_LEVELS; ++l) free_level(d->lv[l]);
   cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc4); cudaFree(d->d_k2info); cudaFree(d->d_work);
-  cudaFree(d->d_items_bits); cudaFree(d->d_items_bytes); cudaFree(d->d_safe); cudaFree(d->d_galign);
+  cudaFree(d->d_items_bytes); cudaFree(d->d_k2task); cudaFree(d->d_safe); cudaFree(d->d_galign);
   cudaFree(d->d_mask); cudaFree(d->d_raw); cudaFree(d->d_cnt); cudaFree(d->d_off);
   cudaFree(d->d_res_own); cudaFree(d->d_counters);
   cudaFree(d->d_finfo); cudaFree(d->d_rlab); cudaFree(d->d_surv2);
@@ -686,6 +688,82 @@ static int prepare_bank(lm_detector* d) {
   return LM_OK;
 }
 
+// Task table of k_coarse_packed for one shard: the full rounds (32 consecutive words of one template) of every item in
+// order as (work item, round), then the remainder words of every item laid end to end as (work item, word), 32 per task.
+// The last remainder task is padded with copies of its last word (the kernel emits nothing for them).  items == null:
+// item i is work item i.
+static void coarse_task_table(const int32_t* items, const int32_t* words, int64_t n, std::vector<int2>& table,
+                              int64_t& n_full, int64_t& n_rem) {
+  table.clear();
+  for (int64_t i = 0; i < n; ++i)
+    for (int r = 0; r < words[i] >> 5; ++r) table.push_back(make_int2(items ? items[i] : (int)i, r));
+  n_full = (int64_t)table.size();
+  for (int64_t i = 0; i < n; ++i)
+    for (int k = words[i] & ~31; k < words[i]; ++k) table.push_back(make_int2(items ? items[i] : (int)i, k));
+  n_rem = (int64_t)table.size() - n_full;
+  while ((table.size() - (size_t)n_full) % 32) table.push_back(table.back());
+}
+
+// Launch shape of k_coarse_packed for `tasks` tasks.  One task per warp (or per TEAM of S warps when the shard has fewer
+// tasks than the GPU has warp slots: the team deals the task's features, so the kernel's latency follows the shard) and
+// one round per CTA where the tasks fit: the CTA size follows the shard, so a small shard spreads over all SMs, and
+// CTA b's share of the table (tasks b, b + grid, ...) never holds more tasks than the CTA has teams.
+struct CoarseShape {
+  bool smem;          // the bit-planes are staged in shared memory (k_coarse_packed<true>)
+  int split, wpc, grid;
+  size_t smem_bytes;  // dynamic shared memory: bit-planes + the teams' partial counters
+};
+static CoarseShape coarse_shape(int64_t tasks, int sm_count, size_t plane_bytes) {
+  CoarseShape c;
+  c.smem = plane_bytes <= LM_BITS_SMEM_LIMIT;
+  const long long slots = (long long)sm_count * (LM_PACK_THREADS / 32);
+  const size_t part_room = LM_K2_SMEM_MAX - (c.smem ? plane_bytes : (size_t)LM_K2_SMEM_MAX - 64 * 1024);
+  int S = 1;
+  while (S < 8 && tasks * (S * 2) <= slots) {
+    const int S2 = S * 2;
+    long long w2 = (tasks * S2 + sm_count - 1) / sm_count;
+    w2 = std::min<long long>(LM_PACK_THREADS / 32, std::max<long long>(std::max(4, S2), (w2 + S2 - 1) / S2 * S2));
+    if ((size_t)(w2 / S2) * (S2 - 1) * 16 * 32 * 4 > part_room) break;
+    S = S2;
+  }
+  c.split = S;
+  const int unit = std::max(4, S);
+  int wpc = (int)((tasks * S + sm_count - 1) / sm_count);
+  c.wpc = std::min(LM_PACK_THREADS / 32, std::max(unit, (wpc + unit - 1) / unit * unit));
+  c.grid = (int)std::max<long long>(1, std::min<long long>(sm_count, (tasks * S + c.wpc - 1) / c.wpc));
+  c.smem_bytes = (c.smem ? plane_bytes : 0) + (size_t)(c.wpc / S) * (S - 1) * 16 * 32 * 4;
+  return c;
+}
+
+extern "C" int lm_coarse_tasks(const int32_t* words, int64_t n_items, int sm_count, int64_t plane_bytes, int32_t* table,
+                               int64_t cap, int64_t* n_entries, int64_t* n_full, int64_t* n_rem, int32_t* shape) {
+  if (n_items < 0 || (n_items > 0 && !words) || sm_count < 1 || plane_bytes < 0) return fail(LM_E_INVALID, "bad arguments");
+  for (int64_t i = 0; i < n_items; ++i)
+    if (words[i] < 1) return fail(LM_E_INVALID, "item %lld has %d position words", (long long)i, words[i]);
+  std::vector<int2> t;
+  int64_t nf = 0, nr = 0;
+  coarse_task_table(nullptr, words, n_items, t, nf, nr);
+  if (n_entries) *n_entries = (int64_t)t.size();
+  if (n_full) *n_full = nf;
+  if (n_rem) *n_rem = nr;
+  const int64_t tasks = nf + (nr + 31) / 32;
+  if (shape) {
+    const CoarseShape c = coarse_shape(tasks, sm_count, (size_t)plane_bytes);
+    shape[0] = (int32_t)tasks;
+    shape[1] = c.split;
+    shape[2] = c.wpc;
+    shape[3] = c.grid;
+  }
+  if (table) {
+    if (cap < (int64_t)t.size()) return fail(LM_E_CAPACITY, "task table has %lld entries, room for %lld", (long long)t.size(), (long long)cap);
+    for (size_t i = 0; i < t.size(); ++i) {
+      table[2 * i] = t[i].x;
+      table[2 * i + 1] = t[i].y;
+    }
+  }
+  return LM_OK;
+}
+
 static int prepare_work(lm_detector* d) {
   if (!d->work_dirty) return LM_OK;
   const int64_t n = d->shard_count;
@@ -698,17 +776,33 @@ static int prepare_work(lm_detector* d) {
   {
     std::vector<int32_t> ib, iy;
     for (int64_t i = 0; i < n; ++i) (d->bits_ok[d->shard_sel[(size_t)i]] ? ib : iy).push_back((int32_t)i);
-    cudaFree(d->d_items_bits); d->d_items_bits = nullptr;
     cudaFree(d->d_items_bytes); d->d_items_bytes = nullptr;
     d->n_items_bits = (int)ib.size();
     d->n_items_bytes = (int)iy.size();
-    if (!ib.empty()) {
-      CU(cudaMalloc(&d->d_items_bits, sizeof(int32_t) * ib.size()));
-      CU(cudaMemcpyAsync(d->d_items_bits, ib.data(), sizeof(int32_t) * ib.size(), cudaMemcpyHostToDevice, d->stream));
-    }
     if (!iy.empty()) {
       CU(cudaMalloc(&d->d_items_bytes, sizeof(int32_t) * iy.size()));
       CU(cudaMemcpyAsync(d->d_items_bytes, iy.data(), sizeof(int32_t) * iy.size(), cudaMemcpyHostToDevice, d->stream));
+    }
+    // the bit-sliced coarse scan's tasks: position words per item for the current frame size
+    cudaFree(d->d_k2task); d->d_k2task = nullptr;
+    d->k2_full = d->k2_rem = d->k2_tasks = 0;
+    std::vector<int2> tasks;
+    if (!ib.empty()) {
+      const LevelHost& low = d->lv[d->L - 1];
+      std::vector<int32_t> words(ib.size());
+      for (size_t i = 0; i < ib.size(); ++i) {
+        const int g = d->shard_sel[(size_t)ib[i]];
+        const int P = d->h_tslot[(size_t)g * d->S + (d->L - 1) * d->M].z;
+        words[i] = std::min(std::max((P + 31) >> 5, 1), low.nwords);
+      }
+      int64_t nf = 0, nr = 0;
+      coarse_task_table(ib.data(), words.data(), (int64_t)ib.size(), tasks, nf, nr);
+      if (nf + (nr + 31) / 32 > INT32_MAX / 32) return fail(LM_E_CAPACITY, "%lld coarse-scan tasks", (long long)(nf + (nr + 31) / 32));
+      d->k2_full = (int)nf;
+      d->k2_rem = (int)nr;
+      d->k2_tasks = (int)(nf + (nr + 31) / 32);
+      CU(cudaMalloc(&d->d_k2task, sizeof(int2) * tasks.size()));
+      CU(cudaMemcpyAsync(d->d_k2task, tasks.data(), sizeof(int2) * tasks.size(), cudaMemcpyHostToDevice, d->stream));
     }
     CU(cudaStreamSynchronize(d->stream));
   }
@@ -1133,7 +1227,7 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
       bp.lbw = low.lbw; bp.plane = low.plane; bp.nwords = low.nwords;
       bp.tslot = d->d_tslot; bp.fdesc4 = d->d_fdesc4; bp.k2info = d->d_k2info; bp.work = d->d_work;
       bp.zero_off = (uint32_t)((size_t)d->M * 8 * low.lbw) * 4u;
-      bp.items = d->d_items_bits; bp.n_items = d->n_items_bits;
+      bp.tasks = d->d_k2task; bp.n_full = d->k2_full; bp.n_rem = d->k2_rem; bp.n_tasks = d->k2_tasks;
       bp.S = d->S; bp.M = d->M; bp.slot_low = (d->L - 1) * d->M;
       bp.threshold = threshold;
       bp.mask = d->d_mask; bp.raw = d->d_raw; bp.cnt = d->d_cnt;
@@ -1148,34 +1242,13 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
       bp.queue = d->d_queue;
       bp.ticket = reinterpret_cast<int*>(d->d_counters + 3);
       const size_t plane_bytes = ((size_t)bp.bp_words * 4 + 15) & ~(size_t)15;
-      const bool smem = plane_bytes <= LM_BITS_SMEM_LIMIT;
-      // tasks of 32 words (full rounds + packed remainders).  One task per warp (or per TEAM of S warps when the shard has
-      // fewer tasks than the GPU has warp slots: the team deals the task's features, so the kernel's latency follows the
-      // shard) and one round per CTA: the CTA size follows the shard, so a small shard spreads over all SMs.
-      // (upper estimate: every template counted with all nwords words; the kernel tabulates the exact tasks)
-      const long long tasks = (long long)d->n_items_bits * (low.nwords / 32) +
-                              ((long long)d->n_items_bits * (low.nwords % 32) + 31) / 32;
-      const long long slots = (long long)d->sm_count * (LM_PACK_THREADS / 32);
-      const size_t part_room = LM_K2_SMEM_MAX - (smem ? plane_bytes : (size_t)LM_K2_SMEM_MAX - 64 * 1024);
-      int S = 1;
-      while (S < 8 && tasks * (S * 2) <= slots) {
-        const int S2 = S * 2;
-        long long w2 = (tasks * S2 + d->sm_count - 1) / d->sm_count;
-        w2 = std::min<long long>(LM_PACK_THREADS / 32, std::max<long long>(std::max(4, S2), (w2 + S2 - 1) / S2 * S2));
-        if ((size_t)(w2 / S2) * (S2 - 1) * 16 * 32 * 4 > part_room) break;
-        S = S2;
-      }
-      bp.split = S;
-      const int unit = std::max(4, S);
-      int wpc = (int)((tasks * S + d->sm_count - 1) / d->sm_count);
-      wpc = std::min(LM_PACK_THREADS / 32, std::max(unit, (wpc + unit - 1) / unit * unit));
-      const int grid = (int)std::max<long long>(1, std::min<long long>(d->sm_count, (tasks * S + wpc - 1) / wpc));
-      const size_t smem_bytes = (smem ? plane_bytes : 0) + (size_t)(wpc / S) * (S - 1) * 16 * 32 * 4;
+      const CoarseShape c = coarse_shape(d->k2_tasks, d->sm_count, plane_bytes);
+      bp.split = c.split;
       cudaError_t e = cudaSuccess;
-      if (smem) {
-        e = launch_pdl(k_coarse_packed<true>, dim3(grid), dim3(wpc * 32), smem_bytes, st, bp);
+      if (c.smem) {
+        e = launch_pdl(k_coarse_packed<true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
       } else {
-        e = launch_pdl(k_coarse_packed<false>, dim3(grid), dim3(wpc * 32), smem_bytes, st, bp);
+        e = launch_pdl(k_coarse_packed<false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
       }
       if (e != cudaSuccess) return fail(LM_E_CUDA, "k_coarse_packed launch failed: %s", cudaGetErrorString(e));
       ++d->launches;

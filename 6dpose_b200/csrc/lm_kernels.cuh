@@ -440,8 +440,10 @@ struct BitScanParams {
   const int2* k2info;   // [G][M]: first descriptor, padded count
   uint32_t zero_off;    // byte offset of the zero words
   const int32_t* work;  // template id per work item
-  const int32_t* items; // work items taken by this kernel
-  int n_items;
+  const int2* tasks;    // task table of the shard (host-built, see k_coarse_packed): n_full (work item, round) entries,
+                        // then 32 (work item, word) entries per remainder task
+  int n_full, n_rem;    // full tasks, remainder words (the last remainder task's entries beyond n_rem are padding)
+  int n_tasks;          // full + remainder tasks
   int S, M, slot_low;
   float threshold;
   uint32_t* mask;  // [n_work][nwords] pass bits, position order
@@ -536,12 +538,14 @@ __global__ void __launch_bounds__(1024) k_scan_counts(int32_t* __restrict__ cnt,
 // template are split in two kinds of tasks:
 //   * FULL rounds (32 consecutive words of one template): the feature descriptors are warp-uniform, so the
 //     plane addressing lives in the uniform datapath -- 15 instructions per feature;
-//   * the REMAINDERS (P/32 mod 32 words per template) of all templates of the CTA, laid end to end and cut
+//   * the REMAINDERS (P/32 mod 32 words per template) of all templates of the shard, laid end to end and cut
 //     into tasks of 32 entries: lane k owns one (template, word) and walks its own template's descriptors
 //     (lanes of 2-3 templates share a warp; 26 instructions per feature, but 32 busy lanes).
-// Both kinds sit in one dynamic queue per CTA (full rounds first).  Either way a lane owns ONE word: two 8-bit
-// vertical counters (H and N planes), the bit-sliced score 4*CH + CN, threshold compare and pass mask.
-#define LM_PACK_CHUNK 512  // templates whose task offsets are tabulated in shared memory at a time
+// The host lists every task of the shard once (full rounds first, p.tasks) and sizes the launch from that exact
+// count; CTA b takes tasks b, b + grid, b + 2 grid, ... of the list through a dynamic queue, so a shard with no more
+// tasks than warp slots runs in one round, and every CTA gets full rounds and the slower remainder tasks in the same
+// proportion (contiguous slices would leave the last CTAs nothing but remainders).  Either way a lane owns ONE
+// word: two 8-bit vertical counters (H and N planes), the bit-sliced score 4*CH + CN, threshold compare and pass mask.
 
 // score = 4*CH + CN (bit-sliced ripple add), positions >= P are zero (LL.cpp:1314), compare with the
 // smallest passing raw score, emit the pass mask and the raw scores of the passing positions
@@ -633,14 +637,12 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
   lm_pdl_wait();
   extern __shared__ __align__(128) uint32_t s_bp[];
   __shared__ __align__(8) unsigned long long s_bar;
-  __shared__ int s_full[LM_PACK_CHUNK + 1];  // full rounds before template i
-  __shared__ int s_rem[LM_PACK_CHUNK + 1];   // remainder words before template i
   __shared__ int s_warp[33];
   __shared__ int s_next;
   __shared__ int s_team_task[LM_PACK_THREADS / 64];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  const int t0 = (int)(((long long)p.n_items * blockIdx.x) / gridDim.x);
-  const int t1 = (int)(((long long)p.n_items * (blockIdx.x + 1)) / gridDim.x);
+  // this CTA's tasks: b, b + grid, b + 2 grid, ... of the table (full rounds and remainders in proportion)
+  const int n_mine = (p.n_tasks - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   const uint32_t* __restrict__ bp = p.bp;
   if (kSmem) {
@@ -667,66 +669,31 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
     bp = s_bp;
   }
 
-  bool staged = !kSmem;
-  for (int c0 = t0; c0 < t1; c0 += LM_PACK_CHUNK) {
-    const int nt = min(LM_PACK_CHUNK, t1 - c0);
-    // task offsets of the chunk's templates (while the bit-planes are still in flight the first time)
-    {
-      const int per = (nt + blockDim.x - 1) / blockDim.x;
-      const int b = min((int)threadIdx.x * per, nt), e = min(b + per, nt);
-      int sum_f = 0, sum_r = 0;
-      for (int i = b; i < e; ++i) {
-        const int g = p.work[p.items[c0 + i]];
-        const int words = min(max((p.tslot[(size_t)g * p.S + p.slot_low].z + 31) >> 5, 1), p.nwords);
-        sum_f += words >> 5;
-        sum_r += words & 31;
-      }
-      int tot_f, tot_r;
-      int run_f = block_exclusive_scan(sum_f, s_warp, &tot_f);
-      int run_r = block_exclusive_scan(sum_r, s_warp, &tot_r);
-      for (int i = b; i < e; ++i) {
-        const int g = p.work[p.items[c0 + i]];
-        const int words = min(max((p.tslot[(size_t)g * p.S + p.slot_low].z + 31) >> 5, 1), p.nwords);
-        s_full[i] = run_f;
-        s_rem[i] = run_r;
-        run_f += words >> 5;
-        run_r += words & 31;
-      }
-      if (threadIdx.x == 0) {
-        s_full[nt] = tot_f;
-        s_rem[nt] = tot_r;
-        s_next = nwarps / p.split;  // one task per team to start with
-      }
-    }
-    __syncthreads();
-    if (!staged) {  // everyone waits for phase 0 of the barrier
-      asm volatile(
-          "{\n"
-          ".reg .pred p;\n"
-          "WAIT_%=:\n"
-          "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n"
-          "@p bra DONE_%=;\n"
-          "bra WAIT_%=;\n"
-          "DONE_%=:\n"
-          "}\n" ::"r"(smem_u32(&s_bar))
-          : "memory");
-      staged = true;
-    }
-    const int n_full = s_full[nt], rem_words = s_rem[nt];
-    const int n_tasks = n_full + ((rem_words + 31) >> 5);
+  if (threadIdx.x == 0) s_next = nwarps / p.split;  // one task per team to start with
+  __syncthreads();
+  if (kSmem) {  // everyone waits for phase 0 of the barrier
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_%=:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n"
+        "@p bra DONE_%=;\n"
+        "bra WAIT_%=;\n"
+        "DONE_%=:\n"
+        "}\n" ::"r"(smem_u32(&s_bar))
+        : "memory");
+  }
+  {
     const int S = p.split, q = warp & (S - 1), team = warp / S;
     uint32_t* s_part = s_bp + (kSmem ? ((p.bp_words + 3u) & ~3u) : 0u) + (size_t)team * (S - 1) * 16 * 32;
-    int task = team;
-    while (task < n_tasks) {
-      if (task < n_full) {
+    int k = team;  // the CTA's k-th task
+    while (k < n_mine) {
+      const int task = (int)blockIdx.x + k * (int)gridDim.x;
+      if (task < p.n_full) {
         // ---- a full round: 32 consecutive words of ONE template, warp-uniform descriptors ----
-        int lo = 0, hi = nt;  // last i with s_full[i] <= task
-        while (hi - lo > 1) {
-          const int mid = (lo + hi) >> 1;
-          if (s_full[mid] <= task) lo = mid; else hi = mid;
-        }
-        const int r = task - s_full[lo];
-        const int w = p.items[c0 + lo];
+        const int2 tk = __ldg(p.tasks + task);  // (work item, round)
+        const int r = tk.y;
+        const int w = tk.x;
         const int g = p.work[w];
         const int P = p.tslot[(size_t)g * p.S + p.slot_low].z;  // equal for all modalities (host checked)
         const int words = min(max((P + 31) >> 5, 1), p.nwords);
@@ -783,20 +750,15 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
         }
         if (q == 0) coarse_emit(p, w, idx, P, nfeat, words, ch, cn);
       } else {
-        // ---- remainders: lane k owns entry e of the chunk's remainder words ----
-        const int e = (task - n_full) * 32 + lane;
-        const bool active = e < rem_words;
-        const int ee = active ? e : rem_words - 1;
-        int lo = 0, hi = nt;  // last i with s_rem[i] <= ee
-        while (hi - lo > 1) {
-          const int mid = (lo + hi) >> 1;
-          if (s_rem[mid] <= ee) lo = mid; else hi = mid;
-        }
-        const int w = p.items[c0 + lo];
+        // ---- remainders: lane k owns entry e of the shard's remainder words ----
+        const int e = (task - p.n_full) * 32 + lane;
+        const bool active = e < p.n_rem;  // padding entries repeat the last word
+        const int2 tk = __ldg(p.tasks + p.n_full + e);  // (work item, word behind the template's full rounds)
+        const int w = tk.x;
         const int g = p.work[w];
         const int P = p.tslot[(size_t)g * p.S + p.slot_low].z;
         const int words = min(max((P + 31) >> 5, 1), p.nwords);
-        const int idx = (words & ~31) + (ee - s_rem[lo]);  // behind the template's full rounds
+        const int idx = tk.y;
         int nfeat = 0;
         uint32_t ch[8], cn[8];
 #pragma unroll
@@ -854,14 +816,13 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
       if (S == 1) {
         int nxt = 0;
         if (lane == 0) nxt = atomicAdd(&s_next, 1);
-        task = __shfl_sync(0xffffffffu, nxt, 0);
+        k = __shfl_sync(0xffffffffu, nxt, 0);
       } else {
         if (q == 0 && lane == 0) s_team_task[team] = atomicAdd(&s_next, 1);
         team_bar(team + 1, S * 32);
-        task = s_team_task[team];
+        k = s_team_task[team];
       }
     }
-    __syncthreads();  // the offset tables and s_next are rebuilt for the next chunk
   }
   if (p.off) {
     // the last CTA to get here owns the scan: every other CTA's masks / counts are fenced before its ticket
@@ -875,18 +836,6 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
       scan_counts_block(p.cnt, p.off, p.n_work, p.hdr, p.capacity, p.shard, p.counters, p.queue, s_warp);
       if (threadIdx.x == 0) *p.ticket = 0;
     }
-  }
-  if (kSmem && !staged) {  // a CTA without templates still has to see its copy land before it exits
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n"
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(smem_u32(&s_bar))
-        : "memory");
   }
 }
 

@@ -124,6 +124,16 @@ int lm_complete(lm_detector* d);
  * shard work lists, run buffers), done now: the first lm_enqueue afterwards only launches.  Needs a frame uploaded or
  * bound (for its size).  SPMD callers use it so that no rank's first frame lags the others'. */
 int lm_prepare(lm_detector* d);
+/* The bit-sliced coarse scan's plan for one shard, as lm_prepare builds it (host only, no device needed).  words[i] =
+ * position words of item i (ceil(P / 32) clamped to 1..nwords; P = template_positions at the lowest level).
+ *   table[n_entries][2]  (item, round) for each of the n_full full tasks (32 consecutive words of one item), items in
+ *                        order; then (item, word) per lane of the remainder tasks: the n_rem remainder words of all
+ *                        items end to end, 32 per task, the last task padded with copies of the last word.  table ==
+ *                        null: only the counts and shape; cap < n_entries: LM_E_CAPACITY (counts still written)
+ *   shape[4]             tasks, warps per team, warps per CTA, CTAs of the launch on sm_count SMs with plane_bytes of
+ *                        bit-planes (zero words included); CTA b takes tasks b, b + CTAs, b + 2 CTAs, ... */
+int lm_coarse_tasks(const int32_t* words, int64_t n_items, int sm_count, int64_t plane_bytes, int32_t* table, int64_t cap,
+                    int64_t* n_entries, int64_t* n_full, int64_t* n_rem, int32_t* shape);
 
 /* Result block of the stages: by default an internal device buffer that grows on demand.  A caller
  * that wants the block in its own device memory (e.g. the send buffer of an NCCL all-gather) sets it

@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer over the hot path (SURVEY.md section 5: race detection / sanitizers hook).
 #   memcheck  : out-of-bounds / misaligned global and shared accesses, leaks of device memory
-#   racecheck : shared-memory hazards (k_linear_memories_band staging, k_coarse_packed task tables + bit-planes,
+#   racecheck : shared-memory hazards (k_linear_memories_band staging, k_coarse_packed task queue + bit-planes,
 #               k_refine<true> / k_refine_bits partial sums, block scans)
 #   synccheck : barrier / mbarrier misuse (the TMA staging of k_coarse_packed, __syncthreads in divergent code)
 # on (a) __graft_entry__.smoke() -- one full match checked against the oracle -- and (b) the fused multi-GPU exchange
