@@ -29,7 +29,7 @@ SYMBOLS = [
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
-    "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations",
+    "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations", "lm_detect_batch",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
     "lm_icp_set_capture", "lm_icp_capture",
@@ -106,6 +106,9 @@ def load():
     L.lm_complete_pose.argtypes = [vp, vp, f64p, f64p, f32p, c_i64, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     L.lm_enqueue_pose_nms.argtypes = [vp, ctypes.c_double]
     L.lm_complete_detect.argtypes = [vp, vp, f64p, f64p, f32p, c_i64] + [ctypes.POINTER(c_i64)] * 4
+    L.lm_detect_batch.argtypes = [vp, c_int, u8p_, u16p, c_int, c_int, ctypes.POINTER(u8p_), c_f, f32p, ctypes.c_double, c_int, c_int,
+                                  c_int, c_int, ctypes.c_double, vp, f64p, f64p, f32p, c_i64, ctypes.POINTER(c_i64),
+                                  ctypes.POINTER(c_i64)]
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -472,6 +475,74 @@ class NativeDetector:
         self.enqueue_pose(sceneK, max_iterations, use_scene_cloud)
         self.enqueue_pose_nms(translation_threshold)
         return self.complete_detect()
+
+    # ---- a batch of frames through one pose stage (include/linemod_b200.h, lm_detect_batch) ----
+    def detect_batch(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30, use_scene_cloud=False,
+                     pose_nms=True, translation_threshold=40.0, cap=None):
+        """rgb [n,H,W,3] u8, depth [n,H,W] u16, masks None or one (mask_color, mask_depth) pair per frame (None or an empty
+        array: no mask), sceneK [n,3,3].  Returns one tuple per frame: what complete_detect returns (pose_nms) or what
+        complete_pose returns.  cap: entries of the first attempt (default: every survivor of every frame); a larger
+        batch result grows it and runs the batch again.  self.batch_counts keeps the last call's [n,4] frame counts
+        (entries, survivors, posed, records)."""
+        rgb = np.ascontiguousarray(rgb)
+        depth = np.ascontiguousarray(depth)
+        if rgb.dtype != np.uint8 or rgb.ndim != 4 or rgb.shape[3] != 3:
+            raise TypeError("rgb must be uint8 [n,H,W,3]")
+        if depth.dtype != np.uint16 or depth.shape != rgb.shape[:3]:
+            raise TypeError("depth must be uint16 [n,H,W] of the colour images' size")
+        n, rows, cols = rgb.shape[:3]
+        sK = np.ascontiguousarray(sceneK, np.float32)
+        if sK.shape != (n, 3, 3):
+            raise ValueError("sceneK must be [%d,3,3], got %s" % (n, sK.shape))
+        u8p = ctypes.POINTER(ctypes.c_uint8)
+        mptr, keep = None, []
+        if masks is not None:
+            if len(masks) != n:
+                raise ValueError("%d mask pairs for %d frames" % (len(masks), n))
+            mptr = (u8p * (2 * n))()
+            for f, pair in enumerate(masks):
+                if len(pair) != 2:
+                    raise RuntimeError("masks.size() == modalities.size()")
+                for m, a in enumerate(pair):
+                    if a is not None and np.asarray(a).size:
+                        a = np.ascontiguousarray(a)
+                        if a.dtype != np.uint8 or a.shape != (rows, cols):
+                            raise RuntimeError("mask.size() == source.size()")
+                        keep.append(a)
+                        mptr[2 * f + m] = a.ctypes.data_as(u8p)
+        bound = top_k if top_k > 0 else 1024
+        cap = n * bound if cap is None else max(int(cap), 1)
+        counts = np.zeros((n, 4), np.int64)
+        f32p, f64p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
+        while True:
+            out = np.empty(cap, MATCH_DTYPE)
+            Ro = np.full((cap, 3, 3), np.nan, np.float64)
+            to = np.full((cap, 3), np.nan, np.float64)
+            res = np.zeros(cap, np.float32)
+            total = ctypes.c_int64()
+            rc = self._L.lm_detect_batch(self._h, n, rgb.ctypes.data_as(u8p), depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows,
+                                         cols, mptr, ctypes.c_float(threshold), sK.ctypes.data_as(f32p), float(iou_threshold), int(top_k),
+                                         int(max_iterations), 1 if use_scene_cloud else 0, 1 if pose_nms else 0,
+                                         float(translation_threshold), out.ctypes.data_as(ctypes.c_void_p), Ro.ctypes.data_as(f64p),
+                                         to.ctypes.data_as(f64p), res.ctypes.data_as(f32p), cap, ctypes.byref(total),
+                                         counts.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)))
+            if rc == LM_E_CAPACITY:
+                cap = int(total.value)
+                continue
+            check(rc)
+            break
+        self.batch_counts = counts
+        frames, at = [], 0
+        for f in range(n):
+            k = int(counts[f, 0])
+            sl = slice(at, at + k)
+            at += k
+            if pose_nms:
+                extra = dict(survivors=int(counts[f, 1]), posed=int(counts[f, 2]), records=int(counts[f, 3]))
+            else:
+                extra = int(counts[f, 3])
+            frames.append((out[sl].copy(), Ro[sl].copy(), to[sl].copy(), res[sl].copy(), extra))
+        return frames
 
     def linear_memories(self, level, modality, shape):
         out = np.zeros(shape, np.uint8)

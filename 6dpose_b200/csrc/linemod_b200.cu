@@ -2091,6 +2091,78 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
   return pose_stage_finish_nms(d->pose, d->stream, out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
 }
 
+extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                               const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+                               int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm, lm_match* out,
+                               double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out, int64_t* frame_counts) {
+  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (!d || !rgb || !depth || !sceneK || !n_out || !frame_counts || (cap > 0 && (!out || !R_out || !t_out || !residual)))
+    return fail(LM_E_INVALID, "null argument");
+  if (n_frames < 1) return fail(LM_E_INVALID, "n_frames %d < 1", n_frames);
+  if (rows <= 0 || cols <= 0) return fail(LM_E_INVALID, "empty frame size %d x %d", rows, cols);
+  if (top_k > LM_POST_MAX) return fail(LM_E_INVALID, "top_k %d > %d", top_k, LM_POST_MAX);
+  if (!(iou_threshold >= 0.0)) return fail(LM_E_INVALID, "IoU threshold must be >= 0");
+  if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
+  if (pose_nms && !(translation_threshold_mm >= 0.0))
+    return fail(LM_E_INVALID, "translation threshold must be >= 0 (NaN given or negative)");
+  if (d->px_rank >= 0) return fail(LM_E_STATE, "lm_detect_batch does not run with a connected peer exchange");
+  if (!d->pose || !pose_stage_covers(d->pose, d->sel.data(), (int64_t)d->sel.size()))
+    return fail(LM_E_STATE, "no template renders registered for every selected template of this bank (lm_set_template_renders)");
+  CU(cudaSetDevice(d->device));
+  cudaStream_t st = d->stream;
+  d->pose_pending = false;  // a batch starts new frames: a pending single-frame pose stage is abandoned
+  d->pose_nms_pending = false;
+  const int bound = top_k > 0 ? top_k : LM_POST_MAX;  // most survivors k_post_nms writes per frame
+  const size_t n0 = (size_t)rows * cols;
+  uint16_t* d_scene = nullptr;
+  lm_match* d_surv = nullptr;
+  int rc = pose_batch_reserve(d->pose, st, n_frames, (int64_t)n0, (int64_t)n_frames * bound, &d_scene, &d_surv);
+  if (rc) return rc;
+  std::vector<int64_t> first((size_t)n_frames + 1, 0);
+  std::vector<lm_match> surv(pose_nms ? 0 : (size_t)n_frames * bound);
+  for (int f = 0; f < n_frames; ++f) {
+    // the single-frame chain up to the box NMS, its capacity retry included
+    rc = lm_upload_images(d, rgb + f * n0 * 3, depth + f * n0, rows, cols, masks ? masks[2 * f] : nullptr, masks ? masks[2 * f + 1] : nullptr);
+    if (rc) return rc;
+    rc = lm_enqueue(d, threshold);
+    if (rc) return rc;
+    rc = lm_enqueue_post(d, iou_threshold, top_k);
+    if (rc) return rc;
+    int64_t n = 0, n_rec = 0;
+    rc = complete_post(d, pose_nms ? nullptr : surv.data() + first[f], bound, &n, &n_rec, !pose_nms);
+    if (rc) return rc;
+    // the next frame's post stage and upload overwrite both: copy them out first, on the stream
+    if (n > 0) CU(cudaMemcpyAsync(d_surv + first[f], d->d_post_out, sizeof(lm_match) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(d_scene + f * n0, d->fe_depth, sizeof(uint16_t) * n0, cudaMemcpyDeviceToDevice, st));
+    first[f + 1] = first[f] + n;
+    frame_counts[4 * f + 1] = n;
+    frame_counts[4 * f + 3] = n_rec;
+  }
+  PoseBatch b;
+  b.n_frames = n_frames; b.srows = rows; b.scols = cols;
+  b.first = first.data(); b.surv = surv.data(); b.sK = sceneK;
+  b.use_scene_cloud = use_scene_cloud ? 1 : 0; b.max_iterations = max_iterations;
+  b.pose_nms = pose_nms ? 1 : 0; b.thr = translation_threshold_mm;
+  b.stream = st;
+  std::vector<int64_t> posed((size_t)n_frames), kept((size_t)n_frames);
+  rc = pose_batch_run(d->pose, b, &d->launches, posed.data(), kept.data());
+  if (rc) return rc;
+  int64_t total = 0;
+  for (int f = 0; f < n_frames; ++f) {
+    frame_counts[4 * f] = kept[f];
+    frame_counts[4 * f + 2] = posed[f];
+    total += kept[f];
+  }
+  *n_out = total;
+  if (total > cap) return fail(LM_E_CAPACITY, "%lld entries in the batch, capacity %lld", (long long)total, (long long)cap);
+  int64_t at = 0;
+  for (int f = 0; f < n_frames; ++f) {
+    pose_batch_frame(d->pose, b, f, out + at, R_out + 9 * at, t_out + 3 * at, residual + at);
+    at += kept[f];
+  }
+  return LM_OK;
+}
+
 extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,
                                   float threshold, lm_match* out, int64_t cap, int64_t* n_out) {
   int rc = upload_quantized(d, quantized, rows, cols, false);  // lm_run synchronises before this call returns

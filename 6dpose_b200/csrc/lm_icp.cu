@@ -828,6 +828,10 @@ struct PoseParams {
   IcpJob* jobs;       // [B]
   int32_t* err;       // 1: a cloud spans more than 2^21 voxels along an axis
   uint8_t* posed;     // [B] 1: survivor i has a template and its box fits the frame (no early return of LL.cpp:52-55)
+  // k_pose_cloud_batch only: slot i belongs to frame frame_of[i], whose depth is scene + frame * srows * scols and whose
+  // intrinsics are sKs + 9 * frame (sK and counts are unused)
+  const int32_t* frame_of;
+  const float* sKs;
 };
 
 __device__ __forceinline__ double pose_backproject(int pix, float c, float f, double z) {
@@ -840,8 +844,10 @@ __device__ __forceinline__ int pose_template(const PoseParams& p, const lm_match
   return (g >= 0 && g < p.n_tpl) ? g : -1;
 }
 
-// One CTA per survivor slot (launched for the bound; slots past the survivor count write empty jobs).
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
+// One CTA per survivor slot.  Single frame (k_pose_cloud): launched for the bound, slots past the survivor count write
+// empty jobs.  Batch (k_pose_cloud_batch): launched for the exact slot count, the frame of each slot from p.frame_of.
+template <bool BATCH>
+__device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   typedef cub::BlockScan<unsigned long long, POSE_THREADS> Scan;
   typedef cub::BlockReduce<double, POSE_THREADS> Reduce;
   __shared__ union {
@@ -855,7 +861,10 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
   IcpJob* job = p.jobs + i;
   lm_match m = {0, 0, 0.f, 0, 0};
   PoseTpl T;
-  bool live = i < p.counts[0];
+  const int frame = BATCH ? p.frame_of[i] : 0;
+  const uint16_t* __restrict__ scene = BATCH ? p.scene + (size_t)frame * p.srows * p.scols : p.scene;
+  const float* __restrict__ bK = BATCH ? p.sKs + 9 * frame : nullptr;
+  bool live = BATCH || i < p.counts[0];
   if (live) {
     m = p.surv[i];
     const int g = pose_template(p, m);
@@ -912,11 +921,11 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
           mx = pose_backproject(mc, T.K[2], T.K[0], mz);
           my = pose_backproject(mr, T.K[5], T.K[4], mz);
         }
-        const uint16_t sd = p.scene[(size_t)sr * p.scols + sc];
+        const uint16_t sd = scene[(size_t)sr * p.scols + sc];
         if (sd > 0) {
           sz = __ddiv_rn((double)sd, 1000.0);
-          sx = pose_backproject(sc, p.sK[2], p.sK[0], sz);
-          sy = pose_backproject(sr, p.sK[5], p.sK[4], sz);
+          sx = pose_backproject(sc, BATCH ? bK[2] : p.sK[2], BATCH ? bK[0] : p.sK[0], sz);
+          sy = pose_backproject(sr, BATCH ? bK[5] : p.sK[5], BATCH ? bK[4] : p.sK[4], sz);
           fs = p.use_scene != 0;
           fc = md > 0 && fabs(__dsub_rn(sz, anchor)) < 0.4;
         }
@@ -984,6 +993,9 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
     p.seg_begin[2 * i + 1] = (int32_t)ss; p.seg_end[2 * i + 1] = (int32_t)ss + ns;
   }
 }
+
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) { pose_cloud<false>(p); }
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch(PoseParams p) { pose_cloud<true>(p); }
 
 // One CTA per cloud slot: mean of every occupied voxel, summed in sorted order (voxel_down_sample).
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals,
@@ -1149,22 +1161,29 @@ struct PoseNmsParams {
   double thr;
   PoseNmsHead* head;
   PoseNmsOut* out;          // kept poses in keep order
+  // k_pose_nms_batch only: CTA f takes the survivors [frame_first[f], frame_first[f + 1]) of surv / posed / outs, writes
+  // head[f] and its kept poses from out + frame_first[f] (counts is unused)
+  const int32_t* frame_first;
 };
 
-// Behind k_icp_point_to_plane: candidates are the survivors with a pose, score -(double)residual.
-__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
+// Behind k_icp_point_to_plane: candidates are the survivors with a pose, score -(double)residual.  One frame per CTA.
+template <bool BATCH>
+__device__ __forceinline__ void pose_nms(const PoseNmsParams& p) {
   const int i = threadIdx.x;
-  const int n = min(p.counts[0], NMS_THREADS);
+  const int first = BATCH ? p.frame_first[blockIdx.x] : 0;
+  const int n = BATCH ? p.frame_first[blockIdx.x + 1] - first : min(p.counts[0], NMS_THREADS);
+  const lm_match* __restrict__ surv = p.surv + first;
+  const IcpOut* __restrict__ outs = p.outs + first;
   bool cand = false;
   double t[3] = {0, 0, 0};
   float res = 0.f;
   int g = 0;
-  if (i < n && p.posed[i]) {
-    const lm_match m = p.surv[i];
+  if (i < n && p.posed[first + i]) {
+    const lm_match m = surv[i];
     g = p.class_begin[m.class_index] + m.template_id;  // k_pose_cloud found it: in range
     const PoseRt q = p.rt[g];
-    for (int r = 0; r < 3; ++r) t[r] = __dmul_rn(pose_compose(p.outs[i].T, q, r, 3), 1000.0);
-    res = __double2float_rn(p.outs[i].fitness);
+    for (int r = 0; r < 3; ++r) t[r] = __dmul_rn(pose_compose(outs[i].T, q, r, 3), 1000.0);
+    res = __double2float_rn(outs[i].fitness);
     cand = true;
   }
   const int posed = __syncthreads_count(cand);
@@ -1174,18 +1193,21 @@ __global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
     PoseNmsOut o;
     const PoseRt q = p.rt[g];
     for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) o.R[3 * r + c] = pose_compose(p.outs[i].T, q, r, c);
+      for (int c = 0; c < 3; ++c) o.R[3 * r + c] = pose_compose(outs[i].T, q, r, c);
     for (int r = 0; r < 3; ++r) o.t[r] = t[r];
-    o.m = p.surv[i];
+    o.m = surv[i];
     o.residual = res;
-    p.out[rank] = o;
+    p.out[first + rank] = o;
   }
   if (i == 0) {
     PoseNmsHead h;
-    h.kept = kept; h.survivors = p.counts[0]; h.posed = posed; h.pad = 0;
-    *p.head = h;
+    h.kept = kept; h.survivors = BATCH ? n : p.counts[0]; h.posed = posed; h.pad = 0;
+    p.head[BATCH ? blockIdx.x : 0] = h;
   }
 }
+
+__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) { pose_nms<false>(p); }
+__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms_batch(PoseNmsParams p) { pose_nms<true>(p); }
 
 struct TplHost {
   bool set = false;
@@ -1217,6 +1239,17 @@ struct lm_pose_stage {
   uint8_t* d_nms = nullptr; uint8_t* h_nms = nullptr;
   // the enqueued frame
   int bound = 0, srows = 0, scols = 0;
+  // batch of frames (pose_batch_*): scene slots and survivors filled by the caller, then per survivor its frame, ICP
+  // output and posed flag, and the pose NMS blocks (one head per frame, kept poses at the frame's survivor offset)
+  int64_t cap_bscene = 0, cap_bsurv = 0, cap_bS = 0; int cap_bframes = 0;
+  uint16_t* d_bscene = nullptr;
+  lm_match* d_bsurv = nullptr;
+  int32_t* d_bframe = nullptr;  // [cap_bS] frame of each survivor
+  IcpOut* d_bouts = nullptr; IcpOut* h_bouts = nullptr;
+  uint8_t* d_bposed = nullptr;
+  PoseNmsOut* d_bnms = nullptr; PoseNmsOut* h_bnms = nullptr;
+  int32_t* d_bfirst = nullptr; float* d_bsK = nullptr;  // [cap_bframes + 1], [cap_bframes][9]
+  PoseNmsHead* d_bhead = nullptr; PoseNmsHead* h_bhead = nullptr;
 };
 
 static void pose_free_frame(lm_pose_stage* s) {
@@ -1239,6 +1272,9 @@ void pose_stage_destroy(lm_pose_stage* s) {
   pose_free_frame(s);
   cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_err); cudaFree(s->d_rt); cudaFree(s->d_nms);
   cudaFreeHost(s->h_err); cudaFreeHost(s->h_nms);
+  cudaFree(s->d_bscene); cudaFree(s->d_bsurv); cudaFree(s->d_bframe); cudaFree(s->d_bouts); cudaFree(s->d_bposed); cudaFree(s->d_bnms);
+  cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead);
+  cudaFreeHost(s->h_bouts); cudaFreeHost(s->h_bnms); cudaFreeHost(s->h_bhead);
   delete s;
 }
 
@@ -1379,6 +1415,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
   p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
   p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * B;
   p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_posed;
+  p.frame_of = nullptr; p.sKs = nullptr;
   CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
   k_pose_cloud<<<B, POSE_THREADS, 0, st>>>(p);
   // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
@@ -1445,6 +1482,7 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
   p.rt = s->d_rt; p.class_begin = s->d_class_begin;
   p.thr = thr;
   p.head = reinterpret_cast<PoseNmsHead*>(s->d_nms); p.out = nms_entries(s->d_nms);
+  p.frame_first = nullptr;
   k_pose_nms<<<1, NMS_THREADS, 0, st>>>(p);
   CUI(cudaGetLastError());
   ++*launches;
@@ -1474,6 +1512,178 @@ int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, doub
     residual[k] = e[k].residual;
   }
   return LM_OK;
+}
+
+// ---- a batch of frames through one pose stage (lm_detect_batch) ----
+#define POSE_BATCH_CHUNK 1024  // survivor slots per chunk: the single-frame bound for top_k = 0
+
+int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
+                       lm_match** d_surv) {
+  const int64_t pix = (int64_t)n_frames * frame_pixels;
+  if (pix > s->cap_bscene || max_surv > s->cap_bsurv || n_frames > s->cap_bframes) {
+    CUI(cudaStreamSynchronize(st));  // an earlier batch may still read them
+    if (pix > s->cap_bscene) {
+      cudaFree(s->d_bscene); s->d_bscene = nullptr; s->cap_bscene = 0;
+      CUI(cudaMalloc(&s->d_bscene, sizeof(uint16_t) * pix));
+      s->cap_bscene = pix;
+    }
+    if (max_surv > s->cap_bsurv) {
+      cudaFree(s->d_bsurv); s->d_bsurv = nullptr; s->cap_bsurv = 0;
+      CUI(cudaMalloc(&s->d_bsurv, sizeof(lm_match) * max_surv));
+      s->cap_bsurv = max_surv;
+    }
+    if (n_frames > s->cap_bframes) {
+      cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead); cudaFreeHost(s->h_bhead);
+      s->d_bfirst = nullptr; s->d_bsK = nullptr; s->d_bhead = nullptr; s->h_bhead = nullptr; s->cap_bframes = 0;
+      CUI(cudaMalloc(&s->d_bfirst, sizeof(int32_t) * (n_frames + 1)));
+      CUI(cudaMalloc(&s->d_bsK, sizeof(float) * 9 * n_frames));
+      CUI(cudaMalloc(&s->d_bhead, sizeof(PoseNmsHead) * n_frames));
+      CUI(cudaMallocHost(&s->h_bhead, sizeof(PoseNmsHead) * n_frames));
+      s->cap_bframes = n_frames;
+    }
+  }
+  *d_scene = s->d_bscene;
+  *d_surv = s->d_bsurv;
+  return LM_OK;
+}
+
+static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S) {
+  if (S <= s->cap_bS) return LM_OK;
+  CUI(cudaStreamSynchronize(st));
+  cudaFree(s->d_bframe); cudaFree(s->d_bouts); cudaFree(s->d_bposed); cudaFree(s->d_bnms);
+  cudaFreeHost(s->h_bouts); cudaFreeHost(s->h_bnms);
+  s->d_bframe = nullptr; s->d_bouts = nullptr; s->d_bposed = nullptr; s->d_bnms = nullptr; s->h_bouts = nullptr; s->h_bnms = nullptr;
+  s->cap_bS = 0;
+  CUI(cudaMalloc(&s->d_bframe, sizeof(int32_t) * S));
+  CUI(cudaMalloc(&s->d_bouts, sizeof(IcpOut) * S));
+  CUI(cudaMalloc(&s->d_bposed, S));
+  CUI(cudaMalloc(&s->d_bnms, sizeof(PoseNmsOut) * S));
+  CUI(cudaMallocHost(&s->h_bouts, sizeof(IcpOut) * S));
+  CUI(cudaMallocHost(&s->h_bnms, sizeof(PoseNmsOut) * S));
+  s->cap_bS = S;
+  return LM_OK;
+}
+
+int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept) {
+  cudaStream_t st = b.stream;
+  const int nf = b.n_frames;
+  const int64_t S = b.first[nf];
+  if (s->dirty) {
+    int rc = pose_upload(s, st);
+    if (rc) return rc;
+  }
+  int rc = pose_batch_survivors(s, st, std::max<int64_t>(S, 1));
+  if (rc) return rc;
+  rc = pose_buffers(s, st, (int)std::min<int64_t>(std::max<int64_t>(S, 1), POSE_BATCH_CHUNK), s->area_max);
+  if (rc) return rc;
+  const int64_t A = s->cap_area;
+  std::vector<int32_t> frame_of((size_t)S);
+  for (int f = 0; f < nf; ++f)
+    for (int64_t k = b.first[f]; k < b.first[f + 1]; ++k) frame_of[(size_t)k] = f;
+  std::vector<int32_t> first32(b.first, b.first + nf + 1);
+  if (S) CUI(cudaMemcpyAsync(s->d_bframe, frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemcpyAsync(s->d_bfirst, first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
+  CUI(cudaMemcpyAsync(s->d_bsK, b.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
+  for (int64_t c0 = 0; c0 < S; c0 += POSE_BATCH_CHUNK) {
+    const int C = (int)std::min<int64_t>(S - c0, POSE_BATCH_CHUNK);
+    PoseParams p;
+    p.surv = s->d_bsurv + c0; p.counts = nullptr;
+    p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
+    p.tpl = s->d_tpl; p.crops = s->d_crops;
+    p.scene = s->d_bscene; p.srows = b.srows; p.scols = b.scols;
+    memset(p.sK, 0, sizeof(p.sK));
+    p.A = (int32_t)A; p.use_scene = b.use_scene_cloud ? 1 : 0;
+    p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
+    p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * C;
+    p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_bposed + c0;
+    p.frame_of = s->d_bframe + c0; p.sKs = s->d_bsK;
+    k_pose_cloud_batch<<<C, POSE_THREADS, 0, st>>>(p);
+    cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
+    cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
+    size_t tmp_bytes = s->sort_tmp_bytes;
+    CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * C * A), 2 * C, p.seg_begin, p.seg_end, 0,
+                                                 3 * POSE_KEY_BITS, st));
+    k_pose_voxel<<<2 * C, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
+                                                 p.use_scene);
+    dim3 g((unsigned)((A + 127) / 128), (unsigned)C);
+    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+    k_icp_point_to_plane<<<C, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, 0.01 * 0.01, b.max_iterations, 1e-6,
+                                                    1e-6, nullptr);
+    CUI(cudaGetLastError());
+    *launches += 5;
+  }
+  if (b.pose_nms) {
+    PoseNmsParams p;
+    p.surv = s->d_bsurv; p.counts = nullptr; p.posed = s->d_bposed; p.outs = s->d_bouts;
+    p.rt = s->d_rt; p.class_begin = s->d_class_begin;
+    p.thr = b.thr;
+    p.head = s->d_bhead; p.out = s->d_bnms;
+    p.frame_first = s->d_bfirst;
+    k_pose_nms_batch<<<nf, NMS_THREADS, 0, st>>>(p);
+    CUI(cudaGetLastError());
+    ++*launches;
+    CUI(cudaMemcpyAsync(s->h_bhead, s->d_bhead, sizeof(PoseNmsHead) * nf, cudaMemcpyDeviceToHost, st));
+  } else if (S) {
+    CUI(cudaMemcpyAsync(s->h_bouts, s->d_bouts, sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
+  }
+  CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUI(cudaStreamSynchronize(st));
+  CUI(cudaGetLastError());
+  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  if (b.pose_nms) {
+    // the kept poses of every frame, each range where its frame's survivors begin
+    bool more = false;
+    for (int f = 0; f < nf; ++f) {
+      posed[f] = s->h_bhead[f].posed;
+      kept[f] = s->h_bhead[f].kept;
+      if (kept[f] > 0) {
+        CUI(cudaMemcpyAsync(s->h_bnms + b.first[f], s->d_bnms + b.first[f], sizeof(PoseNmsOut) * kept[f], cudaMemcpyDeviceToHost, st));
+        more = true;
+      }
+    }
+    if (more) CUI(cudaStreamSynchronize(st));
+    return LM_OK;
+  }
+  const int n_classes = (int)s->class_begin.size() - 1;
+  for (int f = 0; f < nf; ++f) {
+    posed[f] = 0;
+    kept[f] = b.first[f + 1] - b.first[f];
+    for (int64_t i = b.first[f]; i < b.first[f + 1]; ++i) {
+      const lm_match& m = b.surv[i];
+      const int64_t g = (m.class_index >= 0 && m.class_index < n_classes) ? (int64_t)s->class_begin[m.class_index] + m.template_id : -1;
+      if (g < 0 || g >= (int64_t)s->tpl.size() || !s->tpl[(size_t)g].set)
+        return lm_fail(LM_E_STATE, "frame %d, survivor %lld: template without a registered render", f, (long long)(i - b.first[f]));
+      const TplHost& h = s->tpl[(size_t)g];
+      if (!(m.x + h.box[2] >= b.scols || m.y + h.box[3] >= b.srows)) ++posed[f];  // LL.cpp:52-55
+    }
+  }
+  return LM_OK;
+}
+
+void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual) {
+  const int64_t first = b.first[f], n = b.first[f + 1] - first;
+  if (b.pose_nms) {
+    const PoseNmsOut* e = s->h_bnms + first;
+    for (int k = 0; k < s->h_bhead[f].kept; ++k) {
+      out[k] = e[k].m;
+      memcpy(R_out + 9 * k, e[k].R, sizeof(e[k].R));
+      memcpy(t_out + 3 * k, e[k].t, sizeof(e[k].t));
+      residual[k] = e[k].residual;
+    }
+    return;
+  }
+  // as pose_stage_finish: compose on the host, early returns keep R / t untouched
+  for (int64_t i = 0; i < n; ++i) {
+    const lm_match& m = b.surv[first + i];
+    out[i] = m;
+    const TplHost& h = s->tpl[(size_t)(s->class_begin[m.class_index] + m.template_id)];  // pose_batch_run checked it
+    if (m.x + h.box[2] >= b.scols || m.y + h.box[3] >= b.srows) { residual[i] = -1.f; continue; }  // LL.cpp:52-55
+    float base[16];
+    init_base(h.R, h.t, base);
+    compose(s->h_bouts[first + i].T, base, R_out + 9 * i, t_out + 3 * i);
+    residual[i] = (float)s->h_bouts[first + i].fitness;
+  }
 }
 
 // Steps 3-5 of the pose NMS on caller arrays (lm_nms_translations): the same device routine as k_pose_nms.

@@ -47,3 +47,25 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
 // After the stream has been synchronised: the kept poses in keep order (outputs as lm_complete_detect).
 int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                           int64_t* n_out, int64_t* n_survivors, int64_t* n_posed);
+
+// A batch of frames through one pose stage (lm_detect_batch).  pose_batch_reserve returns room for n_frames scene depths
+// of frame_pixels each (frame f at d_scene + f * frame_pixels) and max_surv survivors, which the caller fills on the
+// stream: frame f's survivors at [first[f], first[f + 1]).
+int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
+                       lm_match** d_surv);
+struct PoseBatch {
+  int n_frames, srows, scols;
+  const int64_t* first;       // [n_frames + 1] survivor offsets (host)
+  const lm_match* surv;       // host copy of the survivors (pose_nms == 0 only)
+  const float* sK;            // [n_frames][9]
+  int use_scene_cloud, max_iterations;
+  int pose_nms;               // 1: the pose NMS per frame (k_pose_nms_batch), 0: the host composes the poses
+  double thr;
+  cudaStream_t stream;
+};
+// The pose stage over every survivor of the batch in chunks of at most 1024 slots, then (pose_nms) one pose NMS launch
+// for all frames; waits.  posed[f] / kept[f]: frame f's survivors with a pose, and its entries (kept poses, or every
+// survivor without the pose NMS).
+int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept);
+// Frame f's kept[f] entries after pose_batch_run, outputs as lm_complete_detect (pose_nms) or lm_complete_pose.
+void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual);

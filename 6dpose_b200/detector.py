@@ -245,15 +245,7 @@ class Detector:
         nat = self._select(list(class_ids))
         out, R, t, res, _ = nat.match_pose(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold),
                                            int(top_k), int(max_iterations), bool(use_scene_cloud))
-        pairs = []
-        for i, m in enumerate(self._to_matches(out)):
-            p = poseRefine()
-            p._residual = float(res[i])
-            if res[i] != -1.0:
-                p._R = R[i].copy()
-                p._t = t[i].reshape(3, 1).copy()
-            pairs.append((m, p))
-        return pairs
+        return self._pose_pairs(out, R, t, res)
 
     def detect(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
                max_iterations=30, use_scene_cloud=False, masks=[]):
@@ -271,12 +263,78 @@ class Detector:
         nat = self._select(list(class_ids))
         out, R, t, res, _ = nat.detect(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold), int(top_k),
                                        int(max_iterations), bool(use_scene_cloud), float(translation_threshold))
+        return self._pose_pairs(out, R, t, res)  # every kept pose has one: residual >= 0
+
+    # ---- a batch of RGB-D frames through one pose stage (lm_detect_batch) ----
+    def match_refine_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
+                           use_scene_cloud=False, masks=[]):
+        """match_refine for many frames in one call: each frame's match and box NMS, then one pose stage for the survivors
+        of all of them, which fills the GPU where one frame's few survivors cannot.  frames: a sequence of [rgb, depth]
+        pairs of one size; sceneK: one 3x3 matrix or one per frame; masks: [] or one masks list per frame.  Returns one
+        list per frame, each equal to match_refine on that frame."""
+        nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "match_refine_batch()")
+        got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
+                               bool(use_scene_cloud), pose_nms=False)
+        return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+
+    def detect_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
+                     max_iterations=30, use_scene_cloud=False, masks=[]):
+        """detect for many frames in one call: each frame's match and box NMS, then one pose stage and one pose NMS for all
+        of them.  Arguments as match_refine_batch; returns one list per frame, each equal to detect on that frame."""
+        nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "detect_batch()")
+        got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
+                               bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold))
+        return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+
+    def _batch_args(self, frames, class_ids, sceneK, masks, what):
+        # everything that needs no device is checked before the native handle exists
+        from .pose_refine import poseRefine
+        frames = list(frames)
+        if not frames:
+            raise ValueError("%s: no frames" % what)
+        rgb, depth = [], []
+        for sources in frames:
+            if len(sources) != 2:
+                raise RuntimeError("sources.size() == modalities.size()")
+            rgb.append(self._as_source(sources[0], 0))
+            depth.append(self._as_source(sources[1], 1))
+        if any(r.shape != rgb[0].shape or d.shape != rgb[0].shape[:2] for r, d in zip(rgb, depth)):
+            raise ValueError("%s: every frame's colour and depth images must have one size" % what)
+        n = len(frames)
+        K = np.asarray(sceneK)
+        if K.size == 9:
+            K = np.repeat(poseRefine._mat(K, np.float32, (3, 3), "sceneK")[None], n, 0)
+        elif K.shape == (n, 3, 3):
+            K = poseRefine._mat(K, np.float32, (n, 3, 3), "sceneK")
+        else:
+            raise ValueError("%s: sceneK must be one 3x3 matrix or %d of them, got shape %s" % (what, n, K.shape))
+        if masks is None:
+            raise TypeError("%s: masks must be a list; pass masks=[]" % what)
+        masks = list(masks)
+        if masks and len(masks) != n:
+            raise ValueError("%s: %d masks lists for %d frames" % (what, len(masks), n))
+        pairs = None
+        if masks:
+            pairs = []
+            for m in masks:
+                m = list(m)
+                if m and len(m) != 2:
+                    raise RuntimeError("masks.size() == modalities.size()")
+                pairs.append(m if m else [None, None])
+        self._whole_bank_only(what)
+        nat = self._select(list(class_ids))
+        return nat, (np.stack(rgb), np.stack(depth), pairs, K)
+
+    def _pose_pairs(self, out, R, t, res):
+        # [(Match, poseRefine)]; a survivor without a pose (residual -1, only without the pose NMS) keeps R / t None
+        from .pose_refine import poseRefine
         pairs = []
         for i, m in enumerate(self._to_matches(out)):
             p = poseRefine()
             p._residual = float(res[i])
-            p._R = R[i].copy()
-            p._t = t[i].reshape(3, 1).copy()
+            if res[i] != -1.0:
+                p._R = R[i].copy()
+                p._t = t[i].reshape(3, 1).copy()
             pairs.append((m, p))
         return pairs
 

@@ -265,6 +265,33 @@ int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, double* t_o
 int lm_nms_translations(int device, int64_t n, const double* t, const double* score, double thr, int32_t* keep,
                         int64_t* n_keep);
 
+/* A batch of RGB-D frames in one call: each frame's match and box NMS, then one pose stage and (pose_nms) one pose NMS
+ * for the survivors of every frame.  Frame f is rgb + f * rows * cols * 3 and depth + f * rows * cols (all frames one
+ * size), masks[2f] / masks[2f + 1] its colour and depth masks (masks NULL: none), sceneK + 9f its intrinsics.  The other
+ * arguments are those of lm_enqueue (threshold), lm_enqueue_post (iou_threshold, top_k), lm_enqueue_pose (max_iterations,
+ * use_scene_cloud) and lm_enqueue_pose_nms (translation_threshold_mm).
+ * Frame f's entries follow those of frames 0..f-1 in out / R_out + 9k / t_out + 3k / residual[k]; bit for bit they are
+ * what the single-frame chain returns for that frame alone:
+ *   pose_nms == 0  lm_upload_images, lm_enqueue, lm_enqueue_post, lm_enqueue_pose, lm_complete_pose: every survivor, in
+ *                  pick order; residual -1 and R / t untouched on the early return of LL.cpp:52-55.
+ *   pose_nms == 1  the same chain plus lm_enqueue_pose_nms, lm_complete_detect: the kept poses, in keep order.
+ * frame_counts[4f .. 4f + 3] = entries, box-NMS survivors, survivors with a pose, kept records the box NMS saw.
+ * *n_out = entries of the whole batch.  LM_E_CAPACITY (with *n_out the total needed) when cap is smaller;
+ * LM_E_INVALID for n_frames < 1 or a NaN / negative translation threshold with pose_nms; LM_E_STATE without renders
+ * for every selected template, and with a connected peer exchange (the batch is single-GPU only).
+ * Each frame runs the single-frame match and box NMS and waits for them (a frame whose records outgrow the result block
+ * is redone there); its survivors and depth are copied aside on the stream.  The pose stage then runs once over all
+ * S survivors in chunks of at most 1024 slots (the single-frame bound for top_k = 0, so its cloud buffers do not grow
+ * with the batch): 5 launches per chunk, plus 1 launch of the pose NMS for every frame.  Extra device memory, kept by
+ * the handle for the next batch: n_frames depth slots (rows * cols * 2 bytes each, 614 KB at 640 x 480),
+ * n_frames * (top_k, or 1024) survivor slots of 20 bytes, and per survivor its ICP output, pose NMS entry, frame index
+ * and posed flag (about 280 bytes, plus a pinned host copy of the first two). */
+int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                    const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+                    int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm,
+                    lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out,
+                    int64_t* frame_counts);
+
 /* Convenience = lm_upload_quantized + lm_run + lm_fetch_records + lm_finish (single GPU):
  * Detector::match after quantization. */
 int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,

@@ -8,7 +8,8 @@
 # with three handles in one process (peer stores, ticket counters, frame flags, the collector's spin wait), and
 # (c) memcheck over the frames and banks that route the refinement to its byte-wise kernels: k_refine<false> on frames
 # the filter does not take, k_refine<true> behind the filter (unsafe templates, three levels), k_refine_prep deriving the
-# H-planes from the byte linear memories.
+# H-planes from the byte linear memories, and (d) memcheck over lm_detect_batch: a batch whose survivors span two pose
+# chunks, and one with early returns and NaN anchors.
 # Usage (on a GPU box):  bash tools/sanitize.sh [outdir]      -> <outdir>/summary.txt, one log per tool x case
 set -u
 OUT=${1:-gpurun_out/sanitize}
@@ -31,4 +32,6 @@ for tool in memcheck racecheck synccheck; do
 done
 run memcheck refine_routes python -m pytest "tests/test_gpu_refine_bounds.py::test_zero_score_patches" \
   "tests/test_gpu_match_parity.py::test_match_bit_exact_synthetic[T6-640-512-96-35-70.0]" -x -q -p no:cacheprovider
+run memcheck detect_batch python -m pytest "tests/test_gpu_detect_batch.py::test_survivors_beyond_one_chunk" \
+  "tests/test_gpu_detect_batch.py::test_early_returns_and_nan_anchors" -x -q -p no:cacheprovider
 echo "done: $(cat "$OUT/summary.txt" | wc -l) runs" | tee -a "$OUT/summary.txt"
