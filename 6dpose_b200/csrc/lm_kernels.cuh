@@ -1046,9 +1046,8 @@ __global__ void __launch_bounds__(256) k_refine_prep(PrepParams p) {
 // the same 16 cells twice, in two halves.  A candidate is a chain of nf / 32 steps.  Lane L decodes descriptor L of the
 // step once (byte offset and shift packed in one register) and stores it to shared memory; every lane picks up four
 // descriptors of its half-warp with one 128-bit broadcast load.  Control flow is warp-uniform.  Every LM_FILTER_CHECK
-// features, once `need` exceeds the features still to come, the partial counters meet (vc_fold) and cells, lanes and
-// whole candidates that can no longer reach `need` are found with a bit-sliced compare and dropped; the last check is at
-// the end.
+// features, once `need` exceeds the features still to come, the partial counters meet (vc_fold) and a candidate none of
+// whose cells can still reach `need` is found with a bit-sliced compare and dropped; the last check is at the end.
 // --------------------------------------------------------------------------------------------
 struct FilterParams {
   const uint32_t* rp;      // H-planes of the filtered level
@@ -1068,7 +1067,7 @@ struct FilterParams {
   uint32_t* surv;          // survivors (candidate indices), unordered
   uint32_t* surv2;         // optional second list: candidates of templates the filter does not take (k_refine_filter_w)
   int* queue;              // [0] next candidate, [1] survivors, [2] entries of surv2
-  unsigned long long* counters;  // [4] features x candidates dropped here, [5] plane words read
+  unsigned long long* counters;  // [4] features x candidates dropped here, [5] plane words read by live lanes
 };
 
 // add eight 1-bit planes into an NB-bit vertical counter
@@ -1139,7 +1138,7 @@ __device__ __forceinline__ uint32_t lm_plane_rows(const char* col, uint32_t v) {
 }
 
 #ifndef LM_FILTER_MIN_CTAS
-#define LM_FILTER_MIN_CTAS 5
+#define LM_FILTER_MIN_CTAS 4  // 64 registers: more of a step's 16 loads in flight per warp (5 CTAs at 48: slower, DESIGN.md §9)
 #endif
 #ifndef LM_FILTER_CHUNK
 #define LM_FILTER_CHUNK 1  // consecutive candidates a warp takes from the queue at a time (2..16 measured: tail imbalance costs more than the L1 reuse buys)
@@ -1225,19 +1224,16 @@ __global__ void __launch_bounds__(256, LM_FILTER_MIN_CTAS) k_refine_filter_w(Fil
           const int py0 = cy + (int)(d >> 23);
           reinterpret_cast<uint32_t*>(sd[sb])[lane] = (((d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd)) << 7) | ((uint32_t)py0 & 15u);
           __syncwarp();
+          // Every lane loads, dead ones too: a dead column keeps adding its true counts, and a column once below the
+          // running bound stays below it (each step adds at most 32 features to a cell and raises the bound by 32), so
+          // the decision is the same as with zeros.  The loads carry no lane-dependent branch, which lets the compiler
+          // issue all 16 of a step before the first one is used; the half-warp reads the same 64-byte window either way.
           uint32_t xh[8];
 #pragma unroll
           for (int m = 0; m < 4; ++m) {
             const uint4 v = sd[sb][hw * 4 + m];  // features i + 16 hw + 4m .. + 3
-            uint32_t r0 = 0u, r1 = 0u, r2 = 0u, r3 = 0u;
-            if (lane_alive) {
-              r0 = lm_plane_rows(col, v.x);
-              r1 = lm_plane_rows(col, v.y);
-              r2 = lm_plane_rows(col, v.z);
-              r3 = lm_plane_rows(col, v.w);
-            }
-            xh[2 * m] = __byte_perm(r0, r1, 0x5410);
-            xh[2 * m + 1] = __byte_perm(r2, r3, 0x5410);
+            xh[2 * m] = __byte_perm(lm_plane_rows(col, v.x), lm_plane_rows(col, v.y), 0x5410);
+            xh[2 * m + 1] = __byte_perm(lm_plane_rows(col, v.z), lm_plane_rows(col, v.w), 0x5410);
           }
           sb ^= 1;
           if (lane_alive) words_read += 16;
