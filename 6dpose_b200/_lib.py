@@ -30,7 +30,8 @@ SYMBOLS = [
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
     "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations", "lm_detect_batch",
-    "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect",
+    "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect", "lm_peer_share_pose",
+    "lm_pose_stats",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
     "lm_icp_set_capture", "lm_icp_capture",
 ]
@@ -86,6 +87,8 @@ def load():
     L.lm_peer_connect.argtypes = [vp, c_int, c_int, u8p_]
     L.lm_peer_connect_local.argtypes = [vp, c_int, c_int, ctypes.POINTER(vp)]
     L.lm_peer_disconnect.argtypes = [vp]
+    L.lm_peer_share_pose.argtypes = [vp, c_int]
+    L.lm_pose_stats.argtypes = [vp, ctypes.POINTER(c_i64)]
     L.lm_device_result.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(c_i64)]
     L.lm_fetch_records.argtypes = [vp, vp, c_i64, ctypes.POINTER(c_i64)]
     L.lm_finish.argtypes = [vp, vp, c_i64, vp, c_i64, ctypes.POINTER(c_i64)]
@@ -344,6 +347,13 @@ class NativeDetector:
     def peer_disconnect(self):
         check(self._L.lm_peer_disconnect(self._h))
 
+    def peer_share_pose(self, on):
+        """Divide the pose stage over the ranks of the connected exchange (lm_peer_share_pose).  Every rank must set the
+        same value before its next frame and, while it is on, run the pose stage of every frame."""
+        if not isinstance(on, (bool, int, np.bool_, np.integer)):
+            raise TypeError("peer_share_pose(on): on must be a bool, got %s" % type(on).__name__)
+        check(self._L.lm_peer_share_pose(self._h, 1 if on else 0))
+
     def device_result(self):
         p, cap = ctypes.c_void_p(), ctypes.c_int64()
         check(self._L.lm_device_result(self._h, ctypes.byref(p), ctypes.byref(cap)))
@@ -571,6 +581,12 @@ class NativeDetector:
 
     def launch_count(self):
         return int(self._L.lm_launch_count(self._h))
+
+    def pose_stats(self):
+        """[survivors, hypotheses this rank refined, launches, 1 if shared] of the last completed pose stage (lm_pose_stats)."""
+        a = (ctypes.c_int64 * 4)()
+        check(self._L.lm_pose_stats(self._h, a))
+        return [int(v) for v in a]
 
 
 class NativeIcp:

@@ -194,6 +194,7 @@ struct lm_detector {
   bool pose_nms_pending = false;        // lm_enqueue_pose_nms: the frame completes through lm_complete_detect
   double pose_nms_thr = 40.0;
   float pose_sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; int pose_max_iter = 30, pose_use_scene = 0;
+  int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
   uint8_t* px_buf = nullptr;            // this rank's exchange buffer (IPC-exportable cudaMalloc)
@@ -203,6 +204,7 @@ struct lm_detector {
   uint8_t* px_base[LM_MAX_PEERS] = {nullptr};
   int32_t px_seq = 0;
   unsigned long long px_timeout_ns = 1000000000ull;  // collector gives up on a peer after 1 s (LINEMOD_B200_PEER_TIMEOUT_MS)
+  bool px_share_pose = false;           // lm_peer_share_pose: the pose stage is divided over the ranks
   PeerExchange* d_px = nullptr;         // device copy of the descriptor (static after connect)
   PeerExchange h_px;
 
@@ -295,6 +297,7 @@ static void peer_release(lm_detector* d) {
   d->d_px = nullptr;
   d->px_world = 0;
   d->px_cap = 0;
+  d->px_share_pose = false;
 }
 
 extern "C" void lm_destroy(lm_detector* d) {
@@ -1564,10 +1567,15 @@ extern "C" int lm_set_result_buffer(lm_detector* d, void* d_block, int64_t capac
   return LM_OK;
 }
 
-static size_t peer_buffer_bytes(int world, int64_t cap) {
-  return 2 * (size_t)world * (sizeof(lm_result_header) + sizeof(lm_record) * (size_t)cap) +
-         sizeof(int32_t) * (2 * LM_MAX_PEERS + 4);
+// The exchange buffer: the record blocks and their flags (PeerExchange), then the pose area of lm_peer_share_pose
+// (lm_pose.h, PoseShare) at a 16-byte aligned offset.
+static size_t peer_pose_offset(int world, int64_t cap) {
+  const size_t records = 2 * (size_t)world * (sizeof(lm_result_header) + sizeof(lm_record) * (size_t)cap) +
+                         sizeof(int32_t) * (2 * LM_MAX_PEERS + 4);
+  return (records + 15) & ~(size_t)15;
 }
+
+static size_t peer_buffer_bytes(int world, int64_t cap) { return peer_pose_offset(world, cap) + pose_share_area_bytes(); }
 
 extern "C" int lm_peer_export(lm_detector* d, int world, int64_t capacity_records, uint8_t* handle_out) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
@@ -1684,6 +1692,13 @@ extern "C" int lm_peer_connect_local(lm_detector* d, int rank, int world, void* 
   d->px_rank = rank;
   d->have_run = false;
   return peer_upload_descriptor(d);
+}
+
+extern "C" int lm_peer_share_pose(lm_detector* d, int on) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (d->px_rank < 0) return fail(LM_E_STATE, "lm_peer_share_pose needs a connected peer exchange");
+  d->px_share_pose = on != 0;
+  return LM_OK;
 }
 
 extern "C" int lm_peer_disconnect(lm_detector* d) {
@@ -2017,7 +2032,21 @@ extern "C" int lm_set_template_renders(lm_detector* d, int64_t first, int64_t n,
 }
 
 static int enqueue_pose(lm_detector* d) {
+  PoseShare sh;
+  const bool share = d->px_rank >= 0 && d->px_share_pose;
+  if (share) {
+    if (d->px_seq < 1) return fail(LM_E_STATE, "pose exchange: no frame has been enqueued on the connected exchange");
+    memset(&sh, 0, sizeof(sh));
+    for (int r = 0; r < d->px_world; ++r) sh.base[r] = d->px_base[r];
+    sh.area_offset = peer_pose_offset(d->px_world, d->px_cap);
+    sh.world = d->px_world; sh.rank = d->px_rank; sh.seq = d->px_seq;
+    sh.timeout_ns = d->px_timeout_ns;
+    void* abort_flag = nullptr;
+    CU(cudaGetSymbolAddress(&abort_flag, g_px_abort));
+    sh.abort_flag = (int*)abort_flag;
+  }
   PoseEnqueue e;
+  e.share = share ? &sh : nullptr;
   e.d_surv = d->d_post_out; e.d_counts = d->d_post_counts;
   e.d_scene = d->fe_depth; e.srows = d->fe[0].rows; e.scols = d->fe[0].cols;
   memcpy(e.sK, d->pose_sK, sizeof(e.sK));
@@ -2056,7 +2085,10 @@ extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, do
   int rc = lm_complete_post(d, out, cap, n_out, n_records);  // waits; on the capacity retry it runs the pose stage again
   d->pose_pending = false;
   if (rc) return rc;
-  return pose_stage_finish(d->pose, d->stream, d->h_post_out, *n_out, R_out, t_out, residual);
+  rc = pose_stage_finish(d->pose, d->stream, d->h_post_out, *n_out, R_out, t_out, residual);
+  if (rc) return rc;
+  pose_stage_stats(d->pose, *n_out, d->pose_stats);
+  return LM_OK;
 }
 
 static int enqueue_pose_nms(lm_detector* d) {
@@ -2088,7 +2120,16 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
   d->pose_pending = false;
   d->pose_nms_pending = false;
   if (rc) return rc;
-  return pose_stage_finish_nms(d->pose, d->stream, out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
+  rc = pose_stage_finish_nms(d->pose, d->stream, out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
+  if (rc) return rc;
+  pose_stage_stats(d->pose, n_surv, d->pose_stats);
+  return LM_OK;
+}
+
+extern "C" int lm_pose_stats(lm_detector* d, int64_t* out4) {
+  if (!d || !out4) return fail(LM_E_INVALID, "null argument");
+  memcpy(out4, d->pose_stats, sizeof(d->pose_stats));
+  return LM_OK;
 }
 
 extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,

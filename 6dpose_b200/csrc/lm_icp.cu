@@ -236,12 +236,70 @@ __device__ void solve6(double A[6][6], double b[6], double x[6]) {
     for (int i = 0; i < 6; ++i) x[i] = 0.0;
 }
 
+// ---- the pose stage shared over the ranks of the peer exchange (lm_pose.h, PoseShare) ----
+// Pose area of every rank's exchange buffer: [2 frame slots][POSE_SHARE_SLOTS] entries indexed by survivor, then
+// [2][LM_MAX_PEERS] int32 pose flags (slot, publishing rank) and an int32 ticket.  Two frame slots suffice: a rank
+// stores frame n + 2's entries only behind its collector of frame n + 2's records, which waits for every peer's records
+// of that frame, and each peer's stream publishes those only after its own frame-n pose collector has read the slot.
+#define POSE_SHARE_SLOTS 1024  // == LM_POST_MAX, the most survivors k_post_nms writes
+#define POSE_COLLECT_THREADS 256
+
+struct PoseShareEntry {  // one survivor: all that pose_stage_finish and k_pose_nms read of it
+  IcpOut out;
+  int32_t posed;         // k_pose_cloud's verdict
+  int32_t err;           // the owner's cloud-overflow flag (the stage's error is the OR over all ranks)
+};
+static_assert(sizeof(PoseShareEntry) == 160 && sizeof(PoseShareEntry) % 16 == 0, "pose area entry layout");
+
+#define POSE_SHARE_FLAGS ((size_t)2 * POSE_SHARE_SLOTS * sizeof(PoseShareEntry))  // byte offset of the flags in the area
+
+size_t pose_share_area_bytes() { return POSE_SHARE_FLAGS + sizeof(int32_t) * (2 * LM_MAX_PEERS + 4); }
+
+struct PoseShareDev {
+  uint8_t* area[LM_MAX_PEERS];  // every rank's pose area
+  int32_t world, rank, seq;
+  const int32_t* counts;        // [0] survivors written by k_post_nms
+  const uint8_t* posed;         // per slot of this rank (k_pose_cloud_share)
+  int32_t* status;              // [0] cloud overflow (the OR over the ranks after k_pose_collect), [1] 1: a peer did not
+                                // publish in time, [2] entries this rank published
+  unsigned long long timeout_ns;
+  int* abort_flag;
+};
+
+// Thread 0 of the CTA of slot blockIdx.x, after its last pass: the entry of its survivor into the same place of every
+// rank's pose area, then the ticket; the last CTA raises this rank's pose flag everywhere.  The ticket counts CTAs in
+// its low 16 bits and published entries above them.
+__device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const IcpOut& o) {
+  const int i = sh.rank + (int)blockIdx.x * sh.world;  // survivor of this slot
+  const bool mine = i < sh.counts[0];
+  const int slot = sh.seq & 1;
+  if (mine) {
+    PoseShareEntry e;
+    e.out = o;
+    e.posed = sh.posed[blockIdx.x];
+    e.err = sh.status[0];
+    const size_t at = ((size_t)slot * POSE_SHARE_SLOTS + i) * sizeof(PoseShareEntry);
+    for (int q = 0; q < sh.world; ++q) *reinterpret_cast<PoseShareEntry*>(sh.area[q] + at) = e;
+  }
+  __threadfence_system();  // release: the entries before the ticket
+  unsigned* ticket = reinterpret_cast<unsigned*>(sh.area[sh.rank] + POSE_SHARE_FLAGS) + 2 * LM_MAX_PEERS;
+  const unsigned old = atomicAdd(ticket, 1u + (mine ? 1u << 16 : 0u));
+  if ((old & 0xFFFFu) != gridDim.x - 1) return;
+  *ticket = 0;
+  sh.status[2] = (int32_t)(old >> 16) + (mine ? 1 : 0);
+  __threadfence_system();
+  for (int q = 0; q < sh.world; ++q)
+    reinterpret_cast<volatile int32_t*>(sh.area[q] + POSE_SHARE_FLAGS)[slot * LM_MAX_PEERS + sh.rank] = sh.seq;
+}
+
 // corr_out (capture only, else null): 2 slots per source point, the correspondence (-1: none) of pass 0 and of the
-// latest later pass.
+// latest later pass.  SHARE (k_icp_point_to_plane<true>): the result goes to the pose areas of the exchange
+// (pose_share_publish) instead of outs; sh is unused otherwise.
+template <bool SHARE>
 __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
-                                                                  const double* __restrict__ normals, IcpOut* __restrict__ outs,
-                                                                  double max_d2, int max_iter, double rel_fitness, double rel_rmse,
-                                                                  int32_t* __restrict__ corr_out) {
+                                                                    const double* __restrict__ normals, IcpOut* __restrict__ outs,
+                                                                    double max_d2, int max_iter, double rel_fitness, double rel_rmse,
+                                                                    int32_t* __restrict__ corr_out, PoseShareDev sh) {
   __shared__ double s_t[ICP_TILE][3];
   __shared__ double s_red[ICP_THREADS / 32][ICP_NACC];
   __shared__ double s_T[16];
@@ -369,7 +427,58 @@ __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob
     IcpOut o;
     for (int k = 0; k < 16; ++k) o.T[k] = s_T[k];
     o.fitness = fitness; o.rmse = rmse; o.iterations = it; o.pad = 0;
-    outs[blockIdx.x] = o;
+    if (SHARE) pose_share_publish(sh, o);
+    else outs[blockIdx.x] = o;
+  }
+}
+
+// One CTA behind k_icp_point_to_plane<true> on each rank's stream: waits (acquire) until every rank's pose flag of the
+// frame has arrived in this rank's pose area, then copies the entries, in survivor order, into the stage's outs / posed.
+__global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShareDev sh, IcpOut* __restrict__ outs,
+                                                                       uint8_t* __restrict__ posed) {
+  __shared__ int s_late;
+  const int tid = threadIdx.x;
+  if (tid == 0) s_late = 0;
+  __syncthreads();
+  const int slot = sh.seq & 1;
+  const uint8_t* mine = sh.area[sh.rank];
+  if (tid < sh.world) {
+    const volatile int32_t* flag = reinterpret_cast<const volatile int32_t*>(mine + POSE_SHARE_FLAGS) + slot * LM_MAX_PEERS + tid;
+    const volatile int* abort_flag = sh.abort_flag;
+    unsigned long long t0, t1;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    while ((int32_t)(*flag - sh.seq) < 0) {
+      if (*abort_flag) { s_late = 1; break; }
+      __nanosleep(200);
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+      if (t1 - t0 > sh.timeout_ns) {  // a peer does not run the pose stage of this frame (or died)
+        atomicExch(sh.abort_flag, 1);
+        s_late = 1;
+        break;
+      }
+    }
+    __threadfence_system();  // acquire: the entries were fenced before the flag
+  }
+  __syncthreads();
+  const int late = s_late;
+  const int n = late ? 0 : min(sh.counts[0], POSE_SHARE_SLOTS);
+  int err = 0;
+  for (int i = tid; i < n; i += POSE_COLLECT_THREADS) {
+    union {
+      int4 v[sizeof(PoseShareEntry) / 16];
+      PoseShareEntry e;
+    } u;
+    const int4* src = reinterpret_cast<const int4*>(mine + ((size_t)slot * POSE_SHARE_SLOTS + i) * sizeof(PoseShareEntry));
+#pragma unroll
+    for (int k = 0; k < (int)(sizeof(PoseShareEntry) / 16); ++k) u.v[k] = __ldcv(src + k);  // peers wrote them
+    outs[i] = u.e.out;
+    posed[i] = (uint8_t)u.e.posed;
+    err |= u.e.err;
+  }
+  err = __syncthreads_or(err);
+  if (tid == 0) {
+    sh.status[0] = err;
+    sh.status[1] = late;
   }
 }
 
@@ -664,8 +773,8 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
       k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, knn_out);
       ++h->launches;
     }
-    k_icp_point_to_plane<<<(unsigned)jobs.size(), ICP_THREADS, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, h->d_outs, 0.01 * 0.01,
-                                                                      max_iterations, 1e-6, 1e-6, corr_out);
+    k_icp_point_to_plane<false><<<(unsigned)jobs.size(), ICP_THREADS, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, h->d_outs, 0.01 * 0.01,
+                                                                             max_iterations, 1e-6, 1e-6, corr_out, PoseShareDev());
     ++h->launches;
     CUI(cudaEventRecord(h->ev1, st));
     CUI(cudaMemcpyAsync(h->h_outs, h->d_outs, jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
@@ -832,6 +941,8 @@ struct PoseParams {
   // intrinsics are sKs + 9 * frame (sK and counts are unused)
   const int32_t* frame_of;
   const float* sKs;
+  // k_pose_cloud_share only: slot i takes survivor rank + i * world (PoseShare)
+  int32_t rank, world;
 };
 
 __device__ __forceinline__ double pose_backproject(int pix, float c, float f, double z) {
@@ -846,7 +957,8 @@ __device__ __forceinline__ int pose_template(const PoseParams& p, const lm_match
 
 // One CTA per survivor slot.  Single frame (k_pose_cloud): launched for the bound, slots past the survivor count write
 // empty jobs.  Batch (k_pose_cloud_batch): launched for the exact slot count, the frame of each slot from p.frame_of.
-template <bool BATCH>
+// Shared (k_pose_cloud_share): launched for this rank's share of the bound, slot i takes survivor p.rank + i * p.world.
+template <bool BATCH, bool SHARE>
 __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   typedef cub::BlockScan<unsigned long long, POSE_THREADS> Scan;
   typedef cub::BlockReduce<double, POSE_THREADS> Reduce;
@@ -864,9 +976,10 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   const int frame = BATCH ? p.frame_of[i] : 0;
   const uint16_t* __restrict__ scene = BATCH ? p.scene + (size_t)frame * p.srows * p.scols : p.scene;
   const float* __restrict__ bK = BATCH ? p.sKs + 9 * frame : nullptr;
-  bool live = BATCH || i < p.counts[0];
+  const int si = SHARE ? p.rank + i * p.world : i;  // survivor of this slot
+  bool live = BATCH || si < p.counts[0];
   if (live) {
-    m = p.surv[i];
+    m = p.surv[si];
     const int g = pose_template(p, m);
     live = g >= 0;
     if (live) {
@@ -994,8 +1107,9 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   }
 }
 
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) { pose_cloud<false>(p); }
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch(PoseParams p) { pose_cloud<true>(p); }
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) { pose_cloud<false, false>(p); }
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch(PoseParams p) { pose_cloud<true, false>(p); }
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_share(PoseParams p) { pose_cloud<false, true>(p); }
 
 // One CTA per cloud slot: mean of every occupied voxel, summed in sorted order (voxel_down_sample).
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals,
@@ -1231,7 +1345,7 @@ struct lm_pose_stage {
   int32_t* d_vals[2] = {nullptr, nullptr};
   int32_t* d_seg = nullptr;
   IcpJob* d_jobs = nullptr; IcpOut* d_outs = nullptr;
-  int32_t* d_err = nullptr;
+  int32_t* d_err = nullptr;  // [0] cloud overflow; shared stage: [1] a peer's poses did not arrive, [2] entries published
   void* d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
   IcpOut* h_outs = nullptr; int32_t* h_err = nullptr;
   uint8_t* d_posed = nullptr;
@@ -1239,6 +1353,9 @@ struct lm_pose_stage {
   uint8_t* d_nms = nullptr; uint8_t* h_nms = nullptr;
   // the enqueued frame
   int bound = 0, srows = 0, scols = 0;
+  // its pose stage: launches, shared over the exchange (frame share_seq, collector timeout share_timeout_ns)
+  int64_t last_launches = 0;
+  bool shared = false; int32_t share_seq = 0; unsigned long long share_timeout_ns = 0;
   // batch of frames (pose_batch_*): scene slots and survivors filled by the caller, then per survivor its frame, ICP
   // output and posed flag, and the pose NMS blocks (one head per frame, kept poses at the frame's survivor offset)
   int64_t cap_bscene = 0, cap_bsurv = 0, cap_bS = 0; int cap_bframes = 0;
@@ -1361,8 +1478,8 @@ static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
 
 static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t area) {
   if (!s->d_err) {
-    CUI(cudaMalloc(&s->d_err, sizeof(int32_t)));
-    CUI(cudaMallocHost(&s->h_err, sizeof(int32_t)));
+    CUI(cudaMalloc(&s->d_err, sizeof(int32_t) * 4));
+    CUI(cudaMallocHost(&s->h_err, sizeof(int32_t) * 4));
   }
   if (bound <= s->cap_bound && area <= s->cap_area) return LM_OK;
   CUI(cudaStreamSynchronize(st));
@@ -1404,6 +1521,8 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
   int rc = pose_buffers(s, st, e.bound, s->area_max);
   if (rc) return rc;
   const int B = e.bound;
+  const PoseShare* sh = e.share;
+  const int Bs = sh ? (B + sh->world - 1) / sh->world : B;  // slots this rank refines
   const int64_t A = s->cap_area;  // slot stride: the buffers' area, which may exceed the current largest crop
   PoseParams p;
   p.surv = e.d_surv; p.counts = e.d_counts;
@@ -1416,27 +1535,63 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
   p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * B;
   p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_posed;
   p.frame_of = nullptr; p.sKs = nullptr;
+  p.rank = sh ? sh->rank : 0; p.world = sh ? sh->world : 1;
   CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
-  k_pose_cloud<<<B, POSE_THREADS, 0, st>>>(p);
+  if (sh) k_pose_cloud_share<<<Bs, POSE_THREADS, 0, st>>>(p);
+  else k_pose_cloud<<<B, POSE_THREADS, 0, st>>>(p);
   // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
   cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
   cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
   size_t tmp_bytes = s->sort_tmp_bytes;
-  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * B * A), 2 * B, p.seg_begin, p.seg_end, 0,
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * Bs * A), 2 * Bs, p.seg_begin, p.seg_end, 0,
                                                3 * POSE_KEY_BITS, st));
-  k_pose_voxel<<<2 * B, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
-                                               p.use_scene);
-  // unchanged ICP kernels, launched for the bound: empty jobs fall through
-  dim3 g((unsigned)((A + 127) / 128), (unsigned)B);
+  k_pose_voxel<<<2 * Bs, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
+                                                p.use_scene);
+  // unchanged ICP kernels, launched for the bound (this rank's share): empty jobs fall through
+  dim3 g((unsigned)((A + 127) / 128), (unsigned)Bs);
   k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
-  k_icp_point_to_plane<<<B, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, 0.01 * 0.01, e.max_iterations, 1e-6, 1e-6,
-                                                  nullptr);
+  if (sh) {
+    PoseShareDev sd;
+    memset(&sd, 0, sizeof(sd));
+    for (int r = 0; r < sh->world; ++r) sd.area[r] = sh->base[r] + sh->area_offset;
+    sd.world = sh->world; sd.rank = sh->rank; sd.seq = sh->seq;
+    sd.counts = e.d_counts; sd.posed = s->d_posed; sd.status = s->d_err;
+    sd.timeout_ns = sh->timeout_ns; sd.abort_flag = sh->abort_flag;
+    k_icp_point_to_plane<true><<<Bs, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr, 0.01 * 0.01, e.max_iterations, 1e-6,
+                                                           1e-6, nullptr, sd);
+    k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_outs, s->d_posed);
+  } else {
+    k_icp_point_to_plane<false><<<B, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, 0.01 * 0.01, e.max_iterations, 1e-6,
+                                                           1e-6, nullptr, PoseShareDev());
+  }
   CUI(cudaGetLastError());
-  *launches += 5;  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals, k_icp_point_to_plane
+  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals, k_icp_point_to_plane (+ k_pose_collect)
+  s->last_launches = sh ? 6 : 5;
+  *launches += s->last_launches;
   CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(B, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
-  CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t) * (sh ? 3 : 1), cudaMemcpyDeviceToHost, st));
   s->bound = B; s->srows = e.srows; s->scols = e.scols;
+  s->shared = sh != nullptr;
+  s->share_seq = sh ? sh->seq : 0;
+  s->share_timeout_ns = sh ? sh->timeout_ns : 0;
   return LM_OK;
+}
+
+// The stage's errors, after the stream has been synchronised.
+static int pose_status(const lm_pose_stage* s) {
+  if (s->shared && s->h_err[1])
+    return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of frame %d within %llu ms (or an earlier collector "
+                   "on this device already gave up); every rank must run the pose stage of every frame while sharing is on",
+                   s->share_seq, s->share_timeout_ns / 1000000ull);
+  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  return LM_OK;
+}
+
+void pose_stage_stats(const lm_pose_stage* s, int64_t n, int64_t* out4) {
+  out4[0] = n;
+  out4[1] = s->shared ? (int64_t)s->h_err[2] : n;
+  out4[2] = s->last_launches;
+  out4[3] = s->shared ? 1 : 0;
 }
 
 int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
@@ -1447,7 +1602,8 @@ int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, i
                         cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
   }
-  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  int rc = pose_status(s);
+  if (rc) return rc;
   const int n_classes = (int)s->class_begin.size() - 1;
   for (int64_t i = 0; i < n; ++i) {
     const lm_match& m = surv[i];
@@ -1493,7 +1649,8 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
 
 int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                           int64_t* n_out, int64_t* n_survivors, int64_t* n_posed) {
-  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  int rc = pose_status(s);
+  if (rc) return rc;
   const PoseNmsHead h = *reinterpret_cast<const PoseNmsHead*>(s->h_nms);
   *n_out = h.kept;
   if (n_survivors) *n_survivors = h.survivors;
@@ -1598,6 +1755,7 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
     p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * C;
     p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_bposed + c0;
     p.frame_of = s->d_bframe + c0; p.sKs = s->d_bsK;
+    p.rank = 0; p.world = 1;
     k_pose_cloud_batch<<<C, POSE_THREADS, 0, st>>>(p);
     cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
     cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
@@ -1608,8 +1766,8 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
                                                  p.use_scene);
     dim3 g((unsigned)((A + 127) / 128), (unsigned)C);
     k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
-    k_icp_point_to_plane<<<C, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, 0.01 * 0.01, b.max_iterations, 1e-6,
-                                                    1e-6, nullptr);
+    k_icp_point_to_plane<false><<<C, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, 0.01 * 0.01, b.max_iterations,
+                                                           1e-6, 1e-6, nullptr, PoseShareDev());
     CUI(cudaGetLastError());
     *launches += 5;
   }

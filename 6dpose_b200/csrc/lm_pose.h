@@ -24,6 +24,23 @@ int pose_stage_register(lm_pose_stage* s, const int32_t* class_begin, int n_clas
 // Every template of the selection has a render.
 bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel);
 
+// The pose stage shared over the ranks of the peer exchange (lm_peer_share_pose).  Survivor i (pick order of k_post_nms,
+// the same on every rank) is refined by rank i % world: this rank's launches are sized for ceil(bound / world) slots,
+// slot j takes survivor rank + j * world.  k_icp_point_to_plane<true> stores each survivor's result into the pose area
+// of every rank's exchange buffer and raises this rank's pose flag there; k_pose_collect waits for the world flags in
+// this rank's buffer and gathers the results in survivor order into the stage's own outputs, so pose_stage_finish and
+// the pose NMS read what the unshared stage leaves.  The pose area: [2 frame slots][1024 survivors] entries of 160 bytes,
+// then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket (pose_share_area_bytes in all).
+struct PoseShare {
+  uint8_t* base[LM_MAX_PEERS];      // every rank's exchange buffer (peer mappings; this rank's own at [rank])
+  uint64_t area_offset;             // byte offset of the pose area in every buffer
+  int world, rank;
+  int32_t seq;                      // the frame's sequence number of the exchange; frame slot = seq & 1
+  unsigned long long timeout_ns;    // the collector gives up on a peer after this long
+  int* abort_flag;                  // the device's abort flag of the exchange: raised on a timeout, honoured at once
+};
+size_t pose_share_area_bytes();
+
 struct PoseEnqueue {
   const lm_match* d_surv;     // survivors in pick order (k_post_nms output)
   const int32_t* d_counts;    // [0] = survivors written
@@ -34,8 +51,12 @@ struct PoseEnqueue {
   int use_scene_cloud;
   int max_iterations;
   cudaStream_t stream;
+  const PoseShare* share;     // null: this rank refines every survivor
 };
 int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches);
+// After pose_stage_finish / pose_stage_finish_nms of a frame with n survivors: what lm_pose_stats returns (survivors,
+// hypotheses this rank refined, launches of the stage, 1 if shared).
+void pose_stage_stats(const lm_pose_stage* s, int64_t n, int64_t* out4);
 // After the stream has been synchronised: surv[n] are the survivors (host copy).  Outputs as lm_icp_process_batch.
 int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
                       float* residual);

@@ -45,10 +45,15 @@ def gather_records(records, group=None):
     return np.concatenate(parts) if parts else np.zeros(0, _lib.RECORD_DTYPE)
 
 
-def connect_peers(detector, group=None, capacity_records=8192, class_ids=()):
+def connect_peers(detector, group=None, capacity_records=8192, class_ids=(), share_pose=False):
     """One-time setup of the fused exchange: every rank exports its buffer's CUDA IPC handle, the
-    handles travel through the process group (any backend), every rank maps the others' buffers."""
+    handles travel through the process group (any backend), every rank maps the others' buffers.
+
+    share_pose: divide the pose stage of Detector.detect / match_refine over the ranks (lm_peer_share_pose).  Only
+    for callers whose every rank runs the pose stage of every frame."""
     import torch.distributed as dist
+    if not isinstance(share_pose, (bool, int, np.bool_, np.integer)):
+        raise TypeError("connect_peers(share_pose=...): a bool, got %s" % type(share_pose).__name__)
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     detector.shard = shard_of(rank, world)
     nat = detector._select(list(class_ids))
@@ -57,6 +62,7 @@ def connect_peers(detector, group=None, capacity_records=8192, class_ids=()):
     dist.all_gather_object(handles, handle, group=group)
     nat.peer_connect(rank, world, handles)
     dist.barrier(group=group)
+    nat.peer_share_pose(bool(share_pose))
     detector._peers = (rank, world)
     return nat
 

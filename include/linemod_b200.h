@@ -166,6 +166,28 @@ int lm_peer_connect(lm_detector* d, int rank, int world, const uint8_t* handles)
 int lm_peer_connect_local(lm_detector* d, int rank, int world, void* const* bases);
 int lm_peer_disconnect(lm_detector* d);
 
+/* The pose stage shared over the ranks of the connected exchange (off by default).  lm_enqueue_pose of a frame then
+ * refines only this rank's share of the box-NMS survivors: survivor i (pick order of the box NMS, the same on every
+ * rank) is refined by rank i % world, so rank r's launches are sized for ceil(bound / world) slots and slot j takes
+ * survivor r + j * world (bound = top_k, or 1024 for every survivor).  The survivor count is read on the device: no host
+ * synchronisation.  The ICP kernel stores each result into the pose area of every rank's exchange buffer over NVLink and
+ * its last CTA raises this rank's pose flag there; a collector kernel behind it waits for all `world` flags and gathers
+ * the results in survivor order.  lm_complete_pose and lm_complete_detect then return on EVERY rank exactly what the
+ * unshared stage returns, bit for bit (R, t, residual, -1 and untouched R / t on the early return of LL.cpp:52-55, NaN
+ * patterns, the pose NMS's keep order and counts): each survivor's ICP is one deterministic job wherever it runs.  A
+ * shared frame's pose stage is 6 launches (5 unshared), whatever the survivor count.
+ *   lm_peer_share_pose  on != 0 turns sharing on.  LM_E_STATE on a handle without a connected exchange.  A promise the
+ *                       caller makes for every rank: every rank of the exchange sets the same value before its next
+ *                       frame, and while it is on every rank runs the pose stage of every frame (a rank that runs the
+ *                       match alone leaves its peers waiting).  lm_peer_disconnect turns it off.  Ranks that are
+ *                       handles of ONE process on ONE device: a pose stage that uploads renders or grows its buffers
+ *                       (the first frame, a larger top_k) frees device memory, which waits for the whole device -- a
+ *                       peer's pose collector included -- so run such a frame unshared first.
+ * A peer whose poses do not arrive within LINEMOD_B200_PEER_TIMEOUT_MS fails the frame with LM_E_STATE (the message names
+ * the pose exchange) and raises the device's abort flag of the exchange, as the record collector does.
+ * lm_detect_batch still refuses a connected exchange. */
+int lm_peer_share_pose(lm_detector* d, int on);
+
 /* Copy the kept records of the last completed run to the host, sorted by (work, seq). */
 int lm_fetch_records(lm_detector* d, lm_record* out, int64_t cap, int64_t* n_out);
 
@@ -325,8 +347,12 @@ int lm_stage_times(lm_detector* d, float* out8);
 /* The CUDA stream all work of this handle is issued on (cudaStream_t as void*). */
 void* lm_stream(lm_detector* d);
 /* Number of kernel launches issued by this handle since creation (the pose stage's CUB segmented sort counts as one;
- * a frame's pose stage is 5, whatever its survivor count). */
+ * a frame's pose stage is 5, whatever its survivor count; 6 when shared over the exchange). */
 int64_t lm_launch_count(lm_detector* d);
+/* About the last pose stage this handle completed (lm_complete_pose / lm_complete_detect): [0] box-NMS survivors,
+ * [1] hypotheses this rank refined (all survivors unshared; its share with lm_peer_share_pose, as counted by the ICP
+ * kernel), [2] launches of the stage, [3] 1 if it was shared.  Zeros before the first.  `out4` has 4 entries. */
+int lm_pose_stats(lm_detector* d, int64_t* out4);
 
 /* ---- poseRefine (reference: linemodLevelup/linemodLevelup.h:8-19, linemodLevelup.cpp:27-155) ---- */
 typedef struct lm_icp lm_icp; /* replaces class poseRefine's compute; the R/t/residual state lives in the caller */

@@ -9,7 +9,8 @@
 # (c) memcheck over the frames and banks that route the refinement to its byte-wise kernels: k_refine<false> on frames
 # the filter does not take, k_refine<true> behind the filter (unsafe templates, three levels), k_refine_prep deriving the
 # H-planes from the byte linear memories, and (d) memcheck over lm_detect_batch: a batch whose survivors span two pose
-# chunks, and one with early returns and NaN anchors.
+# chunks, and one with early returns and NaN anchors, and (e) the pose stage shared over two handles of one process (peer
+# stores of the ICP kernel, its ticket and pose flags, the pose collector's spin wait).
 # Usage (on a GPU box):  bash tools/sanitize.sh [outdir]      -> <outdir>/summary.txt, one log per tool x case
 set -u
 OUT=${1:-gpurun_out/sanitize}
@@ -34,4 +35,8 @@ run memcheck refine_routes python -m pytest "tests/test_gpu_refine_bounds.py::te
   "tests/test_gpu_match_parity.py::test_match_bit_exact_synthetic[T6-640-512-96-35-70.0]" -x -q -p no:cacheprovider
 run memcheck detect_batch python -m pytest "tests/test_gpu_detect_batch.py::test_survivors_beyond_one_chunk" \
   "tests/test_gpu_detect_batch.py::test_early_returns_and_nan_anchors" -x -q -p no:cacheprovider
+for tool in memcheck racecheck synccheck; do
+  run "$tool" pose_share2 python -m pytest "tests/test_gpu_pose_share.py::test_every_rank_returns_the_single_gpu_result[2]" -x -q \
+    -p no:cacheprovider
+done
 echo "done: $(cat "$OUT/summary.txt" | wc -l) runs" | tee -a "$OUT/summary.txt"
