@@ -29,7 +29,7 @@ SYMBOLS = [
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
-    "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations", "lm_detect_batch",
+    "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations", "lm_detect_batch", "lm_peer_detect_batch",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect", "lm_peer_share_pose",
     "lm_pose_stats",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
@@ -112,6 +112,7 @@ def load():
     L.lm_detect_batch.argtypes = [vp, c_int, u8p_, u16p, c_int, c_int, ctypes.POINTER(u8p_), c_f, f32p, ctypes.c_double, c_int, c_int,
                                   c_int, c_int, ctypes.c_double, vp, f64p, f64p, f32p, c_i64, ctypes.POINTER(c_i64),
                                   ctypes.POINTER(c_i64)]
+    L.lm_peer_detect_batch.argtypes = L.lm_detect_batch.argtypes
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -492,8 +493,24 @@ class NativeDetector:
         """rgb [n,H,W,3] u8, depth [n,H,W] u16, masks None or one (mask_color, mask_depth) pair per frame (None or an empty
         array: no mask), sceneK [n,3,3].  Returns one tuple per frame: what complete_detect returns (pose_nms) or what
         complete_pose returns.  cap: entries of the first attempt (default: every survivor of every frame); a larger
-        batch result grows it and runs the batch again.  self.batch_counts keeps the last call's [n,4] frame counts
-        (entries, survivors, posed, records)."""
+        batch result grows it and runs the batch again; any other LM_E_CAPACITY raises.  self.batch_counts keeps the last
+        call's [n,4] frame counts (entries, survivors, posed, records).  The handle keeps the batch's buffers for the next
+        one, sized for its shape: with top_k 0 that includes the pose stage's cloud buffers for 1024 survivors (as a
+        single frame with top_k 0 uses), however few survivors the frames have."""
+        return self._batch(self._L.lm_detect_batch, rgb, depth, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
+                           use_scene_cloud, pose_nms, translation_threshold, cap)
+
+    def peer_detect_batch(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30,
+                          use_scene_cloud=False, pose_nms=True, translation_threshold=40.0, cap=None):
+        """detect_batch over the ranks of the connected exchange (lm_peer_detect_batch): every rank calls it with the same
+        frames and arguments, and every rank returns what detect_batch returns on one unconnected handle over the whole
+        bank.  The retry on too small outputs happens on every rank alike; records beyond the exchange's
+        capacity_records raise LinemodLibraryError on every rank (reconnect with a larger capacity)."""
+        return self._batch(self._L.lm_peer_detect_batch, rgb, depth, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
+                           use_scene_cloud, pose_nms, translation_threshold, cap)
+
+    def _batch(self, fn, rgb, depth, masks, threshold, sceneK, iou_threshold, top_k, max_iterations, use_scene_cloud, pose_nms,
+               translation_threshold, cap):
         rgb = np.ascontiguousarray(rgb)
         depth = np.ascontiguousarray(depth)
         if rgb.dtype != np.uint8 or rgb.ndim != 4 or rgb.shape[3] != 3:
@@ -530,15 +547,15 @@ class NativeDetector:
             to = np.full((cap, 3), np.nan, np.float64)
             res = np.zeros(cap, np.float32)
             total = ctypes.c_int64()
-            rc = self._L.lm_detect_batch(self._h, n, rgb.ctypes.data_as(u8p), depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows,
-                                         cols, mptr, ctypes.c_float(threshold), sK.ctypes.data_as(f32p), float(iou_threshold), int(top_k),
-                                         int(max_iterations), 1 if use_scene_cloud else 0, 1 if pose_nms else 0,
-                                         float(translation_threshold), out.ctypes.data_as(ctypes.c_void_p), Ro.ctypes.data_as(f64p),
-                                         to.ctypes.data_as(f64p), res.ctypes.data_as(f32p), cap, ctypes.byref(total),
-                                         counts.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)))
-            if rc == LM_E_CAPACITY:
+            rc = fn(self._h, n, rgb.ctypes.data_as(u8p), depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows, cols, mptr,
+                    ctypes.c_float(threshold), sK.ctypes.data_as(f32p), float(iou_threshold), int(top_k), int(max_iterations),
+                    1 if use_scene_cloud else 0, 1 if pose_nms else 0, float(translation_threshold), out.ctypes.data_as(ctypes.c_void_p),
+                    Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p), res.ctypes.data_as(f32p), cap, ctypes.byref(total),
+                    counts.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)))
+            if rc == LM_E_CAPACITY and total.value > cap:  # only the outputs were too small: retry with the total
                 cap = int(total.value)
                 continue
+            # any other LM_E_CAPACITY (records beyond the exchange or the result block) would recur on every retry
             check(rc)
             break
         self.batch_counts = counts

@@ -205,6 +205,7 @@ struct lm_detector {
   int32_t px_seq = 0;
   unsigned long long px_timeout_ns = 1000000000ull;  // collector gives up on a peer after 1 s (LINEMOD_B200_PEER_TIMEOUT_MS)
   bool px_share_pose = false;           // lm_peer_share_pose: the pose stage is divided over the ranks
+  int32_t px_pose_seq = 0;              // pose exchanges so far: one per shared frame, one per chunk of a shared batch
   PeerExchange* d_px = nullptr;         // device copy of the descriptor (static after connect)
   PeerExchange h_px;
 
@@ -1593,6 +1594,7 @@ extern "C" int lm_peer_export(lm_detector* d, int world, int64_t capacity_record
   d->px_world = world;
   d->px_cap = capacity_records;
   d->px_seq = 0;
+  d->px_pose_seq = 0;
   {
     const int zero = 0;  // a fresh exchange starts with the device's abort flag down
     CU(cudaMemcpyToSymbol(g_px_abort, &zero, sizeof(int)));
@@ -2031,19 +2033,26 @@ extern "C" int lm_set_template_renders(lm_detector* d, int64_t first, int64_t n,
   return pose_stage_register(d->pose, d->class_begin.data(), d->n_classes, first, n, depths, rows, cols, K, R, t);
 }
 
+// The connected exchange's pose area for the next pose exchange(s), numbered from seq.
+static int pose_share_of(lm_detector* d, int32_t seq, PoseShare* sh) {
+  memset(sh, 0, sizeof(*sh));
+  for (int r = 0; r < d->px_world; ++r) sh->base[r] = d->px_base[r];
+  sh->area_offset = peer_pose_offset(d->px_world, d->px_cap);
+  sh->world = d->px_world; sh->rank = d->px_rank; sh->seq = seq;
+  sh->timeout_ns = d->px_timeout_ns;
+  void* abort_flag = nullptr;
+  CU(cudaGetSymbolAddress(&abort_flag, g_px_abort));
+  sh->abort_flag = (int*)abort_flag;
+  return LM_OK;
+}
+
 static int enqueue_pose(lm_detector* d) {
   PoseShare sh;
   const bool share = d->px_rank >= 0 && d->px_share_pose;
   if (share) {
     if (d->px_seq < 1) return fail(LM_E_STATE, "pose exchange: no frame has been enqueued on the connected exchange");
-    memset(&sh, 0, sizeof(sh));
-    for (int r = 0; r < d->px_world; ++r) sh.base[r] = d->px_base[r];
-    sh.area_offset = peer_pose_offset(d->px_world, d->px_cap);
-    sh.world = d->px_world; sh.rank = d->px_rank; sh.seq = d->px_seq;
-    sh.timeout_ns = d->px_timeout_ns;
-    void* abort_flag = nullptr;
-    CU(cudaGetSymbolAddress(&abort_flag, g_px_abort));
-    sh.abort_flag = (int*)abort_flag;
+    int rc = pose_share_of(d, ++d->px_pose_seq, &sh);
+    if (rc) return rc;
   }
   PoseEnqueue e;
   e.share = share ? &sh : nullptr;
@@ -2132,10 +2141,13 @@ extern "C" int lm_pose_stats(lm_detector* d, int64_t* out4) {
   return LM_OK;
 }
 
-extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
-                               const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
-                               int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm, lm_match* out,
-                               double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out, int64_t* frame_counts) {
+// lm_detect_batch (peers false: refuses a connected exchange) and lm_peer_detect_batch (peers true: needs one).  With
+// peers, each frame's match runs the fused record exchange; every rank then holds the same survivors, so the chunks of
+// the pose stage -- shared or not -- are the same on every rank.
+static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                        const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+                        int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm, lm_match* out,
+                        double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out, int64_t* frame_counts) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !rgb || !depth || !sceneK || !n_out || !frame_counts || (cap > 0 && (!out || !R_out || !t_out || !residual)))
     return fail(LM_E_INVALID, "null argument");
@@ -2146,7 +2158,9 @@ extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb,
   if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
   if (pose_nms && !(translation_threshold_mm >= 0.0))
     return fail(LM_E_INVALID, "translation threshold must be >= 0 (NaN given or negative)");
-  if (d->px_rank >= 0) return fail(LM_E_STATE, "lm_detect_batch does not run with a connected peer exchange");
+  if (!peers && d->px_rank >= 0)
+    return fail(LM_E_STATE, "lm_detect_batch does not run with a connected peer exchange (every rank calls lm_peer_detect_batch)");
+  if (peers && d->px_rank < 0) return fail(LM_E_STATE, "lm_peer_detect_batch needs a connected peer exchange");
   if (!d->pose || !pose_stage_covers(d->pose, d->sel.data(), (int64_t)d->sel.size()))
     return fail(LM_E_STATE, "no template renders registered for every selected template of this bank (lm_set_template_renders)");
   CU(cudaSetDevice(d->device));
@@ -2185,9 +2199,19 @@ extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb,
   b.use_scene_cloud = use_scene_cloud ? 1 : 0; b.max_iterations = max_iterations;
   b.pose_nms = pose_nms ? 1 : 0; b.thr = translation_threshold_mm;
   b.stream = st;
+  PoseShare sh;
+  b.share = nullptr;
+  if (peers && d->px_share_pose) {  // one pose exchange per chunk, numbered on from the single frames' ones
+    rc = pose_share_of(d, d->px_pose_seq + 1, &sh);
+    if (rc) return rc;
+    d->px_pose_seq += pose_batch_chunks(first[n_frames]);
+    b.share = &sh;
+  }
   std::vector<int64_t> posed((size_t)n_frames), kept((size_t)n_frames);
-  rc = pose_batch_run(d->pose, b, &d->launches, posed.data(), kept.data());
+  int64_t stats[4];
+  rc = pose_batch_run(d->pose, b, &d->launches, posed.data(), kept.data(), peers ? stats : nullptr);
   if (rc) return rc;
+  if (peers) memcpy(d->pose_stats, stats, sizeof(stats));
   int64_t total = 0;
   for (int f = 0; f < n_frames; ++f) {
     frame_counts[4 * f] = kept[f];
@@ -2202,6 +2226,23 @@ extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb,
     at += kept[f];
   }
   return LM_OK;
+}
+
+extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                               const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+                               int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm, lm_match* out,
+                               double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out, int64_t* frame_counts) {
+  return detect_batch(d, false, n_frames, rgb, depth, rows, cols, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
+                      use_scene_cloud, pose_nms, translation_threshold_mm, out, R_out, t_out, residual, cap, n_out, frame_counts);
+}
+
+extern "C" int lm_peer_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                                    const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+                                    int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm,
+                                    lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out,
+                                    int64_t* frame_counts) {
+  return detect_batch(d, true, n_frames, rgb, depth, rows, cols, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
+                      use_scene_cloud, pose_nms, translation_threshold_mm, out, R_out, t_out, residual, cap, n_out, frame_counts);
 }
 
 extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,

@@ -237,10 +237,12 @@ __device__ void solve6(double A[6][6], double b[6], double x[6]) {
 }
 
 // ---- the pose stage shared over the ranks of the peer exchange (lm_pose.h, PoseShare) ----
-// Pose area of every rank's exchange buffer: [2 frame slots][POSE_SHARE_SLOTS] entries indexed by survivor, then
-// [2][LM_MAX_PEERS] int32 pose flags (slot, publishing rank) and an int32 ticket.  Two frame slots suffice: a rank
-// stores frame n + 2's entries only behind its collector of frame n + 2's records, which waits for every peer's records
-// of that frame, and each peer's stream publishes those only after its own frame-n pose collector has read the slot.
+// Pose area of every rank's exchange buffer: [2 slots][POSE_SHARE_SLOTS] entries indexed by survivor, then
+// [2][LM_MAX_PEERS] int32 pose flags (slot, publishing rank) and an int32 ticket.  One pose exchange (a shared frame,
+// or one chunk of a shared batch) uses slot seq & 1, seq the exchange's number on the pose counter, which every rank
+// advances once per exchange.  Two slots suffice: a rank stores the entries of exchange e only behind its collector of
+// e - 1, which waited for every peer's flag of e - 1, and each peer raised that flag on its stream behind its own
+// collector of e - 2, the last reader of the slot.
 #define POSE_SHARE_SLOTS 1024  // == LM_POST_MAX, the most survivors k_post_nms writes
 #define POSE_COLLECT_THREADS 256
 
@@ -258,7 +260,7 @@ size_t pose_share_area_bytes() { return POSE_SHARE_FLAGS + sizeof(int32_t) * (2 
 struct PoseShareDev {
   uint8_t* area[LM_MAX_PEERS];  // every rank's pose area
   int32_t world, rank, seq;
-  const int32_t* counts;        // [0] survivors written by k_post_nms
+  const int32_t* counts;        // [0] survivors written by k_post_nms (a batch chunk: the chunk's size)
   const uint8_t* posed;         // per slot of this rank (k_pose_cloud_share)
   int32_t* status;              // [0] cloud overflow (the OR over the ranks after k_pose_collect), [1] 1: a peer did not
                                 // publish in time, [2] entries this rank published
@@ -938,10 +940,10 @@ struct PoseParams {
   int32_t* err;       // 1: a cloud spans more than 2^21 voxels along an axis
   uint8_t* posed;     // [B] 1: survivor i has a template and its box fits the frame (no early return of LL.cpp:52-55)
   // k_pose_cloud_batch only: slot i belongs to frame frame_of[i], whose depth is scene + frame * srows * scols and whose
-  // intrinsics are sKs + 9 * frame (sK and counts are unused)
+  // intrinsics are sKs + 9 * frame (sK is unused, counts too except in k_pose_cloud_batch_share: [0] the chunk's size)
   const int32_t* frame_of;
   const float* sKs;
-  // k_pose_cloud_share only: slot i takes survivor rank + i * world (PoseShare)
+  // k_pose_cloud_share / k_pose_cloud_batch_share only: slot i takes survivor rank + i * world (PoseShare)
   int32_t rank, world;
 };
 
@@ -958,6 +960,8 @@ __device__ __forceinline__ int pose_template(const PoseParams& p, const lm_match
 // One CTA per survivor slot.  Single frame (k_pose_cloud): launched for the bound, slots past the survivor count write
 // empty jobs.  Batch (k_pose_cloud_batch): launched for the exact slot count, the frame of each slot from p.frame_of.
 // Shared (k_pose_cloud_share): launched for this rank's share of the bound, slot i takes survivor p.rank + i * p.world.
+// Shared batch chunk (k_pose_cloud_batch_share): launched for this rank's share of the chunk, slot i takes chunk survivor
+// p.rank + i * p.world (p.counts[0]: the chunk's size) and reads that survivor's frame.
 template <bool BATCH, bool SHARE>
 __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   typedef cub::BlockScan<unsigned long long, POSE_THREADS> Scan;
@@ -973,11 +977,12 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   IcpJob* job = p.jobs + i;
   lm_match m = {0, 0, 0.f, 0, 0};
   PoseTpl T;
-  const int frame = BATCH ? p.frame_of[i] : 0;
+  const int si = SHARE ? p.rank + i * p.world : i;  // survivor of this slot
+  const bool in_chunk = !(BATCH && SHARE) || si < p.counts[0];
+  const int frame = BATCH ? (in_chunk ? p.frame_of[si] : 0) : 0;
   const uint16_t* __restrict__ scene = BATCH ? p.scene + (size_t)frame * p.srows * p.scols : p.scene;
   const float* __restrict__ bK = BATCH ? p.sKs + 9 * frame : nullptr;
-  const int si = SHARE ? p.rank + i * p.world : i;  // survivor of this slot
-  bool live = BATCH || si < p.counts[0];
+  bool live = BATCH ? in_chunk : si < p.counts[0];
   if (live) {
     m = p.surv[si];
     const int g = pose_template(p, m);
@@ -1110,6 +1115,7 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) { pose_cloud<false, false>(p); }
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch(PoseParams p) { pose_cloud<true, false>(p); }
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_share(PoseParams p) { pose_cloud<false, true>(p); }
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch_share(PoseParams p) { pose_cloud<true, true>(p); }
 
 // One CTA per cloud slot: mean of every occupied voxel, summed in sorted order (voxel_down_sample).
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals,
@@ -1367,6 +1373,9 @@ struct lm_pose_stage {
   PoseNmsOut* d_bnms = nullptr; PoseNmsOut* h_bnms = nullptr;
   int32_t* d_bfirst = nullptr; float* d_bsK = nullptr;  // [cap_bframes + 1], [cap_bframes][9]
   PoseNmsHead* d_bhead = nullptr; PoseNmsHead* h_bhead = nullptr;
+  // shared batch: per chunk (at most one per frame) [0] cloud overflow, [1] a peer's poses did not arrive, [2] entries
+  // this rank published, [3] the chunk's size (device, pinned copy)
+  int32_t* d_bstat = nullptr; int32_t* h_bstat = nullptr;
 };
 
 static void pose_free_frame(lm_pose_stage* s) {
@@ -1390,8 +1399,8 @@ void pose_stage_destroy(lm_pose_stage* s) {
   cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_err); cudaFree(s->d_rt); cudaFree(s->d_nms);
   cudaFreeHost(s->h_err); cudaFreeHost(s->h_nms);
   cudaFree(s->d_bscene); cudaFree(s->d_bsurv); cudaFree(s->d_bframe); cudaFree(s->d_bouts); cudaFree(s->d_bposed); cudaFree(s->d_bnms);
-  cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead);
-  cudaFreeHost(s->h_bouts); cudaFreeHost(s->h_bnms); cudaFreeHost(s->h_bhead);
+  cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead); cudaFree(s->d_bstat);
+  cudaFreeHost(s->h_bouts); cudaFreeHost(s->h_bnms); cudaFreeHost(s->h_bhead); cudaFreeHost(s->h_bstat);
   delete s;
 }
 
@@ -1512,6 +1521,18 @@ static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t ar
   return LM_OK;
 }
 
+// The device side of one pose exchange: number seq, survivor count counts[0], this rank's per-slot posed flags, status
+// as PoseShareDev.
+static PoseShareDev share_dev(const PoseShare& sh, int32_t seq, const int32_t* counts, const uint8_t* posed, int32_t* status) {
+  PoseShareDev sd;
+  memset(&sd, 0, sizeof(sd));
+  for (int r = 0; r < sh.world; ++r) sd.area[r] = sh.base[r] + sh.area_offset;
+  sd.world = sh.world; sd.rank = sh.rank; sd.seq = seq;
+  sd.counts = counts; sd.posed = posed; sd.status = status;
+  sd.timeout_ns = sh.timeout_ns; sd.abort_flag = sh.abort_flag;
+  return sd;
+}
+
 int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches) {
   cudaStream_t st = e.stream;
   if (s->dirty) {
@@ -1551,12 +1572,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
   dim3 g((unsigned)((A + 127) / 128), (unsigned)Bs);
   k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
   if (sh) {
-    PoseShareDev sd;
-    memset(&sd, 0, sizeof(sd));
-    for (int r = 0; r < sh->world; ++r) sd.area[r] = sh->base[r] + sh->area_offset;
-    sd.world = sh->world; sd.rank = sh->rank; sd.seq = sh->seq;
-    sd.counts = e.d_counts; sd.posed = s->d_posed; sd.status = s->d_err;
-    sd.timeout_ns = sh->timeout_ns; sd.abort_flag = sh->abort_flag;
+    const PoseShareDev sd = share_dev(*sh, sh->seq, e.d_counts, s->d_posed, s->d_err);
     k_icp_point_to_plane<true><<<Bs, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr, 0.01 * 0.01, e.max_iterations, 1e-6,
                                                            1e-6, nullptr, sd);
     k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_outs, s->d_posed);
@@ -1580,7 +1596,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
 // The stage's errors, after the stream has been synchronised.
 static int pose_status(const lm_pose_stage* s) {
   if (s->shared && s->h_err[1])
-    return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of frame %d within %llu ms (or an earlier collector "
+    return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d within %llu ms (or an earlier collector "
                    "on this device already gave up); every rank must run the pose stage of every frame while sharing is on",
                    s->share_seq, s->share_timeout_ns / 1000000ull);
   if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
@@ -1674,6 +1690,10 @@ int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, doub
 // ---- a batch of frames through one pose stage (lm_detect_batch) ----
 #define POSE_BATCH_CHUNK 1024  // survivor slots per chunk: the single-frame bound for top_k = 0
 
+int pose_batch_chunks(int64_t S) { return (int)((S + POSE_BATCH_CHUNK - 1) / POSE_BATCH_CHUNK); }
+
+static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S);
+
 int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
                        lm_match** d_surv) {
   const int64_t pix = (int64_t)n_frames * frame_pixels;
@@ -1691,14 +1711,28 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
     }
     if (n_frames > s->cap_bframes) {
       cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead); cudaFreeHost(s->h_bhead);
+      cudaFree(s->d_bstat); cudaFreeHost(s->h_bstat);
       s->d_bfirst = nullptr; s->d_bsK = nullptr; s->d_bhead = nullptr; s->h_bhead = nullptr; s->cap_bframes = 0;
+      s->d_bstat = nullptr; s->h_bstat = nullptr;
       CUI(cudaMalloc(&s->d_bfirst, sizeof(int32_t) * (n_frames + 1)));
       CUI(cudaMalloc(&s->d_bsK, sizeof(float) * 9 * n_frames));
       CUI(cudaMalloc(&s->d_bhead, sizeof(PoseNmsHead) * n_frames));
       CUI(cudaMallocHost(&s->h_bhead, sizeof(PoseNmsHead) * n_frames));
+      CUI(cudaMalloc(&s->d_bstat, sizeof(int32_t) * 4 * n_frames));  // chunks <= n_frames: a frame has <= 1024 survivors
+      CUI(cudaMallocHost(&s->h_bstat, sizeof(int32_t) * 4 * n_frames));
       s->cap_bframes = n_frames;
     }
   }
+  // and everything pose_batch_run may need for max_surv survivors: once frames run, no device memory is freed (a free
+  // waits for the whole device, a spinning peer collector of a shared batch included)
+  if (s->dirty) {
+    int rc = pose_upload(s, st);
+    if (rc) return rc;
+  }
+  int rc = pose_batch_survivors(s, st, std::max<int64_t>(max_surv, 1));
+  if (rc) return rc;
+  rc = pose_buffers(s, st, (int)std::min<int64_t>(std::max<int64_t>(max_surv, 1), POSE_BATCH_CHUNK), s->area_max);
+  if (rc) return rc;
   *d_scene = s->d_bscene;
   *d_surv = s->d_bsurv;
   return LM_OK;
@@ -1721,10 +1755,12 @@ static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S) {
   return LM_OK;
 }
 
-int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept) {
+int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4) {
   cudaStream_t st = b.stream;
   const int nf = b.n_frames;
   const int64_t S = b.first[nf];
+  const PoseShare* sh = b.share;
+  const int nc = pose_batch_chunks(S);
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
@@ -1742,34 +1778,52 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
   CUI(cudaMemcpyAsync(s->d_bfirst, first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
   CUI(cudaMemcpyAsync(s->d_bsK, b.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
   CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
+  if (sh && nc) {
+    std::vector<int32_t> stat((size_t)4 * nc, 0);
+    for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_BATCH_CHUNK, POSE_BATCH_CHUNK);
+    CUI(cudaMemcpyAsync(s->d_bstat, stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  }
   for (int64_t c0 = 0; c0 < S; c0 += POSE_BATCH_CHUNK) {
     const int C = (int)std::min<int64_t>(S - c0, POSE_BATCH_CHUNK);
+    const int c = (int)(c0 / POSE_BATCH_CHUNK);
+    // shared: this rank refines chunk survivors rank, rank + world, ... in n slots; a rank without one still publishes
+    const int n = sh ? (C + sh->world - 1) / sh->world : C;
+    int32_t* stat = sh ? s->d_bstat + 4 * c : nullptr;
     PoseParams p;
-    p.surv = s->d_bsurv + c0; p.counts = nullptr;
+    p.surv = s->d_bsurv + c0; p.counts = sh ? stat + 3 : nullptr;
     p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
     p.tpl = s->d_tpl; p.crops = s->d_crops;
     p.scene = s->d_bscene; p.srows = b.srows; p.scols = b.scols;
     memset(p.sK, 0, sizeof(p.sK));
     p.A = (int32_t)A; p.use_scene = b.use_scene_cloud ? 1 : 0;
     p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
-    p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * C;
-    p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_bposed + c0;
+    p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * n;
+    p.jobs = s->d_jobs; p.err = sh ? stat : s->d_err; p.posed = sh ? s->d_posed : s->d_bposed + c0;
     p.frame_of = s->d_bframe + c0; p.sKs = s->d_bsK;
-    p.rank = 0; p.world = 1;
-    k_pose_cloud_batch<<<C, POSE_THREADS, 0, st>>>(p);
+    p.rank = sh ? sh->rank : 0; p.world = sh ? sh->world : 1;
+    if (sh) k_pose_cloud_batch_share<<<n, POSE_THREADS, 0, st>>>(p);
+    else k_pose_cloud_batch<<<C, POSE_THREADS, 0, st>>>(p);
     cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
     cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
     size_t tmp_bytes = s->sort_tmp_bytes;
-    CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * C * A), 2 * C, p.seg_begin, p.seg_end, 0,
+    CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * n * A), 2 * n, p.seg_begin, p.seg_end, 0,
                                                  3 * POSE_KEY_BITS, st));
-    k_pose_voxel<<<2 * C, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
+    k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
                                                  p.use_scene);
-    dim3 g((unsigned)((A + 127) / 128), (unsigned)C);
+    dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
     k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
-    k_icp_point_to_plane<false><<<C, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, 0.01 * 0.01, b.max_iterations,
-                                                           1e-6, 1e-6, nullptr, PoseShareDev());
+    if (sh) {
+      // exchange seq + c: the results travel to every rank; the collector gathers the chunk in survivor order
+      const PoseShareDev sd = share_dev(*sh, sh->seq + c, stat + 3, s->d_posed, stat);
+      k_icp_point_to_plane<true><<<n, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr, 0.01 * 0.01, b.max_iterations, 1e-6,
+                                                            1e-6, nullptr, sd);
+      k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_bouts + c0, s->d_bposed + c0);
+    } else {
+      k_icp_point_to_plane<false><<<C, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, 0.01 * 0.01, b.max_iterations,
+                                                             1e-6, 1e-6, nullptr, PoseShareDev());
+    }
     CUI(cudaGetLastError());
-    *launches += 5;
+    *launches += sh ? 6 : 5;
   }
   if (b.pose_nms) {
     PoseNmsParams p;
@@ -1786,9 +1840,31 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
     CUI(cudaMemcpyAsync(s->h_bouts, s->d_bouts, sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
   }
   CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (sh && nc) CUI(cudaMemcpyAsync(s->h_bstat, s->d_bstat, sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
-  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  // shared: the overflow and late flags are ORed, the published entries summed over the chunks
+  int32_t overflow = *s->h_err, late = -1;
+  int64_t refined = S;
+  if (sh) {
+    refined = 0;
+    for (int c = 0; c < nc; ++c) {
+      overflow |= s->h_bstat[4 * c];
+      if (s->h_bstat[4 * c + 1] && late < 0) late = c;
+      refined += s->h_bstat[4 * c + 2];
+    }
+  }
+  if (late >= 0)
+    return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d (chunk %d of the batch) within %llu ms "
+                   "(or an earlier collector on this device already gave up); every rank must run every batch while sharing is on",
+                   sh->seq + late, late, sh->timeout_ns / 1000000ull);
+  if (overflow) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  if (stats4) {
+    stats4[0] = S;
+    stats4[1] = refined;
+    stats4[2] = (int64_t)nc * (sh ? 6 : 5);
+    stats4[3] = sh ? 1 : 0;
+  }
   if (b.pose_nms) {
     // the kept poses of every frame, each range where its frame's survivors begin
     bool more = false;

@@ -29,13 +29,14 @@ bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel
 // slot j takes survivor rank + j * world.  k_icp_point_to_plane<true> stores each survivor's result into the pose area
 // of every rank's exchange buffer and raises this rank's pose flag there; k_pose_collect waits for the world flags in
 // this rank's buffer and gathers the results in survivor order into the stage's own outputs, so pose_stage_finish and
-// the pose NMS read what the unshared stage leaves.  The pose area: [2 frame slots][1024 survivors] entries of 160 bytes,
-// then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket (pose_share_area_bytes in all).
+// the pose NMS read what the unshared stage leaves.  The pose area: [2 slots][1024 survivors] entries of 160 bytes,
+// then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket (pose_share_area_bytes in all).  Each pose exchange -- a
+// shared frame, or one chunk of a shared batch -- has its own number on the detector's pose counter.
 struct PoseShare {
   uint8_t* base[LM_MAX_PEERS];      // every rank's exchange buffer (peer mappings; this rank's own at [rank])
   uint64_t area_offset;             // byte offset of the pose area in every buffer
   int world, rank;
-  int32_t seq;                      // the frame's sequence number of the exchange; frame slot = seq & 1
+  int32_t seq;                      // the (first) pose exchange's number: slot = seq & 1; a batch's chunk c is seq + c
   unsigned long long timeout_ns;    // the collector gives up on a peer after this long
   int* abort_flag;                  // the device's abort flag of the exchange: raised on a timeout, honoured at once
 };
@@ -69,11 +70,14 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
 int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                           int64_t* n_out, int64_t* n_survivors, int64_t* n_posed);
 
-// A batch of frames through one pose stage (lm_detect_batch).  pose_batch_reserve returns room for n_frames scene depths
-// of frame_pixels each (frame f at d_scene + f * frame_pixels) and max_surv survivors, which the caller fills on the
-// stream: frame f's survivors at [first[f], first[f + 1]).
+// A batch of frames through one pose stage (lm_detect_batch, lm_peer_detect_batch).  pose_batch_reserve returns room for
+// n_frames scene depths of frame_pixels each (frame f at d_scene + f * frame_pixels) and max_surv survivors, which the
+// caller fills on the stream: frame f's survivors at [first[f], first[f + 1]).  It also uploads the renders and grows
+// every buffer pose_batch_run needs for max_surv survivors, so that the batch allocates no device memory once its frames run.
 int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
                        lm_match** d_surv);
+// Chunks of the pose stage of a batch with S survivors (each of at most 1024 slots).
+int pose_batch_chunks(int64_t S);
 struct PoseBatch {
   int n_frames, srows, scols;
   const int64_t* first;       // [n_frames + 1] survivor offsets (host)
@@ -83,10 +87,13 @@ struct PoseBatch {
   int pose_nms;               // 1: the pose NMS per frame (k_pose_nms_batch), 0: the host composes the poses
   double thr;
   cudaStream_t stream;
+  const PoseShare* share;     // null: this rank refines every survivor; else chunk c is pose exchange share->seq + c
 };
 // The pose stage over every survivor of the batch in chunks of at most 1024 slots, then (pose_nms) one pose NMS launch
 // for all frames; waits.  posed[f] / kept[f]: frame f's survivors with a pose, and its entries (kept poses, or every
-// survivor without the pose NMS).
-int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept);
+// survivor without the pose NMS).  Shared: within a chunk of C survivors, survivor i is refined by rank i % world in
+// ceil(C / world) slots (k_pose_cloud_batch_share, k_icp_point_to_plane<true>), and k_pose_collect gathers the chunk
+// into the batch's outputs.  stats4 (may be null): what lm_pose_stats returns for the batch.
+int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4);
 // Frame f's kept[f] entries after pose_batch_run, outputs as lm_complete_detect (pose_nms) or lm_complete_pose.
 void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual);

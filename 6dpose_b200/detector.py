@@ -271,7 +271,8 @@ class Detector:
         """match_refine for many frames in one call: each frame's match and box NMS, then one pose stage for the survivors
         of all of them, which fills the GPU where one frame's few survivors cannot.  frames: a sequence of [rgb, depth]
         pairs of one size; sceneK: one 3x3 matrix or one per frame; masks: [] or one masks list per frame.  Returns one
-        list per frame, each equal to match_refine on that frame."""
+        list per frame, each equal to match_refine on that frame.  The handle keeps the batch's device buffers, sized
+        for the batch's shape (frames, size, top_k; with top_k=0 the pose buffers of 1024 survivors), for the next one."""
         nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "match_refine_batch()")
         got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
                                bool(use_scene_cloud), pose_nms=False)

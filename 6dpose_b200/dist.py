@@ -49,8 +49,9 @@ def connect_peers(detector, group=None, capacity_records=8192, class_ids=(), sha
     """One-time setup of the fused exchange: every rank exports its buffer's CUDA IPC handle, the
     handles travel through the process group (any backend), every rank maps the others' buffers.
 
-    share_pose: divide the pose stage of Detector.detect / match_refine over the ranks (lm_peer_share_pose).  Only
-    for callers whose every rank runs the pose stage of every frame."""
+    share_pose: divide the pose stage of Detector.detect / match_refine and of detect_batch_sharded /
+    match_refine_batch_sharded over the ranks (lm_peer_share_pose).  Only for callers whose every rank runs the pose
+    stage of every frame."""
     import torch.distributed as dist
     if not isinstance(share_pose, (bool, int, np.bool_, np.integer)):
         raise TypeError("connect_peers(share_pose=...): a bool, got %s" % type(share_pose).__name__)
@@ -76,6 +77,37 @@ def disconnect_peers(detector, group=None):
     detector._peers = None
     detector.shard = (0, 1)
     dist.barrier(group=group)
+
+
+def _connected_batch(detector, frames, class_ids, sceneK, masks, group, what):
+    # the native handle and its arguments for lm_peer_detect_batch; nothing touches a device before the checks
+    import torch.distributed as dist
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    if getattr(detector, "_peers", None) != (rank, world):
+        raise RuntimeError("%s needs a detector connected to the peer exchange of rank %d of %d (dist.connect_peers)" % (what, rank, world))
+    return detector._batch_args(frames, class_ids, sceneK, masks, what)
+
+
+def match_refine_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
+                               use_scene_cloud=False, masks=[], group=None):
+    """Detector.match_refine_batch with the bank sharded over the connected peer exchange (lm_peer_detect_batch); with
+    connect_peers(share_pose=True) the pose stage is divided over the ranks too.  Every rank calls it with the same
+    arguments and returns the whole result, equal to match_refine_batch on one unconnected detector."""
+    nat, (rgb, depth, mk, K) = _connected_batch(detector, frames, class_ids, sceneK, masks, group, "match_refine_batch_sharded()")
+    got = nat.peer_detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
+                                bool(use_scene_cloud), pose_nms=False)
+    return [detector._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+
+
+def detect_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
+                         max_iterations=30, use_scene_cloud=False, masks=[], group=None):
+    """Detector.detect_batch with the bank sharded over the connected peer exchange (lm_peer_detect_batch), as
+    match_refine_batch_sharded: every rank calls it and returns the whole result, equal to detect_batch on one
+    unconnected detector."""
+    nat, (rgb, depth, mk, K) = _connected_batch(detector, frames, class_ids, sceneK, masks, group, "detect_batch_sharded()")
+    got = nat.peer_detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
+                                bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold))
+    return [detector._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
 
 def match_quantized_sharded(detector, quantized, threshold, class_ids=(), group=None):

@@ -185,7 +185,9 @@ int lm_peer_disconnect(lm_detector* d);
  *                       peer's pose collector included -- so run such a frame unshared first.
  * A peer whose poses do not arrive within LINEMOD_B200_PEER_TIMEOUT_MS fails the frame with LM_E_STATE (the message names
  * the pose exchange) and raises the device's abort flag of the exchange, as the record collector does.
- * lm_detect_batch still refuses a connected exchange. */
+ * Each pose exchange -- a shared frame, or one chunk of a shared lm_peer_detect_batch -- takes the next number of the
+ * handle's pose counter (reset by lm_peer_export), and consecutive exchanges alternate between the two slots of the pose
+ * area.  lm_detect_batch still refuses a connected exchange; lm_peer_detect_batch is its connected form. */
 int lm_peer_share_pose(lm_detector* d, int on);
 
 /* Copy the kept records of the last completed run to the host, sorted by (work, seq). */
@@ -298,21 +300,53 @@ int lm_nms_translations(int device, int64_t n, const double* t, const double* sc
  *                  pick order; residual -1 and R / t untouched on the early return of LL.cpp:52-55.
  *   pose_nms == 1  the same chain plus lm_enqueue_pose_nms, lm_complete_detect: the kept poses, in keep order.
  * frame_counts[4f .. 4f + 3] = entries, box-NMS survivors, survivors with a pose, kept records the box NMS saw.
- * *n_out = entries of the whole batch.  LM_E_CAPACITY (with *n_out the total needed) when cap is smaller;
+ * *n_out = entries of the whole batch.  LM_E_CAPACITY (with *n_out the total needed) when cap is smaller (an
+ * LM_E_CAPACITY that leaves *n_out unwritten comes from a frame's match, where growing cap does not help);
  * LM_E_INVALID for n_frames < 1 or a NaN / negative translation threshold with pose_nms; LM_E_STATE without renders
- * for every selected template, and with a connected peer exchange (the batch is single-GPU only).
+ * for every selected template, and with a connected peer exchange (use lm_peer_detect_batch there).
  * Each frame runs the single-frame match and box NMS and waits for them (a frame whose records outgrow the result block
  * is redone there); its survivors and depth are copied aside on the stream.  The pose stage then runs once over all
  * S survivors in chunks of at most 1024 slots (the single-frame bound for top_k = 0, so its cloud buffers do not grow
- * with the batch): 5 launches per chunk, plus 1 launch of the pose NMS for every frame.  Extra device memory, kept by
- * the handle for the next batch: n_frames depth slots (rows * cols * 2 bytes each, 614 KB at 640 x 480),
- * n_frames * (top_k, or 1024) survivor slots of 20 bytes, and per survivor its ICP output, pose NMS entry, frame index
- * and posed flag (about 280 bytes, plus a pinned host copy of the first two). */
+ * with the batch): 5 launches per chunk, plus 1 launch of the pose NMS for every frame.  Before its first frame the call
+ * uploads the renders and grows every buffer a batch of its shape (n_frames, rows x cols, top_k) may need.  Extra device
+ * memory, kept by the handle for the next batch: n_frames depth slots (rows * cols * 2 bytes each, 614 KB at 640 x 480),
+ * n_frames * (top_k, or 1024) survivor slots of 20 bytes, for each of those slots an ICP output, pose NMS entry, frame
+ * index and posed flag (about 280 bytes, plus a pinned host copy of the first two), and the pose stage's cloud buffers
+ * for min(n_frames * (top_k, or 1024), 1024) survivors. */
 int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
                     const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
                     int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm,
                     lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out,
                     int64_t* frame_counts);
+
+/* lm_detect_batch over the ranks of a connected peer exchange, with the same arguments and outputs.  Every rank returns
+ * what one unconnected handle over the whole bank returns from lm_detect_batch on the same frames, bit for bit: the
+ * entries, R, t, residual (NaN patterns included) and all four frame_counts of every frame.  Calling it is the caller's
+ * promise that every rank calls it with the same frames and arguments, in the same order as its other frames.
+ *   Match      each frame's match runs the fused record exchange, as a connected single frame does, and its box NMS
+ *              sees every shard's records, so every rank holds the same S survivors and the same chunks.
+ *   Pose       sharing off: every rank refines every survivor (5 launches per chunk).  Sharing on (lm_peer_share_pose):
+ *              within a chunk of C survivors, survivor i is refined by rank i % world in ceil(C / world) slots, and the
+ *              results travel through the pose area as for a shared frame (6 launches per chunk; a rank without a
+ *              survivor in the chunk still publishes).  Each chunk is one pose exchange.  Then 1 pose NMS launch.
+ * LM_E_STATE without a connected exchange; the other argument and state errors are those of lm_detect_batch and come
+ * before any device work.  LM_E_CAPACITY for too small outputs (*n_out = the total needed, > cap) comes on every rank
+ * alike (the totals are the same), so a caller that grows cap and calls again does so on every rank.  LM_E_CAPACITY
+ * with *n_out not written means a frame's records outgrew the exchange (a shard kept more than lm_peer_export's
+ * capacity_records; the message names the peer exchange) or the result block, which does not grow while connected;
+ * every rank sees it at the same frame, and calling again fails again: reconnect with a larger capacity.  A peer whose poses do not arrive in time fails the batch with LM_E_STATE
+ * (the message names the pose exchange).  No device memory is allocated or freed once the first frame is enqueued.
+ * Ranks that are handles of ONE process on ONE device call from their own host threads, and each first runs one
+ * unconnected lm_detect_batch of the largest shape (n_frames, frame size, top_k) it will run connected: that one
+ * uploads the renders and grows the buffers, which frees device memory, and a free waits for the whole device -- a
+ * peer's collector included.  For the same reason, once connected, every rank calls lm_prepare (which grows the result
+ * block to the exchange's size) before any rank enqueues a frame.  lm_pose_stats afterwards: S, the hypotheses this rank refined over all chunks, the pose
+ * stage's launches (chunks x 6 shared, x 5 unshared; the pose NMS not counted) and 1 if shared. */
+int lm_peer_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                         const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+                         int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm,
+                         lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out,
+                         int64_t* frame_counts);
 
 /* Convenience = lm_upload_quantized + lm_run + lm_fetch_records + lm_finish (single GPU):
  * Detector::match after quantization. */
@@ -349,7 +383,8 @@ void* lm_stream(lm_detector* d);
 /* Number of kernel launches issued by this handle since creation (the pose stage's CUB segmented sort counts as one;
  * a frame's pose stage is 5, whatever its survivor count; 6 when shared over the exchange). */
 int64_t lm_launch_count(lm_detector* d);
-/* About the last pose stage this handle completed (lm_complete_pose / lm_complete_detect): [0] box-NMS survivors,
+/* About the last pose stage this handle completed (lm_complete_pose / lm_complete_detect; lm_peer_detect_batch: see there,
+ * lm_detect_batch leaves it as it was): [0] box-NMS survivors,
  * [1] hypotheses this rank refined (all survivors unshared; its share with lm_peer_share_pose, as counted by the ICP
  * kernel), [2] launches of the stage, [3] 1 if it was shared.  Zeros before the first.  `out4` has 4 entries. */
 int lm_pose_stats(lm_detector* d, int64_t* out4);

@@ -10,7 +10,9 @@
 # the filter does not take, k_refine<true> behind the filter (unsafe templates, three levels), k_refine_prep deriving the
 # H-planes from the byte linear memories, and (d) memcheck over lm_detect_batch: a batch whose survivors span two pose
 # chunks, and one with early returns and NaN anchors, and (e) the pose stage shared over two handles of one process (peer
-# stores of the ICP kernel, its ticket and pose flags, the pose collector's spin wait).
+# stores of the ICP kernel, its ticket and pose flags, the pose collector's spin wait), and (f) memcheck over
+# lm_peer_detect_batch with three handles of one process: a shared batch of two pose chunks, one with fewer survivors
+# than ranks and an all-blank one (k_pose_cloud_batch_share, the per-chunk pose exchanges).
 # Usage (on a GPU box):  bash tools/sanitize.sh [outdir]      -> <outdir>/summary.txt, one log per tool x case
 set -u
 OUT=${1:-gpurun_out/sanitize}
@@ -39,4 +41,6 @@ for tool in memcheck racecheck synccheck; do
   run "$tool" pose_share2 python -m pytest "tests/test_gpu_pose_share.py::test_every_rank_returns_the_single_gpu_result[2]" -x -q \
     -p no:cacheprovider
 done
+run memcheck peer_batch3 python -m pytest "tests/test_gpu_peer_batch.py::test_two_chunks_few_survivors_and_a_blank_batch" -x -q \
+  -p no:cacheprovider
 echo "done: $(cat "$OUT/summary.txt" | wc -l) runs" | tee -a "$OUT/summary.txt"
