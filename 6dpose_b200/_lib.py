@@ -31,10 +31,22 @@ SYMBOLS = [
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
     "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations", "lm_detect_batch", "lm_peer_detect_batch",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect", "lm_peer_share_pose",
-    "lm_pose_stats",
+    "lm_pose_stats", "lm_set_pose_estimation",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
-    "lm_icp_set_capture", "lm_icp_capture",
+    "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture",
 ]
+
+# The ICP's estimation step (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT of include/linemod_b200.h) by the name the
+# Python surface takes
+ESTIMATIONS = {"point_to_plane": 0, "point_to_point": 1}
+
+
+def estimation_code(estimation):
+    """The C-ABI value of estimation="point_to_plane" | "point_to_point"; ValueError for anything else (no device work)."""
+    if not isinstance(estimation, str) or estimation not in ESTIMATIONS:
+        raise ValueError("estimation must be one of %s, got %r" % (", ".join(repr(k) for k in ESTIMATIONS), estimation))
+    return ESTIMATIONS[estimation]
+
 
 _lib = None
 
@@ -89,6 +101,7 @@ def load():
     L.lm_peer_disconnect.argtypes = [vp]
     L.lm_peer_share_pose.argtypes = [vp, c_int]
     L.lm_pose_stats.argtypes = [vp, ctypes.POINTER(c_i64)]
+    L.lm_set_pose_estimation.argtypes = [vp, c_int]
     L.lm_device_result.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(c_i64)]
     L.lm_fetch_records.argtypes = [vp, vp, c_i64, ctypes.POINTER(c_i64)]
     L.lm_finish.argtypes = [vp, vp, c_i64, vp, c_i64, ctypes.POINTER(c_i64)]
@@ -123,6 +136,7 @@ def load():
                                        i32p, c_int, f64p, f64p, f32p]
     L.lm_icp_last_stats.argtypes = [vp, f64p]
     L.lm_icp_set_use_scene_cloud.argtypes = [vp, c_int]
+    L.lm_icp_set_estimation.argtypes = [vp, c_int]
     L.lm_icp_launch_count.argtypes = [vp]
     L.lm_icp_launch_count.restype = c_i64
     L.lm_icp_set_capture.argtypes = [vp, c_int]
@@ -427,8 +441,14 @@ class NativeDetector:
         check(self._L.lm_set_template_renders(self._h, int(first), n, ptrs, int(rows), int(cols), K.ctypes.data_as(f32p),
                                               R.ctypes.data_as(f32p), t.ctypes.data_as(f32p)))
 
-    def enqueue_pose(self, sceneK, max_iterations=30, use_scene_cloud=False):
+    def set_pose_estimation(self, estimation):
+        """"point_to_plane" (default) or "point_to_point" for the next pose stage (lm_set_pose_estimation)."""
+        check(self._L.lm_set_pose_estimation(self._h, estimation_code(estimation)))
+
+    def enqueue_pose(self, sceneK, max_iterations=30, use_scene_cloud=False, estimation="point_to_plane"):
+        est = estimation_code(estimation)
         sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+        check(self._L.lm_set_pose_estimation(self._h, est))
         check(self._L.lm_enqueue_pose(self._h, sK.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), int(max_iterations),
                                       1 if use_scene_cloud else 0))
 
@@ -447,12 +467,14 @@ class NativeDetector:
         k = n.value
         return out[:k].copy(), Ro[:k].copy(), to[:k].copy(), res[:k].copy(), int(nrec.value)
 
-    def match_pose(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30, use_scene_cloud=False):
+    def match_pose(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30, use_scene_cloud=False,
+                   estimation="point_to_plane"):
         """upload_images + enqueue + enqueue_post + enqueue_pose + complete_pose: one chain on the detector's stream."""
+        estimation_code(estimation)
         self.upload_images(rgb, depth, masks)
         self.enqueue(threshold)
         self.enqueue_post(iou_threshold, top_k)
-        self.enqueue_pose(sceneK, max_iterations, use_scene_cloud)
+        self.enqueue_pose(sceneK, max_iterations, use_scene_cloud, estimation)
         return self.complete_pose()
 
     # ---- pose NMS behind the pose stage (include/linemod_b200.h, lm_enqueue_pose_nms / lm_complete_detect) ----
@@ -477,40 +499,44 @@ class NativeDetector:
                 dict(survivors=int(ns.value), posed=int(npo.value), records=int(nrec.value)))
 
     def detect(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30, use_scene_cloud=False,
-               translation_threshold=40.0):
+               translation_threshold=40.0, estimation="point_to_plane"):
         """upload_images + enqueue + enqueue_post + enqueue_pose + enqueue_pose_nms + complete_detect: RGB-D frame to the
         object list in one chain on the detector's stream."""
+        estimation_code(estimation)
         self.upload_images(rgb, depth, masks)
         self.enqueue(threshold)
         self.enqueue_post(iou_threshold, top_k)
-        self.enqueue_pose(sceneK, max_iterations, use_scene_cloud)
+        self.enqueue_pose(sceneK, max_iterations, use_scene_cloud, estimation)
         self.enqueue_pose_nms(translation_threshold)
         return self.complete_detect()
 
     # ---- a batch of frames through one pose stage (include/linemod_b200.h, lm_detect_batch) ----
     def detect_batch(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30, use_scene_cloud=False,
-                     pose_nms=True, translation_threshold=40.0, cap=None):
+                     pose_nms=True, translation_threshold=40.0, cap=None, estimation="point_to_plane"):
         """rgb [n,H,W,3] u8, depth [n,H,W] u16, masks None or one (mask_color, mask_depth) pair per frame (None or an empty
         array: no mask), sceneK [n,3,3].  Returns one tuple per frame: what complete_detect returns (pose_nms) or what
         complete_pose returns.  cap: entries of the first attempt (default: every survivor of every frame); a larger
         batch result grows it and runs the batch again; any other LM_E_CAPACITY raises.  self.batch_counts keeps the last
         call's [n,4] frame counts (entries, survivors, posed, records).  The handle keeps the batch's buffers for the next
         one, sized for its shape: with top_k 0 that includes the pose stage's cloud buffers for 1024 survivors (as a
-        single frame with top_k 0 uses), however few survivors the frames have."""
+        single frame with top_k 0 uses), however few survivors the frames have.  estimation: the ICP's estimation step
+        (set_pose_estimation)."""
         return self._batch(self._L.lm_detect_batch, rgb, depth, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
-                           use_scene_cloud, pose_nms, translation_threshold, cap)
+                           use_scene_cloud, pose_nms, translation_threshold, cap, estimation)
 
     def peer_detect_batch(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30,
-                          use_scene_cloud=False, pose_nms=True, translation_threshold=40.0, cap=None):
+                          use_scene_cloud=False, pose_nms=True, translation_threshold=40.0, cap=None, estimation="point_to_plane"):
         """detect_batch over the ranks of the connected exchange (lm_peer_detect_batch): every rank calls it with the same
         frames and arguments, and every rank returns what detect_batch returns on one unconnected handle over the whole
         bank.  The retry on too small outputs happens on every rank alike; records beyond the exchange's
-        capacity_records raise LinemodLibraryError on every rank (reconnect with a larger capacity)."""
+        capacity_records raise LinemodLibraryError on every rank (reconnect with a larger capacity).  Every rank passes the
+        same estimation."""
         return self._batch(self._L.lm_peer_detect_batch, rgb, depth, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
-                           use_scene_cloud, pose_nms, translation_threshold, cap)
+                           use_scene_cloud, pose_nms, translation_threshold, cap, estimation)
 
     def _batch(self, fn, rgb, depth, masks, threshold, sceneK, iou_threshold, top_k, max_iterations, use_scene_cloud, pose_nms,
-               translation_threshold, cap):
+               translation_threshold, cap, estimation="point_to_plane"):
+        est = estimation_code(estimation)
         rgb = np.ascontiguousarray(rgb)
         depth = np.ascontiguousarray(depth)
         if rgb.dtype != np.uint8 or rgb.ndim != 4 or rgb.shape[3] != 3:
@@ -541,6 +567,7 @@ class NativeDetector:
         cap = n * bound if cap is None else max(int(cap), 1)
         counts = np.zeros((n, 4), np.int64)
         f32p, f64p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
+        check(self._L.lm_set_pose_estimation(self._h, est))
         while True:
             out = np.empty(cap, MATCH_DTYPE)
             Ro = np.full((cap, 3, 3), np.nan, np.float64)
@@ -615,6 +642,8 @@ class NativeIcp:
         h = ctypes.c_void_p()
         check(L.lm_icp_create(int(device), ctypes.byref(h)))
         self._h = h
+        self._estimation = "point_to_plane"  # the handle's estimation (lm_icp_set_estimation)
+        self._captured = None               # the estimation of the last process_batch (capture())
 
     def close(self):
         if getattr(self, "_h", None):
@@ -627,9 +656,12 @@ class NativeIcp:
         except Exception:
             pass
 
-    def process_batch(self, scene_depth, model_depths, sceneK, modelKs, Rs, ts, detect_xy, max_iterations=30):
+    def process_batch(self, scene_depth, model_depths, sceneK, modelKs, Rs, ts, detect_xy, max_iterations=30, estimation=None):
         """scene u16 HxW; model_depths list of u16 HxW (same size); modelKs/Rs [n,3,3] f32; ts [n,3] f32;
-        detect_xy [n,2] int.  Returns (R [n,3,3] f64, t [n,3] f64 mm, residual [n] f32)."""
+        detect_xy [n,2] int.  estimation: "point_to_plane" or "point_to_point" for this call and the next ones (None: as
+        set before, point-to-plane on a new handle).  Returns (R [n,3,3] f64, t [n,3] f64 mm, residual [n] f32)."""
+        if estimation is not None:
+            self.set_estimation(estimation)
         n = len(model_depths)
         scene = np.ascontiguousarray(scene_depth, np.uint16)
         models = [np.ascontiguousarray(m, np.uint16) for m in model_depths]
@@ -653,10 +685,16 @@ class NativeIcp:
                                            t.ctypes.data_as(f32p), xy.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
                                            int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
                                            res.ctypes.data_as(f32p)))
+        self._captured = self._estimation
         return Ro, to, res
 
     def set_use_scene_cloud(self, on):
         check(self._L.lm_icp_set_use_scene_cloud(self._h, 1 if on else 0))
+
+    def set_estimation(self, estimation):
+        """"point_to_plane" (the reference's active branch, default) or "point_to_point" (lm_icp_set_estimation)."""
+        check(self._L.lm_icp_set_estimation(self._h, estimation_code(estimation)))
+        self._estimation = estimation
 
     def set_capture(self, on):
         check(self._L.lm_icp_set_capture(self._h, 1 if on else 0))
@@ -668,15 +706,17 @@ class NativeIcp:
     def capture(self, hyp):
         """What the kernels saw and kept for hypothesis `hyp` of the last process_batch with capture on (see
         lm_icp_capture): source / target [n,3] f64, normals [nt,3] f64, init [4,4] f64, T [4,4] f64, fitness, rmse,
-        iterations, knn [nt,30] int32 (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence)."""
+        iterations, knn [nt,30] int32 (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence).  After a
+        point-to-point call normals and knn are None: that estimation computes neither."""
         n, nt = self._capture_item(hyp, 0, np.zeros(2, np.int32)).tolist()
         res = self._capture_item(hyp, 5, np.zeros(19, np.float64))
+        p2pl = self._captured != "point_to_point"
         return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
                     target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)),
-                    normals=self._capture_item(hyp, 3, np.zeros((nt, 3), np.float64)),
+                    normals=self._capture_item(hyp, 3, np.zeros((nt, 3), np.float64)) if p2pl else None,
                     init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
                     T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
-                    knn=self._capture_item(hyp, 6, np.zeros((nt, 30), np.int32)),
+                    knn=self._capture_item(hyp, 6, np.zeros((nt, 30), np.int32)) if p2pl else None,
                     corr_first=self._capture_item(hyp, 7, np.zeros(n, np.int32)),
                     corr_last=self._capture_item(hyp, 8, np.zeros(n, np.int32)))
 

@@ -194,6 +194,8 @@ struct lm_detector {
   bool pose_nms_pending = false;        // lm_enqueue_pose_nms: the frame completes through lm_complete_detect
   double pose_nms_thr = 40.0;
   float pose_sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; int pose_max_iter = 30, pose_use_scene = 0;
+  int pose_estimation = LM_ICP_POINT_TO_PLANE;       // lm_set_pose_estimation: for the next pose stage
+  int pose_frame_estimation = LM_ICP_POINT_TO_PLANE; // the enqueued frame's (its rerun after a retry keeps it)
   int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
@@ -2062,6 +2064,7 @@ static int enqueue_pose(lm_detector* d) {
   e.bound = d->post_top_k > 0 ? std::min(d->post_top_k, LM_POST_MAX) : LM_POST_MAX;
   e.use_scene_cloud = d->pose_use_scene;
   e.max_iterations = d->pose_max_iter;
+  e.estimation = d->pose_frame_estimation;
   e.stream = d->stream;
   return pose_stage_enqueue(d->pose, e, &d->launches);
 }
@@ -2078,6 +2081,7 @@ extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iter
   memcpy(d->pose_sK, sceneK, sizeof(d->pose_sK));
   d->pose_max_iter = max_iterations;
   d->pose_use_scene = use_scene_cloud ? 1 : 0;
+  d->pose_frame_estimation = d->pose_estimation;
   d->pose_nms_pending = false;  // a new pose stage: any pose NMS enqueued before belongs to an abandoned frame
   int rc = enqueue_pose(d);
   if (rc) return rc;
@@ -2132,6 +2136,14 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
   rc = pose_stage_finish_nms(d->pose, d->stream, out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
   if (rc) return rc;
   pose_stage_stats(d->pose, n_surv, d->pose_stats);
+  return LM_OK;
+}
+
+extern "C" int lm_set_pose_estimation(lm_detector* d, int estimation) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT)
+    return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
+  d->pose_estimation = estimation;
   return LM_OK;
 }
 
@@ -2197,6 +2209,7 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
   b.n_frames = n_frames; b.srows = rows; b.scols = cols;
   b.first = first.data(); b.surv = surv.data(); b.sK = sceneK;
   b.use_scene_cloud = use_scene_cloud ? 1 : 0; b.max_iterations = max_iterations;
+  b.estimation = d->pose_estimation;
   b.pose_nms = pose_nms ? 1 : 0; b.thr = translation_threshold_mm;
   b.stream = st;
   PoseShare sh;

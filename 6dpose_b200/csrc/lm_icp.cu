@@ -10,6 +10,9 @@
 //                            nearest-neighbour correspondence search fused with the 6x6 J^T J / J^T r
 //                            accumulation, the 6x6 solve and the convergence test; every iteration of
 //                            one hypothesis runs inside one CTA, one launch for a batch of hypotheses
+//   k_icp_point_to_point  <- RegistrationICP + TransformationEstimationPointToPoint (LL.cpp:131-135, the branch the
+//                            reference takes without USE_OPEN3D_P2PL; lm_icp_set_estimation / lm_set_pose_estimation):
+//                            the same loop with a closed-form rigid fit (Umeyama) per pass, and no normals
 // All arithmetic is double, as in Open3D/Eigen.  The reference's quirks are kept: the ICP target is the
 // down-sampled MODEL cloud (LL.cpp:109), only the z component of the initial translation is converted
 // to metres (LL.cpp:37), `residual` carries the fitness (LL.cpp:148).
@@ -294,23 +297,179 @@ __device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const
     reinterpret_cast<volatile int32_t*>(sh.area[q] + POSE_SHARE_FLAGS)[slot * LM_MAX_PEERS + sh.rank] = sh.seq;
 }
 
+// ---- the estimation step of RegistrationICP: one class per TransformationEstimation ----
+// Each keeps NACC sums per thread, of which [ERR] is the squared distance and [CNT] the number of the correspondences.
+// add() takes one correspondence (p the transformed source point, v its target point, index bj); update() turns the
+// block's totals into the 3x4 update matrix (thread 0).
+
+// TransformationEstimationPointToPlane (LL.cpp:128-130): J^T J and J^T r of r = (p - q) . n_q, the 6x6 solve, and
+// TransformVector6dToMatrix4d of the solution.
+struct IcpPointToPlane {
+  static constexpr int NACC = ICP_NACC, ERR = 27, CNT = 28;
+  const double* __restrict__ Nm;  // target normals (k_icp_normals)
+  __device__ __forceinline__ IcpPointToPlane(const IcpJob& job, const double*, const double* normals)
+      : Nm(normals + (size_t)job.tgt_first * 3) {}
+  __device__ __forceinline__ void add(double* acc, double px, double py, double pz, double vx, double vy, double vz, int bj,
+                                      double best) const {
+    const double nx = Nm[3 * bj], ny = Nm[3 * bj + 1], nz = Nm[3 * bj + 2];
+    const double r = (px - vx) * nx + (py - vy) * ny + (pz - vz) * nz;
+    const double J[6] = {py * nz - pz * ny, pz * nx - px * nz, px * ny - py * nx, nx, ny, nz};
+    int q = 0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+      for (int b = a; b < 6; ++b) acc[q++] += J[a] * J[b];
+#pragma unroll
+    for (int a = 0; a < 6; ++a) acc[21 + a] += J[a] * r;
+    acc[27] += best;
+    acc[28] += 1.0;
+  }
+  __device__ __forceinline__ void update(const double* tot, double* U) const {
+    double A[6][6], b[6], x[6] = {0, 0, 0, 0, 0, 0};
+    int q = 0;
+    for (int a = 0; a < 6; ++a)
+      for (int c = a; c < 6; ++c) { A[a][c] = tot[q]; A[c][a] = tot[q]; ++q; }
+    for (int a = 0; a < 6; ++a) b[a] = -tot[21 + a];
+    solve6(A, b, x);
+    // TransformVector6dToMatrix4d: Rz(x2) Ry(x1) Rx(x0), translation x3..5
+    const double cx = cos(x[0]), sx = sin(x[0]), cy = cos(x[1]), sy = sin(x[1]), cz = cos(x[2]), sz = sin(x[2]);
+    U[0] = cz * cy; U[1] = cz * sy * sx - sz * cx; U[2] = cz * sy * cx + sz * sx; U[3] = x[3];
+    U[4] = sz * cy; U[5] = sz * sy * sx + cz * cx; U[6] = sz * sy * cx - cz * sx; U[7] = x[4];
+    U[8] = -sy;     U[9] = cy * sx;                U[10] = cy * cx;               U[11] = x[5];
+  }
+};
+
+// The rotation of Eigen's umeyama(src, dst, false) from sig = (1/n) sum (q - qbar)(p - pbar)^T: sig = U diag(d) V^T
+// (one-sided Jacobi: plane rotations accumulated into V orthogonalise the columns of sig, d descending), then
+// R = U S V^T with S = diag(1, 1, -1) when det U det V < 0.  U is completed to a right-handed orthonormal basis, which
+// leaves R unchanged where sig has full rank (the sign of U's last column and S flip together) and makes it one of the
+// optimal proper rotations where it has not (one pair: sig = 0 and R = I exactly; two or collinear pairs: rank 1).
+__device__ void umeyama_rotation(const double sig[3][3], double R[3][3]) {
+  double a[3][3], v[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) a[r][c] = sig[r][c];
+  for (int sweep = 0; sweep < 32; ++sweep) {
+    bool rotated = false;
+    for (int p = 0; p < 2; ++p)
+      for (int q = p + 1; q < 3; ++q) {
+        double al = 0, be = 0, ga = 0;
+        for (int k = 0; k < 3; ++k) { al += a[k][p] * a[k][p]; be += a[k][q] * a[k][q]; ga += a[k][p] * a[k][q]; }
+        if (!(fabs(ga) > 1e-15 * sqrt(al) * sqrt(be))) continue;  // columns p, q orthogonal to rounding (or NaN)
+        const double zeta = (be - al) / (2.0 * ga);
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
+        for (int k = 0; k < 3; ++k) {
+          const double ap = a[k][p], aq = a[k][q];
+          a[k][p] = c * ap - s * aq;
+          a[k][q] = s * ap + c * aq;
+          const double vp = v[k][p], vq = v[k][q];
+          v[k][p] = c * vp - s * vq;
+          v[k][q] = s * vp + c * vq;
+        }
+        rotated = true;
+      }
+    if (!rotated) break;
+  }
+  double d[3];
+  for (int c = 0; c < 3; ++c) d[c] = sqrt(a[0][c] * a[0][c] + a[1][c] * a[1][c] + a[2][c] * a[2][c]);
+  int o[3] = {0, 1, 2};  // columns by singular value, descending
+  if (d[o[1]] > d[o[0]]) { const int t = o[0]; o[0] = o[1]; o[1] = t; }
+  if (d[o[2]] > d[o[1]]) { const int t = o[1]; o[1] = o[2]; o[2] = t; }
+  if (d[o[1]] > d[o[0]]) { const int t = o[0]; o[0] = o[1]; o[1] = t; }
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) R[r][c] = r == c ? 1.0 : 0.0;
+  const double d1 = d[o[0]];
+  if (!(d1 > 0.0)) return;  // no spread (one pair), or a NaN
+  double u[3][3];           // u[j]: column j of U
+  for (int k = 0; k < 3; ++k) u[0][k] = a[k][o[0]] / d1;
+  double w[3], dot = 0;
+  for (int k = 0; k < 3; ++k) dot += a[k][o[1]] * u[0][k];
+  for (int k = 0; k < 3; ++k) w[k] = a[k][o[1]] - dot * u[0][k];
+  double nw = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
+  if (!(nw > 1e-13 * d1)) {  // rank 1: any unit vector orthogonal to u0, from the axis u0 is least aligned with
+    int m = 0;
+    if (fabs(u[0][1]) < fabs(u[0][m])) m = 1;
+    if (fabs(u[0][2]) < fabs(u[0][m])) m = 2;
+    for (int k = 0; k < 3; ++k) w[k] = (k == m ? 1.0 : 0.0) - u[0][m] * u[0][k];
+    nw = sqrt(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
+  }
+  for (int k = 0; k < 3; ++k) u[1][k] = w[k] / nw;
+  u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];
+  u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
+  u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+  double vc[3][3];  // vc[j]: column o[j] of V
+  for (int j = 0; j < 3; ++j)
+    for (int k = 0; k < 3; ++k) vc[j][k] = v[k][o[j]];
+  const double det_v = vc[0][0] * (vc[1][1] * vc[2][2] - vc[1][2] * vc[2][1]) - vc[0][1] * (vc[1][0] * vc[2][2] - vc[1][2] * vc[2][0]) +
+                       vc[0][2] * (vc[1][0] * vc[2][1] - vc[1][1] * vc[2][0]);
+  const double s3 = det_v < 0 ? -1.0 : 1.0;  // det U = +1
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) R[r][c] = u[0][r] * vc[0][c] + u[1][r] * vc[1][c] + s3 * u[2][r] * vc[2][c];
+}
+
+// TransformationEstimationPointToPoint with with_scaling = false (the reference's other branch, LL.cpp:131-135) [3p, from
+// memory of Open3D 0.8/0.9 and Eigen 3.3; restated in tests/icp_p2p_oracle.py]: Eigen's umeyama over the correspondences,
+// R as umeyama_rotation and t = qbar - R pbar; no correspondence gives the identity.
+// The sums are taken relative to a reference point c near every pair (the target's middle point in x order, the same on
+// every pass), so sig = S_qp / n - (S_q / n)(S_p / n)^T does not cancel the ~1 m depth of the clouds away.
+struct IcpPointToPoint {
+  static constexpr int NACC = 17, ERR = 15, CNT = 16;  // [0..2] sum p - c, [3..5] sum q - c, [6..14] sum (q - c)(p - c)^T
+  double c0, c1, c2;
+  __device__ __forceinline__ IcpPointToPoint(const IcpJob& job, const double* pts, const double*) : c0(0), c1(0), c2(0) {
+    if (job.tgt_count > 0) {
+      const double* Q = pts + ((size_t)job.tgt_first + job.tgt_count / 2) * 3;
+      c0 = Q[0]; c1 = Q[1]; c2 = Q[2];
+    }
+  }
+  __device__ __forceinline__ void add(double* acc, double px, double py, double pz, double vx, double vy, double vz, int,
+                                      double best) const {
+    const double p[3] = {px - c0, py - c1, pz - c2}, q[3] = {vx - c0, vy - c1, vz - c2};
+#pragma unroll
+    for (int i = 0; i < 3; ++i) { acc[i] += p[i]; acc[3 + i] += q[i]; }
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) acc[6 + 3 * i + j] += q[i] * p[j];
+    acc[15] += best;
+    acc[16] += 1.0;
+  }
+  __device__ __forceinline__ void update(const double* tot, double* U) const {
+    for (int k = 0; k < 12; ++k) U[k] = (k % 5 == 0) ? 1.0 : 0.0;
+    const double n = tot[CNT];
+    if (!(n > 0.0)) return;
+    double mp[3], mq[3], sig[3][3], R[3][3];
+    for (int k = 0; k < 3; ++k) { mp[k] = __ddiv_rn(tot[k], n); mq[k] = __ddiv_rn(tot[3 + k], n); }
+    // no contraction: one pair must give sig = 0 exactly
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) sig[i][j] = __dsub_rn(__ddiv_rn(tot[6 + 3 * i + j], n), __dmul_rn(mq[i], mp[j]));
+    umeyama_rotation(sig, R);
+    const double pb[3] = {mp[0] + c0, mp[1] + c1, mp[2] + c2}, qb[3] = {mq[0] + c0, mq[1] + c1, mq[2] + c2};
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) U[4 * r + c] = R[r][c];
+      U[4 * r + 3] = qb[r] - (R[r][0] * pb[0] + R[r][1] * pb[1] + R[r][2] * pb[2]);
+    }
+  }
+};
+
+// RegistrationICP (Open3D 0.8/0.9) for one job per CTA, all passes in the CTA: the radius search, fitness / rmse, the
+// convergence test and T = update * T; the estimation step is Est's.
 // corr_out (capture only, else null): 2 slots per source point, the correspondence (-1: none) of pass 0 and of the
-// latest later pass.  SHARE (k_icp_point_to_plane<true>): the result goes to the pose areas of the exchange
-// (pose_share_publish) instead of outs; sh is unused otherwise.
-template <bool SHARE>
-__global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
-                                                                    const double* __restrict__ normals, IcpOut* __restrict__ outs,
-                                                                    double max_d2, int max_iter, double rel_fitness, double rel_rmse,
-                                                                    int32_t* __restrict__ corr_out, PoseShareDev sh) {
+// latest later pass.  SHARE: the result goes to the pose areas of the exchange (pose_share_publish) instead of outs; sh
+// is unused otherwise.
+template <bool SHARE, class Est>
+__device__ __forceinline__ void icp_registration(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
+                                                 const double* __restrict__ normals, IcpOut* __restrict__ outs, double max_d2,
+                                                 int max_iter, double rel_fitness, double rel_rmse, int32_t* __restrict__ corr_out,
+                                                 const PoseShareDev& sh) {
   __shared__ double s_t[ICP_TILE][3];
-  __shared__ double s_red[ICP_THREADS / 32][ICP_NACC];
+  __shared__ double s_red[ICP_THREADS / 32][Est::NACC];
   __shared__ double s_T[16];
   __shared__ int s_stop;
   const IcpJob job = jobs[blockIdx.x];
   const int n = job.src_count, nt = job.tgt_count;
   const double* __restrict__ P = pts + (size_t)job.src_first * 3;  // source cloud
   const double* __restrict__ Q = pts + (size_t)job.tgt_first * 3;  // target cloud (== source in the reference, LL.cpp:108-109)
-  const double* __restrict__ Nm = normals + (size_t)job.tgt_first * 3;
+  const Est est(job, pts, normals);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (threadIdx.x < 16) s_T[threadIdx.x] = job.init[threadIdx.x];
   if (threadIdx.x == 0) s_stop = 0;
@@ -322,9 +481,9 @@ __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob
     const double r00 = s_T[0], r01 = s_T[1], r02 = s_T[2], tx = s_T[3];
     const double r10 = s_T[4], r11 = s_T[5], r12 = s_T[6], ty = s_T[7];
     const double r20 = s_T[8], r21 = s_T[9], r22 = s_T[10], tz = s_T[11];
-    double acc[ICP_NACC];
+    double acc[Est::NACC];
 #pragma unroll
-    for (int k = 0; k < ICP_NACC; ++k) acc[k] = 0.0;
+    for (int k = 0; k < Est::NACC; ++k) acc[k] = 0.0;
 
     for (int c0 = 0; c0 < n; c0 += ICP_THREADS) {
       const int i = c0 + threadIdx.x;
@@ -365,52 +524,33 @@ __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob
       if (corr_out && live) corr_out[((size_t)job.src_first + i) * 2 + (pass > 0)] = bj;
       if (bj >= 0) {
         const double vx = Q[3 * bj], vy = Q[3 * bj + 1], vz = Q[3 * bj + 2];
-        const double nx = Nm[3 * bj], ny = Nm[3 * bj + 1], nz = Nm[3 * bj + 2];
-        const double r = (px - vx) * nx + (py - vy) * ny + (pz - vz) * nz;
-        const double J[6] = {py * nz - pz * ny, pz * nx - px * nz, px * ny - py * nx, nx, ny, nz};
-        int q = 0;
-#pragma unroll
-        for (int a = 0; a < 6; ++a)
-#pragma unroll
-          for (int b = a; b < 6; ++b) acc[q++] += J[a] * J[b];
-#pragma unroll
-        for (int a = 0; a < 6; ++a) acc[21 + a] += J[a] * r;
-        acc[27] += best;
-        acc[28] += 1.0;
+        est.add(acc, px, py, pz, vx, vy, vz, bj, best);
       }
     }
-    // block reduction of the 29 sums
+    // block reduction of the sums
 #pragma unroll
-    for (int k = 0; k < ICP_NACC; ++k) acc[k] = warp_sum(acc[k]);
+    for (int k = 0; k < Est::NACC; ++k) acc[k] = warp_sum(acc[k]);
     if (lane == 0)
 #pragma unroll
-      for (int k = 0; k < ICP_NACC; ++k) s_red[warp][k] = acc[k];
+      for (int k = 0; k < Est::NACC; ++k) s_red[warp][k] = acc[k];
     __syncthreads();
     if (threadIdx.x == 0) {
-      double tot[ICP_NACC];
-      for (int k = 0; k < ICP_NACC; ++k) {
+      double tot[Est::NACC];
+      for (int k = 0; k < Est::NACC; ++k) {
         double s = 0;
         for (int w = 0; w < ICP_THREADS / 32; ++w) s += s_red[w][k];
         tot[k] = s;
       }
-      const double ncorr = tot[28];
+      const double ncorr = tot[Est::CNT];
       fitness = n > 0 ? ncorr / (double)n : 0.0;
-      rmse = ncorr > 0 ? sqrt(tot[27] / ncorr) : 0.0;
+      rmse = ncorr > 0 ? sqrt(tot[Est::ERR] / ncorr) : 0.0;
       bool stop = false;
       if (pass > 0 && fabs(fit_prev - fitness) < rel_fitness && fabs(rmse_prev - rmse) < rel_rmse) stop = true;
       if (pass >= max_iter) stop = true;
       if (!stop) {
-        double A[6][6], b[6], x[6] = {0, 0, 0, 0, 0, 0};
-        int q = 0;
-        for (int a = 0; a < 6; ++a)
-          for (int c = a; c < 6; ++c) { A[a][c] = tot[q]; A[c][a] = tot[q]; ++q; }
-        for (int a = 0; a < 6; ++a) b[a] = -tot[21 + a];
-        solve6(A, b, x);
-        // TransformVector6dToMatrix4d: Rz(x2) Ry(x1) Rx(x0), translation x3..5; T = update * T
-        const double cx = cos(x[0]), sx = sin(x[0]), cy = cos(x[1]), sy = sin(x[1]), cz = cos(x[2]), sz = sin(x[2]);
-        const double U[12] = {cz * cy, cz * sy * sx - sz * cx, cz * sy * cx + sz * sx, x[3],
-                              sz * cy, sz * sy * sx + cz * cx, sz * sy * cx - cz * sx, x[4],
-                              -sy,     cy * sx,                cy * cx,                x[5]};
+        double U[12];
+        est.update(tot, U);
+        // T = update * T
         double Tn[12];
         for (int r = 0; r < 3; ++r)
           for (int c = 0; c < 4; ++c)
@@ -434,7 +574,34 @@ __global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob
   }
 }
 
-// One CTA behind k_icp_point_to_plane<true> on each rank's stream: waits (acquire) until every rank's pose flag of the
+template <bool SHARE>
+__global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_plane(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
+                                                                    const double* __restrict__ normals, IcpOut* __restrict__ outs,
+                                                                    double max_d2, int max_iter, double rel_fitness, double rel_rmse,
+                                                                    int32_t* __restrict__ corr_out, PoseShareDev sh) {
+  icp_registration<SHARE, IcpPointToPlane>(jobs, pts, normals, outs, max_d2, max_iter, rel_fitness, rel_rmse, corr_out, sh);
+}
+
+// No normals: k_icp_normals does not run before it (the reference's point-to-point branch calls no EstimateNormals).
+template <bool SHARE>
+__global__ void __launch_bounds__(ICP_THREADS) k_icp_point_to_point(const IcpJob* __restrict__ jobs, const double* __restrict__ pts,
+                                                                    IcpOut* __restrict__ outs, double max_d2, int max_iter,
+                                                                    double rel_fitness, double rel_rmse, int32_t* __restrict__ corr_out,
+                                                                    PoseShareDev sh) {
+  icp_registration<SHARE, IcpPointToPoint>(jobs, pts, nullptr, outs, max_d2, max_iter, rel_fitness, rel_rmse, corr_out, sh);
+}
+
+// The ICP kernel of estimation est over n jobs (point-to-plane reads the normals k_icp_normals left in nrm).
+template <bool SHARE>
+static void launch_icp(int est, unsigned n, cudaStream_t st, const IcpJob* jobs, const double* pts, const double* nrm, IcpOut* outs,
+                       int max_iter, int32_t* corr_out, const PoseShareDev& sd) {
+  if (est == LM_ICP_POINT_TO_POINT)
+    k_icp_point_to_point<SHARE><<<n, ICP_THREADS, 0, st>>>(jobs, pts, outs, 0.01 * 0.01, max_iter, 1e-6, 1e-6, corr_out, sd);
+  else
+    k_icp_point_to_plane<SHARE><<<n, ICP_THREADS, 0, st>>>(jobs, pts, nrm, outs, 0.01 * 0.01, max_iter, 1e-6, 1e-6, corr_out, sd);
+}
+
+// One CTA behind the ICP kernel's SHARE instantiation on each rank's stream: waits (acquire) until every rank's pose flag of the
 // frame has arrived in this rank's pose area, then copies the entries, in survivor order, into the stage's outs / posed.
 __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShareDev sh, IcpOut* __restrict__ outs,
                                                                        uint8_t* __restrict__ posed) {
@@ -495,6 +662,7 @@ struct lm_icp {
   IcpOut* h_outs = nullptr; size_t cap_houts = 0;
   int64_t launches = 0;
   bool use_scene_cloud = false;  // non-reference option: register against the scene cloud
+  int estimation = LM_ICP_POINT_TO_PLANE;
   int last_points = 0, last_iterations = 0;
   double last_rmse = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -503,6 +671,7 @@ struct lm_icp {
   bool capture = false;
   int32_t* d_knn = nullptr; int32_t* d_corr = nullptr; size_t cap_capture = 0;
   struct {
+    int estimation = LM_ICP_POINT_TO_PLANE;  // point-to-point computes no normals and no neighbour lists
     std::vector<IcpJob> jobs;
     std::vector<int> job_of;  // per hypothesis, -1: early return
     std::vector<IcpOut> outs;
@@ -770,13 +939,13 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     if (npts) CUI(cudaMemcpyAsync(h->d_pts, all.data(), npts * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
     CUI(cudaMemcpyAsync(h->d_jobs, jobs.data(), jobs.size() * sizeof(IcpJob), cudaMemcpyHostToDevice, st));
     CUI(cudaEventRecord(h->ev0, st));
-    if (max_count > 0) {
+    if (max_count > 0 && h->estimation == LM_ICP_POINT_TO_PLANE) {
       dim3 g((unsigned)((max_count + 127) / 128), (unsigned)jobs.size());
       k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, knn_out);
       ++h->launches;
     }
-    k_icp_point_to_plane<false><<<(unsigned)jobs.size(), ICP_THREADS, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, h->d_outs, 0.01 * 0.01,
-                                                                             max_iterations, 1e-6, 1e-6, corr_out, PoseShareDev());
+    launch_icp<false>(h->estimation, (unsigned)jobs.size(), st, h->d_jobs, h->d_pts, h->d_nrm, h->d_outs, max_iterations, corr_out,
+                      PoseShareDev());
     ++h->launches;
     CUI(cudaEventRecord(h->ev1, st));
     CUI(cudaMemcpyAsync(h->h_outs, h->d_outs, jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
@@ -788,6 +957,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   }
   if (h->capture) {
     auto& c = h->cap;
+    c.estimation = h->estimation;
     c.jobs = jobs;
     c.job_of = job_of;
     c.outs.assign(h->h_outs, h->h_outs + (jobs.empty() ? 0 : jobs.size()));
@@ -796,8 +966,10 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     c.knn.assign(npts * ICP_KNN, -1);
     c.corr.assign(npts * 2, -1);
     if (npts) {
-      CUI(cudaMemcpy(c.nrm.data(), h->d_nrm, npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
-      CUI(cudaMemcpy(c.knn.data(), h->d_knn, npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
+      if (c.estimation == LM_ICP_POINT_TO_PLANE) {
+        CUI(cudaMemcpy(c.nrm.data(), h->d_nrm, npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+        CUI(cudaMemcpy(c.knn.data(), h->d_knn, npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
+      }
       CUI(cudaMemcpy(c.corr.data(), h->d_corr, npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
     }
   }
@@ -823,7 +995,8 @@ extern "C" int lm_icp_process(lm_icp* h, const uint16_t* scene_depth, int srows,
 }
 
 // [0] points in the down-sampled cloud, [1] ICP iterations, [2] inlier rmse (m), [3] device time of the
-// normals + ICP kernels of the last call in microseconds -- all of the LAST hypothesis processed.
+// normals + ICP kernels (point-to-point: the ICP kernel alone) of the last call in microseconds -- all of the LAST
+// hypothesis processed.
 extern "C" int lm_icp_last_stats(lm_icp* h, double* out4) {
   if (!h || !out4) return lm_fail(LM_E_INVALID, "null argument");
   out4[0] = h->last_points; out4[1] = h->last_iterations; out4[2] = h->last_rmse; out4[3] = h->last_kernel_us;
@@ -835,6 +1008,14 @@ extern "C" int64_t lm_icp_launch_count(lm_icp* h) { return h ? h->launches : 0; 
 extern "C" int lm_icp_set_use_scene_cloud(lm_icp* h, int on) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
   h->use_scene_cloud = on != 0;
+  return LM_OK;
+}
+
+extern "C" int lm_icp_set_estimation(lm_icp* h, int estimation) {
+  if (!h) return lm_fail(LM_E_INVALID, "null handle");
+  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT)
+    return lm_fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
+  h->estimation = estimation;
   return LM_OK;
 }
 
@@ -857,6 +1038,8 @@ extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t c
   int64_t bytes = 0;
   std::vector<int32_t> tmp;
   double res[19];
+  if ((what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN) && c.estimation != LM_ICP_POINT_TO_PLANE)
+    return lm_fail(LM_E_STATE, "capture item %d: the point-to-point estimation computes no normals or neighbour lists", what);
   switch (what) {
     case LM_ICP_CAPTURE_COUNTS:
       tmp = {j.src_count, j.tgt_count};
@@ -1568,21 +1751,23 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
                                                3 * POSE_KEY_BITS, st));
   k_pose_voxel<<<2 * Bs, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
                                                 p.use_scene);
-  // unchanged ICP kernels, launched for the bound (this rank's share): empty jobs fall through
-  dim3 g((unsigned)((A + 127) / 128), (unsigned)Bs);
-  k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+  // the ICP kernels of lm_icp_process_batch, launched for the bound (this rank's share): empty jobs fall through
+  const bool normals = e.estimation == LM_ICP_POINT_TO_PLANE;
+  if (normals) {
+    dim3 g((unsigned)((A + 127) / 128), (unsigned)Bs);
+    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+  }
   if (sh) {
     const PoseShareDev sd = share_dev(*sh, sh->seq, e.d_counts, s->d_posed, s->d_err);
-    k_icp_point_to_plane<true><<<Bs, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr, 0.01 * 0.01, e.max_iterations, 1e-6,
-                                                           1e-6, nullptr, sd);
+    launch_icp<true>(e.estimation, Bs, st, s->d_jobs, s->d_pts, s->d_nrm, nullptr, e.max_iterations, nullptr, sd);
     k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_outs, s->d_posed);
   } else {
-    k_icp_point_to_plane<false><<<B, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, 0.01 * 0.01, e.max_iterations, 1e-6,
-                                                           1e-6, nullptr, PoseShareDev());
+    launch_icp<false>(e.estimation, B, st, s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, e.max_iterations, nullptr, PoseShareDev());
   }
   CUI(cudaGetLastError());
-  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals, k_icp_point_to_plane (+ k_pose_collect)
-  s->last_launches = sh ? 6 : 5;
+  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals (point-to-plane only), the ICP kernel
+  // (+ k_pose_collect)
+  s->last_launches = (sh ? 6 : 5) - (normals ? 0 : 1);
   *launches += s->last_launches;
   CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(B, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
   CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t) * (sh ? 3 : 1), cudaMemcpyDeviceToHost, st));
@@ -1761,6 +1946,8 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
   const int64_t S = b.first[nf];
   const PoseShare* sh = b.share;
   const int nc = pose_batch_chunks(S);
+  const bool normals = b.estimation == LM_ICP_POINT_TO_PLANE;
+  const int chunk_launches = (sh ? 6 : 5) - (normals ? 0 : 1);
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
@@ -1810,20 +1997,20 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
                                                  3 * POSE_KEY_BITS, st));
     k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
                                                  p.use_scene);
-    dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
-    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+    if (normals) {
+      dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
+      k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+    }
     if (sh) {
       // exchange seq + c: the results travel to every rank; the collector gathers the chunk in survivor order
       const PoseShareDev sd = share_dev(*sh, sh->seq + c, stat + 3, s->d_posed, stat);
-      k_icp_point_to_plane<true><<<n, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr, 0.01 * 0.01, b.max_iterations, 1e-6,
-                                                            1e-6, nullptr, sd);
+      launch_icp<true>(b.estimation, n, st, s->d_jobs, s->d_pts, s->d_nrm, nullptr, b.max_iterations, nullptr, sd);
       k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_bouts + c0, s->d_bposed + c0);
     } else {
-      k_icp_point_to_plane<false><<<C, ICP_THREADS, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, 0.01 * 0.01, b.max_iterations,
-                                                             1e-6, 1e-6, nullptr, PoseShareDev());
+      launch_icp<false>(b.estimation, C, st, s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, b.max_iterations, nullptr, PoseShareDev());
     }
     CUI(cudaGetLastError());
-    *launches += sh ? 6 : 5;
+    *launches += chunk_launches;
   }
   if (b.pose_nms) {
     PoseNmsParams p;
@@ -1862,7 +2049,7 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
   if (stats4) {
     stats4[0] = S;
     stats4[1] = refined;
-    stats4[2] = (int64_t)nc * (sh ? 6 : 5);
+    stats4[2] = (int64_t)nc * chunk_launches;
     stats4[3] = sh ? 1 : 0;
   }
   if (b.pose_nms) {

@@ -2,8 +2,8 @@
 //
 // The pose stage refines the NMS survivors of k_post_nms where they lie: per-template render crops registered once
 // (lm_set_template_renders), then per frame k_pose_cloud (box test, back-projection, centroids, voxel keys), a CUB
-// segmented radix sort of the voxel keys, k_pose_voxel (voxel means) and the unchanged k_icp_normals /
-// k_icp_point_to_plane, all on the detector's stream.  The host composes result = T * init_base after the copy.
+// segmented radix sort of the voxel keys, k_pose_voxel (voxel means) and the ICP kernels of lm_icp_process_batch
+// (k_icp_normals + k_icp_point_to_plane, or k_icp_point_to_point alone), all on the detector's stream.  The host composes result = T * init_base after the copy.
 // The pose NMS (k_pose_nms, one CTA behind k_icp_point_to_plane) composes the poses on the device instead, runs the
 // greedy translation NMS of linemod_ros/detect.py over them and compacts the kept ones into one output block.
 #pragma once
@@ -26,7 +26,7 @@ bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel
 
 // The pose stage shared over the ranks of the peer exchange (lm_peer_share_pose).  Survivor i (pick order of k_post_nms,
 // the same on every rank) is refined by rank i % world: this rank's launches are sized for ceil(bound / world) slots,
-// slot j takes survivor rank + j * world.  k_icp_point_to_plane<true> stores each survivor's result into the pose area
+// slot j takes survivor rank + j * world.  The ICP kernel's SHARE instantiation stores each survivor's result into the pose area
 // of every rank's exchange buffer and raises this rank's pose flag there; k_pose_collect waits for the world flags in
 // this rank's buffer and gathers the results in survivor order into the stage's own outputs, so pose_stage_finish and
 // the pose NMS read what the unshared stage leaves.  The pose area: [2 slots][1024 survivors] entries of 160 bytes,
@@ -51,6 +51,7 @@ struct PoseEnqueue {
   int bound;                  // survivors the launches are sized for (top_k, or every survivor k_post_nms may write)
   int use_scene_cloud;
   int max_iterations;
+  int estimation;             // LM_ICP_POINT_TO_PLANE (k_icp_normals + k_icp_point_to_plane) or LM_ICP_POINT_TO_POINT
   cudaStream_t stream;
   const PoseShare* share;     // null: this rank refines every survivor
 };
@@ -84,6 +85,7 @@ struct PoseBatch {
   const lm_match* surv;       // host copy of the survivors (pose_nms == 0 only)
   const float* sK;            // [n_frames][9]
   int use_scene_cloud, max_iterations;
+  int estimation;             // as PoseEnqueue
   int pose_nms;               // 1: the pose NMS per frame (k_pose_nms_batch), 0: the host composes the poses
   double thr;
   cudaStream_t stream;
@@ -92,7 +94,7 @@ struct PoseBatch {
 // The pose stage over every survivor of the batch in chunks of at most 1024 slots, then (pose_nms) one pose NMS launch
 // for all frames; waits.  posed[f] / kept[f]: frame f's survivors with a pose, and its entries (kept poses, or every
 // survivor without the pose NMS).  Shared: within a chunk of C survivors, survivor i is refined by rank i % world in
-// ceil(C / world) slots (k_pose_cloud_batch_share, k_icp_point_to_plane<true>), and k_pose_collect gathers the chunk
+// ceil(C / world) slots (k_pose_cloud_batch_share, the ICP kernel's SHARE instantiation), and k_pose_collect gathers the chunk
 // into the batch's outputs.  stats4 (may be null): what lm_pose_stats returns for the batch.
 int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4);
 // Frame f's kept[f] entries after pose_batch_run, outputs as lm_complete_detect (pose_nms) or lm_complete_pose.

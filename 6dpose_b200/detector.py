@@ -231,12 +231,15 @@ class Detector:
             first += n
 
     def match_refine(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
-                     use_scene_cloud=False, masks=[]):
+                     use_scene_cloud=False, masks=[], estimation="point_to_plane"):
         """match + nms + poseRefine().process for every survivor, as the drivers do (linemod_and_levelup_test.py:
         324-367), in one chain on the GPU: front-end, match, NMS/top-k, cloud building, normals and ICP.  Needs
         setTemplateRenders.  Returns [(Match, poseRefine)] in pick order; each poseRefine is in the state
-        refine_matches leaves it in (residual -1, R / t None where the model box does not fit the frame)."""
+        refine_matches leaves it in (residual -1, R / t None where the model box does not fit the frame).
+        estimation (not in the reference's surface): the ICP's estimation step, "point_to_plane" (the reference's
+        active branch) or "point_to_point" (its other branch, LL.cpp:131-135: no normals, a closed-form rigid fit)."""
         from .pose_refine import poseRefine
+        _lib.estimation_code(estimation)
         if len(sources) != 2:
             raise RuntimeError("sources.size() == modalities.size()")
         sources = [self._as_source(s, i) for i, s in enumerate(sources)]
@@ -244,17 +247,19 @@ class Detector:
         sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
         nat = self._select(list(class_ids))
         out, R, t, res, _ = nat.match_pose(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold),
-                                           int(top_k), int(max_iterations), bool(use_scene_cloud))
+                                           int(top_k), int(max_iterations), bool(use_scene_cloud), estimation)
         return self._pose_pairs(out, R, t, res)
 
     def detect(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
-               max_iterations=30, use_scene_cloud=False, masks=[]):
+               max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane"):
         """The whole frame of linemod_ros/detect.py (:91-141): match, box NMS, poseRefine of every survivor (top_k=0)
         and the greedy translation NMS nms_norms(ts, -residual, translation_threshold) (:41-50, :130-131), in one chain
         on the GPU; only the kept objects are copied back.  Needs setTemplateRenders.  Returns [(Match, poseRefine)] in
         keep order, as match_refine(top_k) followed by pose_refine.nms_translations would.  Survivors whose model box
-        does not fit the frame (no pose) are not returned; equal residuals keep box-NMS pick order."""
+        does not fit the frame (no pose) are not returned; equal residuals keep box-NMS pick order.  estimation as
+        match_refine."""
         from .pose_refine import poseRefine
+        _lib.estimation_code(estimation)
         if len(sources) != 2:
             raise RuntimeError("sources.size() == modalities.size()")
         sources = [self._as_source(s, i) for i, s in enumerate(sources)]
@@ -262,29 +267,33 @@ class Detector:
         sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
         nat = self._select(list(class_ids))
         out, R, t, res, _ = nat.detect(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold), int(top_k),
-                                       int(max_iterations), bool(use_scene_cloud), float(translation_threshold))
+                                       int(max_iterations), bool(use_scene_cloud), float(translation_threshold), estimation)
         return self._pose_pairs(out, R, t, res)  # every kept pose has one: residual >= 0
 
     # ---- a batch of RGB-D frames through one pose stage (lm_detect_batch) ----
     def match_refine_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
-                           use_scene_cloud=False, masks=[]):
+                           use_scene_cloud=False, masks=[], estimation="point_to_plane"):
         """match_refine for many frames in one call: each frame's match and box NMS, then one pose stage for the survivors
         of all of them, which fills the GPU where one frame's few survivors cannot.  frames: a sequence of [rgb, depth]
         pairs of one size; sceneK: one 3x3 matrix or one per frame; masks: [] or one masks list per frame.  Returns one
         list per frame, each equal to match_refine on that frame.  The handle keeps the batch's device buffers, sized
-        for the batch's shape (frames, size, top_k; with top_k=0 the pose buffers of 1024 survivors), for the next one."""
+        for the batch's shape (frames, size, top_k; with top_k=0 the pose buffers of 1024 survivors), for the next one.
+        estimation as match_refine."""
+        _lib.estimation_code(estimation)
         nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "match_refine_batch()")
         got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
-                               bool(use_scene_cloud), pose_nms=False)
+                               bool(use_scene_cloud), pose_nms=False, estimation=estimation)
         return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
     def detect_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
-                     max_iterations=30, use_scene_cloud=False, masks=[]):
+                     max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane"):
         """detect for many frames in one call: each frame's match and box NMS, then one pose stage and one pose NMS for all
         of them.  Arguments as match_refine_batch; returns one list per frame, each equal to detect on that frame."""
+        _lib.estimation_code(estimation)
         nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "detect_batch()")
         got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
-                               bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold))
+                               bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold),
+                               estimation=estimation)
         return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
     def _batch_args(self, frames, class_ids, sceneK, masks, what):

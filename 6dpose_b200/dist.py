@@ -89,24 +89,28 @@ def _connected_batch(detector, frames, class_ids, sceneK, masks, group, what):
 
 
 def match_refine_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
-                               use_scene_cloud=False, masks=[], group=None):
+                               use_scene_cloud=False, masks=[], group=None, estimation="point_to_plane"):
     """Detector.match_refine_batch with the bank sharded over the connected peer exchange (lm_peer_detect_batch); with
     connect_peers(share_pose=True) the pose stage is divided over the ranks too.  Every rank calls it with the same
-    arguments and returns the whole result, equal to match_refine_batch on one unconnected detector."""
+    arguments (estimation included) and returns the whole result, equal to match_refine_batch on one unconnected
+    detector."""
+    _lib.estimation_code(estimation)
     nat, (rgb, depth, mk, K) = _connected_batch(detector, frames, class_ids, sceneK, masks, group, "match_refine_batch_sharded()")
     got = nat.peer_detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
-                                bool(use_scene_cloud), pose_nms=False)
+                                bool(use_scene_cloud), pose_nms=False, estimation=estimation)
     return [detector._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
 
 def detect_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
-                         max_iterations=30, use_scene_cloud=False, masks=[], group=None):
+                         max_iterations=30, use_scene_cloud=False, masks=[], group=None, estimation="point_to_plane"):
     """Detector.detect_batch with the bank sharded over the connected peer exchange (lm_peer_detect_batch), as
     match_refine_batch_sharded: every rank calls it and returns the whole result, equal to detect_batch on one
     unconnected detector."""
+    _lib.estimation_code(estimation)
     nat, (rgb, depth, mk, K) = _connected_batch(detector, frames, class_ids, sceneK, masks, group, "detect_batch_sharded()")
     got = nat.peer_detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
-                                bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold))
+                                bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold),
+                                estimation=estimation)
     return [detector._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
 

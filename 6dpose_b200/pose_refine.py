@@ -20,7 +20,12 @@ def _native(device):
 class poseRefine:
     max_iterations = 30  # Open3D ICPConvergenceCriteria default used by the reference (LL.cpp:128-130)
 
-    def __init__(self):
+    def __init__(self, estimation="point_to_plane"):
+        """estimation (not in the reference's surface, which takes no argument): the ICP's estimation step,
+        "point_to_plane" (TransformationEstimationPointToPlane, the reference's active branch) or "point_to_point"
+        (TransformationEstimationPointToPoint, its other branch at LL.cpp:131-135: no normals, Umeyama's rigid fit)."""
+        _lib.estimation_code(estimation)
+        self.estimation = estimation
         self._residual = -1.0
         self._R = None
         self._t = None
@@ -52,7 +57,7 @@ class poseRefine:
         R = self._mat(modelR, np.float32, (3, 3), "modelR")
         t = self._mat(modelT, np.float32, (3,), "modelT")
         Ro, to, res = _native(self.device).process_batch(scene, [model], sK, mK[None], R[None], t[None],
-                                                         [[int(detectX), int(detectY)]], self.max_iterations)
+                                                         [[int(detectX), int(detectY)]], self.max_iterations, self.estimation)
         self._residual = float(res[0])
         if res[0] == -1.0:  # early return: R_refined / t_refiend keep their previous value (LL.cpp:52-55)
             return
@@ -69,13 +74,14 @@ class poseRefine:
         return self._t
 
 
-def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, modelTs, device=None):
+def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, modelTs, device=None, estimation="point_to_plane"):
     """The drivers' loop over the NMS survivors (linemod_and_levelup_test.py:348-367: one poseRefine per
     match, fed with the render of the matched template's pose) as ONE batched GPU call: hypothesis i is
     matches[i] (its x, y) with modelDepths[i] / modelKs[i] / modelRs[i] / modelTs[i].  Returns a list of
-    poseRefine objects in the state process() would have left them in."""
+    poseRefine objects in the state process() would have left them in.  estimation as poseRefine()."""
+    _lib.estimation_code(estimation)
     n = len(matches)
-    out = [poseRefine() for _ in range(n)]
+    out = [poseRefine(estimation) for _ in range(n)]
     if n == 0:
         return out
     scene = np.asarray(sceneDepth)
@@ -90,7 +96,7 @@ def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, m
     t = np.stack([poseRefine._mat(v, np.float32, (3,), "modelT") for v in modelTs])
     xy = [[int(m.x), int(m.y)] for m in matches]
     dev = out[0].device if device is None else int(device)
-    Ro, to, res = _native(dev).process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations)
+    Ro, to, res = _native(dev).process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
     for i, p in enumerate(out):
         p._residual = float(res[i])
         if res[i] != -1.0:

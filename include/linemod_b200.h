@@ -175,11 +175,13 @@ int lm_peer_disconnect(lm_detector* d);
  * the results in survivor order.  lm_complete_pose and lm_complete_detect then return on EVERY rank exactly what the
  * unshared stage returns, bit for bit (R, t, residual, -1 and untouched R / t on the early return of LL.cpp:52-55, NaN
  * patterns, the pose NMS's keep order and counts): each survivor's ICP is one deterministic job wherever it runs.  A
- * shared frame's pose stage is 6 launches (5 unshared), whatever the survivor count.
+ * shared frame's pose stage is 6 launches (5 unshared), whatever the survivor count; 5 (4) with LM_ICP_POINT_TO_POINT.
  *   lm_peer_share_pose  on != 0 turns sharing on.  LM_E_STATE on a handle without a connected exchange.  A promise the
  *                       caller makes for every rank: every rank of the exchange sets the same value before its next
  *                       frame, and while it is on every rank runs the pose stage of every frame (a rank that runs the
- *                       match alone leaves its peers waiting).  lm_peer_disconnect turns it off.  Ranks that are
+ *                       match alone leaves its peers waiting).  Likewise every rank sets the same lm_set_pose_estimation
+ *                       before its next frame: a shared frame's survivors are refined with the estimation of the rank
+ *                       that owns them.  lm_peer_disconnect turns it off.  Ranks that are
  *                       handles of ONE process on ONE device: a pose stage that uploads renders or grows its buffers
  *                       (the first frame, a larger top_k) frees device memory, which waits for the whole device -- a
  *                       peer's pose collector included -- so run such a frame unshared first.
@@ -249,6 +251,20 @@ int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iterations, int
 int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                      int64_t* n_out, int64_t* n_records);
 
+/* The ICP's estimation step: the two branches of poseRefine::process behind USE_OPEN3D_P2PL (LL.cpp:122-135).  Both run
+ * the same RegistrationICP loop (1 cm radius, the convergence test, max_iterations); only the update of each pass differs.
+ *   POINT_TO_PLANE  TransformationEstimationPointToPlane against EstimateNormals' normals of the target (KNN 30): one
+ *                   normals launch and one ICP launch
+ *   POINT_TO_POINT  TransformationEstimationPointToPoint without scaling: Eigen's umeyama over the correspondences, a
+ *                   closed-form rigid fit; no normals, so one launch.  It may need more passes to converge.
+ * lm_set_pose_estimation sets it for the detector's next lm_enqueue_pose, lm_detect_batch and lm_peer_detect_batch; a frame
+ * keeps the estimation it was enqueued with (the pose stage rerun after a result-block retry included).  No device work.
+ * A frame's pose stage is then 4 launches (5 shared), a batch chunk likewise.  With a connected peer exchange, setting the
+ * same value on every rank is the caller's promise, as with lm_peer_share_pose.  LM_E_INVALID for any other value. */
+#define LM_ICP_POINT_TO_PLANE 0 /* TransformationEstimationPointToPlane, the reference's active branch (default) */
+#define LM_ICP_POINT_TO_POINT 1 /* TransformationEstimationPointToPoint, LL.cpp:131-135 */
+int lm_set_pose_estimation(lm_detector* d, int estimation);
+
 /* Pose NMS on the device: the end of linemod_ros/detect.py's frame (:91-141), which refines every box-NMS survivor and
  * then drops duplicate objects in pose space with nms_norms(ts, -residual, 40.0) (:41-50, :130-131).  One CTA behind the
  * pose stage on the detector's stream; only the kept objects come back.
@@ -307,7 +323,8 @@ int lm_nms_translations(int device, int64_t n, const double* t, const double* sc
  * Each frame runs the single-frame match and box NMS and waits for them (a frame whose records outgrow the result block
  * is redone there); its survivors and depth are copied aside on the stream.  The pose stage then runs once over all
  * S survivors in chunks of at most 1024 slots (the single-frame bound for top_k = 0, so its cloud buffers do not grow
- * with the batch): 5 launches per chunk, plus 1 launch of the pose NMS for every frame.  Before its first frame the call
+ * with the batch): 5 launches per chunk (4 with LM_ICP_POINT_TO_POINT, lm_set_pose_estimation), plus 1 launch of the
+ * pose NMS for every frame.  Before its first frame the call
  * uploads the renders and grows every buffer a batch of its shape (n_frames, rows x cols, top_k) may need.  Extra device
  * memory, kept by the handle for the next batch: n_frames depth slots (rows * cols * 2 bytes each, 614 KB at 640 x 480),
  * n_frames * (top_k, or 1024) survivor slots of 20 bytes, for each of those slots an ICP output, pose NMS entry, frame
@@ -329,6 +346,7 @@ int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint
  *              within a chunk of C survivors, survivor i is refined by rank i % world in ceil(C / world) slots, and the
  *              results travel through the pose area as for a shared frame (6 launches per chunk; a rank without a
  *              survivor in the chunk still publishes).  Each chunk is one pose exchange.  Then 1 pose NMS launch.
+ *              LM_ICP_POINT_TO_POINT takes one launch off each chunk (no normals).
  * LM_E_STATE without a connected exchange; the other argument and state errors are those of lm_detect_batch and come
  * before any device work.  LM_E_CAPACITY for too small outputs (*n_out = the total needed, > cap) comes on every rank
  * alike (the totals are the same), so a caller that grows cap and calls again does so on every rank.  LM_E_CAPACITY
@@ -341,7 +359,8 @@ int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint
  * uploads the renders and grows the buffers, which frees device memory, and a free waits for the whole device -- a
  * peer's collector included.  For the same reason, once connected, every rank calls lm_prepare (which grows the result
  * block to the exchange's size) before any rank enqueues a frame.  lm_pose_stats afterwards: S, the hypotheses this rank refined over all chunks, the pose
- * stage's launches (chunks x 6 shared, x 5 unshared; the pose NMS not counted) and 1 if shared. */
+ * stage's launches (chunks x 6 shared, x 5 unshared, one fewer per chunk with LM_ICP_POINT_TO_POINT; the pose NMS not
+ * counted) and 1 if shared. */
 int lm_peer_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
                          const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
                          int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm,
@@ -381,7 +400,8 @@ int lm_stage_times(lm_detector* d, float* out8);
 /* The CUDA stream all work of this handle is issued on (cudaStream_t as void*). */
 void* lm_stream(lm_detector* d);
 /* Number of kernel launches issued by this handle since creation (the pose stage's CUB segmented sort counts as one;
- * a frame's pose stage is 5, whatever its survivor count; 6 when shared over the exchange). */
+ * a frame's pose stage is 5, whatever its survivor count; 6 when shared over the exchange; one fewer each with
+ * LM_ICP_POINT_TO_POINT). */
 int64_t lm_launch_count(lm_detector* d);
 /* About the last pose stage this handle completed (lm_complete_pose / lm_complete_detect; lm_peer_detect_batch: see there,
  * lm_detect_batch leaves it as it was): [0] box-NMS survivors,
@@ -419,6 +439,10 @@ int lm_icp_last_stats(lm_icp* h, double* out4);
 /* NOT the reference's behaviour (default off): register the model cloud against the down-sampled SCENE
  * cloud, which is what LL.cpp:109 evidently meant to do (it down-samples the model cloud twice). */
 int lm_icp_set_use_scene_cloud(lm_icp* h, int on);
+/* LM_ICP_POINT_TO_PLANE (default: k_icp_normals + the ICP kernel, 2 launches per call) or LM_ICP_POINT_TO_POINT (the ICP
+ * kernel alone, 1 launch; lm_icp_last_stats [3] then times that kernel alone) for the next lm_icp_process_batch.
+ * LM_E_INVALID for any other value. */
+int lm_icp_set_estimation(lm_icp* h, int estimation);
 int64_t lm_icp_launch_count(lm_icp* h);
 
 /* ---- introspection of the ICP kernels, used by the stage-by-stage tests ---- */
@@ -434,8 +458,9 @@ int lm_icp_set_capture(lm_icp* h, int on);
  *   KNN         tgt x 30 int32: the neighbours k_icp_normals kept (target indices, kept order, padded with -1)
  *   CORR_FIRST  src int32: the correspondence (target index, -1: none) of every source point on pass 0
  *   CORR_LAST   src int32: the same for the last pass the kernel ran (the pass whose fitness and rmse are returned)
- * LM_E_STATE for a hypothesis that took the early return, LM_E_CAPACITY when cap is too small, LM_E_INVALID for a
- * hypothesis outside the last captured call. */
+ * LM_E_STATE for a hypothesis that took the early return, and for NORMALS / KNN of a call with LM_ICP_POINT_TO_POINT
+ * (nothing was computed), LM_E_CAPACITY when cap is too small, LM_E_INVALID for a hypothesis outside the last captured
+ * call. */
 #define LM_ICP_CAPTURE_COUNTS 0
 #define LM_ICP_CAPTURE_SOURCE 1
 #define LM_ICP_CAPTURE_TARGET 2
