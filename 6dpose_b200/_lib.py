@@ -31,7 +31,7 @@ SYMBOLS = [
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
     "lm_enqueue_pose_nms", "lm_complete_detect", "lm_nms_translations", "lm_detect_batch", "lm_peer_detect_batch",
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect", "lm_peer_share_pose",
-    "lm_pose_stats", "lm_set_pose_estimation",
+    "lm_pose_stats", "lm_set_pose_estimation", "lm_set_template_depths", "lm_set_depth_gate", "lm_depth_gate_stats",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
     "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture",
 ]
@@ -46,6 +46,16 @@ def estimation_code(estimation):
     if not isinstance(estimation, str) or estimation not in ESTIMATIONS:
         raise ValueError("estimation must be one of %s, got %r" % (", ".join(repr(k) for k in ESTIMATIONS), estimation))
     return ESTIMATIONS[estimation]
+
+
+def depth_gate_tolerance(tolerance):
+    """The depth gate's tolerance as a float in [0, 1); ValueError otherwise (no device work)."""
+    if isinstance(tolerance, (bool, np.bool_)) or not isinstance(tolerance, (int, float, np.integer, np.floating)):
+        raise TypeError("depth gate tolerance must be a number, got %s" % type(tolerance).__name__)
+    t = float(tolerance)
+    if not (0.0 <= t < 1.0):
+        raise ValueError("depth gate tolerance must lie in [0, 1), got %r" % tolerance)
+    return t
 
 
 _lib = None
@@ -102,6 +112,9 @@ def load():
     L.lm_peer_share_pose.argtypes = [vp, c_int]
     L.lm_pose_stats.argtypes = [vp, ctypes.POINTER(c_i64)]
     L.lm_set_pose_estimation.argtypes = [vp, c_int]
+    L.lm_set_template_depths.argtypes = [vp, c_i64, c_i64, ctypes.POINTER(c_f)]
+    L.lm_set_depth_gate.argtypes = [vp, c_int, ctypes.c_double]
+    L.lm_depth_gate_stats.argtypes = [vp, ctypes.POINTER(c_i64)]
     L.lm_device_result.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(c_i64)]
     L.lm_fetch_records.argtypes = [vp, vp, c_i64, ctypes.POINTER(c_i64)]
     L.lm_finish.argtypes = [vp, vp, c_i64, vp, c_i64, ctypes.POINTER(c_i64)]
@@ -422,6 +435,25 @@ class NativeDetector:
         check(self._L.lm_match_top(self._h, ptrs, r, c, ctypes.c_float(threshold), float(iou_threshold), int(top_k),
                                    out.ctypes.data_as(ctypes.c_void_p), out.shape[0], ctypes.byref(n), ctypes.byref(nrec)))
         return out[:n.value].copy(), int(nrec.value)
+
+    # ---- depth gate of the coarse scan (include/linemod_b200.h, lm_set_depth_gate) ----
+    def set_template_depths(self, first, z_mm):
+        """Training distances (mm) of templates [first, first + len(z_mm)) of the bank; NaN or <= 0: never gated."""
+        z = np.ascontiguousarray(z_mm, np.float32).reshape(-1)
+        check(self._L.lm_set_template_depths(self._h, int(first), z.shape[0], z.ctypes.data_as(ctypes.POINTER(ctypes.c_float))))
+
+    def set_depth_gate(self, tolerance):
+        """Gate the coarse scan by scene depth with this tolerance from the next frame on; None turns the gate off."""
+        if tolerance is None:
+            check(self._L.lm_set_depth_gate(self._h, 0, 0.0))
+        else:
+            check(self._L.lm_set_depth_gate(self._h, 1, depth_gate_tolerance(tolerance)))
+
+    def depth_gate_stats(self):
+        """Of the last frame, which ran gated: candidates before / after the gate, empty cells, templates with a distance."""
+        a = (ctypes.c_int64 * 4)()
+        check(self._L.lm_depth_gate_stats(self._h, a))
+        return dict(zip(["before", "after", "empty_cells", "with_distance"], [int(v) for v in a]))
 
     # ---- pose stage behind the NMS (include/linemod_b200.h, lm_*_pose) ----
     def set_template_renders(self, first, depths, K, R, t):

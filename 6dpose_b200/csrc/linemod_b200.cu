@@ -220,6 +220,17 @@ struct lm_detector {
   uint16_t* fe_depth = nullptr; uint8_t* fe_nraw = nullptr;
   bool fe_lut = false;
 
+  // depth gate of the coarse scan (lm_set_depth_gate)
+  std::vector<float> tdepth;            // training distance per template of the bank (mm; NaN / <= 0: never gated)
+  bool gate_on = false; double gate_tau = 0.0;
+  bool gate_frame = false;              // the last enqueued frame ran gated
+  bool gate_dirty = true;               // h_gate_item no longer fits the shard / distances / tolerance
+  std::vector<uint2> h_gate_item;       // per work item of the shard: band and sample-cell offset (DepthGate::item)
+  int64_t gate_with_z = 0;              // work items of the shard with a distance
+  uint2* d_gate_item = nullptr; size_t gate_item_cap = 0;
+  uint32_t* d_cells = nullptr; size_t cells_cap = 0;
+  unsigned* d_gate_before = nullptr;
+
   bool timing = false;
   std::vector<cudaEvent_t> tev;  // timing slots x LM_TEV events (ring)
   int64_t timing_runs = 0;
@@ -271,8 +282,10 @@ extern "C" int lm_create(int device, int n_levels, const int* T, lm_detector** o
   // function attributes are per DEVICE: every handle raises the dynamic shared-memory limits on its own device
   // (a process may hold handles on several GPUs, e.g. lm_peer_connect_local across devices)
   CU(cudaFuncSetAttribute(k_linear_memories_band, cudaFuncAttributeMaxDynamicSharedMemorySize, LM_BAND_SMEM_LIMIT));
-  CU(cudaFuncSetAttribute(k_coarse_packed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LM_K2_SMEM_MAX));
-  CU(cudaFuncSetAttribute(k_coarse_packed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+  CU(cudaFuncSetAttribute(k_coarse_packed<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LM_K2_SMEM_MAX));
+  CU(cudaFuncSetAttribute(k_coarse_packed<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+  CU(cudaFuncSetAttribute(k_coarse_packed<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LM_K2_SMEM_MAX));
+  CU(cudaFuncSetAttribute(k_coarse_packed<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   CU(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
   CU(cudaStreamCreateWithFlags(&d->copy_stream, cudaStreamNonBlocking));
   CU(cudaEventCreateWithFlags(&d->ev_fork, cudaEventDisableTiming));
@@ -324,6 +337,7 @@ extern "C" void lm_destroy(lm_detector* d) {
     cudaFree(d->fe[l].mask[0]); cudaFree(d->fe[l].mask[1]);
   }
   cudaFree(d->fe_depth); cudaFree(d->fe_nraw);
+  cudaFree(d->d_gate_item); cudaFree(d->d_cells); cudaFree(d->d_gate_before);
   pose_stage_destroy(d->pose);
   for (cudaEvent_t e : d->tev) cudaEventDestroy(e);
   if (d->copy_stream) { cudaStreamSynchronize(d->copy_stream); cudaStreamDestroy(d->copy_stream); }
@@ -374,6 +388,8 @@ extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_
   d->class_of.clear();
   d->boxes.clear();  // box sizes belong to the bank they were set for
   d->post_dirty = true;
+  d->tdepth.clear();  // so do the training distances
+  d->gate_dirty = true;
   if (d->pose) pose_stage_clear(d->pose);  // so do the template renders
   d->feats.assign(feats, feats + (size_t)n_feats * 3);
   d->feat_slot.swap(slot_of);
@@ -464,6 +480,7 @@ extern "C" int lm_select_layout(lm_detector* d, const int32_t* class_sel, int n_
   d->sel.swap(sel);  // after the cuts: the lambda reads `sel`
   d->work_dirty = true;
   d->post_dirty = true;
+  d->gate_dirty = true;
   d->have_run = false;
   return LM_OK;
 }
@@ -856,6 +873,52 @@ static int prepare_work(lm_detector* d) {
   return LM_OK;
 }
 
+// The depth gate's per-work-item table for the shard ({zlo | zhi << 16, ox | oy << 16}, see include/linemod_b200.h) and
+// the cell-summary buffer for the frame size.  Only while the gate is on.
+static int prepare_gate(lm_detector* d) {
+  const LevelHost& low = d->lv[d->L - 1];
+  if ((size_t)low.plane > d->cells_cap) {
+    cudaFree(d->d_cells);
+    d->d_cells = nullptr;
+    d->cells_cap = (size_t)low.plane;
+    CU(cudaMalloc(&d->d_cells, sizeof(uint32_t) * d->cells_cap));
+  }
+  if (!d->d_gate_before) CU(cudaMalloc(&d->d_gate_before, sizeof(unsigned)));
+  if (!d->gate_dirty) return LM_OK;
+  const int64_t n = d->shard_count;
+  const int TL = d->T[d->L - 1];
+  d->h_gate_item.resize((size_t)n);
+  d->gate_with_z = 0;
+  for (int64_t w = 0; w < n; ++w) {
+    const int g = d->shard_sel[(size_t)w];
+    const int32_t* m4 = &d->tmeta[((size_t)g * d->S + (d->L - 1) * d->M) * 4];  // lowest level, modality 0
+    const uint32_t ox = (uint32_t)((m4[0] / 2) / TL), oy = (uint32_t)((m4[1] / 2) / TL);
+    const double z = (size_t)g < d->tdepth.size() ? (double)d->tdepth[(size_t)g] : NAN;
+    uint32_t zlo = 0, zhi = 65535;  // no distance: every depth lies in the band
+    if (z > 0.0) {
+      const double lo = std::min(std::max(ceil(z * (1.0 - d->gate_tau)), 0.0), 65535.0);
+      const double hi = std::min(std::max(floor(z * (1.0 + d->gate_tau)), 0.0), 65535.0);
+      zlo = (uint32_t)lo;
+      zhi = (uint32_t)hi;
+      ++d->gate_with_z;
+    }
+    d->h_gate_item[(size_t)w] = make_uint2(zlo | (zhi << 16), ox | (oy << 16));
+  }
+  if ((size_t)n > d->gate_item_cap) {
+    cudaFree(d->d_gate_item);
+    d->d_gate_item = nullptr;
+    d->gate_item_cap = (size_t)n;
+    CU(cudaMalloc(&d->d_gate_item, sizeof(uint2) * d->gate_item_cap));
+  }
+  // on the stream, behind the frames already enqueued (they keep the table they were enqueued with); waited for, since
+  // h_gate_item may change once this returns
+  if (n > 0)
+    CU(cudaMemcpyAsync(d->d_gate_item, d->h_gate_item.data(), sizeof(uint2) * (size_t)n, cudaMemcpyHostToDevice, d->stream));
+  CU(cudaStreamSynchronize(d->stream));
+  d->gate_dirty = false;
+  return LM_OK;
+}
+
 // Smallest raw score that survives remove_if(similarity < threshold) (LL.cpp:1935-1937), host twin of lm_min_kept_raw:
 // the same two IEEE single-precision operations ((raw * 100.f) / (4 * n)).
 static int host_min_kept_raw(float threshold, int nfeat) {
@@ -1225,10 +1288,21 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     int rc1 = launch_k1(d, k1, 0, k1_done);
     if (rc1) return rc1;
     if (d->timing) CU(cudaEventRecord(d->ev[1], st));
+    // depth gate: the frame's cell summary, ahead of K2
+    const bool gated = d->gate_frame;
+    DepthGate gate;  // read by the gated launches only
+    if (gated) {
+      gate.cells = d->d_cells; gate.item = d->d_gate_item; gate.before = d->d_gate_before;
+      gate.Wd = low.Wd; gate.Hd = low.Hd;
+      const int B = low.T << (d->L - 1);  // s * T_L full-resolution pixels per cell side
+      CU(launch_pdl(k_depth_cells, dim3((unsigned)((low.plane + 7) / 8)), dim3(256), 0, st, (const uint16_t*)d->fe_depth,
+                    d->fe[0].rows, d->fe[0].cols, B, low.Wd, low.Hd, d->d_cells, d->d_gate_before));
+      ++d->launches;
+    }
     // K2
     bool scan_fused = false;
     if (d->n_items_bits > 0) {
-      BitScanParams bp;
+      BitScanGateParams bp;
       bp.bp = low.d_bp; bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw + low.bp_zero);  // planes + the zero words
       bp.lbw = low.lbw; bp.plane = low.plane; bp.nwords = low.nwords;
       bp.tslot = d->d_tslot; bp.fdesc4 = d->d_fdesc4; bp.k2info = d->d_k2info; bp.work = d->d_work;
@@ -1251,16 +1325,20 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
       const CoarseShape c = coarse_shape(d->k2_tasks, d->sm_count, plane_bytes);
       bp.split = c.split;
       cudaError_t e = cudaSuccess;
-      if (c.smem) {
-        e = launch_pdl(k_coarse_packed<true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
+      if (gated) {
+        bp.gate = gate;
+        e = c.smem ? launch_pdl(k_coarse_packed<true, true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp)
+                   : launch_pdl(k_coarse_packed<false, true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
+      } else if (c.smem) {
+        e = launch_pdl(k_coarse_packed<true, false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, static_cast<const BitScanParams&>(bp));
       } else {
-        e = launch_pdl(k_coarse_packed<false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
+        e = launch_pdl(k_coarse_packed<false, false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, static_cast<const BitScanParams&>(bp));
       }
       if (e != cudaSuccess) return fail(LM_E_CUDA, "k_coarse_packed launch failed: %s", cudaGetErrorString(e));
       ++d->launches;
     }
     if (d->n_items_bytes > 0) {
-      ByteScanParams sp;
+      ByteScanGateParams sp;
       sp.lv = level_dev(low);
       sp.tslot = d->d_tslot; sp.fbase = d->d_fbase; sp.fxy = d->d_fxy; sp.work = d->d_work;
       sp.items = d->d_items_bytes;
@@ -1269,7 +1347,10 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
       sp.mask = d->d_mask; sp.raw = d->d_raw; sp.cnt = d->d_cnt;
       int bs = ((low.plane + 3) / 4 + 31) / 32 * 32;
       bs = std::max(32, std::min(bs, 1024));
-      CU(launch_pdl(k_coarse_bytes, dim3(d->n_items_bytes), dim3(bs), 0, st, sp));
+      if (gated) {
+        sp.gate = gate;
+        CU(launch_pdl(k_coarse_bytes<true>, dim3(d->n_items_bytes), dim3(bs), 0, st, sp));
+      } else CU(launch_pdl(k_coarse_bytes<false>, dim3(d->n_items_bytes), dim3(bs), 0, st, static_cast<const ByteScanParams&>(sp)));
       ++d->launches;
     }
     if (d->timing) CU(cudaEventRecord(d->ev[2], st));
@@ -1504,6 +1585,16 @@ extern "C" int lm_enqueue(lm_detector* d, float threshold) {
   if (rc) return rc;
   rc = ensure_run_buffers(d);
   if (rc) return rc;
+  if (d->gate_on) {
+    bool any_z = false;
+    for (float z : d->tdepth) any_z = any_z || z > 0.f;
+    if (!any_z) return fail(LM_E_STATE, "depth gate on, but no template of the bank has a training distance (lm_set_template_depths)");
+    if (!d->frame_depth)
+      return fail(LM_E_STATE, "depth gate on, but the frame has no depth image (lm_upload_quantized / lm_bind_quantized_device)");
+    rc = prepare_gate(d);
+    if (rc) return rc;
+  }
+  d->gate_frame = d->gate_on;
   d->last_threshold = threshold;
   rc = filter_thresholds(d, threshold);
   if (rc) return rc;
@@ -1520,6 +1611,10 @@ extern "C" int lm_prepare(lm_detector* d) {
   if (rc) return rc;
   rc = prepare_work(d);
   if (rc) return rc;
+  if (d->gate_on) {
+    rc = prepare_gate(d);
+    if (rc) return rc;
+  }
   return ensure_run_buffers(d);
 }
 
@@ -2144,6 +2239,57 @@ extern "C" int lm_set_pose_estimation(lm_detector* d, int estimation) {
   if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT)
     return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
   d->pose_estimation = estimation;
+  return LM_OK;
+}
+
+extern "C" int lm_set_template_depths(lm_detector* d, int64_t first, int64_t n, const float* z_mm) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (first < 0 || n < 0 || first + n > d->G)
+    return fail(LM_E_INVALID, "templates [%lld, %lld) outside the bank's %d", (long long)first, (long long)(first + n), d->G);
+  if (n > 0 && !z_mm) return fail(LM_E_INVALID, "null distances");
+  if (d->tdepth.size() != (size_t)d->G) d->tdepth.assign((size_t)d->G, NAN);
+  for (int64_t i = 0; i < n; ++i) d->tdepth[(size_t)(first + i)] = z_mm[i];
+  d->gate_dirty = true;
+  return LM_OK;
+}
+
+extern "C" int lm_set_depth_gate(lm_detector* d, int on, double tolerance) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (!(tolerance >= 0.0 && tolerance < 1.0)) return fail(LM_E_INVALID, "depth gate tolerance %g outside [0, 1)", tolerance);
+  if (tolerance != d->gate_tau) d->gate_dirty = true;
+  d->gate_on = on != 0;
+  d->gate_tau = tolerance;
+  return LM_OK;
+}
+
+// The result header the last frame's coarse scan wrote (its shard's candidate count): this rank's block of the frame slot
+// with a connected exchange, else the result block (a result-block retry carries the header over to the grown block).
+static const lm_result_header* scan_header(const lm_detector* d) {
+  if (d->px_rank >= 0)
+    return reinterpret_cast<const lm_result_header*>(d->px_buf + (size_t)(d->px_seq & 1) * d->h_px.slot_bytes +
+                                                     (size_t)d->h_px.rank * d->h_px.block_bytes);
+  return d->d_res;
+}
+
+extern "C" int lm_depth_gate_stats(lm_detector* d, int64_t* out4) {
+  if (!d || !out4) return fail(LM_E_INVALID, "null argument");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
+  if (!d->gate_frame || !d->d_res) return fail(LM_E_STATE, "the last frame did not run with the depth gate");
+  CU(cudaSetDevice(d->device));
+  const LevelHost& low = d->lv[d->L - 1];
+  std::vector<uint32_t> cells((size_t)low.plane);
+  unsigned before = 0;
+  lm_result_header hdr;
+  CU(cudaMemcpyAsync(cells.data(), d->d_cells, sizeof(uint32_t) * cells.size(), cudaMemcpyDeviceToHost, d->stream));
+  CU(cudaMemcpyAsync(&before, d->d_gate_before, sizeof(unsigned), cudaMemcpyDeviceToHost, d->stream));
+  CU(cudaMemcpyAsync(&hdr, scan_header(d), sizeof(hdr), cudaMemcpyDeviceToHost, d->stream));
+  CU(cudaStreamSynchronize(d->stream));
+  int64_t empty = 0;
+  for (uint32_t c : cells) empty += (c & 0xFFFFu) > (c >> 16);
+  out4[0] = before;
+  out4[1] = hdr.coarse_candidates;
+  out4[2] = empty;
+  out4[3] = d->gate_with_z;
   return LM_OK;
 }
 

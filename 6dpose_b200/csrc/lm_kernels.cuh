@@ -418,6 +418,62 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int* s_warp, int* tot
 }
 
 // --------------------------------------------------------------------------------------------
+// Depth gate of the coarse scan (lm_set_depth_gate; semantics in include/linemod_b200.h).  k_depth_cells summarises the
+// frame's depth per coarse cell, the gated K2 variants drop a passing position whose sample cell's depth range misses
+// the template's band, before it is counted.
+// --------------------------------------------------------------------------------------------
+struct DepthGate {
+  const uint32_t* cells;  // [Hd][Wd] lo | hi << 16 of the non-zero depths of the cell's block; empty: lo 0xFFFF > hi 0
+  const uint2* item;      // per work item of the shard: zlo | zhi << 16, ox | oy << 16 (sample cell offset)
+  unsigned* before;       // candidates before the gate (zeroed by k_depth_cells)
+  int Wd, Hd;
+};
+
+// one warp per cell: min / max of the non-zero pixels of the full-resolution block [x*B, x*B + B) x [y*B, y*B + B)
+__global__ void __launch_bounds__(256) k_depth_cells(const uint16_t* __restrict__ depth, int rows, int cols, int B, int Wd,
+                                                      int Hd, uint32_t* __restrict__ cells, unsigned* __restrict__ before) {
+  lm_pdl_wait();
+  if (blockIdx.x == 0 && threadIdx.x == 0) *before = 0u;
+  const int cell = (int)blockIdx.x * 8 + ((int)threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (cell >= Wd * Hd) return;
+  const int x0 = (cell % Wd) * B, y0 = (cell / Wd) * B;
+  const int x1 = min(x0 + B, cols), y1 = min(y0 + B, rows);
+  unsigned lo = 0xFFFFu, hi = 0u;
+  for (int i = lane; i < B * B; i += 32) {
+    const int y = y0 + i / B, x = x0 + i % B;
+    if (y < y1 && x < x1) {
+      const unsigned v = __ldg(depth + (size_t)y * cols + x);
+      if (v) { lo = min(lo, v); hi = max(hi, v); }
+    }
+  }
+  lo = __reduce_min_sync(0xffffffffu, lo);
+  hi = __reduce_max_sync(0xffffffffu, hi);
+  if (lane == 0) cells[cell] = lo | (hi << 16);
+}
+
+// the bits of `pass` (positions j0 + b of work item w) that survive the gate
+__device__ __forceinline__ uint32_t depth_gate(const DepthGate& g, int w, int j0, uint32_t pass) {
+  uint32_t keep = pass;
+  if (pass) {
+    const uint2 it = __ldg(g.item + w);
+    const unsigned zlo = it.x & 0xFFFFu, zhi = it.x >> 16;
+    const int ox = (int)(it.y & 0xFFFFu), oy = (int)(it.y >> 16);
+    while (pass) {
+      const int b = __ffs(pass) - 1;
+      pass &= pass - 1;
+      const int j = j0 + b;
+      const int sx = j % g.Wd + ox, sy = j / g.Wd + oy;
+      if (sx < g.Wd && sy < g.Hd) {
+        const uint32_t c = __ldg(g.cells + sy * g.Wd + sx);
+        const unsigned lo = c & 0xFFFFu, hi = c >> 16;
+        if (lo <= hi && (lo > zhi || hi < zlo)) keep &= ~(1u << b);  // a non-empty cell outside the band
+      }
+    }
+  }
+  return keep;
+}
+
+// --------------------------------------------------------------------------------------------
 // K2 (bit-sliced): coarse similarity scan over the lowest pyramid level.
 //
 // The response of a feature with orientation o at a position is 4*H + N with H = spread bit o and
@@ -460,6 +516,12 @@ struct BitScanParams {
   int* ticket;     // zero between launches
   int split;       // warps per team (1, 2, 4 or 8): a task's features are dealt over the team (see k_coarse_packed)
 };
+// the gated variants' parameters (a separate type: the ungated kernels keep their parameter block, and with it their code)
+struct BitScanGateParams : BitScanParams {
+  DepthGate gate;
+};
+template <bool kGate> struct BitScanArgs { typedef BitScanParams type; };
+template <> struct BitScanArgs<true> { typedef BitScanGateParams type; };
 
 #define CSA(sum, carry, a, b, c)                 \
   {                                              \
@@ -549,7 +611,8 @@ __global__ void __launch_bounds__(1024) k_scan_counts(int32_t* __restrict__ cnt,
 
 // score = 4*CH + CN (bit-sliced ripple add), positions >= P are zero (LL.cpp:1314), compare with the
 // smallest passing raw score, emit the pass mask and the raw scores of the passing positions
-__device__ __forceinline__ void coarse_emit(const BitScanParams& p, int w, int idx, int P, int nfeat, int words,
+template <bool kGate>
+__device__ __forceinline__ void coarse_emit(const typename BitScanArgs<kGate>::type& p, int w, int idx, int P, int nfeat, int words,
                                             const uint32_t (&ch)[8], const uint32_t (&cn)[8]) {
   const int raw_min = lm_min_passing_raw(p.threshold, nfeat);
   const int j0 = idx * 32;
@@ -585,6 +648,12 @@ __device__ __forceinline__ void coarse_emit(const BitScanParams& p, int w, int i
     }
     pass = (gt | eq) & valid;
   }
+  if constexpr (kGate) {
+    const uint32_t am = __activemask();  // warp-aggregated count of the candidates before the gate
+    const unsigned n = __reduce_add_sync(am, (unsigned)__popc(pass));
+    if (n && (int)(threadIdx.x & 31) == __ffs(am) - 1) atomicAdd(p.gate.before, n);
+    pass = depth_gate(p.gate, w, j0, pass);
+  }
   p.mask[(size_t)w * p.nwords + idx] = pass;
   int my_count = __popc(pass);
   while (pass) {
@@ -602,6 +671,10 @@ __device__ __forceinline__ void coarse_emit(const BitScanParams& p, int w, int i
       uint32_t ps = 0u;
       if (raw_min == 0) {
         ps = (p.plane - q0 < 32) ? (0xffffffffu >> (32 - (p.plane - q0))) : 0xffffffffu;
+        if constexpr (kGate) {
+          atomicAdd(p.gate.before, (unsigned)__popc(ps));
+          ps = depth_gate(p.gate, w, q0, ps);
+        }
         for (int b = 0; b < 32; ++b)
           if ((ps >> b) & 1u) p.raw[(size_t)w * p.plane + q0 + b] = 0;
       }
@@ -632,8 +705,8 @@ __device__ __forceinline__ void team_bar(int id, int nthreads) {
 // the 8-feature steps q, q + S, ... of every modality, the partial counters meet in shared memory and warp 0 of the team
 // emits.  A task is then a chain S times shorter -- the latency of the kernel follows the shard instead of staying one
 // whole task (what keeps a 1/8 shard from being 8 times faster, and what holds an SM's shared memory for the duration).
-template <bool kSmem>
-__global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanParams p) {
+template <bool kSmem, bool kGate>
+__global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(typename BitScanArgs<kGate>::type p) {
   lm_pdl_wait();
   extern __shared__ __align__(128) uint32_t s_bp[];
   __shared__ __align__(8) unsigned long long s_bar;
@@ -748,7 +821,7 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
           }
           team_bar(team + 1, S * 32);  // the partials are in registers: the others may overwrite them
         }
-        if (q == 0) coarse_emit(p, w, idx, P, nfeat, words, ch, cn);
+        if (q == 0) coarse_emit<kGate>(p, w, idx, P, nfeat, words, ch, cn);
       } else {
         // ---- remainders: lane k owns entry e of the shard's remainder words ----
         const int e = (task - p.n_full) * 32 + lane;
@@ -811,7 +884,7 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(BitScanPar
           }
           team_bar(team + 1, S * 32);  // the partials are in registers: the others may overwrite them
         }
-        if (active && q == 0) coarse_emit(p, w, idx, P, nfeat, words, ch, cn);
+        if (active && q == 0) coarse_emit<kGate>(p, w, idx, P, nfeat, words, ch, cn);
       }
       if (S == 1) {
         int nxt = 0;
@@ -858,10 +931,17 @@ struct ByteScanParams {
   uint16_t* raw;
   int32_t* cnt;
 };
+// the gated variant's parameters (a separate type: the ungated kernel keeps its parameter block, and with it its code)
+struct ByteScanGateParams : ByteScanParams {
+  DepthGate gate;
+};
+template <bool kGate> struct ByteScanArgs { typedef ByteScanParams type; };
+template <> struct ByteScanArgs<true> { typedef ByteScanGateParams type; };
 
 #define SCAN_FEAT_TILE 512
 
-__global__ void __launch_bounds__(1024) k_coarse_bytes(ByteScanParams p) {
+template <bool kGate>
+__global__ void __launch_bounds__(1024) k_coarse_bytes(typename ByteScanArgs<kGate>::type p) {
   lm_pdl_wait();
   __shared__ uint32_t s_base[SCAN_FEAT_TILE];
   __shared__ int s_count;
@@ -876,6 +956,7 @@ __global__ void __launch_bounds__(1024) k_coarse_bytes(ByteScanParams p) {
   for (int m = 0; m < p.M; ++m) nfeat += p.tslot[(size_t)g * p.S + p.slot_low + m].y;
 
   int counted = 0;
+  unsigned ungated = 0;  // kGate: candidates before the gate
   // every thread owns 4 consecutive positions; a warp therefore owns 4 mask words per pass
   const int span = blockDim.x * 4;
   const int plane_up = (plane + 127) & ~127;
@@ -925,8 +1006,15 @@ __global__ void __launch_bounds__(1024) k_coarse_bytes(ByteScanParams p) {
     for (int k = 0; k < 4; ++k)
       if (j + k < plane && lm_score(raw[k], nfeat) > p.threshold) {
         pass |= 1u << k;
-        p.raw[(size_t)w * plane + j + k] = (uint16_t)raw[k];
+        if (!kGate) p.raw[(size_t)w * plane + j + k] = (uint16_t)raw[k];
       }
+    if constexpr (kGate) {
+      ungated += __popc(pass);
+      pass = depth_gate(p.gate, w, j, pass);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if ((pass >> k) & 1u) p.raw[(size_t)w * plane + j + k] = (uint16_t)raw[k];
+    }
     // 8 lanes -> one 32-bit mask word
     uint32_t word = pass << (4 * (lane & 7));
     word |= __shfl_xor_sync(0xffffffffu, word, 1);
@@ -936,6 +1024,10 @@ __global__ void __launch_bounds__(1024) k_coarse_bytes(ByteScanParams p) {
     counted += __popc(pass);
   }
   counted = __reduce_add_sync(0xffffffffu, counted);
+  if constexpr (kGate) {
+    ungated = __reduce_add_sync(0xffffffffu, ungated);
+    if (lane == 0 && ungated) atomicAdd(p.gate.before, ungated);
+  }
   __syncthreads();
   if (lane == 0 && counted) atomicAdd(&s_count, counted);
   __syncthreads();

@@ -65,6 +65,7 @@ class Detector:
         self._bank_dirty = True
         self._class_order = []
         self._selection = None
+        self._template_depths = None  # training distances registered with the native handle (setTemplateDepths)
         self._peers = None  # (rank, world) once dist.connect_peers has wired the fused exchange
         self.device = _default_device()
         self.shard = (0, 1)  # (index, count): template shard matched by this process (multi-GPU)
@@ -122,6 +123,7 @@ class Detector:
             self._native.load_bank(packed, self.pyramid_levels * 2)
             self._bank_dirty = False
             self._selection = None
+            self._template_depths = None  # lm_load_bank drops them
         return self._native
 
     def _select(self, class_ids):
@@ -187,6 +189,59 @@ class Detector:
                 raise ValueError("class %s: %d box sizes for %d templates" % (cid, wh.shape[0], self.bank.num_templates(cid)))
             rows.append(wh)
         nat.set_boxes(np.concatenate(rows, 0))
+
+    # ---- depth gate of the coarse scan (include/linemod_b200.h, lm_set_depth_gate) ----
+    def setTemplateDepths(self, depths):
+        """Training distance (mm) per template for the depth gate: dict class_id -> sequence [n_templates] indexed by
+        template id.  Classes left out, NaN and values <= 0 are never gated.  Loading another bank drops them."""
+        order = self.bank.class_ids()
+        unknown = [c for c in depths if c not in order]
+        if unknown:
+            raise ValueError("setTemplateDepths: classes %s are not in the bank" % ", ".join(repr(c) for c in unknown))
+        rows = []
+        for cid in order:
+            n = self.bank.num_templates(cid)
+            if cid in depths:
+                z = np.asarray(depths[cid], np.float32).reshape(-1)
+                if z.shape[0] != n:
+                    raise ValueError("class %s: %d distances for %d templates" % (cid, z.shape[0], n))
+            else:
+                z = np.full(n, np.nan, np.float32)
+            rows.append(z)
+        z = np.concatenate(rows) if rows else np.zeros(0, np.float32)
+        nat = self._ensure_native()
+        nat.set_template_depths(0, z)
+        self._template_depths = z
+
+    @staticmethod
+    def templateDepthsFromInfo(infos):
+        """The drivers' template-info files (dict class_id -> {template_id: {"cam_t_w2c": [x, y, z], ...}}, as yaml.load
+        reads <class>_info.yaml) to setTemplateDepths' argument: the distance of template i is cam_t_w2c[2] of entry i."""
+        out = {}
+        for cid, info in infos.items():
+            ids = sorted(int(k) for k in info)
+            if ids != list(range(len(ids))):
+                raise ValueError("class %s: info entries are not the template ids 0..%d" % (cid, len(ids) - 1))
+            get = lambda i: info[i] if i in info else info[str(i)]
+            out[cid] = np.asarray([float(get(i)["cam_t_w2c"][2]) for i in ids], np.float32)
+        return out
+
+    def setDepthGate(self, tolerance):
+        """Gate the coarse scan by scene depth (include/linemod_b200.h): a template's candidates only where the depth
+        around its centre lies within [z (1 - tolerance), z (1 + tolerance)] of its training distance z.  Every match
+        path that takes a depth image (match, match_refine, detect, the batch calls, dist's sharded calls) picks it up
+        from the next frame on; paths from quantized images (match_top, match_quantized) have no depth and refuse to run
+        while it is on.  None turns it off."""
+        if tolerance is not None:
+            _lib.depth_gate_tolerance(tolerance)
+            z = self._template_depths
+            if self._bank_dirty or z is None or not (z > 0).any():
+                raise RuntimeError("setDepthGate: no training distances registered for this bank (setTemplateDepths first)")
+        self._ensure_native().set_depth_gate(tolerance)
+
+    def depthGateStats(self):
+        """Of the last frame, which ran gated: dict(before, after, empty_cells, with_distance) (lm_depth_gate_stats)."""
+        return self._ensure_native().depth_gate_stats()
 
     def match_top(self, quantized, threshold, class_ids=(), iou_threshold=0.5, top_k=3):
         """match + nms(dets, iou_threshold)[:top_k] of the reference's drivers (linemod_and_levelup_test.py:

@@ -376,6 +376,42 @@ int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const in
 int lm_match_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, int rows, int cols, const uint8_t* mask_color,
                     const uint8_t* mask_depth, float threshold, lm_match* out, int64_t cap, int64_t* n_out);
 
+/* Depth gate of the coarse scan (off by default).  A bank rendered at several distances (the reference's allScales: 337
+ * views at each of 600 ... 1800 mm) treats each scale as its own object, and small scales match random texture; the gate
+ * keeps a template's coarse candidates only where the scene lies near the distance the template was trained at.
+ * L = the lowest pyramid level, s = 2^(L-1) (levels - 1 halvings), T_L its step, Wd x Hd its coarse grid.  For candidate
+ * position (cx, cy) of template t in the coarse scan, before its pass bit is counted:
+ *   1. Cell summary, per frame: block (x, y) = full-resolution pixels [x*s*T_L, (x+1)*s*T_L) x [y*s*T_L, (y+1)*s*T_L) of
+ *      the uploaded depth (u16 mm; masks do not affect it); lo(x, y) / hi(x, y) = min / max non-zero depth of the block.
+ *      A block without a non-zero pixel is empty.
+ *   2. Sample cell (sx, sy) = (cx + floor(floor(w_t / 2) / T_L), cy + floor(floor(h_t / 2) / T_L)), w_t x h_t =
+ *      Template::width / height of t at level L, modality 0 (tmeta).
+ *   3. Band zlo_t = ceil(z_t * (1 - tau)), zhi_t = floor(z_t * (1 + tau)), in float64, clamped to [0, 65535]; z_t = the
+ *      template's training distance (mm), tau = the tolerance.
+ *   4. The candidate passes iff sx >= Wd, or sy >= Hd, or the sample cell is empty, or t has no distance, or
+ *      (lo <= zhi_t and hi >= zlo_t).  Every other candidate is removed before the candidate list, exactly as if its raw
+ *      score were below the threshold; the match list is the reference's matchClass / sort / unique over the gated
+ *      candidate set (so unique may keep a different template of a collapsed pair).
+ * The gate adds one launch per frame (k_depth_cells, ahead of the coarse scan) and runs the gated variants of the coarse
+ * kernels; with the gate off nothing of the frame changes.
+ *   lm_set_template_depths  z_mm[i] = training distance of template first + i, bank order (as lm_set_boxes); NaN or <= 0:
+ *                           never gated.  Loading another bank drops the distances.  LM_E_INVALID for a range outside the
+ *                           bank.
+ *   lm_set_depth_gate       on != 0 turns the gate on with `tolerance` (tau), for the next lm_enqueue (single frame or
+ *                           batch); no device work, and a frame keeps the setting it was enqueued with (the rerun after a
+ *                           result-block retry included).  LM_E_INVALID for tolerance < 0, >= 1 or NaN.  With the gate on,
+ *                           lm_enqueue fails with LM_E_STATE when no template of the bank has a distance, or when the
+ *                           frame has no depth (lm_upload_quantized / lm_bind_quantized_device).  With a connected peer
+ *                           exchange, every rank setting the same distances and gate before its next frame is the caller's
+ *                           promise, as with lm_peer_share_pose: each rank gates its own shard on its own copy of the frame.
+ *   lm_depth_gate_stats     of the last enqueued frame (single frame, or the last of a batch), which must have run gated
+ *                           (else LM_E_STATE): [0] candidates of this handle's shard before the gate, [1] after it,
+ *                           [2] empty cells, [3] work items of this handle's shard with a distance.  Synchronises the
+ *                           stream. */
+int lm_set_template_depths(lm_detector* d, int64_t first, int64_t n, const float* z_mm);
+int lm_set_depth_gate(lm_detector* d, int on, double tolerance);
+int lm_depth_gate_stats(lm_detector* d, int64_t* out4);
+
 /* ---- introspection used by the parity tests and the benchmark ---- */
 /* Quantized label image of (level, modality) of the uploaded frame: rows*cols bytes. */
 int lm_debug_quantized(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap);
