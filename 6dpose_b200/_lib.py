@@ -23,7 +23,7 @@ HEADER_DTYPE = np.dtype([("count", "<i4"), ("coarse_candidates", "<i4"), ("capac
 PEER_HANDLE_BYTES = 64
 
 SYMBOLS = [
-    "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks",
+    "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks", "lm_coarse_descriptors",
     "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
@@ -87,6 +87,9 @@ def load():
     L.lm_select_layout.argtypes = [vp, i32p, c_int, c_int, c_int, c_int]
     L.lm_prepare.argtypes = [vp]
     L.lm_coarse_tasks.argtypes = [i32p, c_i64, c_int, c_i64, i32p, c_i64] + [ctypes.POINTER(c_i64)] * 3 + [i32p]
+    L.lm_coarse_descriptors.argtypes = [i32p, i32p] + [c_int] * 7 + [ctypes.POINTER(ctypes.c_uint32), c_i64,
+                                                                        ctypes.POINTER(c_i64), i32p, ctypes.POINTER(ctypes.c_uint8),
+                                                                        ctypes.POINTER(ctypes.c_uint32)]
     L.lm_shard_range.argtypes = [vp, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     L.lm_upload_quantized.argtypes = [vp, u8pp, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]
     u8p_ = ctypes.POINTER(ctypes.c_uint8)
@@ -176,6 +179,28 @@ def coarse_tasks(words, sm_count, plane_bytes):
                             ctypes.byref(n_rem), None))
     return table, n_full.value, n_rem.value, dict(tasks=int(shape[0]), split=int(shape[1]), warps_per_cta=int(shape[2]),
                                                   grid=int(shape[3]))
+
+
+def coarse_descriptors(feats, tmeta, M, slot_low, T, rows, cols):
+    """lm_coarse_descriptors: the bit-sliced coarse scan's feature descriptors of a packed bank (feats [n, 3], tmeta
+    [G, S, 4]) at the level of slots slot_low .. slot_low + M - 1 (sampling step T, rows x cols).  Returns (desc uint32,
+    info [G, 2] int32 = first descriptor and feature count, fits [G] bool, zero descriptor); no device needed."""
+    L = load()
+    feats = np.ascontiguousarray(feats, np.int32).reshape(-1, 3)
+    tmeta = np.ascontiguousarray(tmeta, np.int32)
+    G = len(tmeta)
+    tmeta = tmeta.reshape(G, -1, 4)
+    S = tmeta.shape[1]
+    i32p, u32p = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint32)
+    n_desc, zero = ctypes.c_int64(), ctypes.c_uint32()
+    info = np.zeros((G, 2), np.int32)
+    fits = np.zeros(G, np.uint8)
+    args = (feats.ctypes.data_as(i32p), tmeta.ctypes.data_as(i32p), G, S, M, slot_low, T, rows, cols)
+    check(L.lm_coarse_descriptors(*args, None, 0, ctypes.byref(n_desc), info.ctypes.data_as(i32p),
+                                  fits.ctypes.data_as(ctypes.POINTER(ctypes.c_uint8)), ctypes.byref(zero)))
+    desc = np.zeros(n_desc.value, np.uint32)
+    check(L.lm_coarse_descriptors(*args, desc.ctypes.data_as(u32p), len(desc), ctypes.byref(n_desc), None, None, None))
+    return desc, info, fits.astype(bool), int(zero.value)
 
 
 def check(rc):

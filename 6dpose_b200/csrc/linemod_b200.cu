@@ -90,8 +90,15 @@ struct LevelHost {
   uint32_t mod_stride = 0;
   uint32_t* d_bp = nullptr;  // lowest level only: spread bit-planes [M][8][lbw]
   int lbw = 0, nwords = 0, rounds = 0;
-  int bp_zero = 0;   // words of zeros behind the bit-planes (where skipped / padding descriptors point)
 };
+
+// Words per label block of the lowest level's bit-planes: T*T*plane bits, then slack for the reads of lanes beyond the
+// last word (a lane reads words idx and idx + 1 of a window, idx < 32 * rounds).  K1 never writes the slack, so a
+// window that starts at the first slack word reads zeros in every lane (the coarse scan's zero descriptor).
+static size_t bp_label_words(int T, int plane) {
+  const size_t nwords = ((size_t)plane + 31) / 32, rounds = (nwords + 31) / 32;
+  return (((size_t)T * T * plane + 31) / 32 + 32 * rounds + 4 + 3) & ~(size_t)3;
+}
 
 struct lm_detector {
   int device = 0;
@@ -114,10 +121,8 @@ struct lm_detector {
   TSlot* d_tslot = nullptr;
   uint32_t* d_fbase = nullptr;
   uint32_t* d_fxy = nullptr;
-  uint4* d_fdesc4 = nullptr;         // lowest-level features for k_coarse_packed: byte offsets of the label's plane window and of
-                                     // its two neighbour labels' (x, y, z) + bit shift (w); per (template, modality) padded to
-                                     // a multiple of 8 with entries that point at the all-zero words behind the planes
-  int2* d_k2info = nullptr;          // [G][M]: first descriptor, padded count
+  uint32_t* d_fdesc = nullptr;       // lowest-level features for k_coarse_packed, one word each (coarse_descriptors)
+  int2* d_k2info = nullptr;          // [G]: first descriptor, lowest-level features
   std::vector<uint8_t> bits_ok;      // per template: the bit-sliced coarse kernel may take it
   std::vector<uint8_t> safe;         // per template: refinement never skips a feature (LL.cpp:1394)
   uint8_t* d_safe = nullptr;
@@ -323,7 +328,7 @@ extern "C" void lm_destroy(lm_detector* d) {
   if (d->stream) cudaStreamSynchronize(d->stream);
   peer_release(d);
   for (int l = 0; l < LM_MAX_LEVELS; ++l) free_level(d->lv[l]);
-  cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc4); cudaFree(d->d_k2info); cudaFree(d->d_work);
+  cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc); cudaFree(d->d_k2info); cudaFree(d->d_work);
   cudaFree(d->d_items_bytes); cudaFree(d->d_k2task); cudaFree(d->d_safe); cudaFree(d->d_galign);
   cudaFree(d->d_mask); cudaFree(d->d_raw); cudaFree(d->d_cnt); cudaFree(d->d_off);
   cudaFree(d->d_res_own); cudaFree(d->d_counters);
@@ -393,8 +398,8 @@ extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_
   if (d->pose) pose_stage_clear(d->pose);  // so do the template renders
   d->feats.assign(feats, feats + (size_t)n_feats * 3);
   d->feat_slot.swap(slot_of);
-  cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc4); cudaFree(d->d_k2info);
-  d->d_tslot = nullptr; d->d_fbase = nullptr; d->d_fxy = nullptr; d->d_fdesc4 = nullptr; d->d_k2info = nullptr;
+  cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc); cudaFree(d->d_k2info);
+  d->d_tslot = nullptr; d->d_fbase = nullptr; d->d_fxy = nullptr; d->d_fdesc = nullptr; d->d_k2info = nullptr;
   if (d->device >= 0 && G > 0) CU(cudaMalloc(&d->d_tslot, sizeof(TSlot) * (size_t)G * n_slots));
   if (d->device >= 0 && n_feats > 0) {
     CU(cudaMalloc(&d->d_fbase, sizeof(uint32_t) * (size_t)n_feats));
@@ -492,6 +497,88 @@ extern "C" int lm_shard_range(lm_detector* d, int64_t* begin, int64_t* count) {
   return LM_OK;
 }
 
+// k_coarse_packed's feature descriptors: one word per lowest-level feature,
+//   bits 0-4  bit shift of the window inside its first word (inner & 31),
+//   bit 5     label 0: the lower neighbour label's plane is 7 planes up,
+//   bit 6     label 7: the upper neighbour label's plane is 7 planes down,
+//   bits 7-31 word offset of the window in the plane buffer: (m * 8 + label) * lbw + (inner >> 5),
+// with inner = the feature's bit position inside its label block.  The neighbour labels' windows lie one plane below and
+// above (lbw words), or 7 planes the other way at the two ends.  Features outside the level (LL.cpp:1330) and the padding
+// get the zero descriptor: a window at the first slack word of label block 1, whose own and neighbours' windows read
+// zeros (bp_label_words), so the kernel's loop has neither a skip branch nor a bounds check.  The features of a template
+// (all modalities, in order) lie end to end from info.x, info.y of them, padded to a multiple of 32 so that one warp
+// loads 32 of them with one aligned 128-byte load.  A template fits when every word offset does (25 bits); one that
+// does not gets no descriptors and fits = 0.
+#define LM_DESC_WORD_BITS 25
+static uint32_t coarse_zero_descriptor(int T, int plane) {
+  return (uint32_t)((bp_label_words(T, plane) + ((size_t)T * T * plane + 31) / 32) << 7);
+}
+static void coarse_descriptors(const int32_t* feats, const int32_t* tmeta, int G, int S, int M, int slot_low, int T, int rows,
+                               int cols, std::vector<uint32_t>& desc, std::vector<int2>& info, std::vector<uint8_t>& fits) {
+  const int Wd = cols / T, Hd = rows / T, plane = Wd * Hd;
+  const uint64_t lbw = bp_label_words(T, plane);
+  const uint32_t zero = coarse_zero_descriptor(T, plane);
+  const bool zero_fits = lbw + ((uint64_t)T * T * plane + 31) / 32 < (1ull << LM_DESC_WORD_BITS);
+  desc.clear();
+  info.assign((size_t)G, make_int2(0, 0));
+  fits.assign((size_t)G, 0);
+  for (int g = 0; g < G; ++g) {
+    const size_t first = desc.size();
+    bool ok = zero_fits;
+    int n = 0;
+    for (int m = 0; m < M; ++m) {
+      const int32_t* tm = &tmeta[((size_t)g * S + slot_low + m) * 4];
+      for (int k = 0; k < tm[3]; ++k, ++n) {
+        const int32_t* f = &feats[3 * ((size_t)tm[2] + k)];
+        const int x = f[0], y = f[1], lab = f[2];
+        if (x >= cols || y >= rows) {
+          desc.push_back(zero);
+          continue;
+        }
+        const uint64_t inner = (uint64_t)((y % T) * T + (x % T)) * plane + (uint64_t)(y / T) * Wd + (x / T);
+        const uint64_t wh = (uint64_t)(m * 8 + lab) * lbw + (inner >> 5);
+        ok = ok && wh < (1ull << LM_DESC_WORD_BITS);
+        desc.push_back((uint32_t)(wh << 7) | ((lab == 7) ? 0x40u : 0u) | ((lab == 0) ? 0x20u : 0u) | (uint32_t)(inner & 31));
+      }
+    }
+    if (!ok) {
+      desc.resize(first);
+      info[(size_t)g] = make_int2((int)first, 0);
+      continue;
+    }
+    while ((desc.size() - first) % 32) desc.push_back(zero);
+    info[(size_t)g] = make_int2((int)first, n);
+    fits[(size_t)g] = 1;
+  }
+}
+
+extern "C" int lm_coarse_descriptors(const int32_t* feats, const int32_t* tmeta, int G, int S, int M, int slot_low, int T,
+                                     int rows, int cols, uint32_t* desc, int64_t cap, int64_t* n_desc, int32_t* info,
+                                     uint8_t* fits, uint32_t* zero) {
+  if (G < 0 || (G > 0 && (!feats || !tmeta)) || M < 1 || slot_low < 0 || slot_low + M > S || T < 1 ||
+      rows < T || cols < T)
+    return fail(LM_E_INVALID, "bad arguments");
+  for (int64_t i = 0; i < (int64_t)G * M; ++i) {
+    const int32_t* tm = &tmeta[((size_t)(i / M) * S + slot_low + i % M) * 4];
+    if (tm[2] < 0 || tm[3] < 0) return fail(LM_E_INVALID, "template %lld: bad feature range", (long long)(i / M));
+  }
+  std::vector<uint32_t> d;
+  std::vector<int2> k2;
+  std::vector<uint8_t> ok;
+  coarse_descriptors(feats, tmeta, G, S, M, slot_low, T, rows, cols, d, k2, ok);
+  if (n_desc) *n_desc = (int64_t)d.size();
+  if (zero) *zero = coarse_zero_descriptor(T, (cols / T) * (rows / T));
+  for (int g = 0; g < G; ++g) {
+    if (info) { info[2 * g] = k2[(size_t)g].x; info[2 * g + 1] = k2[(size_t)g].y; }
+    if (fits) fits[g] = ok[(size_t)g];
+  }
+  if (desc) {
+    if (cap < (int64_t)d.size()) return fail(LM_E_CAPACITY, "%lld descriptors, room for %lld", (long long)d.size(), (long long)cap);
+    std::copy(d.begin(), d.end(), desc);
+  }
+  return LM_OK;
+}
+
 // Feature addresses depend on the frame size (Wd, Hd); recomputed when it changes.
 static int prepare_bank(lm_detector* d) {
   bool same = d->prepared;
@@ -544,42 +631,21 @@ static int prepare_bank(lm_detector* d) {
       d->bits_ok[g] = (total <= 255 && same) ? 1 : 0;
     }
   }
-  // k_coarse_packed descriptors: per lowest-level feature the byte offsets (inside the bit-plane buffer) of the window
-  // start of its label's plane and of the two neighbouring labels' planes, and the bit shift.  Features outside the
-  // image (LL.cpp:1330) and the padding to a multiple of 8 per (template, modality) point at the zero words behind the
-  // planes, so the kernel's loop has neither a skip branch nor a bounds check.
-  cudaFree(d->d_fdesc4); d->d_fdesc4 = nullptr;
+  // k_coarse_packed descriptors (coarse_descriptors); a template whose descriptors do not fit goes to k_coarse_bytes
+  cudaFree(d->d_fdesc); d->d_fdesc = nullptr;
   cudaFree(d->d_k2info); d->d_k2info = nullptr;
   {
     const LevelHost& lv = d->lv[low_level];
     if (lv.d_bp && d->G > 0) {
-      std::vector<uint4> f4;
-      std::vector<int2> k2((size_t)d->G * d->M);
-      const uint32_t zoff = (uint32_t)((size_t)d->M * 8 * lv.lbw) * 4u;  // byte offset of the zero words
-      const int T = lv.T;
-      for (int g = 0; g < d->G; ++g)
-        for (int m = 0; m < d->M; ++m) {
-          const int32_t* tm = &d->tmeta[((size_t)g * d->S + low_level * d->M + m) * 4];
-          k2[(size_t)g * d->M + m].x = (int)f4.size();
-          for (int k = 0; k < tm[3]; ++k) {
-            const size_t i = (size_t)tm[2] + k;
-            const int x = d->feats[3 * i], y = d->feats[3 * i + 1], lab = d->feats[3 * i + 2];
-            if (x >= lv.cols || y >= lv.rows) {
-              f4.push_back(make_uint4(zoff, zoff, zoff, 0u));
-              continue;
-            }
-            const uint64_t inner = (uint64_t)((y % T) * T + (x % T)) * lv.plane + (uint64_t)(y / T) * lv.Wd + (x / T);
-            const uint64_t wh = (uint64_t)(m * 8 + lab) * lv.lbw + (inner >> 5);
-            const uint64_t wm = (uint64_t)(m * 8 + ((lab + 7) & 7)) * lv.lbw + (inner >> 5);
-            const uint64_t wp = (uint64_t)(m * 8 + ((lab + 1) & 7)) * lv.lbw + (inner >> 5);
-            f4.push_back(make_uint4((uint32_t)(wh * 4), (uint32_t)(wm * 4), (uint32_t)(wp * 4), (uint32_t)(inner & 31)));
-          }
-          while ((f4.size() - (size_t)k2[(size_t)g * d->M + m].x) % 8) f4.push_back(make_uint4(zoff, zoff, zoff, 0u));
-          k2[(size_t)g * d->M + m].y = (int)(f4.size() - (size_t)k2[(size_t)g * d->M + m].x);
-        }
-      CU(cudaMalloc(&d->d_fdesc4, std::max<size_t>(f4.size(), 1) * sizeof(uint4)));
+      std::vector<uint32_t> desc;
+      std::vector<int2> k2;
+      std::vector<uint8_t> fits;
+      coarse_descriptors(d->feats.data(), d->tmeta.data(), d->G, d->S, d->M, low_level * d->M, lv.T, lv.rows, lv.cols, desc,
+                         k2, fits);
+      for (int g = 0; g < d->G; ++g) d->bits_ok[g] &= fits[g];
+      CU(cudaMalloc(&d->d_fdesc, std::max<size_t>(desc.size(), 1) * sizeof(uint32_t)));
       CU(cudaMalloc(&d->d_k2info, k2.size() * sizeof(int2)));
-      if (!f4.empty()) CU(cudaMemcpyAsync(d->d_fdesc4, f4.data(), f4.size() * sizeof(uint4), cudaMemcpyHostToDevice, d->stream));
+      if (!desc.empty()) CU(cudaMemcpyAsync(d->d_fdesc, desc.data(), desc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
       CU(cudaMemcpyAsync(d->d_k2info, k2.data(), k2.size() * sizeof(int2), cudaMemcpyHostToDevice, d->stream));
       CU(cudaStreamSynchronize(d->stream));
     }
@@ -989,11 +1055,8 @@ static int size_levels(lm_detector* d, const int* rows, const int* cols, bool ne
       lv.nwords = (lv.plane + 31) / 32;
       lv.rounds = (lv.nwords + 31) / 32;
       if (l == d->L - 1 && lv.rounds <= LM_MAX_ROUNDS) {
-        // label block: T*T*plane bits, then slack for the reads of lanes beyond the last word
-        const size_t bits = (size_t)lv.T * lv.T * lv.plane;
-        lv.lbw = (int)(((bits + 31) / 32 + 32 * (size_t)lv.rounds + 4 + 3) & ~(size_t)3);
-        lv.bp_zero = (lv.nwords + 32 * lv.rounds + 8 + 3) & ~3;  // a lane reads words idx and idx + 1 of a window
-        const size_t words = (size_t)d->M * 8 * lv.lbw + lv.bp_zero;
+        lv.lbw = (int)bp_label_words(lv.T, lv.plane);
+        const size_t words = (size_t)d->M * 8 * lv.lbw;
         CU(cudaMalloc(&lv.d_bp, words * 4));
         CU(cudaMemsetAsync(lv.d_bp, 0, words * 4, d->stream));
       }
@@ -1303,10 +1366,10 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     bool scan_fused = false;
     if (d->n_items_bits > 0) {
       BitScanGateParams bp;
-      bp.bp = low.d_bp; bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw + low.bp_zero);  // planes + the zero words
+      bp.bp = low.d_bp; bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw);
       bp.lbw = low.lbw; bp.plane = low.plane; bp.nwords = low.nwords;
-      bp.tslot = d->d_tslot; bp.fdesc4 = d->d_fdesc4; bp.k2info = d->d_k2info; bp.work = d->d_work;
-      bp.zero_off = (uint32_t)((size_t)d->M * 8 * low.lbw) * 4u;
+      bp.tslot = d->d_tslot; bp.fdesc = d->d_fdesc; bp.k2info = d->d_k2info; bp.work = d->d_work;
+      bp.zero_desc = coarse_zero_descriptor(low.T, low.plane);
       bp.tasks = d->d_k2task; bp.n_full = d->k2_full; bp.n_rem = d->k2_rem; bp.n_tasks = d->k2_tasks;
       bp.S = d->S; bp.M = d->M; bp.slot_low = (d->L - 1) * d->M;
       bp.threshold = threshold;

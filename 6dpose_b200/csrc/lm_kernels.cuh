@@ -490,11 +490,10 @@ struct BitScanParams {
   uint32_t bp_words;    // M*8*lbw
   int lbw, plane, nwords;
   const TSlot* tslot;
-  const uint4* fdesc4;  // per feature: byte offsets (inside bp) of the window start of its label's plane (x) and of the two
-                        // neighbouring labels' planes (y, z), bit shift (w); skipped features and the padding to a multiple
-                        // of 8 per (template, modality) point at the zero words behind the planes
-  const int2* k2info;   // [G][M]: first descriptor, padded count
-  uint32_t zero_off;    // byte offset of the zero words
+  const uint32_t* fdesc;  // one word per lowest-level feature (host: coarse_descriptors): window word offset, wrap bits of the
+                          // neighbour labels, bit shift; a template's features end to end, padded to a multiple of 32
+  const int2* k2info;     // [G]: first descriptor (a multiple of 32), lowest-level features of all modalities
+  uint32_t zero_desc;     // the descriptor whose three windows read zeros (features outside the level, padding)
   const int32_t* work;  // template id per work item
   const int2* tasks;    // task table of the shard (host-built, see k_coarse_packed): n_full (work item, round) entries,
                         // then 32 (work item, word) entries per remainder task
@@ -598,11 +597,11 @@ __global__ void __launch_bounds__(1024) k_scan_counts(int32_t* __restrict__ cnt,
 // template_positions, LL.cpp:1309; 33 of the 38 words of the level for the bench bank).  Giving a warp a
 // whole template in rounds of 32 words leaves 31 of 32 lanes idle in the last round, so the words of a
 // template are split in two kinds of tasks:
-//   * FULL rounds (32 consecutive words of one template): the feature descriptors are warp-uniform, so the
-//     plane addressing lives in the uniform datapath -- 15 instructions per feature;
+//   * FULL rounds (32 consecutive words of one template): the feature descriptors are warp-uniform; the warp loads
+//     32 of them with one coalesced load a chunk ahead and hands each step's 8 out by shuffle;
 //   * the REMAINDERS (P/32 mod 32 words per template) of all templates of the shard, laid end to end and cut
-//     into tasks of 32 entries: lane k owns one (template, word) and walks its own template's descriptors
-//     (lanes of 2-3 templates share a warp; 26 instructions per feature, but 32 busy lanes).
+//     into tasks of 32 entries: lane k owns one (template, word) and walks its own template's descriptors, a step
+//     ahead (lanes of 2-3 templates share a warp; more instructions per feature, but 32 busy lanes).
 // The host lists every task of the shard once (full rounds first, p.tasks) and sizes the launch from that exact
 // count; CTA b takes tasks b, b + grid, b + 2 grid, ... of the list through a dynamic queue, so a shard with no more
 // tasks than warp slots runs in one round, and every CTA gets full rounds and the slower remainder tasks in the same
@@ -701,10 +700,26 @@ __device__ __forceinline__ void team_bar(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// One feature of a step for this lane's 32 positions: the H bits (xh) and the N bits ((lower | upper neighbour label) &
+// ~H, xn) from descriptor d (see coarse_descriptors on the host).  lane_base = this lane's word of a window at offset 0,
+// L4 = one label block in bytes.  The funnel shift takes its amount mod 32, i.e. d's low five bits.
+__device__ __forceinline__ void coarse_feature(const char* __restrict__ lane_base, uint32_t d, int L4, uint32_t& xh, uint32_t& xn) {
+  const char* __restrict__ w = lane_base + ((d >> 5) & ~3u);
+  const uint32_t* __restrict__ ph = reinterpret_cast<const uint32_t*>(w);
+  const uint32_t* __restrict__ pm = reinterpret_cast<const uint32_t*>(w + ((d & 0x20u) ? 7 * L4 : -L4));
+  const uint32_t* __restrict__ pp = reinterpret_cast<const uint32_t*>(w + ((d & 0x40u) ? -7 * L4 : L4));
+  const uint32_t h = __funnelshift_r(ph[0], ph[1], d);
+  const uint32_t a = __funnelshift_r(pm[0], pm[1], d);
+  const uint32_t b = __funnelshift_r(pp[0], pp[1], d);
+  xh = h;
+  xn = (a | b) & ~h;
+}
+
 // Feature split (p.split = S > 1, small shards): S warps form a team that owns a task together; warp q of the team adds
-// the 8-feature steps q, q + S, ... of every modality, the partial counters meet in shared memory and warp 0 of the team
-// emits.  A task is then a chain S times shorter -- the latency of the kernel follows the shard instead of staying one
-// whole task (what keeps a 1/8 shard from being 8 times faster, and what holds an SM's shared memory for the duration).
+// the 8-feature steps q, q + S, ... of the template (its modalities end to end), the partial counters meet in shared
+// memory and warp 0 of the team emits.  A task is then a chain S times shorter -- the latency of the kernel follows the
+// shard instead of staying one whole task (what keeps a 1/8 shard from being 8 times faster, and what holds an SM's
+// shared memory for the duration).
 template <bool kSmem, bool kGate>
 __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(typename BitScanArgs<kGate>::type p) {
   lm_pdl_wait();
@@ -758,6 +773,7 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(typename B
   }
   {
     const int S = p.split, q = warp & (S - 1), team = warp / S;
+    const int L4 = p.lbw * 4;
     uint32_t* s_part = s_bp + (kSmem ? ((p.bp_words + 3u) & ~3u) : 0u) + (size_t)team * (S - 1) * 16 * 32;
     int k = team;  // the CTA's k-th task
     while (k < n_mine) {
@@ -771,32 +787,33 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(typename B
         const int P = p.tslot[(size_t)g * p.S + p.slot_low].z;  // equal for all modalities (host checked)
         const int words = min(max((P + 31) >> 5, 1), p.nwords);
         const int idx = 32 * r + lane;
-        int nfeat = 0;
         uint32_t ch[8], cn[8];
 #pragma unroll
         for (int b = 0; b < 8; ++b) ch[b] = cn[b] = 0u;
         const char* __restrict__ lane_base = reinterpret_cast<const char*>(bp + idx);  // this lane's word of every window
-        for (int m = 0; m < p.M; ++m) {
-          nfeat += p.tslot[(size_t)g * p.S + p.slot_low + m].y;
-          const int2 k2 = p.k2info[(size_t)g * p.M + m];
-          const uint4* __restrict__ fd = p.fdesc4 + k2.x;
-          for (int f0 = q * 8; f0 < k2.y; f0 += 8 * S) {  // padded to a multiple of 8: no bounds check, no skip branch
+        const int2 k2 = p.k2info[g];
+        const int nfeat = k2.y;
+        const uint32_t* __restrict__ fd = p.fdesc + k2.x;
+        // lane L holds descriptor L of the current chunk of 32 (4 steps of 8), the next one of this warp's chunks is in
+        // flight meanwhile.  Warp q of a team takes steps q, q + S, ...: with S <= 4 steps q & 3, + S, ... of every chunk,
+        // with S = 8 step q & 3 of every other chunk.
+        const int nsteps = (nfeat + 7) >> 3, nchunks = (nfeat + 31) >> 5;
+        const int cstride = S > 4 ? 2 : 1, sstride = S > 4 ? 4 : S;
+        int c = q >> 2;
+        uint32_t cur = c < nchunks ? __ldg(fd + 32 * c + lane) : 0u;
+        for (; c < nchunks; c += cstride) {
+          const uint32_t nxt = c + cstride < nchunks ? __ldg(fd + 32 * (c + cstride) + lane) : 0u;
+          // lanes 0-7 of win hold the step's descriptors (constant source lanes: no index arithmetic per feature)
+          uint32_t win = __shfl_down_sync(0xffffffffu, cur, 8 * (q & 3));
+          for (int u = q & 3; u < 4 && 4 * c + u < nsteps; u += sstride) {
             uint32_t xh[8], xn[8];
 #pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              const uint4 d = __ldg(fd + f0 + u);  // warp-uniform
-              const uint32_t* __restrict__ ph = reinterpret_cast<const uint32_t*>(lane_base + d.x);
-              const uint32_t* __restrict__ pm = reinterpret_cast<const uint32_t*>(lane_base + d.y);
-              const uint32_t* __restrict__ pp = reinterpret_cast<const uint32_t*>(lane_base + d.z);
-              const uint32_t h = __funnelshift_r(ph[0], ph[1], d.w);
-              const uint32_t a = __funnelshift_r(pm[0], pm[1], d.w);
-              const uint32_t b = __funnelshift_r(pp[0], pp[1], d.w);
-              xh[u] = h;
-              xn[u] = (a | b) & ~h;
-            }
+            for (int k = 0; k < 8; ++k) coarse_feature(lane_base, __shfl_sync(0xffffffffu, win, k), L4, xh[k], xn[k]);
+            win = __shfl_down_sync(0xffffffffu, win, 8 * sstride);
             vc_add8(ch, xh);
             vc_add8(cn, xn);
           }
+          cur = nxt;
         }
         if (S > 1) {  // the team's partial counters meet
           if (q > 0) {
@@ -832,34 +849,36 @@ __global__ void __launch_bounds__(LM_PACK_THREADS, 1) k_coarse_packed(typename B
         const int P = p.tslot[(size_t)g * p.S + p.slot_low].z;
         const int words = min(max((P + 31) >> 5, 1), p.nwords);
         const int idx = tk.y;
-        int nfeat = 0;
         uint32_t ch[8], cn[8];
 #pragma unroll
         for (int b = 0; b < 8; ++b) ch[b] = cn[b] = 0u;
         const char* __restrict__ lane_base = reinterpret_cast<const char*>(bp + idx);
-        const uint4 zdesc = make_uint4(p.zero_off, p.zero_off, p.zero_off, 0u);
-        for (int m = 0; m < p.M; ++m) {
-          nfeat += p.tslot[(size_t)g * p.S + p.slot_low + m].y;
-          const int2 k2 = p.k2info[(size_t)g * p.M + m];
-          const uint4* __restrict__ fd = p.fdesc4 + k2.x;
-          const int maxn = __reduce_max_sync(0xffffffffu, k2.y);
-          for (int f0 = q * 8; f0 < maxn; f0 += 8 * S) {
-            uint32_t xh[8], xn[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              const uint4 d = (f0 < k2.y) ? __ldg(fd + f0 + u) : zdesc;  // lanes of a shorter template read zeros
-              const uint32_t* __restrict__ ph = reinterpret_cast<const uint32_t*>(lane_base + d.x);
-              const uint32_t* __restrict__ pm = reinterpret_cast<const uint32_t*>(lane_base + d.y);
-              const uint32_t* __restrict__ pp = reinterpret_cast<const uint32_t*>(lane_base + d.z);
-              const uint32_t h = __funnelshift_r(ph[0], ph[1], d.w);
-              const uint32_t a = __funnelshift_r(pm[0], pm[1], d.w);
-              const uint32_t b = __funnelshift_r(pp[0], pp[1], d.w);
-              xh[u] = h;
-              xn[u] = (a | b) & ~h;
-            }
-            vc_add8(ch, xh);
-            vc_add8(cn, xn);
-          }
+        const int2 k2 = p.k2info[g];
+        const int nfeat = k2.y;
+        // the lane's own template: 8 descriptors (two 16-byte loads, the run starts at a multiple of 32) per step, the
+        // lane's next step in flight meanwhile; lanes of a shorter template take the zero descriptor
+        const uint4* __restrict__ fd = reinterpret_cast<const uint4*>(p.fdesc + k2.x);
+        const int nsteps = (nfeat + 7) >> 3;
+        const int maxs = __reduce_max_sync(0xffffffffu, nsteps);
+        const uint4 z4 = make_uint4(p.zero_desc, p.zero_desc, p.zero_desc, p.zero_desc);
+        int s = q;
+        uint4 d0 = s < nsteps ? __ldg(fd + 2 * s) : z4, d1 = s < nsteps ? __ldg(fd + 2 * s + 1) : z4;
+        for (; s < maxs; s += S) {
+          const bool more = s + S < nsteps;
+          const uint4 e0 = more ? __ldg(fd + 2 * (s + S)) : z4, e1 = more ? __ldg(fd + 2 * (s + S) + 1) : z4;
+          uint32_t xh[8], xn[8];
+          coarse_feature(lane_base, d0.x, L4, xh[0], xn[0]);
+          coarse_feature(lane_base, d0.y, L4, xh[1], xn[1]);
+          coarse_feature(lane_base, d0.z, L4, xh[2], xn[2]);
+          coarse_feature(lane_base, d0.w, L4, xh[3], xn[3]);
+          coarse_feature(lane_base, d1.x, L4, xh[4], xn[4]);
+          coarse_feature(lane_base, d1.y, L4, xh[5], xn[5]);
+          coarse_feature(lane_base, d1.z, L4, xh[6], xn[6]);
+          coarse_feature(lane_base, d1.w, L4, xh[7], xn[7]);
+          vc_add8(ch, xh);
+          vc_add8(cn, xn);
+          d0 = e0;
+          d1 = e1;
         }
         if (S > 1) {  // the team's partial counters meet
           if (q > 0) {

@@ -131,9 +131,21 @@ int lm_prepare(lm_detector* d);
  *                        items end to end, 32 per task, the last task padded with copies of the last word.  table ==
  *                        null: only the counts and shape; cap < n_entries: LM_E_CAPACITY (counts still written)
  *   shape[4]             tasks, warps per team, warps per CTA, CTAs of the launch on sm_count SMs with plane_bytes of
- *                        bit-planes (zero words included); CTA b takes tasks b, b + CTAs, b + 2 CTAs, ... */
+ *                        bit-planes; CTA b takes tasks b, b + CTAs, b + 2 CTAs, ... */
 int lm_coarse_tasks(const int32_t* words, int64_t n_items, int sm_count, int64_t plane_bytes, int32_t* table, int64_t cap,
                     int64_t* n_entries, int64_t* n_full, int64_t* n_rem, int32_t* shape);
+/* The bit-sliced coarse scan's feature descriptors, as lm_prepare builds them (host only, no device needed), for a bank
+ * in lm_load_bank's layout (feats[n][3] = x, y, label; tmeta[G][S][4] = width, height, first feature, count) at the
+ * lowest level: slots slot_low .. slot_low + M - 1, sampling step T, level size rows x cols.  One word per feature:
+ *   bits 0-4 bit shift inside the window's first word, bit 5 label 0, bit 6 label 7, bits 7-31 word offset of the
+ *   window in the bit-plane buffer ((m * 8 + label) * lbw + word inside the label block, lbw = words per label block).
+ * Features outside the level and padding hold *zero (a window that reads zeros).  A template's features, modalities in
+ * order, lie end to end from info[g][0] (info[g][1] of them), padded to a multiple of 32.  fits[g] = 0: the word offsets
+ * do not fit in 25 bits; the template has no descriptors and goes to the byte-wise coarse scan.  desc == null: only
+ * n_desc, info, fits and zero; cap < n_desc: LM_E_CAPACITY. */
+int lm_coarse_descriptors(const int32_t* feats, const int32_t* tmeta, int G, int S, int M, int slot_low, int T, int rows,
+                          int cols, uint32_t* desc, int64_t cap, int64_t* n_desc, int32_t* info, uint8_t* fits,
+                          uint32_t* zero);
 
 /* Result block of the stages: by default an internal device buffer that grows on demand.  A caller
  * that wants the block in its own device memory (e.g. the send buffer of an NCCL all-gather) sets it
