@@ -4,7 +4,9 @@ Fails loudly when the library is missing or cannot be loaded: there is no CPU / 
 for the hot path.
 """
 import ctypes
+import math
 import os
+import sys
 
 import numpy as np
 
@@ -24,7 +26,8 @@ PEER_HANDLE_BYTES = 64
 
 SYMBOLS = [
     "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks", "lm_coarse_descriptors",
-    "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
+    "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device",
+    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
@@ -56,6 +59,142 @@ def depth_gate_tolerance(tolerance):
     if not (0.0 <= t < 1.0):
         raise ValueError("depth gate tolerance must lie in [0, 1), got %r" % tolerance)
     return t
+
+
+# Depth formats of lm_bind_images_device (include/linemod_b200.h)
+DEPTH_U16_MM, DEPTH_F32 = 0, 1
+
+
+def is_tensor(a):
+    """True for a torch.Tensor.  torch is not imported for this: a caller holding a tensor has imported it already."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(a, torch.Tensor)
+
+
+def depth_scale_value(depth_scale):
+    """depth_scale as a float, finite and > 0; TypeError / ValueError otherwise (no device work)."""
+    if isinstance(depth_scale, (bool, np.bool_)) or not isinstance(depth_scale, (int, float, np.integer, np.floating)):
+        raise TypeError("depth_scale must be a number, got %s" % type(depth_scale).__name__)
+    s = float(depth_scale)
+    if not (math.isfinite(s) and s > 0.0):
+        raise ValueError("depth_scale must be finite and > 0, got %r" % depth_scale)
+    return s
+
+
+class DeviceFrame:
+    """An RGB-D frame already on the GPU, checked for lm_bind_images_device without any library call: rgb uint8 [H, W, 3]
+    with stride(2) == 1 and stride(1) == 3, depth torch.uint16 (mm) or torch.float32 (scaled by depth_scale, converted
+    to u16 mm on the device) [H, W] with stride(1) == 1, masks [] or [mask_color, mask_depth], each None, empty or uint8
+    [H, W] with stride(1) == 1 and one row pitch; every tensor CUDA on `device`.  Row pitches are free (crop views).
+    The frame is read in order on `stream` (device_stream)."""
+
+    def __init__(self, rgb, depth, masks, depth_scale, stream, device):
+        import torch
+        if not (is_tensor(rgb) and is_tensor(depth)):
+            raise TypeError("sources mix numpy arrays and torch tensors: pass both as CUDA tensors or both as numpy arrays")
+        if rgb.dtype != torch.uint8 or rgb.dim() != 3 or rgb.shape[2] != 3:
+            raise TypeError("sources[0] must be a uint8 HxWx3 colour tensor, got %s %s" % (rgb.dtype, tuple(rgb.shape)))
+        if rgb.stride(2) != 1 or rgb.stride(1) != 3:
+            raise ValueError("sources[0]: pixels must be packed within a row (strides (*, 3, 1)), got %s" % (rgb.stride(),))
+        if depth.dtype not in (torch.uint16, torch.float32) or depth.dim() != 2:
+            raise TypeError("sources[1] must be a uint16 (mm) or float32 HxW depth tensor, got %s %s" % (depth.dtype, tuple(depth.shape)))
+        if tuple(depth.shape) != tuple(rgb.shape[:2]):
+            raise ValueError("sources[1] is %s, the colour image %s" % (tuple(depth.shape), tuple(rgb.shape[:2])))
+        if depth.stride(1) != 1:
+            raise ValueError("sources[1]: depth must be packed within a row (stride(1) == 1), got %s" % (depth.stride(),))
+        f32 = depth.dtype == torch.float32
+        scale = depth_scale_value(depth_scale)
+        if not f32 and scale != 1.0:
+            raise ValueError("depth_scale applies to float32 depth; uint16 depth is in mm (depth_scale=%r)" % depth_scale)
+        rows, cols = int(rgb.shape[0]), int(rgb.shape[1])
+        mk = [None, None]
+        if masks:
+            if len(masks) != 2:
+                raise RuntimeError("masks.size() == modalities.size()")
+            for i, m in enumerate(masks):
+                if m is None:
+                    continue
+                if not is_tensor(m):
+                    if np.asarray(m).size:
+                        raise TypeError("masks[%d] is not a tensor: masks of a device frame are CUDA tensors too" % i)
+                    continue
+                if m.numel() == 0:
+                    continue
+                if m.dtype != torch.uint8 or tuple(m.shape) != (rows, cols):
+                    raise RuntimeError("mask.size() == source.size()")
+                if m.stride(1) != 1:
+                    raise ValueError("masks[%d] must be packed within a row (stride(1) == 1), got %s" % (i, m.stride()))
+                mk[i] = m
+            if mk[0] is not None and mk[1] is not None and mk[0].stride(0) != mk[1].stride(0):
+                raise ValueError("the two masks must share one row pitch, got %d and %d" % (mk[0].stride(0), mk[1].stride(0)))
+        for name, t in (("sources[0]", rgb), ("sources[1]", depth), ("masks[0]", mk[0]), ("masks[1]", mk[1])):
+            if t is not None and (not t.is_cuda or t.device.index != int(device)):
+                raise ValueError("%s is on %s; the detector runs on cuda:%d" % (name, t.device, int(device)))
+        mask_pitch = next((m.stride(0) for m in mk if m is not None), cols)
+        self.rows, self.cols = rows, cols
+        self.tensors = [t for t in (rgb, depth, mk[0], mk[1]) if t is not None]
+        self.pitches = (rgb.stride(0), depth.stride(0) * depth.element_size(), mask_pitch)
+        self.rgb, self.depth, self.masks = rgb.data_ptr(), depth.data_ptr(), [m.data_ptr() if m is not None else None for m in mk]
+        self.format = DEPTH_F32 if f32 else DEPTH_U16_MM
+        self.scale = scale
+        self.stream = device_stream(stream, device)
+
+
+class DeviceBatch:
+    """DeviceFrames for lm_detect_batch_device: one size, row pitches, depth dtype, depth_scale and stream, and one row
+    pitch for every mask of the batch.  ValueError otherwise, before any library call."""
+
+    def __init__(self, frames):
+        frames = list(frames)
+        if not frames:
+            raise ValueError("no frames")
+        f0 = frames[0]
+        key = lambda f: (f.rows, f.cols, f.pitches[:2], f.format, f.scale, f.stream)
+        if any(key(f) != key(f0) for f in frames):
+            raise ValueError("every frame's tensors must have one size, row pitch, depth dtype and depth_scale")
+        masked = [f for f in frames if any(m is not None for m in f.masks)]
+        if len({f.pitches[2] for f in masked}) > 1:
+            raise ValueError("the masks of a batch must share one row pitch")
+        vp = ctypes.c_void_p
+        self.n, self.stream = len(frames), f0.stream
+        self.tensors = [t for f in frames for t in f.tensors]
+        masks = (vp * (2 * self.n))(*[m for f in frames for m in f.masks]) if masked else None
+        self.args = (self.n, (vp * self.n)(*[f.rgb for f in frames]), f0.pitches[0], (vp * self.n)(*[f.depth for f in frames]),
+                     f0.pitches[1], f0.format, ctypes.c_float(f0.scale), f0.rows, f0.cols, masks,
+                     masked[0].pitches[2] if masked else f0.cols, f0.stream.cuda_stream)
+
+
+def frame_inputs(rgb, depth, masks, depth_scale, stream, device):
+    """A DeviceFrame for a pair of CUDA tensors (rgb itself when it is one already), None for numpy arrays (the host path,
+    where depth_scale must stay 1.0 and stream None).  TypeError / ValueError before any library call."""
+    if isinstance(rgb, DeviceFrame):
+        return rgb
+    if not (is_tensor(rgb) or is_tensor(depth)):
+        host_frame_options(depth_scale, stream)
+        if masks and any(is_tensor(m) for m in masks if m is not None):
+            raise TypeError("masks are tensors, the frame is numpy arrays")
+        return None
+    return DeviceFrame(rgb, depth, masks, depth_scale, stream, device)
+
+
+def host_frame_options(depth_scale, stream):
+    """A frame of numpy arrays takes neither option: its depth is uint16 mm and it is copied before the call returns."""
+    if stream is not None:
+        raise TypeError("stream applies to frames given as CUDA tensors")
+    if depth_scale_value(depth_scale) != 1.0:
+        raise ValueError("depth_scale applies to float32 depth tensors; numpy depth is uint16 mm")
+
+
+def device_stream(stream, device):
+    """The torch stream a device frame is ordered on: torch.cuda.current_stream(device) for None."""
+    import torch
+    if stream is None:
+        return torch.cuda.current_stream(int(device))
+    if not isinstance(stream, torch.cuda.Stream):
+        raise TypeError("stream must be a torch.cuda.Stream or None, got %s" % type(stream).__name__)
+    if stream.device.index != int(device):
+        raise ValueError("stream is on %s; the detector runs on cuda:%d" % (stream.device, int(device)))
+    return stream
 
 
 _lib = None
@@ -142,6 +281,10 @@ def load():
                                   c_int, c_int, ctypes.c_double, vp, f64p, f64p, f32p, c_i64, ctypes.POINTER(c_i64),
                                   ctypes.POINTER(c_i64)]
     L.lm_peer_detect_batch.argtypes = L.lm_detect_batch.argtypes
+    L.lm_bind_images_device.argtypes = [vp, vp, c_i64, vp, c_i64, c_int, c_f, c_int, c_int, vp, vp, c_i64, vp]
+    L.lm_detect_batch_device.argtypes = [vp, c_int, ctypes.POINTER(vp), c_i64, ctypes.POINTER(vp), c_i64, c_int, c_f, c_int, c_int,
+                                         ctypes.POINTER(vp), c_i64, vp] + L.lm_detect_batch.argtypes[7:]
+    L.lm_debug_depth.argtypes = [vp, u16p, c_i64]
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -225,6 +368,7 @@ class NativeDetector:
         check(L.lm_create(int(device), self.levels, arr, ctypes.byref(h)))
         self._h = h
         self._keep = None
+        self.device = int(device)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -314,7 +458,35 @@ class NativeDetector:
         keep = self._image_args(rgb, depth, masks)
         check(self._L.lm_upload_images(self._h, *keep[3]))
 
-    def match_images(self, rgb, depth, masks, threshold):
+    def bind_frame(self, frame):
+        """lm_bind_images_device of a DeviceFrame, ordered on its stream."""
+        for t in frame.tensors:
+            # the caching allocator reuses the frame only after the stream's work, which waits for the ingest
+            t.record_stream(frame.stream)
+        check(self._L.lm_bind_images_device(self._h, frame.rgb, frame.pitches[0], frame.depth, frame.pitches[1], frame.format,
+                                            ctypes.c_float(frame.scale), frame.rows, frame.cols, frame.masks[0], frame.masks[1],
+                                            frame.pitches[2], frame.stream.cuda_stream))
+
+    def set_frame(self, rgb, depth, masks=None, depth_scale=1.0, stream=None):
+        """upload_images for numpy arrays; bind_frame for CUDA tensors, or for a DeviceFrame passed as rgb."""
+        frame = frame_inputs(rgb, depth, masks, depth_scale, stream, self.device)
+        if frame is None:
+            self.upload_images(rgb, depth, masks)
+        else:
+            self.bind_frame(frame)
+
+    def depth_image(self, shape):
+        """The u16 mm depth of the frame last uploaded or bound (lm_debug_depth)."""
+        out = np.zeros(shape, np.uint16)
+        check(self._L.lm_debug_depth(self._h, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), out.size))
+        return out
+
+    def match_images(self, rgb, depth, masks, threshold, depth_scale=1.0, stream=None):
+        frame = frame_inputs(rgb, depth, masks, depth_scale, stream, self.device)
+        if frame is not None:  # lm_match_images of a bound device frame
+            self.bind_frame(frame)
+            self.run(threshold)
+            return self.finish(self.fetch_records())
         keep = self._image_args(rgb, depth, masks)
         cap = 1 << 12
         while True:
@@ -525,10 +697,10 @@ class NativeDetector:
         return out[:k].copy(), Ro[:k].copy(), to[:k].copy(), res[:k].copy(), int(nrec.value)
 
     def match_pose(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30, use_scene_cloud=False,
-                   estimation="point_to_plane"):
-        """upload_images + enqueue + enqueue_post + enqueue_pose + complete_pose: one chain on the detector's stream."""
+                   estimation="point_to_plane", depth_scale=1.0, stream=None):
+        """set_frame + enqueue + enqueue_post + enqueue_pose + complete_pose: one chain on the detector's stream."""
         estimation_code(estimation)
-        self.upload_images(rgb, depth, masks)
+        self.set_frame(rgb, depth, masks, depth_scale, stream)
         self.enqueue(threshold)
         self.enqueue_post(iou_threshold, top_k)
         self.enqueue_pose(sceneK, max_iterations, use_scene_cloud, estimation)
@@ -556,11 +728,11 @@ class NativeDetector:
                 dict(survivors=int(ns.value), posed=int(npo.value), records=int(nrec.value)))
 
     def detect(self, rgb, depth, masks, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30, use_scene_cloud=False,
-               translation_threshold=40.0, estimation="point_to_plane"):
-        """upload_images + enqueue + enqueue_post + enqueue_pose + enqueue_pose_nms + complete_detect: RGB-D frame to the
-        object list in one chain on the detector's stream."""
+               translation_threshold=40.0, estimation="point_to_plane", depth_scale=1.0, stream=None):
+        """set_frame + enqueue + enqueue_post + enqueue_pose + enqueue_pose_nms + complete_detect: RGB-D frame (numpy, or
+        CUDA tensors) to the object list in one chain on the detector's stream."""
         estimation_code(estimation)
-        self.upload_images(rgb, depth, masks)
+        self.set_frame(rgb, depth, masks, depth_scale, stream)
         self.enqueue(threshold)
         self.enqueue_post(iou_threshold, top_k)
         self.enqueue_pose(sceneK, max_iterations, use_scene_cloud, estimation)
@@ -620,6 +792,24 @@ class NativeDetector:
                             raise RuntimeError("mask.size() == source.size()")
                         keep.append(a)
                         mptr[2 * f + m] = a.ctypes.data_as(u8p)
+        return self._batch_run(fn, (n, rgb.ctypes.data_as(u8p), depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows, cols, mptr),
+                               n, threshold, sK, iou_threshold, top_k, max_iterations, use_scene_cloud, pose_nms, translation_threshold,
+                               cap, est)
+
+    def detect_batch_device(self, batch, threshold, sceneK, iou_threshold=0.5, top_k=0, max_iterations=30, use_scene_cloud=False,
+                            pose_nms=True, translation_threshold=40.0, cap=None, estimation="point_to_plane"):
+        """detect_batch of a DeviceBatch (lm_detect_batch_device), ordered on its stream.  Returns what detect_batch returns."""
+        est = estimation_code(estimation)
+        sK = np.ascontiguousarray(sceneK, np.float32)
+        if sK.shape != (batch.n, 3, 3):
+            raise ValueError("sceneK must be [%d,3,3], got %s" % (batch.n, sK.shape))
+        for t in batch.tensors:
+            t.record_stream(batch.stream)
+        return self._batch_run(self._L.lm_detect_batch_device, batch.args, batch.n, threshold, sK, iou_threshold, top_k,
+                               max_iterations, use_scene_cloud, pose_nms, translation_threshold, cap, est)
+
+    def _batch_run(self, fn, frame_args, n, threshold, sK, iou_threshold, top_k, max_iterations, use_scene_cloud, pose_nms,
+                   translation_threshold, cap, est):
         bound = top_k if top_k > 0 else 1024
         cap = n * bound if cap is None else max(int(cap), 1)
         counts = np.zeros((n, 4), np.int64)
@@ -631,8 +821,7 @@ class NativeDetector:
             to = np.full((cap, 3), np.nan, np.float64)
             res = np.zeros(cap, np.float32)
             total = ctypes.c_int64()
-            rc = fn(self._h, n, rgb.ctypes.data_as(u8p), depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows, cols, mptr,
-                    ctypes.c_float(threshold), sK.ctypes.data_as(f32p), float(iou_threshold), int(top_k), int(max_iterations),
+            rc = fn(self._h, *frame_args, ctypes.c_float(threshold), sK.ctypes.data_as(f32p), float(iou_threshold), int(top_k), int(max_iterations),
                     1 if use_scene_cloud else 0, 1 if pose_nms else 0, float(translation_threshold), out.ctypes.data_as(ctypes.c_void_p),
                     Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p), res.ctypes.data_as(f32p), cap, ctypes.byref(total),
                     counts.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)))

@@ -19,6 +19,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -224,6 +225,8 @@ struct lm_detector {
   } fe[LM_MAX_LEVELS];
   uint16_t* fe_depth = nullptr; uint8_t* fe_nraw = nullptr;
   bool fe_lut = false;
+  // lm_bind_images_device: the caller's stream up to the call -> the ingest -> the caller's stream after it
+  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 
   // depth gate of the coarse scan (lm_set_depth_gate)
   std::vector<float> tdepth;            // training distance per template of the bank (mm; NaN / <= 0: never gated)
@@ -348,6 +351,8 @@ extern "C" void lm_destroy(lm_detector* d) {
   if (d->copy_stream) { cudaStreamSynchronize(d->copy_stream); cudaStreamDestroy(d->copy_stream); }
   if (d->ev_fork) cudaEventDestroy(d->ev_fork);
   if (d->ev_upper) cudaEventDestroy(d->ev_upper);
+  if (d->ev_in) cudaEventDestroy(d->ev_in);
+  if (d->ev_out) cudaEventDestroy(d->ev_out);
   if (d->stream) cudaStreamDestroy(d->stream);
   delete d;
 }
@@ -1137,19 +1142,18 @@ extern "C" int lm_bind_quantized_device(lm_detector* d, const uint8_t* const* d_
 }
 
 // ---- GPU quantization front-end: Detector::match's modality processing (LL.cpp:1709-1741) -------------
-extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
-                                const uint8_t* mask_color, const uint8_t* mask_depth) {
-  if (!d || !rgb || !depth) return fail(LM_E_INVALID, "null argument");
-  if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
-  CU(cudaSetDevice(d->device));
-  int lrows[LM_MAX_LEVELS], lcols[LM_MAX_LEVELS];
+// Pyramid sizes of a rows x cols frame, checked against the frame-size rules of every level.
+static int fe_dims(lm_detector* d, int rows, int cols, int* lrows, int* lcols) {
   for (int l = 0; l < d->L; ++l) {
     lrows[l] = l ? lrows[l - 1] / 2 : rows;  // Size(src.cols / 2, src.rows / 2), LL.cpp:564, 866
     lcols[l] = l ? lcols[l - 1] / 2 : cols;
   }
-  int rc = check_frame_dims(d, lrows, lcols);
-  if (rc) return rc;
-  rc = size_levels(d, lrows, lcols, true);
+  return check_frame_dims(d, lrows, lcols);
+}
+
+// The front-end's buffers for the frame size, and the label buffers of every level; joins an unconsumed upload.
+static int fe_levels(lm_detector* d, const int* lrows, const int* lcols) {
+  int rc = size_levels(d, lrows, lcols, true);
   if (rc) return rc;
   cudaStream_t st = d->stream;
   if (d->upper_pending) CU(cudaStreamWaitEvent(st, d->ev_upper, 0));  // an earlier upload nobody consumed
@@ -1182,12 +1186,12 @@ extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16
       }
     }
   }
-  const size_t n0 = (size_t)rows * cols;
-  CU(cudaMemcpyAsync(d->fe[0].src, rgb, n0 * 3, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d->fe_depth, depth, n0 * 2, cudaMemcpyHostToDevice, st));
-  const uint8_t* masks[2] = {mask_color, mask_depth};
-  for (int m = 0; m < 2; ++m)
-    if (masks[m]) CU(cudaMemcpyAsync(d->fe[0].mask[m], masks[m], n0, cudaMemcpyHostToDevice, st));
+  return LM_OK;
+}
+
+// Label images of every level from the level-0 frame in fe[0].src / fe_depth / fe[0].mask[m] (masks[m]: given).
+static int fe_quantize(lm_detector* d, const bool* masks) {
+  cudaStream_t st = d->stream;
   auto grid2 = [](int w, int h) { return dim3((unsigned)((w + 31) / 32), (unsigned)((h + 7) / 8)); };
   for (int l = 0; l < d->L; ++l) {
     lm_detector::FeLevel& f = d->fe[l];
@@ -1221,12 +1225,139 @@ extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16
     lv.q_src[0] = lv.d_q[0];
     lv.q_src[1] = lv.d_q[1];
   }
-  CU(cudaStreamSynchronize(st));  // the caller's images are only borrowed for the call
-  CU(cudaGetLastError());
+  return LM_OK;
+}
+
+// The frame state after lm_upload_images / lm_bind_images_device: a frame with depth, not yet matched.
+static void fe_bound(lm_detector* d) {
   d->upper_pending = false;
   d->have_frame = true;
   d->frame_depth = true;
   d->have_run = false;
+}
+
+extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
+                                const uint8_t* mask_color, const uint8_t* mask_depth) {
+  if (!d || !rgb || !depth) return fail(LM_E_INVALID, "null argument");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  CU(cudaSetDevice(d->device));
+  int lrows[LM_MAX_LEVELS], lcols[LM_MAX_LEVELS];
+  int rc = fe_dims(d, rows, cols, lrows, lcols);
+  if (rc) return rc;
+  rc = fe_levels(d, lrows, lcols);
+  if (rc) return rc;
+  cudaStream_t st = d->stream;
+  const size_t n0 = (size_t)rows * cols;
+  CU(cudaMemcpyAsync(d->fe[0].src, rgb, n0 * 3, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d->fe_depth, depth, n0 * 2, cudaMemcpyHostToDevice, st));
+  const uint8_t* masks[2] = {mask_color, mask_depth};
+  for (int m = 0; m < 2; ++m)
+    if (masks[m]) CU(cudaMemcpyAsync(d->fe[0].mask[m], masks[m], n0, cudaMemcpyHostToDevice, st));
+  const bool given[2] = {masks[0] != nullptr, masks[1] != nullptr};
+  rc = fe_quantize(d, given);
+  if (rc) return rc;
+  CU(cudaStreamSynchronize(st));  // the caller's images are only borrowed for the call
+  CU(cudaGetLastError());
+  fe_bound(d);
+  return LM_OK;
+}
+
+// ---- frames already in device memory (lm_bind_images_device, lm_detect_batch_device) ------------------
+struct DeviceFrame {
+  const uint8_t* rgb; int64_t rgb_pitch;
+  const void* depth; int64_t depth_pitch; int format; float scale;
+  const uint8_t* mask[2]; int64_t mask_pitch;
+};
+
+// One plane of a device frame: present, on the handle's device, rows at least `row` bytes apart, element-aligned.
+static int check_device_plane(const lm_detector* d, const char* what, const void* p, int64_t pitch, int64_t row, int elem) {
+  if (!p) return fail(LM_E_INVALID, "%s is null", what);
+  if (pitch < row) return fail(LM_E_INVALID, "%s: row pitch %lld bytes is shorter than a row (%lld bytes)", what, (long long)pitch, (long long)row);
+  if ((uintptr_t)p % elem || pitch % elem)
+    return fail(LM_E_INVALID, "%s: pointer %p / pitch %lld not aligned to its %d-byte elements", what, p, (long long)pitch, elem);
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();  // clear the query's error: nothing was enqueued
+    return fail(LM_E_INVALID, "%s: %p is not a CUDA pointer", what, p);
+  }
+  if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != d->device)
+    return fail(LM_E_INVALID, "%s: %p is not device or managed memory of device %d (%s, device %d)", what, p, d->device,
+                a.type == cudaMemoryTypeHost ? "host memory" : a.type == cudaMemoryTypeUnregistered ? "unregistered host memory" : "device memory",
+                a.device);
+  return LM_OK;
+}
+
+// Every check of lm_bind_images_device, none of which touches the device.
+static int check_device_frame(lm_detector* d, const DeviceFrame& f, int rows, int cols, cudaStream_t stream, int* lrows, int* lcols) {
+  int sdev = -1;
+  if (cudaStreamGetDevice(stream, &sdev) != cudaSuccess) {
+    cudaGetLastError();  // clear the query's error: nothing was enqueued
+    return fail(LM_E_INVALID, "stream %p is not a CUDA stream", (void*)stream);
+  }
+  if (sdev != d->device) return fail(LM_E_INVALID, "stream %p belongs to device %d, the handle to device %d", (void*)stream, sdev, d->device);
+  if (f.format != LM_DEPTH_U16_MM && f.format != LM_DEPTH_F32)
+    return fail(LM_E_INVALID, "unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", f.format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
+  if (f.format == LM_DEPTH_F32 && !(std::isfinite(f.scale) && f.scale > 0.f))
+    return fail(LM_E_INVALID, "depth_scale %g: float depth needs a finite scale > 0", (double)f.scale);
+  int rc = fe_dims(d, rows, cols, lrows, lcols);
+  if (rc) return rc;
+  const int esize = f.format == LM_DEPTH_F32 ? 4 : 2;
+  rc = check_device_plane(d, "rgb", f.rgb, f.rgb_pitch, 3ll * cols, 1);
+  if (!rc) rc = check_device_plane(d, "depth", f.depth, f.depth_pitch, (int64_t)esize * cols, esize);
+  for (int m = 0; m < 2 && !rc; ++m)
+    if (f.mask[m]) rc = check_device_plane(d, m ? "mask_depth" : "mask_color", f.mask[m], f.mask_pitch, cols, 1);
+  return rc;
+}
+
+// The ingest of a checked device frame and the front-end behind it, ordered after the caller's stream and before its
+// next work; no host synchronise (beyond lm_upload_images' first-use ones: buffers of a new size, the normal table).
+static int bind_images_device(lm_detector* d, const DeviceFrame& f, int rows, int cols, const int* lrows, const int* lcols,
+                              cudaStream_t caller) {
+  int rc = fe_levels(d, lrows, lcols);
+  if (rc) return rc;
+  if (!d->ev_in) CU(cudaEventCreateWithFlags(&d->ev_in, cudaEventDisableTiming));
+  if (!d->ev_out) CU(cudaEventCreateWithFlags(&d->ev_out, cudaEventDisableTiming));
+  cudaStream_t st = d->stream;
+  CU(cudaEventRecord(d->ev_in, caller));
+  CU(cudaStreamWaitEvent(st, d->ev_in, 0));
+  // a plain launch: it starts once the caller's work and everything before it on the stream have completed
+  const dim3 grid((unsigned)((cols + FE_INGEST_PX - 1) / FE_INGEST_PX), (unsigned)rows);
+  lm_detector::FeLevel& f0 = d->fe[0];
+  k_fe_ingest<<<grid, FE_INGEST_PX, 0, st>>>(f.rgb, f.rgb_pitch, f.depth, f.depth_pitch, f.format == LM_DEPTH_F32 ? 1 : 0, f.scale,
+                                             f.mask[0], f.mask[1], f.mask_pitch, cols, f0.src, d->fe_depth, f0.mask[0], f0.mask[1]);
+  CU(cudaGetLastError());
+  d->launches += 1;
+  CU(cudaEventRecord(d->ev_out, st));
+  CU(cudaStreamWaitEvent(caller, d->ev_out, 0));  // the borrow ends with the ingest
+  const bool given[2] = {f.mask[0] != nullptr, f.mask[1] != nullptr};
+  rc = fe_quantize(d, given);
+  if (rc) return rc;
+  fe_bound(d);
+  return LM_OK;
+}
+
+extern "C" int lm_bind_images_device(lm_detector* d, const uint8_t* rgb, int64_t rgb_pitch, const void* depth, int64_t depth_pitch,
+                                     int depth_format, float depth_scale, int rows, int cols, const uint8_t* mask_color,
+                                     const uint8_t* mask_depth, int64_t mask_pitch, void* stream) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  CU(cudaSetDevice(d->device));
+  const DeviceFrame f = {rgb, rgb_pitch, depth, depth_pitch, depth_format, depth_scale, {mask_color, mask_depth}, mask_pitch};
+  int lrows[LM_MAX_LEVELS], lcols[LM_MAX_LEVELS];
+  int rc = check_device_frame(d, f, rows, cols, (cudaStream_t)stream, lrows, lcols);
+  if (rc) return rc;
+  return bind_images_device(d, f, rows, cols, lrows, lcols, (cudaStream_t)stream);
+}
+
+extern "C" int lm_debug_depth(lm_detector* d, uint16_t* out, int64_t cap) {
+  if (!d || !out) return fail(LM_E_INVALID, "null argument");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
+  if (!d->have_frame || !d->frame_depth) return fail(LM_E_STATE, "no frame with depth uploaded or bound");
+  const int64_t n = (int64_t)d->fe[0].rows * d->fe[0].cols;
+  if (n > cap) return fail(LM_E_CAPACITY, "need %lld elements", (long long)n);
+  CU(cudaSetDevice(d->device));
+  CU(cudaMemcpyAsync(out, d->fe_depth, (size_t)n * 2, cudaMemcpyDeviceToHost, d->stream));
+  CU(cudaStreamSynchronize(d->stream));
   return LM_OK;
 }
 
@@ -2365,12 +2496,25 @@ extern "C" int lm_pose_stats(lm_detector* d, int64_t* out4) {
 // lm_detect_batch (peers false: refuses a connected exchange) and lm_peer_detect_batch (peers true: needs one).  With
 // peers, each frame's match runs the fused record exchange; every rank then holds the same survivors, so the chunks of
 // the pose stage -- shared or not -- are the same on every rank.
-static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
-                        const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
+// lm_detect_batch_device's frames: frame f is device frame (rgb[f], depth[f], masks[2f], masks[2f + 1]), one pitch per plane.
+struct DeviceFrames {
+  const uint8_t* const* rgb; int64_t rgb_pitch;
+  const void* const* depth; int64_t depth_pitch; int format; float scale;
+  const uint8_t* const* masks; int64_t mask_pitch;
+  cudaStream_t stream;
+  DeviceFrame frame(int f) const {
+    return {rgb[f], rgb_pitch, depth[f], depth_pitch, format, scale, {masks ? masks[2 * f] : nullptr, masks ? masks[2 * f + 1] : nullptr},
+            mask_pitch};
+  }
+};
+
+// dev NULL: host frames rgb / depth (lm_detect_batch, lm_peer_detect_batch); else dev's device frames, rgb / depth NULL.
+static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t* rgb, const uint16_t* depth, const DeviceFrames* dev,
+                        int rows, int cols, const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
                         int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm, lm_match* out,
                         double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out, int64_t* frame_counts) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
-  if (!d || !rgb || !depth || !sceneK || !n_out || !frame_counts || (cap > 0 && (!out || !R_out || !t_out || !residual)))
+  if (!d || (dev ? (!dev->rgb || !dev->depth) : (!rgb || !depth)) || !sceneK || !n_out || !frame_counts || (cap > 0 && (!out || !R_out || !t_out || !residual)))
     return fail(LM_E_INVALID, "null argument");
   if (n_frames < 1) return fail(LM_E_INVALID, "n_frames %d < 1", n_frames);
   if (rows <= 0 || cols <= 0) return fail(LM_E_INVALID, "empty frame size %d x %d", rows, cols);
@@ -2385,6 +2529,11 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
   if (!d->pose || !pose_stage_covers(d->pose, d->sel.data(), (int64_t)d->sel.size()))
     return fail(LM_E_STATE, "no template renders registered for every selected template of this bank (lm_set_template_renders)");
   CU(cudaSetDevice(d->device));
+  int lrows[LM_MAX_LEVELS], lcols[LM_MAX_LEVELS];
+  for (int f = 0; dev && f < n_frames; ++f) {
+    int rc = check_device_frame(d, dev->frame(f), rows, cols, dev->stream, lrows, lcols);
+    if (rc) return fail(rc, "frame %d: %s", f, std::string(g_err).c_str());
+  }
   cudaStream_t st = d->stream;
   d->pose_pending = false;  // a batch starts new frames: a pending single-frame pose stage is abandoned
   d->pose_nms_pending = false;
@@ -2398,7 +2547,8 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
   std::vector<lm_match> surv(pose_nms ? 0 : (size_t)n_frames * bound);
   for (int f = 0; f < n_frames; ++f) {
     // the single-frame chain up to the box NMS, its capacity retry included
-    rc = lm_upload_images(d, rgb + f * n0 * 3, depth + f * n0, rows, cols, masks ? masks[2 * f] : nullptr, masks ? masks[2 * f + 1] : nullptr);
+    rc = dev ? bind_images_device(d, dev->frame(f), rows, cols, lrows, lcols, dev->stream)
+             : lm_upload_images(d, rgb + f * n0 * 3, depth + f * n0, rows, cols, masks ? masks[2 * f] : nullptr, masks ? masks[2 * f + 1] : nullptr);
     if (rc) return rc;
     rc = lm_enqueue(d, threshold);
     if (rc) return rc;
@@ -2454,7 +2604,7 @@ extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb,
                                const uint8_t* const* masks, float threshold, const float* sceneK, double iou_threshold, int top_k,
                                int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm, lm_match* out,
                                double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out, int64_t* frame_counts) {
-  return detect_batch(d, false, n_frames, rgb, depth, rows, cols, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
+  return detect_batch(d, false, n_frames, rgb, depth, nullptr, rows, cols, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
                       use_scene_cloud, pose_nms, translation_threshold_mm, out, R_out, t_out, residual, cap, n_out, frame_counts);
 }
 
@@ -2463,8 +2613,20 @@ extern "C" int lm_peer_detect_batch(lm_detector* d, int n_frames, const uint8_t*
                                     int max_iterations, int use_scene_cloud, int pose_nms, double translation_threshold_mm,
                                     lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out,
                                     int64_t* frame_counts) {
-  return detect_batch(d, true, n_frames, rgb, depth, rows, cols, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
+  return detect_batch(d, true, n_frames, rgb, depth, nullptr, rows, cols, masks, threshold, sceneK, iou_threshold, top_k, max_iterations,
                       use_scene_cloud, pose_nms, translation_threshold_mm, out, R_out, t_out, residual, cap, n_out, frame_counts);
+}
+
+extern "C" int lm_detect_batch_device(lm_detector* d, int n_frames, const uint8_t* const* rgb, int64_t rgb_pitch, const void* const* depth,
+                                      int64_t depth_pitch, int depth_format, float depth_scale, int rows, int cols,
+                                      const uint8_t* const* masks, int64_t mask_pitch, void* stream, float threshold, const float* sceneK,
+                                      double iou_threshold, int top_k, int max_iterations, int use_scene_cloud, int pose_nms,
+                                      double translation_threshold_mm, lm_match* out, double* R_out, double* t_out, float* residual,
+                                      int64_t cap, int64_t* n_out, int64_t* frame_counts) {
+  const DeviceFrames dev = {rgb, rgb_pitch, depth, depth_pitch, depth_format, depth_scale, masks, mask_pitch, (cudaStream_t)stream};
+  return detect_batch(d, false, n_frames, nullptr, nullptr, &dev, rows, cols, masks, threshold, sceneK, iou_threshold, top_k,
+                      max_iterations, use_scene_cloud, pose_nms, translation_threshold_mm, out, R_out, t_out, residual, cap, n_out,
+                      frame_counts);
 }
 
 extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,

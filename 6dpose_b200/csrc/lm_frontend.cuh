@@ -8,6 +8,8 @@
 //   k_fe_normals     <- quantizedNormals (before the median)                            LL.cpp:729-817
 //   k_fe_median      <- medianBlur(dst, dst, 5) + mask (quantize)                       LL.cpp:818, 882-886
 //   k_fe_decimate    <- resize(..., INTER_NEAREST) of labels / masks                    LL.cpp:865-879
+//   k_fe_ingest      <- the driver's host copy of a frame and its float depth conversion
+//                       (linemod_and_levelup_test.py:315-317), for frames already in device memory
 //
 // The OpenCV calls are restated in the arithmetic OpenCV itself uses for these types, each verified
 // bit-exact against cv2 4.13 (tests/test_gpu_frontend.py; models in tests/test_frontend_models.py):
@@ -253,6 +255,39 @@ __global__ void __launch_bounds__(256) k_fe_median(const uint8_t* __restrict__ i
   const uint8_t val = med ? (uint8_t)(1u << (med - 1)) : 0;
   normal[(size_t)y * W + x] = val;
   quantized[(size_t)y * W + x] = (mask && mask[(size_t)y * W + x] == 0) ? 0 : val;
+}
+
+// ---- ingest of a borrowed device frame (lm_bind_images_device) --------------------------------------
+// Float depth to u16 mm as the reference's driver converts it on the host (depth *= depth_scale;
+// depth.astype(np.uint16), linemod_and_levelup_test.py:315-317): one float32 product, truncated.  Products outside
+// [0, 65536) -- NaN, negatives, infinities, >= 65536 -- are 0 (no depth), where numpy's cast is platform-defined.
+__device__ __forceinline__ uint16_t fe_depth_mm(float d, float scale) {
+  const float v = __fmul_rn(d, scale);
+  return (v >= 0.f && v < 65536.f) ? (uint16_t)__float2uint_rz(v) : (uint16_t)0;
+}
+
+#define FE_INGEST_PX 256  // pixels of one row per CTA
+
+// Copies rows x cols pixels of pitched planes (pixels packed within a row) into the front-end's packed buffers: rgb
+// bytes, depth (u16 copied, f32 converted by fe_depth_mm) and the masks given.  CTA (bx, y) takes pixels
+// [bx * FE_INGEST_PX, +FE_INGEST_PX) of row y; consecutive threads read consecutive addresses of every plane's row.
+__global__ void __launch_bounds__(FE_INGEST_PX) k_fe_ingest(const uint8_t* __restrict__ rgb, int64_t rgb_pitch, const void* __restrict__ depth,
+                                                          int64_t depth_pitch, int depth_f32, float scale, const uint8_t* __restrict__ mask0,
+                                                          const uint8_t* __restrict__ mask1, int64_t mask_pitch, int W,
+                                                          uint8_t* __restrict__ src, uint16_t* __restrict__ depth_out,
+                                                          uint8_t* __restrict__ mask_out0, uint8_t* __restrict__ mask_out1) {
+  const int y = blockIdx.y, x0 = blockIdx.x * FE_INGEST_PX;
+  const int n = min(FE_INGEST_PX, W - x0);
+  const uint8_t* in = rgb + y * rgb_pitch + 3 * x0;
+  uint8_t* out = src + ((size_t)y * W + x0) * 3;
+  for (int i = threadIdx.x; i < 3 * n; i += FE_INGEST_PX) out[i] = in[i];
+  if ((int)threadIdx.x >= n) return;
+  const int x = x0 + threadIdx.x;
+  const size_t o = (size_t)y * W + x;
+  const uint8_t* drow = (const uint8_t*)depth + y * depth_pitch;
+  depth_out[o] = depth_f32 ? fe_depth_mm(((const float*)drow)[x], scale) : ((const uint16_t*)drow)[x];
+  if (mask0) mask_out0[o] = mask0[y * mask_pitch + x];
+  if (mask1) mask_out1[o] = mask1[y * mask_pitch + x];
 }
 
 // resize(INTER_NEAREST) to half size (labels and masks); optional mask applied to a second output

@@ -149,16 +149,26 @@ class Detector:
         """The host front-end: list over levels of [color_labels, normal_labels] (u8)."""
         return frontend.quantize_pyramid(sources, self.pyramid_levels, masks, self.num_features)
 
-    def match(self, sources, threshold, class_ids, masks=None):
+    def match(self, sources, threshold, class_ids, masks=None, depth_scale=1.0, stream=None):
         """Detector::match (LL.cpp:1702-1777) -> list[Match], sorted, duplicates pruned.
 
         As in the reference binding the declared default for `masks` is not convertible; every caller
-        passes masks=[] (linemod_and_levelup_test.py:324)."""
+        passes masks=[] (linemod_and_levelup_test.py:324).
+
+        Beyond the reference: sources may be [rgb, depth] CUDA tensors on the detector's device (a frame already on the
+        GPU; see _lib.DeviceFrame for dtypes and strides, masks then tensors too).  float32 depth is scaled by depth_scale
+        and converted to u16 mm on the device as the driver converts it on the host; the frame is read in order on
+        `stream` (None: torch.cuda.current_stream) without a host synchronise.  Tensors always take the GPU front-end,
+        whatever `frontend` says."""
         if masks is None:
             raise TypeError("match(): incompatible function arguments (masks must be a list; pass masks=[])")
         if len(sources) != 2:
             raise RuntimeError("sources.size() == modalities.size()")  # CV_Assert LL.cpp:1707
-        sources = [self._as_source(s, i) for i, s in enumerate(sources)]
+        sources = self._frame_sources(sources, masks, depth_scale, stream)
+        if isinstance(sources[0], _lib.DeviceFrame):
+            self._whole_bank_only("match()")
+            nat = self._select(list(class_ids))
+            return self._to_matches(nat.match_images(sources[0], None, None, float(threshold)))
         self._whole_bank_only("match()")
         if self.frontend == "gpu" and self.shard[1] == 1:
             nat = self._select(list(class_ids))
@@ -286,18 +296,17 @@ class Detector:
             first += n
 
     def match_refine(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
-                     use_scene_cloud=False, masks=[], estimation="point_to_plane"):
+                     use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
         """match + nms + poseRefine().process for every survivor, as the drivers do (linemod_and_levelup_test.py:
         324-367), in one chain on the GPU: front-end, match, NMS/top-k, cloud building, normals and ICP.  Needs
         setTemplateRenders.  Returns [(Match, poseRefine)] in pick order; each poseRefine is in the state
         refine_matches leaves it in (residual -1, R / t None where the model box does not fit the frame).
         estimation (not in the reference's surface): the ICP's estimation step, "point_to_plane" (the reference's
-        active branch) or "point_to_point" (its other branch, LL.cpp:131-135: no normals, a closed-form rigid fit)."""
+        active branch) or "point_to_point" (its other branch, LL.cpp:131-135: no normals, a closed-form rigid fit).
+        sources, depth_scale and stream as match: a frame may be CUDA tensors."""
         from .pose_refine import poseRefine
         _lib.estimation_code(estimation)
-        if len(sources) != 2:
-            raise RuntimeError("sources.size() == modalities.size()")
-        sources = [self._as_source(s, i) for i, s in enumerate(sources)]
+        sources = self._frame_sources(sources, masks, depth_scale, stream)
         self._whole_bank_only("match_refine()")
         sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
         nat = self._select(list(class_ids))
@@ -306,18 +315,16 @@ class Detector:
         return self._pose_pairs(out, R, t, res)
 
     def detect(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
-               max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane"):
+               max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
         """The whole frame of linemod_ros/detect.py (:91-141): match, box NMS, poseRefine of every survivor (top_k=0)
         and the greedy translation NMS nms_norms(ts, -residual, translation_threshold) (:41-50, :130-131), in one chain
         on the GPU; only the kept objects are copied back.  Needs setTemplateRenders.  Returns [(Match, poseRefine)] in
         keep order, as match_refine(top_k) followed by pose_refine.nms_translations would.  Survivors whose model box
         does not fit the frame (no pose) are not returned; equal residuals keep box-NMS pick order.  estimation as
-        match_refine."""
+        match_refine; sources, depth_scale and stream as match: a frame may be CUDA tensors."""
         from .pose_refine import poseRefine
         _lib.estimation_code(estimation)
-        if len(sources) != 2:
-            raise RuntimeError("sources.size() == modalities.size()")
-        sources = [self._as_source(s, i) for i, s in enumerate(sources)]
+        sources = self._frame_sources(sources, masks, depth_scale, stream)
         self._whole_bank_only("detect()")
         sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
         nat = self._select(list(class_ids))
@@ -327,44 +334,65 @@ class Detector:
 
     # ---- a batch of RGB-D frames through one pose stage (lm_detect_batch) ----
     def match_refine_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
-                           use_scene_cloud=False, masks=[], estimation="point_to_plane"):
+                           use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
         """match_refine for many frames in one call: each frame's match and box NMS, then one pose stage for the survivors
         of all of them, which fills the GPU where one frame's few survivors cannot.  frames: a sequence of [rgb, depth]
         pairs of one size; sceneK: one 3x3 matrix or one per frame; masks: [] or one masks list per frame.  Returns one
         list per frame, each equal to match_refine on that frame.  The handle keeps the batch's device buffers, sized
         for the batch's shape (frames, size, top_k; with top_k=0 the pose buffers of 1024 survivors), for the next one.
-        estimation as match_refine."""
+        estimation as match_refine.  frames may be CUDA tensor pairs (match), all of one size, row pitches and depth dtype,
+        with depth_scale and stream as match."""
         _lib.estimation_code(estimation)
-        nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "match_refine_batch()")
-        got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
-                               bool(use_scene_cloud), pose_nms=False, estimation=estimation)
+        inputs, K = self._batch_inputs(frames, sceneK, masks, "match_refine_batch()", depth_scale, stream)
+        self._whole_bank_only("match_refine_batch()")
+        nat = self._select(list(class_ids))
+        call, inputs = (nat.detect_batch_device, (inputs,)) if isinstance(inputs, _lib.DeviceBatch) else (nat.detect_batch, inputs)
+        got = call(*inputs, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations), bool(use_scene_cloud),
+                   pose_nms=False, estimation=estimation)
         return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
     def detect_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
-                     max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane"):
+                     max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
         """detect for many frames in one call: each frame's match and box NMS, then one pose stage and one pose NMS for all
         of them.  Arguments as match_refine_batch; returns one list per frame, each equal to detect on that frame."""
         _lib.estimation_code(estimation)
-        nat, (rgb, depth, mk, K) = self._batch_args(frames, class_ids, sceneK, masks, "detect_batch()")
-        got = nat.detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
-                               bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold),
-                               estimation=estimation)
+        inputs, K = self._batch_inputs(frames, sceneK, masks, "detect_batch()", depth_scale, stream)
+        self._whole_bank_only("detect_batch()")
+        nat = self._select(list(class_ids))
+        call, inputs = (nat.detect_batch_device, (inputs,)) if isinstance(inputs, _lib.DeviceBatch) else (nat.detect_batch, inputs)
+        got = call(*inputs, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations), bool(use_scene_cloud),
+                   pose_nms=True, translation_threshold=float(translation_threshold), estimation=estimation)
         return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
 
     def _batch_args(self, frames, class_ids, sceneK, masks, what):
-        # everything that needs no device is checked before the native handle exists
+        # the sharded batch calls (dist.py), which take numpy frames: the handle, then (rgb, depth, mask pairs, K)
+        inputs, K = self._batch_inputs(frames, sceneK, masks, what)
+        if isinstance(inputs, _lib.DeviceBatch):
+            raise TypeError("%s takes numpy frames" % what)
+        self._whole_bank_only(what)
+        return self._select(list(class_ids)), inputs + (K,)
+
+    def _batch_inputs(self, frames, sceneK, masks, what, depth_scale=1.0, stream=None):
+        # every check that needs no device, before the native handle exists.  Returns (inputs, K): inputs is a
+        # _lib.DeviceBatch for CUDA tensor frames, else (rgb [n,H,W,3], depth [n,H,W], mask pairs or None)
         from .pose_refine import poseRefine
         frames = list(frames)
         if not frames:
             raise ValueError("%s: no frames" % what)
-        rgb, depth = [], []
         for sources in frames:
             if len(sources) != 2:
                 raise RuntimeError("sources.size() == modalities.size()")
-            rgb.append(self._as_source(sources[0], 0))
-            depth.append(self._as_source(sources[1], 1))
-        if any(r.shape != rgb[0].shape or d.shape != rgb[0].shape[:2] for r, d in zip(rgb, depth)):
-            raise ValueError("%s: every frame's colour and depth images must have one size" % what)
+        on_device = [_lib.is_tensor(s[0]) or _lib.is_tensor(s[1]) for s in frames]
+        if any(on_device) and not all(on_device):
+            raise TypeError("%s: frames mix numpy arrays and torch tensors" % what)
+        rgb, depth = [], []
+        if not on_device[0]:
+            _lib.host_frame_options(depth_scale, stream)
+            for sources in frames:
+                rgb.append(self._as_source(sources[0], 0))
+                depth.append(self._as_source(sources[1], 1))
+            if any(r.shape != rgb[0].shape or d.shape != rgb[0].shape[:2] for r, d in zip(rgb, depth)):
+                raise ValueError("%s: every frame's colour and depth images must have one size" % what)
         n = len(frames)
         K = np.asarray(sceneK)
         if K.size == 9:
@@ -386,9 +414,13 @@ class Detector:
                 if m and len(m) != 2:
                     raise RuntimeError("masks.size() == modalities.size()")
                 pairs.append(m if m else [None, None])
-        self._whole_bank_only(what)
-        nat = self._select(list(class_ids))
-        return nat, (np.stack(rgb), np.stack(depth), pairs, K)
+        if on_device[0]:
+            try:
+                return _lib.DeviceBatch([_lib.DeviceFrame(s[0], s[1], pairs[f] if pairs else None, depth_scale, stream, self.device)
+                                         for f, s in enumerate(frames)]), K
+            except ValueError as e:
+                raise ValueError("%s: %s" % (what, e)) from None
+        return (np.stack(rgb), np.stack(depth), pairs), K
 
     def _pose_pairs(self, out, R, t, res):
         # [(Match, poseRefine)]; a survivor without a pose (residual -1, only without the pose NMS) keeps R / t None
@@ -409,6 +441,15 @@ class Detector:
         names = self._class_order
         return list(map(Match, out["x"].tolist(), out["y"].tolist(), out["similarity"].tolist(),
                         [names[c] for c in out["class_index"].tolist()], out["template_id"].tolist()))
+
+    def _frame_sources(self, sources, masks, depth_scale, stream):
+        # [DeviceFrame, None] for CUDA tensors, checked here once, before any library call; the numpy sources otherwise
+        if len(sources) != 2:
+            raise RuntimeError("sources.size() == modalities.size()")
+        frame = _lib.frame_inputs(sources[0], sources[1], list(masks) if masks is not None else None, depth_scale, stream, self.device)
+        if frame is not None:
+            return [frame, None]
+        return [self._as_source(s, i) for i, s in enumerate(sources)]
 
     @staticmethod
     def _as_source(a, i):

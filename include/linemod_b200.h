@@ -111,6 +111,34 @@ int lm_bind_quantized_device(lm_detector* d, const uint8_t* const* d_quantized, 
 int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
                      const uint8_t* mask_color, const uint8_t* mask_depth);
 
+/* lm_upload_images for a frame already in device memory (a GPU decoder's output, a depth network's, a camera rig's
+ * device buffers): one launch of k_fe_ingest copies it into the front-end's buffers, then the same front-end runs.
+ *   Layout     rgb u8 rows x cols x 3, depth and the masks one element per pixel; pixels packed within a row, rows
+ *              rgb_pitch / depth_pitch / mask_pitch BYTES apart (a crop view of a larger image is fine).  Every pointer
+ *              is device or managed memory of the handle's device.  mask_color / mask_depth NULL: none (255 = valid).
+ *   Depth      LM_DEPTH_U16_MM: u16 mm, copied as is.  LM_DEPTH_F32: float32 d, stored as v = d * depth_scale rounded
+ *              once in float32, truncated to u16 for 0 <= v < 65536 -- for every such value bit for bit the reference
+ *              driver's host conversion (depth *= depth_scale; depth.astype(np.uint16), linemod_and_levelup_test.py:
+ *              315-317), i.e. (d_f32 * np.float32(depth_scale)).astype(np.uint16).  Deviation: NaN, negative, infinite
+ *              and >= 65536 products, where numpy's cast is platform-defined, are 0 (no depth).
+ *   Ordering   no host synchronise.  The call records an event on `stream` (a cudaStream_t; NULL = the legacy default
+ *              stream) and the handle's stream waits on it, so what the producer enqueued on `stream` before the call
+ *              has completed before the ingest reads the frame; after the ingest the handle records a second event and
+ *              `stream` waits on it, so the caller's next write to the frame is ordered after the read.  The borrow
+ *              ends when the ingest has run, not at lm_complete*.
+ * A bound frame is a frame with depth exactly like an uploaded one: lm_enqueue (depth gate included), lm_enqueue_post,
+ * lm_enqueue_pose and lm_enqueue_pose_nms take it unchanged, and lm_bind_images_device + lm_run + lm_fetch_records +
+ * lm_finish is lm_match_images.  Beyond first use at a frame size (buffers, the normal table) nothing from the bind to
+ * lm_enqueue_pose_nms synchronises the host after lm_prepare.
+ * LM_E_INVALID, before any device work, for a null rgb or depth; a stream of another device; a pointer that is not device
+ * or managed memory of the handle's device; a pitch shorter than a row; a depth pointer or pitch not aligned to its element size; an unknown
+ * depth_format; a non-finite or non-positive depth_scale with LM_DEPTH_F32; and lm_upload_images' frame-size rules. */
+#define LM_DEPTH_U16_MM 0
+#define LM_DEPTH_F32 1
+int lm_bind_images_device(lm_detector* d, const uint8_t* rgb, int64_t rgb_pitch, const void* depth, int64_t depth_pitch,
+                          int depth_format, float depth_scale, int rows, int cols, const uint8_t* mask_color,
+                          const uint8_t* mask_depth, int64_t mask_pitch, void* stream);
+
 /* GPU stages on the uploaded frame: spread/response/linearize (LL.cpp:1094-1243), coarse similarity
  * scan + threshold (LL.cpp:1284-1354, 1836-1852), local 16x16 refinement up the pyramid
  * (LL.cpp:1366-1428, 1855-1938).  Leaves the ordered candidate records in device memory. */
@@ -379,6 +407,18 @@ int lm_peer_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const
                          lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap, int64_t* n_out,
                          int64_t* frame_counts);
 
+/* lm_detect_batch from frames already in device memory: frame f's upload is replaced by lm_bind_images_device of
+ * (rgb[f], depth[f], masks ? masks[2f] : NULL, masks ? masks[2f + 1] : NULL) with the common pitches, depth format, scale
+ * and stream -- n_frames device pointers per plane, held in host arrays.  From threshold on, the arguments, outputs,
+ * frame_counts and errors are lm_detect_batch's; lm_bind_images_device's checks are made for every frame before any
+ * device work.  Each frame's borrow ends with its ingest, ordered on `stream` as lm_bind_images_device orders it. */
+int lm_detect_batch_device(lm_detector* d, int n_frames, const uint8_t* const* rgb, int64_t rgb_pitch, const void* const* depth,
+                           int64_t depth_pitch, int depth_format, float depth_scale, int rows, int cols,
+                           const uint8_t* const* masks, int64_t mask_pitch, void* stream, float threshold, const float* sceneK,
+                           double iou_threshold, int top_k, int max_iterations, int use_scene_cloud, int pose_nms,
+                           double translation_threshold_mm, lm_match* out, double* R_out, double* t_out, float* residual,
+                           int64_t cap, int64_t* n_out, int64_t* frame_counts);
+
 /* Convenience = lm_upload_quantized + lm_run + lm_fetch_records + lm_finish (single GPU):
  * Detector::match after quantization. */
 int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,
@@ -427,6 +467,8 @@ int lm_depth_gate_stats(lm_detector* d, int64_t* out4);
 /* ---- introspection used by the parity tests and the benchmark ---- */
 /* Quantized label image of (level, modality) of the uploaded frame: rows*cols bytes. */
 int lm_debug_quantized(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap);
+/* Depth image (u16 mm, rows*cols) of the frame lm_upload_images uploaded or lm_bind_images_device bound. */
+int lm_debug_depth(lm_detector* d, uint16_t* out, int64_t cap);
 /* Linear memories of (level, modality) of the last lm_run: [8][T*T][(cols/T)*(rows/T)] bytes. */
 int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap);
 /* Counters of the last lm_run: [0] templates scanned, [1] coarse candidates, [2] algorithmic bytes of
