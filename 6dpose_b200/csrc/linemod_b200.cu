@@ -2346,15 +2346,11 @@ static int enqueue_pose(lm_detector* d) {
     if (rc) return rc;
   }
   PoseEnqueue e;
-  e.share = share ? &sh : nullptr;
+  e.o = {d->fe[0].rows, d->fe[0].cols, d->pose_use_scene, d->pose_max_iter, d->pose_frame_estimation, d->stream, share ? &sh : nullptr};
   e.d_surv = d->d_post_out; e.d_counts = d->d_post_counts;
-  e.d_scene = d->fe_depth; e.srows = d->fe[0].rows; e.scols = d->fe[0].cols;
+  e.d_scene = d->fe_depth;
   memcpy(e.sK, d->pose_sK, sizeof(e.sK));
   e.bound = d->post_top_k > 0 ? std::min(d->post_top_k, LM_POST_MAX) : LM_POST_MAX;
-  e.use_scene_cloud = d->pose_use_scene;
-  e.max_iterations = d->pose_max_iter;
-  e.estimation = d->pose_frame_estimation;
-  e.stream = d->stream;
   return pose_stage_enqueue(d->pose, e, &d->launches);
 }
 
@@ -2564,21 +2560,18 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     frame_counts[4 * f + 1] = n;
     frame_counts[4 * f + 3] = n_rec;
   }
-  PoseBatch b;
-  b.n_frames = n_frames; b.srows = rows; b.scols = cols;
-  b.first = first.data(); b.surv = surv.data(); b.sK = sceneK;
-  b.use_scene_cloud = use_scene_cloud ? 1 : 0; b.max_iterations = max_iterations;
-  b.estimation = d->pose_estimation;
-  b.pose_nms = pose_nms ? 1 : 0; b.thr = translation_threshold_mm;
-  b.stream = st;
   PoseShare sh;
-  b.share = nullptr;
-  if (peers && d->px_share_pose) {  // one pose exchange per chunk, numbered on from the single frames' ones
+  const bool share = peers && d->px_share_pose;
+  if (share) {  // one pose exchange per chunk, numbered on from the single frames' ones
     rc = pose_share_of(d, d->px_pose_seq + 1, &sh);
     if (rc) return rc;
     d->px_pose_seq += pose_batch_chunks(first[n_frames]);
-    b.share = &sh;
   }
+  PoseBatch b;
+  b.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr};
+  b.n_frames = n_frames;
+  b.first = first.data(); b.surv = surv.data(); b.sK = sceneK;
+  b.pose_nms = pose_nms ? 1 : 0; b.thr = translation_threshold_mm;
   std::vector<int64_t> posed((size_t)n_frames), kept((size_t)n_frames);
   int64_t stats[4];
   rc = pose_batch_run(d->pose, b, &d->launches, posed.data(), kept.data(), peers ? stats : nullptr);

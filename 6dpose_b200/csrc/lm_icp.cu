@@ -19,7 +19,9 @@
 //
 // The pose stage (lm_pose.h, end of this file) does the host's cloud building on the device for the detector's NMS
 // survivors: k_pose_cloud + a CUB segmented sort + k_pose_voxel build the same clouds and initial guesses, bit for
-// bit, and feed the same two ICP kernels.
+// bit, and feed the same ICP kernels; k_pose_nms may follow.  A frame, a batch chunk and their shared forms are all
+// one chunk to pose_chunk and to the kernels, told apart by data only: the survivor count on the device, an optional
+// frame table, and the slot rule survivor = rank + slot * world.
 
 #include "linemod_b200.h"
 #include "lm_pose.h"
@@ -1103,7 +1105,7 @@ struct PoseTpl {  // per template of the bank, registered once
 
 struct PoseParams {
   const lm_match* surv;
-  const int32_t* counts;
+  const int32_t* counts;    // [0] survivors of the chunk
   const int32_t* class_begin;
   int32_t n_classes, n_tpl;
   const PoseTpl* tpl;
@@ -1121,13 +1123,12 @@ struct PoseParams {
   int32_t* seg_end;
   IcpJob* jobs;       // [B]
   int32_t* err;       // 1: a cloud spans more than 2^21 voxels along an axis
-  uint8_t* posed;     // [B] 1: survivor i has a template and its box fits the frame (no early return of LL.cpp:52-55)
-  // k_pose_cloud_batch only: slot i belongs to frame frame_of[i], whose depth is scene + frame * srows * scols and whose
-  // intrinsics are sKs + 9 * frame (sK is unused, counts too except in k_pose_cloud_batch_share: [0] the chunk's size)
+  uint8_t* posed;     // [B] 1: slot i's survivor has a template and its box fits the frame (no early return of LL.cpp:52-55)
+  // null: every survivor is of one frame, depth scene and intrinsics sK.  Else survivor si belongs to frame
+  // frame_of[si], whose depth is scene + frame * srows * scols and whose intrinsics are sKs + 9 * frame.
   const int32_t* frame_of;
   const float* sKs;
-  // k_pose_cloud_share / k_pose_cloud_batch_share only: slot i takes survivor rank + i * world (PoseShare)
-  int32_t rank, world;
+  int32_t rank, world;  // slot i takes survivor rank + i * world (lm_pose.h)
 };
 
 __device__ __forceinline__ double pose_backproject(int pix, float c, float f, double z) {
@@ -1140,13 +1141,9 @@ __device__ __forceinline__ int pose_template(const PoseParams& p, const lm_match
   return (g >= 0 && g < p.n_tpl) ? g : -1;
 }
 
-// One CTA per survivor slot.  Single frame (k_pose_cloud): launched for the bound, slots past the survivor count write
-// empty jobs.  Batch (k_pose_cloud_batch): launched for the exact slot count, the frame of each slot from p.frame_of.
-// Shared (k_pose_cloud_share): launched for this rank's share of the bound, slot i takes survivor p.rank + i * p.world.
-// Shared batch chunk (k_pose_cloud_batch_share): launched for this rank's share of the chunk, slot i takes chunk survivor
-// p.rank + i * p.world (p.counts[0]: the chunk's size) and reads that survivor's frame.
-template <bool BATCH, bool SHARE>
-__device__ __forceinline__ void pose_cloud(const PoseParams& p) {
+// One CTA per survivor slot: slot i takes survivor si = p.rank + i * p.world, live iff si < p.counts[0] and the survivor
+// has a template whose box fits the frame.  Slots that are not write empty jobs.
+__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
   typedef cub::BlockScan<unsigned long long, POSE_THREADS> Scan;
   typedef cub::BlockReduce<double, POSE_THREADS> Reduce;
   __shared__ union {
@@ -1160,12 +1157,12 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
   IcpJob* job = p.jobs + i;
   lm_match m = {0, 0, 0.f, 0, 0};
   PoseTpl T;
-  const int si = SHARE ? p.rank + i * p.world : i;  // survivor of this slot
-  const bool in_chunk = !(BATCH && SHARE) || si < p.counts[0];
-  const int frame = BATCH ? (in_chunk ? p.frame_of[si] : 0) : 0;
-  const uint16_t* __restrict__ scene = BATCH ? p.scene + (size_t)frame * p.srows * p.scols : p.scene;
-  const float* __restrict__ bK = BATCH ? p.sKs + 9 * frame : nullptr;
-  bool live = BATCH ? in_chunk : si < p.counts[0];
+  const int si = p.rank + i * p.world;  // survivor of this slot
+  bool live = si < p.counts[0];
+  const int frame = live && p.frame_of ? p.frame_of[si] : 0;
+  const uint16_t* __restrict__ scene = p.scene + (size_t)frame * p.srows * p.scols;
+  const float* __restrict__ fK = p.frame_of ? p.sKs + 9 * frame : nullptr;
+  const float fx = fK ? fK[0] : p.sK[0], cx = fK ? fK[2] : p.sK[2], fy = fK ? fK[4] : p.sK[4], cy = fK ? fK[5] : p.sK[5];
   if (live) {
     m = p.surv[si];
     const int g = pose_template(p, m);
@@ -1225,8 +1222,8 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
         const uint16_t sd = scene[(size_t)sr * p.scols + sc];
         if (sd > 0) {
           sz = __ddiv_rn((double)sd, 1000.0);
-          sx = pose_backproject(sc, BATCH ? bK[2] : p.sK[2], BATCH ? bK[0] : p.sK[0], sz);
-          sy = pose_backproject(sr, BATCH ? bK[5] : p.sK[5], BATCH ? bK[4] : p.sK[4], sz);
+          sx = pose_backproject(sc, cx, fx, sz);
+          sy = pose_backproject(sr, cy, fy, sz);
           fs = p.use_scene != 0;
           fc = md > 0 && fabs(__dsub_rn(sz, anchor)) < 0.4;
         }
@@ -1294,11 +1291,6 @@ __device__ __forceinline__ void pose_cloud(const PoseParams& p) {
     p.seg_begin[2 * i + 1] = (int32_t)ss; p.seg_end[2 * i + 1] = (int32_t)ss + ns;
   }
 }
-
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) { pose_cloud<false, false>(p); }
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch(PoseParams p) { pose_cloud<true, false>(p); }
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_share(PoseParams p) { pose_cloud<false, true>(p); }
-__global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud_batch_share(PoseParams p) { pose_cloud<true, true>(p); }
 
 // One CTA per cloud slot: mean of every occupied voxel, summed in sorted order (voxel_down_sample).
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals,
@@ -1456,25 +1448,23 @@ __device__ __forceinline__ double pose_compose(const double* T, const PoseRt& q,
 
 struct PoseNmsParams {
   const lm_match* surv;
-  const int32_t* counts;    // [0] survivors written by k_post_nms
+  const int32_t* counts;    // [0] survivors written by k_post_nms (without frame_first)
   const uint8_t* posed;     // k_pose_cloud's verdict per survivor
   const IcpOut* outs;
   const PoseRt* rt;
   const int32_t* class_begin;
   double thr;
-  PoseNmsHead* head;
-  PoseNmsOut* out;          // kept poses in keep order
-  // k_pose_nms_batch only: CTA f takes the survivors [frame_first[f], frame_first[f + 1]) of surv / posed / outs, writes
-  // head[f] and its kept poses from out + frame_first[f] (counts is unused)
+  PoseNmsHead* head;        // [frame]
+  PoseNmsOut* out;          // kept poses in keep order, frame f's from out + frame_first[f]
+  // null: one frame, survivors [0, counts[0]).  Else frame f's survivors are [frame_first[f], frame_first[f + 1]).
   const int32_t* frame_first;
 };
 
-// Behind k_icp_point_to_plane: candidates are the survivors with a pose, score -(double)residual.  One frame per CTA.
-template <bool BATCH>
-__device__ __forceinline__ void pose_nms(const PoseNmsParams& p) {
+// Behind the ICP kernel: candidates are the survivors with a pose, score -(double)residual.  One frame per CTA.
+__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
   const int i = threadIdx.x;
-  const int first = BATCH ? p.frame_first[blockIdx.x] : 0;
-  const int n = BATCH ? p.frame_first[blockIdx.x + 1] - first : min(p.counts[0], NMS_THREADS);
+  const int first = p.frame_first ? p.frame_first[blockIdx.x] : 0;
+  const int n = p.frame_first ? p.frame_first[blockIdx.x + 1] - first : min(p.counts[0], NMS_THREADS);
   const lm_match* __restrict__ surv = p.surv + first;
   const IcpOut* __restrict__ outs = p.outs + first;
   bool cand = false;
@@ -1504,13 +1494,10 @@ __device__ __forceinline__ void pose_nms(const PoseNmsParams& p) {
   }
   if (i == 0) {
     PoseNmsHead h;
-    h.kept = kept; h.survivors = BATCH ? n : p.counts[0]; h.posed = posed; h.pad = 0;
-    p.head[BATCH ? blockIdx.x : 0] = h;
+    h.kept = kept; h.survivors = p.frame_first ? n : p.counts[0]; h.posed = posed; h.pad = 0;
+    p.head[blockIdx.x] = h;
   }
 }
-
-__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) { pose_nms<false>(p); }
-__global__ void __launch_bounds__(NMS_THREADS) k_pose_nms_batch(PoseNmsParams p) { pose_nms<true>(p); }
 
 struct TplHost {
   bool set = false;
@@ -1556,8 +1543,8 @@ struct lm_pose_stage {
   PoseNmsOut* d_bnms = nullptr; PoseNmsOut* h_bnms = nullptr;
   int32_t* d_bfirst = nullptr; float* d_bsK = nullptr;  // [cap_bframes + 1], [cap_bframes][9]
   PoseNmsHead* d_bhead = nullptr; PoseNmsHead* h_bhead = nullptr;
-  // shared batch: per chunk (at most one per frame) [0] cloud overflow, [1] a peer's poses did not arrive, [2] entries
-  // this rank published, [3] the chunk's size (device, pinned copy)
+  // per chunk (at most one per frame) [0] cloud overflow, shared [1] a peer's poses did not arrive, [2] entries this
+  // rank published, [3] the chunk's size (device, pinned copy)
   int32_t* d_bstat = nullptr; int32_t* h_bstat = nullptr;
 };
 
@@ -1716,83 +1703,160 @@ static PoseShareDev share_dev(const PoseShare& sh, int32_t seq, const int32_t* c
   return sd;
 }
 
+// One chunk of the pose stage (lm_pose.h): survivors surv[0, counts[0]), counts on the device, of one frame (frame_of
+// null: depth scene, intrinsics sK) or of the frames frame_of gives.  The launches are sized for `slots` survivors.
+// Their results go to outs / posed; status: [0] cloud overflow, shared [1] a peer's poses did not arrive, [2] entries
+// this rank published.  seq: the chunk's pose exchange (shared).
+struct PoseChunk {
+  const lm_match* surv;
+  const int32_t* counts;
+  int slots;
+  const uint16_t* scene;
+  const int32_t* frame_of;
+  const float* sKs;
+  const float* sK;
+  IcpOut* outs;
+  uint8_t* posed;
+  int32_t* status;
+  int32_t seq;
+};
+
+// k_pose_cloud, the segmented sort, k_pose_voxel, k_icp_normals (point-to-plane only) and the ICP kernel over this
+// rank's ceil(slots / world) slots, then (shared) k_pose_collect.  Unshared, the cloud's posed flags and the ICP results
+// go straight to the chunk's outputs; shared, to the stage's per-slot scratch, and k_pose_collect writes the outputs.
+// Returns the chunk's launches (the sort counted once), or an error code (< 0).
+static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c) {
+  cudaStream_t st = o.stream;
+  const PoseShare* sh = o.share;
+  const int world = sh ? sh->world : 1;
+  const int n = (c.slots + world - 1) / world;  // a rank without a survivor still publishes
+  const int64_t A = s->cap_area;  // slot stride: the buffers' area, which may exceed the current largest crop
+  PoseParams p;
+  p.surv = c.surv; p.counts = c.counts;
+  p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
+  p.tpl = s->d_tpl; p.crops = s->d_crops;
+  p.scene = c.scene; p.srows = o.srows; p.scols = o.scols;
+  if (c.sK) memcpy(p.sK, c.sK, sizeof(p.sK));
+  else memset(p.sK, 0, sizeof(p.sK));
+  p.A = (int32_t)A; p.use_scene = o.use_scene_cloud ? 1 : 0;
+  p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
+  p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * n;
+  p.jobs = s->d_jobs; p.err = c.status; p.posed = sh ? s->d_posed : c.posed;
+  p.frame_of = c.frame_of; p.sKs = c.sKs;
+  p.rank = sh ? sh->rank : 0; p.world = world;
+  k_pose_cloud<<<n, POSE_THREADS, 0, st>>>(p);
+  // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
+  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
+  cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
+  size_t tmp_bytes = s->sort_tmp_bytes;
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * n * A), 2 * n, p.seg_begin, p.seg_end, 0,
+                                               3 * POSE_KEY_BITS, st));
+  k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
+                                               p.use_scene);
+  // the ICP kernels of lm_icp_process_batch: empty jobs fall through
+  const bool normals = o.estimation == LM_ICP_POINT_TO_PLANE;
+  if (normals) {
+    dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
+    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+  }
+  if (sh) {
+    // the results travel to every rank; the collector gathers the chunk in survivor order
+    const PoseShareDev sd = share_dev(*sh, c.seq, c.counts, s->d_posed, c.status);
+    launch_icp<true>(o.estimation, n, st, s->d_jobs, s->d_pts, s->d_nrm, nullptr, o.max_iterations, nullptr, sd);
+    k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, c.outs, c.posed);
+  } else {
+    launch_icp<false>(o.estimation, n, st, s->d_jobs, s->d_pts, s->d_nrm, c.outs, o.max_iterations, nullptr, PoseShareDev());
+  }
+  CUI(cudaGetLastError());
+  return (sh ? 6 : 5) - (normals ? 0 : 1);
+}
+
 int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches) {
-  cudaStream_t st = e.stream;
+  const PoseOptions& o = e.o;
+  cudaStream_t st = o.stream;
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
   }
   int rc = pose_buffers(s, st, e.bound, s->area_max);
   if (rc) return rc;
-  const int B = e.bound;
-  const PoseShare* sh = e.share;
-  const int Bs = sh ? (B + sh->world - 1) / sh->world : B;  // slots this rank refines
-  const int64_t A = s->cap_area;  // slot stride: the buffers' area, which may exceed the current largest crop
-  PoseParams p;
-  p.surv = e.d_surv; p.counts = e.d_counts;
-  p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
-  p.tpl = s->d_tpl; p.crops = s->d_crops;
-  p.scene = e.d_scene; p.srows = e.srows; p.scols = e.scols;
-  memcpy(p.sK, e.sK, sizeof(p.sK));
-  p.A = (int32_t)A; p.use_scene = e.use_scene_cloud ? 1 : 0;
-  p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
-  p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * B;
-  p.jobs = s->d_jobs; p.err = s->d_err; p.posed = s->d_posed;
-  p.frame_of = nullptr; p.sKs = nullptr;
-  p.rank = sh ? sh->rank : 0; p.world = sh ? sh->world : 1;
+  const PoseShare* sh = o.share;
   CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
-  if (sh) k_pose_cloud_share<<<Bs, POSE_THREADS, 0, st>>>(p);
-  else k_pose_cloud<<<B, POSE_THREADS, 0, st>>>(p);
-  // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
-  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
-  cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
-  size_t tmp_bytes = s->sort_tmp_bytes;
-  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * Bs * A), 2 * Bs, p.seg_begin, p.seg_end, 0,
-                                               3 * POSE_KEY_BITS, st));
-  k_pose_voxel<<<2 * Bs, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
-                                                p.use_scene);
-  // the ICP kernels of lm_icp_process_batch, launched for the bound (this rank's share): empty jobs fall through
-  const bool normals = e.estimation == LM_ICP_POINT_TO_PLANE;
-  if (normals) {
-    dim3 g((unsigned)((A + 127) / 128), (unsigned)Bs);
-    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
-  }
-  if (sh) {
-    const PoseShareDev sd = share_dev(*sh, sh->seq, e.d_counts, s->d_posed, s->d_err);
-    launch_icp<true>(e.estimation, Bs, st, s->d_jobs, s->d_pts, s->d_nrm, nullptr, e.max_iterations, nullptr, sd);
-    k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_outs, s->d_posed);
-  } else {
-    launch_icp<false>(e.estimation, B, st, s->d_jobs, s->d_pts, s->d_nrm, s->d_outs, e.max_iterations, nullptr, PoseShareDev());
-  }
-  CUI(cudaGetLastError());
-  // k_pose_cloud, the segmented sort (counted once), k_pose_voxel, k_icp_normals (point-to-plane only), the ICP kernel
-  // (+ k_pose_collect)
-  s->last_launches = (sh ? 6 : 5) - (normals ? 0 : 1);
-  *launches += s->last_launches;
-  CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(B, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
+  PoseChunk c;
+  c.surv = e.d_surv; c.counts = e.d_counts; c.slots = e.bound;
+  c.scene = e.d_scene; c.frame_of = nullptr; c.sKs = nullptr; c.sK = e.sK;
+  c.outs = s->d_outs; c.posed = s->d_posed; c.status = s->d_err; c.seq = sh ? sh->seq : 0;
+  const int k = pose_chunk(s, o, c);
+  if (k < 0) return k;
+  s->last_launches = k;
+  *launches += k;
+  CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(e.bound, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
   CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t) * (sh ? 3 : 1), cudaMemcpyDeviceToHost, st));
-  s->bound = B; s->srows = e.srows; s->scols = e.scols;
+  s->bound = e.bound; s->srows = o.srows; s->scols = o.scols;
   s->shared = sh != nullptr;
   s->share_seq = sh ? sh->seq : 0;
   s->share_timeout_ns = sh ? sh->timeout_ns : 0;
   return LM_OK;
 }
 
-// The stage's errors, after the stream has been synchronised.
-static int pose_status(const lm_pose_stage* s) {
-  if (s->shared && s->h_err[1])
-    return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d within %llu ms (or an earlier collector "
-                   "on this device already gave up); every rank must run the pose stage of every frame while sharing is on",
-                   s->share_seq, s->share_timeout_ns / 1000000ull);
-  if (*s->h_err) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+// After the stream has been synchronised: the error of nb status blocks of 4 int32 (PoseChunk), block c that of pose
+// exchange seq + c when shared; a batch's message names the chunk.  *published (may be null): the entries summed.
+static int pose_status(const int32_t* h, int nb, bool shared, int32_t seq, unsigned long long timeout_ns, bool batch,
+                       int64_t* published) {
+  int32_t overflow = 0;
+  int64_t sum = 0;
+  for (int c = 0; c < nb; ++c) {
+    const int32_t* b = h + 4 * c;
+    if (shared && b[1]) {
+      if (batch)
+        return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d (chunk %d of the batch) within %llu ms "
+                       "(or an earlier collector on this device already gave up); every rank must run every batch while sharing is on",
+                       seq + c, c, timeout_ns / 1000000ull);
+      return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d within %llu ms (or an earlier collector "
+                     "on this device already gave up); every rank must run the pose stage of every frame while sharing is on",
+                     seq + c, timeout_ns / 1000000ull);
+    }
+    overflow |= b[0];
+    if (shared) sum += b[2];
+  }
+  if (overflow) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  if (published) *published = sum;
   return LM_OK;
 }
 
-void pose_stage_stats(const lm_pose_stage* s, int64_t n, int64_t* out4) {
+// What lm_pose_stats returns for a stage of n survivors.
+static void pose_stats(int64_t* out4, int64_t n, bool shared, int64_t published, int64_t launches) {
   out4[0] = n;
-  out4[1] = s->shared ? (int64_t)s->h_err[2] : n;
-  out4[2] = s->last_launches;
-  out4[3] = s->shared ? 1 : 0;
+  out4[1] = shared ? published : n;
+  out4[2] = launches;
+  out4[3] = shared ? 1 : 0;
+}
+
+void pose_stage_stats(const lm_pose_stage* s, int64_t n, int64_t* out4) {
+  pose_stats(out4, n, s->shared, s->h_err[2], s->last_launches);
+}
+
+// Survivor m's registered render, or null.
+static const TplHost* survivor_render(const lm_pose_stage* s, const lm_match& m) {
+  const int n_classes = (int)s->class_begin.size() - 1;
+  const int64_t g = (m.class_index >= 0 && m.class_index < n_classes) ? (int64_t)s->class_begin[m.class_index] + m.template_id : -1;
+  return (g >= 0 && g < (int64_t)s->tpl.size() && s->tpl[(size_t)g].set) ? &s->tpl[(size_t)g] : nullptr;
+}
+
+// LL.cpp:52-55: the reference returns early where the render's box, placed at the match, leaves the frame.
+static bool survivor_fits(const TplHost& h, const lm_match& m, int srows, int scols) {
+  return !(m.x + h.box[2] >= scols || m.y + h.box[3] >= srows);
+}
+
+// Survivor m's pose as lm_complete_pose returns it: T * init_base and the fitness, or residual -1 and R / t untouched
+// where the reference returns early.
+static void survivor_pose(const TplHost& h, const lm_match& m, int srows, int scols, const IcpOut& o, double* R_out, double* t_out,
+                          float* residual) {
+  if (!survivor_fits(h, m, srows, scols)) { *residual = -1.f; return; }
+  float base[16];
+  init_base(h.R, h.t, base);
+  compose(o.T, base, R_out, t_out);
+  *residual = (float)o.fitness;
 }
 
 int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
@@ -1803,20 +1867,12 @@ int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, i
                         cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
   }
-  int rc = pose_status(s);
+  int rc = pose_status(s->h_err, 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
   if (rc) return rc;
-  const int n_classes = (int)s->class_begin.size() - 1;
   for (int64_t i = 0; i < n; ++i) {
-    const lm_match& m = surv[i];
-    const int64_t g = (m.class_index >= 0 && m.class_index < n_classes) ? (int64_t)s->class_begin[m.class_index] + m.template_id : -1;
-    if (g < 0 || g >= (int64_t)s->tpl.size() || !s->tpl[(size_t)g].set)
-      return lm_fail(LM_E_STATE, "survivor %lld: template without a registered render", (long long)i);
-    const TplHost& h = s->tpl[(size_t)g];
-    if (m.x + h.box[2] >= s->scols || m.y + h.box[3] >= s->srows) { residual[i] = -1.f; continue; }  // LL.cpp:52-55
-    float base[16];
-    init_base(h.R, h.t, base);
-    compose(s->h_outs[i].T, base, R_out + 9 * i, t_out + 3 * i);
-    residual[i] = (float)s->h_outs[i].fitness;
+    const TplHost* h = survivor_render(s, surv[i]);
+    if (!h) return lm_fail(LM_E_STATE, "survivor %lld: template without a registered render", (long long)i);
+    survivor_pose(*h, surv[i], s->srows, s->scols, s->h_outs[i], R_out + 9 * i, t_out + 3 * i, residual + i);
   }
   return LM_OK;
 }
@@ -1826,6 +1882,32 @@ int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, i
 
 static PoseNmsOut* nms_entries(uint8_t* block) { return reinterpret_cast<PoseNmsOut*>(block + sizeof(PoseNmsHead)); }
 
+// k_pose_nms over n_frames frames, as PoseNmsParams.
+static int pose_nms_launch(const lm_pose_stage* s, int n_frames, const lm_match* surv, const int32_t* counts, const int32_t* frame_first,
+                           const uint8_t* posed, const IcpOut* outs, double thr, PoseNmsHead* head, PoseNmsOut* out, cudaStream_t st,
+                           int64_t* launches) {
+  PoseNmsParams p;
+  p.surv = surv; p.counts = counts; p.posed = posed; p.outs = outs;
+  p.rt = s->d_rt; p.class_begin = s->d_class_begin;
+  p.thr = thr;
+  p.head = head; p.out = out;
+  p.frame_first = frame_first;
+  k_pose_nms<<<n_frames, NMS_THREADS, 0, st>>>(p);
+  CUI(cudaGetLastError());
+  ++*launches;
+  return LM_OK;
+}
+
+// n kept poses e[] into the caller's arrays (out may be null).
+static void copy_kept(const PoseNmsOut* e, int n, lm_match* out, double* R_out, double* t_out, float* residual) {
+  for (int k = 0; k < n; ++k) {
+    if (out) out[k] = e[k].m;
+    memcpy(R_out + 9 * k, e[k].R, sizeof(e[k].R));
+    memcpy(t_out + 3 * k, e[k].t, sizeof(e[k].t));
+    residual[k] = e[k].residual;
+  }
+}
+
 int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32_t* d_counts, double thr, cudaStream_t st,
                            int64_t* launches) {
   if (s->bound > NMS_THREADS) return lm_fail(LM_E_STATE, "pose stage launched for %d survivors, the pose NMS takes %d", s->bound, NMS_THREADS);
@@ -1834,15 +1916,9 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
     CUI(cudaMalloc(&s->d_nms, bytes));
     CUI(cudaMallocHost(&s->h_nms, bytes));
   }
-  PoseNmsParams p;
-  p.surv = d_surv; p.counts = d_counts; p.posed = s->d_posed; p.outs = s->d_outs;
-  p.rt = s->d_rt; p.class_begin = s->d_class_begin;
-  p.thr = thr;
-  p.head = reinterpret_cast<PoseNmsHead*>(s->d_nms); p.out = nms_entries(s->d_nms);
-  p.frame_first = nullptr;
-  k_pose_nms<<<1, NMS_THREADS, 0, st>>>(p);
-  CUI(cudaGetLastError());
-  ++*launches;
+  int rc = pose_nms_launch(s, 1, d_surv, d_counts, nullptr, s->d_posed, s->d_outs, thr, reinterpret_cast<PoseNmsHead*>(s->d_nms),
+                           nms_entries(s->d_nms), st, launches);
+  if (rc) return rc;
   // the header and a first window of kept poses; the rest only if there are more
   CUI(cudaMemcpyAsync(s->h_nms, s->d_nms, sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_FIRST_FETCH, cudaMemcpyDeviceToHost, st));
   return LM_OK;
@@ -1850,25 +1926,19 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
 
 int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                           int64_t* n_out, int64_t* n_survivors, int64_t* n_posed) {
-  int rc = pose_status(s);
+  int rc = pose_status(s->h_err, 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
   if (rc) return rc;
   const PoseNmsHead h = *reinterpret_cast<const PoseNmsHead*>(s->h_nms);
   *n_out = h.kept;
   if (n_survivors) *n_survivors = h.survivors;
   if (n_posed) *n_posed = h.posed;
   if (h.kept > cap) return lm_fail(LM_E_CAPACITY, "%d poses kept, capacity %lld", h.kept, (long long)cap);
-  const PoseNmsOut* e = nms_entries(s->h_nms);
   if (h.kept > NMS_FIRST_FETCH) {
     CUI(cudaMemcpyAsync(nms_entries(s->h_nms) + NMS_FIRST_FETCH, nms_entries(s->d_nms) + NMS_FIRST_FETCH,
                         sizeof(PoseNmsOut) * (size_t)(h.kept - NMS_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
   }
-  for (int k = 0; k < h.kept; ++k) {
-    if (out) out[k] = e[k].m;
-    memcpy(R_out + 9 * k, e[k].R, sizeof(e[k].R));
-    memcpy(t_out + 3 * k, e[k].t, sizeof(e[k].t));
-    residual[k] = e[k].residual;
-  }
+  copy_kept(nms_entries(s->h_nms), h.kept, out, R_out, t_out, residual);
   return LM_OK;
 }
 
@@ -1941,13 +2011,12 @@ static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S) {
 }
 
 int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4) {
-  cudaStream_t st = b.stream;
+  const PoseOptions& o = b.o;
+  cudaStream_t st = o.stream;
   const int nf = b.n_frames;
   const int64_t S = b.first[nf];
-  const PoseShare* sh = b.share;
+  const PoseShare* sh = o.share;
   const int nc = pose_batch_chunks(S);
-  const bool normals = b.estimation == LM_ICP_POINT_TO_PLANE;
-  const int chunk_launches = (sh ? 6 : 5) - (normals ? 0 : 1);
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
@@ -1956,102 +2025,43 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
   if (rc) return rc;
   rc = pose_buffers(s, st, (int)std::min<int64_t>(std::max<int64_t>(S, 1), POSE_BATCH_CHUNK), s->area_max);
   if (rc) return rc;
-  const int64_t A = s->cap_area;
   std::vector<int32_t> frame_of((size_t)S);
   for (int f = 0; f < nf; ++f)
     for (int64_t k = b.first[f]; k < b.first[f + 1]; ++k) frame_of[(size_t)k] = f;
   std::vector<int32_t> first32(b.first, b.first + nf + 1);
+  // per chunk a status block (PoseChunk), [3] the chunk's size
+  std::vector<int32_t> stat((size_t)4 * nc, 0);
+  for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_BATCH_CHUNK, POSE_BATCH_CHUNK);
   if (S) CUI(cudaMemcpyAsync(s->d_bframe, frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
   CUI(cudaMemcpyAsync(s->d_bfirst, first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
   CUI(cudaMemcpyAsync(s->d_bsK, b.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
-  if (sh && nc) {
-    std::vector<int32_t> stat((size_t)4 * nc, 0);
-    for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_BATCH_CHUNK, POSE_BATCH_CHUNK);
-    CUI(cudaMemcpyAsync(s->d_bstat, stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
-  }
-  for (int64_t c0 = 0; c0 < S; c0 += POSE_BATCH_CHUNK) {
-    const int C = (int)std::min<int64_t>(S - c0, POSE_BATCH_CHUNK);
-    const int c = (int)(c0 / POSE_BATCH_CHUNK);
-    // shared: this rank refines chunk survivors rank, rank + world, ... in n slots; a rank without one still publishes
-    const int n = sh ? (C + sh->world - 1) / sh->world : C;
-    int32_t* stat = sh ? s->d_bstat + 4 * c : nullptr;
-    PoseParams p;
-    p.surv = s->d_bsurv + c0; p.counts = sh ? stat + 3 : nullptr;
-    p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
-    p.tpl = s->d_tpl; p.crops = s->d_crops;
-    p.scene = s->d_bscene; p.srows = b.srows; p.scols = b.scols;
-    memset(p.sK, 0, sizeof(p.sK));
-    p.A = (int32_t)A; p.use_scene = b.use_scene_cloud ? 1 : 0;
-    p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
-    p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * n;
-    p.jobs = s->d_jobs; p.err = sh ? stat : s->d_err; p.posed = sh ? s->d_posed : s->d_bposed + c0;
-    p.frame_of = s->d_bframe + c0; p.sKs = s->d_bsK;
-    p.rank = sh ? sh->rank : 0; p.world = sh ? sh->world : 1;
-    if (sh) k_pose_cloud_batch_share<<<n, POSE_THREADS, 0, st>>>(p);
-    else k_pose_cloud_batch<<<C, POSE_THREADS, 0, st>>>(p);
-    cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
-    cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
-    size_t tmp_bytes = s->sort_tmp_bytes;
-    CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * n * A), 2 * n, p.seg_begin, p.seg_end, 0,
-                                                 3 * POSE_KEY_BITS, st));
-    k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
-                                                 p.use_scene);
-    if (normals) {
-      dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
-      k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
-    }
-    if (sh) {
-      // exchange seq + c: the results travel to every rank; the collector gathers the chunk in survivor order
-      const PoseShareDev sd = share_dev(*sh, sh->seq + c, stat + 3, s->d_posed, stat);
-      launch_icp<true>(b.estimation, n, st, s->d_jobs, s->d_pts, s->d_nrm, nullptr, b.max_iterations, nullptr, sd);
-      k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, s->d_bouts + c0, s->d_bposed + c0);
-    } else {
-      launch_icp<false>(b.estimation, C, st, s->d_jobs, s->d_pts, s->d_nrm, s->d_bouts + c0, b.max_iterations, nullptr, PoseShareDev());
-    }
-    CUI(cudaGetLastError());
-    *launches += chunk_launches;
+  if (nc) CUI(cudaMemcpyAsync(s->d_bstat, stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  int64_t stage_launches = 0;
+  for (int c = 0; c < nc; ++c) {
+    const int64_t c0 = (int64_t)c * POSE_BATCH_CHUNK;
+    PoseChunk k;
+    k.surv = s->d_bsurv + c0; k.counts = s->d_bstat + 4 * c + 3; k.slots = stat[(size_t)4 * c + 3];
+    k.scene = s->d_bscene; k.frame_of = s->d_bframe + c0; k.sKs = s->d_bsK; k.sK = nullptr;
+    k.outs = s->d_bouts + c0; k.posed = s->d_bposed + c0; k.status = s->d_bstat + 4 * c; k.seq = sh ? sh->seq + c : 0;
+    const int l = pose_chunk(s, o, k);
+    if (l < 0) return l;
+    stage_launches += l;
+    *launches += l;
   }
   if (b.pose_nms) {
-    PoseNmsParams p;
-    p.surv = s->d_bsurv; p.counts = nullptr; p.posed = s->d_bposed; p.outs = s->d_bouts;
-    p.rt = s->d_rt; p.class_begin = s->d_class_begin;
-    p.thr = b.thr;
-    p.head = s->d_bhead; p.out = s->d_bnms;
-    p.frame_first = s->d_bfirst;
-    k_pose_nms_batch<<<nf, NMS_THREADS, 0, st>>>(p);
-    CUI(cudaGetLastError());
-    ++*launches;
+    rc = pose_nms_launch(s, nf, s->d_bsurv, nullptr, s->d_bfirst, s->d_bposed, s->d_bouts, b.thr, s->d_bhead, s->d_bnms, st, launches);
+    if (rc) return rc;
     CUI(cudaMemcpyAsync(s->h_bhead, s->d_bhead, sizeof(PoseNmsHead) * nf, cudaMemcpyDeviceToHost, st));
   } else if (S) {
     CUI(cudaMemcpyAsync(s->h_bouts, s->d_bouts, sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
   }
-  CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  if (sh && nc) CUI(cudaMemcpyAsync(s->h_bstat, s->d_bstat, sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  if (nc) CUI(cudaMemcpyAsync(s->h_bstat, s->d_bstat, sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
-  // shared: the overflow and late flags are ORed, the published entries summed over the chunks
-  int32_t overflow = *s->h_err, late = -1;
-  int64_t refined = S;
-  if (sh) {
-    refined = 0;
-    for (int c = 0; c < nc; ++c) {
-      overflow |= s->h_bstat[4 * c];
-      if (s->h_bstat[4 * c + 1] && late < 0) late = c;
-      refined += s->h_bstat[4 * c + 2];
-    }
-  }
-  if (late >= 0)
-    return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d (chunk %d of the batch) within %llu ms "
-                   "(or an earlier collector on this device already gave up); every rank must run every batch while sharing is on",
-                   sh->seq + late, late, sh->timeout_ns / 1000000ull);
-  if (overflow) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
-  if (stats4) {
-    stats4[0] = S;
-    stats4[1] = refined;
-    stats4[2] = (int64_t)nc * chunk_launches;
-    stats4[3] = sh ? 1 : 0;
-  }
+  int64_t published = 0;
+  rc = pose_status(s->h_bstat, nc, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0, true, &published);
+  if (rc) return rc;
+  if (stats4) pose_stats(stats4, S, sh != nullptr, published, stage_launches);
   if (b.pose_nms) {
     // the kept poses of every frame, each range where its frame's survivors begin
     bool more = false;
@@ -2066,17 +2076,13 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
     if (more) CUI(cudaStreamSynchronize(st));
     return LM_OK;
   }
-  const int n_classes = (int)s->class_begin.size() - 1;
   for (int f = 0; f < nf; ++f) {
     posed[f] = 0;
     kept[f] = b.first[f + 1] - b.first[f];
     for (int64_t i = b.first[f]; i < b.first[f + 1]; ++i) {
-      const lm_match& m = b.surv[i];
-      const int64_t g = (m.class_index >= 0 && m.class_index < n_classes) ? (int64_t)s->class_begin[m.class_index] + m.template_id : -1;
-      if (g < 0 || g >= (int64_t)s->tpl.size() || !s->tpl[(size_t)g].set)
-        return lm_fail(LM_E_STATE, "frame %d, survivor %lld: template without a registered render", f, (long long)(i - b.first[f]));
-      const TplHost& h = s->tpl[(size_t)g];
-      if (!(m.x + h.box[2] >= b.scols || m.y + h.box[3] >= b.srows)) ++posed[f];  // LL.cpp:52-55
+      const TplHost* h = survivor_render(s, b.surv[i]);
+      if (!h) return lm_fail(LM_E_STATE, "frame %d, survivor %lld: template without a registered render", f, (long long)(i - b.first[f]));
+      if (survivor_fits(*h, b.surv[i], o.srows, o.scols)) ++posed[f];
     }
   }
   return LM_OK;
@@ -2085,25 +2091,14 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
 void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual) {
   const int64_t first = b.first[f], n = b.first[f + 1] - first;
   if (b.pose_nms) {
-    const PoseNmsOut* e = s->h_bnms + first;
-    for (int k = 0; k < s->h_bhead[f].kept; ++k) {
-      out[k] = e[k].m;
-      memcpy(R_out + 9 * k, e[k].R, sizeof(e[k].R));
-      memcpy(t_out + 3 * k, e[k].t, sizeof(e[k].t));
-      residual[k] = e[k].residual;
-    }
+    copy_kept(s->h_bnms + first, s->h_bhead[f].kept, out, R_out, t_out, residual);
     return;
   }
-  // as pose_stage_finish: compose on the host, early returns keep R / t untouched
   for (int64_t i = 0; i < n; ++i) {
     const lm_match& m = b.surv[first + i];
     out[i] = m;
-    const TplHost& h = s->tpl[(size_t)(s->class_begin[m.class_index] + m.template_id)];  // pose_batch_run checked it
-    if (m.x + h.box[2] >= b.scols || m.y + h.box[3] >= b.srows) { residual[i] = -1.f; continue; }  // LL.cpp:52-55
-    float base[16];
-    init_base(h.R, h.t, base);
-    compose(s->h_bouts[first + i].T, base, R_out + 9 * i, t_out + 3 * i);
-    residual[i] = (float)s->h_bouts[first + i].fitness;
+    survivor_pose(*survivor_render(s, m), m, b.o.srows, b.o.scols, s->h_bouts[first + i], R_out + 9 * i, t_out + 3 * i,
+                  residual + i);  // pose_batch_run checked the render
   }
 }
 

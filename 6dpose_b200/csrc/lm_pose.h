@@ -24,11 +24,12 @@ int pose_stage_register(lm_pose_stage* s, const int32_t* class_begin, int n_clas
 // Every template of the selection has a render.
 bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel);
 
-// The pose stage shared over the ranks of the peer exchange (lm_peer_share_pose).  Survivor i (pick order of k_post_nms,
-// the same on every rank) is refined by rank i % world: this rank's launches are sized for ceil(bound / world) slots,
-// slot j takes survivor rank + j * world.  The ICP kernel's SHARE instantiation stores each survivor's result into the pose area
-// of every rank's exchange buffer and raises this rank's pose flag there; k_pose_collect waits for the world flags in
-// this rank's buffer and gathers the results in survivor order into the stage's own outputs, so pose_stage_finish and
+// A frame's pose stage is one chunk of survivors, a batch's one chunk per 1024 survivors.  Slot j of a chunk takes
+// survivor rank + j * world, so the launches are sized for ceil(survivors / world) slots; unshared, rank 0 and world 1.
+// Shared over the ranks of the peer exchange (lm_peer_share_pose), survivor i (pick order of k_post_nms, the same on
+// every rank) is thus refined by rank i % world.  The ICP kernel's SHARE instantiation stores each survivor's result into
+// the pose area of every rank's exchange buffer and raises this rank's pose flag there; k_pose_collect waits for the
+// world flags in this rank's buffer and gathers the results in survivor order into the chunk's outputs, so the host and
 // the pose NMS read what the unshared stage leaves.  The pose area: [2 slots][1024 survivors] entries of 160 bytes,
 // then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket (pose_share_area_bytes in all).  Each pose exchange -- a
 // shared frame, or one chunk of a shared batch -- has its own number on the detector's pose counter.
@@ -42,18 +43,21 @@ struct PoseShare {
 };
 size_t pose_share_area_bytes();
 
-struct PoseEnqueue {
-  const lm_match* d_surv;     // survivors in pick order (k_post_nms output)
-  const int32_t* d_counts;    // [0] = survivors written
-  const uint16_t* d_scene;    // scene depth, srows x scols u16 mm
-  int srows, scols;
-  float sK[9];
-  int bound;                  // survivors the launches are sized for (top_k, or every survivor k_post_nms may write)
-  int use_scene_cloud;
-  int max_iterations;
+// What a frame's and a batch's pose stage share.
+struct PoseOptions {
+  int srows, scols;           // scene depth size
+  int use_scene_cloud, max_iterations;
   int estimation;             // LM_ICP_POINT_TO_PLANE (k_icp_normals + k_icp_point_to_plane) or LM_ICP_POINT_TO_POINT
   cudaStream_t stream;
   const PoseShare* share;     // null: this rank refines every survivor
+};
+struct PoseEnqueue {
+  PoseOptions o;
+  const lm_match* d_surv;     // survivors in pick order (k_post_nms output)
+  const int32_t* d_counts;    // [0] = survivors written
+  const uint16_t* d_scene;    // scene depth, srows x scols u16 mm
+  float sK[9];
+  int bound;                  // survivors the launches are sized for (top_k, or every survivor k_post_nms may write)
 };
 int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches);
 // After pose_stage_finish / pose_stage_finish_nms of a frame with n survivors: what lm_pose_stats returns (survivors,
@@ -80,22 +84,17 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
 // Chunks of the pose stage of a batch with S survivors (each of at most 1024 slots).
 int pose_batch_chunks(int64_t S);
 struct PoseBatch {
-  int n_frames, srows, scols;
+  PoseOptions o;              // shared: chunk c is pose exchange o.share->seq + c
+  int n_frames;
   const int64_t* first;       // [n_frames + 1] survivor offsets (host)
   const lm_match* surv;       // host copy of the survivors (pose_nms == 0 only)
   const float* sK;            // [n_frames][9]
-  int use_scene_cloud, max_iterations;
-  int estimation;             // as PoseEnqueue
-  int pose_nms;               // 1: the pose NMS per frame (k_pose_nms_batch), 0: the host composes the poses
+  int pose_nms;               // 1: the pose NMS per frame (one CTA each), 0: the host composes the poses
   double thr;
-  cudaStream_t stream;
-  const PoseShare* share;     // null: this rank refines every survivor; else chunk c is pose exchange share->seq + c
 };
-// The pose stage over every survivor of the batch in chunks of at most 1024 slots, then (pose_nms) one pose NMS launch
-// for all frames; waits.  posed[f] / kept[f]: frame f's survivors with a pose, and its entries (kept poses, or every
-// survivor without the pose NMS).  Shared: within a chunk of C survivors, survivor i is refined by rank i % world in
-// ceil(C / world) slots (k_pose_cloud_batch_share, the ICP kernel's SHARE instantiation), and k_pose_collect gathers the chunk
-// into the batch's outputs.  stats4 (may be null): what lm_pose_stats returns for the batch.
+// The pose stage over every survivor of the batch in chunks of at most 1024 survivors, then (pose_nms) one pose NMS
+// launch for all frames; waits.  posed[f] / kept[f]: frame f's survivors with a pose, and its entries (kept poses, or
+// every survivor without the pose NMS).  stats4 (may be null): what lm_pose_stats returns for the batch.
 int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4);
 // Frame f's kept[f] entries after pose_batch_run, outputs as lm_complete_detect (pose_nms) or lm_complete_pose.
 void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual);

@@ -12,7 +12,7 @@
 # chunks, and one with early returns and NaN anchors, and (e) the pose stage shared over two handles of one process (peer
 # stores of the ICP kernel, its ticket and pose flags, the pose collector's spin wait), and (f) memcheck over
 # lm_peer_detect_batch with three handles of one process: a shared batch of two pose chunks, one with fewer survivors
-# than ranks and an all-blank one (k_pose_cloud_batch_share, the per-chunk pose exchanges).
+# than ranks and an all-blank one (k_pose_cloud's slot and frame indexing of a shared chunk, the per-chunk pose exchanges).
 # Usage (on a GPU box):  bash tools/sanitize.sh [outdir]      -> <outdir>/summary.txt, one log per tool x case
 set -u
 OUT=${1:-gpurun_out/sanitize}
