@@ -27,7 +27,7 @@ PEER_HANDLE_BYTES = 64
 SYMBOLS = [
     "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks", "lm_coarse_descriptors",
     "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device",
-    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
+    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_debug_plan", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
@@ -285,6 +285,7 @@ def load():
     L.lm_detect_batch_device.argtypes = [vp, c_int, ctypes.POINTER(vp), c_i64, ctypes.POINTER(vp), c_i64, c_int, c_f, c_int, c_int,
                                          ctypes.POINTER(vp), c_i64, vp] + L.lm_detect_batch.argtypes[7:]
     L.lm_debug_depth.argtypes = [vp, u16p, c_i64]
+    L.lm_debug_plan.argtypes = [vp, i32p, c_i64]
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -856,6 +857,16 @@ class NativeDetector:
         keys = ["templates", "coarse_candidates", "scan_bytes", "refine_bytes", "kept", "refine_bytes_read",
                 "filter_dropped_bytes", "filter_bytes_read"]
         return dict(zip(keys, [int(v) for v in a]))
+
+    PLAN_KEYS = ["k1_band", "planes_level", "pseg", "k1_smem", "rounds", "bit_planes", "packed_templates", "byte_templates",
+                 "k2_smem", "split", "plane_bytes", "k2_tasks", "filter_ok", "use_bits", "filter_templates", "gated",
+                 "filter_items", "refine_bits_items", "refine_filtered_items", "refine_items"]
+
+    def plan(self):
+        """The kernels and launch shapes of the last run (lm_debug_plan); -1: that kernel did not run."""
+        a = np.zeros(len(self.PLAN_KEYS), np.int32)
+        check(self._L.lm_debug_plan(self._h, self._i32(a), a.size))
+        return dict(zip(self.PLAN_KEYS, [int(v) for v in a]))
 
     def set_timing(self, slots):
         check(self._L.lm_set_timing(self._h, int(slots)))

@@ -2686,6 +2686,57 @@ extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality,
   return LM_OK;
 }
 
+// The routes of the last lm_run, restated from the host state enqueue_stages decided them from (plan_k1, coarse_shape,
+// use_filter / use_bits); only the survivor counts of the filter are read back from the device, behind whatever the
+// stream holds (a frame enqueued since the last lm_complete would be waited for and reported: see the header).
+extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
+  if (!d || !out) return fail(LM_E_INVALID, "null argument");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
+  if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
+  if (cap < LM_PLAN_ENTRIES) return fail(LM_E_CAPACITY, "need %d entries", LM_PLAN_ENTRIES);
+  CU(cudaSetDevice(d->device));
+  int queue[4];
+  CU(cudaMemcpyAsync(queue, d->d_queue, sizeof(queue), cudaMemcpyDeviceToHost, d->stream));
+  CU(cudaStreamSynchronize(d->stream));
+  const LevelHost& low = d->lv[d->L - 1];
+  K1Plan k1;
+  plan_k1(d, planes_level(d), true, k1);
+  const int pl = k1.band ? planes_level(d) : -1;
+  for (int i = 0; i < LM_PLAN_ENTRIES; ++i) out[i] = -1;
+  out[0] = k1.band ? 1 : 0;
+  out[1] = pl;
+  out[2] = pl >= 0 ? k1.p.lv[pl].pseg : 0;
+  out[3] = (int32_t)k1.smem;
+  out[4] = low.rounds;
+  out[5] = low.d_bp ? 1 : 0;
+  out[6] = d->n_items_bits;
+  out[7] = d->n_items_bytes;
+  if (d->n_items_bits > 0) {
+    const size_t plane_bytes = ((size_t)d->M * 8 * low.lbw * 4 + 15) & ~(size_t)15;
+    const CoarseShape c = coarse_shape(d->k2_tasks, d->sm_count, plane_bytes);
+    out[8] = c.smem ? 1 : 0;
+    out[9] = c.split;
+    out[10] = (int32_t)plane_bytes;
+    out[11] = d->k2_tasks;
+  }
+  out[12] = d->filter_ok ? 1 : 0;
+  out[13] = use_bits(d) ? 1 : 0;
+  int eligible = 0;
+  for (const int4& f : d->h_finfo) eligible += (f.w & 2) ? 1 : 0;
+  out[14] = eligible;
+  out[15] = d->gate_frame ? 1 : 0;
+  // work items of the refinement kernels that ran (-1: it did not run); see enqueue_stages
+  const int total = (int)std::min<int64_t>(d->h_res->coarse_candidates, d->cand_cap);
+  const bool filter = use_filter(d), bits_mode = use_bits(d);
+  if (filter) out[16] = total;
+  if (bits_mode) out[17] = std::min(queue[1], total);
+  if (!bits_mode || !d->shard_all_eligible) {
+    if (filter) out[18] = std::min(queue[bits_mode ? 2 : 1], total);
+    else out[19] = total;
+  }
+  return LM_OK;
+}
+
 extern "C" int lm_counters(lm_detector* d, int64_t* out8) {
   if (!d || !out8) return fail(LM_E_INVALID, "null argument");
   if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");

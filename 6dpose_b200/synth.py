@@ -101,12 +101,13 @@ def _coherent_labels(rng, H, W, p_nonzero, label_block, salt, mask_block):
     return np.where(on, 1 << img, 0).astype(np.uint8)
 
 
-def synth_frame(W=640, H=480, levels=2, seed=42, bank=None, plant=8, T=(4, 8)):
+def synth_frame(W=640, H=480, levels=2, seed=42, bank=None, plant=8, T=(4, 8), border=None):
     """Quantized pyramid [[colour, normals] per level] + list of planted (class_id, template_id, x, y).
 
     Level l+1 is the nearest-neighbour decimation of level l (what DepthNormalPyramid::pyrDown does,
     LL.cpp:865-868).  Planted templates are written at every level so both the coarse scan and the
-    refinement see a 100 % match."""
+    refinement see a 100 % match.  Plants keep `border` pixels (default 8 * T[0]) from the frame's edges;
+    small frames at large T need a smaller border to take any."""
     rng = np.random.default_rng(seed)
     q = [[_coherent_labels(rng, H, W, 0.485, 16, 0.04, 2), _coherent_labels(rng, H, W, 0.91, 48, 0.02, 16)]]
     for l in range(1, levels):
@@ -114,7 +115,7 @@ def synth_frame(W=640, H=480, levels=2, seed=42, bank=None, plant=8, T=(4, 8)):
     planted = []
     if bank is not None and plant > 0:
         cids = bank.class_ids()
-        border = 8 * T[0]
+        border = 8 * T[0] if border is None else border
         for k in range(plant):
             cid = cids[k % len(cids)]
             tps = bank.classes[cid]

@@ -471,6 +471,22 @@ int lm_debug_quantized(lm_detector* d, int level, int modality, uint8_t* out, in
 int lm_debug_depth(lm_detector* d, uint16_t* out, int64_t cap);
 /* Linear memories of (level, modality) of the last lm_run: [8][T*T][(cols/T)*(rows/T)] bytes. */
 int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap);
+/* Test getter: which kernels and launch shapes the last lm_run took, restated from the host state the frame was
+ * enqueued from (no launch; one small read of the filter's survivor counts).  LM_PLAN_ENTRIES int32 entries:
+ * [0] linear memories by k_linear_memories_band (1) or k_linear_memories (0), [1] level built as H-planes only (-1:
+ * none), [2] its positions per segment (pseg; 0: none), [3] the band kernel's shared memory (bytes), [4] rounds of
+ * 32 x 32 position words at the lowest level, [5] its spread bit-planes are allocated (1/0), [6] templates on
+ * k_coarse_packed, [7] templates on k_coarse_bytes, [8] k_coarse_packed stages the bit-planes in shared memory (1/0),
+ * [9] its team split S, [10] bit-plane bytes, [11] its tasks ([8]..[11]: -1 without packed templates),
+ * [12] the refinement filter is available for the frame size (1/0), [13] bit-sliced refinement (two levels, 1/0),
+ * [14] templates of the shard the filter takes, [15] the frame ran depth-gated (1/0), then the work items of
+ * [16] k_refine_filter_w, [17] k_refine_bits, [18] k_refine<true>, [19] k_refine<false> (-1: it did not run).
+ * Describes the last completed frame only between lm_complete (or lm_run) and the next lm_enqueue, and while the bank,
+ * the selection, the frame size and the gate stay as they were: the routes are restated from the current host state, and
+ * the survivor counts are read from the device when the getter is called, so after a later lm_enqueue the getter waits
+ * for that frame and reports its counts. */
+#define LM_PLAN_ENTRIES 20
+int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap);
 /* Counters of the last lm_run: [0] templates scanned, [1] coarse candidates, [2] algorithmic bytes of
  * the coarse scan (sum over templates, modalities of features x positions; SURVEY 8d),
  * [3] algorithmic bytes of the refinement (features x 256 per refined candidate and level: the reference's work,

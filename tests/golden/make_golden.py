@@ -147,6 +147,31 @@ def make_reference_checks():
     open(os.path.join(OUT, "bank_127_first_pyramid.yaml"), "w").write("\n".join(lines[:second]) + "\n")
 
 
+def make_shape_checks():
+    """shape_checks.npz: the compiled reference's match lists on SHAPE_CASES (tests/match_shapes.py) -- small frames at
+    the pyramid steps T the other fixtures do not reach (every T of 1..16 at the lowest level, 1..8 at the refined
+    ones, three and four levels), so that the oracle is pinned wherever tests/test_gpu_match_shapes.py holds the GPU to
+    it.  Plus the case list itself, as JSON."""
+    import json
+    sys.path.insert(0, os.path.dirname(OUT))
+    import match_shapes as ms
+    synth = importlib.import_module("6dpose_b200.synth")
+    from oracle import oracle, ref
+    assert ref.build()
+    out = {"cases": np.asarray(json.dumps(ms.SHAPE_CASES))}
+    for i, (T, W, H, n, nf, size, thr) in enumerate(ms.SHAPE_CASES):
+        ms.frame_shape(T, W, H)
+        assert ms.reference_can_run(T, W), "the compiled reference faults at %s %dx%d" % (T, W, H)
+        packed, q, planted = ms.shape_case_data(synth, T, W, H, n, nf, size, thr)
+        assert not ms.reference_overreads(T, W, H, packed), "the compiled reference reads out of bounds at %s %dx%d" % (T, W, H)
+        want = ref.match(q, T, packed, thr)
+        assert len(planted) > 0 and len(want) > 0, (T, W, H)
+        assert np.array_equal(want, oracle.match(q, T, packed, thr)), "restatement and reference disagree at %s %dx%d" % (T, W, H)
+        out["case_%d" % i] = want
+        print(T, W, H, len(want), want[:1])
+    np.savez_compressed(os.path.join(OUT, "shape_checks.npz"), **out)
+
+
 if __name__ == "__main__":
     make_train_golden()
     make_reference_checks()
@@ -155,3 +180,4 @@ if __name__ == "__main__":
     rgb = cv2.imread(CASE + "0000_rgb.png")
     dep = cv2.imread(CASE + "0000_dep.png", cv2.IMREAD_UNCHANGED)
     np.savez_compressed(os.path.join(OUT, "frame_crop_case1.npz"), rgb=rgb[40:360, 200:600].copy(), dep=dep[40:360, 200:600].copy())
+    make_shape_checks()

@@ -133,3 +133,37 @@ def test_cuda_path_reproduces_the_full_allscales_golden_vectors():
             assert np.array_equal(got[k], want[k]), (tag, thr, k)
         c = nat.counters()
         assert [c["coarse_candidates"], c["scan_bytes"], c["refine_bytes"]] == stats.tolist(), (tag, thr)
+
+
+def test_shape_checks_list_is_current():
+    import match_shapes as ms
+    assert ms.stored_shape_cases() == [(T, W, H, n, nf, size, thr) for T, W, H, n, nf, size, thr in ms.SHAPE_CASES]
+
+
+def _shape_ids():
+    import match_shapes as ms
+    return ["%s-%dx%d" % ("_".join(map(str, c[0])), c[1], c[2]) for c in ms.SHAPE_CASES]
+
+
+@pytest.mark.parametrize("i", range(len(_shape_ids())), ids=_shape_ids())
+def test_oracle_equals_compiled_reference_at_new_shapes(oracle, synth, i):
+    """tests/golden/shape_checks.npz: the compiled reference's lists at every pyramid step T the GPU shape matrix runs."""
+    import match_shapes as ms
+    T, W, H, n, nf, size, thr = ms.SHAPE_CASES[i]
+    ms.frame_shape(T, W, H)
+    packed, q, planted = ms.shape_case_data(synth, T, W, H, n, nf, size, thr)
+    # the stored list is the reference's defined result only where it reads nothing past its linear memories
+    assert ms.reference_can_run(T, W) and not ms.reference_overreads(T, W, H, packed)
+    want = np.load(ms.SHAPE_CHECKS)["case_%d" % i]
+    assert len(planted) > 0 and len(want) > 0
+    assert np.array_equal(oracle.match(q, T, packed, thr), want)
+
+
+def test_reference_overreads_at_t1_with_features_on_the_template_side(synth):
+    """What shape_case_data avoids at T = 1: synth_bank puts a feature at x = width (cropTemplates' extent), and the
+    reference's coarse scan then reads past the last grid of its linear memories."""
+    import match_shapes as ms
+    bank = synth.synth_bank(6, num_features=32, levels=1, seed=21, size_range=((8, 32), (8, 32)))
+    over = ms.reference_overreads([1], 64, 64, bank.pack(bank.class_ids(), 2))
+    assert over and max(o[3] for o in over) > 0
+    assert not ms.reference_overreads([2], 64, 64, bank.pack(bank.class_ids(), 2))
