@@ -20,6 +20,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -58,6 +59,7 @@ int lm_fail(int code, const char* fmt, ...) {
 #include "lm_frontend.cuh"
 #include "lm_post.cuh"
 #include "lm_pose.h"
+#include "lm_buffer.h"
 
 // Launch with programmatic stream serialization (see lm_pdl_wait in lm_kernels.cuh).
 template <typename... KArgs, typename... Args>
@@ -84,12 +86,11 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 
 struct LevelHost {
   int T = 0, rows = 0, cols = 0, Wd = 0, Hd = 0, plane = 0;
-  uint8_t* d_q[LM_MAX_MODALITIES] = {nullptr, nullptr};           // owned upload buffers
+  DeviceArray<uint8_t> d_q[LM_MAX_MODALITIES];                   // owned upload buffers
   const uint8_t* q_src[LM_MAX_MODALITIES] = {nullptr, nullptr};  // what K1 reads (owned or caller's device memory)
-  uint8_t* d_lm = nullptr;
-  size_t lm_bytes = 0;
+  DeviceArray<uint8_t> d_lm;
   uint32_t mod_stride = 0;
-  uint32_t* d_bp = nullptr;  // lowest level only: spread bit-planes [M][8][lbw]
+  DeviceArray<uint32_t> d_bp;  // lowest level only: spread bit-planes [M][8][lbw]
   int lbw = 0, nwords = 0, rounds = 0;
 };
 
@@ -103,11 +104,15 @@ static size_t bp_label_words(int T, int plane) {
 
 struct lm_detector {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  // streams and events first: they outlive the buffers, which are freed in reverse order of declaration
+  Stream stream;
   // host uploads: the upper-level label images travel on a second stream while the lowest level's linear
   // memories and the coarse scan already run (they only need the lowest level)
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_upper = nullptr;
+  Stream copy_stream;
+  Event ev_fork, ev_upper;
+  // lm_bind_images_device: the caller's stream up to the call -> the ingest -> the caller's stream after it
+  Event ev_in, ev_out;
+  std::vector<Event> tev;  // timing slots x LM_TEV events (ring)
   bool upper_pending = false;
   int L = 0, M = LM_MAX_MODALITIES;
   int T[LM_MAX_LEVELS] = {0};
@@ -119,34 +124,34 @@ struct lm_detector {
   std::vector<int32_t> class_begin, tmeta, feats;
   std::vector<uint8_t> feat_slot;  // slot (level*M+modality) of every feature
   // bank (device), prepared for the current frame size
-  TSlot* d_tslot = nullptr;
-  uint32_t* d_fbase = nullptr;
-  uint32_t* d_fxy = nullptr;
-  uint32_t* d_fdesc = nullptr;       // lowest-level features for k_coarse_packed, one word each (coarse_descriptors)
-  int2* d_k2info = nullptr;          // [G]: first descriptor, lowest-level features
+  DeviceArray<TSlot> d_tslot;
+  DeviceArray<uint32_t> d_fbase;
+  DeviceArray<uint32_t> d_fxy;
+  DeviceArray<uint32_t> d_fdesc;     // lowest-level features for k_coarse_packed, one word each (coarse_descriptors)
+  DeviceArray<int2> d_k2info;        // [G]: first descriptor, lowest-level features
   std::vector<uint8_t> bits_ok;      // per template: the bit-sliced coarse kernel may take it
   std::vector<uint8_t> safe;         // per template: refinement never skips a feature (LL.cpp:1394)
-  uint8_t* d_safe = nullptr;
-  uint16_t* d_galign = nullptr;      // [G][S][16] feature counts per (address & 15) group
+  DeviceArray<uint8_t> d_safe;
+  DeviceArray<uint16_t> d_galign;    // [G][S][16] feature counts per (address & 15) group
   // refinement filter (k_refine_filter_w) on the first refined level lr = L - 2: column-major H-planes + descriptors
   bool filter_ok = false;            // the current frame size / bank allow it
   int last_planes_level = -1;        // level the last K1 built in planes mode (its byte linear memories are stale)
-  uint32_t* d_rp = nullptr; size_t rp_words = 0; int rp_nyb = 0;
-  uint32_t* d_rdesc = nullptr;       // per feature of level lr, grouped per template, padded to multiples of 32
-  uint8_t* d_rlab = nullptr;         // label per descriptor (8 = padding): k_refine_bits derives the neighbour planes
+  DeviceArray<uint32_t> d_rp; int rp_nyb = 0;
+  DeviceArray<uint32_t> d_rdesc;     // per feature of level lr, grouped per template, padded to multiples of 32
+  DeviceArray<uint8_t> d_rlab;       // label per descriptor (8 = padding): k_refine_bits derives the neighbour planes
   bool shard_all_eligible = false;   // every template of the shard is taken by the filter (no byte-wise refinement)
-  uint32_t* d_surv2 = nullptr;       // candidates of the templates the filter does not take
-  int2* d_rfeat = nullptr;           // per template: first descriptor, count
+  DeviceArray<uint32_t> d_surv2;     // candidates of the templates the filter does not take
+  DeviceArray<int2> d_rfeat;         // per template: first descriptor, count
   std::vector<int2> h_rfeat;
-  int4* d_finfo = nullptr;           // per work item of the shard: first descriptor, count, width | height << 16,
+  DeviceArray<int4> d_finfo;         // per work item of the shard: first descriptor, count, width | height << 16,
                                      // flags | need << 8 (need: for the threshold of the call, see filter_thresholds)
   std::vector<int4> h_finfo;         // .w = flags only
   std::vector<int4> h_finfo_up;      // upload staging
   bool finfo_valid = false; float finfo_threshold = 0.f;
-  uint2* d_cand = nullptr; int64_t cand_cap = 0;   // ordered candidate list (k_refine_prep)
+  DeviceArray<uint2> d_cand;         // ordered candidate list (k_refine_prep), cand_cap entries
   int64_t cand_need = 0;             // candidates of a frame that overflowed the list
-  uint32_t* d_surv = nullptr;        // survivors of the filter [cand_cap]
-  int* d_queue = nullptr;            // [0] next candidate, [1] survivors
+  DeviceArray<uint32_t> d_surv;      // survivors of the filter [cand_cap]
+  DeviceArray<int> d_queue;          // [0] next candidate, [1] survivors
   int prep_rows[LM_MAX_LEVELS] = {0}, prep_cols[LM_MAX_LEVELS] = {0};
   bool prepared = false;
   std::vector<TSlot> h_tslot;
@@ -159,24 +164,24 @@ struct lm_detector {
   int shard_layout = LM_SHARD_CONTIGUOUS;
   int64_t work_base = 0, work_stride = 1;    // entry w of the shard is sel[work_base + w * work_stride]
   std::vector<int32_t> shard_sel;            // global template ids of this shard, in order
-  int32_t* d_work = nullptr;
+  DeviceArray<int32_t> d_work;
   int n_items_bits = 0;                                     // work items per coarse kernel
-  int32_t* d_items_bytes = nullptr; int n_items_bytes = 0;
-  int2* d_k2task = nullptr;                                 // k_coarse_packed's task table of the shard (coarse_task_table)
+  DeviceArray<int32_t> d_items_bytes; int n_items_bytes = 0;
+  DeviceArray<int2> d_k2task;                               // k_coarse_packed's task table of the shard (coarse_task_table)
   int k2_full = 0, k2_rem = 0, k2_tasks = 0;                // full tasks, remainder words, all tasks
   bool work_dirty = true;
 
   // per-run buffers
-  uint32_t* d_mask = nullptr; size_t mask_elems = 0;  // [n_work][nwords] coarse pass bits
-  uint16_t* d_raw = nullptr; size_t raw_elems = 0;    // [n_work][plane] coarse raw scores (passing cells)
-  int32_t* d_cnt = nullptr; int32_t* d_off = nullptr; size_t cnt_elems = 0;
-  // result block (device): lm_result_header + capacity records; internal unless the caller set one
+  DeviceArray<uint32_t> d_mask;      // [n_work][nwords] coarse pass bits
+  DeviceArray<uint16_t> d_raw;       // [n_work][plane] coarse raw scores (passing cells)
+  DeviceArray<int32_t> d_cnt, d_off;
+  // result block (device): lm_result_header + capacity records (res_bytes); internal unless the caller set one
   lm_result_header* d_res = nullptr; int64_t res_cap = 0; bool res_external = false;
-  lm_result_header* d_res_own = nullptr; int64_t res_cap_own = 0;
-  unsigned long long* d_counters = nullptr;
-  unsigned long long* h_counters = nullptr;  // pinned
-  lm_result_header* h_res = nullptr; int64_t h_res_cap = 0;  // pinned staging: header + records
-  int64_t h_valid = 0;                                       // records already copied to h_res
+  DeviceArray<uint8_t> d_res_own;
+  DeviceArray<unsigned long long> d_counters;
+  PinnedArray<unsigned long long> h_counters;
+  PinnedArray<uint8_t> h_res;        // staging: header + records
+  int64_t h_valid = 0;               // records already copied to h_res
   float last_threshold = 0.f;
 
   std::vector<int> class_of;            // template -> class (lm_finish), rebuilt when the bank changes
@@ -186,10 +191,10 @@ struct lm_detector {
 
   // post-match stage (lm_post.cuh): greedy NMS on the device, top-k survivors to the host
   std::vector<int32_t> boxes;           // [G][2] caller's box sizes (empty: L0 template width/height)
-  PostInfo* d_post_info = nullptr; int64_t post_info_n = 0; bool post_dirty = true;
-  lm_match* d_post_out = nullptr; lm_match* h_post_out = nullptr;  // LM_POST_MAX survivors
-  int32_t* d_post_counts = nullptr; int32_t* h_post_counts = nullptr;
-  uint8_t* d_post_live = nullptr; int64_t post_live_cap = 0;
+  DeviceArray<PostInfo> d_post_info; bool post_dirty = true;
+  DeviceArray<lm_match> d_post_out; PinnedArray<lm_match> h_post_out;  // LM_POST_MAX survivors
+  DeviceArray<int32_t> d_post_counts; PinnedArray<int32_t> h_post_counts;
+  DeviceArray<uint8_t> d_post_live;
   bool post_pending = false, post_retry = false;
   double post_iou = 0.5; int post_top_k = 0;
 
@@ -205,7 +210,7 @@ struct lm_detector {
   int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
-  uint8_t* px_buf = nullptr;            // this rank's exchange buffer (IPC-exportable cudaMalloc)
+  DeviceArray<uint8_t> px_buf;          // this rank's exchange buffer (IPC-exportable device memory)
   int64_t px_cap = 0;                   // records per block
   int px_world = 0, px_rank = -1;       // px_rank >= 0: connected
   bool px_ipc = false;                  // peer bases opened with cudaIpcOpenMemHandle
@@ -214,19 +219,17 @@ struct lm_detector {
   unsigned long long px_timeout_ns = 1000000000ull;  // collector gives up on a peer after 1 s (LINEMOD_B200_PEER_TIMEOUT_MS)
   bool px_share_pose = false;           // lm_peer_share_pose: the pose stage is divided over the ranks
   int32_t px_pose_seq = 0;              // pose exchanges so far: one per shared frame, one per chunk of a shared batch
-  PeerExchange* d_px = nullptr;         // device copy of the descriptor (static after connect)
+  DeviceArray<PeerExchange> d_px;       // device copy of the descriptor (static after connect)
   PeerExchange h_px;
 
   // GPU quantization front-end (lm_upload_images): per level colour image, unfiltered bins, gate, normals, masks
   struct FeLevel {
     int rows = 0, cols = 0;
-    uint8_t* src = nullptr; uint8_t* qun = nullptr; uint8_t* strong = nullptr; uint8_t* normal = nullptr;
-    uint8_t* mask[LM_MAX_MODALITIES] = {nullptr, nullptr};
+    DeviceArray<uint8_t> src, qun, strong, normal;
+    DeviceArray<uint8_t> mask[LM_MAX_MODALITIES];
   } fe[LM_MAX_LEVELS];
-  uint16_t* fe_depth = nullptr; uint8_t* fe_nraw = nullptr;
+  DeviceArray<uint16_t> fe_depth; DeviceArray<uint8_t> fe_nraw;
   bool fe_lut = false;
-  // lm_bind_images_device: the caller's stream up to the call -> the ingest -> the caller's stream after it
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 
   // depth gate of the coarse scan (lm_set_depth_gate)
   std::vector<float> tdepth;            // training distance per template of the bank (mm; NaN / <= 0: never gated)
@@ -235,30 +238,26 @@ struct lm_detector {
   bool gate_dirty = true;               // h_gate_item no longer fits the shard / distances / tolerance
   std::vector<uint2> h_gate_item;       // per work item of the shard: band and sample-cell offset (DepthGate::item)
   int64_t gate_with_z = 0;              // work items of the shard with a distance
-  uint2* d_gate_item = nullptr; size_t gate_item_cap = 0;
-  uint32_t* d_cells = nullptr; size_t cells_cap = 0;
-  unsigned* d_gate_before = nullptr;
+  DeviceArray<uint2> d_gate_item;
+  DeviceArray<uint32_t> d_cells;
+  DeviceArray<unsigned> d_gate_before;
 
   bool timing = false;
-  std::vector<cudaEvent_t> tev;  // timing slots x LM_TEV events (ring)
   int64_t timing_runs = 0;
-  cudaEvent_t* ev = nullptr;     // the slot used by the run being enqueued
+  const Event* ev = nullptr;     // the tev slot used by the run being enqueued
   int64_t launches = 0;
   int64_t alg_scan_bytes = 0;
   int sm_count = 132;
+
+  ~lm_detector() { pose_stage_destroy(pose); }
 };
 
-static void free_level(LevelHost& l) {
-  for (int m = 0; m < LM_MAX_MODALITIES; ++m) {
-    if (l.d_q[m]) cudaFree(l.d_q[m]);
-    l.d_q[m] = nullptr;
-    l.q_src[m] = nullptr;
-  }
-  if (l.d_lm) cudaFree(l.d_lm);
-  l.d_lm = nullptr;
-  if (l.d_bp) cudaFree(l.d_bp);
-  l.d_bp = nullptr;
-}
+// A result block: lm_result_header, then records.
+static size_t res_bytes(int64_t records) { return sizeof(lm_result_header) + sizeof(lm_record) * (size_t)records; }
+static int64_t res_records(size_t bytes) { return bytes ? (int64_t)((bytes - sizeof(lm_result_header)) / sizeof(lm_record)) : 0; }
+static lm_result_header* hres(const lm_detector* d) { return reinterpret_cast<lm_result_header*>(d->h_res.get()); }
+// The candidate lists are allocated together, d_surv2 last: its size is theirs.
+static int64_t cand_cap(const lm_detector* d) { return (int64_t)d->d_surv2.size(); }
 
 extern "C" int lm_create(int device, int n_levels, const int* T, lm_detector** out) {
   if (!out) return fail(LM_E_INVALID, "out is null");
@@ -280,7 +279,7 @@ extern "C" int lm_create(int device, int n_levels, const int* T, lm_detector** o
     return fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
   if (device < 0 || device >= ndev) return fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
   CU(cudaSetDevice(device));
-  lm_detector* d = new lm_detector();
+  std::unique_ptr<lm_detector> d(new lm_detector());
   d->device = device;
   d->L = n_levels;
   for (int l = 0; l < n_levels; ++l) d->T[l] = T[l];
@@ -294,17 +293,17 @@ extern "C" int lm_create(int device, int n_levels, const int* T, lm_detector** o
   CU(cudaFuncSetAttribute(k_coarse_packed<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   CU(cudaFuncSetAttribute(k_coarse_packed<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LM_K2_SMEM_MAX));
   CU(cudaFuncSetAttribute(k_coarse_packed<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-  CU(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(&d->copy_stream, cudaStreamNonBlocking));
-  CU(cudaEventCreateWithFlags(&d->ev_fork, cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(&d->ev_upper, cudaEventDisableTiming));
-  CU(cudaMalloc(&d->d_counters, 8 * sizeof(unsigned long long)));
-  CU(cudaMemset(d->d_counters, 0, 8 * sizeof(unsigned long long)));
-  CU(cudaMallocHost(&d->h_counters, 8 * sizeof(unsigned long long)));
-  memset(d->h_counters, 0, 8 * sizeof(unsigned long long));
-  CU(cudaMalloc(&d->d_queue, 4 * sizeof(int)));
-  CU(cudaMemset(d->d_queue, 0, 4 * sizeof(int)));
-  *out = d;
+  CU(d->stream.create(cudaStreamNonBlocking));
+  CU(d->copy_stream.create(cudaStreamNonBlocking));
+  CU(d->ev_fork.create(cudaEventDisableTiming));
+  CU(d->ev_upper.create(cudaEventDisableTiming));
+  CU(d->d_counters.assign(8));
+  CU(cudaMemset(d->d_counters.get(), 0, 8 * sizeof(unsigned long long)));
+  CU(d->h_counters.assign(8));
+  memset(d->h_counters.get(), 0, 8 * sizeof(unsigned long long));
+  CU(d->d_queue.assign(4));
+  CU(cudaMemset(d->d_queue.get(), 0, 4 * sizeof(int)));
+  *out = d.release();
   return LM_OK;
 }
 
@@ -315,10 +314,8 @@ static void peer_release(lm_detector* d) {
   for (int r = 0; r < LM_MAX_PEERS; ++r) d->px_base[r] = nullptr;
   d->px_rank = -1;
   d->px_ipc = false;
-  if (d->px_buf) cudaFree(d->px_buf);
-  d->px_buf = nullptr;
-  if (d->d_px) cudaFree(d->d_px);
-  d->d_px = nullptr;
+  d->px_buf.reset();
+  d->d_px.reset();
   d->px_world = 0;
   d->px_cap = 0;
   d->px_share_pose = false;
@@ -326,38 +323,16 @@ static void peer_release(lm_detector* d) {
 
 extern "C" void lm_destroy(lm_detector* d) {
   if (!d) return;
-  if (d->device < 0) { pose_stage_destroy(d->pose); delete d; return; }
-  cudaSetDevice(d->device);
-  if (d->stream) cudaStreamSynchronize(d->stream);
-  peer_release(d);
-  for (int l = 0; l < LM_MAX_LEVELS; ++l) free_level(d->lv[l]);
-  cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc); cudaFree(d->d_k2info); cudaFree(d->d_work);
-  cudaFree(d->d_items_bytes); cudaFree(d->d_k2task); cudaFree(d->d_safe); cudaFree(d->d_galign);
-  cudaFree(d->d_mask); cudaFree(d->d_raw); cudaFree(d->d_cnt); cudaFree(d->d_off);
-  cudaFree(d->d_res_own); cudaFree(d->d_counters);
-  cudaFree(d->d_finfo); cudaFree(d->d_rlab); cudaFree(d->d_surv2);
-  cudaFree(d->d_rp); cudaFree(d->d_rdesc); cudaFree(d->d_rfeat); cudaFree(d->d_cand); cudaFree(d->d_surv); cudaFree(d->d_queue);
-  cudaFreeHost(d->h_counters); cudaFreeHost(d->h_res);
-  cudaFree(d->d_post_info); cudaFree(d->d_post_out); cudaFree(d->d_post_counts); cudaFree(d->d_post_live);
-  cudaFreeHost(d->h_post_out); cudaFreeHost(d->h_post_counts);
-  for (int l = 0; l < LM_MAX_LEVELS; ++l) {
-    cudaFree(d->fe[l].src); cudaFree(d->fe[l].qun); cudaFree(d->fe[l].strong); cudaFree(d->fe[l].normal);
-    cudaFree(d->fe[l].mask[0]); cudaFree(d->fe[l].mask[1]);
+  if (d->device >= 0) {
+    cudaSetDevice(d->device);
+    if (d->stream.get()) cudaStreamSynchronize(d->stream.get());
+    if (d->copy_stream.get()) cudaStreamSynchronize(d->copy_stream.get());
+    peer_release(d);
   }
-  cudaFree(d->fe_depth); cudaFree(d->fe_nraw);
-  cudaFree(d->d_gate_item); cudaFree(d->d_cells); cudaFree(d->d_gate_before);
-  pose_stage_destroy(d->pose);
-  for (cudaEvent_t e : d->tev) cudaEventDestroy(e);
-  if (d->copy_stream) { cudaStreamSynchronize(d->copy_stream); cudaStreamDestroy(d->copy_stream); }
-  if (d->ev_fork) cudaEventDestroy(d->ev_fork);
-  if (d->ev_upper) cudaEventDestroy(d->ev_upper);
-  if (d->ev_in) cudaEventDestroy(d->ev_in);
-  if (d->ev_out) cudaEventDestroy(d->ev_out);
-  if (d->stream) cudaStreamDestroy(d->stream);
   delete d;
 }
 
-extern "C" void* lm_stream(lm_detector* d) { return d ? (void*)d->stream : nullptr; }
+extern "C" void* lm_stream(lm_detector* d) { return d ? (void*)d->stream.get() : nullptr; }
 extern "C" int64_t lm_launch_count(lm_detector* d) { return d ? d->launches : 0; }
 
 extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_begin, int n_slots, const int32_t* tmeta,
@@ -403,12 +378,11 @@ extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_
   if (d->pose) pose_stage_clear(d->pose);  // so do the template renders
   d->feats.assign(feats, feats + (size_t)n_feats * 3);
   d->feat_slot.swap(slot_of);
-  cudaFree(d->d_tslot); cudaFree(d->d_fbase); cudaFree(d->d_fxy); cudaFree(d->d_fdesc); cudaFree(d->d_k2info);
-  d->d_tslot = nullptr; d->d_fbase = nullptr; d->d_fxy = nullptr; d->d_fdesc = nullptr; d->d_k2info = nullptr;
-  if (d->device >= 0 && G > 0) CU(cudaMalloc(&d->d_tslot, sizeof(TSlot) * (size_t)G * n_slots));
+  d->d_tslot.reset(); d->d_fbase.reset(); d->d_fxy.reset(); d->d_fdesc.reset(); d->d_k2info.reset();
+  if (d->device >= 0 && G > 0) CU(d->d_tslot.assign((size_t)G * n_slots));
   if (d->device >= 0 && n_feats > 0) {
-    CU(cudaMalloc(&d->d_fbase, sizeof(uint32_t) * (size_t)n_feats));
-    CU(cudaMalloc(&d->d_fxy, sizeof(uint32_t) * (size_t)n_feats));
+    CU(d->d_fbase.assign((size_t)n_feats));
+    CU(d->d_fxy.assign((size_t)n_feats));
   }
   d->prepared = false;
   d->have_run = false;
@@ -624,7 +598,7 @@ static int prepare_bank(lm_detector* d) {
   d->bits_ok.assign((size_t)d->G, 0);
   {
     const LevelHost& lv = d->lv[low_level];
-    for (int g = 0; g < d->G && lv.d_bp; ++g) {
+    for (int g = 0; g < d->G && !lv.d_bp.empty(); ++g) {
       int total = 0;
       bool same = true;
       const TSlot& t0 = d->h_tslot[(size_t)g * d->S + low_level * d->M];
@@ -637,22 +611,20 @@ static int prepare_bank(lm_detector* d) {
     }
   }
   // k_coarse_packed descriptors (coarse_descriptors); a template whose descriptors do not fit goes to k_coarse_bytes
-  cudaFree(d->d_fdesc); d->d_fdesc = nullptr;
-  cudaFree(d->d_k2info); d->d_k2info = nullptr;
+  d->d_fdesc.reset();
+  d->d_k2info.reset();
   {
     const LevelHost& lv = d->lv[low_level];
-    if (lv.d_bp && d->G > 0) {
+    if (!lv.d_bp.empty() && d->G > 0) {
       std::vector<uint32_t> desc;
       std::vector<int2> k2;
       std::vector<uint8_t> fits;
       coarse_descriptors(d->feats.data(), d->tmeta.data(), d->G, d->S, d->M, low_level * d->M, lv.T, lv.rows, lv.cols, desc,
                          k2, fits);
       for (int g = 0; g < d->G; ++g) d->bits_ok[g] &= fits[g];
-      CU(cudaMalloc(&d->d_fdesc, std::max<size_t>(desc.size(), 1) * sizeof(uint32_t)));
-      CU(cudaMalloc(&d->d_k2info, k2.size() * sizeof(int2)));
-      if (!desc.empty()) CU(cudaMemcpyAsync(d->d_fdesc, desc.data(), desc.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
-      CU(cudaMemcpyAsync(d->d_k2info, k2.data(), k2.size() * sizeof(int2), cudaMemcpyHostToDevice, d->stream));
-      CU(cudaStreamSynchronize(d->stream));
+      CU(upload(d->d_fdesc, desc, d->stream.get(), 1));
+      CU(upload(d->d_k2info, k2, d->stream.get()));
+      CU(cudaStreamSynchronize(d->stream.get()));
     }
   }
   // "safe" templates: at every refined level the clamp range is regular (max >= border) and every
@@ -695,12 +667,7 @@ static int prepare_bank(lm_detector* d) {
       }
       for (int k = 0; k < n; ++k) { fbase[b0 + k] = tb[k]; fxy[b0 + k] = tx[k]; }
     }
-  cudaFree(d->d_galign);
-  d->d_galign = nullptr;
-  if (!galign.empty()) {
-    CU(cudaMalloc(&d->d_galign, galign.size() * sizeof(uint16_t)));
-    CU(cudaMemcpyAsync(d->d_galign, galign.data(), galign.size() * sizeof(uint16_t), cudaMemcpyHostToDevice, d->stream));
-  }
+  CU(upload(d->d_galign, galign, d->stream.get()));
   // refinement filter (k_refine_filter_w) on the first refined level: column-major H-planes [M*8*T*T][nyb][Wd] and one
   // descriptor per feature = plane word offset (incl. x / T) : 23 | y / T : 9.  Eligible templates ("safe", so that
   // the 16x16 patch of every feature is a true 2-D window of the level, and at most 511 features at that level) get
@@ -719,14 +686,13 @@ static int prepare_bank(lm_detector* d) {
     const size_t tail = (size_t)(nyb + 1) * lv.Wd + 64;
     if (lv.Wd % 4 == 0 && lv.Wd >= 16 && lv.Hd >= 16 && lv.Hd <= 512 && words > 0 && words + tail <= (1u << 23)) {
       d->filter_ok = true;
-      d->rp_nyb = nyb;
-      if (words != d->rp_words) {
-        cudaFree(d->d_rp);
-        d->d_rp = nullptr;
-        d->rp_words = words;
-        CU(cudaMalloc(&d->d_rp, (words + tail) * 4));
-        CU(cudaMemsetAsync(d->d_rp, 0, (words + tail) * 4, d->stream));  // halves no row block covers stay zero
+      // a new layout gets new, zeroed planes: with M and T fixed, size and nyb fix Wd.  Equal sizes of two layouts do
+      // not share: the old planes would lie where the new tail must read zeros
+      if (words + tail != d->d_rp.size() || nyb != d->rp_nyb) {
+        CU(d->d_rp.assign(words + tail));
+        CU(cudaMemsetAsync(d->d_rp.get(), 0, (words + tail) * 4, d->stream.get()));  // halves no row block covers stay zero
       }
+      d->rp_nyb = nyb;
       for (int g = 0; g < d->G; ++g) {
         int nfl = 0;
         for (int m = 0; m < d->M; ++m) nfl += d->tmeta[((size_t)g * d->S + lr * d->M + m) * 4 + 3];
@@ -750,29 +716,21 @@ static int prepare_bank(lm_detector* d) {
     }
   }
   d->h_rfeat = rfeat;
-  cudaFree(d->d_rdesc); d->d_rdesc = nullptr;
-  cudaFree(d->d_rfeat); d->d_rfeat = nullptr;
-  cudaFree(d->d_rlab); d->d_rlab = nullptr;
+  d->d_rdesc.reset();
+  d->d_rfeat.reset();
+  d->d_rlab.reset();
   if (d->filter_ok) {
-    CU(cudaMalloc(&d->d_rlab, std::max<size_t>(rlab.size(), 1)));
-    if (!rlab.empty()) CU(cudaMemcpyAsync(d->d_rlab, rlab.data(), rlab.size(), cudaMemcpyHostToDevice, d->stream));
-    CU(cudaMalloc(&d->d_rdesc, std::max<size_t>(rdesc.size(), 1) * 4));
-    CU(cudaMalloc(&d->d_rfeat, std::max<size_t>(rfeat.size(), 1) * sizeof(int2)));
-    if (!rdesc.empty()) CU(cudaMemcpyAsync(d->d_rdesc, rdesc.data(), rdesc.size() * 4, cudaMemcpyHostToDevice, d->stream));
-    if (!rfeat.empty()) CU(cudaMemcpyAsync(d->d_rfeat, rfeat.data(), rfeat.size() * sizeof(int2), cudaMemcpyHostToDevice, d->stream));
+    CU(upload(d->d_rlab, rlab, d->stream.get(), 1));
+    CU(upload(d->d_rdesc, rdesc, d->stream.get(), 1));
+    CU(upload(d->d_rfeat, rfeat, d->stream.get(), 1));
   }
-  cudaFree(d->d_safe);
-  d->d_safe = nullptr;
-  if (d->G) {
-    CU(cudaMalloc(&d->d_safe, (size_t)d->G));
-    CU(cudaMemcpyAsync(d->d_safe, d->safe.data(), (size_t)d->G, cudaMemcpyHostToDevice, d->stream));
-  }
+  CU(upload(d->d_safe, d->safe, d->stream.get()));
   if (nf) {
-    CU(cudaMemcpyAsync(d->d_fbase, fbase.data(), nf * 4, cudaMemcpyHostToDevice, d->stream));
-    CU(cudaMemcpyAsync(d->d_fxy, fxy.data(), nf * 4, cudaMemcpyHostToDevice, d->stream));
+    CU(cudaMemcpyAsync(d->d_fbase.get(), fbase.data(), nf * 4, cudaMemcpyHostToDevice, d->stream.get()));
+    CU(cudaMemcpyAsync(d->d_fxy.get(), fxy.data(), nf * 4, cudaMemcpyHostToDevice, d->stream.get()));
   }
-  if (d->G) CU(cudaMemcpyAsync(d->d_tslot, d->h_tslot.data(), sizeof(TSlot) * d->h_tslot.size(), cudaMemcpyHostToDevice, d->stream));
-  CU(cudaStreamSynchronize(d->stream));  // host vectors go out of scope
+  if (d->G) CU(cudaMemcpyAsync(d->d_tslot.get(), d->h_tslot.data(), sizeof(TSlot) * d->h_tslot.size(), cudaMemcpyHostToDevice, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));  // host vectors go out of scope
   d->feat_skip_low.assign(nf, 0);
   for (size_t i = 0; i < nf; ++i) d->feat_skip_low[i] = (fxy[i] & LM_SKIP_BIT) ? 1 : 0;
   for (int l = 0; l < d->L; ++l) { d->prep_rows[l] = d->lv[l].rows; d->prep_cols[l] = d->lv[l].cols; }
@@ -861,24 +819,16 @@ extern "C" int lm_coarse_tasks(const int32_t* words, int64_t n_items, int sm_cou
 static int prepare_work(lm_detector* d) {
   if (!d->work_dirty) return LM_OK;
   const int64_t n = d->shard_count;
-  cudaFree(d->d_work); d->d_work = nullptr;
-  if (n > 0) {
-    CU(cudaMalloc(&d->d_work, sizeof(int32_t) * (size_t)n));
-    CU(cudaMemcpyAsync(d->d_work, d->shard_sel.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, d->stream));
-    CU(cudaStreamSynchronize(d->stream));
-  }
+  CU(upload(d->d_work, d->shard_sel, d->stream.get()));
+  if (n > 0) CU(cudaStreamSynchronize(d->stream.get()));
   {
     std::vector<int32_t> ib, iy;
     for (int64_t i = 0; i < n; ++i) (d->bits_ok[d->shard_sel[(size_t)i]] ? ib : iy).push_back((int32_t)i);
-    cudaFree(d->d_items_bytes); d->d_items_bytes = nullptr;
     d->n_items_bits = (int)ib.size();
     d->n_items_bytes = (int)iy.size();
-    if (!iy.empty()) {
-      CU(cudaMalloc(&d->d_items_bytes, sizeof(int32_t) * iy.size()));
-      CU(cudaMemcpyAsync(d->d_items_bytes, iy.data(), sizeof(int32_t) * iy.size(), cudaMemcpyHostToDevice, d->stream));
-    }
+    CU(upload(d->d_items_bytes, iy, d->stream.get()));
     // the bit-sliced coarse scan's tasks: position words per item for the current frame size
-    cudaFree(d->d_k2task); d->d_k2task = nullptr;
+    d->d_k2task.reset();
     d->k2_full = d->k2_rem = d->k2_tasks = 0;
     std::vector<int2> tasks;
     if (!ib.empty()) {
@@ -895,19 +845,16 @@ static int prepare_work(lm_detector* d) {
       d->k2_full = (int)nf;
       d->k2_rem = (int)nr;
       d->k2_tasks = (int)(nf + (nr + 31) / 32);
-      CU(cudaMalloc(&d->d_k2task, sizeof(int2) * tasks.size()));
-      CU(cudaMemcpyAsync(d->d_k2task, tasks.data(), sizeof(int2) * tasks.size(), cudaMemcpyHostToDevice, d->stream));
+      CU(upload(d->d_k2task, tasks, d->stream.get()));
     }
-    CU(cudaStreamSynchronize(d->stream));
+    CU(cudaStreamSynchronize(d->stream.get()));
   }
-  if ((size_t)n + 1 > d->cnt_elems) {
-    cudaFree(d->d_cnt); cudaFree(d->d_off);
-    d->cnt_elems = (size_t)n + 1;
-    CU(cudaMalloc(&d->d_cnt, sizeof(int32_t) * d->cnt_elems));
-    CU(cudaMalloc(&d->d_off, sizeof(int32_t) * d->cnt_elems));
+  if ((size_t)n + 1 > d->d_off.size()) {  // d_off is allocated last: its size is the pair's
+    d->d_cnt.reset(); d->d_off.reset();
+    CU(d->d_cnt.assign((size_t)n + 1));
+    CU(d->d_off.assign((size_t)n + 1));
   }
-  cudaFree(d->d_finfo);
-  d->d_finfo = nullptr;
+  d->d_finfo.reset();
   d->h_finfo.clear();
   if (d->filter_ok && n > 0) {
     const int lr = d->L - 2;
@@ -918,14 +865,14 @@ static int prepare_work(lm_detector* d) {
       d->h_finfo[(size_t)i] = make_int4(d->h_rfeat[(size_t)g].x, d->h_rfeat[(size_t)g].y,
                                         (int)((uint32_t)t0[0] | ((uint32_t)t0[1] << 16)), (int)d->safe[(size_t)g]);
     }
-    CU(cudaMalloc(&d->d_finfo, sizeof(int4) * (size_t)n));
+    CU(d->d_finfo.assign((size_t)n));
     d->finfo_valid = false;  // the threshold-dependent part is filled in by lm_enqueue
     d->shard_all_eligible = true;
     for (const int4& f : d->h_finfo) d->shard_all_eligible = d->shard_all_eligible && (f.w & 2);
   }
   // per-template candidate counts are accumulated with atomics and re-zeroed by k_scan_counts
-  CU(cudaMemsetAsync(d->d_cnt, 0, sizeof(int32_t) * d->cnt_elems, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaMemsetAsync(d->d_cnt.get(), 0, sizeof(int32_t) * d->d_cnt.size(), d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   // algorithmic bytes of the coarse scan for this shard (SURVEY 8d): sum features x positions
   const int low = (d->L - 1) * d->M;
   int64_t bytes = 0;
@@ -948,13 +895,8 @@ static int prepare_work(lm_detector* d) {
 // the cell-summary buffer for the frame size.  Only while the gate is on.
 static int prepare_gate(lm_detector* d) {
   const LevelHost& low = d->lv[d->L - 1];
-  if ((size_t)low.plane > d->cells_cap) {
-    cudaFree(d->d_cells);
-    d->d_cells = nullptr;
-    d->cells_cap = (size_t)low.plane;
-    CU(cudaMalloc(&d->d_cells, sizeof(uint32_t) * d->cells_cap));
-  }
-  if (!d->d_gate_before) CU(cudaMalloc(&d->d_gate_before, sizeof(unsigned)));
+  CU(d->d_cells.reserve((size_t)low.plane));
+  CU(d->d_gate_before.reserve(1));
   if (!d->gate_dirty) return LM_OK;
   const int64_t n = d->shard_count;
   const int TL = d->T[d->L - 1];
@@ -975,17 +917,12 @@ static int prepare_gate(lm_detector* d) {
     }
     d->h_gate_item[(size_t)w] = make_uint2(zlo | (zhi << 16), ox | (oy << 16));
   }
-  if ((size_t)n > d->gate_item_cap) {
-    cudaFree(d->d_gate_item);
-    d->d_gate_item = nullptr;
-    d->gate_item_cap = (size_t)n;
-    CU(cudaMalloc(&d->d_gate_item, sizeof(uint2) * d->gate_item_cap));
-  }
+  CU(d->d_gate_item.reserve((size_t)n));
   // on the stream, behind the frames already enqueued (they keep the table they were enqueued with); waited for, since
   // h_gate_item may change once this returns
   if (n > 0)
-    CU(cudaMemcpyAsync(d->d_gate_item, d->h_gate_item.data(), sizeof(uint2) * (size_t)n, cudaMemcpyHostToDevice, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+    CU(cudaMemcpyAsync(d->d_gate_item.get(), d->h_gate_item.data(), sizeof(uint2) * (size_t)n, cudaMemcpyHostToDevice, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   d->gate_dirty = false;
   return LM_OK;
 }
@@ -1006,7 +943,7 @@ static int host_min_kept_raw(float threshold, int nfeat) {
 // finfo[w].w = flags | need << 8 for this threshold: need = number of features whose label bit must be set at some cell
 // of the patch for the candidate to be able to reach raw_keep (see k_refine_filter_w).
 static int filter_thresholds(lm_detector* d, float threshold) {
-  if (!d->filter_ok || !d->d_finfo || d->h_finfo.empty()) return LM_OK;
+  if (!d->filter_ok || d->d_finfo.empty() || d->h_finfo.empty()) return LM_OK;
   if (d->finfo_valid && memcmp(&threshold, &d->finfo_threshold, sizeof(float)) == 0) return LM_OK;
   d->h_finfo_up = d->h_finfo;
   int last_nf = -1, last_need = 0;
@@ -1019,7 +956,7 @@ static int filter_thresholds(lm_detector* d, float threshold) {
     }
     f.w |= last_need << 8;
   }
-  CU(cudaMemcpyAsync(d->d_finfo, d->h_finfo_up.data(), sizeof(int4) * d->h_finfo_up.size(), cudaMemcpyHostToDevice, d->stream));
+  CU(cudaMemcpyAsync(d->d_finfo.get(), d->h_finfo_up.data(), sizeof(int4) * d->h_finfo_up.size(), cudaMemcpyHostToDevice, d->stream.get()));
   d->finfo_valid = true;
   d->finfo_threshold = threshold;
   return LM_OK;
@@ -1041,12 +978,16 @@ static int check_frame_dims(lm_detector* d, const int* rows, const int* cols) {
   return LM_OK;
 }
 
-// (Re)allocate the per-level device buffers for a frame size.
+// (Re)allocate the per-level device buffers for a frame size.  A level of a new size is built aside and takes the
+// place of the old one (freed first) once every allocation of it has succeeded.
 static int size_levels(lm_detector* d, const int* rows, const int* cols, bool need_upload_buffers) {
   for (int l = 0; l < d->L; ++l) {
-    LevelHost& lv = d->lv[l];
-    if (lv.rows != rows[l] || lv.cols != cols[l] || lv.T != d->T[l]) {
-      free_level(lv);
+    if (d->lv[l].rows != rows[l] || d->lv[l].cols != cols[l] || d->lv[l].T != d->T[l]) {
+      // the old level goes first: until the new one stands, there is no frame and nothing prepared for its size
+      d->lv[l] = LevelHost();
+      d->have_frame = false;
+      d->prepared = false;
+      LevelHost lv;
       lv.T = d->T[l]; lv.rows = rows[l]; lv.cols = cols[l];
       lv.Wd = cols[l] / lv.T; lv.Hd = rows[l] / lv.T; lv.plane = lv.Wd * lv.Hd;
       const size_t per_mod = (size_t)8 * lv.T * lv.T * lv.plane;
@@ -1054,22 +995,20 @@ static int size_levels(lm_detector* d, const int* rows, const int* cols, bool ne
       const size_t slack = (size_t)lv.plane + 16 * (size_t)lv.Wd + 256;
       if (per_mod * d->M + slack > 0xFFFFFFFFull) return fail(LM_E_INVALID, "level %d: linear memories exceed 4 GiB", l);
       lv.mod_stride = (uint32_t)per_mod;
-      lv.lm_bytes = per_mod * d->M + slack;
-      CU(cudaMalloc(&lv.d_lm, lv.lm_bytes));
-      CU(cudaMemsetAsync(lv.d_lm, 0, lv.lm_bytes, d->stream));
+      CU(lv.d_lm.assign(per_mod * d->M + slack));
+      CU(cudaMemsetAsync(lv.d_lm.get(), 0, lv.d_lm.size(), d->stream.get()));
       lv.nwords = (lv.plane + 31) / 32;
       lv.rounds = (lv.nwords + 31) / 32;
       if (l == d->L - 1 && lv.rounds <= LM_MAX_ROUNDS) {
         lv.lbw = (int)bp_label_words(lv.T, lv.plane);
         const size_t words = (size_t)d->M * 8 * lv.lbw;
-        CU(cudaMalloc(&lv.d_bp, words * 4));
-        CU(cudaMemsetAsync(lv.d_bp, 0, words * 4, d->stream));
+        CU(lv.d_bp.assign(words));
+        CU(cudaMemsetAsync(lv.d_bp.get(), 0, words * 4, d->stream.get()));
       }
-      d->prepared = false;  // feature addresses depend on the frame size
+      d->lv[l] = std::move(lv);  // feature addresses depend on the frame size: prepare_bank recomputes them
     }
     if (need_upload_buffers)
-      for (int m = 0; m < d->M; ++m)
-        if (!lv.d_q[m]) CU(cudaMalloc(&lv.d_q[m], (size_t)rows[l] * cols[l]));
+      for (int m = 0; m < d->M; ++m) CU(d->lv[l].d_q[m].reserve((size_t)rows[l] * cols[l]));
   }
   return LM_OK;
 }
@@ -1095,24 +1034,24 @@ static int upload_quantized(lm_detector* d, const uint8_t* const* quantized, con
   // in front of the upper levels' linear memories (enqueue_stages).
   const bool fork = d->L > 1;
   if (fork) {
-    CU(cudaEventRecord(d->ev_fork, d->stream));
-    CU(cudaStreamWaitEvent(d->copy_stream, d->ev_fork, 0));
+    CU(cudaEventRecord(d->ev_fork.get(), d->stream.get()));
+    CU(cudaStreamWaitEvent(d->copy_stream.get(), d->ev_fork.get(), 0));
   }
   for (int l = d->L - 1; l >= 0; --l) {
     LevelHost& lv = d->lv[l];
-    cudaStream_t st = (fork && l < d->L - 1) ? d->copy_stream : d->stream;
+    cudaStream_t st = (fork && l < d->L - 1) ? d->copy_stream.get() : d->stream.get();
     for (int m = 0; m < d->M; ++m) {
-      CU(cudaMemcpyAsync(lv.d_q[m], quantized[l * d->M + m], (size_t)rows[l] * cols[l], cudaMemcpyHostToDevice, st));
-      lv.q_src[m] = lv.d_q[m];
+      CU(cudaMemcpyAsync(lv.d_q[m].get(), quantized[l * d->M + m], (size_t)rows[l] * cols[l], cudaMemcpyHostToDevice, st));
+      lv.q_src[m] = lv.d_q[m].get();
     }
   }
   if (fork) {
-    CU(cudaEventRecord(d->ev_upper, d->copy_stream));
+    CU(cudaEventRecord(d->ev_upper.get(), d->copy_stream.get()));
     d->upper_pending = true;
   }
   if (sync) {  // caller's buffers are only borrowed for the call
-    CU(cudaStreamSynchronize(d->stream));
-    if (fork) CU(cudaStreamSynchronize(d->copy_stream));
+    CU(cudaStreamSynchronize(d->stream.get()));
+    if (fork) CU(cudaStreamSynchronize(d->copy_stream.get()));
   }
   d->have_frame = true;
   d->frame_depth = false;
@@ -1133,7 +1072,7 @@ extern "C" int lm_bind_quantized_device(lm_detector* d, const uint8_t* const* d_
       if (!d_quantized[l * d->M + m]) return fail(LM_E_INVALID, "d_quantized[%d] is null", l * d->M + m);
       d->lv[l].q_src[m] = d_quantized[l * d->M + m];
     }
-  if (d->upper_pending) CU(cudaStreamWaitEvent(d->stream, d->ev_upper, 0));  // an earlier upload nobody consumed
+  if (d->upper_pending) CU(cudaStreamWaitEvent(d->stream.get(), d->ev_upper.get(), 0));  // an earlier upload nobody consumed
   d->upper_pending = false;
   d->have_frame = true;
   d->frame_depth = false;
@@ -1155,8 +1094,8 @@ static int fe_dims(lm_detector* d, int rows, int cols, int* lrows, int* lcols) {
 static int fe_levels(lm_detector* d, const int* lrows, const int* lcols) {
   int rc = size_levels(d, lrows, lcols, true);
   if (rc) return rc;
-  cudaStream_t st = d->stream;
-  if (d->upper_pending) CU(cudaStreamWaitEvent(st, d->ev_upper, 0));  // an earlier upload nobody consumed
+  cudaStream_t st = d->stream.get();
+  if (d->upper_pending) CU(cudaStreamWaitEvent(st, d->ev_upper.get(), 0));  // an earlier upload nobody consumed
   if (!d->fe_lut) {
     // NORMAL_LUT[.][vy][vx] of normal_lut.i: 45-degree sector (offset by half a sector) of atan2(vy-10, vx-10);
     // the rule reproduces all 8000 entries of the reference table (tests/test_frontend.py)
@@ -1172,18 +1111,20 @@ static int fe_levels(lm_detector* d, const int* lrows, const int* lcols) {
     d->fe_lut = true;
   }
   for (int l = 0; l < d->L; ++l) {
-    lm_detector::FeLevel& f = d->fe[l];
-    if (f.rows != lrows[l] || f.cols != lcols[l]) {
-      cudaFree(f.src); cudaFree(f.qun); cudaFree(f.strong); cudaFree(f.normal); cudaFree(f.mask[0]); cudaFree(f.mask[1]);
-      f = lm_detector::FeLevel();
-      f.rows = lrows[l]; f.cols = lcols[l];
-      const size_t n = (size_t)f.rows * f.cols;
-      CU(cudaMalloc(&f.src, n * 3)); CU(cudaMalloc(&f.qun, n)); CU(cudaMalloc(&f.strong, n)); CU(cudaMalloc(&f.normal, n));
-      CU(cudaMalloc(&f.mask[0], n)); CU(cudaMalloc(&f.mask[1], n));
+    if (d->fe[l].rows != lrows[l] || d->fe[l].cols != lcols[l]) {
+      // built aside, recorded once every allocation succeeded (level 0 also sizes fe_depth / fe_nraw)
+      d->fe[l] = lm_detector::FeLevel();
+      d->have_frame = false;
+      lm_detector::FeLevel f;
+      const size_t n = (size_t)lrows[l] * lcols[l];
+      CU(f.src.assign(n * 3)); CU(f.qun.assign(n)); CU(f.strong.assign(n)); CU(f.normal.assign(n));
+      CU(f.mask[0].assign(n)); CU(f.mask[1].assign(n));
       if (l == 0) {
-        cudaFree(d->fe_depth); cudaFree(d->fe_nraw);
-        CU(cudaMalloc(&d->fe_depth, n * 2)); CU(cudaMalloc(&d->fe_nraw, n));
+        d->fe_depth.reset(); d->fe_nraw.reset();
+        CU(d->fe_depth.assign(n)); CU(d->fe_nraw.assign(n));
       }
+      f.rows = lrows[l]; f.cols = lcols[l];
+      d->fe[l] = std::move(f);
     }
   }
   return LM_OK;
@@ -1191,39 +1132,39 @@ static int fe_levels(lm_detector* d, const int* lrows, const int* lcols) {
 
 // Label images of every level from the level-0 frame in fe[0].src / fe_depth / fe[0].mask[m] (masks[m]: given).
 static int fe_quantize(lm_detector* d, const bool* masks) {
-  cudaStream_t st = d->stream;
+  cudaStream_t st = d->stream.get();
   auto grid2 = [](int w, int h) { return dim3((unsigned)((w + 31) / 32), (unsigned)((h + 7) / 8)); };
   for (int l = 0; l < d->L; ++l) {
     lm_detector::FeLevel& f = d->fe[l];
     LevelHost& lv = d->lv[l];
     if (l > 0) {
       lm_detector::FeLevel& up = d->fe[l - 1];
-      CU(launch_pdl(k_fe_pyrdown, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)up.src, up.rows, up.cols, f.src, f.rows, f.cols));
+      CU(launch_pdl(k_fe_pyrdown, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)up.src.get(), up.rows, up.cols, f.src.get(), f.rows, f.cols));
       for (int m = 0; m < 2; ++m)
         if (masks[m])
-          CU(launch_pdl(k_fe_decimate, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)up.mask[m], up.cols, f.mask[m], f.rows,
+          CU(launch_pdl(k_fe_decimate, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)up.mask[m].get(), up.cols, f.mask[m].get(), f.rows,
                         f.cols, (const uint8_t*)nullptr, (uint8_t*)nullptr));
       d->launches += 1 + (masks[0] ? 1 : 0) + (masks[1] ? 1 : 0);
     }
     // colour: weak threshold 10 -> gate on squared magnitude > 100 (ColorGradient(10, nf, 55), LL.cpp:1687)
-    CU(launch_pdl(k_fe_gradient, grid2(f.cols, f.rows), dim3(FE_TW, FE_TH), 0, st, (const uint8_t*)f.src, f.rows, f.cols, 100, f.qun, f.strong));
-    CU(launch_pdl(k_fe_hysteresis, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)f.qun, (const uint8_t*)f.strong,
-                  (const uint8_t*)(masks[0] ? f.mask[0] : nullptr), f.rows, f.cols, lv.d_q[0]));
+    CU(launch_pdl(k_fe_gradient, grid2(f.cols, f.rows), dim3(FE_TW, FE_TH), 0, st, (const uint8_t*)f.src.get(), f.rows, f.cols, 100, f.qun.get(), f.strong.get()));
+    CU(launch_pdl(k_fe_hysteresis, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)f.qun.get(), (const uint8_t*)f.strong.get(),
+                  (const uint8_t*)(masks[0] ? f.mask[0].get() : nullptr), f.rows, f.cols, lv.d_q[0].get()));
     d->launches += 2;
     // depth: DepthNormal(2000, 50, nf, 2), LL.cpp:1688; upper levels decimate the LABELS (LL.cpp:865-868)
     if (l == 0) {
-      CU(launch_pdl(k_fe_normals, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint16_t*)d->fe_depth, f.rows, f.cols, 2000, 50, d->fe_nraw));
-      CU(launch_pdl(k_fe_median, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)d->fe_nraw,
-                    (const uint8_t*)(masks[1] ? f.mask[1] : nullptr), f.rows, f.cols, f.normal, lv.d_q[1]));
+      CU(launch_pdl(k_fe_normals, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint16_t*)d->fe_depth.get(), f.rows, f.cols, 2000, 50, d->fe_nraw.get()));
+      CU(launch_pdl(k_fe_median, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)d->fe_nraw.get(),
+                    (const uint8_t*)(masks[1] ? f.mask[1].get() : nullptr), f.rows, f.cols, f.normal.get(), lv.d_q[1].get()));
       d->launches += 2;
     } else {
       lm_detector::FeLevel& up = d->fe[l - 1];
-      CU(launch_pdl(k_fe_decimate, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)up.normal, up.cols, f.normal, f.rows, f.cols,
-                    (const uint8_t*)(masks[1] ? f.mask[1] : nullptr), lv.d_q[1]));
+      CU(launch_pdl(k_fe_decimate, grid2(f.cols, f.rows), dim3(256), 0, st, (const uint8_t*)up.normal.get(), up.cols, f.normal.get(), f.rows, f.cols,
+                    (const uint8_t*)(masks[1] ? f.mask[1].get() : nullptr), lv.d_q[1].get()));
       d->launches += 1;
     }
-    lv.q_src[0] = lv.d_q[0];
-    lv.q_src[1] = lv.d_q[1];
+    lv.q_src[0] = lv.d_q[0].get();
+    lv.q_src[1] = lv.d_q[1].get();
   }
   return LM_OK;
 }
@@ -1246,13 +1187,13 @@ extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16
   if (rc) return rc;
   rc = fe_levels(d, lrows, lcols);
   if (rc) return rc;
-  cudaStream_t st = d->stream;
+  cudaStream_t st = d->stream.get();
   const size_t n0 = (size_t)rows * cols;
-  CU(cudaMemcpyAsync(d->fe[0].src, rgb, n0 * 3, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d->fe_depth, depth, n0 * 2, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d->fe[0].src.get(), rgb, n0 * 3, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d->fe_depth.get(), depth, n0 * 2, cudaMemcpyHostToDevice, st));
   const uint8_t* masks[2] = {mask_color, mask_depth};
   for (int m = 0; m < 2; ++m)
-    if (masks[m]) CU(cudaMemcpyAsync(d->fe[0].mask[m], masks[m], n0, cudaMemcpyHostToDevice, st));
+    if (masks[m]) CU(cudaMemcpyAsync(d->fe[0].mask[m].get(), masks[m], n0, cudaMemcpyHostToDevice, st));
   const bool given[2] = {masks[0] != nullptr, masks[1] != nullptr};
   rc = fe_quantize(d, given);
   if (rc) return rc;
@@ -1315,20 +1256,20 @@ static int bind_images_device(lm_detector* d, const DeviceFrame& f, int rows, in
                               cudaStream_t caller) {
   int rc = fe_levels(d, lrows, lcols);
   if (rc) return rc;
-  if (!d->ev_in) CU(cudaEventCreateWithFlags(&d->ev_in, cudaEventDisableTiming));
-  if (!d->ev_out) CU(cudaEventCreateWithFlags(&d->ev_out, cudaEventDisableTiming));
-  cudaStream_t st = d->stream;
-  CU(cudaEventRecord(d->ev_in, caller));
-  CU(cudaStreamWaitEvent(st, d->ev_in, 0));
+  if (!d->ev_in.get()) CU(d->ev_in.create(cudaEventDisableTiming));
+  if (!d->ev_out.get()) CU(d->ev_out.create(cudaEventDisableTiming));
+  cudaStream_t st = d->stream.get();
+  CU(cudaEventRecord(d->ev_in.get(), caller));
+  CU(cudaStreamWaitEvent(st, d->ev_in.get(), 0));
   // a plain launch: it starts once the caller's work and everything before it on the stream have completed
   const dim3 grid((unsigned)((cols + FE_INGEST_PX - 1) / FE_INGEST_PX), (unsigned)rows);
   lm_detector::FeLevel& f0 = d->fe[0];
   k_fe_ingest<<<grid, FE_INGEST_PX, 0, st>>>(f.rgb, f.rgb_pitch, f.depth, f.depth_pitch, f.format == LM_DEPTH_F32 ? 1 : 0, f.scale,
-                                             f.mask[0], f.mask[1], f.mask_pitch, cols, f0.src, d->fe_depth, f0.mask[0], f0.mask[1]);
+                                             f.mask[0], f.mask[1], f.mask_pitch, cols, f0.src.get(), d->fe_depth.get(), f0.mask[0].get(), f0.mask[1].get());
   CU(cudaGetLastError());
   d->launches += 1;
-  CU(cudaEventRecord(d->ev_out, st));
-  CU(cudaStreamWaitEvent(caller, d->ev_out, 0));  // the borrow ends with the ingest
+  CU(cudaEventRecord(d->ev_out.get(), st));
+  CU(cudaStreamWaitEvent(caller, d->ev_out.get(), 0));  // the borrow ends with the ingest
   const bool given[2] = {f.mask[0] != nullptr, f.mask[1] != nullptr};
   rc = fe_quantize(d, given);
   if (rc) return rc;
@@ -1356,14 +1297,14 @@ extern "C" int lm_debug_depth(lm_detector* d, uint16_t* out, int64_t cap) {
   const int64_t n = (int64_t)d->fe[0].rows * d->fe[0].cols;
   if (n > cap) return fail(LM_E_CAPACITY, "need %lld elements", (long long)n);
   CU(cudaSetDevice(d->device));
-  CU(cudaMemcpyAsync(out, d->fe_depth, (size_t)n * 2, cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaMemcpyAsync(out, d->fe_depth.get(), (size_t)n * 2, cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   return LM_OK;
 }
 
 static LevelDev level_dev(const LevelHost& h) {
   LevelDev v;
-  v.lm = h.d_lm; v.T = h.T; v.rows = h.rows; v.cols = h.cols; v.Wd = h.Wd; v.Hd = h.Hd; v.plane = h.plane;
+  v.lm = h.d_lm.get(); v.T = h.T; v.rows = h.rows; v.cols = h.cols; v.Wd = h.Wd; v.Hd = h.Hd; v.plane = h.plane;
   v.off = h.T / 2 + (h.T % 2 - 1);
   v.mod_stride = h.mod_stride;
   return v;
@@ -1416,12 +1357,12 @@ static void plan_k1(lm_detector* d, int planes_level, bool with_bit_planes, K1Pl
     const LevelHost& lv = d->lv[l];
     LinMemLevel& q = p.lv[l];
     for (int m = 0; m < d->M; ++m) q.q[m] = lv.q_src[m];
-    q.lm = lv.d_lm; q.bp = with_bit_planes ? lv.d_bp : nullptr; q.lbw = lv.lbw;
+    q.lm = lv.d_lm.get(); q.bp = with_bit_planes ? lv.d_bp.get() : nullptr; q.lbw = lv.lbw;
     q.T = lv.T; q.rows = lv.rows; q.cols = lv.cols; q.Wd = lv.Wd; q.Hd = lv.Hd; q.plane = lv.plane;
     q.mod_stride = lv.mod_stride;
     q.rp = nullptr; q.nyb = 0;
     if (band && l == planes_level) {
-      q.rp = d->d_rp; q.nyb = d->rp_nyb;
+      q.rp = d->d_rp.get(); q.nyb = d->rp_nyb;
       blocks += ((lv.Hd + 15) / 16) * (lv.Wd / q.pseg);
     } else {
       blocks += band ? lv.Hd * q.nseg : (lv.T * lv.T * lv.plane + 255) / 256;
@@ -1437,14 +1378,14 @@ static int launch_k1(lm_detector* d, const K1Plan& k, int first_block, int n_blo
   if (n_blocks <= 0) return LM_OK;
   LinMemParams p = k.p;
   p.block_offset = first_block;
-  if (k.band) CU(launch_pdl(k_linear_memories_band, dim3((unsigned)n_blocks, (unsigned)d->M), dim3(128), k.smem, d->stream, p));
-  else CU(launch_pdl(k_linear_memories, dim3((unsigned)n_blocks, (unsigned)d->M), dim3(256), 0, d->stream, p));
+  if (k.band) CU(launch_pdl(k_linear_memories_band, dim3((unsigned)n_blocks, (unsigned)d->M), dim3(128), k.smem, d->stream.get(), p));
+  else CU(launch_pdl(k_linear_memories, dim3((unsigned)n_blocks, (unsigned)d->M), dim3(256), 0, d->stream.get(), p));
   ++d->launches;
   return LM_OK;
 }
 
 // Which refinement path the current bank / shard / frame size take (see enqueue_stages).
-static bool use_filter(const lm_detector* d) { return d->filter_ok && d->d_rp != nullptr && d->d_finfo != nullptr; }
+static bool use_filter(const lm_detector* d) { return d->filter_ok && !d->d_rp.empty() && !d->d_finfo.empty(); }
 static bool use_bits(const lm_detector* d) { return use_filter(d) && d->L == 2; }
 // level built in planes mode by K1, or -1: only when nothing reads that level's byte linear memories
 static int planes_level(const lm_detector* d) { return use_bits(d) && d->shard_all_eligible ? d->L - 2 : -1; }
@@ -1453,7 +1394,7 @@ static int planes_level(const lm_detector* d) { return use_bits(d) && d->shard_a
 static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
   const int n_work = (int)d->shard_count;
   const LevelHost& low = d->lv[d->L - 1];
-  cudaStream_t st = d->stream;
+  cudaStream_t st = d->stream.get();
   // fused multi-GPU exchange: k_refine appends into block [frame slot][rank] of every rank's buffer
   PeerExchange px;
   memset(&px, 0, sizeof(px));
@@ -1462,7 +1403,7 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     if (refine_only) return fail(LM_E_STATE, "refinement re-run is not available with a connected peer exchange");
     ++d->px_seq;
     px = d->h_px;
-    px_block = reinterpret_cast<lm_result_header*>(d->px_buf + (size_t)(d->px_seq & 1) * px.slot_bytes +
+    px_block = reinterpret_cast<lm_result_header*>(d->px_buf.get() + (size_t)(d->px_seq & 1) * px.slot_bytes +
                                                    (size_t)px.rank * px.block_bytes);
   }
   if (d->timing && !refine_only) {
@@ -1472,7 +1413,7 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
   K1Plan k1;
   int k1_done = 0;
   if (!refine_only) {
-    if (d->timing) CU(cudaEventRecord(d->ev[0], st));
+    if (d->timing) CU(cudaEventRecord(d->ev[0].get(), st));
     // K1: one launch for every level and modality.  Bit-planes are OR-ed in: zero at allocation, re-zeroed by the
     // refinement kernel after every frame.  With a host upload in flight (upper levels still on the copy stream) the
     // launch is split: the lowest level now, the levels above it behind the coarse scan, once their images have landed.
@@ -1481,40 +1422,40 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     k1_done = d->upper_pending ? k1.p.lv[d->L - 1].block_end : k1.blocks;
     int rc1 = launch_k1(d, k1, 0, k1_done);
     if (rc1) return rc1;
-    if (d->timing) CU(cudaEventRecord(d->ev[1], st));
+    if (d->timing) CU(cudaEventRecord(d->ev[1].get(), st));
     // depth gate: the frame's cell summary, ahead of K2
     const bool gated = d->gate_frame;
     DepthGate gate;  // read by the gated launches only
     if (gated) {
-      gate.cells = d->d_cells; gate.item = d->d_gate_item; gate.before = d->d_gate_before;
+      gate.cells = d->d_cells.get(); gate.item = d->d_gate_item.get(); gate.before = d->d_gate_before.get();
       gate.Wd = low.Wd; gate.Hd = low.Hd;
       const int B = low.T << (d->L - 1);  // s * T_L full-resolution pixels per cell side
-      CU(launch_pdl(k_depth_cells, dim3((unsigned)((low.plane + 7) / 8)), dim3(256), 0, st, (const uint16_t*)d->fe_depth,
-                    d->fe[0].rows, d->fe[0].cols, B, low.Wd, low.Hd, d->d_cells, d->d_gate_before));
+      CU(launch_pdl(k_depth_cells, dim3((unsigned)((low.plane + 7) / 8)), dim3(256), 0, st, (const uint16_t*)d->fe_depth.get(),
+                    d->fe[0].rows, d->fe[0].cols, B, low.Wd, low.Hd, d->d_cells.get(), d->d_gate_before.get()));
       ++d->launches;
     }
     // K2
     bool scan_fused = false;
     if (d->n_items_bits > 0) {
       BitScanGateParams bp;
-      bp.bp = low.d_bp; bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw);
+      bp.bp = low.d_bp.get(); bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw);
       bp.lbw = low.lbw; bp.plane = low.plane; bp.nwords = low.nwords;
-      bp.tslot = d->d_tslot; bp.fdesc = d->d_fdesc; bp.k2info = d->d_k2info; bp.work = d->d_work;
+      bp.tslot = d->d_tslot.get(); bp.fdesc = d->d_fdesc.get(); bp.k2info = d->d_k2info.get(); bp.work = d->d_work.get();
       bp.zero_desc = coarse_zero_descriptor(low.T, low.plane);
-      bp.tasks = d->d_k2task; bp.n_full = d->k2_full; bp.n_rem = d->k2_rem; bp.n_tasks = d->k2_tasks;
+      bp.tasks = d->d_k2task.get(); bp.n_full = d->k2_full; bp.n_rem = d->k2_rem; bp.n_tasks = d->k2_tasks;
       bp.S = d->S; bp.M = d->M; bp.slot_low = (d->L - 1) * d->M;
       bp.threshold = threshold;
-      bp.mask = d->d_mask; bp.raw = d->d_raw; bp.cnt = d->d_cnt;
+      bp.mask = d->d_mask.get(); bp.raw = d->d_raw.get(); bp.cnt = d->d_cnt.get();
       const bool fuse_scan = d->n_items_bytes == 0;
       scan_fused = fuse_scan;
-      bp.off = fuse_scan ? d->d_off : nullptr;
+      bp.off = fuse_scan ? d->d_off.get() : nullptr;
       bp.n_work = n_work;
       bp.hdr = px.world > 0 ? px_block : d->d_res;
       bp.capacity = (int)(px.world > 0 ? d->px_cap : d->res_cap);
       bp.shard = d->shard_index;
-      bp.counters = d->d_counters;
-      bp.queue = d->d_queue;
-      bp.ticket = reinterpret_cast<int*>(d->d_counters + 3);
+      bp.counters = d->d_counters.get();
+      bp.queue = d->d_queue.get();
+      bp.ticket = reinterpret_cast<int*>(d->d_counters.get() + 3);
       const size_t plane_bytes = ((size_t)bp.bp_words * 4 + 15) & ~(size_t)15;
       const CoarseShape c = coarse_shape(d->k2_tasks, d->sm_count, plane_bytes);
       bp.split = c.split;
@@ -1534,11 +1475,11 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     if (d->n_items_bytes > 0) {
       ByteScanGateParams sp;
       sp.lv = level_dev(low);
-      sp.tslot = d->d_tslot; sp.fbase = d->d_fbase; sp.fxy = d->d_fxy; sp.work = d->d_work;
-      sp.items = d->d_items_bytes;
+      sp.tslot = d->d_tslot.get(); sp.fbase = d->d_fbase.get(); sp.fxy = d->d_fxy.get(); sp.work = d->d_work.get();
+      sp.items = d->d_items_bytes.get();
       sp.S = d->S; sp.M = d->M; sp.slot_low = (d->L - 1) * d->M; sp.nwords = low.nwords;
       sp.threshold = threshold;
-      sp.mask = d->d_mask; sp.raw = d->d_raw; sp.cnt = d->d_cnt;
+      sp.mask = d->d_mask.get(); sp.raw = d->d_raw.get(); sp.cnt = d->d_cnt.get();
       int bs = ((low.plane + 3) / 4 + 31) / 32 * 32;
       bs = std::max(32, std::min(bs, 1024));
       if (gated) {
@@ -1547,24 +1488,24 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
       } else CU(launch_pdl(k_coarse_bytes<false>, dim3(d->n_items_bytes), dim3(bs), 0, st, static_cast<const ByteScanParams&>(sp)));
       ++d->launches;
     }
-    if (d->timing) CU(cudaEventRecord(d->ev[2], st));
+    if (d->timing) CU(cudaEventRecord(d->ev[2].get(), st));
     if (!scan_fused) {
-      CU(launch_pdl(k_scan_counts, dim3(1), dim3(1024), 0, st, d->d_cnt, d->d_off, n_work,
+      CU(launch_pdl(k_scan_counts, dim3(1), dim3(1024), 0, st, d->d_cnt.get(), d->d_off.get(), n_work,
                     px.world > 0 ? px_block : d->d_res, (int)(px.world > 0 ? d->px_cap : d->res_cap), d->shard_index,
-                    d->d_counters, d->d_queue));
+                    d->d_counters.get(), d->d_queue.get()));
       ++d->launches;
     }
-    if (d->timing) CU(cudaEventRecord(d->ev[3], st));
+    if (d->timing) CU(cudaEventRecord(d->ev[3].get(), st));
     if (k1_done < k1.blocks) {  // the upper levels' linear memories, behind their images
-      CU(cudaStreamWaitEvent(st, d->ev_upper, 0));
+      CU(cudaStreamWaitEvent(st, d->ev_upper.get(), 0));
       int rc2 = launch_k1(d, k1, k1_done, k1.blocks - k1_done);
       if (rc2) return rc2;
     }
     d->upper_pending = false;
   }
   if (refine_only) {
-    CU(cudaMemsetAsync(d->d_counters, 0, 8 * sizeof(unsigned long long), st));  // [3] (the coarse scan's ticket) is 0 between launches
-    CU(cudaMemsetAsync(d->d_queue, 0, 4 * sizeof(int), st));
+    CU(cudaMemsetAsync(d->d_counters.get(), 0, 8 * sizeof(unsigned long long), st));  // [3] (the coarse scan's ticket) is 0 between launches
+    CU(cudaMemsetAsync(d->d_queue.get(), 0, 4 * sizeof(int), st));
     CU(cudaMemsetAsync(&d->d_res->count, 0, sizeof(int32_t), st));
   }
   const bool filter = use_filter(d);
@@ -1574,48 +1515,48 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
   {
     // ordered candidate list (+ the filter's H-planes of the first refined level)
     PrepParams pp;
-    pp.off = d->d_off; pp.mask = d->d_mask;
+    pp.off = d->d_off.get(); pp.mask = d->d_mask.get();
     pp.n_work = n_work; pp.nwords = low.nwords;
-    pp.cand = d->d_cand; pp.cand_cap = (int)d->cand_cap;
+    pp.cand = d->d_cand.get(); pp.cand_cap = (int)cand_cap(d);
     pp.expand_blocks = std::max(1, std::min((n_work + 7) / 8, d->sm_count * 8));
-    pp.lm = lref.d_lm; pp.rp = (filter && d->last_planes_level < 0) ? d->d_rp : nullptr;  // else: K1 wrote the planes
+    pp.lm = lref.d_lm.get(); pp.rp = (filter && d->last_planes_level < 0) ? d->d_rp.get() : nullptr;  // else: K1 wrote the planes
     pp.Wd = lref.Wd; pp.Hd = lref.Hd; pp.plane = lref.plane; pp.nyb = d->rp_nyb;
     pp.n_pb = d->M * 8 * lref.T * lref.T;
     const int plane_blocks = pp.rp ? (int)(((size_t)pp.n_pb * pp.nyb * (pp.Wd / 4) + 255) / 256) : 0;
     CU(launch_pdl(k_refine_prep, dim3((unsigned)(pp.expand_blocks + plane_blocks)), dim3(256), 0, st, pp));
     ++d->launches;
   }
-  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[4], st));
+  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[4].get(), st));
   if (filter) {
     FilterParams fp;
-    fp.rp = d->d_rp; fp.Wd = lref.Wd; fp.nyb = d->rp_nyb;
-    fp.rdesc = d->d_rdesc; fp.rfeat = d->d_rfeat; fp.finfo = d->d_finfo; fp.flags = d->d_safe;
-    fp.tslot = d->d_tslot; fp.work = d->d_work; fp.S = d->S; fp.M = d->M; fp.L = d->L;
+    fp.rp = d->d_rp.get(); fp.Wd = lref.Wd; fp.nyb = d->rp_nyb;
+    fp.rdesc = d->d_rdesc.get(); fp.rfeat = d->d_rfeat.get(); fp.finfo = d->d_finfo.get(); fp.flags = d->d_safe.get();
+    fp.tslot = d->d_tslot.get(); fp.work = d->d_work.get(); fp.S = d->S; fp.M = d->M; fp.L = d->L;
     fp.low = level_dev(low); fp.ref = level_dev(lref);
-    fp.cand = d->d_cand; fp.off = d->d_off; fp.n_work = n_work; fp.cand_cap = (int)d->cand_cap;
+    fp.cand = d->d_cand.get(); fp.off = d->d_off.get(); fp.n_work = n_work; fp.cand_cap = (int)cand_cap(d);
     fp.threshold = threshold;
-    fp.surv = d->d_surv; fp.surv2 = bits_mode ? d->d_surv2 : nullptr; fp.queue = d->d_queue; fp.counters = d->d_counters;
+    fp.surv = d->d_surv.get(); fp.surv2 = bits_mode ? d->d_surv2.get() : nullptr; fp.queue = d->d_queue.get(); fp.counters = d->d_counters.get();
     CU(launch_pdl(k_refine_filter_w, dim3((unsigned)(d->sm_count * LM_FILTER_MIN_CTAS)), dim3(256), 0, st, fp));
     ++d->launches;
   }
-  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[5], st));
+  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[5].get(), st));
   const bool bytes_pass = !bits_mode || !d->shard_all_eligible;  // byte-wise exact refinement needed for this shard
   if (bits_mode) {
     // exact refinement of the survivors, bit-sliced, from the same H-planes
     RefineBitsParams bq;
-    bq.rp = d->d_rp; bq.Wd = lref.Wd; bq.label_stride = lref.T * lref.T * d->rp_nyb * lref.Wd;
-    bq.rdesc = d->d_rdesc; bq.rlab = d->d_rlab; bq.finfo = d->d_finfo;
+    bq.rp = d->d_rp.get(); bq.Wd = lref.Wd; bq.label_stride = lref.T * lref.T * d->rp_nyb * lref.Wd;
+    bq.rdesc = d->d_rdesc.get(); bq.rlab = d->d_rlab.get(); bq.finfo = d->d_finfo.get();
     bq.low = level_dev(low); bq.ref = level_dev(lref);
-    bq.cand = d->d_cand; bq.off = d->d_off; bq.n_work = n_work; bq.cand_cap = (int)d->cand_cap;
-    bq.surv = d->d_surv; bq.queue = d->d_queue;
+    bq.cand = d->d_cand.get(); bq.off = d->d_off.get(); bq.n_work = n_work; bq.cand_cap = (int)cand_cap(d);
+    bq.surv = d->d_surv.get(); bq.queue = d->d_queue.get();
     bq.threshold = threshold;
     bq.work_begin = (int)d->work_base; bq.work_stride = (int)d->work_stride;
     bq.hdr = px.world > 0 ? px_block : d->d_res;
     bq.capacity = (int32_t)(px.world > 0 ? d->px_cap : d->res_cap);
-    bq.px = px.world > 0 ? d->d_px : nullptr; bq.px_seq = d->px_seq;
+    bq.px = px.world > 0 ? d->d_px.get() : nullptr; bq.px_seq = d->px_seq;
     bq.publish = bytes_pass ? 0 : 1;
-    bq.counters = d->d_counters;
-    bq.bp_clear = low.d_bp; bq.bp_words = low.d_bp ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
+    bq.counters = d->d_counters.get();
+    bq.bp_clear = low.d_bp.get(); bq.bp_words = !low.d_bp.empty() ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
     CU(launch_pdl(k_refine_bits, dim3((unsigned)(d->sm_count * 6)), dim3(256), 0, st, bq));
     ++d->launches;
   }
@@ -1623,9 +1564,9 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     // persistent grid: the candidate total is read on the device (no host round trip)
     RefineParams rp;
     for (int l = 0; l < d->L; ++l) rp.lv[l] = level_dev(d->lv[l]);
-    rp.tslot = d->d_tslot; rp.fbase = d->d_fbase; rp.fxy = d->d_fxy; rp.work = d->d_work;
-    rp.off = d->d_off; rp.cand = d->d_cand; rp.cand_cap = (int)d->cand_cap; rp.raw = d->d_raw;
-    rp.surv = filter ? (bits_mode ? d->d_surv2 : d->d_surv) : nullptr; rp.queue = d->d_queue;
+    rp.tslot = d->d_tslot.get(); rp.fbase = d->d_fbase.get(); rp.fxy = d->d_fxy.get(); rp.work = d->d_work.get();
+    rp.off = d->d_off.get(); rp.cand = d->d_cand.get(); rp.cand_cap = (int)cand_cap(d); rp.raw = d->d_raw.get();
+    rp.surv = filter ? (bits_mode ? d->d_surv2.get() : d->d_surv.get()) : nullptr; rp.queue = d->d_queue.get();
     rp.surv_slot = bits_mode ? 2 : 1;
     rp.publish = 1;
     rp.n_work = n_work; rp.L = d->L; rp.S = d->S; rp.M = d->M;
@@ -1633,16 +1574,16 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     rp.work_stride = (int)d->work_stride;
     rp.threshold = threshold;
     rp.hdr = d->d_res; rp.capacity = (int32_t)d->res_cap;
-    rp.px = px.world > 0 ? d->d_px : nullptr;
+    rp.px = px.world > 0 ? d->d_px.get() : nullptr;
     rp.px_seq = d->px_seq;
     if (px.world > 0) {
       rp.hdr = px_block;
       rp.capacity = (int32_t)d->px_cap;
     }
-    rp.counters = d->d_counters;
-    rp.safe = d->d_safe; rp.galign = d->d_galign;
-    rp.bp_clear = bits_mode ? nullptr : low.d_bp;
-    rp.bp_words = (!bits_mode && low.d_bp) ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
+    rp.counters = d->d_counters.get();
+    rp.safe = d->d_safe.get(); rp.galign = d->d_galign.get();
+    rp.bp_clear = bits_mode ? nullptr : low.d_bp.get();
+    rp.bp_words = (!bits_mode && !low.d_bp.empty()) ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
     // 4 CTAs are resident per SM (64 registers x 256 threads); 16 per SM = four waves of equal shares, which
     // balances the very uneven per-candidate cost (row-wise early exit) better than one persistent wave
     // (measured: 4 -> 251 us, 8 -> 241, 12..32 -> 229)
@@ -1654,10 +1595,10 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
   if (px.world > 0) {
     // collector: waits for all ranks' frame flags, packs the blocks into the ordinary result block
     CU(launch_pdl(k_peer_collect, dim3(1), dim3(1024), 0, st, px, d->px_seq, (int32_t)d->px_cap, d->d_res, (int32_t)d->res_cap,
-                  d->d_counters + 2, d->px_timeout_ns));
+                  d->d_counters.get() + 2, d->px_timeout_ns));
     ++d->launches;
   }
-  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[6], st));
+  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[6].get(), st));
   return LM_OK;
 }
 
@@ -1665,11 +1606,11 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
 #define LM_FIRST_FETCH 4096
 
 static int enqueue_readback(lm_detector* d) {
-  cudaStream_t st = d->stream;
+  cudaStream_t st = d->stream.get();
   const int64_t first = std::min<int64_t>(d->res_cap, LM_FIRST_FETCH);
-  CU(cudaMemcpyAsync(d->h_res, d->d_res, sizeof(lm_result_header) + sizeof(lm_record) * (size_t)first,
+  CU(cudaMemcpyAsync(d->h_res.get(), d->d_res, sizeof(lm_result_header) + sizeof(lm_record) * (size_t)first,
                      cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(d->h_counters, d->d_counters, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(d->h_counters.get(), d->d_counters.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   d->h_valid = first;
   return LM_OK;
 }
@@ -1677,55 +1618,28 @@ static int enqueue_readback(lm_detector* d) {
 static int ensure_run_buffers(lm_detector* d) {
   const int64_t n_work = d->shard_count;
   const LevelHost& low = d->lv[d->L - 1];
-  const size_t need_m = (size_t)std::max<int64_t>(n_work, 1) * low.nwords;
-  if (need_m > d->mask_elems) {
-    cudaFree(d->d_mask);
-    d->d_mask = nullptr;
-    d->mask_elems = need_m;
-    CU(cudaMalloc(&d->d_mask, sizeof(uint32_t) * need_m));
-  }
-  const size_t need_r = (size_t)std::max<int64_t>(n_work, 1) * low.plane;
-  if (need_r > d->raw_elems) {
-    cudaFree(d->d_raw);
-    d->d_raw = nullptr;
-    d->raw_elems = need_r;
-    CU(cudaMalloc(&d->d_raw, sizeof(uint16_t) * need_r));
-  }
+  CU(d->d_mask.reserve((size_t)std::max<int64_t>(n_work, 1) * low.nwords));
+  CU(d->d_raw.reserve((size_t)std::max<int64_t>(n_work, 1) * low.plane));
   // ordered candidate list + survivor list: worst case one entry per (template, cell); capped (a frame that overflows
   // the cap is redone from k_refine_prep with a larger list, like the result block)
   {
     const int64_t worst = std::max<int64_t>(n_work, 1) * low.plane;
     const int64_t want = std::min<int64_t>(worst, std::max<int64_t>(LM_CAND_DEFAULT, d->cand_need));
-    if (want > d->cand_cap) {
-      cudaFree(d->d_cand); cudaFree(d->d_surv); cudaFree(d->d_surv2);
-      d->d_cand = nullptr; d->d_surv = nullptr; d->d_surv2 = nullptr;
-      d->cand_cap = want;
-      CU(cudaMalloc(&d->d_cand, sizeof(uint2) * (size_t)want));
-      CU(cudaMalloc(&d->d_surv, sizeof(uint32_t) * (size_t)want));
-      CU(cudaMalloc(&d->d_surv2, sizeof(uint32_t) * (size_t)want));
+    if (want > cand_cap(d)) {
+      d->d_cand.reset(); d->d_surv.reset(); d->d_surv2.reset();
+      CU(d->d_cand.assign((size_t)want));
+      CU(d->d_surv.assign((size_t)want));
+      CU(d->d_surv2.assign((size_t)want));
     }
   }
   if (d->px_rank >= 0 && d->res_external) return fail(LM_E_STATE, "lm_set_result_buffer and a connected peer exchange exclude each other");
-  if (d->px_rank >= 0 && d->res_cap_own < d->px_cap * d->px_world) {
-    cudaFree(d->d_res_own);
-    d->d_res_own = nullptr;
-    d->res_cap_own = d->px_cap * d->px_world;
-    CU(cudaMalloc(&d->d_res_own, sizeof(lm_result_header) + sizeof(lm_record) * (size_t)d->res_cap_own));
-  }
+  if (d->px_rank >= 0) CU(d->d_res_own.reserve(res_bytes(d->px_cap * d->px_world)));
   if (!d->res_external) {
-    if (d->res_cap_own == 0) {
-      d->res_cap_own = 1 << 16;
-      CU(cudaMalloc(&d->d_res_own, sizeof(lm_result_header) + sizeof(lm_record) * (size_t)d->res_cap_own));
-    }
-    d->d_res = d->d_res_own;
-    d->res_cap = d->res_cap_own;
+    if (d->d_res_own.empty()) CU(d->d_res_own.assign(res_bytes(1 << 16)));
+    d->d_res = reinterpret_cast<lm_result_header*>(d->d_res_own.get());
+    d->res_cap = res_records(d->d_res_own.size());
   }
-  if (d->h_res_cap < d->res_cap) {
-    cudaFreeHost(d->h_res);
-    d->h_res = nullptr;
-    d->h_res_cap = d->res_cap;
-    CU(cudaMallocHost(&d->h_res, sizeof(lm_result_header) + sizeof(lm_record) * (size_t)d->h_res_cap));
-  }
+  CU(d->h_res.reserve(res_bytes(d->res_cap)));
   return LM_OK;
 }
 
@@ -1733,25 +1647,19 @@ static int ensure_run_buffers(lm_detector* d) {
 // outputs of the frame are still in place).  The header travels through a stack copy (the pinned staging block is
 // reallocated by ensure_run_buffers) with the new capacity patched in.
 static int grow_and_rerun(lm_detector* d) {
-  lm_result_header hdr = *d->h_res;
+  lm_result_header hdr = *hres(d);
   const bool more_records = (int64_t)hdr.count > d->res_cap;
-  const bool more_cands = (int64_t)hdr.coarse_candidates > d->cand_cap;
+  const bool more_cands = (int64_t)hdr.coarse_candidates > cand_cap(d);
   if (more_records && d->res_external)
     return fail(LM_E_CAPACITY, "%d records kept, caller's result buffer holds %lld", hdr.count, (long long)d->res_cap);
   if (d->px_rank >= 0)
     return fail(LM_E_CAPACITY, "%d records kept of %d candidates: beyond the result block (%lld) or the candidate list (%lld) of a "
-                "connected peer exchange", hdr.count, hdr.coarse_candidates, (long long)d->res_cap, (long long)d->cand_cap);
-  CU(cudaStreamSynchronize(d->stream));
+                "connected peer exchange", hdr.count, hdr.coarse_candidates, (long long)d->res_cap, (long long)cand_cap(d));
+  CU(cudaStreamSynchronize(d->stream.get()));
   if (more_cands) d->cand_need = (int64_t)hdr.coarse_candidates;  // ensure_run_buffers reallocates the lists
   if (more_records || (more_cands && !d->res_external)) {
     // with a truncated candidate list the kept count is a lower bound: leave room, a second pass grows again if needed
-    const int64_t want = std::max<int64_t>((int64_t)hdr.count * 2, d->res_cap_own);
-    if (want > d->res_cap_own) {
-      cudaFree(d->d_res_own);
-      d->d_res_own = nullptr;
-      d->res_cap_own = want;
-      CU(cudaMalloc(&d->d_res_own, sizeof(lm_result_header) + sizeof(lm_record) * (size_t)d->res_cap_own));
-    }
+    CU(d->d_res_own.reserve(res_bytes((int64_t)hdr.count * 2)));
   }
   int rc = ensure_run_buffers(d);
   if (rc) return rc;
@@ -1762,7 +1670,7 @@ static int grow_and_rerun(lm_detector* d) {
   if (rc) return rc;
   rc = enqueue_readback(d);
   if (rc) return rc;
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaStreamSynchronize(d->stream.get()));
   CU(cudaGetLastError());
   return LM_OK;
 }
@@ -1818,7 +1726,7 @@ extern "C" int lm_complete(lm_detector* d) {
   CU(cudaSetDevice(d->device));
   int rc = enqueue_readback(d);
   if (rc) return rc;
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaStreamSynchronize(d->stream.get()));
   CU(cudaGetLastError());
   if (d->px_rank >= 0) {
     if (d->h_counters[2] == 1)
@@ -1828,7 +1736,7 @@ extern "C" int lm_complete(lm_detector* d) {
       return fail(LM_E_CAPACITY, "peer exchange: a shard kept more than %lld records (capacity given to lm_peer_export)",
                   (long long)d->px_cap);
   }
-  for (int pass = 0; pass < 3 && ((int64_t)d->h_res->count > d->res_cap || (int64_t)d->h_res->coarse_candidates > d->cand_cap); ++pass) {
+  for (int pass = 0; pass < 3 && ((int64_t)hres(d)->count > d->res_cap || (int64_t)hres(d)->coarse_candidates > cand_cap(d)); ++pass) {
     rc = grow_and_rerun(d);
     if (rc) return rc;
   }
@@ -1849,7 +1757,7 @@ extern "C" int lm_set_result_buffer(lm_detector* d, void* d_block, int64_t capac
   if (capacity_records > 0x7FFFFFFF) return fail(LM_E_INVALID, "capacity too large");
   if (d_block && d->px_rank >= 0) return fail(LM_E_STATE, "lm_set_result_buffer and a connected peer exchange exclude each other");
   CU(cudaSetDevice(d->device));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaStreamSynchronize(d->stream.get()));
   d->res_external = d_block != nullptr;
   if (d->res_external) {
     d->d_res = (lm_result_header*)d_block;
@@ -1876,11 +1784,11 @@ extern "C" int lm_peer_export(lm_detector* d, int world, int64_t capacity_record
   if (capacity_records < 1 || capacity_records > (1 << 24)) return fail(LM_E_INVALID, "capacity outside 1..2^24");
   if (peer_buffer_bytes(world, capacity_records) > 0xF0000000ull) return fail(LM_E_INVALID, "exchange buffer too large");
   CU(cudaSetDevice(d->device));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaStreamSynchronize(d->stream.get()));
   peer_release(d);
   const size_t bytes = peer_buffer_bytes(world, capacity_records);
-  CU(cudaMalloc(&d->px_buf, bytes));
-  CU(cudaMemset(d->px_buf, 0, bytes));
+  CU(d->px_buf.assign(bytes));
+  CU(cudaMemset(d->px_buf.get(), 0, bytes));
   CU(cudaDeviceSynchronize());
   d->px_world = world;
   d->px_cap = capacity_records;
@@ -1896,7 +1804,7 @@ extern "C" int lm_peer_export(lm_detector* d, int world, int64_t capacity_record
   if (handle_out) {
     static_assert(sizeof(cudaIpcMemHandle_t) <= LM_PEER_HANDLE_BYTES, "IPC handle size");
     cudaIpcMemHandle_t h;
-    CU(cudaIpcGetMemHandle(&h, d->px_buf));
+    CU(cudaIpcGetMemHandle(&h, d->px_buf.get()));
     memset(handle_out, 0, LM_PEER_HANDLE_BYTES);
     memcpy(handle_out, &h, sizeof(h));
   }
@@ -1905,15 +1813,15 @@ extern "C" int lm_peer_export(lm_detector* d, int world, int64_t capacity_record
 
 extern "C" int lm_peer_base(lm_detector* d, void** base) {
   if (!d || !base) return fail(LM_E_INVALID, "null argument");
-  if (!d->px_buf) return fail(LM_E_STATE, "lm_peer_export has not been called");
-  *base = d->px_buf;
+  if (d->px_buf.empty()) return fail(LM_E_STATE, "lm_peer_export has not been called");
+  *base = d->px_buf.get();
   return LM_OK;
 }
 
 static int peer_connect_common(lm_detector* d, int rank, int world) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d) return fail(LM_E_INVALID, "null detector");
-  if (!d->px_buf) return fail(LM_E_STATE, "lm_peer_export has not been called");
+  if (d->px_buf.empty()) return fail(LM_E_STATE, "lm_peer_export has not been called");
   if (world != d->px_world) return fail(LM_E_INVALID, "world %d differs from the exported one (%d)", world, d->px_world);
   if (rank < 0 || rank >= world) return fail(LM_E_INVALID, "rank %d outside 0..%d", rank, world - 1);
   if (d->px_rank >= 0) return fail(LM_E_STATE, "already connected");
@@ -1930,8 +1838,8 @@ static int peer_upload_descriptor(lm_detector* d) {
   px.slot_bytes = px.block_bytes * (uint32_t)d->px_world;
   px.flags_offset = 2u * px.slot_bytes;
   d->h_px = px;
-  if (!d->d_px) CU(cudaMalloc(&d->d_px, sizeof(PeerExchange)));
-  CU(cudaMemcpy(d->d_px, &px, sizeof(px), cudaMemcpyHostToDevice));
+  CU(d->d_px.reserve(1));
+  CU(cudaMemcpy(d->d_px.get(), &px, sizeof(px), cudaMemcpyHostToDevice));
   return LM_OK;
 }
 
@@ -1941,7 +1849,7 @@ extern "C" int lm_peer_connect(lm_detector* d, int rank, int world, const uint8_
   if (!handles) return fail(LM_E_INVALID, "null handles");
   CU(cudaSetDevice(d->device));
   for (int r = 0; r < world; ++r) {
-    if (r == rank) { d->px_base[r] = d->px_buf; continue; }
+    if (r == rank) { d->px_base[r] = d->px_buf.get(); continue; }
     cudaIpcMemHandle_t h;
     memcpy(&h, handles + (size_t)r * LM_PEER_HANDLE_BYTES, sizeof(h));
     void* ptr = nullptr;
@@ -1980,7 +1888,7 @@ extern "C" int lm_peer_connect_local(lm_detector* d, int rank, int world, void* 
     }
     d->px_base[r] = (uint8_t*)bases[r];
   }
-  d->px_base[rank] = d->px_buf;
+  d->px_base[rank] = d->px_buf.get();
   d->px_ipc = false;
   d->px_rank = rank;
   d->have_run = false;
@@ -1998,7 +1906,7 @@ extern "C" int lm_peer_disconnect(lm_detector* d) {
   if (!d) return fail(LM_E_INVALID, "null detector");
   if (d->device < 0) return LM_OK;
   CU(cudaSetDevice(d->device));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaStreamSynchronize(d->stream.get()));
   peer_release(d);
   d->have_run = false;
   return LM_OK;
@@ -2059,14 +1967,14 @@ extern "C" int lm_fetch_records(lm_detector* d, lm_record* out, int64_t cap, int
   if (!d || !n_out) return fail(LM_E_INVALID, "null argument");
   if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
   CU(cudaSetDevice(d->device));
-  const int64_t n = d->h_res->count;
+  const int64_t n = hres(d)->count;
   *n_out = n;
   if (n > cap) return fail(LM_E_CAPACITY, "%lld records, capacity %lld", (long long)n, (long long)cap);
-  lm_record* h = reinterpret_cast<lm_record*>(d->h_res + 1);
+  lm_record* h = reinterpret_cast<lm_record*>(hres(d) + 1);
   if (n > d->h_valid) {  // the rest, beyond the first-fetch window
     CU(cudaMemcpyAsync(h + d->h_valid, reinterpret_cast<lm_record*>(d->d_res + 1) + d->h_valid,
-                       sizeof(lm_record) * (size_t)(n - d->h_valid), cudaMemcpyDeviceToHost, d->stream));
-    CU(cudaStreamSynchronize(d->stream));
+                       sizeof(lm_record) * (size_t)(n - d->h_valid), cudaMemcpyDeviceToHost, d->stream.get()));
+    CU(cudaStreamSynchronize(d->stream.get()));
     d->h_valid = n;
   }
   if (n > 0) {
@@ -2172,18 +2080,11 @@ extern "C" int lm_set_boxes(lm_detector* d, const int32_t* wh, int64_t n_templat
 }
 
 static int prepare_post(lm_detector* d) {
-  if (!d->d_post_out) {
-    CU(cudaMalloc(&d->d_post_out, sizeof(lm_match) * LM_POST_MAX));
-    CU(cudaMallocHost(&d->h_post_out, sizeof(lm_match) * LM_POST_MAX));
-    CU(cudaMalloc(&d->d_post_counts, sizeof(int32_t) * 4));
-    CU(cudaMallocHost(&d->h_post_counts, sizeof(int32_t) * 4));
-  }
-  if (d->post_live_cap < d->res_cap) {
-    cudaFree(d->d_post_live);
-    d->d_post_live = nullptr;
-    d->post_live_cap = d->res_cap;
-    CU(cudaMalloc(&d->d_post_live, (size_t)d->post_live_cap));
-  }
+  CU(d->d_post_out.reserve(LM_POST_MAX));
+  CU(d->h_post_out.reserve(LM_POST_MAX));
+  CU(d->d_post_counts.reserve(4));
+  CU(d->h_post_counts.reserve(4));
+  CU(d->d_post_live.reserve((size_t)d->res_cap));
   if (!d->post_dirty) return LM_OK;
   if (!d->boxes.empty() && (int64_t)d->boxes.size() != 2 * (int64_t)d->G) {
     d->boxes.clear();  // the bank changed under the caller's boxes
@@ -2207,14 +2108,9 @@ static int prepare_post(lm_detector* d) {
       q.height = d->boxes[2 * (size_t)g + 1];
     }
   }
-  if (d->post_info_n < (int64_t)info.size()) {
-    cudaFree(d->d_post_info);
-    d->d_post_info = nullptr;
-    d->post_info_n = (int64_t)info.size();
-    CU(cudaMalloc(&d->d_post_info, sizeof(PostInfo) * info.size()));
-  }
-  CU(cudaMemcpyAsync(d->d_post_info, info.data(), sizeof(PostInfo) * info.size(), cudaMemcpyHostToDevice, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(d->d_post_info.reserve(info.size()));
+  CU(cudaMemcpyAsync(d->d_post_info.get(), info.data(), sizeof(PostInfo) * info.size(), cudaMemcpyHostToDevice, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   d->post_dirty = false;
   return LM_OK;
 }
@@ -2230,11 +2126,11 @@ extern "C" int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k) 
   if (rc) return rc;
   PostParams p;
   p.hdr = d->d_res; p.capacity = (int32_t)d->res_cap;
-  p.info = d->d_post_info; p.n_sel = (int32_t)d->sel.size();
+  p.info = d->d_post_info.get(); p.n_sel = (int32_t)d->sel.size();
   p.iou_threshold = iou_threshold; p.top_k = top_k;
-  p.out = d->d_post_out; p.out_capacity = LM_POST_MAX;
-  p.out_counts = d->d_post_counts; p.live = d->d_post_live;
-  CU(launch_pdl(k_post_nms, dim3(1), dim3(1024), 0, d->stream, p));
+  p.out = d->d_post_out.get(); p.out_capacity = LM_POST_MAX;
+  p.out_counts = d->d_post_counts.get(); p.live = d->d_post_live.get();
+  CU(launch_pdl(k_post_nms, dim3(1), dim3(1024), 0, d->stream.get(), p));
   ++d->launches;
   d->post_iou = iou_threshold;
   d->post_top_k = top_k;
@@ -2251,12 +2147,12 @@ static int complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_
   if (!d || !n_out) return fail(LM_E_INVALID, "null argument");
   if (!d->post_pending) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
   CU(cudaSetDevice(d->device));
-  cudaStream_t st = d->stream;
-  CU(cudaMemcpyAsync(d->h_post_counts, d->d_post_counts, sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+  cudaStream_t st = d->stream.get();
+  CU(cudaMemcpyAsync(d->h_post_counts.get(), d->d_post_counts.get(), sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
   // the common top-k is small: fetch a first window with the counts, the rest only if there is more
   const int first = 16;
-  if (fetch) CU(cudaMemcpyAsync(d->h_post_out, d->d_post_out, sizeof(lm_match) * first, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(d->h_counters, d->d_counters, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (fetch) CU(cudaMemcpyAsync(d->h_post_out.get(), d->d_post_out.get(), sizeof(lm_match) * first, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(d->h_counters.get(), d->d_counters.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
   d->post_pending = false;
@@ -2265,12 +2161,12 @@ static int complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_
   if (d->px_rank >= 0 && d->h_counters[2] == 2) return fail(LM_E_CAPACITY, "peer exchange: a shard kept more than %lld records", (long long)d->px_cap);
   const int64_t n = d->h_post_counts[0];
   if (n_records) *n_records = d->h_post_counts[1];
-  if ((int64_t)d->h_post_counts[1] > d->res_cap || (int64_t)d->h_post_counts[3] > d->cand_cap) {
+  if ((int64_t)d->h_post_counts[1] > d->res_cap || (int64_t)d->h_post_counts[3] > cand_cap(d)) {
     // the NMS did not see every record: grow the block like lm_complete does, redo the refinement, run the NMS again
     if (d->post_retry || d->res_external || d->px_rank >= 0)
       return fail(LM_E_CAPACITY, "%d records kept, the result block holds %lld: the NMS did not see all of them", d->h_post_counts[1],
                   (long long)d->res_cap);
-    CU(cudaMemcpyAsync(d->h_res, d->d_res, sizeof(lm_result_header), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(d->h_res.get(), d->d_res, sizeof(lm_result_header), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     int rc = grow_and_rerun(d);
     if (rc) return rc;
@@ -2293,10 +2189,10 @@ static int complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_
   if (!fetch) return LM_OK;
   if (n > cap) return fail(LM_E_CAPACITY, "%lld survivors, capacity %lld", (long long)n, (long long)cap);
   if (n > first) {
-    CU(cudaMemcpyAsync(d->h_post_out + first, d->d_post_out + first, sizeof(lm_match) * (size_t)(n - first), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(d->h_post_out.get() + first, d->d_post_out.get() + first, sizeof(lm_match) * (size_t)(n - first), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
   }
-  if (n > 0 && out) memcpy(out, d->h_post_out, sizeof(lm_match) * (size_t)n);
+  if (n > 0 && out) memcpy(out, d->h_post_out.get(), sizeof(lm_match) * (size_t)n);
   return LM_OK;
 }
 
@@ -2346,9 +2242,9 @@ static int enqueue_pose(lm_detector* d) {
     if (rc) return rc;
   }
   PoseEnqueue e;
-  e.o = {d->fe[0].rows, d->fe[0].cols, d->pose_use_scene, d->pose_max_iter, d->pose_frame_estimation, d->stream, share ? &sh : nullptr};
-  e.d_surv = d->d_post_out; e.d_counts = d->d_post_counts;
-  e.d_scene = d->fe_depth;
+  e.o = {d->fe[0].rows, d->fe[0].cols, d->pose_use_scene, d->pose_max_iter, d->pose_frame_estimation, d->stream.get(), share ? &sh : nullptr};
+  e.d_surv = d->d_post_out.get(); e.d_counts = d->d_post_counts.get();
+  e.d_scene = d->fe_depth.get();
   memcpy(e.sK, d->pose_sK, sizeof(e.sK));
   e.bound = d->post_top_k > 0 ? std::min(d->post_top_k, LM_POST_MAX) : LM_POST_MAX;
   return pose_stage_enqueue(d->pose, e, &d->launches);
@@ -2383,14 +2279,14 @@ extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, do
   int rc = lm_complete_post(d, out, cap, n_out, n_records);  // waits; on the capacity retry it runs the pose stage again
   d->pose_pending = false;
   if (rc) return rc;
-  rc = pose_stage_finish(d->pose, d->stream, d->h_post_out, *n_out, R_out, t_out, residual);
+  rc = pose_stage_finish(d->pose, d->stream.get(), d->h_post_out.get(), *n_out, R_out, t_out, residual);
   if (rc) return rc;
   pose_stage_stats(d->pose, *n_out, d->pose_stats);
   return LM_OK;
 }
 
 static int enqueue_pose_nms(lm_detector* d) {
-  return pose_stage_enqueue_nms(d->pose, d->d_post_out, d->d_post_counts, d->pose_nms_thr, d->stream, &d->launches);
+  return pose_stage_enqueue_nms(d->pose, d->d_post_out.get(), d->d_post_counts.get(), d->pose_nms_thr, d->stream.get(), &d->launches);
 }
 
 extern "C" int lm_enqueue_pose_nms(lm_detector* d, double translation_threshold_mm) {
@@ -2418,7 +2314,7 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
   d->pose_pending = false;
   d->pose_nms_pending = false;
   if (rc) return rc;
-  rc = pose_stage_finish_nms(d->pose, d->stream, out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
+  rc = pose_stage_finish_nms(d->pose, d->stream.get(), out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
   if (rc) return rc;
   pose_stage_stats(d->pose, n_surv, d->pose_stats);
   return LM_OK;
@@ -2456,7 +2352,7 @@ extern "C" int lm_set_depth_gate(lm_detector* d, int on, double tolerance) {
 // with a connected exchange, else the result block (a result-block retry carries the header over to the grown block).
 static const lm_result_header* scan_header(const lm_detector* d) {
   if (d->px_rank >= 0)
-    return reinterpret_cast<const lm_result_header*>(d->px_buf + (size_t)(d->px_seq & 1) * d->h_px.slot_bytes +
+    return reinterpret_cast<const lm_result_header*>(d->px_buf.get() + (size_t)(d->px_seq & 1) * d->h_px.slot_bytes +
                                                      (size_t)d->h_px.rank * d->h_px.block_bytes);
   return d->d_res;
 }
@@ -2470,10 +2366,10 @@ extern "C" int lm_depth_gate_stats(lm_detector* d, int64_t* out4) {
   std::vector<uint32_t> cells((size_t)low.plane);
   unsigned before = 0;
   lm_result_header hdr;
-  CU(cudaMemcpyAsync(cells.data(), d->d_cells, sizeof(uint32_t) * cells.size(), cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaMemcpyAsync(&before, d->d_gate_before, sizeof(unsigned), cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaMemcpyAsync(&hdr, scan_header(d), sizeof(hdr), cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaMemcpyAsync(cells.data(), d->d_cells.get(), sizeof(uint32_t) * cells.size(), cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaMemcpyAsync(&before, d->d_gate_before.get(), sizeof(unsigned), cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaMemcpyAsync(&hdr, scan_header(d), sizeof(hdr), cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   int64_t empty = 0;
   for (uint32_t c : cells) empty += (c & 0xFFFFu) > (c >> 16);
   out4[0] = before;
@@ -2530,7 +2426,7 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     int rc = check_device_frame(d, dev->frame(f), rows, cols, dev->stream, lrows, lcols);
     if (rc) return fail(rc, "frame %d: %s", f, std::string(g_err).c_str());
   }
-  cudaStream_t st = d->stream;
+  cudaStream_t st = d->stream.get();
   d->pose_pending = false;  // a batch starts new frames: a pending single-frame pose stage is abandoned
   d->pose_nms_pending = false;
   const int bound = top_k > 0 ? top_k : LM_POST_MAX;  // most survivors k_post_nms writes per frame
@@ -2554,8 +2450,8 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     rc = complete_post(d, pose_nms ? nullptr : surv.data() + first[f], bound, &n, &n_rec, !pose_nms);
     if (rc) return rc;
     // the next frame's post stage and upload overwrite both: copy them out first, on the stream
-    if (n > 0) CU(cudaMemcpyAsync(d_surv + first[f], d->d_post_out, sizeof(lm_match) * (size_t)n, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(d_scene + f * n0, d->fe_depth, sizeof(uint16_t) * n0, cudaMemcpyDeviceToDevice, st));
+    if (n > 0) CU(cudaMemcpyAsync(d_surv + first[f], d->d_post_out.get(), sizeof(lm_match) * (size_t)n, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(d_scene + f * n0, d->fe_depth.get(), sizeof(uint16_t) * n0, cudaMemcpyDeviceToDevice, st));
     first[f + 1] = first[f] + n;
     frame_counts[4 * f + 1] = n;
     frame_counts[4 * f + 3] = n_rec;
@@ -2628,7 +2524,7 @@ extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantize
   if (rc) return rc;
   rc = lm_run(d, threshold);
   if (rc) return rc;
-  const int64_t n = d->h_res->count;
+  const int64_t n = hres(d)->count;
   std::vector<lm_record> rec((size_t)n);
   int64_t got = 0;
   rc = lm_fetch_records(d, rec.data(), n, &got);
@@ -2642,7 +2538,7 @@ extern "C" int lm_match_images(lm_detector* d, const uint8_t* rgb, const uint16_
   if (rc) return rc;
   rc = lm_run(d, threshold);
   if (rc) return rc;
-  const int64_t n = d->h_res->count;
+  const int64_t n = hres(d)->count;
   std::vector<lm_record> rec((size_t)n);
   int64_t got = 0;
   rc = lm_fetch_records(d, rec.data(), n, &got);
@@ -2659,8 +2555,8 @@ extern "C" int lm_debug_quantized(lm_detector* d, int level, int modality, uint8
   const int64_t n = (int64_t)lv.rows * lv.cols;
   if (n > cap) return fail(LM_E_CAPACITY, "need %lld bytes", (long long)n);
   CU(cudaSetDevice(d->device));
-  CU(cudaMemcpyAsync(out, lv.q_src[modality], (size_t)n, cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaMemcpyAsync(out, lv.q_src[modality], (size_t)n, cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   return LM_OK;
 }
 
@@ -2681,8 +2577,8 @@ extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality,
     if (rc) return rc;
     d->last_planes_level = -1;
   }
-  CU(cudaMemcpyAsync(out, lv.d_lm + (size_t)modality * lv.mod_stride, lv.mod_stride, cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaMemcpyAsync(out, lv.d_lm.get() + (size_t)modality * lv.mod_stride, lv.mod_stride, cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   return LM_OK;
 }
 
@@ -2696,8 +2592,8 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   if (cap < LM_PLAN_ENTRIES) return fail(LM_E_CAPACITY, "need %d entries", LM_PLAN_ENTRIES);
   CU(cudaSetDevice(d->device));
   int queue[4];
-  CU(cudaMemcpyAsync(queue, d->d_queue, sizeof(queue), cudaMemcpyDeviceToHost, d->stream));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaMemcpyAsync(queue, d->d_queue.get(), sizeof(queue), cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
   const LevelHost& low = d->lv[d->L - 1];
   K1Plan k1;
   plan_k1(d, planes_level(d), true, k1);
@@ -2708,7 +2604,7 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   out[2] = pl >= 0 ? k1.p.lv[pl].pseg : 0;
   out[3] = (int32_t)k1.smem;
   out[4] = low.rounds;
-  out[5] = low.d_bp ? 1 : 0;
+  out[5] = !low.d_bp.empty() ? 1 : 0;
   out[6] = d->n_items_bits;
   out[7] = d->n_items_bytes;
   if (d->n_items_bits > 0) {
@@ -2726,7 +2622,7 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   out[14] = eligible;
   out[15] = d->gate_frame ? 1 : 0;
   // work items of the refinement kernels that ran (-1: it did not run); see enqueue_stages
-  const int total = (int)std::min<int64_t>(d->h_res->coarse_candidates, d->cand_cap);
+  const int total = (int)std::min<int64_t>(hres(d)->coarse_candidates, cand_cap(d));
   const bool filter = use_filter(d), bits_mode = use_bits(d);
   if (filter) out[16] = total;
   if (bits_mode) out[17] = std::min(queue[1], total);
@@ -2741,10 +2637,10 @@ extern "C" int lm_counters(lm_detector* d, int64_t* out8) {
   if (!d || !out8) return fail(LM_E_INVALID, "null argument");
   if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
   out8[0] = d->shard_count;
-  out8[1] = d->h_res->coarse_candidates;
+  out8[1] = hres(d)->coarse_candidates;
   out8[2] = d->alg_scan_bytes;
   out8[3] = (int64_t)(d->h_counters[0] + d->h_counters[4]) * 256;  // the reference's refinement work, whoever disposed of it
-  out8[4] = d->h_res->count;
+  out8[4] = hres(d)->count;
   out8[5] = (int64_t)d->h_counters[1] * 16;
   out8[6] = (int64_t)d->h_counters[4] * 256;  // ... of which: candidates the filter dropped
   out8[7] = (int64_t)d->h_counters[5] * 4;    // bytes of H-planes the filter read
@@ -2755,16 +2651,15 @@ extern "C" int lm_set_timing(lm_detector* d, int slots) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d) return fail(LM_E_INVALID, "null detector");
   CU(cudaSetDevice(d->device));
-  CU(cudaStreamSynchronize(d->stream));
-  for (cudaEvent_t e : d->tev) cudaEventDestroy(e);
+  CU(cudaStreamSynchronize(d->stream.get()));
+  // the old events go first; timing is on only once every new one exists
   d->tev.clear();
   d->timing_runs = 0;
+  d->timing = false;
+  std::vector<Event> tev((size_t)std::max(slots, 0) * LM_TEV);
+  for (Event& e : tev) CU(e.create(cudaEventDefault));
+  d->tev.swap(tev);
   d->timing = slots > 0;
-  for (int i = 0; i < slots * LM_TEV; ++i) {
-    cudaEvent_t e;
-    CU(cudaEventCreate(&e));
-    d->tev.push_back(e);
-  }
   return LM_OK;
 }
 
@@ -2772,7 +2667,7 @@ extern "C" int lm_stage_times(lm_detector* d, float* out8) {
   if (!d || !out8) return fail(LM_E_INVALID, "null argument");
   if (!d->timing || d->timing_runs == 0) return fail(LM_E_STATE, "timing not enabled / no run recorded");
   CU(cudaSetDevice(d->device));
-  CU(cudaStreamSynchronize(d->stream));
+  CU(cudaStreamSynchronize(d->stream.get()));
   const int64_t slots = (int64_t)d->tev.size() / LM_TEV;
   const int64_t n = std::min<int64_t>(slots, d->timing_runs);
   // events: 0 start | 1 linear memories | 2 coarse scan | 3 offsets (+ upper-level linear memories) | 4 candidate list +
@@ -2780,10 +2675,10 @@ extern "C" int lm_stage_times(lm_detector* d, float* out8) {
   static const int from[8] = {0, 1, 2, 3, 0, 3, 4, 5}, to[8] = {1, 2, 3, 6, 6, 4, 5, 6};
   double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   for (int64_t k = 0; k < n; ++k) {
-    cudaEvent_t* ev = d->tev.data() + LM_TEV * k;
+    const Event* ev = d->tev.data() + LM_TEV * k;
     for (int i = 0; i < 8; ++i) {
       float ms;
-      CU(cudaEventElapsedTime(&ms, ev[from[i]], ev[to[i]]));
+      CU(cudaEventElapsedTime(&ms, ev[from[i]].get(), ev[to[i]].get()));
       acc[i] += ms * 1000.0;
     }
   }

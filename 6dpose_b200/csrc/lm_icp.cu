@@ -25,6 +25,7 @@
 
 #include "linemod_b200.h"
 #include "lm_pose.h"
+#include "lm_buffer.h"
 
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
@@ -35,6 +36,7 @@
 
 #include <algorithm>
 #include <limits>
+#include <memory>
 #include <thread>
 #include <vector>
 
@@ -658,20 +660,20 @@ __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShare
 // --------------------------------------------------------------------------------------------
 struct lm_icp {
   int device = 0;
-  cudaStream_t stream = nullptr;
-  double* d_pts = nullptr; double* d_nrm = nullptr; size_t cap_pts = 0;
-  IcpJob* d_jobs = nullptr; IcpOut* d_outs = nullptr; size_t cap_jobs = 0;
-  IcpOut* h_outs = nullptr; size_t cap_houts = 0;
+  Stream stream;  // streams and events first: they outlive the buffers
+  Event ev0, ev1;
+  DeviceArray<double> d_pts, d_nrm;  // [points][3]
+  DeviceArray<IcpJob> d_jobs; DeviceArray<IcpOut> d_outs;
+  PinnedArray<IcpOut> h_outs;
   int64_t launches = 0;
   bool use_scene_cloud = false;  // non-reference option: register against the scene cloud
   int estimation = LM_ICP_POINT_TO_PLANE;
   int last_points = 0, last_iterations = 0;
   double last_rmse = 0;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   float last_kernel_us = 0;
   // lm_icp_set_capture: the kernels' intermediate results of the last lm_icp_process_batch
   bool capture = false;
-  int32_t* d_knn = nullptr; int32_t* d_corr = nullptr; size_t cap_capture = 0;
+  DeviceArray<int32_t> d_knn, d_corr;  // [points][ICP_KNN], [points][2]
   struct {
     int estimation = LM_ICP_POINT_TO_PLANE;  // point-to-point computes no normals and no neighbour lists
     std::vector<IcpJob> jobs;
@@ -690,24 +692,19 @@ extern "C" int lm_icp_create(int device, lm_icp** out) {
     return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
   if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
   CUI(cudaSetDevice(device));
-  lm_icp* h = new lm_icp();
+  std::unique_ptr<lm_icp> h(new lm_icp());
   h->device = device;
-  CUI(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-  CUI(cudaEventCreate(&h->ev0));
-  CUI(cudaEventCreate(&h->ev1));
-  *out = h;
+  CUI(h->stream.create(cudaStreamNonBlocking));
+  CUI(h->ev0.create(cudaEventDefault));
+  CUI(h->ev1.create(cudaEventDefault));
+  *out = h.release();
   return LM_OK;
 }
 
 extern "C" void lm_icp_destroy(lm_icp* h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  cudaStreamSynchronize(h->stream);
-  cudaFree(h->d_pts); cudaFree(h->d_nrm); cudaFree(h->d_jobs); cudaFree(h->d_outs);
-  cudaFree(h->d_knn); cudaFree(h->d_corr);
-  cudaFreeHost(h->h_outs);
-  cudaEventDestroy(h->ev0); cudaEventDestroy(h->ev1);
-  cudaStreamDestroy(h->stream);
+  cudaStreamSynchronize(h->stream.get());
   delete h;
 }
 
@@ -911,50 +908,45 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   }
   const size_t npts = all.size() / 3;
   if (!jobs.empty()) {
-    if (npts > h->cap_pts) {
-      cudaFree(h->d_pts); cudaFree(h->d_nrm);
-      h->cap_pts = std::max<size_t>(npts * 2, 4096);
-      CUI(cudaMalloc(&h->d_pts, h->cap_pts * 3 * sizeof(double)));
-      CUI(cudaMalloc(&h->d_nrm, h->cap_pts * 3 * sizeof(double)));
+    // a pair grows together, its second array allocated last: that one's size is the pair's
+    if (npts * 3 > h->d_nrm.size()) {
+      h->d_pts.reset(); h->d_nrm.reset();
+      const size_t cap = std::max<size_t>(npts * 2, 4096) * 3;
+      CUI(h->d_pts.assign(cap));
+      CUI(h->d_nrm.assign(cap));
     }
-    if (jobs.size() > h->cap_jobs) {
-      cudaFree(h->d_jobs); cudaFree(h->d_outs);
-      h->cap_jobs = std::max<size_t>(jobs.size() * 2, 16);
-      CUI(cudaMalloc(&h->d_jobs, h->cap_jobs * sizeof(IcpJob)));
-      CUI(cudaMalloc(&h->d_outs, h->cap_jobs * sizeof(IcpOut)));
+    if (jobs.size() > h->d_outs.size()) {
+      h->d_jobs.reset(); h->d_outs.reset();
+      const size_t cap = std::max<size_t>(jobs.size() * 2, 16);
+      CUI(h->d_jobs.assign(cap));
+      CUI(h->d_outs.assign(cap));
     }
-    if (jobs.size() > h->cap_houts) {
-      cudaFreeHost(h->h_outs);
-      h->cap_houts = std::max<size_t>(jobs.size() * 2, 16);
-      CUI(cudaMallocHost(&h->h_outs, h->cap_houts * sizeof(IcpOut)));
+    if (jobs.size() > h->h_outs.size()) CUI(h->h_outs.assign(std::max<size_t>(jobs.size() * 2, 16)));
+    if (h->capture && npts * 2 > h->d_corr.size()) {
+      h->d_knn.reset(); h->d_corr.reset();
+      CUI(h->d_knn.assign(npts * ICP_KNN));
+      CUI(h->d_corr.assign(npts * 2));
     }
-    if (h->capture && npts > h->cap_capture) {
-      cudaFree(h->d_knn); cudaFree(h->d_corr);
-      h->d_knn = nullptr; h->d_corr = nullptr; h->cap_capture = 0;
-      CUI(cudaMalloc(&h->d_knn, npts * ICP_KNN * sizeof(int32_t)));
-      CUI(cudaMalloc(&h->d_corr, npts * 2 * sizeof(int32_t)));
-      h->cap_capture = npts;
-    }
-    int32_t* knn_out = h->capture ? h->d_knn : nullptr;
-    int32_t* corr_out = h->capture ? h->d_corr : nullptr;
-    cudaStream_t st = h->stream;
-    if (npts) CUI(cudaMemcpyAsync(h->d_pts, all.data(), npts * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-    CUI(cudaMemcpyAsync(h->d_jobs, jobs.data(), jobs.size() * sizeof(IcpJob), cudaMemcpyHostToDevice, st));
-    CUI(cudaEventRecord(h->ev0, st));
+    int32_t* knn_out = h->capture ? h->d_knn.get() : nullptr;
+    int32_t* corr_out = h->capture ? h->d_corr.get() : nullptr;
+    cudaStream_t st = h->stream.get();
+    if (npts) CUI(cudaMemcpyAsync(h->d_pts.get(), all.data(), npts * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CUI(cudaMemcpyAsync(h->d_jobs.get(), jobs.data(), jobs.size() * sizeof(IcpJob), cudaMemcpyHostToDevice, st));
+    CUI(cudaEventRecord(h->ev0.get(), st));
     if (max_count > 0 && h->estimation == LM_ICP_POINT_TO_PLANE) {
       dim3 g((unsigned)((max_count + 127) / 128), (unsigned)jobs.size());
-      k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs, h->d_pts, h->d_nrm, knn_out);
+      k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), knn_out);
       ++h->launches;
     }
-    launch_icp<false>(h->estimation, (unsigned)jobs.size(), st, h->d_jobs, h->d_pts, h->d_nrm, h->d_outs, max_iterations, corr_out,
-                      PoseShareDev());
+    launch_icp<false>(h->estimation, (unsigned)jobs.size(), st, h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), h->d_outs.get(),
+                      max_iterations, corr_out, PoseShareDev());
     ++h->launches;
-    CUI(cudaEventRecord(h->ev1, st));
-    CUI(cudaMemcpyAsync(h->h_outs, h->d_outs, jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
+    CUI(cudaEventRecord(h->ev1.get(), st));
+    CUI(cudaMemcpyAsync(h->h_outs.get(), h->d_outs.get(), jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
     CUI(cudaGetLastError());
     float ms = 0;
-    CUI(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    CUI(cudaEventElapsedTime(&ms, h->ev0.get(), h->ev1.get()));
     h->last_kernel_us = ms * 1000.f;
   }
   if (h->capture) {
@@ -962,17 +954,17 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     c.estimation = h->estimation;
     c.jobs = jobs;
     c.job_of = job_of;
-    c.outs.assign(h->h_outs, h->h_outs + (jobs.empty() ? 0 : jobs.size()));
+    c.outs.assign(h->h_outs.get(), h->h_outs.get() + (jobs.empty() ? 0 : jobs.size()));
     c.pts = all;
     c.nrm.assign(npts * 3, 0.0);
     c.knn.assign(npts * ICP_KNN, -1);
     c.corr.assign(npts * 2, -1);
     if (npts) {
       if (c.estimation == LM_ICP_POINT_TO_PLANE) {
-        CUI(cudaMemcpy(c.nrm.data(), h->d_nrm, npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
-        CUI(cudaMemcpy(c.knn.data(), h->d_knn, npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        CUI(cudaMemcpy(c.nrm.data(), h->d_nrm.get(), npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+        CUI(cudaMemcpy(c.knn.data(), h->d_knn.get(), npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
       }
-      CUI(cudaMemcpy(c.corr.data(), h->d_corr, npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(c.corr.data(), h->d_corr.get(), npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
     }
   }
   for (int i = 0; i < n_hyp; ++i) {
@@ -1512,21 +1504,20 @@ struct lm_pose_stage {
   std::vector<int32_t> class_begin;
   bool dirty = true;           // the device copy of the renders is stale
   int64_t area_max = 0;        // largest crop
-  PoseTpl* d_tpl = nullptr; uint16_t* d_crops = nullptr; int32_t* d_class_begin = nullptr;
-  PoseRt* d_rt = nullptr;      // per template: R, t of its render (k_pose_nms composes the poses)
-  // per-frame buffers, sized for (bound, area_max)
-  int cap_bound = 0; int64_t cap_area = 0;
-  double* d_raw = nullptr; double* d_cpts = nullptr; double* d_pts = nullptr; double* d_nrm = nullptr;
-  unsigned long long* d_keys[2] = {nullptr, nullptr};
-  int32_t* d_vals[2] = {nullptr, nullptr};
-  int32_t* d_seg = nullptr;
-  IcpJob* d_jobs = nullptr; IcpOut* d_outs = nullptr;
-  int32_t* d_err = nullptr;  // [0] cloud overflow; shared stage: [1] a peer's poses did not arrive, [2] entries published
-  void* d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
-  IcpOut* h_outs = nullptr; int32_t* h_err = nullptr;
-  uint8_t* d_posed = nullptr;
+  DeviceArray<PoseTpl> d_tpl; DeviceArray<uint16_t> d_crops; DeviceArray<int32_t> d_class_begin;
+  DeviceArray<PoseRt> d_rt;    // per template: R, t of its render (k_pose_nms composes the poses)
+  // per-frame buffers for pose_slots() survivors of pose_area() points per crop (pose_buffers)
+  DeviceArray<double> d_raw, d_cpts, d_pts, d_nrm;
+  DeviceArray<unsigned long long> d_keys[2];
+  DeviceArray<int32_t> d_vals[2];
+  DeviceArray<int32_t> d_seg;
+  DeviceArray<IcpJob> d_jobs; DeviceArray<IcpOut> d_outs;
+  DeviceArray<int32_t> d_err;  // [0] cloud overflow; shared stage: [1] a peer's poses did not arrive, [2] entries published
+  DeviceArray<uint8_t> d_sort_tmp;
+  PinnedArray<IcpOut> h_outs; PinnedArray<int32_t> h_err;
+  DeviceArray<uint8_t> d_posed;
   // pose NMS output block: PoseNmsHead + NMS_THREADS PoseNmsOut (device, pinned copy)
-  uint8_t* d_nms = nullptr; uint8_t* h_nms = nullptr;
+  DeviceArray<uint8_t> d_nms; PinnedArray<uint8_t> h_nms;
   // the enqueued frame
   int bound = 0, srows = 0, scols = 0;
   // its pose stage: launches, shared over the exchange (frame share_seq, collector timeout share_timeout_ns)
@@ -1534,45 +1525,31 @@ struct lm_pose_stage {
   bool shared = false; int32_t share_seq = 0; unsigned long long share_timeout_ns = 0;
   // batch of frames (pose_batch_*): scene slots and survivors filled by the caller, then per survivor its frame, ICP
   // output and posed flag, and the pose NMS blocks (one head per frame, kept poses at the frame's survivor offset)
-  int64_t cap_bscene = 0, cap_bsurv = 0, cap_bS = 0; int cap_bframes = 0;
-  uint16_t* d_bscene = nullptr;
-  lm_match* d_bsurv = nullptr;
-  int32_t* d_bframe = nullptr;  // [cap_bS] frame of each survivor
-  IcpOut* d_bouts = nullptr; IcpOut* h_bouts = nullptr;
-  uint8_t* d_bposed = nullptr;
-  PoseNmsOut* d_bnms = nullptr; PoseNmsOut* h_bnms = nullptr;
-  int32_t* d_bfirst = nullptr; float* d_bsK = nullptr;  // [cap_bframes + 1], [cap_bframes][9]
-  PoseNmsHead* d_bhead = nullptr; PoseNmsHead* h_bhead = nullptr;
+  // A group of buffers that grows together is freed as a whole, then allocated in order: its last array is empty
+  // unless every one was allocated, so its size stands for the group's.
+  DeviceArray<uint16_t> d_bscene;
+  DeviceArray<lm_match> d_bsurv;
+  DeviceArray<int32_t> d_bframe;  // frame of each survivor
+  DeviceArray<IcpOut> d_bouts; PinnedArray<IcpOut> h_bouts;
+  DeviceArray<uint8_t> d_bposed;
+  DeviceArray<PoseNmsOut> d_bnms; PinnedArray<PoseNmsOut> h_bnms;  // h_bnms last: survivors
+  DeviceArray<int32_t> d_bfirst; DeviceArray<float> d_bsK;  // [frames + 1], [frames][9]
+  DeviceArray<PoseNmsHead> d_bhead; PinnedArray<PoseNmsHead> h_bhead;
   // per chunk (at most one per frame) [0] cloud overflow, shared [1] a peer's poses did not arrive, [2] entries this
   // rank published, [3] the chunk's size (device, pinned copy)
-  int32_t* d_bstat = nullptr; int32_t* h_bstat = nullptr;
+  DeviceArray<int32_t> d_bstat; PinnedArray<int32_t> h_bstat;  // h_bstat last: frames
 };
 
-static void pose_free_frame(lm_pose_stage* s) {
-  cudaFree(s->d_raw); cudaFree(s->d_cpts); cudaFree(s->d_pts); cudaFree(s->d_nrm);
-  cudaFree(s->d_keys[0]); cudaFree(s->d_keys[1]); cudaFree(s->d_vals[0]); cudaFree(s->d_vals[1]);
-  cudaFree(s->d_seg); cudaFree(s->d_jobs); cudaFree(s->d_outs); cudaFree(s->d_sort_tmp); cudaFree(s->d_posed);
-  cudaFreeHost(s->h_outs);
-  s->d_posed = nullptr;
-  s->d_raw = s->d_cpts = s->d_pts = s->d_nrm = nullptr;
-  s->d_keys[0] = s->d_keys[1] = nullptr; s->d_vals[0] = s->d_vals[1] = nullptr;
-  s->d_seg = nullptr; s->d_jobs = nullptr; s->d_outs = nullptr; s->d_sort_tmp = nullptr; s->sort_tmp_bytes = 0;
-  s->h_outs = nullptr;
-  s->cap_bound = 0; s->cap_area = 0;
+// The per-frame buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
+// allocated last, so both are 0 unless every buffer was allocated.
+static int pose_slots(const lm_pose_stage* s) { return s->d_sort_tmp.empty() ? 0 : (int)s->d_jobs.size(); }
+static int64_t pose_area(const lm_pose_stage* s) {
+  return pose_slots(s) ? (int64_t)(s->d_cpts.size() / (3 * s->d_jobs.size())) : 0;
 }
 
 lm_pose_stage* pose_stage_create() { return new lm_pose_stage(); }
 
-void pose_stage_destroy(lm_pose_stage* s) {
-  if (!s) return;
-  pose_free_frame(s);
-  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_err); cudaFree(s->d_rt); cudaFree(s->d_nms);
-  cudaFreeHost(s->h_err); cudaFreeHost(s->h_nms);
-  cudaFree(s->d_bscene); cudaFree(s->d_bsurv); cudaFree(s->d_bframe); cudaFree(s->d_bouts); cudaFree(s->d_bposed); cudaFree(s->d_bnms);
-  cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead); cudaFree(s->d_bstat);
-  cudaFreeHost(s->h_bouts); cudaFreeHost(s->h_bnms); cudaFreeHost(s->h_bhead); cudaFreeHost(s->h_bstat);
-  delete s;
-}
+void pose_stage_destroy(lm_pose_stage* s) { delete s; }
 
 void pose_stage_clear(lm_pose_stage* s) {
   s->tpl.clear();
@@ -1641,53 +1618,48 @@ static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
   for (size_t g = 0; g < s->tpl.size(); ++g)
     if (!s->tpl[g].crop.empty()) memcpy(crops.data() + tp[g].crop, s->tpl[g].crop.data(), s->tpl[g].crop.size() * sizeof(uint16_t));
   CUI(cudaStreamSynchronize(st));  // an earlier frame may still read the old copy
-  cudaFree(s->d_tpl); cudaFree(s->d_crops); cudaFree(s->d_class_begin); cudaFree(s->d_rt);
-  s->d_tpl = nullptr; s->d_crops = nullptr; s->d_class_begin = nullptr; s->d_rt = nullptr;
-  CUI(cudaMalloc(&s->d_tpl, sizeof(PoseTpl) * tp.size()));
-  CUI(cudaMalloc(&s->d_rt, sizeof(PoseRt) * rt.size()));
-  CUI(cudaMemcpy(s->d_rt, rt.data(), sizeof(PoseRt) * rt.size(), cudaMemcpyHostToDevice));
-  CUI(cudaMalloc(&s->d_crops, sizeof(uint16_t) * crops.size()));
-  CUI(cudaMalloc(&s->d_class_begin, sizeof(int32_t) * s->class_begin.size()));
-  CUI(cudaMemcpy(s->d_tpl, tp.data(), sizeof(PoseTpl) * tp.size(), cudaMemcpyHostToDevice));
-  CUI(cudaMemcpy(s->d_crops, crops.data(), sizeof(uint16_t) * crops.size(), cudaMemcpyHostToDevice));
-  CUI(cudaMemcpy(s->d_class_begin, s->class_begin.data(), sizeof(int32_t) * s->class_begin.size(), cudaMemcpyHostToDevice));
+  s->d_tpl.reset(); s->d_crops.reset(); s->d_class_begin.reset(); s->d_rt.reset();
+  CUI(upload(s->d_tpl, tp, st));
+  CUI(upload(s->d_rt, rt, st));
+  CUI(upload(s->d_crops, crops, st));
+  CUI(upload(s->d_class_begin, s->class_begin, st));
+  CUI(cudaStreamSynchronize(st));  // host vectors go out of scope
   s->dirty = false;
   return LM_OK;
 }
 
 static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t area) {
-  if (!s->d_err) {
-    CUI(cudaMalloc(&s->d_err, sizeof(int32_t) * 4));
-    CUI(cudaMallocHost(&s->h_err, sizeof(int32_t) * 4));
-  }
-  if (bound <= s->cap_bound && area <= s->cap_area) return LM_OK;
+  CUI(s->d_err.reserve(4));
+  CUI(s->h_err.reserve(4));
+  if (bound <= pose_slots(s) && area <= pose_area(s)) return LM_OK;
   CUI(cudaStreamSynchronize(st));
-  const int B = std::max(bound, s->cap_bound);
-  const int64_t A = std::max(area, s->cap_area);
+  const int B = std::max(bound, pose_slots(s));
+  const int64_t A = std::max(area, pose_area(s));
   const int64_t slots = 2 * (int64_t)B * A;  // points of every cloud slot
   if (slots > 0x7FFFFFFFll)
     return lm_fail(LM_E_CAPACITY, "pose stage: %d survivors x %lld-pixel crops exceed 2^31 points: lower top_k", B, (long long)A);
-  pose_free_frame(s);
-  CUI(cudaMalloc(&s->d_raw, sizeof(double) * 3 * slots));
-  CUI(cudaMalloc(&s->d_pts, sizeof(double) * 3 * slots));
-  CUI(cudaMalloc(&s->d_nrm, sizeof(double) * 3 * slots));
-  CUI(cudaMalloc(&s->d_cpts, sizeof(double) * 3 * (slots / 2)));
+  s->d_raw.reset(); s->d_cpts.reset(); s->d_pts.reset(); s->d_nrm.reset();
+  for (int k = 0; k < 2; ++k) { s->d_keys[k].reset(); s->d_vals[k].reset(); }
+  s->d_seg.reset(); s->d_jobs.reset(); s->d_outs.reset(); s->d_sort_tmp.reset(); s->d_posed.reset(); s->h_outs.reset();
+  CUI(s->d_raw.assign(3 * slots));
+  CUI(s->d_pts.assign(3 * slots));
+  CUI(s->d_nrm.assign(3 * slots));
+  CUI(s->d_cpts.assign(3 * (slots / 2)));
   for (int k = 0; k < 2; ++k) {
-    CUI(cudaMalloc(&s->d_keys[k], sizeof(unsigned long long) * slots));
-    CUI(cudaMalloc(&s->d_vals[k], sizeof(int32_t) * slots));
+    CUI(s->d_keys[k].assign(slots));
+    CUI(s->d_vals[k].assign(slots));
   }
-  CUI(cudaMalloc(&s->d_seg, sizeof(int32_t) * 4 * B));
-  CUI(cudaMalloc(&s->d_jobs, sizeof(IcpJob) * B));
-  CUI(cudaMalloc(&s->d_outs, sizeof(IcpOut) * B));
-  CUI(cudaMalloc(&s->d_posed, B));
-  CUI(cudaMallocHost(&s->h_outs, sizeof(IcpOut) * B));
-  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
-  cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
-  CUI(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, s->sort_tmp_bytes, dk, dv, (int)slots, 2 * B, s->d_seg, s->d_seg + 2 * B, 0,
+  CUI(s->d_seg.assign(4 * B));
+  CUI(s->d_jobs.assign(B));
+  CUI(s->d_outs.assign(B));
+  CUI(s->d_posed.assign(B));
+  CUI(s->h_outs.assign(B));
+  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0].get(), s->d_keys[1].get());
+  cub::DoubleBuffer<int32_t> dv(s->d_vals[0].get(), s->d_vals[1].get());
+  size_t tmp_bytes = 0;
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tmp_bytes, dk, dv, (int)slots, 2 * B, s->d_seg.get(), s->d_seg.get() + 2 * B, 0,
                                                3 * POSE_KEY_BITS, st));
-  CUI(cudaMalloc(&s->d_sort_tmp, std::max<size_t>(s->sort_tmp_bytes, 16)));
-  s->cap_bound = B;
-  s->cap_area = A;
+  CUI(s->d_sort_tmp.assign(std::max<size_t>(tmp_bytes, 16)));
   return LM_OK;
 }
 
@@ -1730,42 +1702,42 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   const PoseShare* sh = o.share;
   const int world = sh ? sh->world : 1;
   const int n = (c.slots + world - 1) / world;  // a rank without a survivor still publishes
-  const int64_t A = s->cap_area;  // slot stride: the buffers' area, which may exceed the current largest crop
+  const int64_t A = pose_area(s);  // slot stride: the buffers' area, which may exceed the current largest crop
   PoseParams p;
   p.surv = c.surv; p.counts = c.counts;
-  p.class_begin = s->d_class_begin; p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
-  p.tpl = s->d_tpl; p.crops = s->d_crops;
+  p.class_begin = s->d_class_begin.get(); p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
+  p.tpl = s->d_tpl.get(); p.crops = s->d_crops.get();
   p.scene = c.scene; p.srows = o.srows; p.scols = o.scols;
   if (c.sK) memcpy(p.sK, c.sK, sizeof(p.sK));
   else memset(p.sK, 0, sizeof(p.sK));
   p.A = (int32_t)A; p.use_scene = o.use_scene_cloud ? 1 : 0;
-  p.raw = s->d_raw; p.cpts = s->d_cpts; p.keys = s->d_keys[0]; p.vals = s->d_vals[0];
-  p.seg_begin = s->d_seg; p.seg_end = s->d_seg + 2 * n;
-  p.jobs = s->d_jobs; p.err = c.status; p.posed = sh ? s->d_posed : c.posed;
+  p.raw = s->d_raw.get(); p.cpts = s->d_cpts.get(); p.keys = s->d_keys[0].get(); p.vals = s->d_vals[0].get();
+  p.seg_begin = s->d_seg.get(); p.seg_end = s->d_seg.get() + 2 * n;
+  p.jobs = s->d_jobs.get(); p.err = c.status; p.posed = sh ? s->d_posed.get() : c.posed;
   p.frame_of = c.frame_of; p.sKs = c.sKs;
   p.rank = sh ? sh->rank : 0; p.world = world;
   k_pose_cloud<<<n, POSE_THREADS, 0, st>>>(p);
   // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
-  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0], s->d_keys[1]);
-  cub::DoubleBuffer<int32_t> dv(s->d_vals[0], s->d_vals[1]);
-  size_t tmp_bytes = s->sort_tmp_bytes;
-  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp, tmp_bytes, dk, dv, (int)(2 * n * A), 2 * n, p.seg_begin, p.seg_end, 0,
+  cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0].get(), s->d_keys[1].get());
+  cub::DoubleBuffer<int32_t> dv(s->d_vals[0].get(), s->d_vals[1].get());
+  size_t tmp_bytes = s->d_sort_tmp.size();
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp.get(), tmp_bytes, dk, dv, (int)(2 * n * A), 2 * n, p.seg_begin, p.seg_end, 0,
                                                3 * POSE_KEY_BITS, st));
-  k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw, s->d_pts, s->d_jobs,
+  k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw.get(), s->d_pts.get(), s->d_jobs.get(),
                                                p.use_scene);
   // the ICP kernels of lm_icp_process_batch: empty jobs fall through
   const bool normals = o.estimation == LM_ICP_POINT_TO_PLANE;
   if (normals) {
     dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
-    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs, s->d_pts, s->d_nrm, nullptr);
+    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), nullptr);
   }
   if (sh) {
     // the results travel to every rank; the collector gathers the chunk in survivor order
-    const PoseShareDev sd = share_dev(*sh, c.seq, c.counts, s->d_posed, c.status);
-    launch_icp<true>(o.estimation, n, st, s->d_jobs, s->d_pts, s->d_nrm, nullptr, o.max_iterations, nullptr, sd);
+    const PoseShareDev sd = share_dev(*sh, c.seq, c.counts, s->d_posed.get(), c.status);
+    launch_icp<true>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), nullptr, o.max_iterations, nullptr, sd);
     k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, c.outs, c.posed);
   } else {
-    launch_icp<false>(o.estimation, n, st, s->d_jobs, s->d_pts, s->d_nrm, c.outs, o.max_iterations, nullptr, PoseShareDev());
+    launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.outs, o.max_iterations, nullptr, PoseShareDev());
   }
   CUI(cudaGetLastError());
   return (sh ? 6 : 5) - (normals ? 0 : 1);
@@ -1781,17 +1753,17 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches
   int rc = pose_buffers(s, st, e.bound, s->area_max);
   if (rc) return rc;
   const PoseShare* sh = o.share;
-  CUI(cudaMemsetAsync(s->d_err, 0, sizeof(int32_t), st));
+  CUI(cudaMemsetAsync(s->d_err.get(), 0, sizeof(int32_t), st));
   PoseChunk c;
   c.surv = e.d_surv; c.counts = e.d_counts; c.slots = e.bound;
   c.scene = e.d_scene; c.frame_of = nullptr; c.sKs = nullptr; c.sK = e.sK;
-  c.outs = s->d_outs; c.posed = s->d_posed; c.status = s->d_err; c.seq = sh ? sh->seq : 0;
+  c.outs = s->d_outs.get(); c.posed = s->d_posed.get(); c.status = s->d_err.get(); c.seq = sh ? sh->seq : 0;
   const int k = pose_chunk(s, o, c);
   if (k < 0) return k;
   s->last_launches = k;
   *launches += k;
-  CUI(cudaMemcpyAsync(s->h_outs, s->d_outs, sizeof(IcpOut) * std::min(e.bound, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
-  CUI(cudaMemcpyAsync(s->h_err, s->d_err, sizeof(int32_t) * (sh ? 3 : 1), cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_outs.get(), s->d_outs.get(), sizeof(IcpOut) * std::min(e.bound, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_err.get(), s->d_err.get(), sizeof(int32_t) * (sh ? 3 : 1), cudaMemcpyDeviceToHost, st));
   s->bound = e.bound; s->srows = o.srows; s->scols = o.scols;
   s->shared = sh != nullptr;
   s->share_seq = sh ? sh->seq : 0;
@@ -1863,11 +1835,11 @@ int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, i
                       float* residual) {
   if (n > s->bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, s->bound);
   if (n > POSE_FIRST_FETCH) {
-    CUI(cudaMemcpyAsync(s->h_outs + POSE_FIRST_FETCH, s->d_outs + POSE_FIRST_FETCH, sizeof(IcpOut) * (size_t)(n - POSE_FIRST_FETCH),
+    CUI(cudaMemcpyAsync(s->h_outs.get() + POSE_FIRST_FETCH, s->d_outs.get() + POSE_FIRST_FETCH, sizeof(IcpOut) * (size_t)(n - POSE_FIRST_FETCH),
                         cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
   }
-  int rc = pose_status(s->h_err, 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
+  int rc = pose_status(s->h_err.get(), 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
   if (rc) return rc;
   for (int64_t i = 0; i < n; ++i) {
     const TplHost* h = survivor_render(s, surv[i]);
@@ -1888,7 +1860,7 @@ static int pose_nms_launch(const lm_pose_stage* s, int n_frames, const lm_match*
                            int64_t* launches) {
   PoseNmsParams p;
   p.surv = surv; p.counts = counts; p.posed = posed; p.outs = outs;
-  p.rt = s->d_rt; p.class_begin = s->d_class_begin;
+  p.rt = s->d_rt.get(); p.class_begin = s->d_class_begin.get();
   p.thr = thr;
   p.head = head; p.out = out;
   p.frame_first = frame_first;
@@ -1912,33 +1884,31 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32
                            int64_t* launches) {
   if (s->bound > NMS_THREADS) return lm_fail(LM_E_STATE, "pose stage launched for %d survivors, the pose NMS takes %d", s->bound, NMS_THREADS);
   const size_t bytes = sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_THREADS;
-  if (!s->d_nms) {
-    CUI(cudaMalloc(&s->d_nms, bytes));
-    CUI(cudaMallocHost(&s->h_nms, bytes));
-  }
-  int rc = pose_nms_launch(s, 1, d_surv, d_counts, nullptr, s->d_posed, s->d_outs, thr, reinterpret_cast<PoseNmsHead*>(s->d_nms),
-                           nms_entries(s->d_nms), st, launches);
+  CUI(s->d_nms.reserve(bytes));
+  CUI(s->h_nms.reserve(bytes));
+  int rc = pose_nms_launch(s, 1, d_surv, d_counts, nullptr, s->d_posed.get(), s->d_outs.get(), thr, reinterpret_cast<PoseNmsHead*>(s->d_nms.get()),
+                           nms_entries(s->d_nms.get()), st, launches);
   if (rc) return rc;
   // the header and a first window of kept poses; the rest only if there are more
-  CUI(cudaMemcpyAsync(s->h_nms, s->d_nms, sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_FIRST_FETCH, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_nms.get(), s->d_nms.get(), sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_FIRST_FETCH, cudaMemcpyDeviceToHost, st));
   return LM_OK;
 }
 
 int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
                           int64_t* n_out, int64_t* n_survivors, int64_t* n_posed) {
-  int rc = pose_status(s->h_err, 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
+  int rc = pose_status(s->h_err.get(), 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
   if (rc) return rc;
-  const PoseNmsHead h = *reinterpret_cast<const PoseNmsHead*>(s->h_nms);
+  const PoseNmsHead h = *reinterpret_cast<const PoseNmsHead*>(s->h_nms.get());
   *n_out = h.kept;
   if (n_survivors) *n_survivors = h.survivors;
   if (n_posed) *n_posed = h.posed;
   if (h.kept > cap) return lm_fail(LM_E_CAPACITY, "%d poses kept, capacity %lld", h.kept, (long long)cap);
   if (h.kept > NMS_FIRST_FETCH) {
-    CUI(cudaMemcpyAsync(nms_entries(s->h_nms) + NMS_FIRST_FETCH, nms_entries(s->d_nms) + NMS_FIRST_FETCH,
+    CUI(cudaMemcpyAsync(nms_entries(s->h_nms.get()) + NMS_FIRST_FETCH, nms_entries(s->d_nms.get()) + NMS_FIRST_FETCH,
                         sizeof(PoseNmsOut) * (size_t)(h.kept - NMS_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
   }
-  copy_kept(nms_entries(s->h_nms), h.kept, out, R_out, t_out, residual);
+  copy_kept(nms_entries(s->h_nms.get()), h.kept, out, R_out, t_out, residual);
   return LM_OK;
 }
 
@@ -1951,31 +1921,20 @@ static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S);
 
 int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
                        lm_match** d_surv) {
-  const int64_t pix = (int64_t)n_frames * frame_pixels;
-  if (pix > s->cap_bscene || max_surv > s->cap_bsurv || n_frames > s->cap_bframes) {
+  const size_t pix = (size_t)n_frames * frame_pixels;
+  const bool more_frames = (size_t)n_frames * 4 > s->h_bstat.size();
+  if (pix > s->d_bscene.size() || (size_t)max_surv > s->d_bsurv.size() || more_frames) {
     CUI(cudaStreamSynchronize(st));  // an earlier batch may still read them
-    if (pix > s->cap_bscene) {
-      cudaFree(s->d_bscene); s->d_bscene = nullptr; s->cap_bscene = 0;
-      CUI(cudaMalloc(&s->d_bscene, sizeof(uint16_t) * pix));
-      s->cap_bscene = pix;
-    }
-    if (max_surv > s->cap_bsurv) {
-      cudaFree(s->d_bsurv); s->d_bsurv = nullptr; s->cap_bsurv = 0;
-      CUI(cudaMalloc(&s->d_bsurv, sizeof(lm_match) * max_surv));
-      s->cap_bsurv = max_surv;
-    }
-    if (n_frames > s->cap_bframes) {
-      cudaFree(s->d_bfirst); cudaFree(s->d_bsK); cudaFree(s->d_bhead); cudaFreeHost(s->h_bhead);
-      cudaFree(s->d_bstat); cudaFreeHost(s->h_bstat);
-      s->d_bfirst = nullptr; s->d_bsK = nullptr; s->d_bhead = nullptr; s->h_bhead = nullptr; s->cap_bframes = 0;
-      s->d_bstat = nullptr; s->h_bstat = nullptr;
-      CUI(cudaMalloc(&s->d_bfirst, sizeof(int32_t) * (n_frames + 1)));
-      CUI(cudaMalloc(&s->d_bsK, sizeof(float) * 9 * n_frames));
-      CUI(cudaMalloc(&s->d_bhead, sizeof(PoseNmsHead) * n_frames));
-      CUI(cudaMallocHost(&s->h_bhead, sizeof(PoseNmsHead) * n_frames));
-      CUI(cudaMalloc(&s->d_bstat, sizeof(int32_t) * 4 * n_frames));  // chunks <= n_frames: a frame has <= 1024 survivors
-      CUI(cudaMallocHost(&s->h_bstat, sizeof(int32_t) * 4 * n_frames));
-      s->cap_bframes = n_frames;
+    CUI(s->d_bscene.reserve(pix));
+    CUI(s->d_bsurv.reserve((size_t)max_surv));
+    if (more_frames) {
+      s->d_bfirst.reset(); s->d_bsK.reset(); s->d_bhead.reset(); s->h_bhead.reset(); s->d_bstat.reset(); s->h_bstat.reset();
+      CUI(s->d_bfirst.assign(n_frames + 1));
+      CUI(s->d_bsK.assign(9 * (size_t)n_frames));
+      CUI(s->d_bhead.assign(n_frames));
+      CUI(s->h_bhead.assign(n_frames));
+      CUI(s->d_bstat.assign(4 * (size_t)n_frames));  // chunks <= n_frames: a frame has <= 1024 survivors
+      CUI(s->h_bstat.assign(4 * (size_t)n_frames));
     }
   }
   // and everything pose_batch_run may need for max_surv survivors: once frames run, no device memory is freed (a free
@@ -1988,25 +1947,21 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
   if (rc) return rc;
   rc = pose_buffers(s, st, (int)std::min<int64_t>(std::max<int64_t>(max_surv, 1), POSE_BATCH_CHUNK), s->area_max);
   if (rc) return rc;
-  *d_scene = s->d_bscene;
-  *d_surv = s->d_bsurv;
+  *d_scene = s->d_bscene.get();
+  *d_surv = s->d_bsurv.get();
   return LM_OK;
 }
 
 static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S) {
-  if (S <= s->cap_bS) return LM_OK;
+  if ((size_t)S <= s->h_bnms.size()) return LM_OK;
   CUI(cudaStreamSynchronize(st));
-  cudaFree(s->d_bframe); cudaFree(s->d_bouts); cudaFree(s->d_bposed); cudaFree(s->d_bnms);
-  cudaFreeHost(s->h_bouts); cudaFreeHost(s->h_bnms);
-  s->d_bframe = nullptr; s->d_bouts = nullptr; s->d_bposed = nullptr; s->d_bnms = nullptr; s->h_bouts = nullptr; s->h_bnms = nullptr;
-  s->cap_bS = 0;
-  CUI(cudaMalloc(&s->d_bframe, sizeof(int32_t) * S));
-  CUI(cudaMalloc(&s->d_bouts, sizeof(IcpOut) * S));
-  CUI(cudaMalloc(&s->d_bposed, S));
-  CUI(cudaMalloc(&s->d_bnms, sizeof(PoseNmsOut) * S));
-  CUI(cudaMallocHost(&s->h_bouts, sizeof(IcpOut) * S));
-  CUI(cudaMallocHost(&s->h_bnms, sizeof(PoseNmsOut) * S));
-  s->cap_bS = S;
+  s->d_bframe.reset(); s->d_bouts.reset(); s->d_bposed.reset(); s->d_bnms.reset(); s->h_bouts.reset(); s->h_bnms.reset();
+  CUI(s->d_bframe.assign(S));
+  CUI(s->d_bouts.assign(S));
+  CUI(s->d_bposed.assign(S));
+  CUI(s->d_bnms.assign(S));
+  CUI(s->h_bouts.assign(S));
+  CUI(s->h_bnms.assign(S));
   return LM_OK;
 }
 
@@ -2032,34 +1987,34 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
   // per chunk a status block (PoseChunk), [3] the chunk's size
   std::vector<int32_t> stat((size_t)4 * nc, 0);
   for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_BATCH_CHUNK, POSE_BATCH_CHUNK);
-  if (S) CUI(cudaMemcpyAsync(s->d_bframe, frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bfirst, first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bsK, b.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
-  if (nc) CUI(cudaMemcpyAsync(s->d_bstat, stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  if (S) CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemcpyAsync(s->d_bfirst.get(), first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
+  CUI(cudaMemcpyAsync(s->d_bsK.get(), b.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
+  if (nc) CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
   int64_t stage_launches = 0;
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_BATCH_CHUNK;
     PoseChunk k;
-    k.surv = s->d_bsurv + c0; k.counts = s->d_bstat + 4 * c + 3; k.slots = stat[(size_t)4 * c + 3];
-    k.scene = s->d_bscene; k.frame_of = s->d_bframe + c0; k.sKs = s->d_bsK; k.sK = nullptr;
-    k.outs = s->d_bouts + c0; k.posed = s->d_bposed + c0; k.status = s->d_bstat + 4 * c; k.seq = sh ? sh->seq + c : 0;
+    k.surv = s->d_bsurv.get() + c0; k.counts = s->d_bstat.get() + 4 * c + 3; k.slots = stat[(size_t)4 * c + 3];
+    k.scene = s->d_bscene.get(); k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get(); k.sK = nullptr;
+    k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
     const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
     stage_launches += l;
     *launches += l;
   }
   if (b.pose_nms) {
-    rc = pose_nms_launch(s, nf, s->d_bsurv, nullptr, s->d_bfirst, s->d_bposed, s->d_bouts, b.thr, s->d_bhead, s->d_bnms, st, launches);
+    rc = pose_nms_launch(s, nf, s->d_bsurv.get(), nullptr, s->d_bfirst.get(), s->d_bposed.get(), s->d_bouts.get(), b.thr, s->d_bhead.get(), s->d_bnms.get(), st, launches);
     if (rc) return rc;
-    CUI(cudaMemcpyAsync(s->h_bhead, s->d_bhead, sizeof(PoseNmsHead) * nf, cudaMemcpyDeviceToHost, st));
+    CUI(cudaMemcpyAsync(s->h_bhead.get(), s->d_bhead.get(), sizeof(PoseNmsHead) * nf, cudaMemcpyDeviceToHost, st));
   } else if (S) {
-    CUI(cudaMemcpyAsync(s->h_bouts, s->d_bouts, sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
+    CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
   }
-  if (nc) CUI(cudaMemcpyAsync(s->h_bstat, s->d_bstat, sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  if (nc) CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
   int64_t published = 0;
-  rc = pose_status(s->h_bstat, nc, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0, true, &published);
+  rc = pose_status(s->h_bstat.get(), nc, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0, true, &published);
   if (rc) return rc;
   if (stats4) pose_stats(stats4, S, sh != nullptr, published, stage_launches);
   if (b.pose_nms) {
@@ -2069,7 +2024,7 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
       posed[f] = s->h_bhead[f].posed;
       kept[f] = s->h_bhead[f].kept;
       if (kept[f] > 0) {
-        CUI(cudaMemcpyAsync(s->h_bnms + b.first[f], s->d_bnms + b.first[f], sizeof(PoseNmsOut) * kept[f], cudaMemcpyDeviceToHost, st));
+        CUI(cudaMemcpyAsync(s->h_bnms.get() + b.first[f], s->d_bnms.get() + b.first[f], sizeof(PoseNmsOut) * kept[f], cudaMemcpyDeviceToHost, st));
         more = true;
       }
     }
@@ -2091,7 +2046,7 @@ int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int6
 void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual) {
   const int64_t first = b.first[f], n = b.first[f + 1] - first;
   if (b.pose_nms) {
-    copy_kept(s->h_bnms + first, s->h_bhead[f].kept, out, R_out, t_out, residual);
+    copy_kept(s->h_bnms.get() + first, s->h_bhead[f].kept, out, R_out, t_out, residual);
     return;
   }
   for (int64_t i = 0; i < n; ++i) {
@@ -2116,27 +2071,21 @@ extern "C" int lm_nms_translations(int device, int64_t n, const double* t, const
   CUI(cudaSetDevice(device));
   const size_t m = (size_t)std::max<int64_t>(n, 1);
   // one allocation: t [m][3], score [m], keep [m], n_keep
-  const size_t bytes = sizeof(double) * 4 * m + sizeof(int32_t) * (m + 1);
-  uint8_t* buf = nullptr;
-  CUI(cudaMalloc(&buf, bytes));
-  double* d_t = reinterpret_cast<double*>(buf);
+  DeviceArray<uint8_t> buf;
+  CUI(buf.assign(sizeof(double) * 4 * m + sizeof(int32_t) * (m + 1)));
+  double* d_t = reinterpret_cast<double*>(buf.get());
   double* d_s = d_t + 3 * m;
   int32_t* d_keep = reinterpret_cast<int32_t*>(d_s + m);
   int32_t* d_n = d_keep + m;
-  int32_t got = 0;
-  cudaError_t err = cudaSuccess;
   if (n > 0) {
-    err = cudaMemcpy(d_t, t, sizeof(double) * 3 * n, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(d_s, score, sizeof(double) * n, cudaMemcpyHostToDevice);
+    CUI(cudaMemcpy(d_t, t, sizeof(double) * 3 * n, cudaMemcpyHostToDevice));
+    CUI(cudaMemcpy(d_s, score, sizeof(double) * n, cudaMemcpyHostToDevice));
   }
-  if (err == cudaSuccess) {
-    k_nms_translations<<<1, NMS_THREADS>>>((int)n, d_t, d_s, thr, d_keep, d_n);
-    err = cudaGetLastError();
-  }
-  if (err == cudaSuccess) err = cudaMemcpy(&got, d_n, sizeof(int32_t), cudaMemcpyDeviceToHost);
-  if (err == cudaSuccess && got > 0) err = cudaMemcpy(keep, d_keep, sizeof(int32_t) * got, cudaMemcpyDeviceToHost);
-  cudaFree(buf);
-  if (err != cudaSuccess) return lm_fail(LM_E_CUDA, "lm_nms_translations: %s", cudaGetErrorString(err));
+  k_nms_translations<<<1, NMS_THREADS>>>((int)n, d_t, d_s, thr, d_keep, d_n);
+  CUI(cudaGetLastError());
+  int32_t got = 0;
+  CUI(cudaMemcpy(&got, d_n, sizeof(int32_t), cudaMemcpyDeviceToHost));
+  if (got > 0) CUI(cudaMemcpy(keep, d_keep, sizeof(int32_t) * got, cudaMemcpyDeviceToHost));
   *n_keep = got;
   return LM_OK;
 }

@@ -23,11 +23,15 @@ CS=${CS:-compute-sanitizer}
 run() {  # tool case command...
   local tool=$1 name=$2; shift 2
   local log="$OUT/${tool}_${name}.log"
-  timeout 900 $CS --tool "$tool" --error-exitcode 7 --print-limit 20 --log-file "$log" "$@" > "$OUT/${tool}_${name}.out" 2>&1
+  local extra=""
+  [ "${CS_LEAK:-0}" = 1 ] && extra="--leak-check full"
+  timeout 900 $CS --tool "$tool" $extra --error-exitcode 7 --print-limit 20 --log-file "$log" "$@" > "$OUT/${tool}_${name}.out" 2>&1
   local rc=$?
   local errs
   errs=$(grep -E "ERROR SUMMARY|RACECHECK SUMMARY" "$log" | tail -1)
-  echo "$tool $name rc=$rc :: ${errs:-no summary line}" | tee -a "$OUT/summary.txt"
+  local leaks
+  leaks=$(grep -E "LEAK SUMMARY" "$log" | tail -1)
+  echo "$tool $name rc=$rc :: ${errs:-no summary line}${leaks:+ $leaks}" | tee -a "$OUT/summary.txt"
 }
 for tool in memcheck racecheck synccheck; do
   run "$tool" smoke python -c "import __graft_entry__ as g; g.smoke()"
@@ -43,4 +47,7 @@ for tool in memcheck racecheck synccheck; do
 done
 run memcheck peer_batch3 python -m pytest "tests/test_gpu_peer_batch.py::test_two_chunks_few_survivors_and_a_blank_batch" -x -q \
   -p no:cacheprovider
+# (g) leaks: a detector's batch with pose stage, pose NMS and timing, and one ICP call, both handles closed explicitly;
+# the summary must list no leaked allocation (every buffer the handles own is freed with them)
+CS_LEAK=1 run memcheck leaks python tools/leak_probe.py
 echo "done: $(cat "$OUT/summary.txt" | wc -l) runs" | tee -a "$OUT/summary.txt"
