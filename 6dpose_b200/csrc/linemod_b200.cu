@@ -102,6 +102,18 @@ static size_t bp_label_words(int T, int plane) {
   return (((size_t)T * T * plane + 31) / 32 + 32 * rounds + 4 + 3) & ~(size_t)3;
 }
 
+// The stages enqueued for the handle's frame, each with the arguments a replay needs (complete_frame).  lm_enqueue sets
+// the match's; every later lm_enqueue_* raises its stage's flag, and the completion that waits for a stage lowers it.
+struct FrameChain {
+  float threshold = 0.f; bool gated = false;                // lm_enqueue
+  bool completed = false;  // lm_complete returned: the header, first records and counters are on the host (until a new
+                           // frame, bank, selection, result block or exchange)
+  bool post = false; double iou = 0.5; int top_k = 0;      // lm_enqueue_post
+  bool pose = false; float sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  int max_iter = 30, use_scene = 0, estimation = LM_ICP_POINT_TO_PLANE;  // lm_enqueue_pose
+  bool pose_nms = false; double nms_thr = 40.0;             // lm_enqueue_pose_nms
+};
+
 struct lm_detector {
   int device = 0;
   // streams and events first: they outlive the buffers, which are freed in reverse order of declaration
@@ -117,7 +129,8 @@ struct lm_detector {
   int L = 0, M = LM_MAX_MODALITIES;
   int T[LM_MAX_LEVELS] = {0};
   LevelHost lv[LM_MAX_LEVELS];
-  bool have_frame = false, have_run = false;
+  bool have_frame = false;
+  FrameChain chain;
 
   // bank (host)
   int n_classes = 0, S = 0, G = 0;
@@ -182,7 +195,6 @@ struct lm_detector {
   PinnedArray<unsigned long long> h_counters;
   PinnedArray<uint8_t> h_res;        // staging: header + records
   int64_t h_valid = 0;               // records already copied to h_res
-  float last_threshold = 0.f;
 
   std::vector<int> class_of;            // template -> class (lm_finish), rebuilt when the bank changes
   std::vector<int32_t> order_cnt;       // order_records scratch
@@ -195,18 +207,11 @@ struct lm_detector {
   DeviceArray<lm_match> d_post_out; PinnedArray<lm_match> h_post_out;  // LM_POST_MAX survivors
   DeviceArray<int32_t> d_post_counts; PinnedArray<int32_t> h_post_counts;
   DeviceArray<uint8_t> d_post_live;
-  bool post_pending = false, post_retry = false;
-  double post_iou = 0.5; int post_top_k = 0;
 
   // pose stage behind the NMS (lm_pose.h): per-template render crops, refinement of the survivors on the device
   lm_pose_stage* pose = nullptr;
   bool frame_depth = false;             // the frame came from lm_upload_images: fe_depth holds its depth
-  bool pose_pending = false;
-  bool pose_nms_pending = false;        // lm_enqueue_pose_nms: the frame completes through lm_complete_detect
-  double pose_nms_thr = 40.0;
-  float pose_sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; int pose_max_iter = 30, pose_use_scene = 0;
-  int pose_estimation = LM_ICP_POINT_TO_PLANE;       // lm_set_pose_estimation: for the next pose stage
-  int pose_frame_estimation = LM_ICP_POINT_TO_PLANE; // the enqueued frame's (its rerun after a retry keeps it)
+  int pose_estimation = LM_ICP_POINT_TO_PLANE;  // lm_set_pose_estimation: for the next pose stage
   int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
@@ -234,7 +239,6 @@ struct lm_detector {
   // depth gate of the coarse scan (lm_set_depth_gate)
   std::vector<float> tdepth;            // training distance per template of the bank (mm; NaN / <= 0: never gated)
   bool gate_on = false; double gate_tau = 0.0;
-  bool gate_frame = false;              // the last enqueued frame ran gated
   bool gate_dirty = true;               // h_gate_item no longer fits the shard / distances / tolerance
   std::vector<uint2> h_gate_item;       // per work item of the shard: band and sample-cell offset (DepthGate::item)
   int64_t gate_with_z = 0;              // work items of the shard with a distance
@@ -385,7 +389,7 @@ extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_
     CU(d->d_fxy.assign((size_t)n_feats));
   }
   d->prepared = false;
-  d->have_run = false;
+  d->chain.completed = false;
   // default selection: everything, one shard
   return lm_select(d, nullptr, -1, 0, 1);
 }
@@ -465,7 +469,7 @@ extern "C" int lm_select_layout(lm_detector* d, const int32_t* class_sel, int n_
   d->work_dirty = true;
   d->post_dirty = true;
   d->gate_dirty = true;
-  d->have_run = false;
+  d->chain.completed = false;
   return LM_OK;
 }
 
@@ -1055,7 +1059,7 @@ static int upload_quantized(lm_detector* d, const uint8_t* const* quantized, con
   }
   d->have_frame = true;
   d->frame_depth = false;
-  d->have_run = false;
+  d->chain.completed = false;
   return LM_OK;
 }
 
@@ -1076,7 +1080,7 @@ extern "C" int lm_bind_quantized_device(lm_detector* d, const uint8_t* const* d_
   d->upper_pending = false;
   d->have_frame = true;
   d->frame_depth = false;
-  d->have_run = false;
+  d->chain.completed = false;
   return LM_OK;
 }
 
@@ -1174,7 +1178,7 @@ static void fe_bound(lm_detector* d) {
   d->upper_pending = false;
   d->have_frame = true;
   d->frame_depth = true;
-  d->have_run = false;
+  d->chain.completed = false;
 }
 
 extern "C" int lm_upload_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,
@@ -1424,7 +1428,7 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     if (rc1) return rc1;
     if (d->timing) CU(cudaEventRecord(d->ev[1].get(), st));
     // depth gate: the frame's cell summary, ahead of K2
-    const bool gated = d->gate_frame;
+    const bool gated = d->chain.gated;
     DepthGate gate;  // read by the gated launches only
     if (gated) {
       gate.cells = d->d_cells.get(); gate.item = d->d_gate_item.get(); gate.before = d->d_gate_before.get();
@@ -1643,36 +1647,75 @@ static int ensure_run_buffers(lm_detector* d) {
   return LM_OK;
 }
 
-// More kept records than slots in the internal result block: grow it and redo the refinement stage only (the coarse
-// outputs of the frame are still in place).  The header travels through a stack copy (the pinned staging block is
-// reallocated by ensure_run_buffers) with the new capacity patched in.
-static int grow_and_rerun(lm_detector* d) {
-  lm_result_header hdr = *hres(d);
-  const bool more_records = (int64_t)hdr.count > d->res_cap;
-  const bool more_cands = (int64_t)hdr.coarse_candidates > cand_cap(d);
+static int enqueue_post(lm_detector* d, double iou_threshold, int top_k);
+static int enqueue_pose(lm_detector* d);
+static int enqueue_pose_nms(lm_detector* d);
+
+// A frame kept more records than the result block holds, or passed more coarse candidates than the candidate list
+// holds: grow what it outgrew and replay its chain from the refinement on (the coarse outputs are still in place), then
+// every later stage the chain record holds.  A truncated candidate list makes the kept count a lower bound, so the
+// block gets room for twice as many; if that is still too few, the next pass of complete_frame grows it again.
+static int grow_and_replay(lm_detector* d, int64_t kept, int64_t cands) {
+  const bool more_records = kept > d->res_cap;
+  const bool more_cands = cands > cand_cap(d);
   if (more_records && d->res_external)
-    return fail(LM_E_CAPACITY, "%d records kept, caller's result buffer holds %lld", hdr.count, (long long)d->res_cap);
+    return fail(LM_E_CAPACITY, "%lld records kept, caller's result buffer holds %lld", (long long)kept, (long long)d->res_cap);
   if (d->px_rank >= 0)
-    return fail(LM_E_CAPACITY, "%d records kept of %d candidates: beyond the result block (%lld) or the candidate list (%lld) of a "
-                "connected peer exchange", hdr.count, hdr.coarse_candidates, (long long)d->res_cap, (long long)cand_cap(d));
-  CU(cudaStreamSynchronize(d->stream.get()));
-  if (more_cands) d->cand_need = (int64_t)hdr.coarse_candidates;  // ensure_run_buffers reallocates the lists
-  if (more_records || (more_cands && !d->res_external)) {
-    // with a truncated candidate list the kept count is a lower bound: leave room, a second pass grows again if needed
-    CU(d->d_res_own.reserve(res_bytes((int64_t)hdr.count * 2)));
-  }
+    return fail(LM_E_CAPACITY, "%lld records kept of %lld candidates: beyond the result block (%lld) or the candidate list (%lld) of a "
+                "connected peer exchange", (long long)kept, (long long)cands, (long long)d->res_cap, (long long)cand_cap(d));
+  if (more_cands) d->cand_need = cands;  // ensure_run_buffers reallocates the lists
+  if (more_records || (more_cands && !d->res_external)) CU(d->d_res_own.reserve(res_bytes(kept * 2)));
   int rc = ensure_run_buffers(d);
   if (rc) return rc;
-  hdr.capacity = (int32_t)d->res_cap;
-  hdr.count = 0;
+  // the header the coarse scan wrote, with the new capacity
+  const lm_result_header hdr = {0, (int32_t)cands, (int32_t)d->res_cap, d->shard_index};
   CU(cudaMemcpy(d->d_res, &hdr, sizeof(hdr), cudaMemcpyHostToDevice));
-  rc = enqueue_stages(d, d->last_threshold, true);
-  if (rc) return rc;
-  rc = enqueue_readback(d);
-  if (rc) return rc;
-  CU(cudaStreamSynchronize(d->stream.get()));
-  CU(cudaGetLastError());
-  return LM_OK;
+  const FrameChain& c = d->chain;
+  rc = enqueue_stages(d, c.threshold, true);
+  if (!rc && c.post) rc = enqueue_post(d, c.iou, c.top_k);
+  if (!rc && c.pose) rc = enqueue_pose(d);
+  if (!rc && c.pose_nms) rc = enqueue_pose_nms(d);
+  return rc;
+}
+
+#define LM_POST_FIRST 16      // survivors fetched with the box NMS's counts; the common top-k needs no second copy
+#define LM_COMPLETE_PASSES 3  // grow-and-replay passes of one completion: two always suffice, the first may undercount
+
+// Every completion ends here (lm_complete; with `post`, lm_complete_post / _pose / _detect and each batch frame): the
+// readbacks of the awaited stage (the header, first records and counters; or the box NMS's counts, with `survivors` its
+// first survivors, and the counters), one synchronise, the exchange's status, then the overflow test and at most
+// LM_COMPLETE_PASSES grow-and-replay passes.  A replay also brings the grown frame's header back.
+static int complete_frame(lm_detector* d, bool post, bool survivors) {
+  cudaStream_t st = d->stream.get();
+  for (int pass = 0;; ++pass) {
+    if (!post || pass > 0) {
+      int rc = enqueue_readback(d);
+      if (rc) return rc;
+    }
+    if (post) {
+      CU(cudaMemcpyAsync(d->h_post_counts.get(), d->d_post_counts.get(), sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+      if (survivors) CU(cudaMemcpyAsync(d->h_post_out.get(), d->d_post_out.get(), sizeof(lm_match) * LM_POST_FIRST, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(d->h_counters.get(), d->d_counters.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    if (pass == 0 && d->px_rank >= 0) {
+      if (d->h_counters[2] == 1)
+        return fail(LM_E_STATE, "peer exchange: a rank did not publish frame %d within %llu ms (or an earlier frame already timed out "
+                    "on this device); disconnect and reconnect the exchange", d->px_seq, d->px_timeout_ns / 1000000ull);
+      if (d->h_counters[2] == 2)
+        return fail(LM_E_CAPACITY, "peer exchange: a shard kept more than %lld records (capacity given to lm_peer_export)",
+                    (long long)d->px_cap);
+    }
+    const int64_t kept = post ? d->h_post_counts[1] : hres(d)->count;
+    const int64_t cands = post ? d->h_post_counts[3] : hres(d)->coarse_candidates;
+    if (kept <= d->res_cap && cands <= cand_cap(d)) return LM_OK;
+    if (pass == LM_COMPLETE_PASSES)
+      return fail(LM_E_CAPACITY, "%lld records kept of %lld candidates after %d passes: the result block holds %lld, the candidate "
+                  "list %lld", (long long)kept, (long long)cands, pass, (long long)d->res_cap, (long long)cand_cap(d));
+    int rc = grow_and_replay(d, kept, cands);
+    if (rc) return rc;
+  }
 }
 
 extern "C" int lm_enqueue(lm_detector* d, float threshold) {
@@ -1696,8 +1739,8 @@ extern "C" int lm_enqueue(lm_detector* d, float threshold) {
     rc = prepare_gate(d);
     if (rc) return rc;
   }
-  d->gate_frame = d->gate_on;
-  d->last_threshold = threshold;
+  d->chain.gated = d->gate_on;
+  d->chain.threshold = threshold;
   rc = filter_thresholds(d, threshold);
   if (rc) return rc;
   return enqueue_stages(d, threshold, false);
@@ -1724,23 +1767,9 @@ extern "C" int lm_complete(lm_detector* d) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d) return fail(LM_E_INVALID, "null detector");
   CU(cudaSetDevice(d->device));
-  int rc = enqueue_readback(d);
+  int rc = complete_frame(d, false, false);
   if (rc) return rc;
-  CU(cudaStreamSynchronize(d->stream.get()));
-  CU(cudaGetLastError());
-  if (d->px_rank >= 0) {
-    if (d->h_counters[2] == 1)
-      return fail(LM_E_STATE, "peer exchange: a rank did not publish frame %d within %llu ms (or an earlier frame already timed out "
-                  "on this device); disconnect and reconnect the exchange", d->px_seq, d->px_timeout_ns / 1000000ull);
-    if (d->h_counters[2] == 2)
-      return fail(LM_E_CAPACITY, "peer exchange: a shard kept more than %lld records (capacity given to lm_peer_export)",
-                  (long long)d->px_cap);
-  }
-  for (int pass = 0; pass < 3 && ((int64_t)hres(d)->count > d->res_cap || (int64_t)hres(d)->coarse_candidates > cand_cap(d)); ++pass) {
-    rc = grow_and_rerun(d);
-    if (rc) return rc;
-  }
-  d->have_run = true;
+  d->chain.completed = true;
   return LM_OK;
 }
 
@@ -1763,7 +1792,7 @@ extern "C" int lm_set_result_buffer(lm_detector* d, void* d_block, int64_t capac
     d->d_res = (lm_result_header*)d_block;
     d->res_cap = capacity_records;
   }
-  d->have_run = false;
+  d->chain.completed = false;
   return LM_OK;
 }
 
@@ -1864,7 +1893,7 @@ extern "C" int lm_peer_connect(lm_detector* d, int rank, int world, const uint8_
   }
   d->px_ipc = true;
   d->px_rank = rank;
-  d->have_run = false;
+  d->chain.completed = false;
   return peer_upload_descriptor(d);
 }
 
@@ -1891,7 +1920,7 @@ extern "C" int lm_peer_connect_local(lm_detector* d, int rank, int world, void* 
   d->px_base[rank] = d->px_buf.get();
   d->px_ipc = false;
   d->px_rank = rank;
-  d->have_run = false;
+  d->chain.completed = false;
   return peer_upload_descriptor(d);
 }
 
@@ -1908,7 +1937,7 @@ extern "C" int lm_peer_disconnect(lm_detector* d) {
   CU(cudaSetDevice(d->device));
   CU(cudaStreamSynchronize(d->stream.get()));
   peer_release(d);
-  d->have_run = false;
+  d->chain.completed = false;
   return LM_OK;
 }
 
@@ -1965,7 +1994,7 @@ static void order_records(lm_detector* d, lm_record* r, int64_t n) {
 
 extern "C" int lm_fetch_records(lm_detector* d, lm_record* out, int64_t cap, int64_t* n_out) {
   if (!d || !n_out) return fail(LM_E_INVALID, "null argument");
-  if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
   CU(cudaSetDevice(d->device));
   const int64_t n = hres(d)->count;
   *n_out = n;
@@ -2115,13 +2144,7 @@ static int prepare_post(lm_detector* d) {
   return LM_OK;
 }
 
-extern "C" int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k) {
-  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
-  if (!d) return fail(LM_E_INVALID, "null detector");
-  if (!d->d_res) return fail(LM_E_STATE, "no stages enqueued (call lm_enqueue first)");
-  if (top_k > LM_POST_MAX) return fail(LM_E_INVALID, "top_k %d > %d", top_k, LM_POST_MAX);
-  if (!(iou_threshold >= 0.0)) return fail(LM_E_INVALID, "IoU threshold must be >= 0");
-  CU(cudaSetDevice(d->device));
+static int enqueue_post(lm_detector* d, double iou_threshold, int top_k) {
   int rc = prepare_post(d);
   if (rc) return rc;
   PostParams p;
@@ -2132,64 +2155,43 @@ extern "C" int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k) 
   p.out_counts = d->d_post_counts.get(); p.live = d->d_post_live.get();
   CU(launch_pdl(k_post_nms, dim3(1), dim3(1024), 0, d->stream.get(), p));
   ++d->launches;
-  d->post_iou = iou_threshold;
-  d->post_top_k = top_k;
-  d->post_pending = true;
   return LM_OK;
 }
 
-static int enqueue_pose(lm_detector* d);
-static int enqueue_pose_nms(lm_detector* d);
+extern "C" int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k) {
+  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (!d->d_res) return fail(LM_E_STATE, "no stages enqueued (call lm_enqueue first)");
+  if (top_k > LM_POST_MAX) return fail(LM_E_INVALID, "top_k %d > %d", top_k, LM_POST_MAX);
+  if (!(iou_threshold >= 0.0)) return fail(LM_E_INVALID, "IoU threshold must be >= 0");
+  CU(cudaSetDevice(d->device));
+  int rc = enqueue_post(d, iou_threshold, top_k);
+  if (rc) return rc;
+  d->chain.iou = iou_threshold;
+  d->chain.top_k = top_k;
+  d->chain.post = true;
+  return LM_OK;
+}
 
-// fetch = false (lm_complete_detect): wait and retry as usual, but copy no survivor back
+// The frame completed through its box NMS: n_out survivors (copied to out unless fetch is false, as for
+// lm_complete_detect), n_records the kept records the NMS saw.
 static int complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records, bool fetch) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !n_out) return fail(LM_E_INVALID, "null argument");
-  if (!d->post_pending) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
+  if (!d->chain.post) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
   CU(cudaSetDevice(d->device));
-  cudaStream_t st = d->stream.get();
-  CU(cudaMemcpyAsync(d->h_post_counts.get(), d->d_post_counts.get(), sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
-  // the common top-k is small: fetch a first window with the counts, the rest only if there is more
-  const int first = 16;
-  if (fetch) CU(cudaMemcpyAsync(d->h_post_out.get(), d->d_post_out.get(), sizeof(lm_match) * first, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(d->h_counters.get(), d->d_counters.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  CU(cudaGetLastError());
-  d->post_pending = false;
-  if (d->px_rank >= 0 && d->h_counters[2] == 1)
-    return fail(LM_E_STATE, "peer exchange: a rank did not publish frame %d within %llu ms", d->px_seq, d->px_timeout_ns / 1000000ull);
-  if (d->px_rank >= 0 && d->h_counters[2] == 2) return fail(LM_E_CAPACITY, "peer exchange: a shard kept more than %lld records", (long long)d->px_cap);
+  int rc = complete_frame(d, true, fetch);
+  d->chain.post = false;
+  if (rc) return rc;
   const int64_t n = d->h_post_counts[0];
   if (n_records) *n_records = d->h_post_counts[1];
-  if ((int64_t)d->h_post_counts[1] > d->res_cap || (int64_t)d->h_post_counts[3] > cand_cap(d)) {
-    // the NMS did not see every record: grow the block like lm_complete does, redo the refinement, run the NMS again
-    if (d->post_retry || d->res_external || d->px_rank >= 0)
-      return fail(LM_E_CAPACITY, "%d records kept, the result block holds %lld: the NMS did not see all of them", d->h_post_counts[1],
-                  (long long)d->res_cap);
-    CU(cudaMemcpyAsync(d->h_res.get(), d->d_res, sizeof(lm_result_header), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    int rc = grow_and_rerun(d);
-    if (rc) return rc;
-    rc = lm_enqueue_post(d, d->post_iou, d->post_top_k);
-    if (rc) return rc;
-    if (d->pose_pending) {  // the pose stage ran on the truncated survivor list: run it again behind the new NMS
-      rc = enqueue_pose(d);
-      if (rc) return rc;
-    }
-    if (d->pose_nms_pending) {  // and so did the pose NMS
-      rc = enqueue_pose_nms(d);
-      if (rc) return rc;
-    }
-    d->post_retry = true;
-    rc = complete_post(d, out, cap, n_out, n_records, fetch);
-    d->post_retry = false;
-    return rc;
-  }
   *n_out = n;
   if (!fetch) return LM_OK;
   if (n > cap) return fail(LM_E_CAPACITY, "%lld survivors, capacity %lld", (long long)n, (long long)cap);
-  if (n > first) {
-    CU(cudaMemcpyAsync(d->h_post_out.get() + first, d->d_post_out.get() + first, sizeof(lm_match) * (size_t)(n - first), cudaMemcpyDeviceToHost, st));
+  if (n > LM_POST_FIRST) {
+    cudaStream_t st = d->stream.get();
+    CU(cudaMemcpyAsync(d->h_post_out.get() + LM_POST_FIRST, d->d_post_out.get() + LM_POST_FIRST, sizeof(lm_match) * (size_t)(n - LM_POST_FIRST),
+                       cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
   }
   if (n > 0 && out) memcpy(out, d->h_post_out.get(), sizeof(lm_match) * (size_t)n);
@@ -2241,12 +2243,13 @@ static int enqueue_pose(lm_detector* d) {
     int rc = pose_share_of(d, ++d->px_pose_seq, &sh);
     if (rc) return rc;
   }
+  const FrameChain& c = d->chain;
   PoseEnqueue e;
-  e.o = {d->fe[0].rows, d->fe[0].cols, d->pose_use_scene, d->pose_max_iter, d->pose_frame_estimation, d->stream.get(), share ? &sh : nullptr};
+  e.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr};
   e.d_surv = d->d_post_out.get(); e.d_counts = d->d_post_counts.get();
   e.d_scene = d->fe_depth.get();
-  memcpy(e.sK, d->pose_sK, sizeof(e.sK));
-  e.bound = d->post_top_k > 0 ? std::min(d->post_top_k, LM_POST_MAX) : LM_POST_MAX;
+  memcpy(e.sK, c.sK, sizeof(e.sK));
+  e.bound = c.top_k > 0 ? std::min(c.top_k, LM_POST_MAX) : LM_POST_MAX;
   return pose_stage_enqueue(d->pose, e, &d->launches);
 }
 
@@ -2254,19 +2257,20 @@ extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iter
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !sceneK) return fail(LM_E_INVALID, "null argument");
   if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
-  if (!d->post_pending) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
+  FrameChain& c = d->chain;
+  if (!c.post) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
   if (!d->frame_depth) return fail(LM_E_STATE, "the frame has no depth image: upload it with lm_upload_images");
   if (!d->pose || !pose_stage_covers(d->pose, d->sel.data(), (int64_t)d->sel.size()))
     return fail(LM_E_STATE, "no template renders registered for every selected template of this bank (lm_set_template_renders)");
   CU(cudaSetDevice(d->device));
-  memcpy(d->pose_sK, sceneK, sizeof(d->pose_sK));
-  d->pose_max_iter = max_iterations;
-  d->pose_use_scene = use_scene_cloud ? 1 : 0;
-  d->pose_frame_estimation = d->pose_estimation;
-  d->pose_nms_pending = false;  // a new pose stage: any pose NMS enqueued before belongs to an abandoned frame
+  memcpy(c.sK, sceneK, sizeof(c.sK));
+  c.max_iter = max_iterations;
+  c.use_scene = use_scene_cloud ? 1 : 0;
+  c.estimation = d->pose_estimation;
+  c.pose_nms = false;  // a new pose stage: any pose NMS enqueued before belongs to an abandoned frame
   int rc = enqueue_pose(d);
   if (rc) return rc;
-  d->pose_pending = true;
+  c.pose = true;
   return LM_OK;
 }
 
@@ -2274,10 +2278,10 @@ extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, do
                                 int64_t* n_out, int64_t* n_records) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !n_out || (cap > 0 && (!R_out || !t_out || !residual))) return fail(LM_E_INVALID, "null argument");
-  if (!d->pose_pending) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
-  if (d->pose_nms_pending) return fail(LM_E_STATE, "lm_enqueue_pose_nms is pending: complete the frame with lm_complete_detect");
-  int rc = lm_complete_post(d, out, cap, n_out, n_records);  // waits; on the capacity retry it runs the pose stage again
-  d->pose_pending = false;
+  if (!d->chain.pose) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
+  if (d->chain.pose_nms) return fail(LM_E_STATE, "lm_enqueue_pose_nms is pending: complete the frame with lm_complete_detect");
+  int rc = complete_post(d, out, cap, n_out, n_records, true);
+  d->chain.pose = false;
   if (rc) return rc;
   rc = pose_stage_finish(d->pose, d->stream.get(), d->h_post_out.get(), *n_out, R_out, t_out, residual);
   if (rc) return rc;
@@ -2286,20 +2290,20 @@ extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, do
 }
 
 static int enqueue_pose_nms(lm_detector* d) {
-  return pose_stage_enqueue_nms(d->pose, d->d_post_out.get(), d->d_post_counts.get(), d->pose_nms_thr, d->stream.get(), &d->launches);
+  return pose_stage_enqueue_nms(d->pose, d->d_post_out.get(), d->d_post_counts.get(), d->chain.nms_thr, d->stream.get(), &d->launches);
 }
 
 extern "C" int lm_enqueue_pose_nms(lm_detector* d, double translation_threshold_mm) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d) return fail(LM_E_INVALID, "null detector");
   if (!(translation_threshold_mm >= 0.0)) return fail(LM_E_INVALID, "translation threshold must be >= 0 (NaN given or negative)");
-  if (!d->pose_pending) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
-  if (d->pose_nms_pending) return fail(LM_E_STATE, "lm_enqueue_pose_nms was already called for this frame");
+  if (!d->chain.pose) return fail(LM_E_STATE, "lm_enqueue_pose has not been called");
+  if (d->chain.pose_nms) return fail(LM_E_STATE, "lm_enqueue_pose_nms was already called for this frame");
   CU(cudaSetDevice(d->device));
-  d->pose_nms_thr = translation_threshold_mm;
+  d->chain.nms_thr = translation_threshold_mm;
   int rc = enqueue_pose_nms(d);
   if (rc) return rc;
-  d->pose_nms_pending = true;
+  d->chain.pose_nms = true;
   return LM_OK;
 }
 
@@ -2307,12 +2311,10 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
                                   int64_t* n_out, int64_t* n_survivors, int64_t* n_posed, int64_t* n_records) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !n_out || (cap > 0 && (!out || !R_out || !t_out || !residual))) return fail(LM_E_INVALID, "null argument");
-  if (!d->pose_nms_pending) return fail(LM_E_STATE, "lm_enqueue_pose_nms has not been called");
+  if (!d->chain.pose_nms) return fail(LM_E_STATE, "lm_enqueue_pose_nms has not been called");
   int64_t n_surv = 0;
-  // waits; on the capacity retry it runs the NMS, the pose stage and the pose NMS again
   int rc = complete_post(d, nullptr, 0, &n_surv, n_records, false);
-  d->pose_pending = false;
-  d->pose_nms_pending = false;
+  d->chain.pose = d->chain.pose_nms = false;
   if (rc) return rc;
   rc = pose_stage_finish_nms(d->pose, d->stream.get(), out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
   if (rc) return rc;
@@ -2360,7 +2362,7 @@ static const lm_result_header* scan_header(const lm_detector* d) {
 extern "C" int lm_depth_gate_stats(lm_detector* d, int64_t* out4) {
   if (!d || !out4) return fail(LM_E_INVALID, "null argument");
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
-  if (!d->gate_frame || !d->d_res) return fail(LM_E_STATE, "the last frame did not run with the depth gate");
+  if (!d->chain.gated || !d->d_res) return fail(LM_E_STATE, "the last frame did not run with the depth gate");
   CU(cudaSetDevice(d->device));
   const LevelHost& low = d->lv[d->L - 1];
   std::vector<uint32_t> cells((size_t)low.plane);
@@ -2427,8 +2429,7 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     if (rc) return fail(rc, "frame %d: %s", f, std::string(g_err).c_str());
   }
   cudaStream_t st = d->stream.get();
-  d->pose_pending = false;  // a batch starts new frames: a pending single-frame pose stage is abandoned
-  d->pose_nms_pending = false;
+  d->chain.pose = d->chain.pose_nms = false;  // a batch starts new frames: a pending single-frame pose stage is abandoned
   const int bound = top_k > 0 ? top_k : LM_POST_MAX;  // most survivors k_post_nms writes per frame
   const size_t n0 = (size_t)rows * cols;
   uint16_t* d_scene = nullptr;
@@ -2438,7 +2439,7 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
   std::vector<int64_t> first((size_t)n_frames + 1, 0);
   std::vector<lm_match> surv(pose_nms ? 0 : (size_t)n_frames * bound);
   for (int f = 0; f < n_frames; ++f) {
-    // the single-frame chain up to the box NMS, its capacity retry included
+    // the single-frame chain up to the box NMS, completed as a single frame is (complete_frame)
     rc = dev ? bind_images_device(d, dev->frame(f), rows, cols, lrows, lcols, dev->stream)
              : lm_upload_images(d, rgb + f * n0 * 3, depth + f * n0, rows, cols, masks ? masks[2 * f] : nullptr, masks ? masks[2 * f + 1] : nullptr);
     if (rc) return rc;
@@ -2518,11 +2519,9 @@ extern "C" int lm_detect_batch_device(lm_detector* d, int n_frames, const uint8_
                       frame_counts);
 }
 
-extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,
-                                  float threshold, lm_match* out, int64_t cap, int64_t* n_out) {
-  int rc = upload_quantized(d, quantized, rows, cols, false);  // lm_run synchronises before this call returns
-  if (rc) return rc;
-  rc = lm_run(d, threshold);
+// lm_run + lm_fetch_records + lm_finish of the frame just uploaded: the match list of lm_match_quantized / lm_match_images.
+static int match_frame(lm_detector* d, float threshold, lm_match* out, int64_t cap, int64_t* n_out) {
+  int rc = lm_run(d, threshold);
   if (rc) return rc;
   const int64_t n = hres(d)->count;
   std::vector<lm_record> rec((size_t)n);
@@ -2532,18 +2531,16 @@ extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantize
   return lm_finish(d, rec.data(), got, out, cap, n_out);
 }
 
+extern "C" int lm_match_quantized(lm_detector* d, const uint8_t* const* quantized, const int* rows, const int* cols,
+                                  float threshold, lm_match* out, int64_t cap, int64_t* n_out) {
+  int rc = upload_quantized(d, quantized, rows, cols, false);  // lm_run synchronises before this call returns
+  return rc ? rc : match_frame(d, threshold, out, cap, n_out);
+}
+
 extern "C" int lm_match_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, int rows, int cols, const uint8_t* mask_color,
                                const uint8_t* mask_depth, float threshold, lm_match* out, int64_t cap, int64_t* n_out) {
   int rc = lm_upload_images(d, rgb, depth, rows, cols, mask_color, mask_depth);
-  if (rc) return rc;
-  rc = lm_run(d, threshold);
-  if (rc) return rc;
-  const int64_t n = hres(d)->count;
-  std::vector<lm_record> rec((size_t)n);
-  int64_t got = 0;
-  rc = lm_fetch_records(d, rec.data(), n, &got);
-  if (rc) return rc;
-  return lm_finish(d, rec.data(), got, out, cap, n_out);
+  return rc ? rc : match_frame(d, threshold, out, cap, n_out);
 }
 
 extern "C" int lm_debug_quantized(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap) {
@@ -2562,7 +2559,7 @@ extern "C" int lm_debug_quantized(lm_detector* d, int level, int modality, uint8
 
 extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap) {
   if (!d || !out) return fail(LM_E_INVALID, "null argument");
-  if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
   if (level < 0 || level >= d->L || modality < 0 || modality >= d->M) return fail(LM_E_INVALID, "bad level/modality");
   const LevelHost& lv = d->lv[level];
   if ((int64_t)lv.mod_stride > cap) return fail(LM_E_CAPACITY, "need %u bytes", lv.mod_stride);
@@ -2588,7 +2585,7 @@ extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality,
 extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   if (!d || !out) return fail(LM_E_INVALID, "null argument");
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
-  if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
   if (cap < LM_PLAN_ENTRIES) return fail(LM_E_CAPACITY, "need %d entries", LM_PLAN_ENTRIES);
   CU(cudaSetDevice(d->device));
   int queue[4];
@@ -2620,7 +2617,7 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   int eligible = 0;
   for (const int4& f : d->h_finfo) eligible += (f.w & 2) ? 1 : 0;
   out[14] = eligible;
-  out[15] = d->gate_frame ? 1 : 0;
+  out[15] = d->chain.gated ? 1 : 0;
   // work items of the refinement kernels that ran (-1: it did not run); see enqueue_stages
   const int total = (int)std::min<int64_t>(hres(d)->coarse_candidates, cand_cap(d));
   const bool filter = use_filter(d), bits_mode = use_bits(d);
@@ -2635,7 +2632,7 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
 
 extern "C" int lm_counters(lm_detector* d, int64_t* out8) {
   if (!d || !out8) return fail(LM_E_INVALID, "null argument");
-  if (!d->have_run) return fail(LM_E_STATE, "lm_run has not been called");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
   out8[0] = d->shard_count;
   out8[1] = hres(d)->coarse_candidates;
   out8[2] = d->alg_scan_bytes;

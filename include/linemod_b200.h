@@ -144,8 +144,13 @@ int lm_bind_images_device(lm_detector* d, const uint8_t* rgb, int64_t rgb_pitch,
  * (LL.cpp:1366-1428, 1855-1938).  Leaves the ordered candidate records in device memory. */
 int lm_run(lm_detector* d, float threshold);
 /* lm_run split in two for pipelining: lm_enqueue issues every stage on the detector's stream and
- * returns without synchronising; lm_complete waits, and re-runs the refinement stage if the record
- * buffer was too small for the number of coarse candidates. */
+ * returns without synchronising; lm_complete waits.  Every completion (lm_complete, lm_complete_post,
+ * lm_complete_pose, lm_complete_detect, each frame of a batch) settles an overflow the same way: when the
+ * frame passed more coarse candidates than the candidate list holds, or kept more records than the result
+ * block holds, both grow and the frame is replayed from the refinement on, with every later stage enqueued
+ * for it (box NMS, pose stage, pose NMS), in up to three passes.  A caller's result block
+ * (lm_set_result_buffer) does not grow: LM_E_CAPACITY when the records outgrow it.  Neither grows with a
+ * connected peer exchange: LM_E_CAPACITY. */
 int lm_enqueue(lm_detector* d, float threshold);
 int lm_complete(lm_detector* d);
 /* Everything lm_enqueue does lazily on a new bank / selection / frame size (feature addresses for the frame size,
@@ -249,7 +254,8 @@ int lm_finish(lm_detector* d, const lm_record* records, int64_t n, lm_match* out
  *   lm_set_boxes      wh[n_templates][2]: box size per template in bank order (the drivers take it from their
  *                     template-info files); NULL / never called = Template::width/height of level 0 (LL.h:36-45)
  *   lm_enqueue_post   after lm_enqueue, same stream; top_k <= 0 = every survivor (at most 1024)
- *   lm_complete_post  waits; out[n_out] in pick order (best first); n_records = kept records the NMS saw
+ *   lm_complete_post  waits; out[n_out] in pick order (best first); n_records = kept records the NMS saw.  A frame
+ *                     that overflowed is grown and replayed first (lm_complete)
  *   lm_match_top      lm_upload_quantized + lm_enqueue + lm_enqueue_post + lm_complete_post
  * IoU as in the reference's nms(): float64, "+1" pixel convention, suppressed when ovr > threshold.  Equal
  * similarities (whose order the reference leaves to an unstable sort) are taken in template_id, class, y, x
@@ -283,8 +289,8 @@ int lm_match_top(lm_detector* d, const uint8_t* const* quantized, const int* row
  *                            the post and pose stages.
  *   lm_complete_pose         waits.  out[n_out] are the survivors in pick order (as lm_complete_post); R_out + 9i,
  *                            t_out + 3i, residual[i] are lm_icp_process_batch's outputs for survivor i (residual -1 and
- *                            R/t untouched on the early return of LL.cpp:52-55).  When the records outgrew the result
- *                            block, the refinement, the NMS and the pose stage run again before it returns. */
+ *                            R/t untouched on the early return of LL.cpp:52-55).  A frame that overflowed is grown and
+ *                            replayed first, pose stage included (lm_complete). */
 int lm_set_template_renders(lm_detector* d, int64_t first, int64_t n, const uint16_t* const* depths, int rows, int cols,
                             const float* K, const float* R, const float* t);
 int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iterations, int use_scene_cloud);
@@ -333,9 +339,8 @@ int lm_set_pose_estimation(lm_detector* d, int estimation);
  *                        exchange, every rank enqueues its match before any rank enqueues the post, pose and pose NMS
  *                        stages.
  *   lm_complete_detect   waits; out[n_out], R_out + 9k, t_out + 3k, residual[k] are the kept poses; n_survivors =
- *                        box-NMS survivors, n_posed = those with a pose, n_records as lm_complete_post.  When the records
- *                        outgrew the result block, the refinement, the box NMS, the pose stage and the pose NMS run again
- *                        before it returns.
+ *                        box-NMS survivors, n_posed = those with a pose, n_records as lm_complete_post.  A frame that
+ *                        overflowed is grown and replayed first, pose stage and pose NMS included (lm_complete).
  *   lm_nms_translations  steps 3-5 on caller arrays (t [n][3] f64, score [n] f64), with the same device routine, for the
  *                        poses of lm_icp_process_batch: keep[n_keep] are indices in keep order.  n <= 1024, else
  *                        LM_E_CAPACITY; threshold as above. */
@@ -360,8 +365,8 @@ int lm_nms_translations(int device, int64_t n, const double* t, const double* sc
  * LM_E_CAPACITY that leaves *n_out unwritten comes from a frame's match, where growing cap does not help);
  * LM_E_INVALID for n_frames < 1 or a NaN / negative translation threshold with pose_nms; LM_E_STATE without renders
  * for every selected template, and with a connected peer exchange (use lm_peer_detect_batch there).
- * Each frame runs the single-frame match and box NMS and waits for them (a frame whose records outgrow the result block
- * is redone there); its survivors and depth are copied aside on the stream.  The pose stage then runs once over all
+ * Each frame runs the single-frame match and box NMS and waits for them (a frame that overflows is grown and
+ * replayed there, as lm_complete describes); its survivors and depth are copied aside on the stream.  The pose stage then runs once over all
  * S survivors in chunks of at most 1024 slots (the single-frame bound for top_k = 0, so its cloud buffers do not grow
  * with the batch): 5 launches per chunk (4 with LM_ICP_POINT_TO_POINT, lm_set_pose_estimation), plus 1 launch of the
  * pose NMS for every frame.  Before its first frame the call
