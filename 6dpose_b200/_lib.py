@@ -27,7 +27,7 @@ PEER_HANDLE_BYTES = 64
 SYMBOLS = [
     "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks", "lm_coarse_descriptors",
     "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device",
-    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_debug_plan", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
+    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_debug_plan", "lm_debug_coarse", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
@@ -286,6 +286,7 @@ def load():
                                          ctypes.POINTER(vp), c_i64, vp] + L.lm_detect_batch.argtypes[7:]
     L.lm_debug_depth.argtypes = [vp, u16p, c_i64]
     L.lm_debug_plan.argtypes = [vp, i32p, c_i64]
+    L.lm_debug_coarse.argtypes = [vp, ctypes.POINTER(ctypes.c_uint32), c_i64, u16p, c_i64, i32p]
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -867,6 +868,21 @@ class NativeDetector:
         a = np.zeros(len(self.PLAN_KEYS), np.int32)
         check(self._L.lm_debug_plan(self._h, self._i32(a), a.size))
         return dict(zip(self.PLAN_KEYS, [int(v) for v in a]))
+
+    def coarse(self):
+        """The coarse scan's outputs of the last run (lm_debug_coarse): pass masks uint32 [n_work, nwords] and raw scores
+        uint16 [n_work, plane], 0 wherever the pass bit is clear; work items in this handle's shard order."""
+        dims = np.zeros(3, np.int32)
+        u32p, u16p = ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint16)
+        rc = self._L.lm_debug_coarse(self._h, None, 0, None, 0, self._i32(dims))  # dims only
+        if rc != LM_E_CAPACITY:
+            check(rc)
+        mask = np.zeros((int(dims[0]), int(dims[1])), np.uint32)
+        raw = np.zeros((int(dims[0]), int(dims[2])), np.uint16)
+        if rc == LM_E_CAPACITY:
+            check(self._L.lm_debug_coarse(self._h, mask.ctypes.data_as(u32p), mask.size, raw.ctypes.data_as(u16p), raw.size,
+                                          self._i32(dims)))
+        return mask, raw
 
     def set_timing(self, slots):
         check(self._L.lm_set_timing(self._h, int(slots)))

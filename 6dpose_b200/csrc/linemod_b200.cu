@@ -2630,6 +2630,31 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   return LM_OK;
 }
 
+// The coarse scan's outputs of the last lm_run, read back from the buffers k_refine_prep and k_refine read (no launch):
+// the pass masks whole, the raw scores with every position whose pass bit is clear zeroed here (the device leaves stale
+// values there).
+extern "C" int lm_debug_coarse(lm_detector* d, uint32_t* mask, int64_t mask_cap, uint16_t* raw, int64_t raw_cap, int32_t* dims3) {
+  if (!d || !dims3 || (!mask && mask_cap > 0) || (!raw && raw_cap > 0)) return fail(LM_E_INVALID, "null argument");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
+  const LevelHost& low = d->lv[d->L - 1];
+  const int64_t n_work = d->shard_count, nwords = low.nwords, plane = low.plane;
+  if ((size_t)(n_work * nwords) > d->d_mask.size() || (size_t)(n_work * plane) > d->d_raw.size())
+    return fail(LM_E_STATE, "the selection or the frame size changed since the last lm_run");
+  dims3[0] = (int32_t)n_work; dims3[1] = (int32_t)nwords; dims3[2] = (int32_t)plane;
+  if (n_work * nwords > mask_cap || n_work * plane > raw_cap)
+    return fail(LM_E_CAPACITY, "need %lld mask words and %lld raw scores", (long long)(n_work * nwords), (long long)(n_work * plane));
+  if (n_work == 0) return LM_OK;
+  CU(cudaSetDevice(d->device));
+  CU(cudaMemcpyAsync(mask, d->d_mask.get(), sizeof(uint32_t) * (size_t)(n_work * nwords), cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaMemcpyAsync(raw, d->d_raw.get(), sizeof(uint16_t) * (size_t)(n_work * plane), cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
+  for (int64_t w = 0; w < n_work; ++w)
+    for (int64_t j = 0; j < plane; ++j)
+      if (!((mask[w * nwords + (j >> 5)] >> (j & 31)) & 1u)) raw[w * plane + j] = 0;
+  return LM_OK;
+}
+
 extern "C" int lm_counters(lm_detector* d, int64_t* out8) {
   if (!d || !out8) return fail(LM_E_INVALID, "null argument");
   if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");

@@ -492,6 +492,18 @@ int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* o
  * for that frame and reports its counts. */
 #define LM_PLAN_ENTRIES 20
 int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap);
+/* Test getter: the coarse scan's outputs (k_coarse_packed / k_coarse_bytes) of the last completed frame, per work item of
+ * this handle's shard in shard order.  dims3 = {n_work, nwords, plane} of the lowest level; `mask` receives
+ * [n_work][nwords] pass words (bit j & 31 of word j >> 5: position j passed the coarse threshold, and the depth gate when
+ * the frame ran gated), `raw` [n_work][plane] raw scores: the score at every position whose pass bit is set, 0 at every
+ * other one (zeroed on the host; the device leaves stale values there).  Synchronises the stream and launches nothing.
+ * dims3 is filled before the capacity test: LM_E_CAPACITY when mask_cap < n_work * nwords or raw_cap < n_work * plane
+ * (mask and raw may be null with a capacity of 0, to ask for dims3).
+ * LM_E_STATE on a handle with no completed frame (or a host-only one), or when the selection or the frame size has grown
+ * since that frame.  Like lm_debug_plan it describes the last completed frame only between lm_complete (or lm_run) and
+ * the next lm_enqueue, and while the bank, the selection and the frame size stay as they were; after a batch, its last
+ * frame. */
+int lm_debug_coarse(lm_detector* d, uint32_t* mask, int64_t mask_cap, uint16_t* raw, int64_t raw_cap, int32_t* dims3);
 /* Counters of the last lm_run: [0] templates scanned, [1] coarse candidates, [2] algorithmic bytes of
  * the coarse scan (sum over templates, modalities of features x positions; SURVEY 8d),
  * [3] algorithmic bytes of the refinement (features x 256 per refined candidate and level: the reference's work,
