@@ -2244,13 +2244,13 @@ static int enqueue_pose(lm_detector* d) {
     if (rc) return rc;
   }
   const FrameChain& c = d->chain;
-  PoseEnqueue e;
-  e.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr};
-  e.d_surv = d->d_post_out.get(); e.d_counts = d->d_post_counts.get();
-  e.d_scene = d->fe_depth.get();
-  memcpy(e.sK, c.sK, sizeof(e.sK));
-  e.bound = c.top_k > 0 ? std::min(c.top_k, LM_POST_MAX) : LM_POST_MAX;
-  return pose_stage_enqueue(d->pose, e, &d->launches);
+  PoseRun run;
+  run.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr};
+  run.n_frames = 1; run.first = nullptr; run.d_counts = d->d_post_counts.get();
+  run.bound = c.top_k > 0 ? std::min(c.top_k, LM_POST_MAX) : LM_POST_MAX;
+  run.d_surv = d->d_post_out.get(); run.d_scene = d->fe_depth.get(); run.sK = c.sK;
+  run.pose_nms = 0;  // lm_enqueue_pose_nms may follow
+  return pose_stage_enqueue(d->pose, run, &d->launches);
 }
 
 extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iterations, int use_scene_cloud) {
@@ -2283,14 +2283,15 @@ extern "C" int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, do
   int rc = complete_post(d, out, cap, n_out, n_records, true);
   d->chain.pose = false;
   if (rc) return rc;
-  rc = pose_stage_finish(d->pose, d->stream.get(), d->h_post_out.get(), *n_out, R_out, t_out, residual);
+  int64_t n = 0, counts[4], stats[4];
+  rc = pose_stage_finish(d->pose, d->h_post_out.get(), *n_out, out, R_out, t_out, residual, cap, &n, counts, stats);
   if (rc) return rc;
-  pose_stage_stats(d->pose, *n_out, d->pose_stats);
+  memcpy(d->pose_stats, stats, sizeof(stats));
   return LM_OK;
 }
 
 static int enqueue_pose_nms(lm_detector* d) {
-  return pose_stage_enqueue_nms(d->pose, d->d_post_out.get(), d->d_post_counts.get(), d->chain.nms_thr, d->stream.get(), &d->launches);
+  return pose_stage_enqueue_nms(d->pose, d->chain.nms_thr, &d->launches);
 }
 
 extern "C" int lm_enqueue_pose_nms(lm_detector* d, double translation_threshold_mm) {
@@ -2316,9 +2317,13 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
   int rc = complete_post(d, nullptr, 0, &n_surv, n_records, false);
   d->chain.pose = d->chain.pose_nms = false;
   if (rc) return rc;
-  rc = pose_stage_finish_nms(d->pose, d->stream.get(), out, R_out, t_out, residual, cap, n_out, n_survivors, n_posed);
+  int64_t counts[4], stats[4];
+  rc = pose_stage_finish(d->pose, nullptr, n_surv, out, R_out, t_out, residual, cap, n_out, counts, stats);
+  if (rc && rc != LM_E_CAPACITY) return rc;  // a capacity error comes with the counts
+  if (n_survivors) *n_survivors = counts[1];
+  if (n_posed) *n_posed = counts[2];
   if (rc) return rc;
-  pose_stage_stats(d->pose, n_surv, d->pose_stats);
+  memcpy(d->pose_stats, stats, sizeof(stats));
   return LM_OK;
 }
 
@@ -2464,30 +2469,17 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     if (rc) return rc;
     d->px_pose_seq += pose_batch_chunks(first[n_frames]);
   }
-  PoseBatch b;
-  b.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr};
-  b.n_frames = n_frames;
-  b.first = first.data(); b.surv = surv.data(); b.sK = sceneK;
-  b.pose_nms = pose_nms ? 1 : 0; b.thr = translation_threshold_mm;
-  std::vector<int64_t> posed((size_t)n_frames), kept((size_t)n_frames);
-  int64_t stats[4];
-  rc = pose_batch_run(d->pose, b, &d->launches, posed.data(), kept.data(), peers ? stats : nullptr);
+  PoseRun run;
+  run.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr};
+  run.n_frames = n_frames; run.first = first.data(); run.d_counts = nullptr; run.bound = bound;
+  run.d_surv = d_surv; run.d_scene = d_scene; run.sK = sceneK;
+  run.pose_nms = pose_nms ? 1 : 0;
+  rc = pose_stage_enqueue(d->pose, run, &d->launches);
+  if (!rc && pose_nms) rc = pose_stage_enqueue_nms(d->pose, translation_threshold_mm, &d->launches);
   if (rc) return rc;
-  if (peers) memcpy(d->pose_stats, stats, sizeof(stats));
-  int64_t total = 0;
-  for (int f = 0; f < n_frames; ++f) {
-    frame_counts[4 * f] = kept[f];
-    frame_counts[4 * f + 2] = posed[f];
-    total += kept[f];
-  }
-  *n_out = total;
-  if (total > cap) return fail(LM_E_CAPACITY, "%lld entries in the batch, capacity %lld", (long long)total, (long long)cap);
-  int64_t at = 0;
-  for (int f = 0; f < n_frames; ++f) {
-    pose_batch_frame(d->pose, b, f, out + at, R_out + 9 * at, t_out + 3 * at, residual + at);
-    at += kept[f];
-  }
-  return LM_OK;
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  return pose_stage_finish(d->pose, surv.data(), 0, out, R_out, t_out, residual, cap, n_out, frame_counts, peers ? d->pose_stats : nullptr);
 }
 
 extern "C" int lm_detect_batch(lm_detector* d, int n_frames, const uint8_t* rgb, const uint16_t* depth, int rows, int cols,

@@ -1506,41 +1506,38 @@ struct lm_pose_stage {
   int64_t area_max = 0;        // largest crop
   DeviceArray<PoseTpl> d_tpl; DeviceArray<uint16_t> d_crops; DeviceArray<int32_t> d_class_begin;
   DeviceArray<PoseRt> d_rt;    // per template: R, t of its render (k_pose_nms composes the poses)
-  // per-frame buffers for pose_slots() survivors of pose_area() points per crop (pose_buffers)
+  // per-chunk buffers for pose_slots() survivors of pose_area() points per crop (pose_buffers); d_posed: a shared
+  // chunk's posed flags per slot, which k_pose_collect gathers into the run's
   DeviceArray<double> d_raw, d_cpts, d_pts, d_nrm;
   DeviceArray<unsigned long long> d_keys[2];
   DeviceArray<int32_t> d_vals[2];
   DeviceArray<int32_t> d_seg;
-  DeviceArray<IcpJob> d_jobs; DeviceArray<IcpOut> d_outs;
-  DeviceArray<int32_t> d_err;  // [0] cloud overflow; shared stage: [1] a peer's poses did not arrive, [2] entries published
+  DeviceArray<IcpJob> d_jobs;
   DeviceArray<uint8_t> d_sort_tmp;
-  PinnedArray<IcpOut> h_outs; PinnedArray<int32_t> h_err;
   DeviceArray<uint8_t> d_posed;
-  // pose NMS output block: PoseNmsHead + NMS_THREADS PoseNmsOut (device, pinned copy)
-  DeviceArray<uint8_t> d_nms; PinnedArray<uint8_t> h_nms;
-  // the enqueued frame
-  int bound = 0, srows = 0, scols = 0;
-  // its pose stage: launches, shared over the exchange (frame share_seq, collector timeout share_timeout_ns)
-  int64_t last_launches = 0;
-  bool shared = false; int32_t share_seq = 0; unsigned long long share_timeout_ns = 0;
-  // batch of frames (pose_batch_*): scene slots and survivors filled by the caller, then per survivor its frame, ICP
-  // output and posed flag, and the pose NMS blocks (one head per frame, kept poses at the frame's survivor offset)
   // A group of buffers that grows together is freed as a whole, then allocated in order: its last array is empty
   // unless every one was allocated, so its size stands for the group's.
+  // a batch's scene slots and survivors, filled by the caller (pose_batch_reserve)
   DeviceArray<uint16_t> d_bscene;
   DeviceArray<lm_match> d_bsurv;
-  DeviceArray<int32_t> d_bframe;  // frame of each survivor
-  DeviceArray<IcpOut> d_bouts; PinnedArray<IcpOut> h_bouts;
-  DeviceArray<uint8_t> d_bposed;
-  DeviceArray<PoseNmsOut> d_bnms; PinnedArray<PoseNmsOut> h_bnms;  // h_bnms last: survivors
+  // a run's outputs (pose_outputs), a frame's at offset 0: per survivor its frame, ICP output and posed flag
+  DeviceArray<int32_t> d_bframe;
+  DeviceArray<IcpOut> d_bouts; DeviceArray<uint8_t> d_bposed; PinnedArray<IcpOut> h_bouts;  // h_bouts last: survivors
+  // per frame its first survivor and intrinsics, per chunk (at most one per frame) a status block (PoseChunk; [3] a
+  // batch chunk's size)
   DeviceArray<int32_t> d_bfirst; DeviceArray<float> d_bsK;  // [frames + 1], [frames][9]
-  DeviceArray<PoseNmsHead> d_bhead; PinnedArray<PoseNmsHead> h_bhead;
-  // per chunk (at most one per frame) [0] cloud overflow, shared [1] a peer's poses did not arrive, [2] entries this
-  // rank published, [3] the chunk's size (device, pinned copy)
   DeviceArray<int32_t> d_bstat; PinnedArray<int32_t> h_bstat;  // h_bstat last: frames
+  // the pose NMS block (nms_heads, nms_out)
+  DeviceArray<uint8_t> d_bnms; PinnedArray<uint8_t> h_bnms;
+  // the run last enqueued, its share and survivor offsets copied; its launches, and how many of its ICP outputs (or,
+  // pose NMS enqueued, kept poses) are on their way to the host
+  PoseRun run = {};
+  PoseShare share = {};
+  std::vector<int64_t> first;
+  int64_t launches = 0, fetched = 0;
 };
 
-// The per-frame buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
+// The per-chunk buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
 // allocated last, so both are 0 unless every buffer was allocated.
 static int pose_slots(const lm_pose_stage* s) { return s->d_sort_tmp.empty() ? 0 : (int)s->d_jobs.size(); }
 static int64_t pose_area(const lm_pose_stage* s) {
@@ -1629,8 +1626,6 @@ static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
 }
 
 static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t area) {
-  CUI(s->d_err.reserve(4));
-  CUI(s->h_err.reserve(4));
   if (bound <= pose_slots(s) && area <= pose_area(s)) return LM_OK;
   CUI(cudaStreamSynchronize(st));
   const int B = std::max(bound, pose_slots(s));
@@ -1640,7 +1635,7 @@ static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t ar
     return lm_fail(LM_E_CAPACITY, "pose stage: %d survivors x %lld-pixel crops exceed 2^31 points: lower top_k", B, (long long)A);
   s->d_raw.reset(); s->d_cpts.reset(); s->d_pts.reset(); s->d_nrm.reset();
   for (int k = 0; k < 2; ++k) { s->d_keys[k].reset(); s->d_vals[k].reset(); }
-  s->d_seg.reset(); s->d_jobs.reset(); s->d_outs.reset(); s->d_sort_tmp.reset(); s->d_posed.reset(); s->h_outs.reset();
+  s->d_seg.reset(); s->d_jobs.reset(); s->d_sort_tmp.reset(); s->d_posed.reset();
   CUI(s->d_raw.assign(3 * slots));
   CUI(s->d_pts.assign(3 * slots));
   CUI(s->d_nrm.assign(3 * slots));
@@ -1651,9 +1646,7 @@ static int pose_buffers(lm_pose_stage* s, cudaStream_t st, int bound, int64_t ar
   }
   CUI(s->d_seg.assign(4 * B));
   CUI(s->d_jobs.assign(B));
-  CUI(s->d_outs.assign(B));
   CUI(s->d_posed.assign(B));
-  CUI(s->h_outs.assign(B));
   cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0].get(), s->d_keys[1].get());
   cub::DoubleBuffer<int32_t> dv(s->d_vals[0].get(), s->d_vals[1].get());
   size_t tmp_bytes = 0;
@@ -1743,36 +1736,150 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   return (sh ? 6 : 5) - (normals ? 0 : 1);
 }
 
-int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches) {
-  const PoseOptions& o = e.o;
-  cudaStream_t st = o.stream;
+#define POSE_CHUNK 1024     // survivor slots per chunk: a frame's bound for top_k = 0
+#define NMS_FIRST_FETCH 16
+
+int pose_batch_chunks(int64_t S) { return (int)((S + POSE_CHUNK - 1) / POSE_CHUNK); }
+
+// The pose NMS block of a run of n frames: the frames' heads, then the kept poses, frame f's from its first survivor.
+// One copy thus brings back the heads and the first kept poses.
+static PoseNmsHead* nms_heads(uint8_t* block) { return reinterpret_cast<PoseNmsHead*>(block); }
+static PoseNmsOut* nms_out(uint8_t* block, int n) { return reinterpret_cast<PoseNmsOut*>(block + sizeof(PoseNmsHead) * n); }
+
+// The outputs of a run of up to n_frames frames and S survivors.  Grow-only: an earlier run may still use them.
+static int pose_outputs(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S) {
+  const size_t nms = sizeof(PoseNmsHead) * n_frames + sizeof(PoseNmsOut) * S;
+  const bool frames = (size_t)4 * n_frames > s->h_bstat.size(), surv = (size_t)S > s->h_bouts.size(), block = nms > s->h_bnms.size();
+  if (!frames && !surv && !block) return LM_OK;
+  CUI(cudaStreamSynchronize(st));
+  if (frames) {
+    s->d_bfirst.reset(); s->d_bsK.reset(); s->d_bstat.reset(); s->h_bstat.reset();
+    CUI(s->d_bfirst.assign(n_frames + 1));
+    CUI(s->d_bsK.assign(9 * (size_t)n_frames));
+    CUI(s->d_bstat.assign(4 * (size_t)n_frames));  // chunks <= frames: a frame has <= 1024 survivors
+    CUI(s->h_bstat.assign(4 * (size_t)n_frames));
+  }
+  if (surv) {
+    s->d_bframe.reset(); s->d_bouts.reset(); s->d_bposed.reset(); s->h_bouts.reset();
+    CUI(s->d_bframe.assign(S));
+    CUI(s->d_bouts.assign(S));
+    CUI(s->d_bposed.assign(S));
+    CUI(s->h_bouts.assign(S));
+  }
+  if (block) {
+    s->d_bnms.reset(); s->h_bnms.reset();
+    CUI(s->d_bnms.assign(nms));
+    CUI(s->h_bnms.assign(nms));
+  }
+  return LM_OK;
+}
+
+// The renders on the device and every buffer a run of n_frames frames and S survivors needs.
+static int pose_prepare(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S) {
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
   }
-  int rc = pose_buffers(s, st, e.bound, s->area_max);
+  S = std::max<int64_t>(S, 1);
+  int rc = pose_outputs(s, st, n_frames, S);
   if (rc) return rc;
+  return pose_buffers(s, st, (int)std::min<int64_t>(S, POSE_CHUNK), s->area_max);
+}
+
+int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
+                       lm_match** d_surv) {
+  const size_t pix = (size_t)n_frames * frame_pixels;
+  if (pix > s->d_bscene.size() || (size_t)max_surv > s->d_bsurv.size()) {
+    CUI(cudaStreamSynchronize(st));  // an earlier batch may still read them
+    CUI(s->d_bscene.reserve(pix));
+    CUI(s->d_bsurv.reserve((size_t)max_surv));
+  }
+  // and everything the run may need for max_surv survivors: once frames run, no device memory is freed (a free waits for
+  // the whole device, a spinning peer collector of a shared batch included)
+  int rc = pose_prepare(s, st, n_frames, max_surv);
+  if (rc) return rc;
+  *d_scene = s->d_bscene.get();
+  *d_surv = s->d_bsurv.get();
+  return LM_OK;
+}
+
+int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) {
+  const PoseOptions& o = run.o;
+  cudaStream_t st = o.stream;
   const PoseShare* sh = o.share;
-  CUI(cudaMemsetAsync(s->d_err.get(), 0, sizeof(int32_t), st));
-  PoseChunk c;
-  c.surv = e.d_surv; c.counts = e.d_counts; c.slots = e.bound;
-  c.scene = e.d_scene; c.frame_of = nullptr; c.sKs = nullptr; c.sK = e.sK;
-  c.outs = s->d_outs.get(); c.posed = s->d_posed.get(); c.status = s->d_err.get(); c.seq = sh ? sh->seq : 0;
-  const int k = pose_chunk(s, o, c);
-  if (k < 0) return k;
-  s->last_launches = k;
-  *launches += k;
-  CUI(cudaMemcpyAsync(s->h_outs.get(), s->d_outs.get(), sizeof(IcpOut) * std::min(e.bound, POSE_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
-  CUI(cudaMemcpyAsync(s->h_err.get(), s->d_err.get(), sizeof(int32_t) * (sh ? 3 : 1), cudaMemcpyDeviceToHost, st));
-  s->bound = e.bound; s->srows = o.srows; s->scols = o.scols;
-  s->shared = sh != nullptr;
-  s->share_seq = sh ? sh->seq : 0;
-  s->share_timeout_ns = sh ? sh->timeout_ns : 0;
+  const bool batch = run.first != nullptr;
+  const int nf = run.n_frames;
+  const int64_t S = batch ? run.first[nf] : run.bound;  // survivors the outputs hold
+  const int nc = batch ? pose_batch_chunks(S) : 1;
+  int rc = pose_prepare(s, st, nf, S);
+  if (rc) return rc;
+  if (batch) {  // each survivor's frame, each frame's first survivor and intrinsics, each chunk's status block and size
+    std::vector<int32_t> frame_of((size_t)S);
+    for (int f = 0; f < nf; ++f)
+      for (int64_t k = run.first[f]; k < run.first[f + 1]; ++k) frame_of[(size_t)k] = f;
+    std::vector<int32_t> first32(run.first, run.first + nf + 1);
+    std::vector<int32_t> stat((size_t)4 * nc, 0);
+    for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_CHUNK, POSE_CHUNK);
+    if (S) CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
+    CUI(cudaMemcpyAsync(s->d_bfirst.get(), first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
+    CUI(cudaMemcpyAsync(s->d_bsK.get(), run.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
+    if (nc) CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  } else {  // a frame's survivor count is the box NMS's
+    CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4, st));
+  }
+  int64_t stage_launches = 0;
+  for (int c = 0; c < nc; ++c) {
+    const int64_t c0 = (int64_t)c * POSE_CHUNK;
+    PoseChunk k;
+    k.surv = run.d_surv + c0;
+    k.counts = batch ? s->d_bstat.get() + 4 * c + 3 : run.d_counts;
+    k.slots = batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound;
+    k.scene = run.d_scene; k.frame_of = batch ? s->d_bframe.get() + c0 : nullptr;
+    k.sKs = batch ? s->d_bsK.get() : nullptr; k.sK = batch ? nullptr : run.sK;
+    k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
+    const int l = pose_chunk(s, o, k);
+    if (l < 0) return l;
+    stage_launches += l;
+    *launches += l;
+  }
+  // the status blocks, and unless a pose NMS follows the ICP outputs: a batch's all, a frame's first window
+  const int64_t fetch = run.pose_nms ? 0 : batch ? S : std::min(run.bound, POSE_FIRST_FETCH);
+  if (fetch) CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * fetch, cudaMemcpyDeviceToHost, st));
+  if (nc) CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  s->run = run;
+  s->share = sh ? *sh : PoseShare();
+  s->run.o.share = sh ? &s->share : nullptr;
+  if (batch) s->first.assign(run.first, run.first + nf + 1);
+  s->run.first = batch ? s->first.data() : nullptr;
+  s->launches = stage_launches;
+  s->fetched = fetch;
+  return LM_OK;
+}
+
+int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches) {
+  PoseRun& r = s->run;
+  if (r.bound > NMS_THREADS) return lm_fail(LM_E_STATE, "pose stage launched for %d survivors, the pose NMS takes %d", r.bound, NMS_THREADS);
+  const bool batch = r.first != nullptr;
+  const int nf = r.n_frames;
+  cudaStream_t st = r.o.stream;
+  PoseNmsParams p;
+  p.surv = r.d_surv; p.counts = batch ? nullptr : r.d_counts; p.posed = s->d_bposed.get(); p.outs = s->d_bouts.get();
+  p.rt = s->d_rt.get(); p.class_begin = s->d_class_begin.get();
+  p.thr = thr;
+  p.head = nms_heads(s->d_bnms.get()); p.out = nms_out(s->d_bnms.get(), nf);
+  p.frame_first = batch ? s->d_bfirst.get() : nullptr;
+  k_pose_nms<<<nf, NMS_THREADS, 0, st>>>(p);
+  CUI(cudaGetLastError());
+  ++*launches;
+  // the heads and the kept poses: a batch's all, a frame's first window
+  r.pose_nms = 1;
+  s->fetched = batch ? r.first[nf] : std::min(r.bound, NMS_FIRST_FETCH);
+  CUI(cudaMemcpyAsync(s->h_bnms.get(), s->d_bnms.get(), sizeof(PoseNmsHead) * nf + sizeof(PoseNmsOut) * s->fetched, cudaMemcpyDeviceToHost, st));
   return LM_OK;
 }
 
 // After the stream has been synchronised: the error of nb status blocks of 4 int32 (PoseChunk), block c that of pose
-// exchange seq + c when shared; a batch's message names the chunk.  *published (may be null): the entries summed.
+// exchange seq + c when shared; a batch's message names the chunk.  *published: the entries summed.
 static int pose_status(const int32_t* h, int nb, bool shared, int32_t seq, unsigned long long timeout_ns, bool batch,
                        int64_t* published) {
   int32_t overflow = 0;
@@ -1792,20 +1899,8 @@ static int pose_status(const int32_t* h, int nb, bool shared, int32_t seq, unsig
     if (shared) sum += b[2];
   }
   if (overflow) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
-  if (published) *published = sum;
+  *published = sum;
   return LM_OK;
-}
-
-// What lm_pose_stats returns for a stage of n survivors.
-static void pose_stats(int64_t* out4, int64_t n, bool shared, int64_t published, int64_t launches) {
-  out4[0] = n;
-  out4[1] = shared ? published : n;
-  out4[2] = launches;
-  out4[3] = shared ? 1 : 0;
-}
-
-void pose_stage_stats(const lm_pose_stage* s, int64_t n, int64_t* out4) {
-  pose_stats(out4, n, s->shared, s->h_err[2], s->last_launches);
 }
 
 // Survivor m's registered render, or null.
@@ -1831,48 +1926,9 @@ static void survivor_pose(const TplHost& h, const lm_match& m, int srows, int sc
   *residual = (float)o.fitness;
 }
 
-int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
-                      float* residual) {
-  if (n > s->bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, s->bound);
-  if (n > POSE_FIRST_FETCH) {
-    CUI(cudaMemcpyAsync(s->h_outs.get() + POSE_FIRST_FETCH, s->d_outs.get() + POSE_FIRST_FETCH, sizeof(IcpOut) * (size_t)(n - POSE_FIRST_FETCH),
-                        cudaMemcpyDeviceToHost, st));
-    CUI(cudaStreamSynchronize(st));
-  }
-  int rc = pose_status(s->h_err.get(), 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
-  if (rc) return rc;
-  for (int64_t i = 0; i < n; ++i) {
-    const TplHost* h = survivor_render(s, surv[i]);
-    if (!h) return lm_fail(LM_E_STATE, "survivor %lld: template without a registered render", (long long)i);
-    survivor_pose(*h, surv[i], s->srows, s->scols, s->h_outs[i], R_out + 9 * i, t_out + 3 * i, residual + i);
-  }
-  return LM_OK;
-}
-
-// ---- pose NMS behind the pose stage ----
-#define NMS_FIRST_FETCH 16
-
-static PoseNmsOut* nms_entries(uint8_t* block) { return reinterpret_cast<PoseNmsOut*>(block + sizeof(PoseNmsHead)); }
-
-// k_pose_nms over n_frames frames, as PoseNmsParams.
-static int pose_nms_launch(const lm_pose_stage* s, int n_frames, const lm_match* surv, const int32_t* counts, const int32_t* frame_first,
-                           const uint8_t* posed, const IcpOut* outs, double thr, PoseNmsHead* head, PoseNmsOut* out, cudaStream_t st,
-                           int64_t* launches) {
-  PoseNmsParams p;
-  p.surv = surv; p.counts = counts; p.posed = posed; p.outs = outs;
-  p.rt = s->d_rt.get(); p.class_begin = s->d_class_begin.get();
-  p.thr = thr;
-  p.head = head; p.out = out;
-  p.frame_first = frame_first;
-  k_pose_nms<<<n_frames, NMS_THREADS, 0, st>>>(p);
-  CUI(cudaGetLastError());
-  ++*launches;
-  return LM_OK;
-}
-
 // n kept poses e[] into the caller's arrays (out may be null).
-static void copy_kept(const PoseNmsOut* e, int n, lm_match* out, double* R_out, double* t_out, float* residual) {
-  for (int k = 0; k < n; ++k) {
+static void copy_kept(const PoseNmsOut* e, int64_t n, lm_match* out, double* R_out, double* t_out, float* residual) {
+  for (int64_t k = 0; k < n; ++k) {
     if (out) out[k] = e[k].m;
     memcpy(R_out + 9 * k, e[k].R, sizeof(e[k].R));
     memcpy(t_out + 3 * k, e[k].t, sizeof(e[k].t));
@@ -1880,181 +1936,75 @@ static void copy_kept(const PoseNmsOut* e, int n, lm_match* out, double* R_out, 
   }
 }
 
-int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32_t* d_counts, double thr, cudaStream_t st,
-                           int64_t* launches) {
-  if (s->bound > NMS_THREADS) return lm_fail(LM_E_STATE, "pose stage launched for %d survivors, the pose NMS takes %d", s->bound, NMS_THREADS);
-  const size_t bytes = sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_THREADS;
-  CUI(s->d_nms.reserve(bytes));
-  CUI(s->h_nms.reserve(bytes));
-  int rc = pose_nms_launch(s, 1, d_surv, d_counts, nullptr, s->d_posed.get(), s->d_outs.get(), thr, reinterpret_cast<PoseNmsHead*>(s->d_nms.get()),
-                           nms_entries(s->d_nms.get()), st, launches);
-  if (rc) return rc;
-  // the header and a first window of kept poses; the rest only if there are more
-  CUI(cudaMemcpyAsync(s->h_nms.get(), s->d_nms.get(), sizeof(PoseNmsHead) + sizeof(PoseNmsOut) * NMS_FIRST_FETCH, cudaMemcpyDeviceToHost, st));
-  return LM_OK;
-}
-
-int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
-                          int64_t* n_out, int64_t* n_survivors, int64_t* n_posed) {
-  int rc = pose_status(s->h_err.get(), 1, s->shared, s->share_seq, s->share_timeout_ns, false, nullptr);
-  if (rc) return rc;
-  const PoseNmsHead h = *reinterpret_cast<const PoseNmsHead*>(s->h_nms.get());
-  *n_out = h.kept;
-  if (n_survivors) *n_survivors = h.survivors;
-  if (n_posed) *n_posed = h.posed;
-  if (h.kept > cap) return lm_fail(LM_E_CAPACITY, "%d poses kept, capacity %lld", h.kept, (long long)cap);
-  if (h.kept > NMS_FIRST_FETCH) {
-    CUI(cudaMemcpyAsync(nms_entries(s->h_nms.get()) + NMS_FIRST_FETCH, nms_entries(s->d_nms.get()) + NMS_FIRST_FETCH,
-                        sizeof(PoseNmsOut) * (size_t)(h.kept - NMS_FIRST_FETCH), cudaMemcpyDeviceToHost, st));
-    CUI(cudaStreamSynchronize(st));
-  }
-  copy_kept(nms_entries(s->h_nms.get()), h.kept, out, R_out, t_out, residual);
-  return LM_OK;
-}
-
-// ---- a batch of frames through one pose stage (lm_detect_batch) ----
-#define POSE_BATCH_CHUNK 1024  // survivor slots per chunk: the single-frame bound for top_k = 0
-
-int pose_batch_chunks(int64_t S) { return (int)((S + POSE_BATCH_CHUNK - 1) / POSE_BATCH_CHUNK); }
-
-static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S);
-
-int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
-                       lm_match** d_surv) {
-  const size_t pix = (size_t)n_frames * frame_pixels;
-  const bool more_frames = (size_t)n_frames * 4 > s->h_bstat.size();
-  if (pix > s->d_bscene.size() || (size_t)max_surv > s->d_bsurv.size() || more_frames) {
-    CUI(cudaStreamSynchronize(st));  // an earlier batch may still read them
-    CUI(s->d_bscene.reserve(pix));
-    CUI(s->d_bsurv.reserve((size_t)max_surv));
-    if (more_frames) {
-      s->d_bfirst.reset(); s->d_bsK.reset(); s->d_bhead.reset(); s->h_bhead.reset(); s->d_bstat.reset(); s->h_bstat.reset();
-      CUI(s->d_bfirst.assign(n_frames + 1));
-      CUI(s->d_bsK.assign(9 * (size_t)n_frames));
-      CUI(s->d_bhead.assign(n_frames));
-      CUI(s->h_bhead.assign(n_frames));
-      CUI(s->d_bstat.assign(4 * (size_t)n_frames));  // chunks <= n_frames: a frame has <= 1024 survivors
-      CUI(s->h_bstat.assign(4 * (size_t)n_frames));
-    }
-  }
-  // and everything pose_batch_run may need for max_surv survivors: once frames run, no device memory is freed (a free
-  // waits for the whole device, a spinning peer collector of a shared batch included)
-  if (s->dirty) {
-    int rc = pose_upload(s, st);
-    if (rc) return rc;
-  }
-  int rc = pose_batch_survivors(s, st, std::max<int64_t>(max_surv, 1));
-  if (rc) return rc;
-  rc = pose_buffers(s, st, (int)std::min<int64_t>(std::max<int64_t>(max_surv, 1), POSE_BATCH_CHUNK), s->area_max);
-  if (rc) return rc;
-  *d_scene = s->d_bscene.get();
-  *d_surv = s->d_bsurv.get();
-  return LM_OK;
-}
-
-static int pose_batch_survivors(lm_pose_stage* s, cudaStream_t st, int64_t S) {
-  if ((size_t)S <= s->h_bnms.size()) return LM_OK;
-  CUI(cudaStreamSynchronize(st));
-  s->d_bframe.reset(); s->d_bouts.reset(); s->d_bposed.reset(); s->d_bnms.reset(); s->h_bouts.reset(); s->h_bnms.reset();
-  CUI(s->d_bframe.assign(S));
-  CUI(s->d_bouts.assign(S));
-  CUI(s->d_bposed.assign(S));
-  CUI(s->d_bnms.assign(S));
-  CUI(s->h_bouts.assign(S));
-  CUI(s->h_bnms.assign(S));
-  return LM_OK;
-}
-
-int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4) {
-  const PoseOptions& o = b.o;
-  cudaStream_t st = o.stream;
-  const int nf = b.n_frames;
-  const int64_t S = b.first[nf];
-  const PoseShare* sh = o.share;
-  const int nc = pose_batch_chunks(S);
-  if (s->dirty) {
-    int rc = pose_upload(s, st);
-    if (rc) return rc;
-  }
-  int rc = pose_batch_survivors(s, st, std::max<int64_t>(S, 1));
-  if (rc) return rc;
-  rc = pose_buffers(s, st, (int)std::min<int64_t>(std::max<int64_t>(S, 1), POSE_BATCH_CHUNK), s->area_max);
-  if (rc) return rc;
-  std::vector<int32_t> frame_of((size_t)S);
-  for (int f = 0; f < nf; ++f)
-    for (int64_t k = b.first[f]; k < b.first[f + 1]; ++k) frame_of[(size_t)k] = f;
-  std::vector<int32_t> first32(b.first, b.first + nf + 1);
-  // per chunk a status block (PoseChunk), [3] the chunk's size
-  std::vector<int32_t> stat((size_t)4 * nc, 0);
-  for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_BATCH_CHUNK, POSE_BATCH_CHUNK);
-  if (S) CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bfirst.get(), first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bsK.get(), b.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
-  if (nc) CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
-  int64_t stage_launches = 0;
-  for (int c = 0; c < nc; ++c) {
-    const int64_t c0 = (int64_t)c * POSE_BATCH_CHUNK;
-    PoseChunk k;
-    k.surv = s->d_bsurv.get() + c0; k.counts = s->d_bstat.get() + 4 * c + 3; k.slots = stat[(size_t)4 * c + 3];
-    k.scene = s->d_bscene.get(); k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get(); k.sK = nullptr;
-    k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
-    const int l = pose_chunk(s, o, k);
-    if (l < 0) return l;
-    stage_launches += l;
-    *launches += l;
-  }
-  if (b.pose_nms) {
-    rc = pose_nms_launch(s, nf, s->d_bsurv.get(), nullptr, s->d_bfirst.get(), s->d_bposed.get(), s->d_bouts.get(), b.thr, s->d_bhead.get(), s->d_bnms.get(), st, launches);
-    if (rc) return rc;
-    CUI(cudaMemcpyAsync(s->h_bhead.get(), s->d_bhead.get(), sizeof(PoseNmsHead) * nf, cudaMemcpyDeviceToHost, st));
-  } else if (S) {
-    CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
-  }
-  if (nc) CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
-  CUI(cudaStreamSynchronize(st));
-  CUI(cudaGetLastError());
+int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_match* out, double* R_out, double* t_out, float* residual,
+                      int64_t cap, int64_t* n_out, int64_t* counts, int64_t* stats4) {
+  const PoseRun& r = s->run;
+  const PoseShare* sh = r.o.share;
+  const bool batch = r.first != nullptr;
+  const int nf = r.n_frames;
+  const int64_t frame_first[2] = {0, n};
+  const int64_t* first = batch ? r.first : frame_first;
+  const int64_t S = first[nf];
+  if (!batch && n > r.bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, r.bound);
   int64_t published = 0;
-  rc = pose_status(s->h_bstat.get(), nc, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0, true, &published);
+  int rc = pose_status(s->h_bstat.get(), batch ? pose_batch_chunks(S) : 1, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0,
+                       batch, &published);
   if (rc) return rc;
-  if (stats4) pose_stats(stats4, S, sh != nullptr, published, stage_launches);
-  if (b.pose_nms) {
-    // the kept poses of every frame, each range where its frame's survivors begin
-    bool more = false;
-    for (int f = 0; f < nf; ++f) {
-      posed[f] = s->h_bhead[f].posed;
-      kept[f] = s->h_bhead[f].kept;
-      if (kept[f] > 0) {
-        CUI(cudaMemcpyAsync(s->h_bnms.get() + b.first[f], s->d_bnms.get() + b.first[f], sizeof(PoseNmsOut) * kept[f], cudaMemcpyDeviceToHost, st));
-        more = true;
+  if (stats4) {
+    stats4[0] = S;
+    stats4[1] = sh ? published : S;
+    stats4[2] = s->launches;
+    stats4[3] = sh ? 1 : 0;
+  }
+  const PoseNmsHead* heads = nms_heads(s->h_bnms.get());
+  PoseNmsOut* entries = nms_out(s->h_bnms.get(), nf);
+  int64_t total = 0, end = 0;  // entries, and the end of the host copy they need
+  for (int f = 0; f < nf; ++f) {
+    int64_t* fc = counts + 4 * f;
+    if (r.pose_nms) {
+      fc[0] = heads[f].kept; fc[1] = heads[f].survivors; fc[2] = heads[f].posed;
+    } else {
+      fc[0] = fc[1] = first[f + 1] - first[f];
+      fc[2] = 0;
+      for (int64_t i = first[f]; i < first[f + 1]; ++i) {
+        const TplHost* h = survivor_render(s, surv[i]);
+        if (!h && batch)
+          return lm_fail(LM_E_STATE, "frame %d, survivor %lld: template without a registered render", f, (long long)(i - first[f]));
+        if (!h) return lm_fail(LM_E_STATE, "survivor %lld: template without a registered render", (long long)i);
+        if (survivor_fits(*h, surv[i], r.o.srows, r.o.scols)) ++fc[2];
       }
     }
-    if (more) CUI(cudaStreamSynchronize(st));
+    total += fc[0];
+    end = std::max(end, first[f] + fc[0]);
+  }
+  *n_out = total;
+  if (total > cap) {
+    if (batch) return lm_fail(LM_E_CAPACITY, "%lld entries in the batch, capacity %lld", (long long)total, (long long)cap);
+    return lm_fail(LM_E_CAPACITY, "%lld poses kept, capacity %lld", (long long)total, (long long)cap);
+  }
+  if (end > s->fetched) {  // a frame's entries beyond its first window
+    cudaStream_t st = r.o.stream;
+    if (r.pose_nms)
+      CUI(cudaMemcpyAsync(entries + s->fetched, nms_out(s->d_bnms.get(), nf) + s->fetched, sizeof(PoseNmsOut) * (size_t)(end - s->fetched),
+                          cudaMemcpyDeviceToHost, st));
+    else
+      CUI(cudaMemcpyAsync(s->h_bouts.get() + s->fetched, s->d_bouts.get() + s->fetched, sizeof(IcpOut) * (size_t)(end - s->fetched),
+                          cudaMemcpyDeviceToHost, st));
+    CUI(cudaStreamSynchronize(st));
+  }
+  if (r.pose_nms) {
+    int64_t at = 0;
+    for (int f = 0; f < nf; ++f) {
+      copy_kept(entries + first[f], counts[4 * f], out ? out + at : nullptr, R_out + 9 * at, t_out + 3 * at, residual + at);
+      at += counts[4 * f];
+    }
     return LM_OK;
   }
-  for (int f = 0; f < nf; ++f) {
-    posed[f] = 0;
-    kept[f] = b.first[f + 1] - b.first[f];
-    for (int64_t i = b.first[f]; i < b.first[f + 1]; ++i) {
-      const TplHost* h = survivor_render(s, b.surv[i]);
-      if (!h) return lm_fail(LM_E_STATE, "frame %d, survivor %lld: template without a registered render", f, (long long)(i - b.first[f]));
-      if (survivor_fits(*h, b.surv[i], o.srows, o.scols)) ++posed[f];
-    }
+  for (int64_t i = 0; i < S; ++i) {  // every survivor, frame after frame
+    if (out) out[i] = surv[i];
+    survivor_pose(*survivor_render(s, surv[i]), surv[i], r.o.srows, r.o.scols, s->h_bouts[i], R_out + 9 * i, t_out + 3 * i, residual + i);
   }
   return LM_OK;
-}
-
-void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual) {
-  const int64_t first = b.first[f], n = b.first[f + 1] - first;
-  if (b.pose_nms) {
-    copy_kept(s->h_bnms.get() + first, s->h_bhead[f].kept, out, R_out, t_out, residual);
-    return;
-  }
-  for (int64_t i = 0; i < n; ++i) {
-    const lm_match& m = b.surv[first + i];
-    out[i] = m;
-    survivor_pose(*survivor_render(s, m), m, b.o.srows, b.o.scols, s->h_bouts[first + i], R_out + 9 * i, t_out + 3 * i,
-                  residual + i);  // pose_batch_run checked the render
-  }
 }
 
 // Steps 3-5 of the pose NMS on caller arrays (lm_nms_translations): the same device routine as k_pose_nms.

@@ -1,11 +1,13 @@
 // lm_pose.h -- internal interface between the detector (linemod_b200.cu) and the on-device pose stage (lm_icp.cu).
 //
 // The pose stage refines the NMS survivors of k_post_nms where they lie: per-template render crops registered once
-// (lm_set_template_renders), then per frame k_pose_cloud (box test, back-projection, centroids, voxel keys), a CUB
+// (lm_set_template_renders), then per run k_pose_cloud (box test, back-projection, centroids, voxel keys), a CUB
 // segmented radix sort of the voxel keys, k_pose_voxel (voxel means) and the ICP kernels of lm_icp_process_batch
-// (k_icp_normals + k_icp_point_to_plane, or k_icp_point_to_point alone), all on the detector's stream.  The host composes result = T * init_base after the copy.
-// The pose NMS (k_pose_nms, one CTA behind k_icp_point_to_plane) composes the poses on the device instead, runs the
-// greedy translation NMS of linemod_ros/detect.py over them and compacts the kept ones into one output block.
+// (k_icp_normals + k_icp_point_to_plane, or k_icp_point_to_point alone), all on the detector's stream.  A run is a batch
+// of frames, and a single frame is a one-frame run of the same stage: the same chunks, outputs, readbacks and finish.
+// The host composes result = T * init_base after the copy.  The pose NMS (k_pose_nms, one CTA per frame behind the ICP
+// kernel) composes the poses on the device instead, runs the greedy translation NMS of linemod_ros/detect.py over them
+// and compacts the kept ones into one output block.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,7 +26,7 @@ int pose_stage_register(lm_pose_stage* s, const int32_t* class_begin, int n_clas
 // Every template of the selection has a render.
 bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel);
 
-// A frame's pose stage is one chunk of survivors, a batch's one chunk per 1024 survivors.  Slot j of a chunk takes
+// A run is one chunk per 1024 survivors, a frame's one chunk.  Slot j of a chunk takes
 // survivor rank + j * world, so the launches are sized for ceil(survivors / world) slots; unshared, rank 0 and world 1.
 // Shared over the ranks of the peer exchange (lm_peer_share_pose), survivor i (pick order of k_post_nms, the same on
 // every rank) is thus refined by rank i % world.  The ICP kernel's SHARE instantiation stores each survivor's result into
@@ -43,7 +45,7 @@ struct PoseShare {
 };
 size_t pose_share_area_bytes();
 
-// What a frame's and a batch's pose stage share.
+// What every chunk of a run shares.
 struct PoseOptions {
   int srows, scols;           // scene depth size
   int use_scene_cloud, max_iterations;
@@ -51,50 +53,44 @@ struct PoseOptions {
   cudaStream_t stream;
   const PoseShare* share;     // null: this rank refines every survivor
 };
-struct PoseEnqueue {
+
+// One run of the pose stage: a batch of frames (lm_detect_batch, lm_peer_detect_batch), or a frame as a one-frame run
+// whose survivor count lives on the device.  Chunk c takes survivors [1024 c, 1024 (c + 1)); with a share it is pose
+// exchange share->seq + c.  The stage records the run it last enqueued (share and survivor offsets copied).
+struct PoseRun {
   PoseOptions o;
-  const lm_match* d_surv;     // survivors in pick order (k_post_nms output)
-  const int32_t* d_counts;    // [0] = survivors written
-  const uint16_t* d_scene;    // scene depth, srows x scols u16 mm
-  float sK[9];
-  int bound;                  // survivors the launches are sized for (top_k, or every survivor k_post_nms may write)
+  int n_frames;
+  const int64_t* first;       // batch: [n_frames + 1] survivor offsets (host), frame f's at [first[f], first[f + 1]); frame: null
+  const int32_t* d_counts;    // frame: [0] = survivors written (device)
+  int bound;                  // most survivors of a frame (top_k, or every survivor k_post_nms may write); a frame's launches
+                              // are sized for it
+  const lm_match* d_surv;     // survivors in pick order (device)
+  const uint16_t* d_scene;    // scene depth, srows x scols u16 mm; frame f's at + f * srows * scols
+  const float* sK;            // [n_frames][9]
+  int pose_nms;               // 1: pose_stage_enqueue_nms follows, so the ICP outputs are not read back
 };
-int pose_stage_enqueue(lm_pose_stage* s, const PoseEnqueue& e, int64_t* launches);
-// After pose_stage_finish / pose_stage_finish_nms of a frame with n survivors: what lm_pose_stats returns (survivors,
-// hypotheses this rank refined, launches of the stage, 1 if shared).
-void pose_stage_stats(const lm_pose_stage* s, int64_t n, int64_t* out4);
-// After the stream has been synchronised: surv[n] are the survivors (host copy).  Outputs as lm_icp_process_batch.
-int pose_stage_finish(lm_pose_stage* s, cudaStream_t st, const lm_match* surv, int64_t n, double* R_out, double* t_out,
-                      float* residual);
 
-// Pose NMS behind pose_stage_enqueue on the same stream: d_surv / d_counts as given to it.  Also enqueues the copy of
-// the output block's header and first entries.
-int pose_stage_enqueue_nms(lm_pose_stage* s, const lm_match* d_surv, const int32_t* d_counts, double thr, cudaStream_t st,
-                           int64_t* launches);
-// After the stream has been synchronised: the kept poses in keep order (outputs as lm_complete_detect).
-int pose_stage_finish_nms(lm_pose_stage* s, cudaStream_t st, lm_match* out, double* R_out, double* t_out, float* residual, int64_t cap,
-                          int64_t* n_out, int64_t* n_survivors, int64_t* n_posed);
+// Three calls, in this order, for a frame and a batch alike.
+// The run's chunks on o.stream, each with its status block, then the copies the host will need: the status blocks and
+// (pose_nms 0) the ICP outputs -- a batch's all, a frame's first window.  Grows the buffers for the run (and synchronises
+// then); a batch's were grown by pose_batch_reserve.
+int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches);
+// Pose NMS behind pose_stage_enqueue on the same stream: one k_pose_nms launch, one CTA per frame.  Also enqueues the copy
+// of the frames' heads and their kept poses (a batch's all, a frame's first window).
+int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches);
+// After the caller has synchronised the stream: the run's status, then frame f's entries -- its kept poses (pose NMS), or
+// every survivor with its pose (outputs as lm_complete_pose) -- after those of frames 0..f-1 in out / R_out + 9k /
+// t_out + 3k / residual[k] (out may be null).  surv: the host copy of the survivors (pose_nms 0 only); n: a frame's
+// survivor count as read back.  counts[4f .. 4f + 2] = entries, survivors, survivors with a pose; *n_out = entries in all,
+// LM_E_CAPACITY beyond cap (both written once the status is clean).  stats4 (may be null): what lm_pose_stats returns.
+// Copies and waits again only for a frame's entries beyond its first window.
+int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_match* out, double* R_out, double* t_out, float* residual,
+                      int64_t cap, int64_t* n_out, int64_t* counts, int64_t* stats4);
 
-// A batch of frames through one pose stage (lm_detect_batch, lm_peer_detect_batch).  pose_batch_reserve returns room for
-// n_frames scene depths of frame_pixels each (frame f at d_scene + f * frame_pixels) and max_surv survivors, which the
-// caller fills on the stream: frame f's survivors at [first[f], first[f + 1]).  It also uploads the renders and grows
-// every buffer pose_batch_run needs for max_surv survivors, so that the batch allocates no device memory once its frames run.
+// A batch's scene and survivor slots: room for n_frames scene depths of frame_pixels each (frame f at d_scene + f *
+// frame_pixels) and max_surv survivors, which the caller fills on the stream.  It also uploads the renders and grows
+// every buffer the run needs for max_surv survivors, so that the batch allocates no device memory once its frames run.
 int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
                        lm_match** d_surv);
-// Chunks of the pose stage of a batch with S survivors (each of at most 1024 slots).
+// Chunks of a run with S survivors.
 int pose_batch_chunks(int64_t S);
-struct PoseBatch {
-  PoseOptions o;              // shared: chunk c is pose exchange o.share->seq + c
-  int n_frames;
-  const int64_t* first;       // [n_frames + 1] survivor offsets (host)
-  const lm_match* surv;       // host copy of the survivors (pose_nms == 0 only)
-  const float* sK;            // [n_frames][9]
-  int pose_nms;               // 1: the pose NMS per frame (one CTA each), 0: the host composes the poses
-  double thr;
-};
-// The pose stage over every survivor of the batch in chunks of at most 1024 survivors, then (pose_nms) one pose NMS
-// launch for all frames; waits.  posed[f] / kept[f]: frame f's survivors with a pose, and its entries (kept poses, or
-// every survivor without the pose NMS).  stats4 (may be null): what lm_pose_stats returns for the batch.
-int pose_batch_run(lm_pose_stage* s, const PoseBatch& b, int64_t* launches, int64_t* posed, int64_t* kept, int64_t* stats4);
-// Frame f's kept[f] entries after pose_batch_run, outputs as lm_complete_detect (pose_nms) or lm_complete_pose.
-void pose_batch_frame(const lm_pose_stage* s, const PoseBatch& b, int f, lm_match* out, double* R_out, double* t_out, float* residual);
