@@ -36,7 +36,7 @@ SYMBOLS = [
     "lm_peer_export", "lm_peer_base", "lm_peer_connect", "lm_peer_connect_local", "lm_peer_disconnect", "lm_peer_share_pose",
     "lm_pose_stats", "lm_set_pose_estimation", "lm_set_template_depths", "lm_set_depth_gate", "lm_depth_gate_stats",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
-    "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture",
+    "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture", "lm_icp_process_batch_device",
 ]
 
 # The ICP's estimation step (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT of include/linemod_b200.h) by the name the
@@ -71,13 +71,13 @@ def is_tensor(a):
     return torch is not None and isinstance(a, torch.Tensor)
 
 
-def depth_scale_value(depth_scale):
+def depth_scale_value(depth_scale, name="depth_scale"):
     """depth_scale as a float, finite and > 0; TypeError / ValueError otherwise (no device work)."""
     if isinstance(depth_scale, (bool, np.bool_)) or not isinstance(depth_scale, (int, float, np.integer, np.floating)):
-        raise TypeError("depth_scale must be a number, got %s" % type(depth_scale).__name__)
+        raise TypeError("%s must be a number, got %s" % (name, type(depth_scale).__name__))
     s = float(depth_scale)
     if not (math.isfinite(s) and s > 0.0):
-        raise ValueError("depth_scale must be finite and > 0, got %r" % depth_scale)
+        raise ValueError("%s must be finite and > 0, got %r" % (name, depth_scale))
     return s
 
 
@@ -183,6 +183,77 @@ def host_frame_options(depth_scale, stream):
         raise TypeError("stream applies to frames given as CUDA tensors")
     if depth_scale_value(depth_scale) != 1.0:
         raise ValueError("depth_scale applies to float32 depth tensors; numpy depth is uint16 mm")
+
+
+def _depth_plane(t, name, torch):
+    """(data pointer, row pitch in bytes, format) of a uint16 (mm) or float32 [H, W] tensor packed within a row."""
+    if t.dtype not in (torch.uint16, torch.float32) or t.dim() != 2:
+        raise TypeError("%s must be a uint16 (mm) or float32 HxW depth tensor, got %s %s" % (name, t.dtype, tuple(t.shape)))
+    if t.stride(1) != 1:
+        raise ValueError("%s: depth must be packed within a row (stride(-1) == 1), got %s" % (name, t.stride()))
+    return t.data_ptr(), t.stride(0) * t.element_size(), DEPTH_F32 if t.dtype == torch.float32 else DEPTH_U16_MM
+
+
+def _plane_scale(f32, scale, name, what):
+    s = depth_scale_value(scale, name)
+    if not f32 and s != 1.0:
+        raise ValueError("%s applies to float32 %s; uint16 %s is in mm (%s=%r)" % (name, what, what, name, scale))
+    return s
+
+
+class DeviceDepths:
+    """A scene depth and its renders already on the GPU, checked for lm_icp_process_batch_device without any library call:
+    the scene a torch.uint16 (mm) or torch.float32 [H, W] tensor (scaled by depth_scale), the renders uint16 or float32
+    [h, w] tensors of one dtype and size (scaled by render_scale), given as a list or as one [n, h, w] tensor; every plane
+    packed within a row (stride(-1) == 1) with a free row pitch, every tensor CUDA on `device`.  The planes are read in
+    order on `stream` (device_stream).  n: the renders expected; host: the call's K, R and t by name (host_arrays)."""
+
+    def __init__(self, scene, renders, depth_scale, render_scale, stream, device, n=None, host=None):
+        import torch
+        if is_tensor(renders):
+            if renders.dim() != 3:
+                raise TypeError("renders given as one tensor must be [n, H, W], got %s" % (tuple(renders.shape),))
+            renders = list(renders.unbind(0))
+        renders = list(renders)
+        if not (is_tensor(scene) and all(is_tensor(r) for r in renders)):
+            raise TypeError("depths mix numpy arrays and torch tensors: pass the scene and every render as CUDA tensors or all as numpy arrays")
+        self.scene, self.scene_pitch, self.scene_format = _depth_plane(scene, "sceneDepth", torch)
+        self.depth_scale = _plane_scale(self.scene_format == DEPTH_F32, depth_scale, "depth_scale", "depth")
+        planes = [_depth_plane(r, "modelDepths[%d]" % i, torch) for i, r in enumerate(renders)]
+        if any(r.dtype != renders[0].dtype or r.shape != renders[0].shape for r in renders):
+            raise ValueError("every render must have one dtype and size, got %s" % sorted({(str(r.dtype), tuple(r.shape)) for r in renders}))
+        self.format = planes[0][2] if planes else DEPTH_U16_MM
+        self.render_scale = _plane_scale(self.format == DEPTH_F32, render_scale, "render_scale", "renders")
+        if n is not None and len(renders) != n:
+            raise TypeError("modelDepths: one render per match, got %d renders for %d matches" % (len(renders), n))
+        host_arrays(**(host or {}))
+        for name, t in [("sceneDepth", scene)] + [("modelDepths[%d]" % i, r) for i, r in enumerate(renders)]:
+            if not t.is_cuda or t.device.index != int(device):
+                raise ValueError("%s is on %s; the ICP runs on cuda:%d" % (name, t.device, int(device)))
+        self.srows, self.scols = int(scene.shape[0]), int(scene.shape[1])
+        self.mrows, self.mcols = (int(renders[0].shape[0]), int(renders[0].shape[1])) if renders else (1, 1)
+        self.n = len(renders)
+        self.renders, self.pitches = [p[0] for p in planes], [p[1] for p in planes]
+        self.tensors = [scene] + renders
+        self.stream = device_stream(stream, device)
+
+
+def depth_inputs(scene, renders, depth_scale, render_scale, stream, device, n=None, host=None):
+    """A DeviceDepths when the scene or any render is a tensor, None for numpy arrays (the host path, where depth_scale
+    and render_scale must stay 1.0 and stream None).  TypeError / ValueError before any library call."""
+    if not (is_tensor(scene) or is_tensor(renders) or any(is_tensor(r) for r in renders)):
+        host_frame_options(depth_scale, stream)
+        if depth_scale_value(render_scale, "render_scale") != 1.0:
+            raise ValueError("render_scale applies to float32 render tensors; numpy renders are uint16 mm")
+        return None
+    return DeviceDepths(scene, renders, depth_scale, render_scale, stream, device, n, host)
+
+
+def host_arrays(**arrays):
+    """K, R and t of the ICP stay host arrays whatever the depths are: TypeError for a tensor (no library call)."""
+    for name, a in arrays.items():
+        if is_tensor(a) or (isinstance(a, (list, tuple)) and any(is_tensor(x) for x in a)):
+            raise TypeError("%s must be a host (numpy) array, got a tensor" % name)
 
 
 def device_stream(stream, device):
@@ -302,6 +373,8 @@ def load():
     L.lm_icp_launch_count.restype = c_i64
     L.lm_icp_set_capture.argtypes = [vp, c_int]
     L.lm_icp_capture.argtypes = [vp, c_int, c_int, vp, c_i64]
+    L.lm_icp_process_batch_device.argtypes = [vp, c_int, vp, c_i64, c_int, c_f, c_int, c_int, ctypes.POINTER(vp), ctypes.POINTER(c_i64),
+                                              c_int, c_f, c_int, c_int, f32p, f32p, f32p, f32p, i32p, c_int, f64p, f64p, f32p, vp]
     for name in SYMBOLS:
         getattr(L, name)  # AttributeError if the library does not export a declared symbol
     _lib = L
@@ -915,6 +988,7 @@ class NativeIcp:
         h = ctypes.c_void_p()
         check(L.lm_icp_create(int(device), ctypes.byref(h)))
         self._h = h
+        self.device = int(device)
         self._estimation = "point_to_plane"  # the handle's estimation (lm_icp_set_estimation)
         self._captured = None               # the estimation of the last process_batch (capture())
 
@@ -959,6 +1033,32 @@ class NativeIcp:
                                            int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
                                            res.ctypes.data_as(f32p)))
         self._captured = self._estimation
+        return Ro, to, res
+
+    def process_batch_device(self, depths, sceneK, modelKs, Rs, ts, detect_xy, max_iterations=30, estimation=None):
+        """process_batch for a DeviceDepths (lm_icp_process_batch_device): the same outputs, bit for bit, as process_batch
+        on the u16 images the depths convert to; sceneK, modelKs, Rs, ts and detect_xy as there."""
+        if estimation is not None:
+            self.set_estimation(estimation)
+        n = depths.n
+        f32p, f64p, vp = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double), ctypes.c_void_p
+        sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+        mK = np.ascontiguousarray(modelKs, np.float32).reshape(n, 9)
+        R = np.ascontiguousarray(Rs, np.float32).reshape(n, 9)
+        t = np.ascontiguousarray(ts, np.float32).reshape(n, 3)
+        xy = np.ascontiguousarray(detect_xy, np.int32).reshape(n, 2)
+        Ro = np.full((n, 3, 3), np.nan, np.float64)
+        to = np.full((n, 3), np.nan, np.float64)
+        res = np.zeros(n, np.float32)
+        ptrs = (vp * max(n, 1))(*depths.renders)
+        pitches = (ctypes.c_int64 * max(n, 1))(*depths.pitches)
+        check(self._L.lm_icp_process_batch_device(self._h, n, depths.scene, depths.scene_pitch, depths.scene_format,
+                                                  ctypes.c_float(depths.depth_scale), depths.srows, depths.scols, ptrs, pitches,
+                                                  depths.format, ctypes.c_float(depths.render_scale), depths.mrows, depths.mcols,
+                                                  sK.ctypes.data_as(f32p), mK.ctypes.data_as(f32p), R.ctypes.data_as(f32p),
+                                                  t.ctypes.data_as(f32p), xy.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                                  int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
+                                                  res.ctypes.data_as(f32p), depths.stream.cuda_stream))
         return Ro, to, res
 
     def set_use_scene_cloud(self, on):

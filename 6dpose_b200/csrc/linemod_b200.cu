@@ -1214,8 +1214,8 @@ struct DeviceFrame {
   const uint8_t* mask[2]; int64_t mask_pitch;
 };
 
-// One plane of a device frame: present, on the handle's device, rows at least `row` bytes apart, element-aligned.
-static int check_device_plane(const lm_detector* d, const char* what, const void* p, int64_t pitch, int64_t row, int elem) {
+// One plane of a device frame: present, on `device`, rows at least `row` bytes apart, element-aligned (lm_pose.h).
+int check_device_plane(int device, const char* what, const void* p, int64_t pitch, int64_t row, int elem) {
   if (!p) return fail(LM_E_INVALID, "%s is null", what);
   if (pitch < row) return fail(LM_E_INVALID, "%s: row pitch %lld bytes is shorter than a row (%lld bytes)", what, (long long)pitch, (long long)row);
   if ((uintptr_t)p % elem || pitch % elem)
@@ -1225,32 +1225,39 @@ static int check_device_plane(const lm_detector* d, const char* what, const void
     cudaGetLastError();  // clear the query's error: nothing was enqueued
     return fail(LM_E_INVALID, "%s: %p is not a CUDA pointer", what, p);
   }
-  if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != d->device)
-    return fail(LM_E_INVALID, "%s: %p is not device or managed memory of device %d (%s, device %d)", what, p, d->device,
+  if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != device)
+    return fail(LM_E_INVALID, "%s: %p is not device or managed memory of device %d (%s, device %d)", what, p, device,
                 a.type == cudaMemoryTypeHost ? "host memory" : a.type == cudaMemoryTypeUnregistered ? "unregistered host memory" : "device memory",
                 a.device);
   return LM_OK;
 }
 
 // Every check of lm_bind_images_device, none of which touches the device.
-static int check_device_frame(lm_detector* d, const DeviceFrame& f, int rows, int cols, cudaStream_t stream, int* lrows, int* lcols) {
+// A caller's stream: a CUDA stream of `device` (lm_pose.h).
+int check_device_stream(int device, cudaStream_t stream) {
   int sdev = -1;
   if (cudaStreamGetDevice(stream, &sdev) != cudaSuccess) {
     cudaGetLastError();  // clear the query's error: nothing was enqueued
     return fail(LM_E_INVALID, "stream %p is not a CUDA stream", (void*)stream);
   }
-  if (sdev != d->device) return fail(LM_E_INVALID, "stream %p belongs to device %d, the handle to device %d", (void*)stream, sdev, d->device);
+  if (sdev != device) return fail(LM_E_INVALID, "stream %p belongs to device %d, the handle to device %d", (void*)stream, sdev, device);
+  return LM_OK;
+}
+
+static int check_device_frame(lm_detector* d, const DeviceFrame& f, int rows, int cols, cudaStream_t stream, int* lrows, int* lcols) {
+  int rc = check_device_stream(d->device, stream);
+  if (rc) return rc;
   if (f.format != LM_DEPTH_U16_MM && f.format != LM_DEPTH_F32)
     return fail(LM_E_INVALID, "unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", f.format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
   if (f.format == LM_DEPTH_F32 && !(std::isfinite(f.scale) && f.scale > 0.f))
     return fail(LM_E_INVALID, "depth_scale %g: float depth needs a finite scale > 0", (double)f.scale);
-  int rc = fe_dims(d, rows, cols, lrows, lcols);
+  rc = fe_dims(d, rows, cols, lrows, lcols);
   if (rc) return rc;
   const int esize = f.format == LM_DEPTH_F32 ? 4 : 2;
-  rc = check_device_plane(d, "rgb", f.rgb, f.rgb_pitch, 3ll * cols, 1);
-  if (!rc) rc = check_device_plane(d, "depth", f.depth, f.depth_pitch, (int64_t)esize * cols, esize);
+  rc = check_device_plane(d->device, "rgb", f.rgb, f.rgb_pitch, 3ll * cols, 1);
+  if (!rc) rc = check_device_plane(d->device, "depth", f.depth, f.depth_pitch, (int64_t)esize * cols, esize);
   for (int m = 0; m < 2 && !rc; ++m)
-    if (f.mask[m]) rc = check_device_plane(d, m ? "mask_depth" : "mask_color", f.mask[m], f.mask_pitch, cols, 1);
+    if (f.mask[m]) rc = check_device_plane(d->device, m ? "mask_depth" : "mask_color", f.mask[m], f.mask_pitch, cols, 1);
   return rc;
 }
 

@@ -26,6 +26,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "lm_depth.cuh"
+
 __device__ __forceinline__ void lm_pdl_wait();
 
 // ---- colour: blur + sobel + channel pick + phase bin -----------------------------------------------
@@ -258,18 +260,10 @@ __global__ void __launch_bounds__(256) k_fe_median(const uint8_t* __restrict__ i
 }
 
 // ---- ingest of a borrowed device frame (lm_bind_images_device) --------------------------------------
-// Float depth to u16 mm as the reference's driver converts it on the host (depth *= depth_scale;
-// depth.astype(np.uint16), linemod_and_levelup_test.py:315-317): one float32 product, truncated.  Products outside
-// [0, 65536) -- NaN, negatives, infinities, >= 65536 -- are 0 (no depth), where numpy's cast is platform-defined.
-__device__ __forceinline__ uint16_t fe_depth_mm(float d, float scale) {
-  const float v = __fmul_rn(d, scale);
-  return (v >= 0.f && v < 65536.f) ? (uint16_t)__float2uint_rz(v) : (uint16_t)0;
-}
-
 #define FE_INGEST_PX 256  // pixels of one row per CTA
 
 // Copies rows x cols pixels of pitched planes (pixels packed within a row) into the front-end's packed buffers: rgb
-// bytes, depth (u16 copied, f32 converted by fe_depth_mm) and the masks given.  CTA (bx, y) takes pixels
+// bytes, depth (u16 copied, f32 converted by lm_depth_mm, lm_depth.cuh) and the masks given.  CTA (bx, y) takes pixels
 // [bx * FE_INGEST_PX, +FE_INGEST_PX) of row y; consecutive threads read consecutive addresses of every plane's row.
 __global__ void __launch_bounds__(FE_INGEST_PX) k_fe_ingest(const uint8_t* __restrict__ rgb, int64_t rgb_pitch, const void* __restrict__ depth,
                                                           int64_t depth_pitch, int depth_f32, float scale, const uint8_t* __restrict__ mask0,
@@ -285,7 +279,7 @@ __global__ void __launch_bounds__(FE_INGEST_PX) k_fe_ingest(const uint8_t* __res
   const int x = x0 + threadIdx.x;
   const size_t o = (size_t)y * W + x;
   const uint8_t* drow = (const uint8_t*)depth + y * depth_pitch;
-  depth_out[o] = depth_f32 ? fe_depth_mm(((const float*)drow)[x], scale) : ((const uint16_t*)drow)[x];
+  depth_out[o] = lm_depth_at(drow, x, depth_f32, scale);
   if (mask0) mask_out0[o] = mask0[y * mask_pitch + x];
   if (mask1) mask_out1[o] = mask1[y * mask_pitch + x];
 }

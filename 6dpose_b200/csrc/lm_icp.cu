@@ -21,11 +21,14 @@
 // survivors: k_pose_cloud + a CUB segmented sort + k_pose_voxel build the same clouds and initial guesses, bit for
 // bit, and feed the same ICP kernels; k_pose_nms may follow.  A frame, a batch chunk and their shared forms are all
 // one chunk to pose_chunk and to the kernels, told apart by data only: the survivor count on the device, an optional
-// frame table, and the slot rule survivor = rank + slot * world.
+// frame table, and the slot rule survivor = rank + slot * world.  lm_icp_process_batch_device feeds the same chunks from
+// renders and a scene in the caller's device memory: k_icp_scene, k_icp_render_box and k_icp_render_crop build the
+// per-hypothesis table k_pose_cloud reads (end of this file).
 
 #include "linemod_b200.h"
 #include "lm_pose.h"
 #include "lm_buffer.h"
+#include "lm_depth.cuh"
 
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
@@ -658,6 +661,9 @@ __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShare
 // --------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------
+struct IcpDevice;                    // lm_icp_process_batch_device's buffers (end of this file)
+static void icp_device_free(IcpDevice* d);
+
 struct lm_icp {
   int device = 0;
   Stream stream;  // streams and events first: they outlive the buffers
@@ -682,6 +688,7 @@ struct lm_icp {
     std::vector<double> pts, nrm;
     std::vector<int32_t> knn, corr;
   } cap;
+  IcpDevice* dev = nullptr;  // created by the first lm_icp_process_batch_device
 };
 
 extern "C" int lm_icp_create(int device, lm_icp** out) {
@@ -705,6 +712,7 @@ extern "C" void lm_icp_destroy(lm_icp* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaStreamSynchronize(h->stream.get());
+  icp_device_free(h->dev);
   delete h;
 }
 
@@ -747,20 +755,28 @@ void compose(const double* T, const float* base, double* R_out, double* t_out) {
   }
 }
 
-// dilate(modelDepth > 0, 9x9) + boundingRect (LL.cpp:43-50): the box of the non-zero pixels grown by 4, clipped to the
-// image; an all-zero image gives the empty box
-void model_box(const uint16_t* model, int mrows, int mcols, int* box) {
+}  // namespace
+
+// dilate(modelDepth > 0, 9x9) + boundingRect (LL.cpp:43-50) from the extent [x0, x1] x [y0, y1] of the non-zero pixels
+// (x1 < 0: none): that extent grown by 4, clipped to the image, as (x, y, w, h); no pixel gives the empty box
+__host__ __device__ __forceinline__ void grow_box(int x0, int y0, int x1, int y1, int mrows, int mcols, int* box) {
   const int half = 4;
+  box[0] = box[1] = box[2] = box[3] = 0;
+  if (x1 >= 0) {
+    box[0] = max(x0 - half, 0); box[1] = max(y0 - half, 0);
+    box[2] = min(x1 + half, mcols - 1) - box[0] + 1;
+    box[3] = min(y1 + half, mrows - 1) - box[1] + 1;
+  }
+}
+
+namespace {
+
+void model_box(const uint16_t* model, int mrows, int mcols, int* box) {
   int x0 = mcols, x1 = -1, y0 = mrows, y1 = -1;
   for (int r = 0; r < mrows; ++r)
     for (int q = 0; q < mcols; ++q)
       if (model[(size_t)r * mcols + q] > 0) { x0 = std::min(x0, q); x1 = std::max(x1, q); y0 = std::min(y0, r); y1 = std::max(y1, r); }
-  box[0] = box[1] = box[2] = box[3] = 0;
-  if (x1 >= 0) {
-    box[0] = std::max(x0 - half, 0); box[1] = std::max(y0 - half, 0);
-    box[2] = std::min(x1 + half, mcols - 1) - box[0] + 1;
-    box[3] = std::min(y1 + half, mrows - 1) - box[1] + 1;
-  }
+  grow_box(x0, y0, x1, y1, mrows, mcols, box);
 }
 
 void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* model, int mrows, int mcols, const float* sK,
@@ -1672,7 +1688,17 @@ static PoseShareDev share_dev(const PoseShare& sh, int32_t seq, const int32_t* c
 // null: depth scene, intrinsics sK) or of the frames frame_of gives.  The launches are sized for `slots` survivors.
 // Their results go to outs / posed; status: [0] cloud overflow, shared [1] a peer's poses did not arrive, [2] entries
 // this rank published.  seq: the chunk's pose exchange (shared).
+// The renders a chunk's survivors use: survivor m takes entry class_begin[m.class_index] + m.template_id of tpl (n_tpl
+// entries), whose crop lies in crops.
+struct PoseTable {
+  const PoseTpl* tpl;
+  const uint16_t* crops;
+  const int32_t* class_begin;
+  int32_t n_classes, n_tpl;
+};
+
 struct PoseChunk {
+  PoseTable table;
   const lm_match* surv;
   const int32_t* counts;
   int slots;
@@ -1698,8 +1724,8 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   const int64_t A = pose_area(s);  // slot stride: the buffers' area, which may exceed the current largest crop
   PoseParams p;
   p.surv = c.surv; p.counts = c.counts;
-  p.class_begin = s->d_class_begin.get(); p.n_classes = (int32_t)s->class_begin.size() - 1; p.n_tpl = (int32_t)s->tpl.size();
-  p.tpl = s->d_tpl.get(); p.crops = s->d_crops.get();
+  p.class_begin = c.table.class_begin; p.n_classes = c.table.n_classes; p.n_tpl = c.table.n_tpl;
+  p.tpl = c.table.tpl; p.crops = c.table.crops;
   p.scene = c.scene; p.srows = o.srows; p.scols = o.scols;
   if (c.sK) memcpy(p.sK, c.sK, sizeof(p.sK));
   else memset(p.sK, 0, sizeof(p.sK));
@@ -1831,6 +1857,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_CHUNK;
     PoseChunk k;
+    k.table = {s->d_tpl.get(), s->d_crops.get(), s->d_class_begin.get(), (int32_t)s->class_begin.size() - 1, (int32_t)s->tpl.size()};
     k.surv = run.d_surv + c0;
     k.counts = batch ? s->d_bstat.get() + 4 * c + 3 : run.d_counts;
     k.slots = batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound;
@@ -2037,5 +2064,253 @@ extern "C" int lm_nms_translations(int device, int64_t n, const double* t, const
   CUI(cudaMemcpy(&got, d_n, sizeof(int32_t), cudaMemcpyDeviceToHost));
   if (got > 0) CUI(cudaMemcpy(keep, d_keep, sizeof(int32_t) * got, cudaMemcpyDeviceToHost));
   *n_keep = got;
+  return LM_OK;
+}
+
+// --------------------------------------------------------------------------------------------
+// lm_icp_process_batch_device: the pose stage's chunks fed from the caller's device planes (lm_pose.h)
+// --------------------------------------------------------------------------------------------
+#define ICP_DEV_PX 256       // threads of the scene and render kernels
+#define RENDER_BOX_ROWS 16   // render rows per CTA of k_icp_render_box
+#define RENDER_CROP_ROWS 8   // crop rows per CTA of k_icp_render_crop
+
+struct RenderSrc {  // one render: the caller's plane, rows pitch bytes apart
+  const uint8_t* p;
+  int64_t pitch;
+};
+
+// The scene plane into the packed srows x scols u16 mm buffer k_pose_cloud reads.  CTA (bx, y): pixels
+// [bx * ICP_DEV_PX, +ICP_DEV_PX) of row y.
+__global__ void __launch_bounds__(ICP_DEV_PX) k_icp_scene(const uint8_t* __restrict__ src, int64_t pitch, int f32, float scale, int cols,
+                                                         uint16_t* __restrict__ out) {
+  const int y = blockIdx.y, x = blockIdx.x * ICP_DEV_PX + threadIdx.x;
+  if (x < cols) out[(size_t)y * cols + x] = lm_depth_at(src + y * pitch, x, f32, scale);
+}
+
+// The extent of render blockIdx.x's non-zero pixels (after conversion) over its rows [blockIdx.y * RENDER_BOX_ROWS,
+// +RENDER_BOX_ROWS), merged into ext[4i ..]: min x, min y (unsigned, atomicMin), max x, max y (int, atomicMax), all bytes
+// 0xFF before the launch (no pixel).  Exact in any order.
+__global__ void __launch_bounds__(ICP_DEV_PX) k_icp_render_box(const RenderSrc* __restrict__ src, int f32, float scale, int mrows, int mcols,
+                                                              uint32_t* __restrict__ ext) {
+  const RenderSrc s = src[blockIdx.x];
+  const int r0 = blockIdx.y * RENDER_BOX_ROWS, r1 = min(r0 + RENDER_BOX_ROWS, mrows);
+  unsigned x0 = 0xFFFFFFFFu, y0 = 0xFFFFFFFFu;
+  int x1 = -1, y1 = -1;
+  for (int r = r0; r < r1; ++r) {
+    const uint8_t* row = s.p + r * s.pitch;
+    for (int q = threadIdx.x; q < mcols; q += ICP_DEV_PX)
+      if (lm_depth_at(row, q, f32, scale) > 0) {
+        x0 = min(x0, (unsigned)q); x1 = max(x1, q);
+        y0 = min(y0, (unsigned)r); y1 = max(y1, r);
+      }
+  }
+  x0 = __reduce_min_sync(0xffffffffu, x0); y0 = __reduce_min_sync(0xffffffffu, y0);
+  x1 = __reduce_max_sync(0xffffffffu, x1); y1 = __reduce_max_sync(0xffffffffu, y1);
+  if ((threadIdx.x & 31) == 0 && x1 >= 0) {
+    uint32_t* e = ext + 4 * (size_t)blockIdx.x;
+    atomicMin(e, x0); atomicMin(e + 1, y0);
+    atomicMax(reinterpret_cast<int*>(e) + 2, x1); atomicMax(reinterpret_cast<int*>(e) + 3, y1);
+  }
+}
+
+// Entry i = blockIdx.x of the call's table -- model_box's box grown from ext, the anchor render[mrows / 2][mcols / 2]
+// and K -- and its crop rows [blockIdx.y * RENDER_CROP_ROWS, +RENDER_CROP_ROWS), packed at crops + i * stride.  A crop
+// larger than stride is not written: the host sized stride for every hypothesis with a pose, so k_pose_cloud never reads it.
+__global__ void __launch_bounds__(ICP_DEV_PX) k_icp_render_crop(const RenderSrc* __restrict__ src, int f32, float scale, int mrows, int mcols,
+                                                               const uint32_t* __restrict__ ext, const float* __restrict__ K, int64_t stride,
+                                                               PoseTpl* __restrict__ tpl, uint16_t* __restrict__ crops) {
+  const int i = blockIdx.x;
+  const RenderSrc s = src[i];
+  const uint32_t* e = ext + 4 * (size_t)i;
+  int box[4];
+  grow_box((int)e[0], (int)e[1], (int)e[2], (int)e[3], mrows, mcols, box);
+  if (blockIdx.y == 0 && threadIdx.x == 0) {
+    PoseTpl t;
+    t.bx = box[0]; t.by = box[1]; t.bw = box[2]; t.bh = box[3];
+    t.crop = (int64_t)i * stride;
+    for (int k = 0; k < 9; ++k) t.K[k] = K[9 * i + k];
+    t.anchor = lm_depth_at(s.p + (mrows / 2) * s.pitch, mcols / 2, f32, scale);
+    tpl[i] = t;
+  }
+  const int bw = box[2], r1 = min((int)(blockIdx.y + 1) * RENDER_CROP_ROWS, box[3]);
+  if ((int64_t)bw * box[3] > stride) return;
+  uint16_t* __restrict__ C = crops + (size_t)i * stride;
+  for (int r = blockIdx.y * RENDER_CROP_ROWS; r < r1; ++r) {
+    const uint8_t* row = s.p + (box[1] + r) * s.pitch;
+    for (int q = threadIdx.x; q < bw; q += ICP_DEV_PX) C[(size_t)r * bw + q] = lm_depth_at(row, box[0] + q, f32, scale);
+  }
+}
+
+struct IcpDevice {
+  lm_pose_stage stage;  // the chunks' cloud buffers (pose_buffers); no registered render
+  Event ev_in, ev_out;  // the caller's stream -> the reads -> the caller's stream
+  DeviceArray<uint8_t> in;  // the call's inputs in one copy: renders, K, survivors, chunk sizes, class_begin
+  DeviceArray<uint16_t> scene, crops;
+  DeviceArray<uint32_t> ext; PinnedArray<uint32_t> h_ext;  // [n][4] extents (k_icp_render_box)
+  DeviceArray<PoseTpl> tpl;
+  DeviceArray<IcpOut> outs; DeviceArray<uint8_t> posed; PinnedArray<IcpOut> h_outs;
+  DeviceArray<int32_t> status; PinnedArray<int32_t> h_status;  // 4 per chunk (PoseChunk); the host's copy then holds the
+                                                               // source count of the last hypothesis with a pose
+};
+
+static void icp_device_free(IcpDevice* d) { delete d; }
+
+// A device depth plane's format and scale.
+static int check_depth_format(const char* what, int format, float scale) {
+  if (format != LM_DEPTH_U16_MM && format != LM_DEPTH_F32)
+    return lm_fail(LM_E_INVALID, "%s: unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", what, format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
+  if (format == LM_DEPTH_F32 && !(std::isfinite(scale) && scale > 0.f))
+    return lm_fail(LM_E_INVALID, "%s: scale %g: float depth needs a finite scale > 0", what, (double)scale);
+  return LM_OK;
+}
+
+static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, int64_t scene_pitch, int scene_format,
+                                           float scene_scale, int srows, int scols, const void* const* model_depths,
+                                           const int64_t* model_pitches, int model_format, float model_scale, int mrows, int mcols,
+                                           const float* sceneK, const float* modelK, const float* R, const float* t,
+                                           const int32_t* detect_xy, int max_iterations, double* R_out, double* t_out, float* residual,
+                                           void* stream) {
+  if (!h || n_hyp < 0 || !scene_depth || !model_depths || !model_pitches || !sceneK || !modelK || !R || !t || !detect_xy || !R_out ||
+      !t_out || !residual)
+    return lm_fail(LM_E_INVALID, "null argument");
+  if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
+  if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
+  if (h->capture) return lm_fail(LM_E_STATE, "capture is on: it records lm_icp_process_batch's host-built clouds only");
+  int rc = check_depth_format("scene_depth", scene_format, scene_scale);
+  if (!rc) rc = check_depth_format("model_depths", model_format, model_scale);
+  if (rc) return rc;
+  cudaStream_t caller = (cudaStream_t)stream;
+  rc = check_device_stream(h->device, caller);
+  const int sz = scene_format == LM_DEPTH_F32 ? 4 : 2, mz = model_format == LM_DEPTH_F32 ? 4 : 2;
+  if (!rc) rc = check_device_plane(h->device, "scene_depth", scene_depth, scene_pitch, (int64_t)sz * scols, sz);
+  for (int i = 0; i < n_hyp && !rc; ++i) {
+    char what[40];
+    snprintf(what, sizeof(what), "model_depths[%d]", i);
+    rc = check_device_plane(h->device, what, model_depths[i], model_pitches[i], (int64_t)mz * mcols, mz);
+  }
+  if (rc) return rc;
+  if (n_hyp == 0) return LM_OK;
+  CUI(cudaSetDevice(h->device));
+  if (!h->dev) h->dev = new IcpDevice();
+  IcpDevice& d = *h->dev;
+  if (!d.ev_in.get()) CUI(d.ev_in.create(cudaEventDisableTiming));
+  if (!d.ev_out.get()) CUI(d.ev_out.create(cudaEventDisableTiming));
+  const int n = n_hyp, nc = pose_batch_chunks(n);
+  // the inputs: survivor i is hypothesis i (class 0, template i) at detect_xy[i]; chunk c holds min(n - 1024 c, 1024)
+  const size_t o_K = align16(sizeof(RenderSrc) * n), o_surv = align16(o_K + sizeof(float) * 9 * n);
+  const size_t o_cnt = align16(o_surv + sizeof(lm_match) * n), o_cb = align16(o_cnt + sizeof(int32_t) * nc);
+  std::vector<uint8_t> in(o_cb + 2 * sizeof(int32_t));
+  RenderSrc* src = reinterpret_cast<RenderSrc*>(in.data());
+  lm_match* surv = reinterpret_cast<lm_match*>(in.data() + o_surv);
+  int32_t* cnt = reinterpret_cast<int32_t*>(in.data() + o_cnt);
+  for (int i = 0; i < n; ++i) {
+    src[i] = {static_cast<const uint8_t*>(model_depths[i]), model_pitches[i]};
+    surv[i] = {detect_xy[2 * i], detect_xy[2 * i + 1], 0.f, 0, i};
+  }
+  memcpy(in.data() + o_K, modelK, sizeof(float) * 9 * n);
+  for (int c = 0; c < nc; ++c) cnt[c] = std::min(n - c * POSE_CHUNK, POSE_CHUNK);
+  const int32_t class_begin[2] = {0, n};
+  memcpy(in.data() + o_cb, class_begin, sizeof(class_begin));
+  // grow-only: a call of the same shape allocates nothing (the handle's stream is idle between calls)
+  CUI(d.in.reserve(in.size()));
+  CUI(d.scene.reserve((size_t)srows * scols));
+  CUI(d.ext.reserve(4 * (size_t)n)); CUI(d.h_ext.reserve(4 * (size_t)n));
+  CUI(d.tpl.reserve(n));
+  CUI(d.outs.reserve(n)); CUI(d.posed.reserve(n)); CUI(d.h_outs.reserve(n));
+  CUI(d.status.reserve(4 * (size_t)nc)); CUI(d.h_status.reserve(4 * (size_t)nc + 1));
+  const RenderSrc* d_src = reinterpret_cast<const RenderSrc*>(d.in.get());
+  const float* d_K = reinterpret_cast<const float*>(d.in.get() + o_K);
+  const int f32 = model_format == LM_DEPTH_F32 ? 1 : 0;
+  // the reads of the caller's planes start behind its stream's work
+  cudaStream_t st = h->stream.get();
+  CUI(cudaEventRecord(d.ev_in.get(), caller));
+  CUI(cudaStreamWaitEvent(st, d.ev_in.get(), 0));
+  CUI(cudaEventRecord(h->ev0.get(), st));
+  CUI(cudaMemcpyAsync(d.in.get(), in.data(), in.size(), cudaMemcpyHostToDevice, st));
+  CUI(cudaMemsetAsync(d.ext.get(), 0xFF, sizeof(uint32_t) * 4 * n, st));
+  k_icp_scene<<<dim3((unsigned)((scols + ICP_DEV_PX - 1) / ICP_DEV_PX), (unsigned)srows), ICP_DEV_PX, 0, st>>>(
+      static_cast<const uint8_t*>(scene_depth), scene_pitch, scene_format == LM_DEPTH_F32 ? 1 : 0, scene_scale, scols, d.scene.get());
+  k_icp_render_box<<<dim3((unsigned)n, (unsigned)((mrows + RENDER_BOX_ROWS - 1) / RENDER_BOX_ROWS)), ICP_DEV_PX, 0, st>>>(
+      d_src, f32, model_scale, mrows, mcols, d.ext.get());
+  CUI(cudaGetLastError());
+  h->launches += 2;
+  // the one read-back: the boxes size the crops and the clouds' slots
+  CUI(cudaMemcpyAsync(d.h_ext.get(), d.ext.get(), sizeof(uint32_t) * 4 * n, cudaMemcpyDeviceToHost, st));
+  CUI(cudaStreamSynchronize(st));
+  std::vector<uint8_t> posed((size_t)n);
+  int64_t stride = 1;
+  int max_bh = 1, last = -1;
+  for (int i = 0; i < n; ++i) {
+    const uint32_t* e = d.h_ext.get() + 4 * (size_t)i;
+    int b[4];
+    grow_box((int)e[0], (int)e[1], (int)e[2], (int)e[3], mrows, mcols, b);
+    if ((int64_t)b[2] * b[3] >= (1ll << POSE_KEY_BITS))
+      return lm_fail(LM_E_INVALID, "model_depths[%d]: box of %d x %d pixels is too large", i, b[2], b[3]);
+    posed[(size_t)i] = !(detect_xy[2 * i] + b[2] >= scols || detect_xy[2 * i + 1] + b[3] >= srows);  // LL.cpp:52-55
+    if (!posed[(size_t)i]) continue;
+    stride = std::max<int64_t>(stride, (int64_t)b[2] * b[3]);
+    max_bh = std::max(max_bh, b[3]);
+    last = i;
+  }
+  if (last >= 0) {
+    CUI(d.crops.reserve((size_t)n * stride));
+    rc = pose_buffers(&d.stage, st, std::min(n, POSE_CHUNK), stride);
+    if (rc) return rc;
+    k_icp_render_crop<<<dim3((unsigned)n, (unsigned)((max_bh + RENDER_CROP_ROWS - 1) / RENDER_CROP_ROWS)), ICP_DEV_PX, 0, st>>>(
+        d_src, f32, model_scale, mrows, mcols, d.ext.get(), d_K, stride, d.tpl.get(), d.crops.get());
+    CUI(cudaGetLastError());
+    ++h->launches;
+  }
+  // the crops were the last reads of the caller's planes
+  CUI(cudaEventRecord(d.ev_out.get(), st));
+  CUI(cudaStreamWaitEvent(caller, d.ev_out.get(), 0));
+  if (last < 0) {  // every hypothesis takes the early return: no cloud to build
+    for (int i = 0; i < n; ++i) residual[i] = -1.f;
+    return LM_OK;
+  }
+  CUI(cudaMemsetAsync(d.status.get(), 0, sizeof(int32_t) * 4 * nc, st));
+  PoseOptions o;
+  o.srows = srows; o.scols = scols; o.use_scene_cloud = h->use_scene_cloud ? 1 : 0; o.max_iterations = max_iterations;
+  o.estimation = h->estimation; o.stream = st; o.share = nullptr;
+  const PoseTable table = {d.tpl.get(), d.crops.get(), reinterpret_cast<const int32_t*>(d.in.get() + o_cb), 1, n};
+  const lm_match* d_surv = reinterpret_cast<const lm_match*>(d.in.get() + o_surv);
+  const int32_t* d_cnt = reinterpret_cast<const int32_t*>(d.in.get() + o_cnt);
+  for (int c = 0; c < nc; ++c) {
+    const int c0 = c * POSE_CHUNK;
+    PoseChunk k;
+    k.table = table;
+    k.surv = d_surv + c0; k.counts = d_cnt + c; k.slots = cnt[c];
+    k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK;
+    k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.status = d.status.get() + 4 * c; k.seq = 0;
+    const int l = pose_chunk(&d.stage, o, k);
+    if (l < 0) return l;
+    h->launches += l;
+    if (last >= c0 && last < c0 + cnt[c])  // the chunk's jobs are overwritten by the next chunk's
+      CUI(cudaMemcpyAsync(d.h_status.get() + 4 * nc, &d.stage.d_jobs.get()[last - c0].src_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  }
+  CUI(cudaEventRecord(h->ev1.get(), st));
+  CUI(cudaMemcpyAsync(d.h_outs.get(), d.outs.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(d.h_status.get(), d.status.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  CUI(cudaStreamSynchronize(st));
+  CUI(cudaGetLastError());
+  float ms = 0;
+  CUI(cudaEventElapsedTime(&ms, h->ev0.get(), h->ev1.get()));
+  h->last_kernel_us = ms * 1000.f;
+  for (int c = 0; c < nc; ++c)
+    if (d.h_status[4 * (size_t)c])
+      return lm_fail(LM_E_INVALID, "a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  for (int i = 0; i < n; ++i) {
+    if (!posed[(size_t)i]) { residual[i] = -1.f; continue; }
+    const IcpOut& q = d.h_outs[(size_t)i];
+    float base[16];
+    init_base(R + 9 * i, t + 3 * i, base);
+    compose(q.T, base, R_out + 9 * i, t_out + 3 * i);
+    residual[i] = (float)q.fitness;
+  }
+  h->last_points = d.h_status[4 * (size_t)nc];
+  h->last_iterations = d.h_outs[(size_t)last].iterations;
+  h->last_rmse = d.h_outs[(size_t)last].rmse;
   return LM_OK;
 }

@@ -94,3 +94,18 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
                        lm_match** d_surv);
 // Chunks of a run with S survivors.
 int pose_batch_chunks(int64_t S);
+
+// lm_icp_process_batch_device feeds the same chunks (pose_chunk in lm_icp.cu) from renders it is handed per call instead
+// of registered ones.  Its table has one entry per hypothesis, written on the device: k_icp_render_box reduces every
+// render's non-zero extent, the host reads the extents back once (n x 16 bytes, one synchronise of the handle's stream),
+// then k_icp_render_crop writes each entry (model_box's box, the anchor, K) and its crop.  The read-back sizes what the
+// host cannot know before: the crop pool (n x the largest crop a posed hypothesis has) and the clouds' slot stride of the
+// chunk buffers (that largest crop).  Sizing for whole renders instead (n x mrows x mcols) would cost a full-frame render
+// ~2 x 300 000 points of cloud slots per hypothesis, far more device memory than any crop needs.  Survivor i of the
+// call is hypothesis i: class 0, template i, at (x_i, y_i).
+
+// Checks of a caller's device plane and stream (linemod_b200.cu), none of which touches the device: LM_E_INVALID unless
+// p is device or managed memory of `device`, rows are at least `row` bytes apart and p and pitch are multiples of elem;
+// unless stream is a CUDA stream of `device`.
+int check_device_plane(int device, const char* what, const void* p, int64_t pitch, int64_t row, int elem);
+int check_device_stream(int device, cudaStream_t stream);

@@ -2,7 +2,11 @@
 linemodLevelup/pybind11.cpp:9-14).  process() runs the ICP on the GPU through the C-ABI
 (lm_icp_process); getR/getT/getResidual keep the reference's conventions: None before the first
 successful call (an empty cv::Mat converts to None), residual = ICP fitness, -1 initially and after
-the early return of LL.cpp:52-55."""
+the early return of LL.cpp:52-55.
+
+process() and refine_matches() also take depths already in device memory: the scene and the renders as CUDA tensors
+(uint16 mm, or float32 scaled by depth_scale / render_scale), read in order on `stream` (lm_icp_process_batch_device).
+The results are bit for bit those of the same call on the converted uint16 numpy images."""
 import numpy as np
 
 from . import _lib
@@ -47,17 +51,28 @@ class poseRefine:
             raise TypeError("%s must be a uint16 HxW depth image (mm)" % name)
         return a
 
-    def process(self, sceneDepth, modelDepth, sceneK, modelK, modelR, modelT, detectX, detectY):
-        scene = np.asarray(sceneDepth)
-        model = np.asarray(modelDepth)
-        if scene.dtype != np.uint16 or scene.ndim != 2 or model.dtype != np.uint16 or model.ndim != 2:
-            raise TypeError("sceneDepth / modelDepth must be uint16 HxW depth images (mm)")
+    def process(self, sceneDepth, modelDepth, sceneK, modelK, modelR, modelT, detectX, detectY, depth_scale=1.0, render_scale=1.0,
+                stream=None):
+        """sceneDepth / modelDepth: uint16 HxW numpy images (mm), or CUDA tensors on this object's device: uint16 (mm) or
+        float32 [H, W], pixels packed within a row.  depth_scale / render_scale convert float32 depth to mm (the driver's
+        depth_ren.astype(np.uint16) is render_scale 1.0); stream: the torch stream the tensors are ordered on (None: the
+        current stream)."""
+        dev = _lib.depth_inputs(sceneDepth, [modelDepth], depth_scale, render_scale, stream, self.device,
+                                host=dict(sceneK=sceneK, modelK=modelK, modelR=modelR, modelT=modelT))
+        if dev is None:
+            scene = np.asarray(sceneDepth)
+            model = np.asarray(modelDepth)
+            if scene.dtype != np.uint16 or scene.ndim != 2 or model.dtype != np.uint16 or model.ndim != 2:
+                raise TypeError("sceneDepth / modelDepth must be uint16 HxW depth images (mm)")
         sK = self._mat(sceneK, np.float32, (3, 3), "sceneK")
         mK = self._mat(modelK, np.float32, (3, 3), "modelK")
         R = self._mat(modelR, np.float32, (3, 3), "modelR")
         t = self._mat(modelT, np.float32, (3,), "modelT")
-        Ro, to, res = _native(self.device).process_batch(scene, [model], sK, mK[None], R[None], t[None],
-                                                         [[int(detectX), int(detectY)]], self.max_iterations, self.estimation)
+        args = (sK, mK[None], R[None], t[None], [[int(detectX), int(detectY)]], self.max_iterations, self.estimation)
+        if dev is None:
+            Ro, to, res = _native(self.device).process_batch(scene, [model], *args)
+        else:
+            Ro, to, res = _native(self.device).process_batch_device(dev, *args)
         self._residual = float(res[0])
         if res[0] == -1.0:  # early return: R_refined / t_refiend keep their previous value (LL.cpp:52-55)
             return
@@ -74,29 +89,39 @@ class poseRefine:
         return self._t
 
 
-def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, modelTs, device=None, estimation="point_to_plane"):
+def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, modelTs, device=None, estimation="point_to_plane",
+                   depth_scale=1.0, render_scale=1.0, stream=None):
     """The drivers' loop over the NMS survivors (linemod_and_levelup_test.py:348-367: one poseRefine per
     match, fed with the render of the matched template's pose) as ONE batched GPU call: hypothesis i is
     matches[i] (its x, y) with modelDepths[i] / modelKs[i] / modelRs[i] / modelTs[i].  Returns a list of
-    poseRefine objects in the state process() would have left them in.  estimation as poseRefine()."""
+    poseRefine objects in the state process() would have left them in.  estimation as poseRefine().
+    Depths in device memory: sceneDepth a CUDA tensor and modelDepths a list of [H, W] CUDA tensors or one [n, H, W]
+    tensor, with depth_scale, render_scale and stream as poseRefine.process."""
     _lib.estimation_code(estimation)
     n = len(matches)
+    dev = _default_device() if device is None else int(device)
+    renders = modelDepths if _lib.is_tensor(modelDepths) else list(modelDepths)
+    inputs = _lib.depth_inputs(sceneDepth, renders, depth_scale, render_scale, stream, dev, n,
+                               dict(sceneK=sceneK, modelKs=modelKs, modelRs=modelRs, modelTs=modelTs))
     out = [poseRefine(estimation) for _ in range(n)]
     if n == 0:
         return out
-    scene = np.asarray(sceneDepth)
-    if scene.dtype != np.uint16 or scene.ndim != 2:
-        raise TypeError("sceneDepth must be a uint16 HxW depth image (mm)")
-    models = [np.asarray(m) for m in modelDepths]
-    if len(models) != n or any(m.dtype != np.uint16 or m.ndim != 2 for m in models):
-        raise TypeError("modelDepths: one uint16 HxW render per match")
+    if inputs is None:
+        scene = np.asarray(sceneDepth)
+        if scene.dtype != np.uint16 or scene.ndim != 2:
+            raise TypeError("sceneDepth must be a uint16 HxW depth image (mm)")
+        models = [np.asarray(m) for m in renders]
+        if len(models) != n or any(m.dtype != np.uint16 or m.ndim != 2 for m in models):
+            raise TypeError("modelDepths: one uint16 HxW render per match")
     sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
     mK = np.stack([poseRefine._mat(k, np.float32, (3, 3), "modelK") for k in modelKs])
     R = np.stack([poseRefine._mat(r, np.float32, (3, 3), "modelR") for r in modelRs])
     t = np.stack([poseRefine._mat(v, np.float32, (3,), "modelT") for v in modelTs])
     xy = [[int(m.x), int(m.y)] for m in matches]
-    dev = out[0].device if device is None else int(device)
-    Ro, to, res = _native(dev).process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
+    if inputs is None:
+        Ro, to, res = _native(dev).process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
+    else:
+        Ro, to, res = _native(dev).process_batch_device(inputs, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
     for i, p in enumerate(out):
         p._residual = float(res[i])
         if res[i] != -1.0:

@@ -556,8 +556,40 @@ int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int 
                          const float* R, const float* t, const int32_t* detect_xy, int max_iterations, double* R_out,
                          double* t_out, float* residual);
 
+/* lm_icp_process_batch for a scene and renders already in device memory (a GPU decoder's depth, a depth network's, a GPU
+ * renderer's output): the clouds are built on the device by the pose stage's kernels (k_pose_cloud, a segmented sort,
+ * k_pose_voxel), fed by k_icp_scene, k_icp_render_box and k_icp_render_crop, then the same ICP kernels run.
+ *   Inputs     scene_depth srows x scols, rows scene_pitch BYTES apart; model_depths[i] mrows x mcols, rows
+ *              model_pitches[i] bytes apart (pointers may repeat; crop views are fine).  Pixels packed within a row; every
+ *              plane is device or managed memory of the handle's device.  scene_format / model_format: LM_DEPTH_U16_MM
+ *              (u16 mm, as is) or LM_DEPTH_F32 (float32 d to u16 mm with scene_scale / model_scale, exactly as
+ *              lm_bind_images_device converts it).  sceneK, modelK, R, t, detect_xy and the outputs are host arrays, as
+ *              in lm_icp_process_batch.
+ *   Semantics  R_out, t_out and residual are bit for bit lm_icp_process_batch's on the converted u16 images, for every
+ *              input: the early return of LL.cpp:52-55 (residual -1, R_out / t_out untouched), all-zero renders, a zero
+ *              anchor and the NaN patterns they give included.  The handle's estimation and use_scene_cloud apply.
+ *   Ordering   as lm_bind_images_device: an event recorded on `stream` (a cudaStream_t; NULL = the legacy default stream)
+ *              gates the reads, and `stream` waits on a second event behind the last read.  The call returns once the
+ *              outputs are on the host; it synchronises the handle's stream only (twice: the render boxes are read back
+ *              once to size the crops, lm_pose.h).
+ *   Launches   3 (k_icp_scene, k_icp_render_box, k_icp_render_crop) plus, per chunk of 1024 hypotheses, the pose stage's
+ *              5 (point-to-plane) or 4 (point-to-point); 2 when every hypothesis takes the early return; none for n_hyp 0.
+ * LM_E_INVALID before any device work for a null argument, an empty image, max_iterations < 0, an unknown format, a
+ * non-finite or non-positive scale with LM_DEPTH_F32, a stream of another device, a plane that is not device memory of
+ * the handle's device or whose pitch is shorter than a row or not aligned to its elements; LM_E_INVALID after the box
+ * read-back for a render whose box has 2^21 pixels or more (lm_set_template_renders' limit).  LM_E_STATE while capture
+ * is on (lm_icp_set_capture records the host path only).  lm_icp_last_stats and lm_icp_launch_count cover the call. */
+int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, int64_t scene_pitch, int scene_format,
+                                float scene_scale, int srows, int scols, const void* const* model_depths,
+                                const int64_t* model_pitches, int model_format, float model_scale, int mrows, int mcols,
+                                const float* sceneK, const float* modelK, const float* R, const float* t,
+                                const int32_t* detect_xy, int max_iterations, double* R_out, double* t_out, float* residual,
+                                void* stream);
+
 /* Of the last hypothesis processed: [0] points in the down-sampled cloud, [1] ICP iterations run,
- * [2] inlier rmse (m), [3] device time of the normals + ICP kernels of the last call (us). */
+ * [2] inlier rmse (m), [3] device time of the normals + ICP kernels of the last call (us); after
+ * lm_icp_process_batch_device the device time from its input copy to the end of its last ICP kernel, the box read-back
+ * included. */
 int lm_icp_last_stats(lm_icp* h, double* out4);
 /* NOT the reference's behaviour (default off): register the model cloud against the down-sampled SCENE
  * cloud, which is what LL.cpp:109 evidently meant to do (it down-samples the model cloud twice). */
