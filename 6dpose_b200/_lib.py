@@ -934,7 +934,7 @@ class NativeDetector:
 
     PLAN_KEYS = ["k1_band", "planes_level", "pseg", "k1_smem", "rounds", "bit_planes", "packed_templates", "byte_templates",
                  "k2_smem", "split", "plane_bytes", "k2_tasks", "filter_ok", "use_bits", "filter_templates", "gated",
-                 "filter_items", "refine_bits_items", "refine_filtered_items", "refine_items"]
+                 "filter_items", "refine_bits_items", "refine_filtered_items", "refine_items", "refine_bits_ctas"]
 
     def plan(self):
         """The kernels and launch shapes of the last run (lm_debug_plan); -1: that kernel did not run."""

@@ -149,9 +149,10 @@ struct lm_detector {
   // refinement filter (k_refine_filter_w) on the first refined level lr = L - 2: column-major H-planes + descriptors
   bool filter_ok = false;            // the current frame size / bank allow it
   int last_planes_level = -1;        // level the last K1 built in planes mode (its byte linear memories are stale)
-  DeviceArray<uint32_t> d_rp; int rp_nyb = 0;
+  // H-planes + zero tail, then the N-planes + zero tail at word rp_noff (N word = H word + rp_noff)
+  DeviceArray<uint32_t> d_rp; int rp_nyb = 0; uint32_t rp_noff = 0;
   DeviceArray<uint32_t> d_rdesc;     // per feature of level lr, grouped per template, padded to multiples of 32
-  DeviceArray<uint8_t> d_rlab;       // label per descriptor (8 = padding): k_refine_bits derives the neighbour planes
+  int bits_grid = 0;                 // k_refine_bits CTAs: the resident ones (occupancy x SMs), 0 = not yet asked
   bool shard_all_eligible = false;   // every template of the shard is taken by the filter (no byte-wise refinement)
   DeviceArray<uint32_t> d_surv2;     // candidates of the templates the filter does not take
   DeviceArray<int2> d_rfeat;         // per template: first descriptor, count
@@ -675,10 +676,10 @@ static int prepare_bank(lm_detector* d) {
   // refinement filter (k_refine_filter_w) on the first refined level: column-major H-planes [M*8*T*T][nyb][Wd] and one
   // descriptor per feature = plane word offset (incl. x / T) : 23 | y / T : 9.  Eligible templates ("safe", so that
   // the 16x16 patch of every feature is a true 2-D window of the level, and at most 511 features at that level) get
-  // bit 1 of their flag byte; the others go to k_refine unfiltered.
+  // bit 1 of their flag byte; the others go to k_refine unfiltered.  The exact pass (k_refine_bits) also reads the
+  // N-planes, same layout, behind the H-planes and their tail: a descriptor's N window is its H window + rp_noff words.
   d->filter_ok = false;
   std::vector<uint32_t> rdesc;
-  std::vector<uint8_t> rlab;
   std::vector<int2> rfeat((size_t)d->G, make_int2(0, 0));
   if (d->L >= 2) {
     const int lr = d->L - 2;
@@ -691,12 +692,13 @@ static int prepare_bank(lm_detector* d) {
     if (lv.Wd % 4 == 0 && lv.Wd >= 16 && lv.Hd >= 16 && lv.Hd <= 512 && words > 0 && words + tail <= (1u << 23)) {
       d->filter_ok = true;
       // a new layout gets new, zeroed planes: with M and T fixed, size and nyb fix Wd.  Equal sizes of two layouts do
-      // not share: the old planes would lie where the new tail must read zeros
-      if (words + tail != d->d_rp.size() || nyb != d->rp_nyb) {
-        CU(d->d_rp.assign(words + tail));
-        CU(cudaMemsetAsync(d->d_rp.get(), 0, (words + tail) * 4, d->stream.get()));  // halves no row block covers stay zero
+      // not share: the old planes would lie where the new tails must read zeros
+      if (2 * (words + tail) != d->d_rp.size() || nyb != d->rp_nyb) {
+        CU(d->d_rp.assign(2 * (words + tail)));
+        CU(cudaMemsetAsync(d->d_rp.get(), 0, 2 * (words + tail) * 4, d->stream.get()));  // halves no row block covers stay zero
       }
       d->rp_nyb = nyb;
+      d->rp_noff = (uint32_t)(words + tail);
       for (int g = 0; g < d->G; ++g) {
         int nfl = 0;
         for (int m = 0; m < d->M; ++m) nfl += d->tmeta[((size_t)g * d->S + lr * d->M + m) * 4 + 3];
@@ -709,22 +711,16 @@ static int prepare_bank(lm_detector* d) {
             const int32_t* f = &d->feats[3 * ((size_t)tm[2] + k)];
             const uint32_t pb = (uint32_t)((m * 8 + f[2]) * T2 + (f[1] % T) * T + (f[0] % T));
             rdesc.push_back((pb * (uint32_t)nyb * (uint32_t)lv.Wd + (uint32_t)(f[0] / T)) | ((uint32_t)(f[1] / T) << 23));
-            rlab.push_back((uint8_t)f[2]);
           }
         }
-        while (rdesc.size() % 32) {  // padding: the zero tail, row 0
-          rdesc.push_back((uint32_t)words);
-          rlab.push_back(8);
-        }
+        while (rdesc.size() % 32) rdesc.push_back((uint32_t)words);  // padding: the zero tail (+ rp_noff: the N tail), row 0
       }
     }
   }
   d->h_rfeat = rfeat;
   d->d_rdesc.reset();
   d->d_rfeat.reset();
-  d->d_rlab.reset();
   if (d->filter_ok) {
-    CU(upload(d->d_rlab, rlab, d->stream.get(), 1));
     CU(upload(d->d_rdesc, rdesc, d->stream.get(), 1));
     CU(upload(d->d_rfeat, rfeat, d->stream.get(), 1));
   }
@@ -1530,10 +1526,14 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     pp.n_work = n_work; pp.nwords = low.nwords;
     pp.cand = d->d_cand.get(); pp.cand_cap = (int)cand_cap(d);
     pp.expand_blocks = std::max(1, std::min((n_work + 7) / 8, d->sm_count * 8));
-    pp.lm = lref.d_lm.get(); pp.rp = (filter && d->last_planes_level < 0) ? d->d_rp.get() : nullptr;  // else: K1 wrote the planes
-    pp.Wd = lref.Wd; pp.Hd = lref.Hd; pp.plane = lref.plane; pp.nyb = d->rp_nyb;
-    pp.n_pb = d->M * 8 * lref.T * lref.T;
-    const int plane_blocks = pp.rp ? (int)(((size_t)pp.n_pb * pp.nyb * (pp.Wd / 4) + 255) / 256) : 0;
+    // H- and N-planes from the byte linear memories, or, after K1 in planes mode, N from K1's H-planes (eight labels a thread)
+    pp.rp = filter ? d->d_rp.get() : nullptr;
+    pp.lm = d->last_planes_level < 0 ? lref.d_lm.get() : nullptr;
+    pp.Wd = lref.Wd; pp.Hd = lref.Hd; pp.plane = lref.plane; pp.nyb = d->rp_nyb; pp.n_off = d->rp_noff;
+    pp.t2 = lref.T * lref.T;
+    pp.n_pb = d->M * 8 * pp.t2;
+    const size_t plane_threads = (size_t)(pp.lm ? pp.n_pb : pp.n_pb / 8) * pp.nyb * (pp.Wd / 4);
+    const int plane_blocks = pp.rp ? (int)((plane_threads + 255) / 256) : 0;
     CU(launch_pdl(k_refine_prep, dim3((unsigned)(pp.expand_blocks + plane_blocks)), dim3(256), 0, st, pp));
     ++d->launches;
   }
@@ -1555,8 +1555,8 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
   if (bits_mode) {
     // exact refinement of the survivors, bit-sliced, from the same H-planes
     RefineBitsParams bq;
-    bq.rp = d->d_rp.get(); bq.Wd = lref.Wd; bq.label_stride = lref.T * lref.T * d->rp_nyb * lref.Wd;
-    bq.rdesc = d->d_rdesc.get(); bq.rlab = d->d_rlab.get(); bq.finfo = d->d_finfo.get();
+    bq.rp = d->d_rp.get(); bq.Wd = lref.Wd; bq.n_off = d->rp_noff;
+    bq.rdesc = d->d_rdesc.get(); bq.finfo = d->d_finfo.get();
     bq.low = level_dev(low); bq.ref = level_dev(lref);
     bq.cand = d->d_cand.get(); bq.off = d->d_off.get(); bq.n_work = n_work; bq.cand_cap = (int)cand_cap(d);
     bq.surv = d->d_surv.get(); bq.queue = d->d_queue.get();
@@ -1568,7 +1568,12 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     bq.publish = bytes_pass ? 0 : 1;
     bq.counters = d->d_counters.get();
     bq.bp_clear = low.d_bp.get(); bq.bp_words = !low.d_bp.empty() ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
-    CU(launch_pdl(k_refine_bits, dim3((unsigned)(d->sm_count * 6)), dim3(256), 0, st, bq));
+    if (d->bits_grid == 0) {  // one wave: the survivors are dealt over the CTAs that are resident at once
+      int per_sm = 0;
+      CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refine_bits, 256, 0));
+      d->bits_grid = std::max(1, per_sm) * d->sm_count;
+    }
+    CU(launch_pdl(k_refine_bits, dim3((unsigned)d->bits_grid), dim3(256), 0, st, bq));
     ++d->launches;
   }
   if (bytes_pass) {
@@ -2621,7 +2626,10 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   const int total = (int)std::min<int64_t>(hres(d)->coarse_candidates, cand_cap(d));
   const bool filter = use_filter(d), bits_mode = use_bits(d);
   if (filter) out[16] = total;
-  if (bits_mode) out[17] = std::min(queue[1], total);
+  if (bits_mode) {
+    out[17] = std::min(queue[1], total);
+    out[20] = d->bits_grid;
+  }
   if (!bits_mode || !d->shard_all_eligible) {
     if (filter) out[18] = std::min(queue[bits_mode ? 2 : 1], total);
     else out[19] = total;

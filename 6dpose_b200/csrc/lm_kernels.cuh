@@ -1064,7 +1064,9 @@ __global__ void __launch_bounds__(1024) k_coarse_bytes(typename ByteScanArgs<kGa
 //     lm_response).  COLUMN-major and overlapping: word (x, yb) of block (modality, label, grid) holds rows
 //     16*yb .. 16*yb + 31 of column x, so the 16 rows of ANY 16x16 patch column are bits s .. s+15 of ONE word, and the 16
 //     columns of a patch are 16 consecutive words (64 contiguous bytes) -- against 16 rows x 16 bytes in 16 different
-//     128-byte lines of the byte linear memories.
+//     128-byte lines of the byte linear memories.  N-planes for the exact pass, same layout n_off words further on:
+//     bit = (response == 1) = a neighbouring label's spread bit without the label's own.  After K1 in planes mode (H-planes
+//     only, no byte linear memories) N is derived word for word from the H-planes of the three labels.
 // --------------------------------------------------------------------------------------------
 struct PrepParams {
   const int32_t* off;    // [n_work + 1]
@@ -1073,9 +1075,10 @@ struct PrepParams {
   uint2* cand;
   int cand_cap;
   int expand_blocks;     // blocks [0, expand_blocks) expand, the others build planes
-  const uint8_t* lm;     // byte linear memories of the filtered level, [M*8*T*T][plane]
-  uint32_t* rp;          // [M*8*T*T][nyb][Wd], null: no planes
-  int Wd, Hd, plane, nyb, n_pb;
+  const uint8_t* lm;     // byte linear memories of the filtered level, [M*8*T*T][plane]; null: K1 wrote the H-planes
+  uint32_t* rp;          // [M*8*T*T][nyb][Wd] H-planes, the N-planes at rp + n_off; null: no planes
+  int Wd, Hd, plane, nyb, n_pb, t2;  // n_pb = M * 8 * t2 planes
+  uint32_t n_off;        // a multiple of 4 (128-bit accesses)
 };
 
 __global__ void __launch_bounds__(256) k_refine_prep(PrepParams p) {
@@ -1110,14 +1113,34 @@ __global__ void __launch_bounds__(256) k_refine_prep(PrepParams p) {
     return;
   }
   if (!p.rp) return;
-  // planes: one thread = 4 neighbouring columns of one word row (32-bit loads of 4 response bytes, one 128-bit store)
   const int wq = p.Wd >> 2;
-  const int n = p.n_pb * p.nyb * wq;
   const int t = ((int)blockIdx.x - p.expand_blocks) * 256 + (int)threadIdx.x;
+  if (!p.lm) {
+    // N from the H-planes: one thread = 4 neighbouring words of one word row of one (modality, grid), all eight labels
+    const int per_label = p.t2 * p.nyb * p.Wd;                  // words between the planes of consecutive labels
+    if (t >= (p.n_pb >> 3) * p.nyb * wq) return;
+    const int x4 = t % wq, r = t / wq;                           // r = (m * t2 + g) * nyb + yb
+    const int m = r / (p.t2 * p.nyb);
+    uint4* const h = reinterpret_cast<uint4*>(p.rp + (size_t)m * 8 * per_label + (size_t)(r - m * p.t2 * p.nyb) * p.Wd) + x4;
+    const int ls = per_label / 4;                                // uint4 between consecutive labels
+    uint4 v[8];
+#pragma unroll
+    for (int o = 0; o < 8; ++o) v[o] = h[o * ls];
+    uint4* const nw = reinterpret_cast<uint4*>(p.rp + p.n_off + (h - reinterpret_cast<uint4*>(p.rp)) * 4);
+#pragma unroll
+    for (int o = 0; o < 8; ++o) {
+      const uint4 a = v[(o + 1) & 7], b = v[(o + 7) & 7], c = v[o];
+      nw[o * ls] = make_uint4((a.x | b.x) & ~c.x, (a.y | b.y) & ~c.y, (a.z | b.z) & ~c.z, (a.w | b.w) & ~c.w);
+    }
+    return;
+  }
+  // planes from the byte linear memories: one thread = 4 neighbouring columns of one word row (32-bit loads of 4 response
+  // bytes, one 128-bit store per plane)
+  const int n = p.n_pb * p.nyb * wq;
   if (t >= n) return;
   const int x4 = t % wq, yb = (t / wq) % p.nyb, pb = t / (wq * p.nyb);
   const uint32_t* __restrict__ src = reinterpret_cast<const uint32_t*>(p.lm + (size_t)pb * p.plane) + x4;
-  uint32_t o0 = 0, o1 = 0, o2 = 0, o3 = 0;
+  uint32_t o0 = 0, o1 = 0, o2 = 0, o3 = 0, n0 = 0, n1 = 0, n2 = 0, n3 = 0;
   const int r0 = 16 * yb;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {  // 8 rows at a time: byte c of t collects the 8 row bits of column c
@@ -1127,15 +1150,24 @@ __global__ void __launch_bounds__(256) k_refine_prep(PrepParams p) {
       const int r = r0 + 8 * k + b;
       v[b] = (r < p.Hd) ? __ldg(src + (size_t)r * wq) : 0u;
     }
-    uint32_t t = 0u;
+    uint32_t t = 0u, tn = 0u;
 #pragma unroll
-    for (int b = 0; b < 8; ++b) t += ((v[b] >> 2) & 0x01010101u) << b;  // response 4 <=> bit 2; the bits never meet
+    for (int b = 0; b < 8; ++b) {
+      t += ((v[b] >> 2) & 0x01010101u) << b;  // response 4 <=> bit 2; the bits never meet
+      tn += (v[b] & 0x01010101u) << b;        // response 1 <=> bit 0
+    }
     o0 |= (t & 0xFFu) << (8 * k);
     o1 |= ((t >> 8) & 0xFFu) << (8 * k);
     o2 |= ((t >> 16) & 0xFFu) << (8 * k);
     o3 |= (t >> 24) << (8 * k);
+    n0 |= (tn & 0xFFu) << (8 * k);
+    n1 |= ((tn >> 8) & 0xFFu) << (8 * k);
+    n2 |= ((tn >> 16) & 0xFFu) << (8 * k);
+    n3 |= (tn >> 24) << (8 * k);
   }
-  *reinterpret_cast<uint4*>(p.rp + ((size_t)pb * p.nyb + yb) * p.Wd + 4 * x4) = make_uint4(o0, o1, o2, o3);
+  uint32_t* const h = p.rp + ((size_t)pb * p.nyb + yb) * p.Wd + 4 * x4;
+  *reinterpret_cast<uint4*>(h) = make_uint4(o0, o1, o2, o3);
+  *reinterpret_cast<uint4*>(h + p.n_off) = make_uint4(n0, n1, n2, n3);
 }
 
 // --------------------------------------------------------------------------------------------
@@ -1729,17 +1761,17 @@ __global__ void __launch_bounds__(256, LM_REFINE_MIN_CTAS) k_refine(RefineParams
 // similarityLocal's response is 4*H + N with H = the feature's label bit in the spread mask and N = (either neighbouring
 // label bit) & ~H (lm_response), so the exact 16x16 sums are raw = 4*CH + CN.  Same warp layout as k_refine_filter_w
 // (lane k of each half-warp holds patch column k, the half-warps deal the features of a step between them, two features
-// per register), but three H-plane windows per feature (labels o - 1, o, o + 1) and two vertical counters.  The partial
+// per register), but two plane windows per feature at the same word index: the H-plane and the N-plane n_off words
+// further on (k_refine_prep writes N, it depends on the frame only), and two vertical counters.  The partial
 // counters meet once, at the end; the score 4*CH + CN, the best cell (max raw, lowest cell index = first maximum in
 // row-major order, LL.cpp:1910-1927) and the keep test (LL.cpp:1935-1937) are evaluated bit-sliced.  The byte linear
 // memories are never touched.
 // --------------------------------------------------------------------------------------------
 struct RefineBitsParams {
-  const uint32_t* rp;      // H-planes of level 0 (k_refine_prep), zero tail behind
+  const uint32_t* rp;      // H-planes of level 0 (k_refine_prep or K1), zero tail behind; the N-planes at rp + n_off
   int Wd;
-  int label_stride;        // words between the planes of consecutive labels: T*T * nyb * Wd
+  uint32_t n_off;
   const uint32_t* rdesc;   // as FilterParams (padded to multiples of 32 per template)
-  const uint8_t* rlab;     // per descriptor: the feature's label 0..7, 8 = padding
   const int4* finfo;
   LevelDev low, ref;
   const uint2* cand;
@@ -1770,27 +1802,32 @@ __device__ __forceinline__ void vc_add(uint32_t (&c)[LM_FILTER_BITS], const uint
   }
 }
 
-// Four warps share a survivor (a candidate is a chain of nf / 32 dependent steps, and the survivors are too few to hide
-// it with other warps): warp q of the quad takes the 32-feature steps q, q + 4, ..., the partial counters meet in shared
-// memory and warp 0 of the quad finishes the candidate.
+// A survivor is a chain of nf / 32 dependent steps, and the survivors are few, so a TEAM of ts warps of one CTA shares
+// one: warp q of the team takes the 32-feature steps q, q + ts, ..., the partial counters meet in shared memory and warp
+// 0 of the team finishes the candidate.  The grid is the CTAs resident at once (the host sizes it from the occupancy),
+// and ts is the largest of 8, 4, 2, 1 that still gives every survivor a team in ONE round: a second round, run by a few
+// CTAs while the others idle, would add a whole chain.  Round r deals survivor r * teams + t * gridDim.x + blockIdx.x
+// to team t of CTA blockIdx.x, so a partial round spreads over all SMs.
 __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
   lm_pdl_wait();
   __shared__ uint32_t s_part[8][2 * LM_FILTER_BITS][32];
-  __shared__ uint4 s_desc[8][2][3][8];  // per warp: the decoded descriptors of a step (three planes), as k_refine_filter_w
+  __shared__ uint4 s_desc[8][2][8];  // per warp: the decoded descriptors of a step, two buffers (as k_refine_filter_w)
   const int lane = threadIdx.x & 31, hw = lane >> 4, ck = lane & 15, warp = threadIdx.x >> 5;
-  const int quad = warp >> 2, q = warp & 3;
-  uint4 (*const sd)[3][8] = s_desc[warp];
+  uint4 (*const sd)[8] = s_desc[warp];
   int sb = 0;
   const int total = min(p.off[p.n_work], p.cand_cap);
   const int n_items = min(__ldcg(p.queue + 1), total);
+  int ts = 8;  // grid-uniform
+  while (ts > 1 && (long long)n_items * ts > (long long)gridDim.x * 8) ts >>= 1;
+  const int team = warp / ts, q = warp & (ts - 1), teams = 8 / ts;
   const int T = p.ref.T, border = 8 * T;
   const int Wd = p.Wd;
   unsigned feats_done = 0, words_read = 0;
   if (p.bp_clear)
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.bp_words; i += gridDim.x * blockDim.x) p.bp_clear[i] = 0u;
 
-  for (int base = blockIdx.x * 2; base < n_items; base += gridDim.x * 2) {
-    const int it = base + quad;
+  for (int base = 0; base < n_items; base += (int)gridDim.x * teams) {
+    const int it = base + team * (int)gridDim.x + (int)blockIdx.x;
     const bool valid = it < n_items;
     int c = 0, w = 0, x = 0, y = 0, nf = 0;
     uint32_t ch[LM_FILTER_BITS], cn[LM_FILTER_BITS];
@@ -1811,26 +1848,19 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
       x = min(x, p.ref.cols - (fi.z & 0xFFFF) - border);
       y = min(y, p.ref.rows - (int)((unsigned)fi.z >> 16) - border);
       const char* __restrict__ col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + ck));
+      const char* __restrict__ coln = reinterpret_cast<const char*>(p.rp + p.n_off + (x / T - 8 + ck));
       const int cy = y / T - 8;
       const uint32_t* __restrict__ fd = p.rdesc + fi.x;
-      const uint8_t* __restrict__ fl = p.rlab + fi.x;
       const int nfp = (nf + 31) & ~31;
       if (q == 0) feats_done += (unsigned)nf;
 
-      for (int i = q * 32; i < nfp; i += 128) {
-        // lane L decodes feature i + L: word offsets of the three label planes (row block of this candidate included)
-        // : 27 | row shift : 5
-        const uint32_t d = __ldg(fd + i + lane);
-        const int o = (int)__ldg(fl + i + lane);
+      uint32_t d_next = (q * 32 < nfp) ? __ldg(fd + q * 32 + lane) : 0u;
+      for (int i = q * 32; i < nfp; i += ts * 32) {
+        // lane L decodes feature i + L: plane byte offset (row block of this candidate included) : 27 | row shift : 5
+        const uint32_t d = d_next;
+        if (i + ts * 32 < nfp) d_next = __ldg(fd + i + ts * 32 + lane);  // one step ahead
         const int py0 = cy + (int)(d >> 23);
-        const uint32_t idx = (d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd);
-        const uint32_t sft = (uint32_t)py0 & 15u;
-        const int dm = o >= 8 ? 0 : (o == 0 ? 7 * p.label_stride : -p.label_stride);
-        const int dp = o >= 7 ? (o == 7 ? -7 * p.label_stride : 0) : p.label_stride;
-        uint32_t* const sw = reinterpret_cast<uint32_t*>(sd[sb]);
-        sw[lane] = (idx << 7) | sft;  // byte offset : 27 | row shift : 5
-        sw[32 + lane] = ((uint32_t)((int)idx + dm) << 7) | sft;
-        sw[64 + lane] = ((uint32_t)((int)idx + dp) << 7) | sft;
+        reinterpret_cast<uint32_t*>(sd[sb])[lane] = (((d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd)) << 7) | ((uint32_t)py0 & 15u);
         __syncwarp();
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
@@ -1838,19 +1868,11 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
 #pragma unroll
           for (int m = 0; m < 2; ++m) {
             // features i + 16 hw + 8 half + 4m .. + 3, two per register
-            const uint4 a0 = sd[sb][0][hw * 4 + half * 2 + m];
-            const uint4 am = sd[sb][1][hw * 4 + half * 2 + m];
-            const uint4 ap = sd[sb][2][hw * 4 + half * 2 + m];
-            const uint32_t h0 = __byte_perm(lm_plane_rows(col, a0.x), lm_plane_rows(col, a0.y), 0x5410);
-            const uint32_t n0 = __byte_perm(lm_plane_rows(col, am.x), lm_plane_rows(col, am.y), 0x5410) |
-                                __byte_perm(lm_plane_rows(col, ap.x), lm_plane_rows(col, ap.y), 0x5410);
-            const uint32_t h1 = __byte_perm(lm_plane_rows(col, a0.z), lm_plane_rows(col, a0.w), 0x5410);
-            const uint32_t n1 = __byte_perm(lm_plane_rows(col, am.z), lm_plane_rows(col, am.w), 0x5410) |
-                                __byte_perm(lm_plane_rows(col, ap.z), lm_plane_rows(col, ap.w), 0x5410);
-            xh[2 * m] = h0;
-            xn[2 * m] = n0 & ~h0;
-            xh[2 * m + 1] = h1;
-            xn[2 * m + 1] = n1 & ~h1;
+            const uint4 a = sd[sb][hw * 4 + half * 2 + m];
+            xh[2 * m] = __byte_perm(lm_plane_rows(col, a.x), lm_plane_rows(col, a.y), 0x5410);
+            xn[2 * m] = __byte_perm(lm_plane_rows(coln, a.x), lm_plane_rows(coln, a.y), 0x5410);
+            xh[2 * m + 1] = __byte_perm(lm_plane_rows(col, a.z), lm_plane_rows(col, a.w), 0x5410);
+            xn[2 * m + 1] = __byte_perm(lm_plane_rows(coln, a.z), lm_plane_rows(coln, a.w), 0x5410);
           }
           // four 1-bit planes into each vertical counter
           uint32_t t1a, t1b, t2;
@@ -1866,21 +1888,22 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
           for (int b = 2; b < LM_FILTER_BITS; ++b) { const uint32_t k = cn[b] & t2; cn[b] ^= t2; t2 = k; }
         }
         sb ^= 1;
-        words_read += 48;
+        words_read += 32;
       }
     }
-    // the quad's partial counters meet
-    if (q != 0) {
+    // the team's partial counters meet
+    if (ts > 1) {
+      if (q != 0) {
 #pragma unroll
-      for (int b = 0; b < LM_FILTER_BITS; ++b) {
-        s_part[warp][b][lane] = ch[b];
-        s_part[warp][LM_FILTER_BITS + b][lane] = cn[b];
+        for (int b = 0; b < LM_FILTER_BITS; ++b) {
+          s_part[warp][b][lane] = ch[b];
+          s_part[warp][LM_FILTER_BITS + b][lane] = cn[b];
+        }
       }
+      __syncthreads();
     }
-    __syncthreads();
     if (q == 0 && valid) {
-#pragma unroll
-      for (int k = 1; k < 4; ++k) {
+      for (int k = 1; k < ts; ++k) {
         uint32_t oh[LM_FILTER_BITS], on[LM_FILTER_BITS];
 #pragma unroll
         for (int b = 0; b < LM_FILTER_BITS; ++b) {
@@ -1930,7 +1953,7 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
       if (lane == 0 && !(sim < p.threshold))  // remove_if(similarity < threshold), LL.cpp:1935-1937
         append_record(p.hdr, p.capacity, p.px, p.px_seq, x, y, sim, p.work_begin + w * p.work_stride, c);
     }
-    __syncthreads();  // before the next candidate's partials overwrite these
+    if (ts > 1) __syncthreads();  // before the next candidate's partials overwrite these
   }
   words_read = __reduce_add_sync(0xffffffffu, words_read);
   if (lane == 0 && (feats_done | words_read)) {

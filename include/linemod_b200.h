@@ -485,12 +485,13 @@ int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* o
  * [9] its team split S, [10] bit-plane bytes, [11] its tasks ([8]..[11]: -1 without packed templates),
  * [12] the refinement filter is available for the frame size (1/0), [13] bit-sliced refinement (two levels, 1/0),
  * [14] templates of the shard the filter takes, [15] the frame ran depth-gated (1/0), then the work items of
- * [16] k_refine_filter_w, [17] k_refine_bits, [18] k_refine<true>, [19] k_refine<false> (-1: it did not run).
+ * [16] k_refine_filter_w, [17] k_refine_bits, [18] k_refine<true>, [19] k_refine<false> (-1: it did not run), [20] the
+ * CTAs k_refine_bits runs with (the ones resident at once; -1: it did not run).
  * Describes the last completed frame only between lm_complete (or lm_run) and the next lm_enqueue, and while the bank,
  * the selection, the frame size and the gate stay as they were: the routes are restated from the current host state, and
  * the survivor counts are read from the device when the getter is called, so after a later lm_enqueue the getter waits
  * for that frame and reports its counts. */
-#define LM_PLAN_ENTRIES 20
+#define LM_PLAN_ENTRIES 21
 int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap);
 /* Test getter: the coarse scan's outputs (k_coarse_packed / k_coarse_bytes) of the last completed frame, per work item of
  * this handle's shard in shard order.  dims3 = {n_work, nwords, plane} of the lowest level; `mask` receives
