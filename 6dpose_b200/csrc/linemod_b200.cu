@@ -208,6 +208,7 @@ struct lm_detector {
   DeviceArray<lm_match> d_post_out; PinnedArray<lm_match> h_post_out;  // LM_POST_MAX survivors
   DeviceArray<int32_t> d_post_counts; PinnedArray<int32_t> h_post_counts;
   DeviceArray<uint8_t> d_post_live;
+  DeviceArray<PostKey> d_post_keys;  // k_post_nms's sort keys beyond LM_POST_SMEM_KEYS records
 
   // pose stage behind the NMS (lm_pose.h): per-template render crops, refinement of the survivors on the device
   lm_pose_stage* pose = nullptr;
@@ -298,6 +299,7 @@ extern "C" int lm_create(int device, int n_levels, const int* T, lm_detector** o
   CU(cudaFuncSetAttribute(k_coarse_packed<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   CU(cudaFuncSetAttribute(k_coarse_packed<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LM_K2_SMEM_MAX));
   CU(cudaFuncSetAttribute(k_coarse_packed<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+  CU(cudaFuncSetAttribute(k_post_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(PostKey) * LM_POST_SMEM_KEYS)));
   CU(d->stream.create(cudaStreamNonBlocking));
   CU(d->copy_stream.create(cudaStreamNonBlocking));
   CU(d->ev_fork.create(cudaEventDisableTiming));
@@ -347,10 +349,15 @@ extern "C" int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_
   if (n_slots != d->L * d->M)
     return fail(LM_E_INVALID, "template pyramids have %d templates, detector expects %d (levels x modalities)", n_slots,
                 d->L * d->M);
+  // the box NMS orders matches by a key of 12 bits of class and 20 of template_id (lm_post.cuh)
+  if (n_classes > 4096) return fail(LM_E_INVALID, "bank of %d classes: at most 4096", n_classes);
   const int G = class_begin[n_classes];
   if (class_begin[0] != 0) return fail(LM_E_INVALID, "class_begin[0] must be 0");
-  for (int c = 0; c < n_classes; ++c)
+  for (int c = 0; c < n_classes; ++c) {
     if (class_begin[c + 1] < class_begin[c]) return fail(LM_E_INVALID, "class_begin not monotone");
+    if (class_begin[c + 1] - class_begin[c] > (1 << 20))
+      return fail(LM_E_INVALID, "class %d has %d templates: at most 1048576", c, class_begin[c + 1] - class_begin[c]);
+  }
   std::vector<uint8_t> slot_of((size_t)n_feats, 255);
   for (int g = 0; g < G; ++g)
     for (int s = 0; s < n_slots; ++s) {
@@ -2126,6 +2133,9 @@ static int prepare_post(lm_detector* d) {
   CU(d->d_post_counts.reserve(4));
   CU(d->h_post_counts.reserve(4));
   CU(d->d_post_live.reserve((size_t)d->res_cap));
+  size_t keys = 1;
+  while (keys < (size_t)d->res_cap) keys <<= 1;
+  if (keys > LM_POST_SMEM_KEYS) CU(d->d_post_keys.reserve(keys));
   if (!d->post_dirty) return LM_OK;
   if (!d->boxes.empty() && (int64_t)d->boxes.size() != 2 * (int64_t)d->G) {
     d->boxes.clear();  // the bank changed under the caller's boxes
@@ -2164,8 +2174,8 @@ static int enqueue_post(lm_detector* d, double iou_threshold, int top_k) {
   p.info = d->d_post_info.get(); p.n_sel = (int32_t)d->sel.size();
   p.iou_threshold = iou_threshold; p.top_k = top_k;
   p.out = d->d_post_out.get(); p.out_capacity = LM_POST_MAX;
-  p.out_counts = d->d_post_counts.get(); p.live = d->d_post_live.get();
-  CU(launch_pdl(k_post_nms, dim3(1), dim3(1024), 0, d->stream.get(), p));
+  p.out_counts = d->d_post_counts.get(); p.live = d->d_post_live.get(); p.keys = d->d_post_keys.get();
+  CU(launch_pdl(k_post_nms, dim3(1), dim3(1024), sizeof(PostKey) * LM_POST_SMEM_KEYS, d->stream.get(), p));
   ++d->launches;
   return LM_OK;
 }

@@ -73,8 +73,9 @@ void lm_destroy(lm_detector* d);
  *   tmeta[G][n_slots][4]      {width, height, feat_begin, feat_count}; n_slots = n_levels*2, slot =
  *                             level*2 + modality (LL.cpp:1964)
  *   feats[n_feats][3]         {x, y, label} (struct Feature, LL.h:23-34)
- * Fails with LM_E_INVALID on label outside [0,8), negative coordinates, or > 8191 features in a
- * template (CV_Assert LL.cpp:1291). */
+ * Fails with LM_E_INVALID on label outside [0,8), negative coordinates, > 8191 features in a
+ * template (CV_Assert LL.cpp:1291), more than 4096 classes or more than 2^20 templates in a class (the
+ * box NMS's canonical key, lm_enqueue_post). */
 int lm_load_bank(lm_detector* d, int n_classes, const int32_t* class_begin, int n_slots, const int32_t* tmeta,
                  const int32_t* feats, int64_t n_feats);
 
@@ -257,9 +258,15 @@ int lm_finish(lm_detector* d, const lm_record* records, int64_t n, lm_match* out
  *   lm_complete_post  waits; out[n_out] in pick order (best first); n_records = kept records the NMS saw.  A frame
  *                     that overflowed is grown and replayed first (lm_complete)
  *   lm_match_top      lm_upload_quantized + lm_enqueue + lm_enqueue_post + lm_complete_post
- * IoU as in the reference's nms(): float64, "+1" pixel convention, suppressed when ovr > threshold.  Equal
- * similarities (whose order the reference leaves to an unstable sort) are taken in template_id, class, y, x
- * order. */
+ * The survivors are those of the drivers' pipeline, nms() on the finished match list (after std::sort + std::unique,
+ * LL.cpp:1772-1774), restated without the unstable sorts: the kept records are put in the canonical order --
+ * similarity descending, then template_id, class, y, x ascending (equal similarities, which the reference leaves to an
+ * unstable sort, taken in that order) -- and each record equal to its predecessor there in (x, y, similarity, class)
+ * is dropped, as std::unique drops it (Match::operator== ignores template_id).  Then the greedy NMS in that order,
+ * IoU as in the reference's nms(): float64, "+1" pixel convention, suppressed when ovr > threshold.  A threshold
+ * >= 1 suppresses nothing: the survivors are every record the canonical dedupe keeps, in pick order; there the
+ * reference's own list also keeps duplicates that its sort's tie permutation did not make adjacent.  Banks of more
+ * than 4096 classes or 2^20 templates per class are refused by lm_load_bank (the canonical key's widths). */
 int lm_set_boxes(lm_detector* d, const int32_t* wh, int64_t n_templates);
 int lm_enqueue_post(lm_detector* d, double iou_threshold, int top_k);
 int lm_complete_post(lm_detector* d, lm_match* out, int64_t cap, int64_t* n_out, int64_t* n_records);
