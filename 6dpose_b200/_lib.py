@@ -28,7 +28,7 @@ SYMBOLS = [
     "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks", "lm_coarse_descriptors",
     "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device",
     "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_debug_plan", "lm_debug_coarse", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
-    "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_counters", "lm_set_timing",
+    "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_debug_time_k1", "lm_debug_bit_planes", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
     "lm_set_template_renders", "lm_enqueue_pose", "lm_complete_pose",
@@ -334,6 +334,8 @@ def load():
     L.lm_match_quantized.argtypes = [vp, u8pp, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_f, vp, c_i64,
                                      ctypes.POINTER(c_i64)]
     L.lm_debug_linear_memories.argtypes = [vp, c_int, c_int, ctypes.POINTER(ctypes.c_uint8), c_i64]
+    L.lm_debug_time_k1.argtypes = [vp, c_int, c_int, ctypes.POINTER(c_f)]
+    L.lm_debug_bit_planes.argtypes = [vp, ctypes.POINTER(ctypes.c_uint32), c_i64, ctypes.POINTER(c_i64)]
     L.lm_counters.argtypes = [vp, ctypes.POINTER(c_i64)]
     L.lm_set_timing.argtypes = [vp, c_int]
     L.lm_stage_times.argtypes = [vp, ctypes.POINTER(c_f)]
@@ -925,6 +927,24 @@ class NativeDetector:
                                                out.size))
         return out
 
+    def bit_planes(self):
+        """The lowest level's spread bit-planes of the last run (lm_debug_bit_planes): uint32 [M * 8 * lbw]."""
+        n = ctypes.c_int64()
+        rc = self._L.lm_debug_bit_planes(self._h, None, 0, ctypes.byref(n))
+        if rc != LM_E_CAPACITY:
+            check(rc)
+        out = np.zeros(int(n.value), np.uint32)
+        if out.size:
+            check(self._L.lm_debug_bit_planes(self._h, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint32)), out.size,
+                                              ctypes.byref(n)))
+        return out
+
+    def time_k1_us(self, level, reps):
+        """Mean device time of `reps` launches of the K1 blocks of `level` (-1: all of K1), as the last run planned them."""
+        us = ctypes.c_float()
+        check(self._L.lm_debug_time_k1(self._h, int(level), int(reps), ctypes.byref(us)))
+        return float(us.value)
+
     def counters(self):
         a = (ctypes.c_int64 * 8)()
         check(self._L.lm_counters(self._h, a))
@@ -934,7 +954,7 @@ class NativeDetector:
 
     PLAN_KEYS = ["k1_band", "planes_level", "pseg", "k1_smem", "rounds", "bit_planes", "packed_templates", "byte_templates",
                  "k2_smem", "split", "plane_bytes", "k2_tasks", "filter_ok", "use_bits", "filter_templates", "gated",
-                 "filter_items", "refine_bits_items", "refine_filtered_items", "refine_items", "refine_bits_ctas"]
+                 "filter_items", "refine_bits_items", "refine_filtered_items", "refine_items", "refine_bits_ctas", "k1_low_mode"]
 
     def plan(self):
         """The kernels and launch shapes of the last run (lm_debug_plan); -1: that kernel did not run."""

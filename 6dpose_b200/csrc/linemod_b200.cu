@@ -148,7 +148,8 @@ struct lm_detector {
   DeviceArray<uint16_t> d_galign;    // [G][S][16] feature counts per (address & 15) group
   // refinement filter (k_refine_filter_w) on the first refined level lr = L - 2: column-major H-planes + descriptors
   bool filter_ok = false;            // the current frame size / bank allow it
-  int last_planes_level = -1;        // level the last K1 built in planes mode (its byte linear memories are stale)
+  int lm_stale = 0;                  // levels (bit l) whose byte linear memories the last K1 did not build: the level built
+                                     // as H-planes only, the lowest level when nothing read its bytes
   // H-planes + zero tail, then the N-planes + zero tail at word rp_noff (N word = H word + rp_noff)
   DeviceArray<uint32_t> d_rp; int rp_nyb = 0; uint32_t rp_noff = 0;
   DeviceArray<uint32_t> d_rdesc;     // per feature of level lr, grouped per template, padded to multiples of 32
@@ -1326,7 +1327,9 @@ static LevelDev level_dev(const LevelHost& h) {
 
 
 // K1 launch plan: block ranges per level (lowest level first), kernel variant and shared memory.  planes_level >= 0: that
-// level is built in planes mode (column-major H-planes only, no byte linear memories; see spread_planes_block).
+// level is built in planes mode (column-major H-planes only, no byte linear memories; see spread_planes_block).  low_bytes:
+// the lowest level gets its byte linear memories too (only k_coarse_bytes and the debug getter read them); with_bit_planes:
+// it gets its spread bit-planes (band kernel: CTAs of their own ahead of its byte CTAs, see spread_bits_block).
 struct K1Plan {
   LinMemParams p;
   bool band = false;
@@ -1334,7 +1337,7 @@ struct K1Plan {
   int blocks = 0;
 };
 
-static void plan_k1(lm_detector* d, int planes_level, bool with_bit_planes, K1Plan& k) {
+static void plan_k1(lm_detector* d, int planes_level, bool low_bytes, bool with_bit_planes, K1Plan& k) {
   LinMemParams& p = k.p;
   memset(&p, 0, sizeof(p));
   p.L = d->L; p.M = d->M; p.block_offset = 0;
@@ -1365,27 +1368,45 @@ static void plan_k1(lm_detector* d, int planes_level, bool with_bit_planes, K1Pl
   }
   band = band && smem <= LM_BAND_SMEM_LIMIT;
   int blocks = 0;
-  // block index order = lowest level first: its CTAs are the heavy ones (T*T = 64 grids per position row plus
-  // the bit-plane atomics), started last they would be the tail of the launch
+  // block index order = lowest level first: its CTAs are the heavy ones (T*T = 64 grids per position row), started last
+  // they would be the tail of the launch; and a launch of the lowest level alone stays one block range (upper_pending)
   for (int l = d->L - 1; l >= 0; --l) {
     const LevelHost& lv = d->lv[l];
     LinMemLevel& q = p.lv[l];
+    const bool low = l == d->L - 1;
     for (int m = 0; m < d->M; ++m) q.q[m] = lv.q_src[m];
-    q.lm = lv.d_lm.get(); q.bp = with_bit_planes ? lv.d_bp.get() : nullptr; q.lbw = lv.lbw;
+    q.lm = low && !low_bytes ? nullptr : lv.d_lm.get();
+    q.bp = low && with_bit_planes ? lv.d_bp.get() : nullptr;  // allocated for the lowest level only
+    q.lbw = lv.lbw;
     q.T = lv.T; q.rows = lv.rows; q.cols = lv.cols; q.Wd = lv.Wd; q.Hd = lv.Hd; q.plane = lv.plane;
     q.mod_stride = lv.mod_stride;
-    q.rp = nullptr; q.nyb = 0;
-    if (band && l == planes_level) {
-      q.rp = d->d_rp.get(); q.nyb = d->rp_nyb;
-      blocks += ((lv.Hd + 15) / 16) * (lv.Wd / q.pseg);
+    q.rp = nullptr; q.nyb = 0; q.bit_blocks = 0;
+    const int n = lv.T * lv.T * lv.plane;
+    if (!band) {
+      blocks += q.lm || q.bp ? (n + 255) / 256 : 0;  // one thread per index builds both
     } else {
-      blocks += band ? lv.Hd * q.nseg : (lv.T * lv.T * lv.plane + 255) / 256;
+      if (q.bp) q.bit_blocks = ((n + 31) / 32 + LM_BP_CTA_WORDS - 1) / LM_BP_CTA_WORDS;
+      blocks += q.bit_blocks;
+      if (l == planes_level) {
+        q.rp = d->d_rp.get(); q.nyb = d->rp_nyb;
+        blocks += ((lv.Hd + 15) / 16) * (lv.Wd / q.pseg);
+      } else if (q.lm) {
+        blocks += lv.Hd * q.nseg;
+      }
     }
     q.block_end = blocks;
   }
   k.band = band;
   k.smem = smem;
   k.blocks = blocks;
+}
+
+// levels (bit l) whose byte linear memories a K1 launch of this plan leaves unbuilt
+static int k1_stale(const lm_detector* d, const K1Plan& k) {
+  int stale = 0;
+  for (int l = 0; l < d->L; ++l)
+    if (!k.p.lv[l].lm || k.p.lv[l].rp) stale |= 1 << l;
+  return stale;
 }
 
 static int launch_k1(lm_detector* d, const K1Plan& k, int first_block, int n_blocks) {
@@ -1403,6 +1424,8 @@ static bool use_filter(const lm_detector* d) { return d->filter_ok && !d->d_rp.e
 static bool use_bits(const lm_detector* d) { return use_filter(d) && d->L == 2; }
 // level built in planes mode by K1, or -1: only when nothing reads that level's byte linear memories
 static int planes_level(const lm_detector* d) { return use_bits(d) && d->shard_all_eligible ? d->L - 2 : -1; }
+// the lowest level's byte linear memories are built only for the byte-wise coarse scan (the refinement starts a level up)
+static bool low_bytes(const lm_detector* d) { return d->n_items_bytes > 0; }
 
 // Enqueue every GPU stage of one frame on the detector's stream; no host synchronisation.
 static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
@@ -1428,11 +1451,11 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
   int k1_done = 0;
   if (!refine_only) {
     if (d->timing) CU(cudaEventRecord(d->ev[0].get(), st));
-    // K1: one launch for every level and modality.  Bit-planes are OR-ed in: zero at allocation, re-zeroed by the
-    // refinement kernel after every frame.  With a host upload in flight (upper levels still on the copy stream) the
-    // launch is split: the lowest level now, the levels above it behind the coarse scan, once their images have landed.
-    plan_k1(d, planes_level(d), true, k1);
-    d->last_planes_level = k1.band ? planes_level(d) : -1;
+    // K1: one launch for every level and modality.  Every live bit-plane word is stored whole each frame (the slack behind
+    // them stays zero from allocation).  With a host upload in flight (upper levels still on the copy stream) the launch
+    // is split: the lowest level now, the levels above it behind the coarse scan, once their images have landed.
+    plan_k1(d, planes_level(d), low_bytes(d), true, k1);
+    d->lm_stale = k1_stale(d, k1);
     k1_done = d->upper_pending ? k1.p.lv[d->L - 1].block_end : k1.blocks;
     int rc1 = launch_k1(d, k1, 0, k1_done);
     if (rc1) return rc1;
@@ -1535,7 +1558,7 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     pp.expand_blocks = std::max(1, std::min((n_work + 7) / 8, d->sm_count * 8));
     // H- and N-planes from the byte linear memories, or, after K1 in planes mode, N from K1's H-planes (eight labels a thread)
     pp.rp = filter ? d->d_rp.get() : nullptr;
-    pp.lm = d->last_planes_level < 0 ? lref.d_lm.get() : nullptr;
+    pp.lm = (d->lm_stale >> (d->L >= 2 ? d->L - 2 : 0)) & 1 ? nullptr : lref.d_lm.get();
     pp.Wd = lref.Wd; pp.Hd = lref.Hd; pp.plane = lref.plane; pp.nyb = d->rp_nyb; pp.n_off = d->rp_noff;
     pp.t2 = lref.T * lref.T;
     pp.n_pb = d->M * 8 * pp.t2;
@@ -1574,7 +1597,6 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     bq.px = px.world > 0 ? d->d_px.get() : nullptr; bq.px_seq = d->px_seq;
     bq.publish = bytes_pass ? 0 : 1;
     bq.counters = d->d_counters.get();
-    bq.bp_clear = low.d_bp.get(); bq.bp_words = !low.d_bp.empty() ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
     if (d->bits_grid == 0) {  // one wave: the survivors are dealt over the CTAs that are resident at once
       int per_sm = 0;
       CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_refine_bits, 256, 0));
@@ -1605,8 +1627,6 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     }
     rp.counters = d->d_counters.get();
     rp.safe = d->d_safe.get(); rp.galign = d->d_galign.get();
-    rp.bp_clear = bits_mode ? nullptr : low.d_bp.get();
-    rp.bp_words = (!bits_mode && !low.d_bp.empty()) ? (uint32_t)((size_t)d->M * 8 * low.lbw) : 0u;
     // 4 CTAs are resident per SM (64 registers x 256 threads); 16 per SM = four waves of equal shares, which
     // balances the very uneven per-candidate cost (row-wise early exit) better than one persistent wave
     // (measured: 4 -> 251 us, 8 -> 241, 12..32 -> 229)
@@ -2578,18 +2598,58 @@ extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality,
   const LevelHost& lv = d->lv[level];
   if ((int64_t)lv.mod_stride > cap) return fail(LM_E_CAPACITY, "need %u bytes", lv.mod_stride);
   CU(cudaSetDevice(d->device));
-  if (level == d->last_planes_level) {
-    // the last run built this level as H-planes only (nothing reads its bytes): build the bytes now, from the frame that
-    // is still bound, without touching the bit-planes
+  if ((d->lm_stale >> level) & 1) {
+    // the last run did not build this level's bytes (H-planes only, or a lowest level nothing read them from): build them
+    // now, from the frame that is still bound, without touching the bit-planes
     K1Plan k;
-    plan_k1(d, -1, false, k);
+    plan_k1(d, -1, true, false, k);
     const int b0 = level == d->L - 1 ? 0 : k.p.lv[level + 1].block_end;
     int rc = launch_k1(d, k, b0, k.p.lv[level].block_end - b0);
     if (rc) return rc;
-    d->last_planes_level = -1;
+    d->lm_stale &= ~(1 << level);
   }
   CU(cudaMemcpyAsync(out, lv.d_lm.get() + (size_t)modality * lv.mod_stride, lv.mod_stride, cudaMemcpyDeviceToHost, d->stream.get()));
   CU(cudaStreamSynchronize(d->stream.get()));
+  return LM_OK;
+}
+
+// The lowest level's spread bit-planes as the last lm_run left them: [M][8][lbw] words (live words, then the slack the
+// coarse scan's zero descriptor reads).
+extern "C" int lm_debug_bit_planes(lm_detector* d, uint32_t* out, int64_t cap, int64_t* n_words) {
+  if (!d || !n_words || (!out && cap > 0)) return fail(LM_E_INVALID, "null argument");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
+  const LevelHost& low = d->lv[d->L - 1];
+  *n_words = (int64_t)low.d_bp.size();
+  if (*n_words > cap) return fail(LM_E_CAPACITY, "need %lld words", (long long)*n_words);
+  if (*n_words == 0) return LM_OK;
+  CU(cudaSetDevice(d->device));
+  CU(cudaMemcpyAsync(out, low.d_bp.get(), sizeof(uint32_t) * (size_t)*n_words, cudaMemcpyDeviceToHost, d->stream.get()));
+  CU(cudaStreamSynchronize(d->stream.get()));
+  return LM_OK;
+}
+
+extern "C" int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us) {
+  if (!d || !us) return fail(LM_E_INVALID, "null argument");
+  if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
+  if (level < -1 || level >= d->L || reps < 1) return fail(LM_E_INVALID, "bad level/reps");
+  CU(cudaSetDevice(d->device));
+  K1Plan k;
+  plan_k1(d, planes_level(d), low_bytes(d), true, k);
+  const int b0 = level < 0 || level == d->L - 1 ? 0 : k.p.lv[level + 1].block_end;
+  const int b1 = level < 0 ? k.blocks : k.p.lv[level].block_end;
+  Event e0, e1;
+  CU(e0.create(cudaEventDefault));
+  CU(e1.create(cudaEventDefault));
+  CU(cudaEventRecord(e0.get(), d->stream.get()));
+  for (int r = 0; r < reps; ++r) {
+    int rc = launch_k1(d, k, b0, b1 - b0);
+    if (rc) return rc;
+  }
+  CU(cudaEventRecord(e1.get(), d->stream.get()));
+  CU(cudaEventSynchronize(e1.get()));
+  float ms = 0.f;
+  CU(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
+  *us = ms * 1000.f / (float)reps;
   return LM_OK;
 }
 
@@ -2607,7 +2667,7 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   CU(cudaStreamSynchronize(d->stream.get()));
   const LevelHost& low = d->lv[d->L - 1];
   K1Plan k1;
-  plan_k1(d, planes_level(d), true, k1);
+  plan_k1(d, planes_level(d), low_bytes(d), true, k1);
   const int pl = k1.band ? planes_level(d) : -1;
   for (int i = 0; i < LM_PLAN_ENTRIES; ++i) out[i] = -1;
   out[0] = k1.band ? 1 : 0;
@@ -2644,6 +2704,8 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
     if (filter) out[18] = std::min(queue[bits_mode ? 2 : 1], total);
     else out[19] = total;
   }
+  const LinMemLevel& kl = k1.p.lv[d->L - 1];
+  out[21] = (kl.bp ? 1 : 0) | (kl.lm ? 2 : 0);
   return LM_OK;
 }
 

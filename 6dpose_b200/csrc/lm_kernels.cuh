@@ -79,7 +79,7 @@ __device__ __forceinline__ void lm_pdl_wait() { asm volatile("griddepcontrol.wai
 // --------------------------------------------------------------------------------------------
 struct LinMemLevel {
   const uint8_t* q[LM_MAX_MODALITIES];  // quantized u8 rows x cols
-  uint8_t* lm;
+  uint8_t* lm;   // byte linear memories; null: not built (nothing reads them this frame)
   uint32_t* bp;  // optional: [M][8][lbw] words, bit (grid*plane + pos) of block (m, o) = spread bit o
   int lbw;
   int T, rows, cols, Wd, Hd, plane;
@@ -91,6 +91,7 @@ struct LinMemLevel {
   uint32_t* rp;   // non-null: planes mode
   int nyb;        // words per column: word yb = rows 16*yb .. 16*yb + 31
   int pseg;       // positions per column segment of a planes-mode CTA
+  int bit_blocks; // band kernel: the level's first bit_blocks CTAs build bp (LM_BP_CTA_WORDS words each), the rest lm / rp
 };
 
 struct LinMemParams {
@@ -132,7 +133,6 @@ __global__ void __launch_bounds__(256) k_linear_memories(LinMemParams p) {
   const int m = blockIdx.y;
   const int n = lv.T * lv.T * lv.plane;
   const uint8_t* __restrict__ q = (m == 0) ? lv.q[0] : lv.q[1];
-  uint8_t* __restrict__ out = lv.lm + (size_t)m * lv.mod_stride;
   const int i = (bx - first) * 256 + (int)threadIdx.x;  // 32-aligned across a warp
   uint32_t v = 0;
   if (i < n) {
@@ -147,10 +147,12 @@ __global__ void __launch_bounds__(256) k_linear_memories(LinMemParams p) {
       case 8: v = spread_window<8>(q, lv.cols, lv.rows, x, y, 8); break;
       default: v = spread_window<0>(q, lv.cols, lv.rows, x, y, lv.T); break;
     }
+    uint8_t* __restrict__ out = lv.lm + (size_t)m * lv.mod_stride;  // lm null: bit-planes only, no bytes
 #pragma unroll
-    for (int o = 0; o < 8; ++o) out[(size_t)o * n + i] = (uint8_t)lm_response(v, o);
+    for (int o = 0; o < 8; ++o)
+      if (lv.lm) out[(size_t)o * n + i] = (uint8_t)lm_response(v, o);
   }
-  if (lv.bp) {  // block-uniform
+  if (lv.bp) {  // block-uniform; whole words, plain stores
 #pragma unroll
     for (int o = 0; o < 8; ++o) {
       const uint32_t b = __ballot_sync(0xffffffffu, (v >> o) & 1u);
@@ -164,7 +166,7 @@ __global__ void __launch_bounds__(256) k_linear_memories(LinMemParams p) {
 // (horizontal then vertical, 4 pixels per 32-bit op), and the responses of 4 consecutive positions of
 // one (label, grid) plane are computed SIMD-in-register and written with one 32-bit store.  Needs
 // cols % 4 == 0 and Wd % 4 == 0 (every BASELINE size); other sizes use k_linear_memories above.
-// Bit-planes are OR-ed in with atomics (the caller zeroes them first).
+// Bit-planes come from CTAs of their own (spread_bits_block).
 // (row, column) of flat index i in a [rows][width] grid, advanced by `step` without a division
 struct RowCol {
   int r, c;
@@ -256,11 +258,67 @@ __device__ __forceinline__ void linear_memories_band_level(const LinMemLevel& lv
       const uint32_t hit = (V >> o) & 0x01010101u;
       const uint32_t nb = ((V >> ((o + 1) & 7)) | (V >> ((o + 7) & 7))) & 0x01010101u;
       *reinterpret_cast<uint32_t*>(o0 + (size_t)o * n) = (hit << 2) | (nb & ~hit);
-      if (lv.bp) {
-        const uint32_t nib = ((hit * 0x01020408u) >> 24) & 0xFu;  // the 4 hit bits, position order
-        if (nib) atomicOr(lv.bp + (size_t)(m * 8 + o) * lv.lbw + (pos >> 5), nib << (pos & 31));
-      }
     }
+  }
+}
+
+// OR of the forward TxT window at (x, y) from aligned 32-bit loads (needs cols % 4 == 0): the window's rows are OR-ed word
+// by word, then its T bytes from x & 3 on are folded into one.  Clipped at the bottom/right image edge like spread_window
+// (with cols % 4 == 0 a word lies wholly inside or wholly outside a row).
+template <int TT>
+__device__ __forceinline__ uint32_t spread_window_words(const uint8_t* __restrict__ q, int cols, int rows, int x, int y) {
+  constexpr int NW = (TT + 6) / 4;  // words a window of TT bytes can touch: 2 (T = 4), 3 (T = 8)
+  const int sh = x & 3;
+  const int nw = min((sh + TT + 3) >> 2, (cols - (x - sh)) >> 2);
+  const int ny = min(TT, rows - y);
+  const int pitch = cols >> 2;
+  const uint32_t* __restrict__ p = reinterpret_cast<const uint32_t*>(q + (size_t)y * cols + (x - sh));
+  uint32_t a[NW];
+#pragma unroll
+  for (int k = 0; k < NW; ++k) a[k] = 0u;
+#pragma unroll
+  for (int dy = 0; dy < TT; ++dy)
+#pragma unroll
+    for (int k = 0; k < NW; ++k)
+      if (dy < ny && k < nw) a[k] |= __ldg(p + dy * pitch + k);
+  uint32_t z = __funnelshift_r(a[0], a[1], 8 * sh);  // bytes sh .. sh + 3
+  if (TT == 8) z |= __funnelshift_r(a[1], a[2], 8 * sh);  // bytes sh + 4 .. sh + 7
+  z |= z >> 16;
+  z |= z >> 8;
+  return z & 0xFFu;
+}
+
+// K1, bit-planes of the lowest level: CTA bi builds words [bi * LM_BP_CTA_WORDS, +LM_BP_CTA_WORDS) of the eight label planes
+// of modality m, each whole.  Lane j of the warp that owns word w takes index 32w + j (grid g = index / plane, position
+// index % plane: words straddle rows of positions and grids), forms its spread mask straight from the frame, and one
+// ballot per label gives the eight words; lane o stores label o's.  Every live word is stored every frame, so nothing has
+// to clear the planes; the slack behind the last live word (read by the coarse scan's zero descriptor) is never written.
+#define LM_BP_CTA_WORDS 8
+template <int TT>
+__device__ __forceinline__ void spread_bits_block(const LinMemLevel& lv, int m, int bi) {
+  const int T = TT > 0 ? TT : lv.T;
+  const int n = T * T * lv.plane, lane = threadIdx.x & 31;
+  const int w_end = min((n + 31) >> 5, (bi + 1) * LM_BP_CTA_WORDS);
+  const uint8_t* __restrict__ q = (m == 0) ? lv.q[0] : lv.q[1];
+  uint32_t* __restrict__ bp = lv.bp + (size_t)m * 8 * lv.lbw;
+  for (int w = bi * LM_BP_CTA_WORDS + (int)(threadIdx.x >> 5); w < w_end; w += (int)(blockDim.x >> 5)) {  // warp-uniform
+    const int i = 32 * w + lane;
+    uint32_t v = 0;
+    if (i < n) {
+      const int g = i / lv.plane, pos = i - g * lv.plane;
+      const int py = pos / lv.Wd, px = pos - py * lv.Wd;
+      const int gy = g / T, gx = g - gy * T;
+      const int x = px * T + gx, y = py * T + gy;
+      if constexpr (TT > 0) v = spread_window_words<TT>(q, lv.cols, lv.rows, x, y);
+      else v = spread_window<0>(q, lv.cols, lv.rows, x, y, T);
+    }
+    uint32_t mine = 0;
+#pragma unroll
+    for (int o = 0; o < 8; ++o) {
+      const uint32_t b = __ballot_sync(0xffffffffu, (v >> o) & 1u);
+      if (lane == o) mine = b;
+    }
+    if (lane < 8) bp[(size_t)lane * lv.lbw + w] = mine;
   }
 }
 
@@ -371,7 +429,16 @@ __global__ void __launch_bounds__(256) k_linear_memories_band(LinMemParams p) {
   int l = p.L - 1, first = 0;
   while (l > 0 && bx >= p.lv[l].block_end) { first = p.lv[l].block_end; --l; }
   const LinMemLevel& lv = p.lv[l];
-  const int bi = bx - first;
+  int bi = bx - first;
+  if (bi < lv.bit_blocks) {  // bit-planes
+    switch (lv.T) {
+      case 4: spread_bits_block<4>(lv, blockIdx.y, bi); break;
+      case 8: spread_bits_block<8>(lv, blockIdx.y, bi); break;
+      default: spread_bits_block<0>(lv, blockIdx.y, bi); break;
+    }
+    return;
+  }
+  bi -= lv.bit_blocks;
   if (lv.rp) {  // planes mode
     switch (lv.T) {
       case 4: spread_planes_block<4>(lv, blockIdx.y, bi, s_band); break;
@@ -1499,8 +1566,6 @@ struct RefineParams {
                                  // offset is applied (LL.cpp:1394 never skips) -> 128-bit row loads
   const uint16_t* galign;        // [G][S][16]: features per (fbase & 15) group (refined levels are stored
                                  // grouped by it)
-  uint32_t* bp_clear;            // lowest level's bit-planes: consumed by the coarse scan of this frame,
-  uint32_t bp_words;             // cleared here for the next frame's K1 (which ORs its bits in)
 };
 
 // One lane pair = one row of the 16x16 patch: lane `half` loads the aligned 16-byte chunk (a >> 4) +
@@ -1563,8 +1628,6 @@ __global__ void __launch_bounds__(256, LM_REFINE_MIN_CTAS) k_refine(RefineParams
   const LevelDev low = p.lv[p.L - 1];
   const int row = lane >> 1, half = lane & 1;
   unsigned feats_done = 0, rows_read = 0;  // per warp: a few candidates x (features x 16 rows)
-  if (p.bp_clear)
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.bp_words; i += gridDim.x * blockDim.x) p.bp_clear[i] = 0u;
 
   // work items: the survivors of k_refine_filter_w (unordered candidate indices), or every candidate
   const int n_items = p.surv ? min(__ldcg(p.queue + p.surv_slot), total) : total;
@@ -1787,8 +1850,6 @@ struct RefineBitsParams {
   int32_t px_seq;
   int publish;
   unsigned long long* counters;  // [0] features x candidates refined here, [5] plane words read
-  uint32_t* bp_clear;
-  uint32_t bp_words;
 };
 
 // bit-sliced add of two vertical counters
@@ -1823,8 +1884,6 @@ __global__ void __launch_bounds__(256, 4) k_refine_bits(RefineBitsParams p) {
   const int T = p.ref.T, border = 8 * T;
   const int Wd = p.Wd;
   unsigned feats_done = 0, words_read = 0;
-  if (p.bp_clear)
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < p.bp_words; i += gridDim.x * blockDim.x) p.bp_clear[i] = 0u;
 
   for (int base = 0; base < n_items; base += (int)gridDim.x * teams) {
     const int it = base + team * (int)gridDim.x + (int)blockIdx.x;

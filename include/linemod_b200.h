@@ -481,8 +481,18 @@ int lm_depth_gate_stats(lm_detector* d, int64_t* out4);
 int lm_debug_quantized(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap);
 /* Depth image (u16 mm, rows*cols) of the frame lm_upload_images uploaded or lm_bind_images_device bound. */
 int lm_debug_depth(lm_detector* d, uint16_t* out, int64_t cap);
-/* Linear memories of (level, modality) of the last lm_run: [8][T*T][(cols/T)*(rows/T)] bytes. */
+/* Linear memories of (level, modality) of the last lm_run: [8][T*T][(cols/T)*(rows/T)] bytes.  A level whose bytes that
+ * run did not build (nothing read them) is built here first, from the frame still bound. */
 int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* out, int64_t cap);
+/* Test getter: the lowest level's spread bit-planes of the last lm_run, [M][8][lbw] uint32 words (bit i of a label's
+ * words: spread bit of linear-memory index i = grid * plane + position; the words behind the T*T*plane live bits are
+ * zero).  *n_words (M*8*lbw; 0 when the level has none) is set before the capacity test (LM_E_CAPACITY when cap is
+ * smaller; out may be null with cap 0).  Synchronises the stream. */
+int lm_debug_bit_planes(lm_detector* d, uint32_t* out, int64_t cap, int64_t* n_words);
+/* Development probe: the mean device time in microseconds of `reps` back-to-back launches of the K1 blocks of one level
+ * (level -1: the whole launch), planned as the last lm_run planned them, rebuilding that frame's outputs in place.
+ * Synchronises the stream.  LM_E_STATE before the first lm_run. */
+int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us);
 /* Test getter: which kernels and launch shapes the last lm_run took, restated from the host state the frame was
  * enqueued from (no launch; one small read of the filter's survivor counts).  LM_PLAN_ENTRIES int32 entries:
  * [0] linear memories by k_linear_memories_band (1) or k_linear_memories (0), [1] level built as H-planes only (-1:
@@ -493,12 +503,13 @@ int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* o
  * [12] the refinement filter is available for the frame size (1/0), [13] bit-sliced refinement (two levels, 1/0),
  * [14] templates of the shard the filter takes, [15] the frame ran depth-gated (1/0), then the work items of
  * [16] k_refine_filter_w, [17] k_refine_bits, [18] k_refine<true>, [19] k_refine<false> (-1: it did not run), [20] the
- * CTAs k_refine_bits runs with (the ones resident at once; -1: it did not run).
+ * CTAs k_refine_bits runs with (the ones resident at once; -1: it did not run), [21] what K1 builds of the lowest level:
+ * bit 0 its spread bit-planes, bit 1 its byte linear memories (built only when k_coarse_bytes has templates).
  * Describes the last completed frame only between lm_complete (or lm_run) and the next lm_enqueue, and while the bank,
  * the selection, the frame size and the gate stay as they were: the routes are restated from the current host state, and
  * the survivor counts are read from the device when the getter is called, so after a later lm_enqueue the getter waits
  * for that frame and reports its counts. */
-#define LM_PLAN_ENTRIES 21
+#define LM_PLAN_ENTRIES 22
 int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap);
 /* Test getter: the coarse scan's outputs (k_coarse_packed / k_coarse_bytes) of the last completed frame, per work item of
  * this handle's shard in shard order.  dims3 = {n_work, nwords, plane} of the lowest level; `mask` receives
