@@ -102,10 +102,44 @@ static size_t bp_label_words(int T, int plane) {
   return (((size_t)T * T * plane + 31) / 32 + 32 * rounds + 4 + 3) & ~(size_t)3;
 }
 
+// K1 launch plan (plan_k1): block ranges per level (lowest level first), kernel variant and shared memory.
+struct K1Plan {
+  LinMemParams p;
+  bool band = false;
+  size_t smem = 0;
+  int blocks = 0;
+};
+
+// Launch shape of k_coarse_packed (coarse_shape).
+struct CoarseShape {
+  bool smem;          // the bit-planes are staged in shared memory (k_coarse_packed<true>)
+  int split, wpc, grid;
+  size_t smem_bytes;  // dynamic shared memory: bit-planes + the teams' partial counters
+};
+
+// The kernel routes of the handle's frame, decided once by plan_frame: its stages launch from it, an overflow replay
+// reruns its refinement from it, lm_debug_plan reports it.  Decisions only: what a replay may grow is resolved at launch.
+struct FramePlan {
+  K1Plan k1;                  // one K1 launch for every level: byte linear memories, H-planes, the lowest level's bit-planes
+  int planes_level = -1;      // level K1 builds as H-planes only (-1: none)
+  int stale = 0;              // levels (bit l) K1 leaves without byte linear memories (lm_debug_linear_memories builds them)
+  bool gated = false;         // k_depth_cells, then the coarse kernels' gated instantiations
+  bool packed = false;        // k_coarse_packed on the templates the bit-sliced scan takes, launched as `coarse`
+  CoarseShape coarse = {};
+  size_t plane_bytes = 0;     // the lowest level's bit-planes, which k_coarse_packed's shape follows
+  bool bytes = false;         // k_coarse_bytes on the others
+  bool scan_fused = false;    // k_coarse_packed scans the candidate counts itself: no k_scan_counts
+  bool filter = false;        // k_refine_filter_w on the first refined level
+  bool bits = false;          // k_refine_bits finishes the filter's survivors (two levels)
+  bool bits_publish = false;  // ... and, as the frame's last appending kernel, publishes it to the peers
+  bool refine = false;        // k_refine<filter>, byte-wise: the templates the filter does not take, or every candidate
+  bool exchange = false;      // records go to this rank's block of the peer exchange, packed by k_peer_collect
+};
+
 // The stages enqueued for the handle's frame, each with the arguments a replay needs (complete_frame).  lm_enqueue sets
 // the match's; every later lm_enqueue_* raises its stage's flag, and the completion that waits for a stage lowers it.
 struct FrameChain {
-  float threshold = 0.f; bool gated = false;                // lm_enqueue
+  float threshold = 0.f; FramePlan plan;                    // lm_enqueue
   bool completed = false;  // lm_complete returned: the header, first records and counters are on the host (until a new
                            // frame, bank, selection, result block or exchange)
   bool post = false; double iou = 0.5; int top_k = 0;      // lm_enqueue_post
@@ -148,8 +182,6 @@ struct lm_detector {
   DeviceArray<uint16_t> d_galign;    // [G][S][16] feature counts per (address & 15) group
   // refinement filter (k_refine_filter_w) on the first refined level lr = L - 2: column-major H-planes + descriptors
   bool filter_ok = false;            // the current frame size / bank allow it
-  int lm_stale = 0;                  // levels (bit l) whose byte linear memories the last K1 did not build: the level built
-                                     // as H-planes only, the lowest level when nothing read its bytes
   // H-planes + zero tail, then the N-planes + zero tail at word rp_noff (N word = H word + rp_noff)
   DeviceArray<uint32_t> d_rp; int rp_nyb = 0; uint32_t rp_noff = 0;
   DeviceArray<uint32_t> d_rdesc;     // per feature of level lr, grouped per template, padded to multiples of 32
@@ -251,7 +283,6 @@ struct lm_detector {
 
   bool timing = false;
   int64_t timing_runs = 0;
-  const Event* ev = nullptr;     // the tev slot used by the run being enqueued
   int64_t launches = 0;
   int64_t alg_scan_bytes = 0;
   int sm_count = 132;
@@ -768,11 +799,6 @@ static void coarse_task_table(const int32_t* items, const int32_t* words, int64_
 // tasks than the GPU has warp slots: the team deals the task's features, so the kernel's latency follows the shard) and
 // one round per CTA where the tasks fit: the CTA size follows the shard, so a small shard spreads over all SMs, and
 // CTA b's share of the table (tasks b, b + grid, ...) never holds more tasks than the CTA has teams.
-struct CoarseShape {
-  bool smem;          // the bit-planes are staged in shared memory (k_coarse_packed<true>)
-  int split, wpc, grid;
-  size_t smem_bytes;  // dynamic shared memory: bit-planes + the teams' partial counters
-};
 static CoarseShape coarse_shape(int64_t tasks, int sm_count, size_t plane_bytes) {
   CoarseShape c;
   c.smem = plane_bytes <= LM_BITS_SMEM_LIMIT;
@@ -1039,7 +1065,7 @@ static int upload_quantized(lm_detector* d, const uint8_t* const* quantized, con
     if (!quantized[i]) return fail(LM_E_INVALID, "quantized[%d] is null", i);
   // lowest level first, on the main stream: its linear memories and the coarse scan need nothing else.  The
   // larger upper levels follow on the copy stream (ordered behind everything already enqueued) and are joined
-  // in front of the upper levels' linear memories (enqueue_stages).
+  // in front of the upper levels' linear memories (enqueue_match).
   const bool fork = d->L > 1;
   if (fork) {
     CU(cudaEventRecord(d->ev_fork.get(), d->stream.get()));
@@ -1326,17 +1352,10 @@ static LevelDev level_dev(const LevelHost& h) {
 }
 
 
-// K1 launch plan: block ranges per level (lowest level first), kernel variant and shared memory.  planes_level >= 0: that
-// level is built in planes mode (column-major H-planes only, no byte linear memories; see spread_planes_block).  low_bytes:
-// the lowest level gets its byte linear memories too (only k_coarse_bytes and the debug getter read them); with_bit_planes:
-// it gets its spread bit-planes (band kernel: CTAs of their own ahead of its byte CTAs, see spread_bits_block).
-struct K1Plan {
-  LinMemParams p;
-  bool band = false;
-  size_t smem = 0;
-  int blocks = 0;
-};
-
+// K1 launch plan.  planes_level >= 0: that level is built in planes mode (column-major H-planes only, no byte linear
+// memories; see spread_planes_block).  low_bytes: the lowest level gets its byte linear memories too (only
+// k_coarse_bytes and the debug getter read them); with_bit_planes: it gets its spread bit-planes (band kernel: CTAs of
+// their own ahead of its byte CTAs, see spread_bits_block).
 static void plan_k1(lm_detector* d, int planes_level, bool low_bytes, bool with_bit_planes, K1Plan& k) {
   LinMemParams& p = k.p;
   memset(&p, 0, sizeof(p));
@@ -1401,14 +1420,6 @@ static void plan_k1(lm_detector* d, int planes_level, bool low_bytes, bool with_
   k.blocks = blocks;
 }
 
-// levels (bit l) whose byte linear memories a K1 launch of this plan leaves unbuilt
-static int k1_stale(const lm_detector* d, const K1Plan& k) {
-  int stale = 0;
-  for (int l = 0; l < d->L; ++l)
-    if (!k.p.lv[l].lm || k.p.lv[l].rp) stale |= 1 << l;
-  return stale;
-}
-
 static int launch_k1(lm_detector* d, const K1Plan& k, int first_block, int n_blocks) {
   if (n_blocks <= 0) return LM_OK;
   LinMemParams p = k.p;
@@ -1419,136 +1430,151 @@ static int launch_k1(lm_detector* d, const K1Plan& k, int first_block, int n_blo
   return LM_OK;
 }
 
-// Which refinement path the current bank / shard / frame size take (see enqueue_stages).
-static bool use_filter(const lm_detector* d) { return d->filter_ok && !d->d_rp.empty() && !d->d_finfo.empty(); }
-static bool use_bits(const lm_detector* d) { return use_filter(d) && d->L == 2; }
-// level built in planes mode by K1, or -1: only when nothing reads that level's byte linear memories
-static int planes_level(const lm_detector* d) { return use_bits(d) && d->shard_all_eligible ? d->L - 2 : -1; }
-// the lowest level's byte linear memories are built only for the byte-wise coarse scan (the refinement starts a level up)
-static bool low_bytes(const lm_detector* d) { return d->n_items_bytes > 0; }
+// The frame's routes (FramePlan), from the bank, shard, frame size, gate and exchange the prepare steps left.
+static void plan_frame(lm_detector* d) {
+  FramePlan& pl = d->chain.plan;
+  pl.gated = d->gate_on;
+  pl.exchange = d->px_rank >= 0;
+  pl.filter = d->filter_ok && !d->d_rp.empty() && !d->d_finfo.empty();
+  // two pyramid levels: the filtered level is the last one, its survivors are finished bit-sliced (k_refine_bits)
+  pl.bits = pl.filter && d->L == 2;
+  // byte-wise exact refinement: the templates the filter does not take, or every candidate without the bit-sliced pass
+  pl.refine = !pl.bits || !d->shard_all_eligible;
+  pl.bits_publish = pl.bits && !pl.refine;
+  // K1 builds the filtered level as H-planes only when nothing reads its byte linear memories, and the lowest level's
+  // bytes only for the byte-wise coarse scan (the refinement starts a level up)
+  const int planes = pl.bits && !pl.refine ? d->L - 2 : -1;
+  plan_k1(d, planes, d->n_items_bytes > 0, true, pl.k1);
+  pl.planes_level = pl.k1.band ? planes : -1;  // only the band kernel has a planes mode
+  pl.stale = 0;
+  for (int l = 0; l < d->L; ++l)
+    if (!pl.k1.p.lv[l].lm || pl.k1.p.lv[l].rp) pl.stale |= 1 << l;
+  pl.packed = d->n_items_bits > 0;
+  pl.bytes = d->n_items_bytes > 0;
+  pl.scan_fused = pl.packed && !pl.bytes;
+  pl.plane_bytes = ((size_t)d->M * 8 * d->lv[d->L - 1].lbw * 4 + 15) & ~(size_t)15;
+  pl.coarse = pl.packed ? coarse_shape(d->k2_tasks, d->sm_count, pl.plane_bytes) : CoarseShape{};
+}
 
-// Enqueue every GPU stage of one frame on the detector's stream; no host synchronisation.
-static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
+// This rank's block of the current frame slot of the peer exchange.
+static lm_result_header* exchange_block(const lm_detector* d) {
+  return reinterpret_cast<lm_result_header*>(d->px_buf.get() + (size_t)(d->px_seq & 1) * d->h_px.slot_bytes +
+                                             (size_t)d->h_px.rank * d->h_px.block_bytes);
+}
+
+// The block the frame's stages append records to, and its capacity.  Resolved at launch, never recorded: a replay may
+// grow and move the result block.
+struct AppendTarget { lm_result_header* hdr; int32_t capacity; };
+static AppendTarget append_target(const lm_detector* d) {
+  if (d->chain.plan.exchange) return {exchange_block(d), (int32_t)d->px_cap};
+  return {d->d_res, (int32_t)d->res_cap};
+}
+
+// The frame's match up to its candidate offsets, as planned: K1, the depth gate's cell summary, the coarse scan and the
+// scan of its counts, then K1's upper levels.  ev: the run's timing events (null: not timed).  No host synchronisation.
+static int enqueue_match(lm_detector* d, const Event* ev) {
+  const FramePlan& pl = d->chain.plan;
+  const float threshold = d->chain.threshold;
   const int n_work = (int)d->shard_count;
   const LevelHost& low = d->lv[d->L - 1];
   cudaStream_t st = d->stream.get();
-  // fused multi-GPU exchange: k_refine appends into block [frame slot][rank] of every rank's buffer
-  PeerExchange px;
-  memset(&px, 0, sizeof(px));
-  lm_result_header* px_block = nullptr;
-  if (d->px_rank >= 0) {
-    if (refine_only) return fail(LM_E_STATE, "refinement re-run is not available with a connected peer exchange");
-    ++d->px_seq;
-    px = d->h_px;
-    px_block = reinterpret_cast<lm_result_header*>(d->px_buf.get() + (size_t)(d->px_seq & 1) * px.slot_bytes +
-                                                   (size_t)px.rank * px.block_bytes);
+  if (pl.exchange) ++d->px_seq;  // the frame's number, and its slot of the exchange buffer
+  if (ev) CU(cudaEventRecord(ev[0].get(), st));
+  // K1: one launch for every level and modality.  Every live bit-plane word is stored whole each frame (the slack behind
+  // them stays zero from allocation).  With a host upload in flight (upper levels still on the copy stream) the launch
+  // is split: the lowest level now, the levels above it behind the coarse scan, once their images have landed.
+  const K1Plan& k1 = pl.k1;
+  const int k1_done = d->upper_pending ? k1.p.lv[d->L - 1].block_end : k1.blocks;
+  int rc = launch_k1(d, k1, 0, k1_done);
+  if (rc) return rc;
+  if (ev) CU(cudaEventRecord(ev[1].get(), st));
+  // depth gate: the frame's cell summary, ahead of K2
+  DepthGate gate;  // read by the gated launches only
+  if (pl.gated) {
+    gate.cells = d->d_cells.get(); gate.item = d->d_gate_item.get(); gate.before = d->d_gate_before.get();
+    gate.Wd = low.Wd; gate.Hd = low.Hd;
+    const int B = low.T << (d->L - 1);  // s * T_L full-resolution pixels per cell side
+    CU(launch_pdl(k_depth_cells, dim3((unsigned)((low.plane + 7) / 8)), dim3(256), 0, st, (const uint16_t*)d->fe_depth.get(),
+                  d->fe[0].rows, d->fe[0].cols, B, low.Wd, low.Hd, d->d_cells.get(), d->d_gate_before.get()));
+    ++d->launches;
   }
-  if (d->timing && !refine_only) {
-    d->ev = d->tev.data() + LM_TEV * (size_t)(d->timing_runs % (int64_t)(d->tev.size() / LM_TEV));
-    ++d->timing_runs;
+  const AppendTarget out = append_target(d);
+  // K2
+  if (pl.packed) {
+    BitScanGateParams bp;
+    bp.bp = low.d_bp.get(); bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw);
+    bp.lbw = low.lbw; bp.plane = low.plane; bp.nwords = low.nwords;
+    bp.tslot = d->d_tslot.get(); bp.fdesc = d->d_fdesc.get(); bp.k2info = d->d_k2info.get(); bp.work = d->d_work.get();
+    bp.zero_desc = coarse_zero_descriptor(low.T, low.plane);
+    bp.tasks = d->d_k2task.get(); bp.n_full = d->k2_full; bp.n_rem = d->k2_rem; bp.n_tasks = d->k2_tasks;
+    bp.S = d->S; bp.M = d->M; bp.slot_low = (d->L - 1) * d->M;
+    bp.threshold = threshold;
+    bp.mask = d->d_mask.get(); bp.raw = d->d_raw.get(); bp.cnt = d->d_cnt.get();
+    bp.off = pl.scan_fused ? d->d_off.get() : nullptr;
+    bp.n_work = n_work;
+    bp.hdr = out.hdr; bp.capacity = out.capacity;
+    bp.shard = d->shard_index;
+    bp.counters = d->d_counters.get();
+    bp.queue = d->d_queue.get();
+    bp.ticket = reinterpret_cast<int*>(d->d_counters.get() + 3);
+    const CoarseShape& c = pl.coarse;
+    bp.split = c.split;
+    cudaError_t e = cudaSuccess;
+    if (pl.gated) {
+      bp.gate = gate;
+      e = c.smem ? launch_pdl(k_coarse_packed<true, true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp)
+                 : launch_pdl(k_coarse_packed<false, true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
+    } else if (c.smem) {
+      e = launch_pdl(k_coarse_packed<true, false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, static_cast<const BitScanParams&>(bp));
+    } else {
+      e = launch_pdl(k_coarse_packed<false, false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, static_cast<const BitScanParams&>(bp));
+    }
+    if (e != cudaSuccess) return fail(LM_E_CUDA, "k_coarse_packed launch failed: %s", cudaGetErrorString(e));
+    ++d->launches;
   }
-  K1Plan k1;
-  int k1_done = 0;
-  if (!refine_only) {
-    if (d->timing) CU(cudaEventRecord(d->ev[0].get(), st));
-    // K1: one launch for every level and modality.  Every live bit-plane word is stored whole each frame (the slack behind
-    // them stays zero from allocation).  With a host upload in flight (upper levels still on the copy stream) the launch
-    // is split: the lowest level now, the levels above it behind the coarse scan, once their images have landed.
-    plan_k1(d, planes_level(d), low_bytes(d), true, k1);
-    d->lm_stale = k1_stale(d, k1);
-    k1_done = d->upper_pending ? k1.p.lv[d->L - 1].block_end : k1.blocks;
-    int rc1 = launch_k1(d, k1, 0, k1_done);
-    if (rc1) return rc1;
-    if (d->timing) CU(cudaEventRecord(d->ev[1].get(), st));
-    // depth gate: the frame's cell summary, ahead of K2
-    const bool gated = d->chain.gated;
-    DepthGate gate;  // read by the gated launches only
-    if (gated) {
-      gate.cells = d->d_cells.get(); gate.item = d->d_gate_item.get(); gate.before = d->d_gate_before.get();
-      gate.Wd = low.Wd; gate.Hd = low.Hd;
-      const int B = low.T << (d->L - 1);  // s * T_L full-resolution pixels per cell side
-      CU(launch_pdl(k_depth_cells, dim3((unsigned)((low.plane + 7) / 8)), dim3(256), 0, st, (const uint16_t*)d->fe_depth.get(),
-                    d->fe[0].rows, d->fe[0].cols, B, low.Wd, low.Hd, d->d_cells.get(), d->d_gate_before.get()));
-      ++d->launches;
-    }
-    // K2
-    bool scan_fused = false;
-    if (d->n_items_bits > 0) {
-      BitScanGateParams bp;
-      bp.bp = low.d_bp.get(); bp.bp_words = (uint32_t)((size_t)d->M * 8 * low.lbw);
-      bp.lbw = low.lbw; bp.plane = low.plane; bp.nwords = low.nwords;
-      bp.tslot = d->d_tslot.get(); bp.fdesc = d->d_fdesc.get(); bp.k2info = d->d_k2info.get(); bp.work = d->d_work.get();
-      bp.zero_desc = coarse_zero_descriptor(low.T, low.plane);
-      bp.tasks = d->d_k2task.get(); bp.n_full = d->k2_full; bp.n_rem = d->k2_rem; bp.n_tasks = d->k2_tasks;
-      bp.S = d->S; bp.M = d->M; bp.slot_low = (d->L - 1) * d->M;
-      bp.threshold = threshold;
-      bp.mask = d->d_mask.get(); bp.raw = d->d_raw.get(); bp.cnt = d->d_cnt.get();
-      const bool fuse_scan = d->n_items_bytes == 0;
-      scan_fused = fuse_scan;
-      bp.off = fuse_scan ? d->d_off.get() : nullptr;
-      bp.n_work = n_work;
-      bp.hdr = px.world > 0 ? px_block : d->d_res;
-      bp.capacity = (int)(px.world > 0 ? d->px_cap : d->res_cap);
-      bp.shard = d->shard_index;
-      bp.counters = d->d_counters.get();
-      bp.queue = d->d_queue.get();
-      bp.ticket = reinterpret_cast<int*>(d->d_counters.get() + 3);
-      const size_t plane_bytes = ((size_t)bp.bp_words * 4 + 15) & ~(size_t)15;
-      const CoarseShape c = coarse_shape(d->k2_tasks, d->sm_count, plane_bytes);
-      bp.split = c.split;
-      cudaError_t e = cudaSuccess;
-      if (gated) {
-        bp.gate = gate;
-        e = c.smem ? launch_pdl(k_coarse_packed<true, true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp)
-                   : launch_pdl(k_coarse_packed<false, true>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, bp);
-      } else if (c.smem) {
-        e = launch_pdl(k_coarse_packed<true, false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, static_cast<const BitScanParams&>(bp));
-      } else {
-        e = launch_pdl(k_coarse_packed<false, false>, dim3(c.grid), dim3(c.wpc * 32), c.smem_bytes, st, static_cast<const BitScanParams&>(bp));
-      }
-      if (e != cudaSuccess) return fail(LM_E_CUDA, "k_coarse_packed launch failed: %s", cudaGetErrorString(e));
-      ++d->launches;
-    }
-    if (d->n_items_bytes > 0) {
-      ByteScanGateParams sp;
-      sp.lv = level_dev(low);
-      sp.tslot = d->d_tslot.get(); sp.fbase = d->d_fbase.get(); sp.fxy = d->d_fxy.get(); sp.work = d->d_work.get();
-      sp.items = d->d_items_bytes.get();
-      sp.S = d->S; sp.M = d->M; sp.slot_low = (d->L - 1) * d->M; sp.nwords = low.nwords;
-      sp.threshold = threshold;
-      sp.mask = d->d_mask.get(); sp.raw = d->d_raw.get(); sp.cnt = d->d_cnt.get();
-      int bs = ((low.plane + 3) / 4 + 31) / 32 * 32;
-      bs = std::max(32, std::min(bs, 1024));
-      if (gated) {
-        sp.gate = gate;
-        CU(launch_pdl(k_coarse_bytes<true>, dim3(d->n_items_bytes), dim3(bs), 0, st, sp));
-      } else CU(launch_pdl(k_coarse_bytes<false>, dim3(d->n_items_bytes), dim3(bs), 0, st, static_cast<const ByteScanParams&>(sp)));
-      ++d->launches;
-    }
-    if (d->timing) CU(cudaEventRecord(d->ev[2].get(), st));
-    if (!scan_fused) {
-      CU(launch_pdl(k_scan_counts, dim3(1), dim3(1024), 0, st, d->d_cnt.get(), d->d_off.get(), n_work,
-                    px.world > 0 ? px_block : d->d_res, (int)(px.world > 0 ? d->px_cap : d->res_cap), d->shard_index,
-                    d->d_counters.get(), d->d_queue.get()));
-      ++d->launches;
-    }
-    if (d->timing) CU(cudaEventRecord(d->ev[3].get(), st));
-    if (k1_done < k1.blocks) {  // the upper levels' linear memories, behind their images
-      CU(cudaStreamWaitEvent(st, d->ev_upper.get(), 0));
-      int rc2 = launch_k1(d, k1, k1_done, k1.blocks - k1_done);
-      if (rc2) return rc2;
-    }
-    d->upper_pending = false;
+  if (pl.bytes) {
+    ByteScanGateParams sp;
+    sp.lv = level_dev(low);
+    sp.tslot = d->d_tslot.get(); sp.fbase = d->d_fbase.get(); sp.fxy = d->d_fxy.get(); sp.work = d->d_work.get();
+    sp.items = d->d_items_bytes.get();
+    sp.S = d->S; sp.M = d->M; sp.slot_low = (d->L - 1) * d->M; sp.nwords = low.nwords;
+    sp.threshold = threshold;
+    sp.mask = d->d_mask.get(); sp.raw = d->d_raw.get(); sp.cnt = d->d_cnt.get();
+    int bs = ((low.plane + 3) / 4 + 31) / 32 * 32;
+    bs = std::max(32, std::min(bs, 1024));
+    if (pl.gated) {
+      sp.gate = gate;
+      CU(launch_pdl(k_coarse_bytes<true>, dim3(d->n_items_bytes), dim3(bs), 0, st, sp));
+    } else CU(launch_pdl(k_coarse_bytes<false>, dim3(d->n_items_bytes), dim3(bs), 0, st, static_cast<const ByteScanParams&>(sp)));
+    ++d->launches;
   }
-  if (refine_only) {
-    CU(cudaMemsetAsync(d->d_counters.get(), 0, 8 * sizeof(unsigned long long), st));  // [3] (the coarse scan's ticket) is 0 between launches
-    CU(cudaMemsetAsync(d->d_queue.get(), 0, 4 * sizeof(int), st));
-    CU(cudaMemsetAsync(&d->d_res->count, 0, sizeof(int32_t), st));
+  if (ev) CU(cudaEventRecord(ev[2].get(), st));
+  if (!pl.scan_fused) {
+    CU(launch_pdl(k_scan_counts, dim3(1), dim3(1024), 0, st, d->d_cnt.get(), d->d_off.get(), n_work, out.hdr, (int)out.capacity,
+                  d->shard_index, d->d_counters.get(), d->d_queue.get()));
+    ++d->launches;
   }
-  const bool filter = use_filter(d);
-  // two pyramid levels: the filtered level is the last one, its survivors are finished bit-sliced (k_refine_bits)
-  const bool bits_mode = use_bits(d);
-  const LevelHost& lref = d->lv[d->L >= 2 ? d->L - 2 : 0];
+  if (ev) CU(cudaEventRecord(ev[3].get(), st));
+  if (k1_done < k1.blocks) {  // the upper levels' linear memories, behind their images
+    CU(cudaStreamWaitEvent(st, d->ev_upper.get(), 0));
+    rc = launch_k1(d, k1, k1_done, k1.blocks - k1_done);
+    if (rc) return rc;
+  }
+  d->upper_pending = false;
+  return LM_OK;
+}
+
+// The frame's refinement, as planned: candidate list, filter, exact passes, the exchange's collector.  An overflow replay
+// runs it again (the coarse outputs are still in place) with ev null, so lm_stage_times covers a frame's first pass.
+static int enqueue_refine(lm_detector* d, const Event* ev) {
+  const FramePlan& pl = d->chain.plan;
+  const float threshold = d->chain.threshold;
+  const int n_work = (int)d->shard_count;
+  const LevelHost& low = d->lv[d->L - 1];
+  const int lr = d->L >= 2 ? d->L - 2 : 0;
+  const LevelHost& lref = d->lv[lr];
+  cudaStream_t st = d->stream.get();
+  const AppendTarget out = append_target(d);
   {
     // ordered candidate list (+ the filter's H-planes of the first refined level)
     PrepParams pp;
@@ -1557,8 +1583,8 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     pp.cand = d->d_cand.get(); pp.cand_cap = (int)cand_cap(d);
     pp.expand_blocks = std::max(1, std::min((n_work + 7) / 8, d->sm_count * 8));
     // H- and N-planes from the byte linear memories, or, after K1 in planes mode, N from K1's H-planes (eight labels a thread)
-    pp.rp = filter ? d->d_rp.get() : nullptr;
-    pp.lm = (d->lm_stale >> (d->L >= 2 ? d->L - 2 : 0)) & 1 ? nullptr : lref.d_lm.get();
+    pp.rp = pl.filter ? d->d_rp.get() : nullptr;
+    pp.lm = (pl.stale >> lr) & 1 ? nullptr : lref.d_lm.get();
     pp.Wd = lref.Wd; pp.Hd = lref.Hd; pp.plane = lref.plane; pp.nyb = d->rp_nyb; pp.n_off = d->rp_noff;
     pp.t2 = lref.T * lref.T;
     pp.n_pb = d->M * 8 * pp.t2;
@@ -1567,8 +1593,8 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     CU(launch_pdl(k_refine_prep, dim3((unsigned)(pp.expand_blocks + plane_blocks)), dim3(256), 0, st, pp));
     ++d->launches;
   }
-  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[4].get(), st));
-  if (filter) {
+  if (ev) CU(cudaEventRecord(ev[4].get(), st));
+  if (pl.filter) {
     FilterParams fp;
     fp.rp = d->d_rp.get(); fp.Wd = lref.Wd; fp.nyb = d->rp_nyb;
     fp.rdesc = d->d_rdesc.get(); fp.rfeat = d->d_rfeat.get(); fp.finfo = d->d_finfo.get(); fp.flags = d->d_safe.get();
@@ -1576,13 +1602,12 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     fp.low = level_dev(low); fp.ref = level_dev(lref);
     fp.cand = d->d_cand.get(); fp.off = d->d_off.get(); fp.n_work = n_work; fp.cand_cap = (int)cand_cap(d);
     fp.threshold = threshold;
-    fp.surv = d->d_surv.get(); fp.surv2 = bits_mode ? d->d_surv2.get() : nullptr; fp.queue = d->d_queue.get(); fp.counters = d->d_counters.get();
+    fp.surv = d->d_surv.get(); fp.surv2 = pl.bits ? d->d_surv2.get() : nullptr; fp.queue = d->d_queue.get(); fp.counters = d->d_counters.get();
     CU(launch_pdl(k_refine_filter_w, dim3((unsigned)(d->sm_count * LM_FILTER_MIN_CTAS)), dim3(256), 0, st, fp));
     ++d->launches;
   }
-  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[5].get(), st));
-  const bool bytes_pass = !bits_mode || !d->shard_all_eligible;  // byte-wise exact refinement needed for this shard
-  if (bits_mode) {
+  if (ev) CU(cudaEventRecord(ev[5].get(), st));
+  if (pl.bits) {
     // exact refinement of the survivors, bit-sliced, from the same H-planes
     RefineBitsParams bq;
     bq.rp = d->d_rp.get(); bq.Wd = lref.Wd; bq.n_off = d->rp_noff;
@@ -1592,10 +1617,9 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     bq.surv = d->d_surv.get(); bq.queue = d->d_queue.get();
     bq.threshold = threshold;
     bq.work_begin = (int)d->work_base; bq.work_stride = (int)d->work_stride;
-    bq.hdr = px.world > 0 ? px_block : d->d_res;
-    bq.capacity = (int32_t)(px.world > 0 ? d->px_cap : d->res_cap);
-    bq.px = px.world > 0 ? d->d_px.get() : nullptr; bq.px_seq = d->px_seq;
-    bq.publish = bytes_pass ? 0 : 1;
+    bq.hdr = out.hdr; bq.capacity = out.capacity;
+    bq.px = pl.exchange ? d->d_px.get() : nullptr; bq.px_seq = d->px_seq;
+    bq.publish = pl.bits_publish ? 1 : 0;
     bq.counters = d->d_counters.get();
     if (d->bits_grid == 0) {  // one wave: the survivors are dealt over the CTAs that are resident at once
       int per_sm = 0;
@@ -1605,43 +1629,39 @@ static int enqueue_stages(lm_detector* d, float threshold, bool refine_only) {
     CU(launch_pdl(k_refine_bits, dim3((unsigned)d->bits_grid), dim3(256), 0, st, bq));
     ++d->launches;
   }
-  if (bytes_pass) {
+  if (pl.refine) {
     // persistent grid: the candidate total is read on the device (no host round trip)
     RefineParams rp;
     for (int l = 0; l < d->L; ++l) rp.lv[l] = level_dev(d->lv[l]);
     rp.tslot = d->d_tslot.get(); rp.fbase = d->d_fbase.get(); rp.fxy = d->d_fxy.get(); rp.work = d->d_work.get();
     rp.off = d->d_off.get(); rp.cand = d->d_cand.get(); rp.cand_cap = (int)cand_cap(d); rp.raw = d->d_raw.get();
-    rp.surv = filter ? (bits_mode ? d->d_surv2.get() : d->d_surv.get()) : nullptr; rp.queue = d->d_queue.get();
-    rp.surv_slot = bits_mode ? 2 : 1;
+    rp.surv = pl.filter ? (pl.bits ? d->d_surv2.get() : d->d_surv.get()) : nullptr; rp.queue = d->d_queue.get();
+    rp.surv_slot = pl.bits ? 2 : 1;
     rp.publish = 1;
     rp.n_work = n_work; rp.L = d->L; rp.S = d->S; rp.M = d->M;
     rp.work_begin = (int)d->work_base;
     rp.work_stride = (int)d->work_stride;
     rp.threshold = threshold;
-    rp.hdr = d->d_res; rp.capacity = (int32_t)d->res_cap;
-    rp.px = px.world > 0 ? d->d_px.get() : nullptr;
+    rp.hdr = out.hdr; rp.capacity = out.capacity;
+    rp.px = pl.exchange ? d->d_px.get() : nullptr;
     rp.px_seq = d->px_seq;
-    if (px.world > 0) {
-      rp.hdr = px_block;
-      rp.capacity = (int32_t)d->px_cap;
-    }
     rp.counters = d->d_counters.get();
     rp.safe = d->d_safe.get(); rp.galign = d->d_galign.get();
     // 4 CTAs are resident per SM (64 registers x 256 threads); 16 per SM = four waves of equal shares, which
     // balances the very uneven per-candidate cost (row-wise early exit) better than one persistent wave
     // (measured: 4 -> 251 us, 8 -> 241, 12..32 -> 229)
     // behind the filter the work items are its few survivors: four warps share one (k_refine<true>)
-    if (filter) CU(launch_pdl(k_refine<true>, dim3(d->sm_count * 16), dim3(256), 0, st, rp));
+    if (pl.filter) CU(launch_pdl(k_refine<true>, dim3(d->sm_count * 16), dim3(256), 0, st, rp));
     else CU(launch_pdl(k_refine<false>, dim3(d->sm_count * 16), dim3(256), 0, st, rp));
     ++d->launches;
   }
-  if (px.world > 0) {
+  if (pl.exchange) {
     // collector: waits for all ranks' frame flags, packs the blocks into the ordinary result block
-    CU(launch_pdl(k_peer_collect, dim3(1), dim3(1024), 0, st, px, d->px_seq, (int32_t)d->px_cap, d->d_res, (int32_t)d->res_cap,
+    CU(launch_pdl(k_peer_collect, dim3(1), dim3(1024), 0, st, d->h_px, d->px_seq, (int32_t)d->px_cap, d->d_res, (int32_t)d->res_cap,
                   d->d_counters.get() + 2, d->px_timeout_ns));
     ++d->launches;
   }
-  if (d->timing && !refine_only) CU(cudaEventRecord(d->ev[6].get(), st));
+  if (ev) CU(cudaEventRecord(ev[6].get(), st));
   return LM_OK;
 }
 
@@ -1709,8 +1729,12 @@ static int grow_and_replay(lm_detector* d, int64_t kept, int64_t cands) {
   // the header the coarse scan wrote, with the new capacity
   const lm_result_header hdr = {0, (int32_t)cands, (int32_t)d->res_cap, d->shard_index};
   CU(cudaMemcpy(d->d_res, &hdr, sizeof(hdr), cudaMemcpyHostToDevice));
+  cudaStream_t st = d->stream.get();
+  CU(cudaMemsetAsync(d->d_counters.get(), 0, 8 * sizeof(unsigned long long), st));  // [3] (the coarse scan's ticket) is 0 between launches
+  CU(cudaMemsetAsync(d->d_queue.get(), 0, 4 * sizeof(int), st));
+  CU(cudaMemsetAsync(&d->d_res->count, 0, sizeof(int32_t), st));
   const FrameChain& c = d->chain;
-  rc = enqueue_stages(d, c.threshold, true);
+  rc = enqueue_refine(d, nullptr);
   if (!rc && c.post) rc = enqueue_post(d, c.iou, c.top_k);
   if (!rc && c.pose) rc = enqueue_pose(d);
   if (!rc && c.pose_nms) rc = enqueue_pose_nms(d);
@@ -1757,50 +1781,40 @@ static int complete_frame(lm_detector* d, bool post, bool survivors) {
   }
 }
 
-extern "C" int lm_enqueue(lm_detector* d, float threshold) {
-  if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
-  if (!d) return fail(LM_E_INVALID, "null detector");
-  if (!d->have_frame) return fail(LM_E_STATE, "no frame uploaded");
-  if (d->S == 0) return fail(LM_E_STATE, "no template bank loaded");
-  CU(cudaSetDevice(d->device));
-  int rc = prepare_bank(d);
-  if (rc) return rc;
-  rc = prepare_work(d);
-  if (rc) return rc;
-  rc = ensure_run_buffers(d);
-  if (rc) return rc;
-  if (d->gate_on) {
-    bool any_z = false;
-    for (float z : d->tdepth) any_z = any_z || z > 0.f;
-    if (!any_z) return fail(LM_E_STATE, "depth gate on, but no template of the bank has a training distance (lm_set_template_depths)");
-    if (!d->frame_depth)
-      return fail(LM_E_STATE, "depth gate on, but the frame has no depth image (lm_upload_quantized / lm_bind_quantized_device)");
-    rc = prepare_gate(d);
-    if (rc) return rc;
-  }
-  d->chain.gated = d->gate_on;
-  d->chain.threshold = threshold;
-  rc = filter_thresholds(d, threshold);
-  if (rc) return rc;
-  return enqueue_stages(d, threshold, false);
-}
-
-extern "C" int lm_prepare(lm_detector* d) {
+// The lazy host steps of a run, in this order: feature addresses for the frame size, the shard's work lists, the run
+// buffers, then the depth gate's tables (refused when the gate has nothing to gate by).  lm_prepare takes them ahead of
+// the first frame, lm_enqueue before each one.
+static int prepare_run(lm_detector* d) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d) return fail(LM_E_INVALID, "null detector");
   if (!d->have_frame) return fail(LM_E_STATE, "no frame uploaded (the frame size decides the feature addresses)");
   if (d->S == 0) return fail(LM_E_STATE, "no template bank loaded");
   CU(cudaSetDevice(d->device));
   int rc = prepare_bank(d);
-  if (rc) return rc;
-  rc = prepare_work(d);
-  if (rc) return rc;
-  if (d->gate_on) {
-    rc = prepare_gate(d);
-    if (rc) return rc;
-  }
-  return ensure_run_buffers(d);
+  if (!rc) rc = prepare_work(d);
+  if (!rc) rc = ensure_run_buffers(d);
+  if (rc || !d->gate_on) return rc;
+  if (std::none_of(d->tdepth.begin(), d->tdepth.end(), [](float z) { return z > 0.f; }))
+    return fail(LM_E_STATE, "depth gate on, but no template of the bank has a training distance (lm_set_template_depths)");
+  if (!d->frame_depth)
+    return fail(LM_E_STATE, "depth gate on, but the frame has no depth image (lm_upload_quantized / lm_bind_quantized_device)");
+  return prepare_gate(d);
 }
+
+extern "C" int lm_enqueue(lm_detector* d, float threshold) {
+  int rc = prepare_run(d);
+  if (rc) return rc;
+  d->chain.threshold = threshold;
+  rc = filter_thresholds(d, threshold);
+  if (rc) return rc;
+  plan_frame(d);
+  // the run's timing events: the next slot of the ring (null: not timed)
+  const Event* ev = d->timing ? d->tev.data() + LM_TEV * (size_t)(d->timing_runs++ % (int64_t)(d->tev.size() / LM_TEV)) : nullptr;
+  rc = enqueue_match(d, ev);
+  return rc ? rc : enqueue_refine(d, ev);
+}
+
+extern "C" int lm_prepare(lm_detector* d) { return prepare_run(d); }
 
 extern "C" int lm_complete(lm_detector* d) {
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
@@ -2397,19 +2411,10 @@ extern "C" int lm_set_depth_gate(lm_detector* d, int on, double tolerance) {
   return LM_OK;
 }
 
-// The result header the last frame's coarse scan wrote (its shard's candidate count): this rank's block of the frame slot
-// with a connected exchange, else the result block (a result-block retry carries the header over to the grown block).
-static const lm_result_header* scan_header(const lm_detector* d) {
-  if (d->px_rank >= 0)
-    return reinterpret_cast<const lm_result_header*>(d->px_buf.get() + (size_t)(d->px_seq & 1) * d->h_px.slot_bytes +
-                                                     (size_t)d->h_px.rank * d->h_px.block_bytes);
-  return d->d_res;
-}
-
 extern "C" int lm_depth_gate_stats(lm_detector* d, int64_t* out4) {
   if (!d || !out4) return fail(LM_E_INVALID, "null argument");
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
-  if (!d->chain.gated || !d->d_res) return fail(LM_E_STATE, "the last frame did not run with the depth gate");
+  if (!d->chain.plan.gated || !d->d_res) return fail(LM_E_STATE, "the last frame did not run with the depth gate");
   CU(cudaSetDevice(d->device));
   const LevelHost& low = d->lv[d->L - 1];
   std::vector<uint32_t> cells((size_t)low.plane);
@@ -2417,7 +2422,9 @@ extern "C" int lm_depth_gate_stats(lm_detector* d, int64_t* out4) {
   lm_result_header hdr;
   CU(cudaMemcpyAsync(cells.data(), d->d_cells.get(), sizeof(uint32_t) * cells.size(), cudaMemcpyDeviceToHost, d->stream.get()));
   CU(cudaMemcpyAsync(&before, d->d_gate_before.get(), sizeof(unsigned), cudaMemcpyDeviceToHost, d->stream.get()));
-  CU(cudaMemcpyAsync(&hdr, scan_header(d), sizeof(hdr), cudaMemcpyDeviceToHost, d->stream.get()));
+  // the header the coarse scan wrote, with its shard's candidate count (a result-block retry carries it to the grown block)
+  const lm_result_header* scan = d->px_rank >= 0 ? exchange_block(d) : d->d_res;
+  CU(cudaMemcpyAsync(&hdr, scan, sizeof(hdr), cudaMemcpyDeviceToHost, d->stream.get()));
   CU(cudaStreamSynchronize(d->stream.get()));
   int64_t empty = 0;
   for (uint32_t c : cells) empty += (c & 0xFFFFu) > (c >> 16);
@@ -2598,7 +2605,7 @@ extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality,
   const LevelHost& lv = d->lv[level];
   if ((int64_t)lv.mod_stride > cap) return fail(LM_E_CAPACITY, "need %u bytes", lv.mod_stride);
   CU(cudaSetDevice(d->device));
-  if ((d->lm_stale >> level) & 1) {
+  if ((d->chain.plan.stale >> level) & 1) {
     // the last run did not build this level's bytes (H-planes only, or a lowest level nothing read them from): build them
     // now, from the frame that is still bound, without touching the bit-planes
     K1Plan k;
@@ -2606,7 +2613,7 @@ extern "C" int lm_debug_linear_memories(lm_detector* d, int level, int modality,
     const int b0 = level == d->L - 1 ? 0 : k.p.lv[level + 1].block_end;
     int rc = launch_k1(d, k, b0, k.p.lv[level].block_end - b0);
     if (rc) return rc;
-    d->lm_stale &= ~(1 << level);
+    d->chain.plan.stale &= ~(1 << level);
   }
   CU(cudaMemcpyAsync(out, lv.d_lm.get() + (size_t)modality * lv.mod_stride, lv.mod_stride, cudaMemcpyDeviceToHost, d->stream.get()));
   CU(cudaStreamSynchronize(d->stream.get()));
@@ -2633,8 +2640,7 @@ extern "C" int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us) 
   if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
   if (level < -1 || level >= d->L || reps < 1) return fail(LM_E_INVALID, "bad level/reps");
   CU(cudaSetDevice(d->device));
-  K1Plan k;
-  plan_k1(d, planes_level(d), low_bytes(d), true, k);
+  const K1Plan& k = d->chain.plan.k1;
   const int b0 = level < 0 || level == d->L - 1 ? 0 : k.p.lv[level + 1].block_end;
   const int b1 = level < 0 ? k.blocks : k.p.lv[level].block_end;
   Event e0, e1;
@@ -2653,9 +2659,9 @@ extern "C" int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us) 
   return LM_OK;
 }
 
-// The routes of the last lm_run, restated from the host state enqueue_stages decided them from (plan_k1, coarse_shape,
-// use_filter / use_bits); only the survivor counts of the filter are read back from the device, behind whatever the
-// stream holds (a frame enqueued since the last lm_complete would be waited for and reported: see the header).
+// The last frame's routes as its plan recorded them, beside the shard's and the frame size's figures the prepare steps
+// left; only the survivor counts of the filter are read back from the device, behind whatever the stream holds (a frame
+// enqueued since the last lm_complete would be waited for and reported: see the header).
 extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   if (!d || !out) return fail(LM_E_INVALID, "null argument");
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
@@ -2665,46 +2671,39 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   int queue[4];
   CU(cudaMemcpyAsync(queue, d->d_queue.get(), sizeof(queue), cudaMemcpyDeviceToHost, d->stream.get()));
   CU(cudaStreamSynchronize(d->stream.get()));
+  const FramePlan& pl = d->chain.plan;
   const LevelHost& low = d->lv[d->L - 1];
-  K1Plan k1;
-  plan_k1(d, planes_level(d), low_bytes(d), true, k1);
-  const int pl = k1.band ? planes_level(d) : -1;
   for (int i = 0; i < LM_PLAN_ENTRIES; ++i) out[i] = -1;
-  out[0] = k1.band ? 1 : 0;
-  out[1] = pl;
-  out[2] = pl >= 0 ? k1.p.lv[pl].pseg : 0;
-  out[3] = (int32_t)k1.smem;
+  out[0] = pl.k1.band ? 1 : 0;
+  out[1] = pl.planes_level;
+  out[2] = pl.planes_level >= 0 ? pl.k1.p.lv[pl.planes_level].pseg : 0;
+  out[3] = (int32_t)pl.k1.smem;
   out[4] = low.rounds;
   out[5] = !low.d_bp.empty() ? 1 : 0;
   out[6] = d->n_items_bits;
   out[7] = d->n_items_bytes;
-  if (d->n_items_bits > 0) {
-    const size_t plane_bytes = ((size_t)d->M * 8 * low.lbw * 4 + 15) & ~(size_t)15;
-    const CoarseShape c = coarse_shape(d->k2_tasks, d->sm_count, plane_bytes);
-    out[8] = c.smem ? 1 : 0;
-    out[9] = c.split;
-    out[10] = (int32_t)plane_bytes;
+  if (pl.packed) {
+    out[8] = pl.coarse.smem ? 1 : 0;
+    out[9] = pl.coarse.split;
+    out[10] = (int32_t)pl.plane_bytes;
     out[11] = d->k2_tasks;
   }
   out[12] = d->filter_ok ? 1 : 0;
-  out[13] = use_bits(d) ? 1 : 0;
-  int eligible = 0;
-  for (const int4& f : d->h_finfo) eligible += (f.w & 2) ? 1 : 0;
-  out[14] = eligible;
-  out[15] = d->chain.gated ? 1 : 0;
-  // work items of the refinement kernels that ran (-1: it did not run); see enqueue_stages
+  out[13] = pl.bits ? 1 : 0;
+  out[14] = (int32_t)std::count_if(d->h_finfo.begin(), d->h_finfo.end(), [](const int4& f) { return (f.w & 2) != 0; });
+  out[15] = pl.gated ? 1 : 0;
+  // work items of the refinement kernels that ran (-1: it did not run)
   const int total = (int)std::min<int64_t>(hres(d)->coarse_candidates, cand_cap(d));
-  const bool filter = use_filter(d), bits_mode = use_bits(d);
-  if (filter) out[16] = total;
-  if (bits_mode) {
+  if (pl.filter) out[16] = total;
+  if (pl.bits) {
     out[17] = std::min(queue[1], total);
     out[20] = d->bits_grid;
   }
-  if (!bits_mode || !d->shard_all_eligible) {
-    if (filter) out[18] = std::min(queue[bits_mode ? 2 : 1], total);
+  if (pl.refine) {
+    if (pl.filter) out[18] = std::min(queue[pl.bits ? 2 : 1], total);
     else out[19] = total;
   }
-  const LinMemLevel& kl = k1.p.lv[d->L - 1];
+  const LinMemLevel& kl = pl.k1.p.lv[d->L - 1];
   out[21] = (kl.bp ? 1 : 0) | (kl.lm ? 2 : 0);
   return LM_OK;
 }

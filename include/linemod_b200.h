@@ -155,8 +155,9 @@ int lm_run(lm_detector* d, float threshold);
 int lm_enqueue(lm_detector* d, float threshold);
 int lm_complete(lm_detector* d);
 /* Everything lm_enqueue does lazily on a new bank / selection / frame size (feature addresses for the frame size,
- * shard work lists, run buffers), done now: the first lm_enqueue afterwards only launches.  Needs a frame uploaded or
- * bound (for its size).  SPMD callers use it so that no rank's first frame lags the others'. */
+ * shard work lists, run buffers, the depth gate's tables), done now, with lm_enqueue's checks: the first lm_enqueue
+ * afterwards only launches.  Needs a frame uploaded or bound (for its size).  SPMD callers use it so that no rank's
+ * first frame lags the others'. */
 int lm_prepare(lm_detector* d);
 /* The bit-sliced coarse scan's plan for one shard, as lm_prepare builds it (host only, no device needed).  words[i] =
  * position words of item i (ceil(P / 32) clamped to 1..nwords; P = template_positions at the lowest level).
@@ -464,7 +465,7 @@ int lm_match_images(lm_detector* d, const uint8_t* rgb, const uint16_t* depth, i
  *   lm_set_depth_gate       on != 0 turns the gate on with `tolerance` (tau), for the next lm_enqueue (single frame or
  *                           batch); no device work, and a frame keeps the setting it was enqueued with (the rerun after a
  *                           result-block retry included).  LM_E_INVALID for tolerance < 0, >= 1 or NaN.  With the gate on,
- *                           lm_enqueue fails with LM_E_STATE when no template of the bank has a distance, or when the
+ *                           lm_enqueue and lm_prepare fail with LM_E_STATE when no template of the bank has a distance, or when the
  *                           frame has no depth (lm_upload_quantized / lm_bind_quantized_device).  With a connected peer
  *                           exchange, every rank setting the same distances and gate before its next frame is the caller's
  *                           promise, as with lm_peer_share_pose: each rank gates its own shard on its own copy of the frame.
@@ -490,11 +491,11 @@ int lm_debug_linear_memories(lm_detector* d, int level, int modality, uint8_t* o
  * smaller; out may be null with cap 0).  Synchronises the stream. */
 int lm_debug_bit_planes(lm_detector* d, uint32_t* out, int64_t cap, int64_t* n_words);
 /* Development probe: the mean device time in microseconds of `reps` back-to-back launches of the K1 blocks of one level
- * (level -1: the whole launch), planned as the last lm_run planned them, rebuilding that frame's outputs in place.
+ * (level -1: the whole launch), from the K1 plan the last frame recorded, rebuilding that frame's outputs in place.
  * Synchronises the stream.  LM_E_STATE before the first lm_run. */
 int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us);
-/* Test getter: which kernels and launch shapes the last lm_run took, restated from the host state the frame was
- * enqueued from (no launch; one small read of the filter's survivor counts).  LM_PLAN_ENTRIES int32 entries:
+/* Test getter: which kernels and launch shapes the last lm_run took, as the frame's plan recorded them when it was
+ * enqueued (no launch; one small read of the filter's survivor counts).  LM_PLAN_ENTRIES int32 entries:
  * [0] linear memories by k_linear_memories_band (1) or k_linear_memories (0), [1] level built as H-planes only (-1:
  * none), [2] its positions per segment (pseg; 0: none), [3] the band kernel's shared memory (bytes), [4] rounds of
  * 32 x 32 position words at the lowest level, [5] its spread bit-planes are allocated (1/0), [6] templates on
@@ -505,10 +506,9 @@ int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us);
  * [16] k_refine_filter_w, [17] k_refine_bits, [18] k_refine<true>, [19] k_refine<false> (-1: it did not run), [20] the
  * CTAs k_refine_bits runs with (the ones resident at once; -1: it did not run), [21] what K1 builds of the lowest level:
  * bit 0 its spread bit-planes, bit 1 its byte linear memories (built only when k_coarse_bytes has templates).
- * Describes the last completed frame only between lm_complete (or lm_run) and the next lm_enqueue, and while the bank,
- * the selection, the frame size and the gate stay as they were: the routes are restated from the current host state, and
- * the survivor counts are read from the device when the getter is called, so after a later lm_enqueue the getter waits
- * for that frame and reports its counts. */
+ * Describes the last completed frame only between lm_complete (or lm_run) and the next lm_enqueue, which records its own
+ * frame's plan; the survivor counts are read from the device when the getter is called, so after a later lm_enqueue the
+ * getter waits for that frame and reports its counts. */
 #define LM_PLAN_ENTRIES 22
 int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap);
 /* Test getter: the coarse scan's outputs (k_coarse_packed / k_coarse_bytes) of the last completed frame, per work item of
