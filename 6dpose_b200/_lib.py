@@ -37,6 +37,7 @@ SYMBOLS = [
     "lm_pose_stats", "lm_set_pose_estimation", "lm_set_template_depths", "lm_set_depth_gate", "lm_depth_gate_stats",
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
     "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture", "lm_icp_process_batch_device",
+    "lm_set_pose_verify", "lm_pose_verify", "lm_pose_verify_points", "lm_icp_set_verify", "lm_icp_verify",
 ]
 
 # The ICP's estimation step (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT of include/linemod_b200.h) by the name the
@@ -49,6 +50,48 @@ def estimation_code(estimation):
     if not isinstance(estimation, str) or estimation not in ESTIMATIONS:
         raise ValueError("estimation must be one of %s, got %r" % (", ".join(repr(k) for k in ESTIMATIONS), estimation))
     return ESTIMATIONS[estimation]
+
+
+# Pose verification (lm_set_pose_verify): the pose NMS's ranking by the name the Python surface takes, and the names of
+# the six counts
+VERIFY_RANKS = {"fitness": 0, "score": 1}
+VERIFY_COUNTS = ("n_model", "outside", "missing", "inlier", "occluded", "violation")
+
+
+def _real(v, what):
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)):
+        raise TypeError("%s must be a number, got %s" % (what, type(v).__name__))
+    return float(v)
+
+
+def inlier_mm(v):
+    """The verification's inlier distance delta (mm) as a float: finite and >= 0, else ValueError (no device work)."""
+    d = _real(v, "inlier_mm")
+    if not (math.isfinite(d) and d >= 0.0):
+        raise ValueError("inlier_mm must be finite and >= 0, got %r" % v)
+    return d
+
+
+def verify_options(inlier, rank_by="fitness", min_score=None):
+    """lm_set_pose_verify's (on, inlier_mm, rank_by, min_score) for Detector.setPoseVerification; inlier None turns
+    verification off, which takes neither rank_by="score" nor a min_score.  ValueError / TypeError before any device work."""
+    if not isinstance(rank_by, str) or rank_by not in VERIFY_RANKS:
+        raise ValueError("rank_by must be one of %s, got %r" % (", ".join(repr(k) for k in VERIFY_RANKS), rank_by))
+    lo = -math.inf
+    if min_score is not None:
+        lo = _real(min_score, "min_score")
+        if math.isnan(lo):
+            raise ValueError("min_score is NaN")
+    if inlier is None:
+        if rank_by != "fitness" or min_score is not None:
+            raise ValueError("rank_by=\"score\" and min_score need pose verification on (inlier_mm not None)")
+        return 0, 10.0, 0, -math.inf
+    return 1, inlier_mm(inlier), VERIFY_RANKS[rank_by], lo
+
+
+def verify_arrays(score, counts):
+    """[(score, {count name: value})] of lm_pose_verify's / lm_icp_verify's outputs."""
+    return [(float(s), dict(zip(VERIFY_COUNTS, (int(v) for v in c)))) for s, c in zip(score.tolist(), counts)]
 
 
 def depth_gate_tolerance(tolerance):
@@ -361,6 +404,11 @@ def load():
     L.lm_debug_plan.argtypes = [vp, i32p, c_i64]
     L.lm_debug_coarse.argtypes = [vp, ctypes.POINTER(ctypes.c_uint32), c_i64, u16p, c_i64, i32p]
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
+    L.lm_set_pose_verify.argtypes = [vp, c_int, ctypes.c_double, c_int, ctypes.c_double]
+    L.lm_pose_verify.argtypes = [vp, f32p, i32p, c_i64, ctypes.POINTER(c_i64)]
+    L.lm_pose_verify_points.argtypes = [c_int, f64p, c_i64, f64p, u16p, c_int, c_int, f32p, ctypes.c_double, i32p, f32p]
+    L.lm_icp_set_verify.argtypes = [vp, c_int, ctypes.c_double]
+    L.lm_icp_verify.argtypes = [vp, f32p, i32p, c_i64, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
     L.lm_icp_destroy.restype = None
@@ -992,6 +1040,16 @@ class NativeDetector:
     def launch_count(self):
         return int(self._L.lm_launch_count(self._h))
 
+    def set_pose_verify(self, on, inlier_mm=10.0, rank_by=0, min_score=-math.inf):
+        """lm_set_pose_verify for the next pose stage: on, the inlier distance (mm), the pose NMS's ranking (0 fitness, 1
+        score) and its minimum score (-inf: none)."""
+        check(self._L.lm_set_pose_verify(self._h, 1 if on else 0, float(inlier_mm), int(rank_by), float(min_score)))
+
+    def pose_verify(self):
+        """The verification of the last completed frame or batch (lm_pose_verify): (score [n] f32, counts [n,6] int32) in
+        the order of its entries."""
+        return _verify_results(self._L.lm_pose_verify, self._h)
+
     def pose_stats(self):
         """[survivors, hypotheses this rank refined, launches, 1 if shared] of the last completed pose stage (lm_pose_stats)."""
         a = (ctypes.c_int64 * 4)()
@@ -1089,6 +1147,15 @@ class NativeIcp:
         check(self._L.lm_icp_set_estimation(self._h, estimation_code(estimation)))
         self._estimation = estimation
 
+    def set_verify(self, inlier_mm):
+        """Pose verification for the next calls (lm_icp_set_verify): the inlier distance in mm, or None for off."""
+        d = 10.0 if inlier_mm is None else float(inlier_mm)
+        check(self._L.lm_icp_set_verify(self._h, 0 if inlier_mm is None else 1, d))
+
+    def verify(self):
+        """The verification of the last call (lm_icp_verify): (score [n] f32, counts [n,6] int32) per hypothesis."""
+        return _verify_results(self._L.lm_icp_verify, self._h)
+
     def set_capture(self, on):
         check(self._L.lm_icp_set_capture(self._h, 1 if on else 0))
 
@@ -1137,3 +1204,36 @@ def nms_translations(t, score, thr, device=0):
     check(L.lm_nms_translations(int(device), n, t.ctypes.data_as(f64p), score.ctypes.data_as(f64p), float(thr),
                                 keep.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), ctypes.byref(nk)))
     return keep[:nk.value].astype(np.int64)
+
+
+def _verify_results(fn, h):
+    n = ctypes.c_int64()
+    f32p, i32p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int32)
+    rc = fn(h, None, None, 0, ctypes.byref(n))
+    if rc != LM_E_CAPACITY:
+        check(rc)
+    score = np.zeros(n.value, np.float32)
+    counts = np.zeros((n.value, 6), np.int32)
+    if n.value:
+        check(fn(h, score.ctypes.data_as(f32p), counts.ctypes.data_as(i32p), n.value, ctypes.byref(n)))
+    return score, counts
+
+
+def pose_verify_points(pts, T, scene, sceneK, inlier_mm=10.0, device=0):
+    """Steps 3-5 of the pose verification on caller arrays (lm_pose_verify_points): pts [n,3] f64 (m), T [4,4] f64,
+    scene HxW u16 mm, sceneK 3x3 f32.  Returns (score, counts [6] int32)."""
+    L = load()
+    pts = np.ascontiguousarray(pts, np.float64).reshape(-1, 3)
+    T = np.ascontiguousarray(T, np.float64).reshape(16)
+    scene = np.ascontiguousarray(scene)
+    if scene.dtype != np.uint16 or scene.ndim != 2:
+        raise TypeError("scene must be a uint16 HxW depth image (mm)")
+    sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+    counts = np.zeros(6, np.int32)
+    score = ctypes.c_float()
+    f64p = ctypes.POINTER(ctypes.c_double)
+    check(L.lm_pose_verify_points(int(device), pts.ctypes.data_as(f64p), pts.shape[0], T.ctypes.data_as(f64p),
+                                  scene.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), scene.shape[0], scene.shape[1],
+                                  sK.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), float(inlier_mm),
+                                  counts.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), ctypes.byref(score)))
+    return float(score.value), counts

@@ -145,6 +145,7 @@ struct FrameChain {
   bool post = false; double iou = 0.5; int top_k = 0;      // lm_enqueue_post
   bool pose = false; float sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   int max_iter = 30, use_scene = 0, estimation = LM_ICP_POINT_TO_PLANE;  // lm_enqueue_pose
+  PoseVerifyOptions verify = {0, LM_VERIFY_RANK_FITNESS, 10.0, -INFINITY};
   bool pose_nms = false; double nms_thr = 40.0;             // lm_enqueue_pose_nms
 };
 
@@ -247,6 +248,7 @@ struct lm_detector {
   lm_pose_stage* pose = nullptr;
   bool frame_depth = false;             // the frame came from lm_upload_images: fe_depth holds its depth
   int pose_estimation = LM_ICP_POINT_TO_PLANE;  // lm_set_pose_estimation: for the next pose stage
+  PoseVerifyOptions pose_verify = {0, LM_VERIFY_RANK_FITNESS, 10.0, -INFINITY};  // lm_set_pose_verify: likewise
   int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
@@ -2301,7 +2303,7 @@ static int enqueue_pose(lm_detector* d) {
   }
   const FrameChain& c = d->chain;
   PoseRun run;
-  run.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr};
+  run.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr, c.verify};
   run.n_frames = 1; run.first = nullptr; run.d_counts = d->d_post_counts.get();
   run.bound = c.top_k > 0 ? std::min(c.top_k, LM_POST_MAX) : LM_POST_MAX;
   run.d_surv = d->d_post_out.get(); run.d_scene = d->fe_depth.get(); run.sK = c.sK;
@@ -2323,6 +2325,7 @@ extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iter
   c.max_iter = max_iterations;
   c.use_scene = use_scene_cloud ? 1 : 0;
   c.estimation = d->pose_estimation;
+  c.verify = d->pose_verify;
   c.pose_nms = false;  // a new pose stage: any pose NMS enqueued before belongs to an abandoned frame
   int rc = enqueue_pose(d);
   if (rc) return rc;
@@ -2389,6 +2392,24 @@ extern "C" int lm_set_pose_estimation(lm_detector* d, int estimation) {
     return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
   d->pose_estimation = estimation;
   return LM_OK;
+}
+
+extern "C" int lm_set_pose_verify(lm_detector* d, int on, double inlier_mm, int rank_by, double min_score) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (!(std::isfinite(inlier_mm) && inlier_mm >= 0.0)) return fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
+  if (rank_by != LM_VERIFY_RANK_FITNESS && rank_by != LM_VERIFY_RANK_SCORE)
+    return fail(LM_E_INVALID, "unknown rank_by %d (LM_VERIFY_RANK_FITNESS 0, LM_VERIFY_RANK_SCORE 1)", rank_by);
+  if (std::isnan(min_score)) return fail(LM_E_INVALID, "min_score is NaN (-INFINITY: no minimum)");
+  if (!on && (rank_by != LM_VERIFY_RANK_FITNESS || min_score != -INFINITY))
+    return fail(LM_E_INVALID, "rank_by score and min_score need pose verification on");
+  d->pose_verify = {on ? 1 : 0, rank_by, inlier_mm, min_score};
+  return LM_OK;
+}
+
+extern "C" int lm_pose_verify(lm_detector* d, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  if (!d->pose) return fail(LM_E_STATE, "no pose stage has run");
+  return pose_stage_verify(d->pose, score, counts6, cap, n);
 }
 
 extern "C" int lm_set_template_depths(lm_detector* d, int64_t first, int64_t n, const float* z_mm) {
@@ -2488,7 +2509,7 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
   const size_t n0 = (size_t)rows * cols;
   uint16_t* d_scene = nullptr;
   lm_match* d_surv = nullptr;
-  int rc = pose_batch_reserve(d->pose, st, n_frames, (int64_t)n0, (int64_t)n_frames * bound, &d_scene, &d_surv);
+  int rc = pose_batch_reserve(d->pose, st, n_frames, (int64_t)n0, (int64_t)n_frames * bound, d->pose_verify.on != 0, &d_scene, &d_surv);
   if (rc) return rc;
   std::vector<int64_t> first((size_t)n_frames + 1, 0);
   std::vector<lm_match> surv(pose_nms ? 0 : (size_t)n_frames * bound);
@@ -2519,7 +2540,7 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     d->px_pose_seq += pose_batch_chunks(first[n_frames]);
   }
   PoseRun run;
-  run.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr};
+  run.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr, d->pose_verify};
   run.n_frames = n_frames; run.first = first.data(); run.d_counts = nullptr; run.bound = bound;
   run.d_surv = d_surv; run.d_scene = d_scene; run.sK = sceneK;
   run.pose_nms = pose_nms ? 1 : 0;

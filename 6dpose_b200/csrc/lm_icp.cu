@@ -23,7 +23,8 @@
 // one chunk to pose_chunk and to the kernels, told apart by data only: the survivor count on the device, an optional
 // frame table, and the slot rule survivor = rank + slot * world.  lm_icp_process_batch_device feeds the same chunks from
 // renders and a scene in the caller's device memory: k_icp_scene, k_icp_render_box and k_icp_render_crop build the
-// per-hypothesis table k_pose_cloud reads (end of this file).
+// per-hypothesis table k_pose_cloud reads (end of this file).  With verification on (lm_set_pose_verify, lm_icp_set_verify)
+// k_pose_verify follows the ICP kernel of an unshared chunk, and of lm_icp_process_batch, and k_pose_nms<true> reads it.
 
 #include "linemod_b200.h"
 #include "lm_pose.h"
@@ -67,6 +68,12 @@ struct IcpOut {
   double T[16];  // row-major final transformation_
   double fitness, rmse;
   int32_t iterations, pad;
+};
+
+struct PoseVerify {  // one survivor / hypothesis (lm_set_pose_verify)
+  int32_t counts[6];  // n_model, outside, missing, inlier, occluded, violation
+  float score;        // -1: no pose
+  int32_t pad;
 };
 
 // --------------------------------------------------------------------------------------------
@@ -260,8 +267,9 @@ struct PoseShareEntry {  // one survivor: all that pose_stage_finish and k_pose_
   IcpOut out;
   int32_t posed;         // k_pose_cloud's verdict
   int32_t err;           // the owner's cloud-overflow flag (the stage's error is the OR over all ranks)
+  PoseVerify ver;        // the owner's verification (k_pose_verify<true>); zero when the stage does not verify
 };
-static_assert(sizeof(PoseShareEntry) == 160 && sizeof(PoseShareEntry) % 16 == 0, "pose area entry layout");
+static_assert(sizeof(PoseShareEntry) == 192 && sizeof(PoseShareEntry) % 16 == 0, "pose area entry layout");
 
 #define POSE_SHARE_FLAGS ((size_t)2 * POSE_SHARE_SLOTS * sizeof(PoseShareEntry))  // byte offset of the flags in the area
 
@@ -278,10 +286,11 @@ struct PoseShareDev {
   int* abort_flag;
 };
 
-// Thread 0 of the CTA of slot blockIdx.x, after its last pass: the entry of its survivor into the same place of every
-// rank's pose area, then the ticket; the last CTA raises this rank's pose flag everywhere.  The ticket counts CTAs in
-// its low 16 bits and published entries above them.
-__device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const IcpOut& o) {
+// Thread 0 of the CTA of slot blockIdx.x, after its last pass (the ICP kernel's SHARE instantiation, or k_pose_verify's
+// behind the unshared ICP kernel when the stage verifies): the entry of its survivor into the same place of every rank's
+// pose area, then the ticket; the last CTA raises this rank's pose flag everywhere.  The ticket counts CTAs in its low 16
+// bits and published entries above them.
+__device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const IcpOut& o, const PoseVerify& v) {
   const int i = sh.rank + (int)blockIdx.x * sh.world;  // survivor of this slot
   const bool mine = i < sh.counts[0];
   const int slot = sh.seq & 1;
@@ -290,6 +299,7 @@ __device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const
     e.out = o;
     e.posed = sh.posed[blockIdx.x];
     e.err = sh.status[0];
+    e.ver = v;
     const size_t at = ((size_t)slot * POSE_SHARE_SLOTS + i) * sizeof(PoseShareEntry);
     for (int q = 0; q < sh.world; ++q) *reinterpret_cast<PoseShareEntry*>(sh.area[q] + at) = e;
   }
@@ -576,7 +586,7 @@ __device__ __forceinline__ void icp_registration(const IcpJob* __restrict__ jobs
     IcpOut o;
     for (int k = 0; k < 16; ++k) o.T[k] = s_T[k];
     o.fitness = fitness; o.rmse = rmse; o.iterations = it; o.pad = 0;
-    if (SHARE) pose_share_publish(sh, o);
+    if (SHARE) pose_share_publish(sh, o, PoseVerify());
     else outs[blockIdx.x] = o;
   }
 }
@@ -610,8 +620,9 @@ static void launch_icp(int est, unsigned n, cudaStream_t st, const IcpJob* jobs,
 
 // One CTA behind the ICP kernel's SHARE instantiation on each rank's stream: waits (acquire) until every rank's pose flag of the
 // frame has arrived in this rank's pose area, then copies the entries, in survivor order, into the stage's outs / posed.
+// ver (a verifying stage, else null): the entries' verification, in the same order.
 __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShareDev sh, IcpOut* __restrict__ outs,
-                                                                       uint8_t* __restrict__ posed) {
+                                                                       uint8_t* __restrict__ posed, PoseVerify* __restrict__ ver) {
   __shared__ int s_late;
   const int tid = threadIdx.x;
   if (tid == 0) s_late = 0;
@@ -649,6 +660,7 @@ __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShare
     for (int k = 0; k < (int)(sizeof(PoseShareEntry) / 16); ++k) u.v[k] = __ldcv(src + k);  // peers wrote them
     outs[i] = u.e.out;
     posed[i] = (uint8_t)u.e.posed;
+    if (ver) ver[i] = u.e.ver;
     err |= u.e.err;
   }
   err = __syncthreads_or(err);
@@ -689,7 +701,16 @@ struct lm_icp {
     std::vector<int32_t> knn, corr;
   } cap;
   IcpDevice* dev = nullptr;  // created by the first lm_icp_process_batch_device
+  // lm_icp_set_verify, and the verification of the last call's hypotheses (verified false: that call did not verify)
+  bool verify = false;
+  double verify_mm = 10.0;
+  bool verified = false;
+  std::vector<PoseVerify> ver;
+  DeviceArray<uint8_t> d_vbuf;  // the host path's verification inputs and outputs (icp_verify_host)
 };
+
+static int icp_verify_host(lm_icp* h, const std::vector<int>& job_of, const std::vector<std::vector<double>>& raw,
+                           const uint16_t* scene, int srows, int scols, const float* sK);
 
 extern "C" int lm_icp_create(int device, lm_icp** out) {
   if (!out) return lm_fail(LM_E_INVALID, "out is null");
@@ -720,6 +741,7 @@ namespace {
 
 struct Cloud {
   std::vector<double> pts;    // down-sampled model cloud, xyz
+  std::vector<double> raw;    // the model cloud before down-sampling (only kept when asked for)
   std::vector<double> scene;  // down-sampled scene cloud (only built when asked for)
   double init[16];
   float base[16];  // init_base, row-major
@@ -780,7 +802,7 @@ void model_box(const uint16_t* model, int mrows, int mcols, int* box) {
 }
 
 void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* model, int mrows, int mcols, const float* sK,
-                 const float* mK, const float* R, const float* t, int detectX, int detectY, bool want_scene, Cloud& c) {
+                 const float* mK, const float* R, const float* t, int detectX, int detectY, bool want_scene, bool want_raw, Cloud& c) {
   init_base(R, t, c.base);
   const int half = 4;
   int box[4];
@@ -833,6 +855,7 @@ void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* mo
   for (int k = 0; k < 3; ++k) c.init[4 * k + 3] = cs[k] - cm[k];
   voxel_down_sample(mp, c.pts);
   if (want_scene) voxel_down_sample(sp, c.scene);
+  if (want_raw) c.raw = std::move(mp);
 }
 
 // PointCloud::VoxelDownSample(0.0025) (LL.cpp:106-109): mean of the points of every occupied voxel;
@@ -884,6 +907,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
   if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
   CUI(cudaSetDevice(h->device));
+  h->verified = false;
   std::vector<Cloud> clouds((size_t)n_hyp);
   std::vector<IcpJob> jobs;
   std::vector<int> job_of((size_t)n_hyp, -1);
@@ -896,7 +920,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     // NMS survivors of the drivers, linemod_and_levelup_test.py:348-367)
     auto build = [&](int i) {
       build_cloud(scene_depth, srows, scols, model_depths[i], mrows, mcols, sceneK, modelK + 9 * i, R + 9 * i, t + 3 * i,
-                  detect_xy[2 * i], detect_xy[2 * i + 1], h->use_scene_cloud, clouds[i]);
+                  detect_xy[2 * i], detect_xy[2 * i + 1], h->use_scene_cloud, h->verify, clouds[i]);
     };
     std::vector<std::thread> workers;
     for (int i = 1; i < n_hyp && i < 16; ++i) workers.emplace_back(build, i);
@@ -965,6 +989,13 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     CUI(cudaEventElapsedTime(&ms, h->ev0.get(), h->ev1.get()));
     h->last_kernel_us = ms * 1000.f;
   }
+  if (h->verify) {
+    std::vector<std::vector<double>> raw(jobs.size());
+    for (int i = 0; i < n_hyp; ++i)
+      if (job_of[i] >= 0) raw[(size_t)job_of[i]] = std::move(clouds[i].raw);
+    int rc = icp_verify_host(h, job_of, raw, scene_depth, srows, scols, sceneK);
+    if (rc) return rc;
+  }
   if (h->capture) {
     auto& c = h->cap;
     c.estimation = h->estimation;
@@ -1027,6 +1058,23 @@ extern "C" int lm_icp_set_estimation(lm_icp* h, int estimation) {
     return lm_fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
   h->estimation = estimation;
   return LM_OK;
+}
+
+extern "C" int lm_icp_set_verify(lm_icp* h, int on, double inlier_mm) {
+  if (!h) return lm_fail(LM_E_INVALID, "null handle");
+  if (!(std::isfinite(inlier_mm) && inlier_mm >= 0.0))
+    return lm_fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
+  h->verify = on != 0;
+  h->verify_mm = inlier_mm;
+  return LM_OK;
+}
+
+static int copy_verify(const PoseVerify* v, int64_t count, float* score, int32_t* counts6, int64_t cap, int64_t* n);
+
+extern "C" int lm_icp_verify(lm_icp* h, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
+  if (!h) return lm_fail(LM_E_INVALID, "null handle");
+  if (!h->verified) return lm_fail(LM_E_STATE, "the last call did not verify (lm_icp_set_verify)");
+  return copy_verify(h->ver.data(), (int64_t)h->ver.size(), score, counts6, cap, n);
 }
 
 extern "C" int lm_icp_set_capture(lm_icp* h, int on) {
@@ -1346,6 +1394,152 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long
 }
 
 // --------------------------------------------------------------------------------------------
+// pose verification (include/linemod_b200.h, lm_set_pose_verify): the raw model cloud moved by the ICP's T, projected
+// into the scene depth
+// --------------------------------------------------------------------------------------------
+#define VERIFY_THREADS 256
+enum { VERIFY_OUTSIDE, VERIFY_MISSING, VERIFY_INLIER, VERIFY_OCCLUDED, VERIFY_VIOLATION, VERIFY_CLASSES };
+
+struct VerifyScene {
+  const uint16_t* depth;  // rows x cols u16 mm
+  int32_t rows, cols;
+  float fx, fy, cx, cy;
+};
+
+// Steps 3-4 for one point p of the model cloud, T's first three rows in T[0..11]; every operation correctly rounded.
+__device__ __forceinline__ int verify_point(const double* T, double px, double py, double pz, const VerifyScene& sc, double delta) {
+  double q[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    q[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4 * r], px), __dmul_rn(T[4 * r + 1], py)), __dmul_rn(T[4 * r + 2], pz)), T[4 * r + 3]);
+  if (!(q[2] > 0.0)) return VERIFY_OUTSIDE;
+  const double u = __dadd_rn(__dmul_rn((double)sc.fx, __ddiv_rn(q[0], q[2])), (double)sc.cx);
+  const double v = __dadd_rn(__dmul_rn((double)sc.fy, __ddiv_rn(q[1], q[2])), (double)sc.cy);
+  if (!isfinite(u) || !isfinite(v)) return VERIFY_OUTSIDE;
+  const double c = floor(__dadd_rn(u, 0.5)), r = floor(__dadd_rn(v, 0.5));
+  if (!(c >= 0.0 && c < (double)sc.cols && r >= 0.0 && r < (double)sc.rows)) return VERIFY_OUTSIDE;
+  const uint16_t zs = sc.depth[(size_t)r * sc.cols + (size_t)c];
+  if (zs == 0) return VERIFY_MISSING;
+  const double d = __dsub_rn((double)zs, __dmul_rn(q[2], 1000.0));
+  if (fabs(d) <= delta) return VERIFY_INLIER;
+  return d < 0.0 ? VERIFY_OCCLUDED : VERIFY_VIOLATION;
+}
+
+// The CTA's n points P classified and counted (step 5), returned on thread 0.  The counts are exact in any order.
+__device__ PoseVerify verify_block(const double* __restrict__ P, int n, const double* T, const VerifyScene& sc, double delta) {
+  __shared__ int s_cnt[VERIFY_CLASSES];
+  if (threadIdx.x < VERIFY_CLASSES) s_cnt[threadIdx.x] = 0;
+  __syncthreads();
+  int cnt[VERIFY_CLASSES] = {0, 0, 0, 0, 0};
+  for (int j = threadIdx.x; j < n; j += blockDim.x) {
+    const int k = verify_point(T, P[3 * j], P[3 * j + 1], P[3 * j + 2], sc, delta);
+#pragma unroll
+    for (int q = 0; q < VERIFY_CLASSES; ++q) cnt[q] += k == q;
+  }
+#pragma unroll
+  for (int q = 0; q < VERIFY_CLASSES; ++q) {
+    const int w = __reduce_add_sync(0xffffffffu, cnt[q]);
+    if ((threadIdx.x & 31) == 0 && w) atomicAdd(&s_cnt[q], w);
+  }
+  __syncthreads();
+  PoseVerify o;
+  o.counts[0] = n;
+  for (int q = 0; q < VERIFY_CLASSES; ++q) o.counts[1 + q] = s_cnt[q];
+  const int den = s_cnt[VERIFY_INLIER] + s_cnt[VERIFY_OCCLUDED] + s_cnt[VERIFY_VIOLATION];
+  o.score = den > 0 ? __fdiv_rn((float)s_cnt[VERIFY_INLIER], (float)den) : 0.f;
+  o.pad = 0;
+  return o;
+}
+
+// One CTA per chunk slot behind the unshared ICP kernel: slot i's raw model cloud (k_pose_cloud's model slot, segment
+// 2i) moved by outs[i].T, against the scene of its survivor's frame.  A slot without a pose gets score -1 and zero
+// counts.  Unshared, the result goes to out[i]; SHARE (a shared stage that verifies), slot i's ICP output and its
+// verification go to the pose areas of the exchange (pose_share_publish), and out is unused.
+template <bool SHARE>
+__global__ void __launch_bounds__(VERIFY_THREADS) k_pose_verify(PoseParams p, const IcpOut* __restrict__ outs, double delta,
+                                                                PoseVerify* __restrict__ out, PoseShareDev sh) {
+  __shared__ double s_T[12];
+  const int i = blockIdx.x;
+  PoseVerify v;
+  if (!p.posed[i]) {  // block-uniform
+    for (int q = 0; q < 6; ++q) v.counts[q] = 0;
+    v.score = -1.f;
+    v.pad = 0;
+  } else {
+    const int frame = p.frame_of ? p.frame_of[p.rank + i * p.world] : 0;
+    const float* fK = p.frame_of ? p.sKs + 9 * frame : nullptr;
+    VerifyScene sc;
+    sc.depth = p.scene + (size_t)frame * p.srows * p.scols;
+    sc.rows = p.srows; sc.cols = p.scols;
+    sc.fx = fK ? fK[0] : p.sK[0]; sc.cx = fK ? fK[2] : p.sK[2]; sc.fy = fK ? fK[4] : p.sK[4]; sc.cy = fK ? fK[5] : p.sK[5];
+    if (threadIdx.x < 12) s_T[threadIdx.x] = outs[i].T[threadIdx.x];
+    __syncthreads();
+    const int b = p.seg_begin[2 * i];
+    v = verify_block(p.raw + (size_t)b * 3, p.seg_end[2 * i] - b, s_T, sc, delta);
+  }
+  if (threadIdx.x == 0) {
+    if (SHARE) pose_share_publish(sh, outs[i], v);
+    else out[i] = v;
+  }
+}
+
+static bool verify_delta_ok(double inlier_mm) { return std::isfinite(inlier_mm) && inlier_mm >= 0.0; }
+
+// lm_icp_process_batch's verification: job j's raw model cloud raw[j] (uploaded with the scene) moved by the ICP's output
+// h->d_outs[j], one k_pose_verify launch over the jobs; then h->ver per hypothesis (score -1 on the early return).
+static int icp_verify_host(lm_icp* h, const std::vector<int>& job_of, const std::vector<std::vector<double>>& raw,
+                           const uint16_t* scene, int srows, int scols, const float* sK) {
+  const size_t J = raw.size(), npix = (size_t)srows * scols;
+  h->ver.assign(job_of.size(), PoseVerify());
+  for (PoseVerify& v : h->ver) v.score = -1.f;
+  if (J) {
+    // one buffer: scene, segments [4J] (slot j's begin at 2j, its end at 2J + 2j), posed flags [J], points, results [J]
+    size_t npts = 0;
+    for (const auto& r : raw) npts += r.size() / 3;
+    if (npts > 0x7FFFFFFFu) return lm_fail(LM_E_CAPACITY, "%zu model points to verify, at most 2^31 - 1", npts);
+    auto a16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t o_seg = a16(sizeof(uint16_t) * npix), o_posed = a16(o_seg + sizeof(int32_t) * 4 * J);
+    const size_t o_pts = a16(o_posed + J), o_ver = a16(o_pts + sizeof(double) * 3 * npts);
+    std::vector<uint8_t> in(o_ver);
+    memcpy(in.data(), scene, sizeof(uint16_t) * npix);
+    int32_t* seg = reinterpret_cast<int32_t*>(in.data() + o_seg);
+    double* pts = reinterpret_cast<double*>(in.data() + o_pts);
+    size_t at = 0;
+    for (size_t j = 0; j < J; ++j) {
+      seg[2 * j] = (int32_t)at;
+      memcpy(pts + 3 * at, raw[j].data(), sizeof(double) * raw[j].size());
+      at += raw[j].size() / 3;
+      seg[2 * J + 2 * j] = (int32_t)at;
+      in[o_posed + j] = 1;
+    }
+    CUI(h->d_vbuf.reserve(o_ver + sizeof(PoseVerify) * J));
+    cudaStream_t st = h->stream.get();
+    uint8_t* b = h->d_vbuf.get();
+    CUI(cudaMemcpyAsync(b, in.data(), in.size(), cudaMemcpyHostToDevice, st));
+    PoseParams p;
+    memset(&p, 0, sizeof(p));
+    p.scene = reinterpret_cast<const uint16_t*>(b);
+    p.srows = srows; p.scols = scols;
+    memcpy(p.sK, sK, sizeof(p.sK));
+    p.raw = reinterpret_cast<double*>(b + o_pts);
+    p.seg_begin = reinterpret_cast<int32_t*>(b + o_seg); p.seg_end = p.seg_begin + 2 * J;
+    p.posed = b + o_posed;
+    p.rank = 0; p.world = 1;
+    k_pose_verify<false><<<(unsigned)J, VERIFY_THREADS, 0, st>>>(p, h->d_outs.get(), h->verify_mm, reinterpret_cast<PoseVerify*>(b + o_ver),
+                                                                 PoseShareDev());
+    CUI(cudaGetLastError());
+    ++h->launches;
+    std::vector<PoseVerify> out(J);
+    CUI(cudaMemcpyAsync(out.data(), b + o_ver, sizeof(PoseVerify) * J, cudaMemcpyDeviceToHost, st));
+    CUI(cudaStreamSynchronize(st));
+    for (size_t i = 0; i < job_of.size(); ++i)
+      if (job_of[i] >= 0) h->ver[i] = out[(size_t)job_of[i]];
+  }
+  h->verified = true;
+  return LM_OK;
+}
+
+// --------------------------------------------------------------------------------------------
 // pose NMS (lm_pose.h): the greedy translation NMS of linemod_ros/detect.py:41-50, 130-131 behind the pose stage
 // --------------------------------------------------------------------------------------------
 // One CTA, one entry per thread (n <= NMS_THREADS).  Each round picks the best live entry with a block-wide arg-max
@@ -1466,9 +1660,18 @@ struct PoseNmsParams {
   PoseNmsOut* out;          // kept poses in keep order, frame f's from out + frame_first[f]
   // null: one frame, survivors [0, counts[0]).  Else frame f's survivors are [frame_first[f], frame_first[f + 1]).
   const int32_t* frame_first;
+  // VERIFY only: per survivor its verification (k_pose_verify), per kept pose its copy (at out's index), and the
+  // ranking and minimum score of lm_set_pose_verify
+  const PoseVerify* ver;
+  PoseVerify* vout;
+  int32_t rank_by;
+  double min_score;
 };
 
 // Behind the ICP kernel: candidates are the survivors with a pose, score -(double)residual.  One frame per CTA.
+// VERIFY (behind k_pose_verify): a survivor scoring below min_score is no candidate, rank_by may put the score first, and
+// every kept pose's verification goes to vout.
+template <bool VERIFY>
 __global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
   const int i = threadIdx.x;
   const int first = p.frame_first ? p.frame_first[blockIdx.x] : 0;
@@ -1488,8 +1691,15 @@ __global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
     cand = true;
   }
   const int posed = __syncthreads_count(cand);
+  unsigned long long key = nms_score_key(-(double)res);
+  if (VERIFY && cand) {
+    const float score = p.ver[first + i].score;
+    if ((double)score < p.min_score) cand = false;
+    if (p.rank_by == LM_VERIFY_RANK_SCORE) key = nms_score_key((double)score);
+  }
   int rank;
-  const int kept = nms_translations_block(cand, nms_score_key(-(double)res), t[0], t[1], t[2], p.thr, nullptr, rank);
+  const int kept = nms_translations_block(cand, key, t[0], t[1], t[2], p.thr, nullptr, rank);
+  if (VERIFY && rank >= 0) p.vout[first + rank] = p.ver[first + i];
   if (rank >= 0) {
     PoseNmsOut o;
     const PoseRt q = p.rt[g];
@@ -1538,6 +1748,10 @@ struct lm_pose_stage {
   DeviceArray<lm_match> d_bsurv;
   // a run's outputs (pose_outputs), a frame's at offset 0: per survivor its frame, ICP output and posed flag
   DeviceArray<int32_t> d_bframe;
+  // only once a run verifies: per survivor its verification and per kept pose its copy, the host's copy of either
+  // (h_bver last: survivors), and per chunk slot the ICP output a verifying shared stage publishes from
+  DeviceArray<PoseVerify> d_bver, d_bvkept; PinnedArray<PoseVerify> h_bver;
+  DeviceArray<IcpOut> d_souts;
   DeviceArray<IcpOut> d_bouts; DeviceArray<uint8_t> d_bposed; PinnedArray<IcpOut> h_bouts;  // h_bouts last: survivors
   // per frame its first survivor and intrinsics, per chunk (at most one per frame) a status block (PoseChunk; [3] a
   // batch chunk's size)
@@ -1551,6 +1765,9 @@ struct lm_pose_stage {
   PoseShare share = {};
   std::vector<int64_t> first;
   int64_t launches = 0, fetched = 0;
+  // the verification of the entries of the run last finished (pose_stage_verify); verified false: it did not verify
+  bool verified = false;
+  std::vector<PoseVerify> ver;
 };
 
 // The per-chunk buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
@@ -1708,12 +1925,14 @@ struct PoseChunk {
   const float* sK;
   IcpOut* outs;
   uint8_t* posed;
+  PoseVerify* ver;  // o.verify.on: per survivor its verification
   int32_t* status;
   int32_t seq;
 };
 
 // k_pose_cloud, the segmented sort, k_pose_voxel, k_icp_normals (point-to-plane only) and the ICP kernel over this
-// rank's ceil(slots / world) slots, then (shared) k_pose_collect.  Unshared, the cloud's posed flags and the ICP results
+// rank's ceil(slots / world) slots, then (o.verify.on) k_pose_verify, then (shared) k_pose_collect.  A shared stage that
+// verifies runs the ICP kernel's unshared instantiation into d_souts, and k_pose_verify<true> publishes.  Unshared, the cloud's posed flags and the ICP results
 // go straight to the chunk's outputs; shared, to the stage's per-slot scratch, and k_pose_collect writes the outputs.
 // Returns the chunk's launches (the sort counted once), or an error code (< 0).
 static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c) {
@@ -1753,13 +1972,20 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   if (sh) {
     // the results travel to every rank; the collector gathers the chunk in survivor order
     const PoseShareDev sd = share_dev(*sh, c.seq, c.counts, s->d_posed.get(), c.status);
-    launch_icp<true>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), nullptr, o.max_iterations, nullptr, sd);
-    k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, c.outs, c.posed);
+    if (o.verify.on) {  // the owner verifies (it holds the cloud), then publishes the pose and its verification
+      launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), s->d_souts.get(), o.max_iterations, nullptr,
+                        PoseShareDev());
+      k_pose_verify<true><<<n, VERIFY_THREADS, 0, st>>>(p, s->d_souts.get(), o.verify.inlier_mm, nullptr, sd);
+    } else {
+      launch_icp<true>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), nullptr, o.max_iterations, nullptr, sd);
+    }
+    k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, c.outs, c.posed, o.verify.on ? c.ver : nullptr);
   } else {
     launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.outs, o.max_iterations, nullptr, PoseShareDev());
+    if (o.verify.on) k_pose_verify<false><<<n, VERIFY_THREADS, 0, st>>>(p, c.outs, o.verify.inlier_mm, c.ver, PoseShareDev());
   }
   CUI(cudaGetLastError());
-  return (sh ? 6 : 5) - (normals ? 0 : 1);
+  return (sh ? 6 : 5) - (normals ? 0 : 1) + (o.verify.on ? 1 : 0);
 }
 
 #define POSE_CHUNK 1024     // survivor slots per chunk: a frame's bound for top_k = 0
@@ -1800,20 +2026,34 @@ static int pose_outputs(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t
   return LM_OK;
 }
 
-// The renders on the device and every buffer a run of n_frames frames and S survivors needs.
-static int pose_prepare(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S) {
+// The renders on the device and every buffer a run of n_frames frames and S survivors needs (verify: a verifying run's
+// too).
+static int pose_prepare(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S, bool verify) {
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
   }
   S = std::max<int64_t>(S, 1);
   int rc = pose_outputs(s, st, n_frames, S);
-  if (rc) return rc;
-  return pose_buffers(s, st, (int)std::min<int64_t>(S, POSE_CHUNK), s->area_max);
+  if (!rc) rc = pose_buffers(s, st, (int)std::min<int64_t>(S, POSE_CHUNK), s->area_max);
+  if (rc || !verify) return rc;
+  if ((size_t)S > s->h_bver.size()) {
+    CUI(cudaStreamSynchronize(st));
+    s->d_bver.reset(); s->d_bvkept.reset(); s->h_bver.reset();
+    CUI(s->d_bver.assign(S));
+    CUI(s->d_bvkept.assign(S));
+    CUI(s->h_bver.assign(S));
+  }
+  if ((size_t)pose_slots(s) > s->d_souts.size()) {
+    CUI(cudaStreamSynchronize(st));
+    s->d_souts.reset();
+    CUI(s->d_souts.assign(pose_slots(s)));
+  }
+  return LM_OK;
 }
 
-int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
-                       lm_match** d_surv) {
+int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, bool verify,
+                       uint16_t** d_scene, lm_match** d_surv) {
   const size_t pix = (size_t)n_frames * frame_pixels;
   if (pix > s->d_bscene.size() || (size_t)max_surv > s->d_bsurv.size()) {
     CUI(cudaStreamSynchronize(st));  // an earlier batch may still read them
@@ -1822,7 +2062,7 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
   }
   // and everything the run may need for max_surv survivors: once frames run, no device memory is freed (a free waits for
   // the whole device, a spinning peer collector of a shared batch included)
-  int rc = pose_prepare(s, st, n_frames, max_surv);
+  int rc = pose_prepare(s, st, n_frames, max_surv, verify);
   if (rc) return rc;
   *d_scene = s->d_bscene.get();
   *d_surv = s->d_bsurv.get();
@@ -1837,7 +2077,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
   const int nf = run.n_frames;
   const int64_t S = batch ? run.first[nf] : run.bound;  // survivors the outputs hold
   const int nc = batch ? pose_batch_chunks(S) : 1;
-  int rc = pose_prepare(s, st, nf, S);
+  int rc = pose_prepare(s, st, nf, S, o.verify.on != 0);
   if (rc) return rc;
   if (batch) {  // each survivor's frame, each frame's first survivor and intrinsics, each chunk's status block and size
     std::vector<int32_t> frame_of((size_t)S);
@@ -1863,7 +2103,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
     k.slots = batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound;
     k.scene = run.d_scene; k.frame_of = batch ? s->d_bframe.get() + c0 : nullptr;
     k.sKs = batch ? s->d_bsK.get() : nullptr; k.sK = batch ? nullptr : run.sK;
-    k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
+    k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.ver = s->d_bver.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
     const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
     stage_launches += l;
@@ -1872,6 +2112,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
   // the status blocks, and unless a pose NMS follows the ICP outputs: a batch's all, a frame's first window
   const int64_t fetch = run.pose_nms ? 0 : batch ? S : std::min(run.bound, POSE_FIRST_FETCH);
   if (fetch) CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * fetch, cudaMemcpyDeviceToHost, st));
+  if (fetch && o.verify.on) CUI(cudaMemcpyAsync(s->h_bver.get(), s->d_bver.get(), sizeof(PoseVerify) * fetch, cudaMemcpyDeviceToHost, st));
   if (nc) CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
   s->run = run;
   s->share = sh ? *sh : PoseShare();
@@ -1895,13 +2136,17 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches) {
   p.thr = thr;
   p.head = nms_heads(s->d_bnms.get()); p.out = nms_out(s->d_bnms.get(), nf);
   p.frame_first = batch ? s->d_bfirst.get() : nullptr;
-  k_pose_nms<<<nf, NMS_THREADS, 0, st>>>(p);
+  const PoseVerifyOptions& v = r.o.verify;
+  p.ver = s->d_bver.get(); p.vout = s->d_bvkept.get(); p.rank_by = v.rank_by; p.min_score = v.min_score;
+  if (v.on) k_pose_nms<true><<<nf, NMS_THREADS, 0, st>>>(p);
+  else k_pose_nms<false><<<nf, NMS_THREADS, 0, st>>>(p);
   CUI(cudaGetLastError());
   ++*launches;
-  // the heads and the kept poses: a batch's all, a frame's first window
+  // the heads and the kept poses (and their verification): a batch's all, a frame's first window
   r.pose_nms = 1;
   s->fetched = batch ? r.first[nf] : std::min(r.bound, NMS_FIRST_FETCH);
   CUI(cudaMemcpyAsync(s->h_bnms.get(), s->d_bnms.get(), sizeof(PoseNmsHead) * nf + sizeof(PoseNmsOut) * s->fetched, cudaMemcpyDeviceToHost, st));
+  if (v.on) CUI(cudaMemcpyAsync(s->h_bver.get(), s->d_bvkept.get(), sizeof(PoseVerify) * s->fetched, cudaMemcpyDeviceToHost, st));
   return LM_OK;
 }
 
@@ -1973,6 +2218,9 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
   const int64_t* first = batch ? r.first : frame_first;
   const int64_t S = first[nf];
   if (!batch && n > r.bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, r.bound);
+  const bool verify = r.o.verify.on != 0;
+  s->verified = false;
+  s->ver.clear();
   int64_t published = 0;
   int rc = pose_status(s->h_bstat.get(), batch ? pose_batch_chunks(S) : 1, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0,
                        batch, &published);
@@ -2011,6 +2259,9 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
   }
   if (end > s->fetched) {  // a frame's entries beyond its first window
     cudaStream_t st = r.o.stream;
+    if (verify)
+      CUI(cudaMemcpyAsync(s->h_bver.get() + s->fetched, (r.pose_nms ? s->d_bvkept.get() : s->d_bver.get()) + s->fetched,
+                          sizeof(PoseVerify) * (size_t)(end - s->fetched), cudaMemcpyDeviceToHost, st));
     if (r.pose_nms)
       CUI(cudaMemcpyAsync(entries + s->fetched, nms_out(s->d_bnms.get(), nf) + s->fetched, sizeof(PoseNmsOut) * (size_t)(end - s->fetched),
                           cudaMemcpyDeviceToHost, st));
@@ -2023,14 +2274,83 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
     int64_t at = 0;
     for (int f = 0; f < nf; ++f) {
       copy_kept(entries + first[f], counts[4 * f], out ? out + at : nullptr, R_out + 9 * at, t_out + 3 * at, residual + at);
+      if (verify) s->ver.insert(s->ver.end(), s->h_bver.get() + first[f], s->h_bver.get() + first[f] + counts[4 * f]);
       at += counts[4 * f];
     }
+    s->verified = verify;
     return LM_OK;
   }
   for (int64_t i = 0; i < S; ++i) {  // every survivor, frame after frame
     if (out) out[i] = surv[i];
     survivor_pose(*survivor_render(s, surv[i]), surv[i], r.o.srows, r.o.scols, s->h_bouts[i], R_out + 9 * i, t_out + 3 * i, residual + i);
   }
+  if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + S);
+  s->verified = verify;
+  return LM_OK;
+}
+
+// n verification results v[] into score[k] / counts6 + 6k (LM_E_CAPACITY beyond cap, *n written either way).
+static int copy_verify(const PoseVerify* v, int64_t count, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
+  if (!n || (cap > 0 && (!score || !counts6))) return lm_fail(LM_E_INVALID, "null argument");
+  *n = count;
+  if (count > cap) return lm_fail(LM_E_CAPACITY, "%lld verified entries, capacity %lld", (long long)count, (long long)cap);
+  for (int64_t k = 0; k < count; ++k) {
+    score[k] = v[k].score;
+    memcpy(counts6 + 6 * k, v[k].counts, sizeof(v[k].counts));
+  }
+  return LM_OK;
+}
+
+int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
+  if (!s || !s->verified) return lm_fail(LM_E_STATE, "the last completed pose stage did not verify (lm_set_pose_verify)");
+  return copy_verify(s->ver.data(), (int64_t)s->ver.size(), score, counts6, cap, n);
+}
+
+extern "C" int lm_pose_verify_points(int device, const double* pts, int64_t n, const double* T, const uint16_t* scene, int rows,
+                                     int cols, const float* sK, double inlier_mm, int32_t* counts6, float* score) {
+  if (n < 0 || (n > 0 && !pts) || !T || !scene || !sK || !counts6 || !score) return lm_fail(LM_E_INVALID, "null argument or n < 0");
+  if (rows <= 0 || cols <= 0) return lm_fail(LM_E_INVALID, "empty scene %d x %d", rows, cols);
+  if (n > 0x7FFFFFFFll) return lm_fail(LM_E_CAPACITY, "%lld points, at most 2^31 - 1", (long long)n);
+  if (!verify_delta_ok(inlier_mm)) return lm_fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
+  CUI(cudaSetDevice(device));
+  // k_pose_verify over one slot: one allocation of pts [n][3], the pose (IcpOut), the segments (begin 0 at [0], end n at
+  // [2]), the posed flag, the result and the scene [rows][cols]
+  IcpOut o;
+  memset(&o, 0, sizeof(o));
+  memcpy(o.T, T, sizeof(o.T));
+  const int32_t seg[4] = {0, 0, (int32_t)n, 0};
+  const uint8_t posed = 1;
+  const size_t o_out = sizeof(double) * 3 * (size_t)n, o_icp = o_out + sizeof(PoseVerify), o_seg = o_icp + sizeof(IcpOut);
+  const size_t o_posed = o_seg + sizeof(seg), o_scene = o_posed + 16;
+  DeviceArray<uint8_t> buf;
+  CUI(buf.assign(o_scene + sizeof(uint16_t) * (size_t)rows * cols));
+  uint8_t* b = buf.get();
+  if (n > 0) CUI(cudaMemcpy(b, pts, o_out, cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_icp, &o, sizeof(o), cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_seg, seg, sizeof(seg), cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_posed, &posed, 1, cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_scene, scene, sizeof(uint16_t) * (size_t)rows * cols, cudaMemcpyHostToDevice));
+  PoseParams p;
+  memset(&p, 0, sizeof(p));
+  p.scene = reinterpret_cast<const uint16_t*>(b + o_scene);
+  p.srows = rows; p.scols = cols;
+  memcpy(p.sK, sK, sizeof(p.sK));
+  p.raw = reinterpret_cast<double*>(b);
+  p.seg_begin = reinterpret_cast<int32_t*>(b + o_seg); p.seg_end = p.seg_begin + 2;
+  p.posed = b + o_posed;
+  p.rank = 0; p.world = 1;
+  PoseVerify* d_out = reinterpret_cast<PoseVerify*>(b + o_out);
+  k_pose_verify<false><<<1, VERIFY_THREADS>>>(p, reinterpret_cast<const IcpOut*>(b + o_icp), inlier_mm, d_out, PoseShareDev());
+  CUI(cudaGetLastError());
+  PoseVerify v;
+  CUI(cudaMemcpy(&v, d_out, sizeof(v), cudaMemcpyDeviceToHost));
+  memcpy(counts6, v.counts, sizeof(v.counts));
+  *score = v.score;
   return LM_OK;
 }
 
@@ -2151,6 +2471,7 @@ struct IcpDevice {
   DeviceArray<IcpOut> outs; DeviceArray<uint8_t> posed; PinnedArray<IcpOut> h_outs;
   DeviceArray<int32_t> status; PinnedArray<int32_t> h_status;  // 4 per chunk (PoseChunk); the host's copy then holds the
                                                                // source count of the last hypothesis with a pose
+  DeviceArray<PoseVerify> ver; PinnedArray<PoseVerify> h_ver;  // lm_icp_set_verify: per hypothesis
 };
 
 static void icp_device_free(IcpDevice* d) { delete d; }
@@ -2191,7 +2512,12 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     rc = check_device_plane(h->device, what, model_depths[i], model_pitches[i], (int64_t)mz * mcols, mz);
   }
   if (rc) return rc;
-  if (n_hyp == 0) return LM_OK;
+  h->verified = false;
+  if (n_hyp == 0) {
+    h->ver.clear();
+    h->verified = h->verify;
+    return LM_OK;
+  }
   CUI(cudaSetDevice(h->device));
   if (!h->dev) h->dev = new IcpDevice();
   IcpDevice& d = *h->dev;
@@ -2220,6 +2546,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   CUI(d.tpl.reserve(n));
   CUI(d.outs.reserve(n)); CUI(d.posed.reserve(n)); CUI(d.h_outs.reserve(n));
   CUI(d.status.reserve(4 * (size_t)nc)); CUI(d.h_status.reserve(4 * (size_t)nc + 1));
+  if (h->verify) { CUI(d.ver.reserve(n)); CUI(d.h_ver.reserve(n)); }
   const RenderSrc* d_src = reinterpret_cast<const RenderSrc*>(d.in.get());
   const float* d_K = reinterpret_cast<const float*>(d.in.get() + o_K);
   const int f32 = model_format == LM_DEPTH_F32 ? 1 : 0;
@@ -2268,12 +2595,18 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   CUI(cudaStreamWaitEvent(caller, d.ev_out.get(), 0));
   if (last < 0) {  // every hypothesis takes the early return: no cloud to build
     for (int i = 0; i < n; ++i) residual[i] = -1.f;
+    if (h->verify) {
+      h->ver.assign((size_t)n, PoseVerify());
+      for (PoseVerify& v : h->ver) v.score = -1.f;
+      h->verified = true;
+    }
     return LM_OK;
   }
   CUI(cudaMemsetAsync(d.status.get(), 0, sizeof(int32_t) * 4 * nc, st));
   PoseOptions o;
   o.srows = srows; o.scols = scols; o.use_scene_cloud = h->use_scene_cloud ? 1 : 0; o.max_iterations = max_iterations;
   o.estimation = h->estimation; o.stream = st; o.share = nullptr;
+  o.verify = {h->verify ? 1 : 0, LM_VERIFY_RANK_FITNESS, h->verify_mm, -INFINITY};
   const PoseTable table = {d.tpl.get(), d.crops.get(), reinterpret_cast<const int32_t*>(d.in.get() + o_cb), 1, n};
   const lm_match* d_surv = reinterpret_cast<const lm_match*>(d.in.get() + o_surv);
   const int32_t* d_cnt = reinterpret_cast<const int32_t*>(d.in.get() + o_cnt);
@@ -2283,7 +2616,8 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     k.table = table;
     k.surv = d_surv + c0; k.counts = d_cnt + c; k.slots = cnt[c];
     k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK;
-    k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.status = d.status.get() + 4 * c; k.seq = 0;
+    k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.ver = h->verify ? d.ver.get() + c0 : nullptr;
+    k.status = d.status.get() + 4 * c; k.seq = 0;
     const int l = pose_chunk(&d.stage, o, k);
     if (l < 0) return l;
     h->launches += l;
@@ -2293,6 +2627,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   CUI(cudaEventRecord(h->ev1.get(), st));
   CUI(cudaMemcpyAsync(d.h_outs.get(), d.outs.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
   CUI(cudaMemcpyAsync(d.h_status.get(), d.status.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  if (h->verify) CUI(cudaMemcpyAsync(d.h_ver.get(), d.ver.get(), sizeof(PoseVerify) * n, cudaMemcpyDeviceToHost, st));
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
   float ms = 0;
@@ -2308,6 +2643,10 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     init_base(R + 9 * i, t + 3 * i, base);
     compose(q.T, base, R_out + 9 * i, t_out + 3 * i);
     residual[i] = (float)q.fitness;
+  }
+  if (h->verify) {
+    h->ver.assign(d.h_ver.get(), d.h_ver.get() + n);
+    h->verified = true;
   }
   h->last_points = d.h_status[4 * (size_t)nc];
   h->last_iterations = d.h_outs[(size_t)last].iterations;

@@ -30,9 +30,10 @@ bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel
 // survivor rank + j * world, so the launches are sized for ceil(survivors / world) slots; unshared, rank 0 and world 1.
 // Shared over the ranks of the peer exchange (lm_peer_share_pose), survivor i (pick order of k_post_nms, the same on
 // every rank) is thus refined by rank i % world.  The ICP kernel's SHARE instantiation stores each survivor's result into
-// the pose area of every rank's exchange buffer and raises this rank's pose flag there; k_pose_collect waits for the
+// the pose area of every rank's exchange buffer and raises this rank's pose flag there (a verifying stage: the unshared ICP kernel, then k_pose_verify<true>, which
+// verifies each survivor on the rank that holds its cloud and stores result and verification); k_pose_collect waits for the
 // world flags in this rank's buffer and gathers the results in survivor order into the chunk's outputs, so the host and
-// the pose NMS read what the unshared stage leaves.  The pose area: [2 slots][1024 survivors] entries of 160 bytes,
+// the pose NMS read what the unshared stage leaves.  The pose area: [2 slots][1024 survivors] entries of 192 bytes,
 // then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket (pose_share_area_bytes in all).  Each pose exchange -- a
 // shared frame, or one chunk of a shared batch -- has its own number on the detector's pose counter.
 struct PoseShare {
@@ -45,6 +46,13 @@ struct PoseShare {
 };
 size_t pose_share_area_bytes();
 
+// Pose verification (lm_set_pose_verify): on adds k_pose_verify behind each chunk's ICP kernel (shared: on the rank that
+// refined the survivor, before its result is published); rank_by and min_score steer the pose NMS.
+struct PoseVerifyOptions {
+  int on, rank_by;
+  double inlier_mm, min_score;
+};
+
 // What every chunk of a run shares.
 struct PoseOptions {
   int srows, scols;           // scene depth size
@@ -52,6 +60,7 @@ struct PoseOptions {
   int estimation;             // LM_ICP_POINT_TO_PLANE (k_icp_normals + k_icp_point_to_plane) or LM_ICP_POINT_TO_POINT
   cudaStream_t stream;
   const PoseShare* share;     // null: this rank refines every survivor
+  PoseVerifyOptions verify;  // zero: off
 };
 
 // One run of the pose stage: a batch of frames (lm_detect_batch, lm_peer_detect_batch), or a frame as a one-frame run
@@ -87,11 +96,15 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches);
 int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_match* out, double* R_out, double* t_out, float* residual,
                       int64_t cap, int64_t* n_out, int64_t* counts, int64_t* stats4);
 
+// The verification of the entries of the run last finished, in their order (lm_pose_verify): LM_E_STATE when it did not
+// verify, LM_E_CAPACITY (with *n) beyond cap.
+int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, int64_t cap, int64_t* n);
+
 // A batch's scene and survivor slots: room for n_frames scene depths of frame_pixels each (frame f at d_scene + f *
 // frame_pixels) and max_surv survivors, which the caller fills on the stream.  It also uploads the renders and grows
 // every buffer the run needs for max_surv survivors, so that the batch allocates no device memory once its frames run.
-int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, uint16_t** d_scene,
-                       lm_match** d_surv);
+int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t frame_pixels, int64_t max_surv, bool verify,
+                       uint16_t** d_scene, lm_match** d_surv);
 // Chunks of a run with S survivors.
 int pose_batch_chunks(int64_t S);
 

@@ -67,6 +67,7 @@ class Detector:
         self._selection = None
         self._template_depths = None  # training distances registered with the native handle (setTemplateDepths)
         self._peers = None  # (rank, world) once dist.connect_peers has wired the fused exchange
+        self._verify = _lib.verify_options(None)  # lm_set_pose_verify's arguments (setPoseVerification)
         self.device = _default_device()
         self.shard = (0, 1)  # (index, count): template shard matched by this process (multi-GPU)
         self.shard_layout = _lib.SHARD_CONTIGUOUS
@@ -295,6 +296,31 @@ class Detector:
                 raise ValueError("class %s: %d renders for %d templates" % (cid, got, n))
             first += n
 
+    def setPoseVerification(self, inlier_mm=10.0, rank_by="fitness", min_score=None):
+        """Verify every refined pose against the scene depth (include/linemod_b200.h, lm_set_pose_verify), for
+        match_refine, detect, the batch calls and dist's sharded calls: the poseRefine objects they return then carry
+        getScore() and getVerification().  inlier_mm: the distance (mm) within which a model point's depth agrees with the
+        scene's; None turns verification off (the default).  rank_by: the pose NMS's order in detect / detect_batch,
+        "fitness" (-residual, as without verification) or "score" (score descending).  min_score: detect's posed
+        survivors scoring below it are dropped before the pose NMS.  A pose stage shared over the ranks verifies too."""
+        self._verify = _lib.verify_options(inlier_mm, rank_by, min_score)
+
+    def _pose_native(self, class_ids):
+        nat = self._select(list(class_ids))
+        nat.set_pose_verify(*self._verify)
+        return nat
+
+    def _verification(self, nat, sizes):
+        # per run of `sizes` entries, the [(score, counts)] of the last completed pose stage; None without verification
+        if not self._verify[0]:
+            return [None] * len(sizes)
+        pairs = _lib.verify_arrays(*nat.pose_verify())
+        out, at = [], 0
+        for k in sizes:
+            out.append(pairs[at:at + k])
+            at += k
+        return out
+
     def match_refine(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
                      use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
         """match + nms + poseRefine().process for every survivor, as the drivers do (linemod_and_levelup_test.py:
@@ -309,10 +335,10 @@ class Detector:
         sources = self._frame_sources(sources, masks, depth_scale, stream)
         self._whole_bank_only("match_refine()")
         sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
-        nat = self._select(list(class_ids))
+        nat = self._pose_native(class_ids)
         out, R, t, res, _ = nat.match_pose(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold),
                                            int(top_k), int(max_iterations), bool(use_scene_cloud), estimation)
-        return self._pose_pairs(out, R, t, res)
+        return self._pose_pairs(out, R, t, res, self._verification(nat, [len(out)])[0])
 
     def detect(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
                max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
@@ -327,10 +353,10 @@ class Detector:
         sources = self._frame_sources(sources, masks, depth_scale, stream)
         self._whole_bank_only("detect()")
         sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
-        nat = self._select(list(class_ids))
+        nat = self._pose_native(class_ids)
         out, R, t, res, _ = nat.detect(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold), int(top_k),
                                        int(max_iterations), bool(use_scene_cloud), float(translation_threshold), estimation)
-        return self._pose_pairs(out, R, t, res)  # every kept pose has one: residual >= 0
+        return self._pose_pairs(out, R, t, res, self._verification(nat, [len(out)])[0])  # every kept pose has one: residual >= 0
 
     # ---- a batch of RGB-D frames through one pose stage (lm_detect_batch) ----
     def match_refine_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
@@ -345,11 +371,11 @@ class Detector:
         _lib.estimation_code(estimation)
         inputs, K = self._batch_inputs(frames, sceneK, masks, "match_refine_batch()", depth_scale, stream)
         self._whole_bank_only("match_refine_batch()")
-        nat = self._select(list(class_ids))
+        nat = self._pose_native(class_ids)
         call, inputs = (nat.detect_batch_device, (inputs,)) if isinstance(inputs, _lib.DeviceBatch) else (nat.detect_batch, inputs)
         got = call(*inputs, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations), bool(use_scene_cloud),
                    pose_nms=False, estimation=estimation)
-        return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+        return self._batch_pairs(nat, got)
 
     def detect_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
                      max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
@@ -358,11 +384,16 @@ class Detector:
         _lib.estimation_code(estimation)
         inputs, K = self._batch_inputs(frames, sceneK, masks, "detect_batch()", depth_scale, stream)
         self._whole_bank_only("detect_batch()")
-        nat = self._select(list(class_ids))
+        nat = self._pose_native(class_ids)
         call, inputs = (nat.detect_batch_device, (inputs,)) if isinstance(inputs, _lib.DeviceBatch) else (nat.detect_batch, inputs)
         got = call(*inputs, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations), bool(use_scene_cloud),
                    pose_nms=True, translation_threshold=float(translation_threshold), estimation=estimation)
-        return [self._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+        return self._batch_pairs(nat, got)
+
+    def _batch_pairs(self, nat, got):
+        # one [(Match, poseRefine)] list per frame of a batch call's result
+        ver = self._verification(nat, [len(g[0]) for g in got])
+        return [self._pose_pairs(out, R, t, res, v) for (out, R, t, res, _), v in zip(got, ver)]
 
     def _batch_args(self, frames, class_ids, sceneK, masks, what):
         # the sharded batch calls (dist.py), which take numpy frames: the handle, then (rgb, depth, mask pairs, K)
@@ -370,7 +401,7 @@ class Detector:
         if isinstance(inputs, _lib.DeviceBatch):
             raise TypeError("%s takes numpy frames" % what)
         self._whole_bank_only(what)
-        return self._select(list(class_ids)), inputs + (K,)
+        return self._pose_native(class_ids), inputs + (K,)
 
     def _batch_inputs(self, frames, sceneK, masks, what, depth_scale=1.0, stream=None):
         # every check that needs no device, before the native handle exists.  Returns (inputs, K): inputs is a
@@ -422,13 +453,16 @@ class Detector:
                 raise ValueError("%s: %s" % (what, e)) from None
         return (np.stack(rgb), np.stack(depth), pairs), K
 
-    def _pose_pairs(self, out, R, t, res):
-        # [(Match, poseRefine)]; a survivor without a pose (residual -1, only without the pose NMS) keeps R / t None
+    def _pose_pairs(self, out, R, t, res, ver=None):
+        # [(Match, poseRefine)]; a survivor without a pose (residual -1, only without the pose NMS) keeps R / t None.
+        # ver: per entry (score, counts) of the pose verification, or None
         from .pose_refine import poseRefine
         pairs = []
         for i, m in enumerate(self._to_matches(out)):
             p = poseRefine()
             p._residual = float(res[i])
+            if ver is not None:
+                p._score, p._verification = ver[i]
             if res[i] != -1.0:
                 p._R = R[i].copy()
                 p._t = t[i].reshape(3, 1).copy()

@@ -98,7 +98,7 @@ def match_refine_batch_sharded(detector, frames, threshold, class_ids, sceneK, i
     nat, (rgb, depth, mk, K) = _connected_batch(detector, frames, class_ids, sceneK, masks, group, "match_refine_batch_sharded()")
     got = nat.peer_detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
                                 bool(use_scene_cloud), pose_nms=False, estimation=estimation)
-    return [detector._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+    return detector._batch_pairs(nat, got)
 
 
 def detect_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
@@ -111,7 +111,7 @@ def detect_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_thr
     got = nat.peer_detect_batch(rgb, depth, mk, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations),
                                 bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold),
                                 estimation=estimation)
-    return [detector._pose_pairs(out, R, t, res) for out, R, t, res, _ in got]
+    return detector._batch_pairs(nat, got)
 
 
 def match_quantized_sharded(detector, quantized, threshold, class_ids=(), group=None):

@@ -33,6 +33,8 @@ class poseRefine:
         self._residual = -1.0
         self._R = None
         self._t = None
+        self._score = None         # pose verification (verify_mm, Detector.setPoseVerification): score, counts
+        self._verification = None
         self.device = _default_device()
 
     @staticmethod
@@ -52,11 +54,15 @@ class poseRefine:
         return a
 
     def process(self, sceneDepth, modelDepth, sceneK, modelK, modelR, modelT, detectX, detectY, depth_scale=1.0, render_scale=1.0,
-                stream=None):
+                stream=None, verify_mm=None):
         """sceneDepth / modelDepth: uint16 HxW numpy images (mm), or CUDA tensors on this object's device: uint16 (mm) or
         float32 [H, W], pixels packed within a row.  depth_scale / render_scale convert float32 depth to mm (the driver's
         depth_ren.astype(np.uint16) is render_scale 1.0); stream: the torch stream the tensors are ordered on (None: the
-        current stream)."""
+        current stream).  verify_mm (not in the reference's surface): verify the refined pose against the scene depth with
+        this inlier distance in mm (include/linemod_b200.h, lm_set_pose_verify); getScore / getVerification then return
+        the result.  None: no verification."""
+        if verify_mm is not None:
+            _lib.inlier_mm(verify_mm)
         dev = _lib.depth_inputs(sceneDepth, [modelDepth], depth_scale, render_scale, stream, self.device,
                                 host=dict(sceneK=sceneK, modelK=modelK, modelR=modelR, modelT=modelT))
         if dev is None:
@@ -69,11 +75,14 @@ class poseRefine:
         R = self._mat(modelR, np.float32, (3, 3), "modelR")
         t = self._mat(modelT, np.float32, (3,), "modelT")
         args = (sK, mK[None], R[None], t[None], [[int(detectX), int(detectY)]], self.max_iterations, self.estimation)
+        icp = _native(self.device)
+        icp.set_verify(verify_mm)
         if dev is None:
-            Ro, to, res = _native(self.device).process_batch(scene, [model], *args)
+            Ro, to, res = icp.process_batch(scene, [model], *args)
         else:
-            Ro, to, res = _native(self.device).process_batch_device(dev, *args)
+            Ro, to, res = icp.process_batch_device(dev, *args)
         self._residual = float(res[0])
+        self._score, self._verification = _lib.verify_arrays(*icp.verify())[0] if verify_mm is not None else (None, None)
         if res[0] == -1.0:  # early return: R_refined / t_refiend keep their previous value (LL.cpp:52-55)
             return
         self._R = Ro[0].copy()
@@ -88,16 +97,29 @@ class poseRefine:
     def getT(self):
         return self._t
 
+    def getScore(self):
+        """The pose verification's depth-consistency score: inlier / (inlier + occluded + violation), 0 when that sum is 0,
+        -1 without a pose; None when the call did not verify."""
+        return self._score
+
+    def getVerification(self):
+        """The pose verification's counts, a dict of n_model, outside, missing, inlier, occluded and violation (the last five
+        sum to n_model); None when the call did not verify."""
+        return self._verification
+
 
 def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, modelTs, device=None, estimation="point_to_plane",
-                   depth_scale=1.0, render_scale=1.0, stream=None):
+                   depth_scale=1.0, render_scale=1.0, stream=None, verify_mm=None):
     """The drivers' loop over the NMS survivors (linemod_and_levelup_test.py:348-367: one poseRefine per
     match, fed with the render of the matched template's pose) as ONE batched GPU call: hypothesis i is
     matches[i] (its x, y) with modelDepths[i] / modelKs[i] / modelRs[i] / modelTs[i].  Returns a list of
     poseRefine objects in the state process() would have left them in.  estimation as poseRefine().
     Depths in device memory: sceneDepth a CUDA tensor and modelDepths a list of [H, W] CUDA tensors or one [n, H, W]
-    tensor, with depth_scale, render_scale and stream as poseRefine.process."""
+    tensor, with depth_scale, render_scale and stream as poseRefine.process.  verify_mm as poseRefine.process: every
+    survivor comes back with its score, none is dropped."""
     _lib.estimation_code(estimation)
+    if verify_mm is not None:
+        _lib.inlier_mm(verify_mm)
     n = len(matches)
     dev = _default_device() if device is None else int(device)
     renders = modelDepths if _lib.is_tensor(modelDepths) else list(modelDepths)
@@ -118,12 +140,16 @@ def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, m
     R = np.stack([poseRefine._mat(r, np.float32, (3, 3), "modelR") for r in modelRs])
     t = np.stack([poseRefine._mat(v, np.float32, (3,), "modelT") for v in modelTs])
     xy = [[int(m.x), int(m.y)] for m in matches]
+    icp = _native(dev)
+    icp.set_verify(verify_mm)
     if inputs is None:
-        Ro, to, res = _native(dev).process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
+        Ro, to, res = icp.process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
     else:
-        Ro, to, res = _native(dev).process_batch_device(inputs, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
+        Ro, to, res = icp.process_batch_device(inputs, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
+    ver = _lib.verify_arrays(*icp.verify()) if verify_mm is not None else [(None, None)] * n
     for i, p in enumerate(out):
         p._residual = float(res[i])
+        p._score, p._verification = ver[i]
         if res[i] != -1.0:
             p._R = Ro[i].copy()
             p._t = to[i].reshape(3, 1).copy()

@@ -358,6 +358,55 @@ int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, double* t_o
 int lm_nms_translations(int device, int64_t n, const double* t, const double* score, double thr, int32_t* keep,
                         int64_t* n_keep);
 
+/* Pose verification on the device (default off): a depth-consistency score per refined pose, from the scene depth.
+ * For survivor / hypothesis i with a pose (no early return of LL.cpp:52-55):
+ *   1. Points: the model cloud the pose stage builds before voxel down-sampling -- every crop pixel with render depth > 0,
+ *      back-projected with the template's K as the cloud building does (metres, double, row-major crop order).
+ *      n_model is their count.
+ *   2. Pose: T, the ICP's final 4x4 transformation (row-major double, lm_icp_capture's RESULT), which maps that cloud
+ *      into the scene camera; used as is, whatever the estimation and use_scene_cloud.
+ *   3. Transform and project: q_r = ((T[r][0] p_x + T[r][1] p_y) + T[r][2] p_z) + T[r][3], every operation correctly
+ *      rounded, no FMA.  !(q_z > 0): outside.  Else u = (double)fx * (q_x / q_z) + (double)cx, v likewise with fy, cy,
+ *      each operation rounded; column c = floor(u + 0.5), row r = floor(v + 0.5).  u or v not finite, or (c, r) off
+ *      the frame: outside.
+ *   4. Compare: z_s = scene depth at (r, c) (u16 mm), z_q = q_z * 1000 (mm).  z_s == 0: missing.  Else d = (double)z_s -
+ *      z_q: |d| <= delta inlier, d < -delta occluded (something lies in front of the model), d > delta violation (the
+ *      scene lies behind the model's surface, which would hide it).
+ *   5. Outputs: six int32 counts n_model, outside, missing, inlier, occluded, violation (the last five sum to n_model),
+ *      and score = inlier / (inlier + occluded + violation) as float (__fdiv_rn), 0 when that sum is 0.  A survivor
+ *      without a pose: score -1 and zero counts (as its residual -1).  A NaN pose (zero anchor depth) puts every point
+ *      outside: score 0.
+ *   6. delta: inlier_mm, finite and >= 0; 10 mm (the ICP's correspondence radius) is the usual choice.
+ * This is the surface the template's render sees, moved by T -- not a render at the refined pose: points the render hid
+ * stay hidden, and faces the refined pose would newly show are not checked.  A score says how well the scene agrees
+ * with that surface; it does not by itself tell a true object from a false one.
+ * With verification on, the pose NMS can use it:
+ *   rank_by  LM_VERIFY_RANK_FITNESS: today's score -(double)residual (the default); LM_VERIFY_RANK_SCORE: the
+ *            verification score, descending.  Either way equal keys keep box-NMS pick order.
+ *   min_score  a posed survivor whose score is below it is no pose-NMS candidate: it is neither kept nor suppresses
+ *            others, as one without a pose.  -INFINITY: no minimum.
+ * Without the pose NMS every survivor comes back with its score; nothing is dropped.
+ *   lm_set_pose_verify   for the detector's next lm_enqueue_pose, lm_detect_batch and lm_peer_detect_batch; a frame keeps
+ *                        the setting it was enqueued with (the replay after a result-block retry included).  No device
+ *                        work.  With a connected peer exchange every rank sets the same value.  LM_E_INVALID for a NaN
+ *                        or negative inlier_mm, an unknown rank_by, a NaN min_score, and for LM_VERIFY_RANK_SCORE or a
+ *                        min_score other than -INFINITY with on == 0.  Each chunk of a pose stage takes one more launch
+ *                        (k_pose_verify behind the ICP kernel).  A pose stage shared over the ranks (lm_peer_share_pose)
+ *                        verifies each survivor on the rank that refined it, and its result travels with the pose: every
+ *                        rank returns what the unshared stage returns.  The device buffers for the results are allocated
+ *                        by the first run that verifies.
+ *   lm_pose_verify       score[k], counts6 + 6k of entry k of the last completed frame or batch (lm_complete_pose /
+ *                        lm_complete_detect / lm_detect_batch), in the order of its entries; *n their number.
+ *                        LM_E_STATE when that run did not verify, LM_E_CAPACITY (with *n) when cap is smaller.
+ *   lm_pose_verify_points  steps 3-5 on caller arrays with the same device routine: pts [n][3] f64 (m), T [16] f64,
+ *                        scene rows x cols u16 mm, sK [9] f32. */
+#define LM_VERIFY_RANK_FITNESS 0
+#define LM_VERIFY_RANK_SCORE 1
+int lm_set_pose_verify(lm_detector* d, int on, double inlier_mm, int rank_by, double min_score);
+int lm_pose_verify(lm_detector* d, float* score, int32_t* counts6, int64_t cap, int64_t* n);
+int lm_pose_verify_points(int device, const double* pts, int64_t n, const double* T, const uint16_t* scene, int rows, int cols,
+                          const float* sK, double inlier_mm, int32_t* counts6, float* score);
+
 /* A batch of RGB-D frames in one call: each frame's match and box NMS, then one pose stage and (pose_nms) one pose NMS
  * for the survivors of every frame.  Frame f is rgb + f * rows * cols * 3 and depth + f * rows * cols (all frames one
  * size), masks[2f] / masks[2f + 1] its colour and depth masks (masks NULL: none), sceneK + 9f its intrinsics.  The other
@@ -606,9 +655,10 @@ int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, i
                                 void* stream);
 
 /* Of the last hypothesis processed: [0] points in the down-sampled cloud, [1] ICP iterations run,
- * [2] inlier rmse (m), [3] device time of the normals + ICP kernels of the last call (us); after
- * lm_icp_process_batch_device the device time from its input copy to the end of its last ICP kernel, the box read-back
- * included. */
+ * [2] inlier rmse (m), [3] device time of the last call (us).  After lm_icp_process_batch: the normals and ICP kernels
+ * only; a verification (lm_icp_set_verify) runs behind them and is not included.  After lm_icp_process_batch_device: from
+ * its input copy to the end of its last chunk's kernels, the box read-back included, and k_pose_verify included when the
+ * call verifies. */
 int lm_icp_last_stats(lm_icp* h, double* out4);
 /* NOT the reference's behaviour (default off): register the model cloud against the down-sampled SCENE
  * cloud, which is what LL.cpp:109 evidently meant to do (it down-samples the model cloud twice). */
@@ -618,6 +668,12 @@ int lm_icp_set_use_scene_cloud(lm_icp* h, int on);
  * LM_E_INVALID for any other value. */
 int lm_icp_set_estimation(lm_icp* h, int estimation);
 int64_t lm_icp_launch_count(lm_icp* h);
+/* Pose verification (see lm_set_pose_verify) for the next lm_icp_process_batch and lm_icp_process_batch_device: one more
+ * launch per call (per chunk of 1024 hypotheses on the device path); the host path also uploads its raw model clouds and
+ * the scene.  lm_icp_last_stats [3] includes that launch on the device path only.  lm_icp_verify: score[k], counts6 + 6k of hypothesis k of the last call, *n the hypotheses;
+ * LM_E_STATE when that call did not verify.  LM_E_INVALID for a NaN or negative inlier_mm. */
+int lm_icp_set_verify(lm_icp* h, int on, double inlier_mm);
+int lm_icp_verify(lm_icp* h, float* score, int32_t* counts6, int64_t cap, int64_t* n);
 
 /* ---- introspection of the ICP kernels, used by the stage-by-stage tests ---- */
 /* While capture is on (default off), lm_icp_process_batch keeps, per hypothesis, what its kernels saw and kept in the
