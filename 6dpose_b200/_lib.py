@@ -6,6 +6,7 @@ for the hot path.
 import ctypes
 import math
 import os
+import re
 import sys
 
 import numpy as np
@@ -15,6 +16,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LINEMOD_B200_LIB") or os.path.join(_HERE, "csrc", "liblinemod_b200.so")
 
 LM_OK, LM_E_INVALID, LM_E_CUDA, LM_E_STATE, LM_E_CAPACITY = 0, -1, -2, -3, -4
+# capture items of lm_icp_capture and lm_debug_pose_clouds (include/linemod_b200.h)
+CAPTURE_ITEMS = dict(counts=0, source=1, target=2, normals=3, init=4, result=5, knn=6, corr_first=7, corr_last=8, slots=9, posed=10,
+                     raw_model=11, raw_scene=12)
 SHARD_CONTIGUOUS, SHARD_INTERLEAVED = 0, 1
 
 MATCH_DTYPE = np.dtype([("x", "<i4"), ("y", "<i4"), ("similarity", "<f4"), ("class_index", "<i4"), ("template_id", "<i4")])
@@ -27,7 +31,7 @@ PEER_HANDLE_BYTES = 64
 SYMBOLS = [
     "lm_last_error", "lm_create", "lm_destroy", "lm_load_bank", "lm_select", "lm_select_layout", "lm_shard_range", "lm_prepare", "lm_coarse_tasks", "lm_coarse_descriptors",
     "lm_upload_quantized", "lm_upload_images", "lm_match_images", "lm_debug_quantized", "lm_bind_quantized_device",
-    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_debug_plan", "lm_debug_coarse", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
+    "lm_bind_images_device", "lm_detect_batch_device", "lm_debug_depth", "lm_debug_plan", "lm_debug_coarse", "lm_debug_pose_clouds", "lm_run", "lm_enqueue", "lm_complete", "lm_set_result_buffer", "lm_device_result", "lm_fetch_records",
     "lm_finish", "lm_match_quantized", "lm_debug_linear_memories", "lm_debug_time_k1", "lm_debug_bit_planes", "lm_counters", "lm_set_timing",
     "lm_stage_times", "lm_stream", "lm_launch_count",
     "lm_set_boxes", "lm_enqueue_post", "lm_complete_post", "lm_match_top",
@@ -403,6 +407,7 @@ def load():
     L.lm_debug_depth.argtypes = [vp, u16p, c_i64]
     L.lm_debug_plan.argtypes = [vp, i32p, c_i64]
     L.lm_debug_coarse.argtypes = [vp, ctypes.POINTER(ctypes.c_uint32), c_i64, u16p, c_i64, i32p]
+    L.lm_debug_pose_clouds.argtypes = [vp, c_int, c_int, vp, c_i64]
     L.lm_nms_translations.argtypes = [c_int, c_i64, f64p, f64p, ctypes.c_double, i32p, ctypes.POINTER(c_i64)]
     L.lm_set_pose_verify.argtypes = [vp, c_int, ctypes.c_double, c_int, ctypes.c_double]
     L.lm_pose_verify.argtypes = [vp, f32p, i32p, c_i64, ctypes.POINTER(c_i64)]
@@ -1025,6 +1030,38 @@ class NativeDetector:
                                           self._i32(dims)))
         return mask, raw
 
+    def _pose_item(self, slot, what, out):
+        check(self._L.lm_debug_pose_clouds(self._h, int(slot), CAPTURE_ITEMS[what], out.ctypes.data_as(ctypes.c_void_p), out.nbytes))
+        return out
+
+    def pose_clouds(self):
+        """The clouds of the last pose-stage chunk this handle enqueued (lm_debug_pose_clouds): (head, slots).  head is a
+        dict of the chunk's slots, rank, world and first (slot i holds survivor first + rank + i * world); slots has one
+        dict per slot: posed (bool) and, where posed, counts (src, tgt), source / target [n,3] f64 (down-sampled), init
+        [4,4] f64, raw_model / raw_scene [n,3] f64 (before down-sampling)."""
+        head = self._pose_item(-1, "slots", np.zeros(4, np.int32))
+        out = []
+        for i in range(int(head[0])):
+            posed = bool(self._pose_item(i, "posed", np.zeros(1, np.uint8))[0])
+            d = dict(posed=posed)
+            if posed:
+                n, nt = self._pose_item(i, "counts", np.zeros(2, np.int32)).tolist()
+                d.update(counts=(n, nt), source=self._pose_item(i, "source", np.zeros((n, 3))),
+                         target=self._pose_item(i, "target", np.zeros((nt, 3))), init=self._pose_item(i, "init", np.zeros((4, 4))))
+                for item in ("raw_model", "raw_scene"):  # sized by asking: LM_E_CAPACITY names the bytes
+                    d[item] = self._pose_raw(i, item)
+            out.append(d)
+        return dict(zip(("slots", "rank", "world", "first"), [int(v) for v in head])), out
+
+    def _pose_raw(self, slot, what):
+        rc = self._L.lm_debug_pose_clouds(self._h, int(slot), CAPTURE_ITEMS[what], ctypes.byref(ctypes.c_uint8()), 0)
+        if rc == LM_OK:
+            return np.zeros((0, 3))
+        if rc != LM_E_CAPACITY:
+            check(rc)
+        need = int(re.search(r"needs (\d+) bytes", self._L.lm_last_error().decode()).group(1))
+        return self._pose_item(slot, what, np.zeros((need // 24, 3)))
+
     def set_timing(self, slots):
         check(self._L.lm_set_timing(self._h, int(slots)))
 
@@ -1069,6 +1106,7 @@ class NativeIcp:
         self.device = int(device)
         self._estimation = "point_to_plane"  # the handle's estimation (lm_icp_set_estimation)
         self._captured = None               # the estimation of the last process_batch (capture())
+        self._captured_device = False       # the last call was process_batch_device: clouds, init and result only
 
     def close(self):
         if getattr(self, "_h", None):
@@ -1111,6 +1149,7 @@ class NativeIcp:
                                            int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
                                            res.ctypes.data_as(f32p)))
         self._captured = self._estimation
+        self._captured_device = False
         return Ro, to, res
 
     def process_batch_device(self, depths, sceneK, modelKs, Rs, ts, detect_xy, max_iterations=30, estimation=None):
@@ -1137,6 +1176,8 @@ class NativeIcp:
                                                   t.ctypes.data_as(f32p), xy.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
                                                   int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
                                                   res.ctypes.data_as(f32p), depths.stream.cuda_stream))
+        self._captured = self._estimation
+        self._captured_device = True
         return Ro, to, res
 
     def set_use_scene_cloud(self, on):
@@ -1167,10 +1208,17 @@ class NativeIcp:
         """What the kernels saw and kept for hypothesis `hyp` of the last process_batch with capture on (see
         lm_icp_capture): source / target [n,3] f64, normals [nt,3] f64, init [4,4] f64, T [4,4] f64, fitness, rmse,
         iterations, knn [nt,30] int32 (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence).  After a
-        point-to-point call normals and knn are None: that estimation computes neither."""
+        point-to-point call normals and knn are None: that estimation computes neither.  After process_batch_device
+        normals, knn, corr_first and corr_last are None: that path keeps the clouds, init and result only."""
         n, nt = self._capture_item(hyp, 0, np.zeros(2, np.int32)).tolist()
         res = self._capture_item(hyp, 5, np.zeros(19, np.float64))
         p2pl = self._captured != "point_to_point"
+        if self._captured_device:
+            return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
+                        target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)), normals=None,
+                        init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
+                        T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
+                        knn=None, corr_first=None, corr_last=None)
         return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
                     target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)),
                     normals=self._capture_item(hyp, 3, np.zeros((nt, 3), np.float64)) if p2pl else None,

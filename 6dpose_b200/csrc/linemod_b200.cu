@@ -2412,6 +2412,15 @@ extern "C" int lm_pose_verify(lm_detector* d, float* score, int32_t* counts6, in
   return pose_stage_verify(d->pose, score, counts6, cap, n);
 }
 
+extern "C" int lm_debug_pose_clouds(lm_detector* d, int slot, int what, void* out, int64_t cap) {
+  if (!d || !out) return fail(LM_E_INVALID, "null argument");
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle");
+  if (!d->pose) return fail(LM_E_STATE, "no pose stage has run");
+  CU(cudaSetDevice(d->device));
+  CU(cudaStreamSynchronize(d->stream.get()));
+  return pose_stage_clouds(d->pose, slot, what, out, cap);
+}
+
 extern "C" int lm_set_template_depths(lm_detector* d, int64_t first, int64_t n, const float* z_mm) {
   if (!d) return fail(LM_E_INVALID, "null detector");
   if (first < 0 || n < 0 || first + n > d->G)

@@ -689,11 +689,12 @@ struct lm_icp {
   int last_points = 0, last_iterations = 0;
   double last_rmse = 0;
   float last_kernel_us = 0;
-  // lm_icp_set_capture: the kernels' intermediate results of the last lm_icp_process_batch
+  // lm_icp_set_capture: the kernels' intermediate results of the last lm_icp_process_batch (or _device)
   bool capture = false;
   DeviceArray<int32_t> d_knn, d_corr;  // [points][ICP_KNN], [points][2]
   struct {
     int estimation = LM_ICP_POINT_TO_PLANE;  // point-to-point computes no normals and no neighbour lists
+    bool device = false;                     // lm_icp_process_batch_device: clouds, initial guesses and results only
     std::vector<IcpJob> jobs;
     std::vector<int> job_of;  // per hypothesis, -1: early return
     std::vector<IcpOut> outs;
@@ -746,10 +747,11 @@ struct Cloud {
   double init[16];
   float base[16];  // init_base, row-major
   bool early = false;
+  bool unkeyed = false;  // a point's voxel index is not finite or beyond int64 (a zero or non-finite K)
 };
 
 // LL.cpp:34-109 for one hypothesis.
-void voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out);
+bool voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out);
 
 // init_base = [R | t] with only t.z converted to metres (LL.cpp:34-38)
 void init_base(const float* R, const float* t, float* base) {
@@ -853,27 +855,31 @@ void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* mo
   for (int k = 0; k < 3; ++k) { cm[k] /= nm; cs[k] /= (double)ncs; }  // 0/0 -> NaN as in the reference
   for (int i = 0; i < 16; ++i) c.init[i] = (i % 5 == 0) ? 1.0 : 0.0;
   for (int k = 0; k < 3; ++k) c.init[4 * k + 3] = cs[k] - cm[k];
-  voxel_down_sample(mp, c.pts);
-  if (want_scene) voxel_down_sample(sp, c.scene);
+  c.unkeyed = !voxel_down_sample(mp, c.pts);
+  if (want_scene && !voxel_down_sample(sp, c.scene)) c.unkeyed = true;
   if (want_raw) c.raw = std::move(mp);
 }
 
 // PointCloud::VoxelDownSample(0.0025) (LL.cpp:106-109): mean of the points of every occupied voxel;
-// Open3D emits them in hash-map order, here in sorted voxel order (affects summation order only).
-void voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out) {
+// Open3D emits them in hash-map order, here in sorted voxel order (affects summation order only).  False (out empty)
+// when a voxel index is NaN or beyond int64, which no conversion to an integer key can hold.
+bool voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out) {
   const double voxel = 0.0025;
   const size_t n = mp.size() / 3;
   out.clear();
-  if (n == 0) return;
+  if (n == 0) return true;
   double mn[3] = {mp[0], mp[1], mp[2]};
   for (size_t i = 1; i < n; ++i)
     for (int k = 0; k < 3; ++k) mn[k] = std::min(mn[k], mp[3 * i + k]);
   struct Key { int64_t a, b, c; size_t i; };
   std::vector<Key> keys(n);
   for (size_t i = 0; i < n; ++i) {
-    keys[i].a = (int64_t)floor((mp[3 * i] - (mn[0] - voxel * 0.5)) / voxel);
-    keys[i].b = (int64_t)floor((mp[3 * i + 1] - (mn[1] - voxel * 0.5)) / voxel);
-    keys[i].c = (int64_t)floor((mp[3 * i + 2] - (mn[2] - voxel * 0.5)) / voxel);
+    double v[3];
+    for (int k = 0; k < 3; ++k) {
+      v[k] = floor((mp[3 * i + k] - (mn[k] - voxel * 0.5)) / voxel);
+      if (!(v[k] >= -9223372036854775808.0 && v[k] < 9223372036854775808.0)) return false;
+    }
+    keys[i].a = (int64_t)v[0]; keys[i].b = (int64_t)v[1]; keys[i].c = (int64_t)v[2];
     keys[i].i = i;
   }
   std::stable_sort(keys.begin(), keys.end(), [](const Key& p, const Key& q) {
@@ -891,6 +897,7 @@ void voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out) 
     for (int k = 0; k < 3; ++k) out.push_back(acc[k] / (double)(e - s));
     s = e;
   }
+  return true;
 }
 
 }  // namespace
@@ -908,6 +915,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
   CUI(cudaSetDevice(h->device));
   h->verified = false;
+  h->cap.job_of.clear();  // a call that fails keeps no capture
   std::vector<Cloud> clouds((size_t)n_hyp);
   std::vector<IcpJob> jobs;
   std::vector<int> job_of((size_t)n_hyp, -1);
@@ -928,6 +936,9 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     for (int i = 16; i < n_hyp; ++i) build(i);
     for (std::thread& w : workers) w.join();
   }
+  for (int i = 0; i < n_hyp; ++i)
+    if (clouds[i].unkeyed)
+      return lm_fail(LM_E_INVALID, "hypothesis %d: a cloud point has no voxel index (NaN or beyond int64: a zero or non-finite K?)", i);
   for (int i = 0; i < n_hyp; ++i) {
     if (clouds[i].early) continue;
     IcpJob j;
@@ -999,6 +1010,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   if (h->capture) {
     auto& c = h->cap;
     c.estimation = h->estimation;
+    c.device = false;
     c.jobs = jobs;
     c.job_of = job_of;
     c.outs.assign(h->h_outs.get(), h->h_outs.get() + (jobs.empty() ? 0 : jobs.size()));
@@ -1098,6 +1110,9 @@ extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t c
   double res[19];
   if ((what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN) && c.estimation != LM_ICP_POINT_TO_PLANE)
     return lm_fail(LM_E_STATE, "capture item %d: the point-to-point estimation computes no normals or neighbour lists", what);
+  if (c.device && (what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN || what == LM_ICP_CAPTURE_CORR_FIRST ||
+                   what == LM_ICP_CAPTURE_CORR_LAST))
+    return lm_fail(LM_E_STATE, "capture item %d: lm_icp_process_batch_device keeps no normals, neighbour lists or correspondences", what);
   switch (what) {
     case LM_ICP_CAPTURE_COUNTS:
       tmp = {j.src_count, j.tgt_count};
@@ -1768,6 +1783,15 @@ struct lm_pose_stage {
   // the verification of the entries of the run last finished (pose_stage_verify); verified false: it did not verify
   bool verified = false;
   std::vector<PoseVerify> ver;
+  // the last chunk pose_chunk enqueued (pose_stage_clouds): its slots, rank and world, its first survivor in the run and
+  // its posed flags per slot.  valid false before the first chunk and from the next pose_prepare on, which may move the
+  // buffers.
+  struct {
+    bool valid = false;
+    int slots = 0, rank = 0, world = 1;
+    int64_t first = 0;
+    const uint8_t* posed = nullptr;
+  } last;
 };
 
 // The per-chunk buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
@@ -1919,6 +1943,7 @@ struct PoseChunk {
   const lm_match* surv;
   const int32_t* counts;
   int slots;
+  int64_t first;    // the run's index of surv[0]
   const uint16_t* scene;
   const int32_t* frame_of;
   const float* sKs;
@@ -1985,7 +2010,68 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
     if (o.verify.on) k_pose_verify<false><<<n, VERIFY_THREADS, 0, st>>>(p, c.outs, o.verify.inlier_mm, c.ver, PoseShareDev());
   }
   CUI(cudaGetLastError());
+  s->last.valid = true;
+  s->last.slots = n; s->last.rank = p.rank; s->last.world = world;
+  s->last.first = c.first;
+  s->last.posed = p.posed;
   return (sh ? 6 : 5) - (normals ? 0 : 1) + (o.verify.on ? 1 : 0);
+}
+
+int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int64_t cap) {
+  if (!out) return lm_fail(LM_E_INVALID, "null argument");
+  const auto& l = s->last;
+  if (!l.valid) return lm_fail(LM_E_STATE, "no pose stage has run since the buffers last changed");
+  int32_t head[4];
+  uint8_t posed = 0;
+  IcpJob j;
+  int32_t seg[2] = {0, 0};
+  const void* src = nullptr;
+  int64_t bytes = 0;
+  bool host = true;  // src is a host copy
+  if (what == LM_POSE_CAPTURE_SLOTS) {
+    if (slot != -1) return lm_fail(LM_E_INVALID, "LM_POSE_CAPTURE_SLOTS takes slot -1, not %d", slot);
+    head[0] = l.slots; head[1] = l.rank; head[2] = l.world; head[3] = (int32_t)l.first;
+    src = head; bytes = sizeof(head);
+  } else {
+    if (slot < 0 || slot >= l.slots) return lm_fail(LM_E_INVALID, "slot %d outside the %d of the last chunk", slot, l.slots);
+    if (what != LM_POSE_CAPTURE_POSED && what != LM_ICP_CAPTURE_COUNTS && what != LM_ICP_CAPTURE_SOURCE &&
+        what != LM_ICP_CAPTURE_TARGET && what != LM_ICP_CAPTURE_INIT && what != LM_POSE_CAPTURE_RAW_MODEL &&
+        what != LM_POSE_CAPTURE_RAW_SCENE)
+      return lm_fail(LM_E_INVALID, "unknown pose stage capture item %d", what);
+    CUI(cudaMemcpy(&posed, l.posed + slot, 1, cudaMemcpyDeviceToHost));
+    if (what == LM_POSE_CAPTURE_POSED) {
+      src = &posed; bytes = 1;
+    } else {
+      if (!posed) return lm_fail(LM_E_STATE, "slot %d has no pose (no template, or its box leaves the frame): no cloud", slot);
+      CUI(cudaMemcpy(&j, s->d_jobs.get() + slot, sizeof(j), cudaMemcpyDeviceToHost));
+      const int k = 2 * slot + (what == LM_POSE_CAPTURE_RAW_SCENE ? 1 : 0);  // seg_end follows the chunk's 2 slots begins
+      CUI(cudaMemcpy(&seg[0], s->d_seg.get() + k, sizeof(int32_t), cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(&seg[1], s->d_seg.get() + 2 * l.slots + k, sizeof(int32_t), cudaMemcpyDeviceToHost));
+      switch (what) {
+        case LM_ICP_CAPTURE_COUNTS:
+          head[0] = j.src_count; head[1] = j.tgt_count;
+          src = head; bytes = 2 * sizeof(int32_t);
+          break;
+        case LM_ICP_CAPTURE_SOURCE:
+          src = s->d_pts.get() + (size_t)j.src_first * 3; bytes = (int64_t)j.src_count * 3 * sizeof(double); host = false;
+          break;
+        case LM_ICP_CAPTURE_TARGET:
+          src = s->d_pts.get() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double); host = false;
+          break;
+        case LM_ICP_CAPTURE_INIT:
+          src = j.init; bytes = sizeof(j.init);
+          break;
+        default:  // RAW_MODEL, RAW_SCENE
+          src = s->d_raw.get() + (size_t)seg[0] * 3; bytes = (int64_t)(seg[1] - seg[0]) * 3 * sizeof(double); host = false;
+          break;
+      }
+    }
+  }
+  if (cap < bytes) return lm_fail(LM_E_CAPACITY, "pose stage capture item %d of slot %d needs %lld bytes, cap is %lld", what, slot,
+                                  (long long)bytes, (long long)cap);
+  if (bytes && host) memcpy(out, src, (size_t)bytes);
+  if (bytes && !host) CUI(cudaMemcpy(out, src, (size_t)bytes, cudaMemcpyDeviceToHost));
+  return LM_OK;
 }
 
 #define POSE_CHUNK 1024     // survivor slots per chunk: a frame's bound for top_k = 0
@@ -2029,6 +2115,7 @@ static int pose_outputs(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t
 // The renders on the device and every buffer a run of n_frames frames and S survivors needs (verify: a verifying run's
 // too).
 static int pose_prepare(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S, bool verify) {
+  s->last.valid = false;
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
@@ -2101,6 +2188,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
     k.surv = run.d_surv + c0;
     k.counts = batch ? s->d_bstat.get() + 4 * c + 3 : run.d_counts;
     k.slots = batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound;
+    k.first = c0;
     k.scene = run.d_scene; k.frame_of = batch ? s->d_bframe.get() + c0 : nullptr;
     k.sKs = batch ? s->d_bsK.get() : nullptr; k.sK = batch ? nullptr : run.sK;
     k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.ver = s->d_bver.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
@@ -2498,7 +2586,6 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     return lm_fail(LM_E_INVALID, "null argument");
   if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
   if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
-  if (h->capture) return lm_fail(LM_E_STATE, "capture is on: it records lm_icp_process_batch's host-built clouds only");
   int rc = check_depth_format("scene_depth", scene_format, scene_scale);
   if (!rc) rc = check_depth_format("model_depths", model_format, model_scale);
   if (rc) return rc;
@@ -2513,9 +2600,27 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   }
   if (rc) return rc;
   h->verified = false;
+  // capture: what each posed hypothesis's chunk built, copied out behind the chunk; kept only when the call succeeds
+  std::vector<IcpJob> cjobs;
+  std::vector<int> cjob_of((size_t)n_hyp, -1);
+  std::vector<double> cpts;
+  auto keep_capture = [&](const IcpOut* outs) {
+    auto& c = h->cap;
+    c.estimation = h->estimation;
+    c.device = true;
+    c.jobs = cjobs;
+    c.job_of = cjob_of;
+    c.outs.clear();
+    for (int i = 0; i < n_hyp; ++i)
+      if (cjob_of[(size_t)i] >= 0) c.outs.push_back(outs[i]);
+    c.pts = cpts;
+    c.nrm.clear(); c.knn.clear(); c.corr.clear();
+  };
+  if (h->capture) h->cap.job_of.clear();
   if (n_hyp == 0) {
     h->ver.clear();
     h->verified = h->verify;
+    if (h->capture) keep_capture(nullptr);
     return LM_OK;
   }
   CUI(cudaSetDevice(h->device));
@@ -2600,6 +2705,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
       for (PoseVerify& v : h->ver) v.score = -1.f;
       h->verified = true;
     }
+    if (h->capture) keep_capture(nullptr);
     return LM_OK;
   }
   CUI(cudaMemsetAsync(d.status.get(), 0, sizeof(int32_t) * 4 * nc, st));
@@ -2614,7 +2720,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     const int c0 = c * POSE_CHUNK;
     PoseChunk k;
     k.table = table;
-    k.surv = d_surv + c0; k.counts = d_cnt + c; k.slots = cnt[c];
+    k.surv = d_surv + c0; k.counts = d_cnt + c; k.slots = cnt[c]; k.first = c0;
     k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK;
     k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.ver = h->verify ? d.ver.get() + c0 : nullptr;
     k.status = d.status.get() + 4 * c; k.seq = 0;
@@ -2623,6 +2729,35 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     h->launches += l;
     if (last >= c0 && last < c0 + cnt[c])  // the chunk's jobs are overwritten by the next chunk's
       CUI(cudaMemcpyAsync(d.h_status.get() + 4 * nc, &d.stage.d_jobs.get()[last - c0].src_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (h->capture) {  // the chunk's jobs and clouds, before the next chunk reuses the buffers
+      CUI(cudaStreamSynchronize(st));
+      std::vector<IcpJob> jobs((size_t)cnt[c]);
+      CUI(cudaMemcpy(jobs.data(), d.stage.d_jobs.get(), sizeof(IcpJob) * jobs.size(), cudaMemcpyDeviceToHost));
+      auto append = [&](int32_t first, int32_t count) {  // points [first, first + count) of the stage's clouds -> cpts
+        const size_t at = cpts.size();
+        cpts.resize(at + (size_t)count * 3);
+        if (count) CUI(cudaMemcpy(cpts.data() + at, d.stage.d_pts.get() + (size_t)first * 3, sizeof(double) * 3 * count, cudaMemcpyDeviceToHost));
+        return LM_OK;
+      };
+      for (int i = 0; i < cnt[c]; ++i) {
+        if (!posed[(size_t)(c0 + i)]) continue;
+        IcpJob j = jobs[(size_t)i];
+        const bool own_target = j.tgt_first != j.src_first;
+        const int32_t src_at = (int32_t)(cpts.size() / 3);
+        rc = append(j.src_first, j.src_count);
+        if (!rc && own_target) {
+          const int32_t tgt_at = (int32_t)(cpts.size() / 3);
+          rc = append(j.tgt_first, j.tgt_count);
+          j.tgt_first = tgt_at;
+        } else {
+          j.tgt_first = src_at;
+        }
+        if (rc) return rc;
+        j.src_first = src_at;
+        cjob_of[(size_t)(c0 + i)] = (int)cjobs.size();
+        cjobs.push_back(j);
+      }
+    }
   }
   CUI(cudaEventRecord(h->ev1.get(), st));
   CUI(cudaMemcpyAsync(d.h_outs.get(), d.outs.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
@@ -2648,6 +2783,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     h->ver.assign(d.h_ver.get(), d.h_ver.get() + n);
     h->verified = true;
   }
+  if (h->capture) keep_capture(d.h_outs.get());
   h->last_points = d.h_status[4 * (size_t)nc];
   h->last_iterations = d.h_outs[(size_t)last].iterations;
   h->last_rmse = d.h_outs[(size_t)last].rmse;

@@ -100,6 +100,10 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
 // verify, LM_E_CAPACITY (with *n) beyond cap.
 int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, int64_t cap, int64_t* n);
 
+// Slot `slot`'s item `what` of the last chunk enqueued (lm_debug_pose_clouds), after the caller has synchronised the
+// stream.  Launches nothing.
+int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int64_t cap);
+
 // A batch's scene and survivor slots: room for n_frames scene depths of frame_pixels each (frame f at d_scene + f *
 // frame_pixels) and max_surv survivors, which the caller fills on the stream.  It also uploads the renders and grows
 // every buffer the run needs for max_surv survivors, so that the batch allocates no device memory once its frames run.

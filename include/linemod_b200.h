@@ -282,7 +282,9 @@ int lm_match_top(lm_detector* d, const uint8_t* const* quantized, const int* row
  * the device.  Per frame the device builds the clouds (scan-compacted in row-major order), the centroids and the
  * voxel down-sampling (CUB segmented radix sort + voxel means) and runs the ICP kernels; only the survivors and their
  * poses come back.  Clouds, initial guesses, R, t and residual are bit-identical to lm_icp_process_batch on the same
- * survivors and renders, NaN patterns included.
+ * survivors and renders, NaN patterns included (lm_debug_pose_clouds shows the clouds), except where a cloud spans more
+ * than 2^21 voxels of 2.5 mm along an axis (a tiny, zero or non-finite K): the device then fails the frame with
+ * LM_E_INVALID, while lm_icp_process_batch fails only where a voxel index is NaN or beyond int64 (a zero or non-finite K).
  *   lm_set_template_renders  templates [first, first+n) of the bank (bank order, as lm_set_boxes); depths[i] is
  *                            rows x cols u16 mm, K + 9i / R + 9i row-major f32, t + 3i f32 mm.  May be called in
  *                            several ranges.  LM_E_INVALID for a render without a non-zero pixel or a range outside
@@ -572,6 +574,26 @@ int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap);
  * the next lm_enqueue, and while the bank, the selection and the frame size stay as they were; after a batch, its last
  * frame. */
 int lm_debug_coarse(lm_detector* d, uint32_t* mask, int64_t mask_cap, uint16_t* raw, int64_t raw_cap, int32_t* dims3);
+/* Test getter: the clouds the device pose stage built for the last chunk this handle enqueued (a frame is one chunk, a
+ * batch one per 1024 survivors), copied from the stage's buffers to `out` (cap bytes).  Synchronises the stream and
+ * launches nothing.  slot -1 with LM_POSE_CAPTURE_SLOTS: 4 int32 -- the chunk's slots, this rank's rank and world (0 and 1
+ * unless the stage was shared, lm_peer_share_pose) and the run's index `first` of the chunk's first survivor: slot i
+ * holds survivor first + rank + i * world (a batch's survivors in frame order).  Per slot:
+ *   LM_POSE_CAPTURE_POSED      1 uint8: 1 when the survivor has a template whose box fits the frame (LL.cpp:52-55)
+ *   LM_ICP_CAPTURE_COUNTS      2 int32: points of the down-sampled source and target clouds
+ *   LM_ICP_CAPTURE_SOURCE      source cloud (the down-sampled model cloud), src x 3 f64
+ *   LM_ICP_CAPTURE_TARGET      target cloud, tgt x 3 f64 (the source again unless use_scene_cloud)
+ *   LM_ICP_CAPTURE_INIT        initial guess, 16 f64 row-major
+ *   LM_POSE_CAPTURE_RAW_MODEL  the model cloud before down-sampling (what k_pose_verify reads), row-major pixel order
+ *   LM_POSE_CAPTURE_RAW_SCENE  the scene cloud before down-sampling (empty without use_scene_cloud)
+ * LM_E_STATE before any pose stage has run (and after a later one failed before it enqueued a chunk), and for every
+ * item but POSED of a slot without a pose; LM_E_CAPACITY when cap is too small; LM_E_INVALID for a slot outside the chunk or an
+ * item not listed.  Describes the last chunk only, until the next pose stage is enqueued. */
+#define LM_POSE_CAPTURE_SLOTS 9
+#define LM_POSE_CAPTURE_POSED 10
+#define LM_POSE_CAPTURE_RAW_MODEL 11
+#define LM_POSE_CAPTURE_RAW_SCENE 12
+int lm_debug_pose_clouds(lm_detector* d, int slot, int what, void* out, int64_t cap);
 /* Counters of the last lm_run: [0] templates scanned, [1] coarse candidates, [2] algorithmic bytes of
  * the coarse scan (sum over templates, modalities of features x positions; SURVEY 8d),
  * [3] algorithmic bytes of the refinement (features x 256 per refined candidate and level: the reference's work,
@@ -633,9 +655,11 @@ int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int 
  *              (u16 mm, as is) or LM_DEPTH_F32 (float32 d to u16 mm with scene_scale / model_scale, exactly as
  *              lm_bind_images_device converts it).  sceneK, modelK, R, t, detect_xy and the outputs are host arrays, as
  *              in lm_icp_process_batch.
- *   Semantics  R_out, t_out and residual are bit for bit lm_icp_process_batch's on the converted u16 images, for every
- *              input: the early return of LL.cpp:52-55 (residual -1, R_out / t_out untouched), all-zero renders, a zero
- *              anchor and the NaN patterns they give included.  The handle's estimation and use_scene_cloud apply.
+ *   Semantics  R_out, t_out and residual are bit for bit lm_icp_process_batch's on the converted u16 images: the early
+ *              return of LL.cpp:52-55 (residual -1, R_out / t_out untouched), all-zero renders, a zero anchor and the
+ *              NaN patterns they give included.  Where a cloud spans more than 2^21 voxels along an axis the call fails
+ *              with LM_E_INVALID instead (lm_set_template_renders' pose stage).  The handle's estimation and
+ *              use_scene_cloud apply.
  *   Ordering   as lm_bind_images_device: an event recorded on `stream` (a cudaStream_t; NULL = the legacy default stream)
  *              gates the reads, and `stream` waits on a second event behind the last read.  The call returns once the
  *              outputs are on the host; it synchronises the handle's stream only (twice: the render boxes are read back
@@ -645,8 +669,9 @@ int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int 
  * LM_E_INVALID before any device work for a null argument, an empty image, max_iterations < 0, an unknown format, a
  * non-finite or non-positive scale with LM_DEPTH_F32, a stream of another device, a plane that is not device memory of
  * the handle's device or whose pitch is shorter than a row or not aligned to its elements; LM_E_INVALID after the box
- * read-back for a render whose box has 2^21 pixels or more (lm_set_template_renders' limit).  LM_E_STATE while capture
- * is on (lm_icp_set_capture records the host path only).  lm_icp_last_stats and lm_icp_launch_count cover the call. */
+ * read-back for a render whose box has 2^21 pixels or more (lm_set_template_renders' limit), and after the chunks for a
+ * cloud beyond 2^21 voxels.  With capture on (lm_icp_set_capture) the call also synchronises behind each chunk and
+ * copies its clouds out; the outputs do not change.  lm_icp_last_stats and lm_icp_launch_count cover the call. */
 int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, int64_t scene_pitch, int scene_format,
                                 float scene_scale, int srows, int scols, const void* const* model_depths,
                                 const int64_t* model_pitches, int model_format, float model_scale, int mrows, int mcols,
@@ -676,8 +701,11 @@ int lm_icp_set_verify(lm_icp* h, int on, double inlier_mm);
 int lm_icp_verify(lm_icp* h, float* score, int32_t* counts6, int64_t cap, int64_t* n);
 
 /* ---- introspection of the ICP kernels, used by the stage-by-stage tests ---- */
-/* While capture is on (default off), lm_icp_process_batch keeps, per hypothesis, what its kernels saw and kept in the
- * last call.  Turning it on or off drops what was kept.  The outputs do not depend on it. */
+/* While capture is on (default off), lm_icp_process_batch and lm_icp_process_batch_device keep, per hypothesis, what
+ * their kernels saw and kept in the last call; a call that fails past its argument checks keeps nothing.
+ * lm_icp_process_batch_device keeps COUNTS, SOURCE, TARGET, INIT and RESULT (the clouds the pose stage's kernels
+ * built); its NORMALS, KNN and CORR_* are LM_E_STATE.  Turning capture on or off drops what was kept.  The outputs do
+ * not depend on it. */
 int lm_icp_set_capture(lm_icp* h, int on);
 /* Copies item `what` of hypothesis `hyp` of the last call to `out` (cap bytes):
  *   COUNTS      2 int32: source and target points

@@ -19,6 +19,8 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from oracle import icp_oracle
+import pose_cloud_model
+from pose_cloud_model import seq_sum, voxel_down_sample_seq  # noqa: F401 (the model's, re-exported)
 
 KNN = 30
 MAX_D2 = icp_oracle.MAX_DIST ** 2
@@ -188,59 +190,15 @@ def all_cases():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# clouds as poseRefine builds them, with sequential sums (the host's order)
+# clouds as poseRefine builds them, with sequential sums (the host's order): tests/pose_cloud_model.py
 # ------------------------------------------------------------------------------------------------------------------
-def seq_sum(a):
-    """Sum along axis 0 one term after another (np.cumsum is sequential; np.sum is pairwise)."""
-    a = np.asarray(a, np.float64)
-    return np.cumsum(a, 0)[-1] if a.shape[0] else np.zeros(a.shape[1:])
-
-
-def voxel_down_sample_seq(pts, voxel=icp_oracle.VOXEL):
-    """icp_oracle.voxel_down_sample with every voxel summed sequentially in stable-sort order."""
-    if pts.shape[0] == 0:
-        return pts
-    origin = pts.min(0) - voxel * 0.5
-    idx = np.floor((pts - origin) / voxel).astype(np.int64)
-    order = np.lexsort((idx[:, 2], idx[:, 1], idx[:, 0]))  # stable
-    idx, p = idx[order], pts[order]
-    new = np.ones(len(idx), bool)
-    new[1:] = np.any(idx[1:] != idx[:-1], 1)
-    starts = np.nonzero(new)[0]
-    counts = np.diff(np.append(starts, len(idx)))
-    acc = np.zeros((len(starts), 3))
-    for k in range(int(counts.max())):
-        sel = counts > k
-        acc[sel] += p[starts[sel] + k]
-    return acc / counts[:, None]
-
-
 def host_clouds(c, use_scene):
     """(source, target, init 4x4, oracle init) of case c: the clouds and initial guess lm_icp_process_batch builds."""
-    bbox = icp_oracle.model_bbox(c.model)
-    mp, cm_np, cs_np, sp = icp_oracle.build_clouds(c.scene, c.model, c.K, c.K, c.xy[0], c.xy[1], bbox)
-    # the scene points of the centroid, in row-major order: the oracle's selection, restated
-    bx, by, bw, bh = bbox
-    rr, cc = np.mgrid[0:bh, 0:bw]
-    sr, sc = np.maximum(rr + c.xy[1] - 4, 0), np.maximum(cc + c.xy[0] - 4, 0)
-    md = c.model[rr + by, cc + bx]
-    sd = c.scene[sr, sc]
-    K = c.K
-    zs = sd.astype(np.float64) / 1000.0
-    xs = ((sc.astype(np.float32) - K[0, 2]) / K[0, 0]).astype(np.float64) * zs
-    ys = ((sr.astype(np.float32) - K[1, 2]) / K[1, 1]).astype(np.float64) * zs
-    anchor = float(c.model[H // 2, W // 2]) / 1000.0
-    sel = (sd > 0) & (md > 0) & (np.abs(zs - anchor) < 0.4)
-    with np.errstate(divide="ignore", invalid="ignore"):
-        cm = seq_sum(mp) / mp.shape[0]
-        cs = seq_sum(np.stack([xs[sel], ys[sel], zs[sel]], 1)) / int(sel.sum())
-    init = np.eye(4)
-    init[:3, 3] = cs - cm
+    m = pose_cloud_model.clouds(c.scene, c.model, c.K, c.K, c.xy[0], c.xy[1], use_scene)
+    _, cm_np, cs_np, _ = icp_oracle.build_clouds(c.scene, c.model, c.K, c.K, c.xy[0], c.xy[1], m["box"])
     init_np = np.eye(4)
     init_np[:3, 3] = cs_np - cm_np
-    src = voxel_down_sample_seq(mp)
-    tgt = voxel_down_sample_seq(sp) if use_scene else src
-    return src, tgt, init, init_np
+    return m["source"], m["target"], m["init"], init_np
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -310,15 +310,29 @@ def test_pose_refine_surface_takes_tensors(data, estimation, use_scene):
         native.set_use_scene_cloud(False)
 
 
-def test_refusals(data, icp):
+def test_capture_of_a_device_call(data, icp):
+    """Capture keeps a device call's clouds, initial guess and result, and refuses what that path does not keep."""
+    g = data["g"]
+    args = (data["sK"], data["K"][:1], data["R"][:1], data["t"][:1], [[300, 200]])
+    icp.set_capture(True)
+    try:
+        icp.process_batch_device(lib.DeviceDepths(cuda(g["depth"]), [cuda(g["render"])], 1.0, 1.0, None, 0), *args)
+        buf = np.zeros(1 << 20, np.uint8)
+        L = lib.load()
+        for what in ("normals", "knn", "corr_first", "corr_last"):
+            rc = L.lm_icp_capture(icp._h, 0, lib.CAPTURE_ITEMS[what], buf.ctypes.data, buf.nbytes)
+            assert rc == lib.LM_E_STATE and "device" in L.lm_last_error().decode(), what
+        for what in ("counts", "source", "target", "init", "result"):
+            assert L.lm_icp_capture(icp._h, 0, lib.CAPTURE_ITEMS[what], buf.ctypes.data, buf.nbytes) == lib.LM_OK, what
+    finally:
+        icp.set_capture(False)
+
+
+def test_argument_refusals(data, icp):
     g = data["g"]
     scene = cuda(g["depth"])
     r = cuda(g["render"])
     args = (data["sK"], data["K"][:1], data["R"][:1], data["t"][:1], [[300, 200]])
-    icp.set_capture(True)
-    with pytest.raises(RuntimeError, match="capture"):
-        icp.process_batch_device(lib.DeviceDepths(scene, [r], 1.0, 1.0, None, 0), *args)
-    icp.set_capture(False)
     wide = np.zeros((2100, 1100), np.uint16)
     wide[1:2099, 1:1099] = 1000                                # a 1100 x 2100 box: 2^21 pixels or more
     with pytest.raises(RuntimeError, match="too large"):
