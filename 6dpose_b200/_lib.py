@@ -18,7 +18,7 @@ LIB_PATH = os.environ.get("LINEMOD_B200_LIB") or os.path.join(_HERE, "csrc", "li
 LM_OK, LM_E_INVALID, LM_E_CUDA, LM_E_STATE, LM_E_CAPACITY = 0, -1, -2, -3, -4
 # capture items of lm_icp_capture and lm_debug_pose_clouds (include/linemod_b200.h)
 CAPTURE_ITEMS = dict(counts=0, source=1, target=2, normals=3, init=4, result=5, knn=6, corr_first=7, corr_last=8, slots=9, posed=10,
-                     raw_model=11, raw_scene=12)
+                     raw_model=11, raw_scene=12, search=13)
 SHARD_CONTIGUOUS, SHARD_INTERLEAVED = 0, 1
 
 MATCH_DTYPE = np.dtype([("x", "<i4"), ("y", "<i4"), ("similarity", "<f4"), ("class_index", "<i4"), ("template_id", "<i4")])
@@ -42,15 +42,17 @@ SYMBOLS = [
     "lm_icp_create", "lm_icp_destroy", "lm_icp_process", "lm_icp_process_batch", "lm_icp_last_stats", "lm_icp_launch_count", "lm_icp_set_use_scene_cloud",
     "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture", "lm_icp_process_batch_device",
     "lm_set_pose_verify", "lm_pose_verify", "lm_pose_verify_points", "lm_icp_set_verify", "lm_icp_verify",
+    "lm_set_pose_search", "lm_icp_set_pose_search", "lm_pose_search_points",
 ]
 
-# The ICP's estimation step (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT of include/linemod_b200.h) by the name the
-# Python surface takes
-ESTIMATIONS = {"point_to_plane": 0, "point_to_point": 1}
+# The pose stage's estimation (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT / LM_POSE_PSO of include/linemod_b200.h) by
+# the name the Python surface takes
+ESTIMATIONS = {"point_to_plane": 0, "point_to_point": 1, "pso": 3}
 
 
 def estimation_code(estimation):
-    """The C-ABI value of estimation="point_to_plane" | "point_to_point"; ValueError for anything else (no device work)."""
+    """The C-ABI value of estimation="point_to_plane" | "point_to_point" | "pso"; ValueError for anything else (no device
+    work)."""
     if not isinstance(estimation, str) or estimation not in ESTIMATIONS:
         raise ValueError("estimation must be one of %s, got %r" % (", ".join(repr(k) for k in ESTIMATIONS), estimation))
     return ESTIMATIONS[estimation]
@@ -91,6 +93,47 @@ def verify_options(inlier, rank_by="fitness", min_score=None):
             raise ValueError("rank_by=\"score\" and min_score need pose verification on (inlier_mm not None)")
         return 0, 10.0, 0, -math.inf
     return 1, inlier_mm(inlier), VERIFY_RANKS[rank_by], lo
+
+
+# The particle swarm of estimation="pso" (lm_set_pose_search): its settings by name, with their defaults and limits
+POSE_SEARCH_DEFAULTS = dict(particles=64, iterations=40, dt_mm=40.0, dr_deg=30.0, clamp_mm=20.0, seed=0)
+POSE_SEARCH_LIMITS = dict(particles=(1, 256), iterations=(0, 1000), dt_mm=(0.0, 10000.0), dr_deg=(0.0, 45.0), clamp_mm=(0.0, 1e6))
+
+
+def pose_search_options(particles=64, iterations=40, dt_mm=40.0, dr_deg=30.0, clamp_mm=20.0, seed=0):
+    """lm_set_pose_search's (particles, iterations, dt_mm, dr_deg, clamp_mm, seed) for Detector.setPoseSearch and the
+    pose_search keyword of poseRefine.process / refine_matches.  TypeError / ValueError before any device work."""
+    out = []
+    for name, v in (("particles", particles), ("iterations", iterations)):
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+            raise TypeError("%s must be an int, got %s" % (name, type(v).__name__))
+        lo, hi = POSE_SEARCH_LIMITS[name]
+        if not lo <= int(v) <= hi:
+            raise ValueError("%s must lie in [%d, %d], got %r" % (name, lo, hi, v))
+        out.append(int(v))
+    for name, v in (("dt_mm", dt_mm), ("dr_deg", dr_deg), ("clamp_mm", clamp_mm)):
+        x = _real(v, name)
+        lo, hi = POSE_SEARCH_LIMITS[name]
+        if not (math.isfinite(x) and lo <= x <= hi):
+            raise ValueError("%s must be finite and in [%g, %g], got %r" % (name, lo, hi, v))
+        out.append(x)
+    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)):
+        raise TypeError("seed must be an int, got %s" % type(seed).__name__)
+    if not 0 <= int(seed) < 1 << 64:
+        raise ValueError("seed must lie in [0, 2^64), got %r" % seed)
+    out.append(int(seed))
+    return tuple(out)
+
+
+def search_record(words, particles, iterations):
+    """A swarm record (LM_ICP_CAPTURE_SEARCH, lm_pose_search_points) as a dict: cost_start, cost and best (int), c [3]
+    f64, trace [I] int64 (the global-best cost after each iteration), x, v, p [P,6] f64 and cost_best [P] int64."""
+    w = np.ascontiguousarray(words, np.int64)
+    P, I = int(particles), int(iterations)
+    sw = w[6 + I:]
+    return dict(cost_start=int(w[0]), cost=int(w[1]), best=int(w[2]), c=w[3:6].view(np.float64).copy(), trace=w[6:6 + I].copy(),
+                x=sw[:6 * P].view(np.float64).reshape(P, 6).copy(), v=sw[6 * P:12 * P].view(np.float64).reshape(P, 6).copy(),
+                p=sw[12 * P:18 * P].view(np.float64).reshape(P, 6).copy(), cost_best=sw[18 * P:19 * P].copy())
 
 
 def verify_arrays(score, counts):
@@ -414,6 +457,10 @@ def load():
     L.lm_pose_verify_points.argtypes = [c_int, f64p, c_i64, f64p, u16p, c_int, c_int, f32p, ctypes.c_double, i32p, f32p]
     L.lm_icp_set_verify.argtypes = [vp, c_int, ctypes.c_double]
     L.lm_icp_verify.argtypes = [vp, f32p, i32p, c_i64, ctypes.POINTER(c_i64)]
+    search = [c_int, c_int, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_uint64]
+    L.lm_set_pose_search.argtypes = [vp] + search
+    L.lm_icp_set_pose_search.argtypes = [vp] + search
+    L.lm_pose_search_points.argtypes = [c_int, f64p, c_i64, f64p, u16p, c_int, c_int, f32p] + search + [c_i64, f64p, vp, c_i64]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
     L.lm_icp_destroy.restype = None
@@ -801,8 +848,13 @@ class NativeDetector:
                                               R.ctypes.data_as(f32p), t.ctypes.data_as(f32p)))
 
     def set_pose_estimation(self, estimation):
-        """"point_to_plane" (default) or "point_to_point" for the next pose stage (lm_set_pose_estimation)."""
+        """"point_to_plane" (default), "point_to_point" or "pso" for the next pose stage (lm_set_pose_estimation)."""
         check(self._L.lm_set_pose_estimation(self._h, estimation_code(estimation)))
+
+    def set_pose_search(self, particles=64, iterations=40, dt_mm=40.0, dr_deg=30.0, clamp_mm=20.0, seed=0):
+        """The particle swarm of estimation="pso" for the next pose stage (lm_set_pose_search)."""
+        check(self._L.lm_set_pose_search(self._h, int(particles), int(iterations), float(dt_mm), float(dr_deg), float(clamp_mm),
+                                         int(seed)))
 
     def enqueue_pose(self, sceneK, max_iterations=30, use_scene_cloud=False, estimation="point_to_plane"):
         est = estimation_code(estimation)
@@ -1105,7 +1157,9 @@ class NativeIcp:
         self._h = h
         self.device = int(device)
         self._estimation = "point_to_plane"  # the handle's estimation (lm_icp_set_estimation)
+        self._search = pose_search_options()  # its swarm settings (lm_icp_set_pose_search)
         self._captured = None               # the estimation of the last process_batch (capture())
+        self._captured_search = None        # and its swarm settings
         self._captured_device = False       # the last call was process_batch_device: clouds, init and result only
 
     def close(self):
@@ -1149,6 +1203,7 @@ class NativeIcp:
                                            int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
                                            res.ctypes.data_as(f32p)))
         self._captured = self._estimation
+        self._captured_search = self._search
         self._captured_device = False
         return Ro, to, res
 
@@ -1184,9 +1239,15 @@ class NativeIcp:
         check(self._L.lm_icp_set_use_scene_cloud(self._h, 1 if on else 0))
 
     def set_estimation(self, estimation):
-        """"point_to_plane" (the reference's active branch, default) or "point_to_point" (lm_icp_set_estimation)."""
+        """"point_to_plane" (the reference's active branch, default), "point_to_point" or "pso" (lm_icp_set_estimation)."""
         check(self._L.lm_icp_set_estimation(self._h, estimation_code(estimation)))
         self._estimation = estimation
+
+    def set_pose_search(self, particles=64, iterations=40, dt_mm=40.0, dr_deg=30.0, clamp_mm=20.0, seed=0):
+        """The particle swarm of estimation="pso" for the next calls (lm_icp_set_pose_search)."""
+        opts = (int(particles), int(iterations), float(dt_mm), float(dr_deg), float(clamp_mm), int(seed))
+        check(self._L.lm_icp_set_pose_search(self._h, *opts))
+        self._search = opts
 
     def set_verify(self, inlier_mm):
         """Pose verification for the next calls (lm_icp_set_verify): the inlier distance in mm, or None for off."""
@@ -1209,10 +1270,20 @@ class NativeIcp:
         lm_icp_capture): source / target [n,3] f64, normals [nt,3] f64, init [4,4] f64, T [4,4] f64, fitness, rmse,
         iterations, knn [nt,30] int32 (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence).  After a
         point-to-point call normals and knn are None: that estimation computes neither.  After process_batch_device
-        normals, knn, corr_first and corr_last are None: that path keeps the clouds, init and result only."""
+        normals, knn, corr_first and corr_last are None: that path keeps the clouds, init and result only.  After a "pso"
+        call of process_batch normals, knn and the correspondences are None and `search` is the swarm record
+        (search_record)."""
         n, nt = self._capture_item(hyp, 0, np.zeros(2, np.int32)).tolist()
         res = self._capture_item(hyp, 5, np.zeros(19, np.float64))
-        p2pl = self._captured != "point_to_point"
+        p2pl = self._captured == "point_to_plane"
+        if self._captured == "pso" and not self._captured_device:
+            P, I = self._captured_search[:2]
+            words = self._capture_item(hyp, 13, np.zeros(6 + I + 19 * P, np.int64))
+            return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
+                        target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)), normals=None,
+                        init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
+                        T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
+                        knn=None, corr_first=None, corr_last=None, search=search_record(words, P, I))
         if self._captured_device:
             return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
                         target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)), normals=None,
@@ -1265,6 +1336,29 @@ def _verify_results(fn, h):
     if n.value:
         check(fn(h, score.ctypes.data_as(f32p), counts.ctypes.data_as(i32p), n.value, ctypes.byref(n)))
     return score, counts
+
+
+def pose_search_points(pts, start_t, scene, sceneK, job=0, device=0, **search):
+    """k_pose_pso on caller arrays (lm_pose_search_points): pts [n,3] f64 (m), start_t [3] f64 (the start pose's
+    translation, m), scene HxW u16 mm, sceneK 3x3 f32, job the job number of the draws, search as pose_search_options.
+    Returns (T [4,4] f64, the swarm record as search_record gives it)."""
+    L = load()
+    opts = pose_search_options(**search)
+    pts = np.ascontiguousarray(pts, np.float64).reshape(-1, 3)
+    st = np.ascontiguousarray(start_t, np.float64).reshape(3)
+    scene = np.ascontiguousarray(scene)
+    if scene.dtype != np.uint16 or scene.ndim != 2:
+        raise TypeError("scene must be a uint16 HxW depth image (mm)")
+    sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+    P, I = opts[:2]
+    words = np.zeros(6 + I + 19 * P, np.int64)
+    T = np.zeros(16, np.float64)
+    f64p = ctypes.POINTER(ctypes.c_double)
+    check(L.lm_pose_search_points(int(device), pts.ctypes.data_as(f64p), pts.shape[0], st.ctypes.data_as(f64p),
+                                  scene.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), scene.shape[0], scene.shape[1],
+                                  sK.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), *opts, int(job), T.ctypes.data_as(f64p),
+                                  words.ctypes.data_as(ctypes.c_void_p), words.nbytes))
+    return T.reshape(4, 4), search_record(words, P, I)
 
 
 def pose_verify_points(pts, T, scene, sceneK, inlier_mm=10.0, device=0):

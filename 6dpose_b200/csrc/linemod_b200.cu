@@ -146,6 +146,7 @@ struct FrameChain {
   bool pose = false; float sK[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   int max_iter = 30, use_scene = 0, estimation = LM_ICP_POINT_TO_PLANE;  // lm_enqueue_pose
   PoseVerifyOptions verify = {0, LM_VERIFY_RANK_FITNESS, 10.0, -INFINITY};
+  PoseSearch search = pose_search_default();                // LM_POSE_PSO's settings
   bool pose_nms = false; double nms_thr = 40.0;             // lm_enqueue_pose_nms
 };
 
@@ -249,6 +250,7 @@ struct lm_detector {
   bool frame_depth = false;             // the frame came from lm_upload_images: fe_depth holds its depth
   int pose_estimation = LM_ICP_POINT_TO_PLANE;  // lm_set_pose_estimation: for the next pose stage
   PoseVerifyOptions pose_verify = {0, LM_VERIFY_RANK_FITNESS, 10.0, -INFINITY};  // lm_set_pose_verify: likewise
+  PoseSearch pose_search = pose_search_default();  // lm_set_pose_search: likewise
   int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
@@ -2303,7 +2305,7 @@ static int enqueue_pose(lm_detector* d) {
   }
   const FrameChain& c = d->chain;
   PoseRun run;
-  run.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr, c.verify};
+  run.o = {d->fe[0].rows, d->fe[0].cols, c.use_scene, c.max_iter, c.estimation, d->stream.get(), share ? &sh : nullptr, c.verify, c.search};
   run.n_frames = 1; run.first = nullptr; run.d_counts = d->d_post_counts.get();
   run.bound = c.top_k > 0 ? std::min(c.top_k, LM_POST_MAX) : LM_POST_MAX;
   run.d_surv = d->d_post_out.get(); run.d_scene = d->fe_depth.get(); run.sK = c.sK;
@@ -2315,6 +2317,8 @@ extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iter
   if (d && d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (!d || !sceneK) return fail(LM_E_INVALID, "null argument");
   if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
+  if (d->pose_estimation == LM_POSE_PSO && d->px_rank >= 0 && d->px_share_pose)
+    return fail(LM_E_STATE, "the pose stage shared over the ranks does not run LM_POSE_PSO: turn lm_peer_share_pose off");
   FrameChain& c = d->chain;
   if (!c.post) return fail(LM_E_STATE, "lm_enqueue_post has not been called");
   if (!d->frame_depth) return fail(LM_E_STATE, "the frame has no depth image: upload it with lm_upload_images");
@@ -2326,6 +2330,7 @@ extern "C" int lm_enqueue_pose(lm_detector* d, const float* sceneK, int max_iter
   c.use_scene = use_scene_cloud ? 1 : 0;
   c.estimation = d->pose_estimation;
   c.verify = d->pose_verify;
+  c.search = d->pose_search;
   c.pose_nms = false;  // a new pose stage: any pose NMS enqueued before belongs to an abandoned frame
   int rc = enqueue_pose(d);
   if (rc) return rc;
@@ -2388,10 +2393,16 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
 
 extern "C" int lm_set_pose_estimation(lm_detector* d, int estimation) {
   if (!d) return fail(LM_E_INVALID, "null detector");
-  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT)
-    return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
+  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT && estimation != LM_POSE_PSO)
+    return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1, LM_POSE_PSO 3)", estimation);
   d->pose_estimation = estimation;
   return LM_OK;
+}
+
+extern "C" int lm_set_pose_search(lm_detector* d, int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm,
+                                  uint64_t seed) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  return pose_search_make(particles, iterations, dt_mm, dr_deg, clamp_mm, seed, &d->pose_search);
 }
 
 extern "C" int lm_set_pose_verify(lm_detector* d, int on, double inlier_mm, int rank_by, double min_score) {
@@ -2504,6 +2515,8 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
   if (!peers && d->px_rank >= 0)
     return fail(LM_E_STATE, "lm_detect_batch does not run with a connected peer exchange (every rank calls lm_peer_detect_batch)");
   if (peers && d->px_rank < 0) return fail(LM_E_STATE, "lm_peer_detect_batch needs a connected peer exchange");
+  if (peers && d->px_share_pose && d->pose_estimation == LM_POSE_PSO)
+    return fail(LM_E_STATE, "the pose stage shared over the ranks does not run LM_POSE_PSO: turn lm_peer_share_pose off");
   if (!d->pose || !pose_stage_covers(d->pose, d->sel.data(), (int64_t)d->sel.size()))
     return fail(LM_E_STATE, "no template renders registered for every selected template of this bank (lm_set_template_renders)");
   CU(cudaSetDevice(d->device));
@@ -2549,7 +2562,8 @@ static int detect_batch(lm_detector* d, bool peers, int n_frames, const uint8_t*
     d->px_pose_seq += pose_batch_chunks(first[n_frames]);
   }
   PoseRun run;
-  run.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr, d->pose_verify};
+  run.o = {rows, cols, use_scene_cloud ? 1 : 0, max_iterations, d->pose_estimation, st, share ? &sh : nullptr, d->pose_verify,
+           d->pose_search};
   run.n_frames = n_frames; run.first = first.data(); run.d_counts = nullptr; run.bound = bound;
   run.d_surv = d_surv; run.d_scene = d_scene; run.sK = sceneK;
   run.pose_nms = pose_nms ? 1 : 0;

@@ -41,6 +41,7 @@
 #include <algorithm>
 #include <limits>
 #include <memory>
+#include <mutex>
 #include <thread>
 #include <vector>
 
@@ -75,6 +76,54 @@ struct PoseVerify {  // one survivor / hypothesis (lm_set_pose_verify)
   float score;        // -1: no pose
   int32_t pad;
 };
+
+// LM_POSE_PSO's limits, settings and kernel parameters (the kernel: k_pose_pso, behind pose verification below)
+#define PSO_THREADS 256
+#define PSO_CHUNK 2048       // source points held in shared memory at once; larger clouds are swept in chunks
+#define PSO_MAX_PARTICLES 256
+#define PSO_MAX_ITERATIONS 1000
+#define PSO_MAX_JOB (1ll << 40)
+#define PSO_PARTICLE_BYTES (30 * 8 + 2 * 8)  // T [12], x, v, p [6] each (f64); cost, best cost (int64)
+
+PoseSearch pose_search_default() { return PoseSearch{64, 40, 0.040, 30.0 * 0.017453292519943295, 20.0, 0ull}; }
+
+int pose_search_make(int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm, uint64_t seed, PoseSearch* out) {
+  if (particles < 1 || particles > PSO_MAX_PARTICLES)
+    return lm_fail(LM_E_INVALID, "pose search: %d particles, must lie in [1, %d]", particles, PSO_MAX_PARTICLES);
+  if (iterations < 0 || iterations > PSO_MAX_ITERATIONS)
+    return lm_fail(LM_E_INVALID, "pose search: %d iterations, must lie in [0, %d]", iterations, PSO_MAX_ITERATIONS);
+  if (!(std::isfinite(dt_mm) && dt_mm >= 0.0 && dt_mm <= 10000.0))
+    return lm_fail(LM_E_INVALID, "pose search: translation bound %g mm, must be finite and in [0, 10000]", dt_mm);
+  if (!(std::isfinite(dr_deg) && dr_deg >= 0.0 && dr_deg <= 45.0))
+    return lm_fail(LM_E_INVALID, "pose search: rotation bound %g degrees, must be finite and in [0, 45]", dr_deg);
+  if (!(std::isfinite(clamp_mm) && clamp_mm >= 0.0 && clamp_mm <= 1e6))
+    return lm_fail(LM_E_INVALID, "pose search: cost clamp %g mm, must be finite and in [0, 1e6]", clamp_mm);
+  *out = PoseSearch{particles, iterations, dt_mm / 1000.0, dr_deg * 0.017453292519943295, clamp_mm, (unsigned long long)seed};
+  return LM_OK;
+}
+
+// Words of 8 bytes of one swarm record (LM_ICP_CAPTURE_SEARCH).
+static int64_t pso_record_words(const PoseSearch& s) { return 6 + s.iterations + 19 * (int64_t)s.particles; }
+
+struct PsoParams {
+  const IcpJob* jobs;         // [n] the slots' source clouds (in pts) and start poses
+  const double* pts;
+  IcpOut* outs;
+  int32_t n;
+  const uint16_t* scene;      // as PoseParams: frame f's depth at scene + f * srows * scols
+  int32_t srows, scols;
+  float sK[9];
+  const int32_t* frame_of;    // null: one frame, intrinsics sK; else per slot its frame, intrinsics sKs + 9 * frame
+  const float* sKs;
+  const int32_t* frame_first; // batch: frame f's first survivor in the run (job = first + slot - frame_first[frame])
+  int64_t first;              // run index of slot 0's survivor
+  const int64_t* job;         // per slot its job number (lm_icp_process_batch, lm_pose_search_points); null: as above
+  PoseSearch s;
+  long long* record;          // null, or the slots' swarm records, record_words apart
+  int64_t record_words;
+};
+
+static int launch_pso(const PsoParams& p, cudaStream_t st);
 
 // --------------------------------------------------------------------------------------------
 // normals: covariance of the 30 nearest neighbours, eigenvector of the smallest eigenvalue
@@ -686,6 +735,9 @@ struct lm_icp {
   int64_t launches = 0;
   bool use_scene_cloud = false;  // non-reference option: register against the scene cloud
   int estimation = LM_ICP_POINT_TO_PLANE;
+  PoseSearch search = pose_search_default();  // lm_icp_set_pose_search (LM_POSE_PSO)
+  DeviceArray<uint8_t> d_sbuf;  // LM_POSE_PSO on the host path: the scene, the jobs' hypothesis numbers, their swarm records
+  PinnedArray<uint8_t> h_sbuf;  // and the host staging of the first two (a call ends in a synchronise: it is free again)
   int last_points = 0, last_iterations = 0;
   double last_rmse = 0;
   float last_kernel_us = 0;
@@ -700,6 +752,8 @@ struct lm_icp {
     std::vector<IcpOut> outs;
     std::vector<double> pts, nrm;
     std::vector<int32_t> knn, corr;
+    std::vector<long long> record;  // LM_POSE_PSO (host path): the jobs' swarm records, record_words apart
+    int64_t record_words = 0;
   } cap;
   IcpDevice* dev = nullptr;  // created by the first lm_icp_process_batch_device
   // lm_icp_set_verify, and the verification of the last call's hypotheses (verified false: that call did not verify)
@@ -916,6 +970,8 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
   CUI(cudaSetDevice(h->device));
   h->verified = false;
   h->cap.job_of.clear();  // a call that fails keeps no capture
+  const bool pso = h->estimation == LM_POSE_PSO;
+  const bool scene_cloud = h->use_scene_cloud && !pso;  // the swarm registers against no target
   std::vector<Cloud> clouds((size_t)n_hyp);
   std::vector<IcpJob> jobs;
   std::vector<int> job_of((size_t)n_hyp, -1);
@@ -928,7 +984,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     // NMS survivors of the drivers, linemod_and_levelup_test.py:348-367)
     auto build = [&](int i) {
       build_cloud(scene_depth, srows, scols, model_depths[i], mrows, mcols, sceneK, modelK + 9 * i, R + 9 * i, t + 3 * i,
-                  detect_xy[2 * i], detect_xy[2 * i + 1], h->use_scene_cloud, h->verify, clouds[i]);
+                  detect_xy[2 * i], detect_xy[2 * i + 1], scene_cloud, h->verify, clouds[i]);
     };
     std::vector<std::thread> workers;
     for (int i = 1; i < n_hyp && i < 16; ++i) workers.emplace_back(build, i);
@@ -947,7 +1003,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     all.insert(all.end(), clouds[i].pts.begin(), clouds[i].pts.end());
     j.tgt_first = j.src_first;  // scene_pcd_down = model_pcd->VoxelDownSample (LL.cpp:109)
     j.tgt_count = j.src_count;
-    if (h->use_scene_cloud) {
+    if (scene_cloud) {
       j.tgt_first = (int32_t)(all.size() / 3);
       j.tgt_count = (int32_t)(clouds[i].scene.size() / 3);
       all.insert(all.end(), clouds[i].scene.begin(), clouds[i].scene.end());
@@ -958,6 +1014,7 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     max_count = std::max(max_count, j.tgt_count);
   }
   const size_t npts = all.size() / 3;
+  const int64_t words = pso_record_words(h->search);
   if (!jobs.empty()) {
     // a pair grows together, its second array allocated last: that one's size is the pair's
     if (npts * 3 > h->d_nrm.size()) {
@@ -983,16 +1040,46 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
     cudaStream_t st = h->stream.get();
     if (npts) CUI(cudaMemcpyAsync(h->d_pts.get(), all.data(), npts * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
     CUI(cudaMemcpyAsync(h->d_jobs.get(), jobs.data(), jobs.size() * sizeof(IcpJob), cudaMemcpyHostToDevice, st));
-    CUI(cudaEventRecord(h->ev0.get(), st));
-    if (max_count > 0 && h->estimation == LM_ICP_POINT_TO_PLANE) {
-      dim3 g((unsigned)((max_count + 127) / 128), (unsigned)jobs.size());
-      k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), knn_out);
-      ++h->launches;
+    PsoParams q;
+    if (pso) {  // one buffer: the scene, per job its hypothesis (the job number of its draws), then (capture) the records
+      const size_t npix = (size_t)srows * scols, o_hyp = (sizeof(uint16_t) * npix + 15) & ~(size_t)15;
+      const size_t o_rec = o_hyp + sizeof(int64_t) * jobs.size();
+      CUI(h->h_sbuf.reserve(o_rec));
+      uint8_t* hb = h->h_sbuf.get();
+      memcpy(hb, scene_depth, sizeof(uint16_t) * npix);
+      int64_t* hyp = reinterpret_cast<int64_t*>(hb + o_hyp);
+      for (int i = 0; i < n_hyp; ++i)
+        if (job_of[i] >= 0) hyp[(size_t)job_of[i]] = i;
+      CUI(h->d_sbuf.reserve(o_rec + (h->capture ? sizeof(long long) * words * jobs.size() : 0)));
+      uint8_t* b = h->d_sbuf.get();
+      CUI(cudaMemcpyAsync(b, hb, o_rec, cudaMemcpyHostToDevice, st));
+      memset(&q, 0, sizeof(q));
+      q.jobs = h->d_jobs.get(); q.pts = h->d_pts.get(); q.outs = h->d_outs.get(); q.n = (int32_t)jobs.size();
+      q.scene = reinterpret_cast<const uint16_t*>(b); q.srows = srows; q.scols = scols;
+      memcpy(q.sK, sceneK, sizeof(q.sK));
+      q.job = reinterpret_cast<const int64_t*>(b + o_hyp);
+      q.s = h->search;
+      q.record = h->capture ? reinterpret_cast<long long*>(b + o_rec) : nullptr; q.record_words = words;
     }
-    launch_icp<false>(h->estimation, (unsigned)jobs.size(), st, h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), h->d_outs.get(),
-                      max_iterations, corr_out, PoseShareDev());
+    CUI(cudaEventRecord(h->ev0.get(), st));
+    if (pso) {
+      int rc = launch_pso(q, st);
+      if (rc) return rc;
+    } else {
+      if (max_count > 0 && h->estimation == LM_ICP_POINT_TO_PLANE) {
+        dim3 g((unsigned)((max_count + 127) / 128), (unsigned)jobs.size());
+        k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), knn_out);
+        ++h->launches;
+      }
+      launch_icp<false>(h->estimation, (unsigned)jobs.size(), st, h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), h->d_outs.get(),
+                        max_iterations, corr_out, PoseShareDev());
+    }
     ++h->launches;
     CUI(cudaEventRecord(h->ev1.get(), st));
+    if (pso && h->capture) {
+      h->cap.record.resize((size_t)words * jobs.size());
+      CUI(cudaMemcpyAsync(h->cap.record.data(), q.record, sizeof(long long) * h->cap.record.size(), cudaMemcpyDeviceToHost, st));
+    }
     CUI(cudaMemcpyAsync(h->h_outs.get(), h->d_outs.get(), jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
     CUI(cudaGetLastError());
@@ -1023,8 +1110,10 @@ extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_
         CUI(cudaMemcpy(c.nrm.data(), h->d_nrm.get(), npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
         CUI(cudaMemcpy(c.knn.data(), h->d_knn.get(), npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
       }
-      CUI(cudaMemcpy(c.corr.data(), h->d_corr.get(), npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
+      if (!pso) CUI(cudaMemcpy(c.corr.data(), h->d_corr.get(), npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
     }
+    if (!pso || jobs.empty()) c.record.clear();
+    c.record_words = words;
   }
   for (int i = 0; i < n_hyp; ++i) {
     if (job_of[i] < 0) { residual[i] = -1.f; continue; }
@@ -1066,10 +1155,15 @@ extern "C" int lm_icp_set_use_scene_cloud(lm_icp* h, int on) {
 
 extern "C" int lm_icp_set_estimation(lm_icp* h, int estimation) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
-  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT)
-    return lm_fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1)", estimation);
+  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT && estimation != LM_POSE_PSO)
+    return lm_fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1, LM_POSE_PSO 3)", estimation);
   h->estimation = estimation;
   return LM_OK;
+}
+
+extern "C" int lm_icp_set_pose_search(lm_icp* h, int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm, uint64_t seed) {
+  if (!h) return lm_fail(LM_E_INVALID, "null handle");
+  return pose_search_make(particles, iterations, dt_mm, dr_deg, clamp_mm, seed, &h->search);
 }
 
 extern "C" int lm_icp_set_verify(lm_icp* h, int on, double inlier_mm) {
@@ -1108,8 +1202,13 @@ extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t c
   int64_t bytes = 0;
   std::vector<int32_t> tmp;
   double res[19];
+  if (c.estimation == LM_POSE_PSO && (what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN || what == LM_ICP_CAPTURE_CORR_FIRST ||
+                                       what == LM_ICP_CAPTURE_CORR_LAST))
+    return lm_fail(LM_E_STATE, "capture item %d: the particle swarm computes no normals, neighbour lists or correspondences", what);
   if ((what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN) && c.estimation != LM_ICP_POINT_TO_PLANE)
     return lm_fail(LM_E_STATE, "capture item %d: the point-to-point estimation computes no normals or neighbour lists", what);
+  if (what == LM_ICP_CAPTURE_SEARCH && (c.estimation != LM_POSE_PSO || c.device))
+    return lm_fail(LM_E_STATE, "capture item %d: only an LM_POSE_PSO call of lm_icp_process_batch keeps swarm records", what);
   if (c.device && (what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN || what == LM_ICP_CAPTURE_CORR_FIRST ||
                    what == LM_ICP_CAPTURE_CORR_LAST))
     return lm_fail(LM_E_STATE, "capture item %d: lm_icp_process_batch_device keeps no normals, neighbour lists or correspondences", what);
@@ -1134,6 +1233,9 @@ extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t c
       memcpy(res, o.T, sizeof(o.T));
       res[16] = o.fitness; res[17] = o.rmse; res[18] = o.iterations;
       src = res; bytes = sizeof(res);
+      break;
+    case LM_ICP_CAPTURE_SEARCH:
+      src = c.record.data() + (size_t)c.job_of[hyp] * c.record_words; bytes = c.record_words * (int64_t)sizeof(long long);
       break;
     case LM_ICP_CAPTURE_KNN:
       src = c.knn.data() + (size_t)j.tgt_first * ICP_KNN; bytes = (int64_t)j.tgt_count * ICP_KNN * sizeof(int32_t);
@@ -1422,7 +1524,10 @@ struct VerifyScene {
 };
 
 // Steps 3-4 for one point p of the model cloud, T's first three rows in T[0..11]; every operation correctly rounded.
-__device__ __forceinline__ int verify_point(const double* T, double px, double py, double pz, const VerifyScene& sc, double delta) {
+// *d receives z_s - z_q (mm) when the point is compared (inlier, occluded or violation).  k_pose_pso's cost uses the
+// same routine with delta = +inf, where every compared point is an inlier.
+__device__ __forceinline__ int verify_point(const double* T, double px, double py, double pz, const VerifyScene& sc, double delta,
+                                            double* dz) {
   double q[3];
 #pragma unroll
   for (int r = 0; r < 3; ++r)
@@ -1436,6 +1541,7 @@ __device__ __forceinline__ int verify_point(const double* T, double px, double p
   const uint16_t zs = sc.depth[(size_t)r * sc.cols + (size_t)c];
   if (zs == 0) return VERIFY_MISSING;
   const double d = __dsub_rn((double)zs, __dmul_rn(q[2], 1000.0));
+  *dz = d;
   if (fabs(d) <= delta) return VERIFY_INLIER;
   return d < 0.0 ? VERIFY_OCCLUDED : VERIFY_VIOLATION;
 }
@@ -1447,7 +1553,8 @@ __device__ PoseVerify verify_block(const double* __restrict__ P, int n, const do
   __syncthreads();
   int cnt[VERIFY_CLASSES] = {0, 0, 0, 0, 0};
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
-    const int k = verify_point(T, P[3 * j], P[3 * j + 1], P[3 * j + 2], sc, delta);
+    double d;
+    const int k = verify_point(T, P[3 * j], P[3 * j + 1], P[3 * j + 2], sc, delta, &d);
 #pragma unroll
     for (int q = 0; q < VERIFY_CLASSES; ++q) cnt[q] += k == q;
   }
@@ -1551,6 +1658,311 @@ static int icp_verify_host(lm_icp* h, const std::vector<int>& job_of, const std:
       if (job_of[i] >= 0) h->ver[i] = out[(size_t)job_of[i]];
   }
   h->verified = true;
+  return LM_OK;
+}
+
+// --------------------------------------------------------------------------------------------
+// LM_POSE_PSO (include/linemod_b200.h): a particle swarm over rotations about the cloud's centroid and translations,
+// scored against the scene depth with pose verification's projection
+// --------------------------------------------------------------------------------------------
+__device__ __forceinline__ double pso_draw(unsigned long long seed, long long job, int k, int i, int q) {
+  const unsigned long long number = (((unsigned long long)job * 1024ull + (unsigned long long)k) * 1024ull + (unsigned long long)i) * 16ull +
+                                    (unsigned long long)q;
+  unsigned long long z = seed + (number + 1ull) * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z ^= z >> 31;
+  return __dmul_rn((double)(z >> 11), 0x1.0p-53);
+}
+
+// T(x) = Trans(c + t) Rot(w) Trans(-c) S as [R | u] into T[0..11] (include/linemod_b200.h).
+__device__ __forceinline__ void pso_pose(const double* x, const double* c, const double* s, double* T) {
+  const double w0 = x[0], w1 = x[1], w2 = x[2];
+  const double y = __dadd_rn(__dadd_rn(__dmul_rn(w0, w0), __dmul_rn(w1, w1)), __dmul_rn(w2, w2));
+  double R[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+  if (y != 0.0) {
+    const double SA[11] = {0x1.0000000000000p+0, -0x1.5555555555555p-3, 0x1.1111111111111p-7, -0x1.a01a01a01a01ap-13,
+                           0x1.71de3a556c734p-19, -0x1.ae64567f544e4p-26, 0x1.6124613a86d09p-33, -0x1.ae7f3e733b81fp-41,
+                           0x1.952c77030ad4ap-49, -0x1.2f49b46814157p-57, 0x1.71b8ef6dcf572p-66};
+    const double SB[11] = {0x1.0000000000000p-1, -0x1.5555555555555p-5, 0x1.6c16c16c16c17p-10, -0x1.a01a01a01a01ap-16,
+                           0x1.27e4fb7789f5cp-22, -0x1.1eed8eff8d898p-29, 0x1.93974a8c07c9dp-37, -0x1.ae7f3e733b81fp-45,
+                           0x1.6827863b97d97p-53, -0x1.e542ba4020225p-62, 0x1.0ce396db7f853p-70};
+    double A = SA[10], B = SB[10];
+#pragma unroll
+    for (int k = 9; k >= 0; --k) { A = __dadd_rn(SA[k], __dmul_rn(y, A)); B = __dadd_rn(SB[k], __dmul_rn(y, B)); }
+    const double w[3] = {w0, w1, w2};
+    const double K[9] = {0.0, -w2, w1, w2, 0.0, -w0, -w1, w0, 0.0};
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int q = 0; q < 3; ++q) {
+        const double k2 = r == q ? __dsub_rn(__dmul_rn(w[r], w[r]), y) : __dmul_rn(w[r], w[q]);
+        R[3 * r + q] = __dadd_rn(__dadd_rn(r == q ? 1.0 : 0.0, __dmul_rn(A, K[3 * r + q])), __dmul_rn(B, k2));
+      }
+  }
+  const double a[3] = {__dsub_rn(s[0], c[0]), __dsub_rn(s[1], c[1]), __dsub_rn(s[2], c[2])};
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const double m = __dadd_rn(__dadd_rn(__dmul_rn(R[3 * r], a[0]), __dmul_rn(R[3 * r + 1], a[1])), __dmul_rn(R[3 * r + 2], a[2]));
+    T[4 * r] = R[3 * r]; T[4 * r + 1] = R[3 * r + 1]; T[4 * r + 2] = R[3 * r + 2];
+    T[4 * r + 3] = __dadd_rn(__dadd_rn(s[r], __dsub_rn(m, a[r])), x[3 + r]);
+  }
+}
+
+__device__ __forceinline__ long long warp_sum_ll(long long v) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+  return v;
+}
+
+// One CTA per slot, persistent over the slots (grid <= n).  Dynamic shared memory: the chunk of points [PSO_CHUNK][3],
+// then per particle its pose, position, velocity and personal best, then its cost and best cost.  Warp w scores
+// particles w, w + 8, ...: its lanes sweep the chunk's points and a warp reduction gives the particle's sum, which only
+// that warp adds to.  The scene is read through L1 / L2.
+__global__ void __launch_bounds__(PSO_THREADS) k_pose_pso(PsoParams p) {
+  extern __shared__ __align__(16) double pso_smem[];
+  __shared__ double s_c[3], s_g[6];
+  __shared__ long long s_fs, s_fg;
+  __shared__ int s_gi;
+  const int P = p.s.particles, I = p.s.iterations, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  double* s_pts = pso_smem;                      // [PSO_CHUNK][3]
+  double* s_T = s_pts + 3 * PSO_CHUNK;           // [P][12]
+  double* s_x = s_T + 12 * P;                    // [P][6]
+  double* s_v = s_x + 6 * P;
+  double* s_p = s_v + 6 * P;
+  long long* s_f = reinterpret_cast<long long*>(s_p + 6 * P);  // [P]
+  long long* s_fp = s_f + P;                                   // [P]
+  const int clamp_um = (int)floor(__dmul_rn(p.s.clamp_mm, 1000.0));
+  for (int slot = blockIdx.x; slot < p.n; slot += gridDim.x) {
+    const IcpJob job = p.jobs[slot];
+    const int n = job.src_count;
+    const double* __restrict__ P3 = p.pts + (size_t)job.src_first * 3;
+    const double S[3] = {job.init[3], job.init[7], job.init[11]};
+    if (n == 0) {  // no cloud (a slot without a pose): S, no search
+      if (tid == 0) {
+        IcpOut o;
+        for (int k = 0; k < 16; ++k) o.T[k] = job.init[k];
+        o.fitness = 0.0; o.rmse = 0.0; o.iterations = I; o.pad = 0;
+        p.outs[slot] = o;
+      }
+      continue;  // block-uniform
+    }
+    const int frame = p.frame_of ? p.frame_of[slot] : 0;
+    const long long J = p.job ? p.job[slot] : p.first + slot - (p.frame_first ? p.frame_first[frame] : 0);
+    const float* fK = p.frame_of ? p.sKs + 9 * frame : p.sK;
+    VerifyScene sc;
+    sc.depth = p.scene + (size_t)frame * p.srows * p.scols;
+    sc.rows = p.srows; sc.cols = p.scols;
+    sc.fx = fK[0]; sc.cx = fK[2]; sc.fy = fK[4]; sc.cy = fK[5];
+    __syncthreads();  // the previous slot's last reads of the shared arrays
+    if (tid < 3) {  // the centroid under S, in index order
+      double a = 0.0;
+      const double st = tid == 0 ? S[0] : (tid == 1 ? S[1] : S[2]);
+      for (int j = 0; j < n; ++j) a = __dadd_rn(a, __dadd_rn(P3[3 * j + tid], st));
+      s_c[tid] = __ddiv_rn(a, (double)n);
+    }
+    const int nchunks = (n + PSO_CHUNK - 1) / PSO_CHUNK;
+    auto load_chunk = [&](int c0) {
+      const int m = min(PSO_CHUNK, n - c0);
+      for (int k = tid; k < 3 * m; k += PSO_THREADS) s_pts[k] = P3[(size_t)3 * c0 + k];
+    };
+    if (nchunks == 1) load_chunk(0);
+    const int np = I > 0 ? P : 1;  // I = 0: the start alone
+    const int rounds = I > 0 ? I : 1;
+    for (int k = 0; k < rounds; ++k) {
+      // positions: the start (iteration 0), or the move
+      for (int e = tid; e < 6 * np; e += PSO_THREADS) {
+        const int i = e / 6, q = e - 6 * i;
+        const double D = q < 3 ? p.s.dr : p.s.dt;
+        double& x = s_x[e];
+        double& v = s_v[e];
+        if (k == 0) {
+          v = 0.0;
+          x = i == 0 ? 0.0 : __dsub_rn(__dmul_rn(__dmul_rn(2.0, D), pso_draw(p.s.seed, J, 0, i, q)), D);
+          s_p[e] = x;
+        } else {
+          const double r1 = pso_draw(p.s.seed, J, k, i, q), r2 = pso_draw(p.s.seed, J, k, i, 6 + q);
+          const double g = s_gi < 0 ? 0.0 : s_g[q];
+          double nv = __dadd_rn(__dadd_rn(__dmul_rn(0.7298, v), __dmul_rn(__dmul_rn(1.49618, r1), __dsub_rn(s_p[e], x))),
+                                __dmul_rn(__dmul_rn(1.49618, r2), __dsub_rn(g, x)));
+          if (nv > D) nv = D;
+          else if (nv < -D) nv = -D;
+          double nx = __dadd_rn(x, nv);
+          if (nx > D) { nx = D; nv = 0.0; }
+          else if (nx < -D) { nx = -D; nv = 0.0; }
+          x = nx;
+          v = nv;
+        }
+      }
+      __syncthreads();
+      for (int i = tid; i < np; i += PSO_THREADS) {
+        pso_pose(s_x + 6 * i, s_c, S, s_T + 12 * i);
+        s_f[i] = 0;
+        if (k == 0) s_fp[i] = 0x7FFFFFFFFFFFFFFFll;
+      }
+      __syncthreads();
+      // the costs
+      for (int ch = 0; ch < nchunks; ++ch) {
+        const int c0 = ch * PSO_CHUNK, m = min(PSO_CHUNK, n - c0);
+        if (nchunks > 1) {
+          __syncthreads();
+          load_chunk(c0);
+          __syncthreads();
+        }
+        for (int i = warp; i < np; i += PSO_THREADS / 32) {
+          double T[12];
+#pragma unroll
+          for (int q = 0; q < 12; ++q) T[q] = s_T[12 * i + q];
+          long long sum = 0;
+          for (int j = lane; j < m; j += 32) {
+            double d = 0.0;
+            const int cls = verify_point(T, s_pts[3 * j], s_pts[3 * j + 1], s_pts[3 * j + 2], sc, INFINITY, &d);
+            sum += cls == VERIFY_INLIER ? (int)floor(__dmul_rn(fmin(fabs(d), p.s.clamp_mm), 1000.0)) : clamp_um;
+          }
+          sum = warp_sum_ll(sum);
+          if (lane == 0) s_f[i] += sum;
+        }
+      }
+      __syncthreads();
+      if (k == 0 && tid == 0) { s_fs = s_f[0]; s_fg = s_f[0]; s_gi = -1; }
+      if (I > 0) {
+        for (int i = tid; i < P; i += PSO_THREADS)
+          if (s_f[i] < s_fp[i]) {
+            s_fp[i] = s_f[i];
+            for (int q = 0; q < 6; ++q) s_p[6 * i + q] = s_x[6 * i + q];
+          }
+        __syncthreads();
+        if (tid == 0) {
+          for (int i = 0; i < P; ++i)
+            if (s_fp[i] < s_fg) { s_fg = s_fp[i]; s_gi = i; }
+          if (p.record) p.record[(size_t)slot * p.record_words + 6 + k] = s_fg;
+        }
+        __syncthreads();
+        if (tid < 6 && s_gi >= 0) s_g[tid] = s_p[6 * s_gi + tid];
+      }
+      __syncthreads();
+    }
+    if (tid == 0) {
+      IcpOut o;
+      if (s_gi < 0) {
+        for (int q = 0; q < 16; ++q) o.T[q] = job.init[q];
+      } else {
+        pso_pose(s_g, s_c, S, o.T);
+        o.T[12] = 0.0; o.T[13] = 0.0; o.T[14] = 0.0; o.T[15] = 1.0;
+      }
+      o.fitness = __ddiv_rn(__ddiv_rn((double)s_fg, (double)n), 1000.0);
+      o.rmse = __ddiv_rn(__ddiv_rn((double)s_fs, (double)n), 1000.0);
+      o.iterations = I; o.pad = 0;
+      p.outs[slot] = o;
+    }
+    if (p.record) {
+      long long* r = p.record + (size_t)slot * p.record_words;
+      if (tid == 0) {
+        r[0] = s_fs; r[1] = s_fg; r[2] = s_gi;
+        for (int q = 0; q < 3; ++q) r[3 + q] = __double_as_longlong(s_c[q]);
+      }
+      long long* sw = r + 6 + I;
+      for (int e = tid; e < 6 * P; e += PSO_THREADS) {
+        const bool set = e < 6 * np;
+        sw[e] = __double_as_longlong(set ? s_x[e] : 0.0);
+        sw[6 * P + e] = __double_as_longlong(set ? s_v[e] : 0.0);
+        sw[12 * P + e] = __double_as_longlong(set ? s_p[e] : 0.0);
+      }
+      for (int i = tid; i < P; i += PSO_THREADS) sw[18 * P + i] = I > 0 ? s_fp[i] : 0x7FFFFFFFFFFFFFFFll;
+    }
+  }
+}
+
+static size_t pso_smem_bytes(int particles) { return sizeof(double) * 3 * PSO_CHUNK + (size_t)PSO_PARTICLE_BYTES * particles; }
+
+// k_pose_pso over p.n slots on st: a grid of at most the CTAs resident at once.
+// The CTAs of k_pose_pso resident at once on the current device with P particles: found once per (device, P), with the
+// kernel's shared-memory limit raised on the device the first time.
+static int pso_resident(int particles, int* out) {
+  static std::mutex mu;
+  static std::vector<std::vector<int>> resident;  // [device][P]: 0 until known
+  int dev = 0;
+  CUI(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  if ((int)resident.size() <= dev) resident.resize((size_t)dev + 1);
+  std::vector<int>& r = resident[(size_t)dev];
+  if (r.empty()) {
+    CUI(cudaFuncSetAttribute(k_pose_pso, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pso_smem_bytes(PSO_MAX_PARTICLES)));
+    r.assign(PSO_MAX_PARTICLES + 1, 0);
+  }
+  if (!r[(size_t)particles]) {
+    int sms = 0, per_sm = 0;
+    CUI(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    CUI(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pose_pso, PSO_THREADS, pso_smem_bytes(particles)));
+    r[(size_t)particles] = std::max(1, sms * per_sm);
+  }
+  *out = r[(size_t)particles];
+  return LM_OK;
+}
+
+static int launch_pso(const PsoParams& p, cudaStream_t st) {
+  if (p.n <= 0) return LM_OK;
+  const size_t smem = pso_smem_bytes(p.s.particles);
+  int resident = 1;
+  const int rc = pso_resident(p.s.particles, &resident);
+  if (rc) return rc;
+  const int grid = std::min(p.n, resident);
+  k_pose_pso<<<grid, PSO_THREADS, smem, st>>>(p);
+  CUI(cudaGetLastError());
+  return LM_OK;
+}
+
+extern "C" int lm_pose_search_points(int device, const double* pts, int64_t n, const double* start_t, const uint16_t* scene, int rows,
+                                     int cols, const float* sK, int particles, int iterations, double dt_mm, double dr_deg,
+                                     double clamp_mm, uint64_t seed, int64_t job, double* T_out, void* record, int64_t cap) {
+  if (!pts || !start_t || !scene || !sK || !T_out || (cap > 0 && !record)) return lm_fail(LM_E_INVALID, "null argument");
+  if (n < 1 || n > 0x7FFFFFFFll) return lm_fail(LM_E_INVALID, "%lld points, must lie in [1, 2^31 - 1]", (long long)n);
+  if (rows <= 0 || cols <= 0) return lm_fail(LM_E_INVALID, "empty scene %d x %d", rows, cols);
+  if (job < 0 || job >= PSO_MAX_JOB) return lm_fail(LM_E_INVALID, "job %lld outside [0, 2^40)", (long long)job);
+  PoseSearch s;
+  int rc = pose_search_make(particles, iterations, dt_mm, dr_deg, clamp_mm, seed, &s);
+  if (rc) return rc;
+  const int64_t words = pso_record_words(s);
+  if (cap > 0 && cap < 8 * words)
+    return lm_fail(LM_E_CAPACITY, "the swarm record needs %lld bytes, cap is %lld", (long long)(8 * words), (long long)cap);
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
+  CUI(cudaSetDevice(device));
+  // one allocation: pts [n][3], the job, its number, the output, the record, the scene
+  IcpJob j;
+  memset(&j, 0, sizeof(j));
+  j.src_first = j.tgt_first = 0; j.src_count = j.tgt_count = (int32_t)n;
+  for (int k = 0; k < 16; ++k) j.init[k] = (k % 5 == 0) ? 1.0 : 0.0;
+  for (int r = 0; r < 3; ++r) j.init[4 * r + 3] = start_t[r];
+  const int64_t jn = job;
+  auto a16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+  const size_t o_job = a16(sizeof(double) * 3 * (size_t)n), o_num = o_job + a16(sizeof(IcpJob)), o_out = o_num + 16;
+  const size_t o_rec = o_out + a16(sizeof(IcpOut)), o_scene = o_rec + a16(8 * (size_t)words);
+  DeviceArray<uint8_t> buf;
+  CUI(buf.assign(o_scene + sizeof(uint16_t) * (size_t)rows * cols));
+  uint8_t* b = buf.get();
+  CUI(cudaMemcpy(b, pts, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_job, &j, sizeof(j), cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_num, &jn, sizeof(jn), cudaMemcpyHostToDevice));
+  CUI(cudaMemcpy(b + o_scene, scene, sizeof(uint16_t) * (size_t)rows * cols, cudaMemcpyHostToDevice));
+  PsoParams p;
+  memset(&p, 0, sizeof(p));
+  p.jobs = reinterpret_cast<const IcpJob*>(b + o_job); p.pts = reinterpret_cast<const double*>(b);
+  p.outs = reinterpret_cast<IcpOut*>(b + o_out); p.n = 1;
+  p.scene = reinterpret_cast<const uint16_t*>(b + o_scene); p.srows = rows; p.scols = cols;
+  memcpy(p.sK, sK, sizeof(p.sK));
+  p.job = reinterpret_cast<const int64_t*>(b + o_num);
+  p.s = s;
+  p.record = reinterpret_cast<long long*>(b + o_rec); p.record_words = words;
+  rc = launch_pso(p, 0);
+  if (rc) return rc;
+  IcpOut o;
+  CUI(cudaMemcpy(&o, b + o_out, sizeof(o), cudaMemcpyDeviceToHost));
+  memcpy(T_out, o.T, sizeof(o.T));
+  if (cap > 0) CUI(cudaMemcpy(record, b + o_rec, 8 * (size_t)words, cudaMemcpyDeviceToHost));
   return LM_OK;
 }
 
@@ -1948,6 +2360,7 @@ struct PoseChunk {
   const int32_t* frame_of;
   const float* sKs;
   const float* sK;
+  const int32_t* frame_first;  // a batch's: frame f's first survivor in the run (k_pose_pso's job numbers); else null
   IcpOut* outs;
   uint8_t* posed;
   PoseVerify* ver;  // o.verify.on: per survivor its verification
@@ -1955,8 +2368,8 @@ struct PoseChunk {
   int32_t seq;
 };
 
-// k_pose_cloud, the segmented sort, k_pose_voxel, k_icp_normals (point-to-plane only) and the ICP kernel over this
-// rank's ceil(slots / world) slots, then (o.verify.on) k_pose_verify, then (shared) k_pose_collect.  A shared stage that
+// k_pose_cloud, the segmented sort, k_pose_voxel, k_icp_normals (point-to-plane only) and the ICP kernel (or k_pose_pso,
+// unshared only) over this rank's ceil(slots / world) slots, then (o.verify.on) k_pose_verify, then (shared) k_pose_collect.  A shared stage that
 // verifies runs the ICP kernel's unshared instantiation into d_souts, and k_pose_verify<true> publishes.  Unshared, the cloud's posed flags and the ICP results
 // go straight to the chunk's outputs; shared, to the stage's per-slot scratch, and k_pose_collect writes the outputs.
 // Returns the chunk's launches (the sort counted once), or an error code (< 0).
@@ -1973,7 +2386,8 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   p.scene = c.scene; p.srows = o.srows; p.scols = o.scols;
   if (c.sK) memcpy(p.sK, c.sK, sizeof(p.sK));
   else memset(p.sK, 0, sizeof(p.sK));
-  p.A = (int32_t)A; p.use_scene = o.use_scene_cloud ? 1 : 0;
+  const bool pso = o.estimation == LM_POSE_PSO;
+  p.A = (int32_t)A; p.use_scene = o.use_scene_cloud && !pso ? 1 : 0;  // the swarm registers against no target
   p.raw = s->d_raw.get(); p.cpts = s->d_cpts.get(); p.keys = s->d_keys[0].get(); p.vals = s->d_vals[0].get();
   p.seg_begin = s->d_seg.get(); p.seg_end = s->d_seg.get() + 2 * n;
   p.jobs = s->d_jobs.get(); p.err = c.status; p.posed = sh ? s->d_posed.get() : c.posed;
@@ -2006,7 +2420,19 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
     }
     k_pose_collect<<<1, POSE_COLLECT_THREADS, 0, st>>>(sd, c.outs, c.posed, o.verify.on ? c.ver : nullptr);
   } else {
-    launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.outs, o.max_iterations, nullptr, PoseShareDev());
+    if (pso) {
+      PsoParams q;
+      memset(&q, 0, sizeof(q));
+      q.jobs = s->d_jobs.get(); q.pts = s->d_pts.get(); q.outs = c.outs; q.n = n;
+      q.scene = c.scene; q.srows = o.srows; q.scols = o.scols;
+      memcpy(q.sK, p.sK, sizeof(q.sK));
+      q.frame_of = c.frame_of; q.sKs = c.sKs; q.frame_first = c.frame_first; q.first = c.first;
+      q.s = o.search;
+      const int rc = launch_pso(q, st);
+      if (rc) return rc;
+    } else {
+      launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.outs, o.max_iterations, nullptr, PoseShareDev());
+    }
     if (o.verify.on) k_pose_verify<false><<<n, VERIFY_THREADS, 0, st>>>(p, c.outs, o.verify.inlier_mm, c.ver, PoseShareDev());
   }
   CUI(cudaGetLastError());
@@ -2164,6 +2590,8 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
   const int nf = run.n_frames;
   const int64_t S = batch ? run.first[nf] : run.bound;  // survivors the outputs hold
   const int nc = batch ? pose_batch_chunks(S) : 1;
+  if (sh && o.estimation == LM_POSE_PSO)
+    return lm_fail(LM_E_STATE, "the pose stage shared over the ranks does not run LM_POSE_PSO: turn lm_peer_share_pose off");
   int rc = pose_prepare(s, st, nf, S, o.verify.on != 0);
   if (rc) return rc;
   if (batch) {  // each survivor's frame, each frame's first survivor and intrinsics, each chunk's status block and size
@@ -2190,7 +2618,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
     k.slots = batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound;
     k.first = c0;
     k.scene = run.d_scene; k.frame_of = batch ? s->d_bframe.get() + c0 : nullptr;
-    k.sKs = batch ? s->d_bsK.get() : nullptr; k.sK = batch ? nullptr : run.sK;
+    k.sKs = batch ? s->d_bsK.get() : nullptr; k.sK = batch ? nullptr : run.sK; k.frame_first = batch ? s->d_bfirst.get() : nullptr;
     k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.ver = s->d_bver.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
     const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
@@ -2713,6 +3141,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   o.srows = srows; o.scols = scols; o.use_scene_cloud = h->use_scene_cloud ? 1 : 0; o.max_iterations = max_iterations;
   o.estimation = h->estimation; o.stream = st; o.share = nullptr;
   o.verify = {h->verify ? 1 : 0, LM_VERIFY_RANK_FITNESS, h->verify_mm, -INFINITY};
+  o.search = h->search;
   const PoseTable table = {d.tpl.get(), d.crops.get(), reinterpret_cast<const int32_t*>(d.in.get() + o_cb), 1, n};
   const lm_match* d_surv = reinterpret_cast<const lm_match*>(d.in.get() + o_surv);
   const int32_t* d_cnt = reinterpret_cast<const int32_t*>(d.in.get() + o_cnt);
@@ -2721,7 +3150,7 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     PoseChunk k;
     k.table = table;
     k.surv = d_surv + c0; k.counts = d_cnt + c; k.slots = cnt[c]; k.first = c0;
-    k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK;
+    k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK; k.frame_first = nullptr;
     k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.ver = h->verify ? d.ver.get() + c0 : nullptr;
     k.status = d.status.get() + 4 * c; k.seq = 0;
     const int l = pose_chunk(&d.stage, o, k);

@@ -3,7 +3,8 @@
 // The pose stage refines the NMS survivors of k_post_nms where they lie: per-template render crops registered once
 // (lm_set_template_renders), then per run k_pose_cloud (box test, back-projection, centroids, voxel keys), a CUB
 // segmented radix sort of the voxel keys, k_pose_voxel (voxel means) and the ICP kernels of lm_icp_process_batch
-// (k_icp_normals + k_icp_point_to_plane, or k_icp_point_to_point alone), all on the detector's stream.  A run is a batch
+// (k_icp_normals + k_icp_point_to_plane, or k_icp_point_to_point alone), or the particle swarm k_pose_pso in their
+// place (LM_POSE_PSO), all on the detector's stream.  A run is a batch
 // of frames, and a single frame is a one-frame run of the same stage: the same chunks, outputs, readbacks and finish.
 // The host composes result = T * init_base after the copy.  The pose NMS (k_pose_nms, one CTA per frame behind the ICP
 // kernel) composes the poses on the device instead, runs the greedy translation NMS of linemod_ros/detect.py over them
@@ -53,14 +54,28 @@ struct PoseVerifyOptions {
   double inlier_mm, min_score;
 };
 
+// The particle swarm of LM_POSE_PSO (lm_set_pose_search, include/linemod_b200.h): P, I, the bounds in metres and
+// radians, the cost clamp in mm and the seed of the generator.
+struct PoseSearch {
+  int particles, iterations;
+  double dt, dr, clamp_mm;
+  unsigned long long seed;
+};
+// The defaults (64 particles, 40 iterations, 40 mm, 30 degrees, 20 mm, seed 0).
+PoseSearch pose_search_default();
+// LM_E_INVALID (with the message) unless the arguments of lm_set_pose_search lie within its limits; else *out.
+int pose_search_make(int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm, uint64_t seed, PoseSearch* out);
+
 // What every chunk of a run shares.
 struct PoseOptions {
   int srows, scols;           // scene depth size
   int use_scene_cloud, max_iterations;
-  int estimation;             // LM_ICP_POINT_TO_PLANE (k_icp_normals + k_icp_point_to_plane) or LM_ICP_POINT_TO_POINT
+  int estimation;             // LM_ICP_POINT_TO_PLANE (k_icp_normals + k_icp_point_to_plane), LM_ICP_POINT_TO_POINT or
+                              // LM_POSE_PSO (k_pose_pso; no target cloud is built)
   cudaStream_t stream;
-  const PoseShare* share;     // null: this rank refines every survivor
+  const PoseShare* share;     // null: this rank refines every survivor (LM_POSE_PSO: always)
   PoseVerifyOptions verify;  // zero: off
+  PoseSearch search;          // LM_POSE_PSO only
 };
 
 // One run of the pose stage: a batch of frames (lm_detect_batch, lm_peer_detect_batch), or a frame as a one-frame run

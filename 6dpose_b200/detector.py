@@ -68,6 +68,7 @@ class Detector:
         self._template_depths = None  # training distances registered with the native handle (setTemplateDepths)
         self._peers = None  # (rank, world) once dist.connect_peers has wired the fused exchange
         self._verify = _lib.verify_options(None)  # lm_set_pose_verify's arguments (setPoseVerification)
+        self._search = _lib.pose_search_options()  # lm_set_pose_search's arguments (setPoseSearch)
         self.device = _default_device()
         self.shard = (0, 1)  # (index, count): template shard matched by this process (multi-GPU)
         self.shard_layout = _lib.SHARD_CONTIGUOUS
@@ -305,9 +306,18 @@ class Detector:
         survivors scoring below it are dropped before the pose NMS.  A pose stage shared over the ranks verifies too."""
         self._verify = _lib.verify_options(inlier_mm, rank_by, min_score)
 
+    def setPoseSearch(self, particles=64, iterations=40, dt_mm=40.0, dr_deg=30.0, clamp_mm=20.0, seed=0):
+        """The particle swarm of estimation="pso" (include/linemod_b200.h, LM_POSE_PSO / lm_set_pose_search) for
+        match_refine, detect, the batch calls and dist's unshared sharded calls: particles, iterations, the bounds of the
+        search about the ICP's initial guess (translation dt_mm per axis, rotation dr_deg per axis about the cloud's
+        centroid), the per-point cost clamp in mm and the seed of its random numbers.  Checked here, before any device
+        work; the defaults are 64, 40, 40 mm, 30 degrees, 20 mm and 0."""
+        self._search = _lib.pose_search_options(particles, iterations, dt_mm, dr_deg, clamp_mm, seed)
+
     def _pose_native(self, class_ids):
         nat = self._select(list(class_ids))
         nat.set_pose_verify(*self._verify)
+        nat.set_pose_search(*self._search)
         return nat
 
     def _verification(self, nat, sizes):

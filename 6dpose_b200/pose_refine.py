@@ -26,8 +26,9 @@ class poseRefine:
 
     def __init__(self, estimation="point_to_plane"):
         """estimation (not in the reference's surface, which takes no argument): the ICP's estimation step,
-        "point_to_plane" (TransformationEstimationPointToPlane, the reference's active branch) or "point_to_point"
-        (TransformationEstimationPointToPoint, its other branch at LL.cpp:131-135: no normals, Umeyama's rigid fit)."""
+        "point_to_plane" (TransformationEstimationPointToPlane, the reference's active branch), "point_to_point"
+        (TransformationEstimationPointToPoint, its other branch at LL.cpp:131-135: no normals, Umeyama's rigid fit) or
+        "pso" (a particle swarm against the scene depth, include/linemod_b200.h LM_POSE_PSO; see process's pose_search)."""
         _lib.estimation_code(estimation)
         self.estimation = estimation
         self._residual = -1.0
@@ -54,15 +55,17 @@ class poseRefine:
         return a
 
     def process(self, sceneDepth, modelDepth, sceneK, modelK, modelR, modelT, detectX, detectY, depth_scale=1.0, render_scale=1.0,
-                stream=None, verify_mm=None):
+                stream=None, verify_mm=None, pose_search=None):
         """sceneDepth / modelDepth: uint16 HxW numpy images (mm), or CUDA tensors on this object's device: uint16 (mm) or
         float32 [H, W], pixels packed within a row.  depth_scale / render_scale convert float32 depth to mm (the driver's
         depth_ren.astype(np.uint16) is render_scale 1.0); stream: the torch stream the tensors are ordered on (None: the
         current stream).  verify_mm (not in the reference's surface): verify the refined pose against the scene depth with
         this inlier distance in mm (include/linemod_b200.h, lm_set_pose_verify); getScore / getVerification then return
-        the result.  None: no verification."""
+        the result.  None: no verification.  pose_search (estimation "pso" only): a dict of the swarm's settings
+        (Detector.setPoseSearch's keywords); None: the defaults."""
         if verify_mm is not None:
             _lib.inlier_mm(verify_mm)
+        search = _lib.pose_search_options(**(pose_search or {}))
         dev = _lib.depth_inputs(sceneDepth, [modelDepth], depth_scale, render_scale, stream, self.device,
                                 host=dict(sceneK=sceneK, modelK=modelK, modelR=modelR, modelT=modelT))
         if dev is None:
@@ -77,6 +80,7 @@ class poseRefine:
         args = (sK, mK[None], R[None], t[None], [[int(detectX), int(detectY)]], self.max_iterations, self.estimation)
         icp = _native(self.device)
         icp.set_verify(verify_mm)
+        icp.set_pose_search(*search)
         if dev is None:
             Ro, to, res = icp.process_batch(scene, [model], *args)
         else:
@@ -109,17 +113,19 @@ class poseRefine:
 
 
 def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, modelTs, device=None, estimation="point_to_plane",
-                   depth_scale=1.0, render_scale=1.0, stream=None, verify_mm=None):
+                   depth_scale=1.0, render_scale=1.0, stream=None, verify_mm=None, pose_search=None):
     """The drivers' loop over the NMS survivors (linemod_and_levelup_test.py:348-367: one poseRefine per
     match, fed with the render of the matched template's pose) as ONE batched GPU call: hypothesis i is
     matches[i] (its x, y) with modelDepths[i] / modelKs[i] / modelRs[i] / modelTs[i].  Returns a list of
     poseRefine objects in the state process() would have left them in.  estimation as poseRefine().
     Depths in device memory: sceneDepth a CUDA tensor and modelDepths a list of [H, W] CUDA tensors or one [n, H, W]
     tensor, with depth_scale, render_scale and stream as poseRefine.process.  verify_mm as poseRefine.process: every
-    survivor comes back with its score, none is dropped."""
+    survivor comes back with its score, none is dropped.  pose_search as poseRefine.process; match i draws the swarm's
+    random numbers as job i."""
     _lib.estimation_code(estimation)
     if verify_mm is not None:
         _lib.inlier_mm(verify_mm)
+    search = _lib.pose_search_options(**(pose_search or {}))
     n = len(matches)
     dev = _default_device() if device is None else int(device)
     renders = modelDepths if _lib.is_tensor(modelDepths) else list(modelDepths)
@@ -142,6 +148,7 @@ def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, m
     xy = [[int(m.x), int(m.y)] for m in matches]
     icp = _native(dev)
     icp.set_verify(verify_mm)
+    icp.set_pose_search(*search)
     if inputs is None:
         Ro, to, res = icp.process_batch(scene, models, sK, mK, R, t, xy, poseRefine.max_iterations, estimation)
     else:

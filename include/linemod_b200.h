@@ -316,10 +316,73 @@ int lm_complete_pose(lm_detector* d, lm_match* out, double* R_out, double* t_out
  * lm_set_pose_estimation sets it for the detector's next lm_enqueue_pose, lm_detect_batch and lm_peer_detect_batch; a frame
  * keeps the estimation it was enqueued with (the pose stage rerun after a result-block retry included).  No device work.
  * A frame's pose stage is then 4 launches (5 shared), a batch chunk likewise.  With a connected peer exchange, setting the
- * same value on every rank is the caller's promise, as with lm_peer_share_pose.  LM_E_INVALID for any other value. */
+ * same value on every rank is the caller's promise, as with lm_peer_share_pose.  LM_POSE_PSO (below) replaces the ICP
+ * with a particle swarm.  LM_E_INVALID for any other value. */
 #define LM_ICP_POINT_TO_PLANE 0 /* TransformationEstimationPointToPlane, the reference's active branch (default) */
 #define LM_ICP_POINT_TO_POINT 1 /* TransformationEstimationPointToPoint, LL.cpp:131-135 */
+#define LM_POSE_PSO 3           /* particle swarm against the scene depth (below); 2 is not assigned and stays refused */
 int lm_set_pose_estimation(lm_detector* d, int estimation);
+
+/* LM_POSE_PSO: a third estimation, correspondence-free.  It replaces the ICP kernel of the pose stage with k_pose_pso
+ * (one CTA per slot, persistent over the slots); the clouds before it and everything after it (the composition
+ * T * init_base, verification, the pose NMS, the readbacks, the chunks) are unchanged.  k_icp_normals does not run, so a
+ * frame's pose stage is 4 launches, as with point-to-point.  The item the reference's author left open
+ * (linemodLevelup/notes.md: "PSO ... Correspondence-free pose estimation for 3D objects from noisy depth data").
+ * Every operation below is correctly rounded (no FMA), in the order written, so tests/pose_pso_model.py restates it bit for
+ * bit in numpy float64.  "a + b" etc. are double operations unless marked.
+ *   Points   p_j, j < n: the down-sampled source cloud the ICP would register (metres, double, its order).  n = 0: T = S,
+ *            fitness = rmse = 0.
+ *   Start    S = the ICP's initial guess, identity rotation and translation s (the centroid difference).  A slot without
+ *            a pose stays without one (residual -1, the early return of LL.cpp:52-55).  c_r = (sum_j (p_jr + s_r)) / n,
+ *            summed from 0.0 in index order: the centroid under S.
+ *   Particle x = (w0, w1, w2, t0, t1, t2), |w_k| <= dr (rad), |t_k| <= dt (m).  Its pose T(x) = Trans(c + t) Rot(w)
+ *            Trans(-c) S, as [R | u]:
+ *              y = (w0*w0 + w1*w1) + w2*w2.  y == 0: R = I.  Else A = sin(sqrt y)/sqrt y and B = (1 - cos(sqrt y))/y by
+ *              their Taylor series to y^10 in Horner form (acc = a_10; acc = a_k + y*acc for k = 9..0; coefficients
+ *              (-1)^k/(2k+1)! and (-1)^k/(2k+2)! as the nearest doubles; dr <= 45 degrees keeps them exact to rounding),
+ *              K = [w]x, K2_rc = w_r*w_c (r != c), K2_rr = w_r*w_r - y, R_rc = (I_rc + A*K_rc) + B*K2_rc (Rodrigues).
+ *              a_r = s_r - c_r;  u_r = (s_r + ((((R_r0*a_0) + R_r1*a_1) + R_r2*a_2) - a_r)) + t_r.
+ *            x = 0 gives R = I and u = s.
+ *   Cost     per point: q = T(x) p and its pixel exactly as pose verification's steps 3-4 (one shared device routine).
+ *            Outside the frame or missing depth: e = clamp; else e = min(|d|, clamp), d in mm.  cost_j = (int32)floor(e *
+ *            1000) (micrometres), the particle's cost sum_j cost_j in int64: exact in any order.  Lower is better.
+ *   Swarm    P particles, I iterations.  Particle 0 starts at x = 0, particle i >= 1 at x_k = (2 D_k) * r - D_k with
+ *            D = (dr, dr, dr, dt, dt, dt) and r = draw (i, iteration 0, k); velocities start at 0.  The best is the start
+ *            (cost(S), evaluated as particle 0 of iteration 0).  Iteration k = 0 .. I-1: for k > 0 every particle moves,
+ *              v = ((w*v + (c1*r1)*(p - x)) + (c2*r2)*(g - x)), r1 = draw (i, k, coordinate), r2 = draw (i, k, 6 +
+ *              coordinate), w = 0.7298, c1 = c2 = 1.49618 (Clerc); v clamped to [-D, D]; x = x + v; where x leaves
+ *              [-D, D] it is clamped to it and that coordinate of v set to 0;
+ *            then every particle is evaluated; a particle's best p takes x when its cost is strictly lower (the first
+ *            evaluation always); then the global best g takes the best personal best, the lowest index on ties, when its
+ *            cost is strictly lower.  I = 0 evaluates the start alone.
+ *   Draws    draw (i, k, q) of job J: splitmix64 seeded with `seed`, its output number ((J * 1024 + k) * 1024 + i) * 16 + q
+ *            (0-based): z = seed + (number + 1) * 0x9E3779B97F4A7C15; z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9; z = (z ^ z >>
+ *            27) * 0x94D049BB133111EB; z ^= z >> 31 (all mod 2^64), r = (z >> 11) * 2^-53 in [0, 1).  J is the
+ *            survivor's index in its frame's pick order (lm_icp: the hypothesis index), so a batch frame, a single frame
+ *            and a sharded unshared batch draw the same numbers for the same survivor.
+ *   Output   the IcpOut of the slot: T = S while the start stays the best, else T(g); fitness = cost(g) / n / 1000 (mm per
+ *            point, lower is better, so the pose NMS's -residual keeps its meaning); rmse = cost(S) / n / 1000 (what the
+ *            search gained); iterations = I.  So cost(result) <= cost(S), and P = 1 or I = 0 returns S bit for bit.
+ * The objective sees the surface the template's render sees, moved by T(x), as verification does: faces the new pose would
+ * show are not checked.  use_scene_cloud has no effect: no target cloud is built.  The pose stage shared over the ranks
+ * (lm_peer_share_pose) does not run it: lm_enqueue_pose and lm_peer_detect_batch return LM_E_STATE there.
+ *   lm_set_pose_search      P (1..256), I (0..1000), dt_mm (0..10000), dr_deg (0..45), clamp_mm (0..1e6), all finite,
+ *                           and the seed, for the detector's next pose stage; a frame keeps the settings it was
+ *                           enqueued with, as the estimation.  LM_E_INVALID outside those limits.  No device work.
+ *                           Defaults: 64, 40, 40 mm, 30 degrees, 20 mm, seed 0.
+ *   lm_icp_set_pose_search  the same for the next lm_icp_process_batch / _device.
+ *   lm_pose_search_points   the kernel on caller arrays: pts [n][3] f64 (m, 1 <= n < 2^31), start_t [3] f64 (s), scene
+ *                           rows x cols u16 mm, sK [9] f32, the search settings and the job number J (0 <= J < 2^40).
+ *                           T_out [16] f64 the result.  record (cap bytes, 8-byte words; may be null with cap 0): the
+ *                           swarm record of LM_ICP_CAPTURE_SEARCH.
+ * Swarm record (8 * (6 + I + 19 P) bytes): int64 cost(S), int64 cost(result), int64 index of the best particle (-1: the
+ * start), f64 c[3], int64 global-best cost after each iteration [I], then the final f64 positions [P][6], velocities
+ * [P][6] and personal bests [P][6], and int64 personal-best costs [P] (before any evaluation: INT64_MAX). */
+int lm_set_pose_search(lm_detector* d, int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm,
+                       uint64_t seed);
+int lm_pose_search_points(int device, const double* pts, int64_t n, const double* start_t, const uint16_t* scene, int rows,
+                          int cols, const float* sK, int particles, int iterations, double dt_mm, double dr_deg,
+                          double clamp_mm, uint64_t seed, int64_t job, double* T_out, void* record, int64_t cap);
 
 /* Pose NMS on the device: the end of linemod_ros/detect.py's frame (:91-141), which refines every box-NMS survivor and
  * then drops duplicate objects in pose space with nms_norms(ts, -residual, 40.0) (:41-50, :130-131).  One CTA behind the
@@ -692,6 +755,10 @@ int lm_icp_set_use_scene_cloud(lm_icp* h, int on);
  * kernel alone, 1 launch; lm_icp_last_stats [3] then times that kernel alone) for the next lm_icp_process_batch.
  * LM_E_INVALID for any other value. */
 int lm_icp_set_estimation(lm_icp* h, int estimation);
+/* LM_POSE_PSO's settings for this handle (see lm_set_pose_search); with LM_POSE_PSO lm_icp_process_batch uploads the scene
+ * and runs k_pose_pso alone (1 launch, timed by lm_icp_last_stats [3]). */
+int lm_icp_set_pose_search(lm_icp* h, int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm,
+                           uint64_t seed);
 int64_t lm_icp_launch_count(lm_icp* h);
 /* Pose verification (see lm_set_pose_verify) for the next lm_icp_process_batch and lm_icp_process_batch_device: one more
  * launch per call (per chunk of 1024 hypotheses on the device path); the host path also uploads its raw model clouds and
@@ -716,9 +783,11 @@ int lm_icp_set_capture(lm_icp* h, int on);
  *   KNN         tgt x 30 int32: the neighbours k_icp_normals kept (target indices, kept order, padded with -1)
  *   CORR_FIRST  src int32: the correspondence (target index, -1: none) of every source point on pass 0
  *   CORR_LAST   src int32: the same for the last pass the kernel ran (the pass whose fitness and rmse are returned)
+ *   SEARCH      the swarm record of an LM_POSE_PSO call (lm_set_pose_search), lm_icp_process_batch only
  * LM_E_STATE for a hypothesis that took the early return, and for NORMALS / KNN of a call with LM_ICP_POINT_TO_POINT
- * (nothing was computed), LM_E_CAPACITY when cap is too small, LM_E_INVALID for a hypothesis outside the last captured
- * call. */
+ * or LM_POSE_PSO (nothing was computed), CORR_* of an LM_POSE_PSO call and SEARCH of any other call or of
+ * lm_icp_process_batch_device, LM_E_CAPACITY when cap is too small, LM_E_INVALID for a hypothesis outside the last
+ * captured call. */
 #define LM_ICP_CAPTURE_COUNTS 0
 #define LM_ICP_CAPTURE_SOURCE 1
 #define LM_ICP_CAPTURE_TARGET 2
@@ -728,6 +797,7 @@ int lm_icp_set_capture(lm_icp* h, int on);
 #define LM_ICP_CAPTURE_KNN 6
 #define LM_ICP_CAPTURE_CORR_FIRST 7
 #define LM_ICP_CAPTURE_CORR_LAST 8
+#define LM_ICP_CAPTURE_SEARCH 13
 int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t cap);
 
 #ifdef __cplusplus
