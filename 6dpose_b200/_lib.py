@@ -329,7 +329,7 @@ class DeviceDepths:
 
 
 def depth_inputs(scene, renders, depth_scale, render_scale, stream, device, n=None, host=None):
-    """A DeviceDepths when the scene or any render is a tensor, None for numpy arrays (the host path, where depth_scale
+    """A DeviceDepths when the scene or any render is a tensor, None for numpy arrays (process_batch, where depth_scale
     and render_scale must stay 1.0 and stream None).  TypeError / ValueError before any library call."""
     if not (is_tensor(scene) or is_tensor(renders) or any(is_tensor(r) for r in renders)):
         host_frame_options(depth_scale, stream)
@@ -1158,9 +1158,8 @@ class NativeIcp:
         self.device = int(device)
         self._estimation = "point_to_plane"  # the handle's estimation (lm_icp_set_estimation)
         self._search = pose_search_options()  # its swarm settings (lm_icp_set_pose_search)
-        self._captured = None               # the estimation of the last process_batch (capture())
+        self._captured = None               # the estimation of the last call (capture())
         self._captured_search = None        # and its swarm settings
-        self._captured_device = False       # the last call was process_batch_device: clouds, init and result only
 
     def close(self):
         if getattr(self, "_h", None):
@@ -1175,8 +1174,9 @@ class NativeIcp:
 
     def process_batch(self, scene_depth, model_depths, sceneK, modelKs, Rs, ts, detect_xy, max_iterations=30, estimation=None):
         """scene u16 HxW; model_depths list of u16 HxW (same size); modelKs/Rs [n,3,3] f32; ts [n,3] f32;
-        detect_xy [n,2] int.  estimation: "point_to_plane" or "point_to_point" for this call and the next ones (None: as
-        set before, point-to-plane on a new handle).  Returns (R [n,3,3] f64, t [n,3] f64 mm, residual [n] f32)."""
+        detect_xy [n,2] int.  estimation: "point_to_plane", "point_to_point" or "pso" for this call and the next ones (None:
+        as set before, point-to-plane on a new handle).  The scene and each distinct render are copied to the device once,
+        then the call runs as process_batch_device.  Returns (R [n,3,3] f64, t [n,3] f64 mm, residual [n] f32)."""
         if estimation is not None:
             self.set_estimation(estimation)
         n = len(model_depths)
@@ -1204,12 +1204,11 @@ class NativeIcp:
                                            res.ctypes.data_as(f32p)))
         self._captured = self._estimation
         self._captured_search = self._search
-        self._captured_device = False
         return Ro, to, res
 
     def process_batch_device(self, depths, sceneK, modelKs, Rs, ts, detect_xy, max_iterations=30, estimation=None):
-        """process_batch for a DeviceDepths (lm_icp_process_batch_device): the same outputs, bit for bit, as process_batch
-        on the u16 images the depths convert to; sceneK, modelKs, Rs, ts and detect_xy as there."""
+        """process_batch for a DeviceDepths (lm_icp_process_batch_device), read where they lie: the same outputs, bit for
+        bit, as process_batch on the u16 images the depths convert to; sceneK, modelKs, Rs, ts and detect_xy as there."""
         if estimation is not None:
             self.set_estimation(estimation)
         n = depths.n
@@ -1232,7 +1231,7 @@ class NativeIcp:
                                                   int(max_iterations), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p),
                                                   res.ctypes.data_as(f32p), depths.stream.cuda_stream))
         self._captured = self._estimation
-        self._captured_device = True
+        self._captured_search = self._search
         return Ro, to, res
 
     def set_use_scene_cloud(self, on):
@@ -1266,38 +1265,24 @@ class NativeIcp:
         return out
 
     def capture(self, hyp):
-        """What the kernels saw and kept for hypothesis `hyp` of the last process_batch with capture on (see
-        lm_icp_capture): source / target [n,3] f64, normals [nt,3] f64, init [4,4] f64, T [4,4] f64, fitness, rmse,
-        iterations, knn [nt,30] int32 (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence).  After a
-        point-to-point call normals and knn are None: that estimation computes neither.  After process_batch_device
-        normals, knn, corr_first and corr_last are None: that path keeps the clouds, init and result only.  After a "pso"
-        call of process_batch normals, knn and the correspondences are None and `search` is the swarm record
-        (search_record)."""
+        """What the kernels saw and kept for hypothesis `hyp` of the last call with capture on (see lm_icp_capture): source
+        / target [n,3] f64, normals [nt,3] f64, init [4,4] f64, T [4,4] f64, fitness, rmse, iterations, knn [nt,30] int32
+        (-1 padded), corr_first / corr_last [n] int32 (-1: no correspondence), search the swarm record (search_record).
+        An item is None where the call's estimation computed nothing: normals and knn but under "point_to_plane", the
+        correspondences under "pso", search but under "pso"."""
         n, nt = self._capture_item(hyp, 0, np.zeros(2, np.int32)).tolist()
         res = self._capture_item(hyp, 5, np.zeros(19, np.float64))
-        p2pl = self._captured == "point_to_plane"
-        if self._captured == "pso" and not self._captured_device:
-            P, I = self._captured_search[:2]
-            words = self._capture_item(hyp, 13, np.zeros(6 + I + 19 * P, np.int64))
-            return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
-                        target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)), normals=None,
-                        init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
-                        T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
-                        knn=None, corr_first=None, corr_last=None, search=search_record(words, P, I))
-        if self._captured_device:
-            return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
-                        target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)), normals=None,
-                        init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
-                        T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
-                        knn=None, corr_first=None, corr_last=None)
+        p2pl, pso = self._captured == "point_to_plane", self._captured == "pso"
+        P, I = self._captured_search[:2]
         return dict(source=self._capture_item(hyp, 1, np.zeros((n, 3), np.float64)),
                     target=self._capture_item(hyp, 2, np.zeros((nt, 3), np.float64)),
                     normals=self._capture_item(hyp, 3, np.zeros((nt, 3), np.float64)) if p2pl else None,
                     init=self._capture_item(hyp, 4, np.zeros((4, 4), np.float64)),
                     T=res[:16].reshape(4, 4).copy(), fitness=float(res[16]), rmse=float(res[17]), iterations=int(res[18]),
                     knn=self._capture_item(hyp, 6, np.zeros((nt, 30), np.int32)) if p2pl else None,
-                    corr_first=self._capture_item(hyp, 7, np.zeros(n, np.int32)),
-                    corr_last=self._capture_item(hyp, 8, np.zeros(n, np.int32)))
+                    corr_first=None if pso else self._capture_item(hyp, 7, np.zeros(n, np.int32)),
+                    corr_last=None if pso else self._capture_item(hyp, 8, np.zeros(n, np.int32)),
+                    search=search_record(self._capture_item(hyp, 13, np.zeros(6 + I + 19 * P, np.int64)), P, I) if pso else None)
 
     def last_stats(self):
         a = (ctypes.c_double * 4)()

@@ -3,9 +3,10 @@
 // Reference being replaced: poseRefine::process, linemodLevelup/linemodLevelup.cpp:27-155 of
 // meiqua/6DPose @ 619be57 ("LL.cpp"), and the Open3D calls it makes (Open3D is external and unpinned
 // in the reference -- oracle/icp_oracle.py documents the restated semantics; PARITY UNPINNED).
-//   host (this file)      <- mask dilation + bounding box, cloud construction, voxel down-sampling
+//   k_pose_cloud, a CUB segmented sort, k_pose_voxel
+//                         <- mask dilation + bounding box, cloud construction, voxel down-sampling
 //                            (LL.cpp:34-109; PointCloud::VoxelDownSample)
-//   k_icp_normals         <- PointCloud::EstimateNormals, KNN = 30 (LL.cpp:127)
+//   k_icp_normals        <- PointCloud::EstimateNormals, KNN = 30 (LL.cpp:127)
 //   k_icp_point_to_plane  <- RegistrationICP + TransformationEstimationPointToPlane (LL.cpp:128-130):
 //                            nearest-neighbour correspondence search fused with the 6x6 J^T J / J^T r
 //                            accumulation, the 6x6 solve and the convergence test; every iteration of
@@ -17,14 +18,14 @@
 // down-sampled MODEL cloud (LL.cpp:109), only the z component of the initial translation is converted
 // to metres (LL.cpp:37), `residual` carries the fitness (LL.cpp:148).
 //
-// The pose stage (lm_pose.h, end of this file) does the host's cloud building on the device for the detector's NMS
-// survivors: k_pose_cloud + a CUB segmented sort + k_pose_voxel build the same clouds and initial guesses, bit for
-// bit, and feed the same ICP kernels; k_pose_nms may follow.  A frame, a batch chunk and their shared forms are all
-// one chunk to pose_chunk and to the kernels, told apart by data only: the survivor count on the device, an optional
-// frame table, and the slot rule survivor = rank + slot * world.  lm_icp_process_batch_device feeds the same chunks from
-// renders and a scene in the caller's device memory: k_icp_scene, k_icp_render_box and k_icp_render_crop build the
-// per-hypothesis table k_pose_cloud reads (end of this file).  With verification on (lm_set_pose_verify, lm_icp_set_verify)
-// k_pose_verify follows the ICP kernel of an unshared chunk, and of lm_icp_process_batch, and k_pose_nms<true> reads it.
+// The pose stage (lm_pose.h, end of this file) builds the clouds and initial guesses and feeds them to the ICP kernels;
+// k_pose_nms may follow.  A frame, a batch chunk and their shared forms are all one chunk to pose_chunk and to the
+// kernels, told apart by data only: the survivor count on the device, an optional frame table, and the slot rule
+// survivor = rank + slot * world.  lm_icp_process_batch and lm_icp_process_batch_device feed the same chunks from renders
+// and a scene (staged from the host, or in the caller's device memory): k_icp_scene, k_icp_render_box and
+// k_icp_render_crop build the per-hypothesis table k_pose_cloud reads (end of this file).  With verification on
+// (lm_set_pose_verify, lm_icp_set_verify) k_pose_verify follows the ICP kernel of an unshared chunk, and k_pose_nms<true>
+// reads it.
 
 #include "linemod_b200.h"
 #include "lm_pose.h"
@@ -42,7 +43,7 @@
 #include <limits>
 #include <memory>
 #include <mutex>
-#include <thread>
+#include <unordered_map>
 #include <vector>
 
 int lm_fail(int code, const char* fmt, ...);  // linemod_b200.cu
@@ -117,7 +118,7 @@ struct PsoParams {
   const float* sKs;
   const int32_t* frame_first; // batch: frame f's first survivor in the run (job = first + slot - frame_first[frame])
   int64_t first;              // run index of slot 0's survivor
-  const int64_t* job;         // per slot its job number (lm_icp_process_batch, lm_pose_search_points); null: as above
+  const int64_t* job;         // per slot its job number (lm_pose_search_points); null: as above
   PoseSearch s;
   long long* record;          // null, or the slots' swarm records, record_words apart
   int64_t record_words;
@@ -167,7 +168,7 @@ __device__ void smallest_eigenvector_3x3(double a00, double a01, double a02, dou
   else { n[0] = 0; n[1] = 0; n[2] = 1; }
 }
 
-// The clouds come out of voxel_down_sample sorted by voxel (x major), so index distance is spatial distance along
+// The clouds come out of k_pose_voxel sorted by voxel (x major), so index distance is spatial distance along
 // x: tiles are visited outwards from the CTA's own points, and a side is abandoned once the x gap alone puts every
 // remaining candidate beyond the current 30th neighbour of every thread (exact: a point of voxel column a has
 // x in [lo_a, lo_a + ICP_VOXEL)).  The kept set is the 30 smallest (distance, index) pairs in that order --
@@ -564,7 +565,7 @@ __device__ __forceinline__ void icp_registration(const IcpJob* __restrict__ jobs
       double best = max_d2;  // radius search, strict <
       int bj = -1;
       for (int t0 = 0; t0 < nt; t0 += ICP_TILE) {
-        // The target cloud is sorted by voxel, x major (voxel_down_sample), so a tile covers the x range
+        // The target cloud is sorted by voxel, x major (k_pose_voxel), so a tile covers the x range
         // [x(first) - voxel, x(last) + voxel]: a tile whose range is farther from EVERY source point of this pass than its
         // best squared distance so far cannot change any correspondence (strict <) and is skipped -- exact, and most
         // tiles go: the search radius is 1 cm, the cloud is ~10 cm wide
@@ -722,50 +723,41 @@ __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShare
 // --------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------
-struct IcpDevice;                    // lm_icp_process_batch_device's buffers (end of this file)
+struct IcpDevice;                    // the calls' buffers (end of this file)
+static IcpDevice* icp_device_new();
 static void icp_device_free(IcpDevice* d);
 
 struct lm_icp {
   int device = 0;
   Stream stream;  // streams and events first: they outlive the buffers
   Event ev0, ev1;
-  DeviceArray<double> d_pts, d_nrm;  // [points][3]
-  DeviceArray<IcpJob> d_jobs; DeviceArray<IcpOut> d_outs;
-  PinnedArray<IcpOut> h_outs;
+  Event ev_in, ev_out;  // lm_icp_process_batch_device: the caller's stream -> the call -> the caller's stream
   int64_t launches = 0;
   bool use_scene_cloud = false;  // non-reference option: register against the scene cloud
   int estimation = LM_ICP_POINT_TO_PLANE;
   PoseSearch search = pose_search_default();  // lm_icp_set_pose_search (LM_POSE_PSO)
-  DeviceArray<uint8_t> d_sbuf;  // LM_POSE_PSO on the host path: the scene, the jobs' hypothesis numbers, their swarm records
-  PinnedArray<uint8_t> h_sbuf;  // and the host staging of the first two (a call ends in a synchronise: it is free again)
   int last_points = 0, last_iterations = 0;
   double last_rmse = 0;
   float last_kernel_us = 0;
-  // lm_icp_set_capture: the kernels' intermediate results of the last lm_icp_process_batch (or _device)
+  // lm_icp_set_capture: the kernels' intermediate results of the last call, per point in the order of pts
   bool capture = false;
-  DeviceArray<int32_t> d_knn, d_corr;  // [points][ICP_KNN], [points][2]
   struct {
     int estimation = LM_ICP_POINT_TO_PLANE;  // point-to-point computes no normals and no neighbour lists
-    bool device = false;                     // lm_icp_process_batch_device: clouds, initial guesses and results only
     std::vector<IcpJob> jobs;
     std::vector<int> job_of;  // per hypothesis, -1: early return
     std::vector<IcpOut> outs;
     std::vector<double> pts, nrm;
     std::vector<int32_t> knn, corr;
-    std::vector<long long> record;  // LM_POSE_PSO (host path): the jobs' swarm records, record_words apart
+    std::vector<long long> record;  // LM_POSE_PSO: the jobs' swarm records, record_words apart
     int64_t record_words = 0;
   } cap;
-  IcpDevice* dev = nullptr;  // created by the first lm_icp_process_batch_device
+  IcpDevice* dev = nullptr;
   // lm_icp_set_verify, and the verification of the last call's hypotheses (verified false: that call did not verify)
   bool verify = false;
   double verify_mm = 10.0;
   bool verified = false;
   std::vector<PoseVerify> ver;
-  DeviceArray<uint8_t> d_vbuf;  // the host path's verification inputs and outputs (icp_verify_host)
 };
-
-static int icp_verify_host(lm_icp* h, const std::vector<int>& job_of, const std::vector<std::vector<double>>& raw,
-                           const uint16_t* scene, int srows, int scols, const float* sK);
 
 extern "C" int lm_icp_create(int device, lm_icp** out) {
   if (!out) return lm_fail(LM_E_INVALID, "out is null");
@@ -780,6 +772,9 @@ extern "C" int lm_icp_create(int device, lm_icp** out) {
   CUI(h->stream.create(cudaStreamNonBlocking));
   CUI(h->ev0.create(cudaEventDefault));
   CUI(h->ev1.create(cudaEventDefault));
+  CUI(h->ev_in.create(cudaEventDisableTiming));
+  CUI(h->ev_out.create(cudaEventDisableTiming));
+  h->dev = icp_device_new();
   *out = h.release();
   return LM_OK;
 }
@@ -793,19 +788,6 @@ extern "C" void lm_icp_destroy(lm_icp* h) {
 }
 
 namespace {
-
-struct Cloud {
-  std::vector<double> pts;    // down-sampled model cloud, xyz
-  std::vector<double> raw;    // the model cloud before down-sampling (only kept when asked for)
-  std::vector<double> scene;  // down-sampled scene cloud (only built when asked for)
-  double init[16];
-  float base[16];  // init_base, row-major
-  bool early = false;
-  bool unkeyed = false;  // a point's voxel index is not finite or beyond int64 (a zero or non-finite K)
-};
-
-// LL.cpp:34-109 for one hypothesis.
-bool voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out);
 
 // init_base = [R | t] with only t.z converted to metres (LL.cpp:34-38)
 void init_base(const float* R, const float* t, float* base) {
@@ -857,275 +839,7 @@ void model_box(const uint16_t* model, int mrows, int mcols, int* box) {
   grow_box(x0, y0, x1, y1, mrows, mcols, box);
 }
 
-void build_cloud(const uint16_t* scene, int srows, int scols, const uint16_t* model, int mrows, int mcols, const float* sK,
-                 const float* mK, const float* R, const float* t, int detectX, int detectY, bool want_scene, bool want_raw, Cloud& c) {
-  init_base(R, t, c.base);
-  const int half = 4;
-  int box[4];
-  model_box(model, mrows, mcols, box);
-  const int bx = box[0], by = box[1], bw = box[2], bh = box[3];
-  c.early = (detectX + bw >= scols) || (detectY + bh >= srows);  // LL.cpp:52-55
-  if (c.early) return;
-  // clouds (LL.cpp:57-99)
-  std::vector<double> mp, sp;
-  double cm[3] = {0, 0, 0}, cs[3] = {0, 0, 0};
-  long ncs = 0;
-  const double anchor = model[(size_t)(mrows / 2) * mcols + mcols / 2] / 1000.0;
-  auto in_mask = [&](int mr, int mc) {  // dilated mask
-    for (int dy = -half; dy <= half; ++dy) {
-      const int yy = mr + dy;
-      if (yy < 0 || yy >= mrows) continue;
-      for (int dx = -half; dx <= half; ++dx) {
-        const int xx = mc + dx;
-        if (xx >= 0 && xx < mcols && model[(size_t)yy * mcols + xx] > 0) return true;
-      }
-    }
-    return false;
-  };
-  for (int r = 0; r < bh; ++r)
-    for (int q = 0; q < bw; ++q) {
-      const int mr = r + by, mc = q + bx;
-      int sr = r + detectY - half; if (sr < 0) sr = 0;
-      int sc = q + detectX - half; if (sc < 0) sc = 0;
-      const uint16_t md = model[(size_t)mr * mcols + mc];
-      if (md == 0 && !in_mask(mr, mc)) continue;
-      if (md > 0) {
-        const double z = md / 1000.0;
-        const double x = (mc - mK[2]) / mK[0] * z;  // int - float -> float, / float, * double
-        const double y = (mr - mK[5]) / mK[4] * z;
-        mp.push_back(x); mp.push_back(y); mp.push_back(z);
-        cm[0] += x; cm[1] += y; cm[2] += z;
-      }
-      const uint16_t sd = scene[(size_t)sr * scols + sc];
-      if (sd > 0) {
-        const double z = sd / 1000.0;
-        const double x = (sc - sK[2]) / sK[0] * z;
-        const double y = (sr - sK[5]) / sK[4] * z;
-        if (want_scene) { sp.push_back(x); sp.push_back(y); sp.push_back(z); }
-        if (fabs(z - anchor) < 0.4 && md > 0) { cs[0] += x; cs[1] += y; cs[2] += z; ++ncs; }
-      }
-    }
-  const double nm = (double)(mp.size() / 3);
-  for (int k = 0; k < 3; ++k) { cm[k] /= nm; cs[k] /= (double)ncs; }  // 0/0 -> NaN as in the reference
-  for (int i = 0; i < 16; ++i) c.init[i] = (i % 5 == 0) ? 1.0 : 0.0;
-  for (int k = 0; k < 3; ++k) c.init[4 * k + 3] = cs[k] - cm[k];
-  c.unkeyed = !voxel_down_sample(mp, c.pts);
-  if (want_scene && !voxel_down_sample(sp, c.scene)) c.unkeyed = true;
-  if (want_raw) c.raw = std::move(mp);
-}
-
-// PointCloud::VoxelDownSample(0.0025) (LL.cpp:106-109): mean of the points of every occupied voxel;
-// Open3D emits them in hash-map order, here in sorted voxel order (affects summation order only).  False (out empty)
-// when a voxel index is NaN or beyond int64, which no conversion to an integer key can hold.
-bool voxel_down_sample(const std::vector<double>& mp, std::vector<double>& out) {
-  const double voxel = 0.0025;
-  const size_t n = mp.size() / 3;
-  out.clear();
-  if (n == 0) return true;
-  double mn[3] = {mp[0], mp[1], mp[2]};
-  for (size_t i = 1; i < n; ++i)
-    for (int k = 0; k < 3; ++k) mn[k] = std::min(mn[k], mp[3 * i + k]);
-  struct Key { int64_t a, b, c; size_t i; };
-  std::vector<Key> keys(n);
-  for (size_t i = 0; i < n; ++i) {
-    double v[3];
-    for (int k = 0; k < 3; ++k) {
-      v[k] = floor((mp[3 * i + k] - (mn[k] - voxel * 0.5)) / voxel);
-      if (!(v[k] >= -9223372036854775808.0 && v[k] < 9223372036854775808.0)) return false;
-    }
-    keys[i].a = (int64_t)v[0]; keys[i].b = (int64_t)v[1]; keys[i].c = (int64_t)v[2];
-    keys[i].i = i;
-  }
-  std::stable_sort(keys.begin(), keys.end(), [](const Key& p, const Key& q) {
-    if (p.a != q.a) return p.a < q.a;
-    if (p.b != q.b) return p.b < q.b;
-    return p.c < q.c;
-  });
-  for (size_t s = 0; s < n;) {
-    size_t e = s;
-    double acc[3] = {0, 0, 0};
-    while (e < n && keys[e].a == keys[s].a && keys[e].b == keys[s].b && keys[e].c == keys[s].c) {
-      for (int k = 0; k < 3; ++k) acc[k] += mp[3 * keys[e].i + k];
-      ++e;
-    }
-    for (int k = 0; k < 3; ++k) out.push_back(acc[k] / (double)(e - s));
-    s = e;
-  }
-  return true;
-}
-
 }  // namespace
-
-// Batch of hypotheses against one scene depth image.  For hypothesis h: model_depths[h] (mrows x mcols
-// u16), modelK + 9h, R + 9h, t + 3h, detect_xy[2h..2h+1].  Outputs R_out + 9h (row-major f64),
-// t_out + 3h (mm), residual[h] (fitness; -1 on the early return of LL.cpp:52-55, outputs untouched).
-extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int srows, int scols,
-                                    const uint16_t* const* model_depths, int mrows, int mcols, const float* sceneK,
-                                    const float* modelK, const float* R, const float* t, const int32_t* detect_xy,
-                                    int max_iterations, double* R_out, double* t_out, float* residual) {
-  if (!h || n_hyp < 0 || !scene_depth || !model_depths || !sceneK || !modelK || !R || !t || !detect_xy || !R_out || !t_out || !residual)
-    return lm_fail(LM_E_INVALID, "null argument");
-  if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
-  if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
-  CUI(cudaSetDevice(h->device));
-  h->verified = false;
-  h->cap.job_of.clear();  // a call that fails keeps no capture
-  const bool pso = h->estimation == LM_POSE_PSO;
-  const bool scene_cloud = h->use_scene_cloud && !pso;  // the swarm registers against no target
-  std::vector<Cloud> clouds((size_t)n_hyp);
-  std::vector<IcpJob> jobs;
-  std::vector<int> job_of((size_t)n_hyp, -1);
-  std::vector<double> all;
-  int max_count = 0;
-  for (int i = 0; i < n_hyp; ++i)
-    if (!model_depths[i]) return lm_fail(LM_E_INVALID, "model_depths[%d] is null", i);
-  {
-    // the hypotheses' clouds are independent: hypothesis 0 on this thread, the others on their own (a batch is the three
-    // NMS survivors of the drivers, linemod_and_levelup_test.py:348-367)
-    auto build = [&](int i) {
-      build_cloud(scene_depth, srows, scols, model_depths[i], mrows, mcols, sceneK, modelK + 9 * i, R + 9 * i, t + 3 * i,
-                  detect_xy[2 * i], detect_xy[2 * i + 1], scene_cloud, h->verify, clouds[i]);
-    };
-    std::vector<std::thread> workers;
-    for (int i = 1; i < n_hyp && i < 16; ++i) workers.emplace_back(build, i);
-    if (n_hyp > 0) build(0);
-    for (int i = 16; i < n_hyp; ++i) build(i);
-    for (std::thread& w : workers) w.join();
-  }
-  for (int i = 0; i < n_hyp; ++i)
-    if (clouds[i].unkeyed)
-      return lm_fail(LM_E_INVALID, "hypothesis %d: a cloud point has no voxel index (NaN or beyond int64: a zero or non-finite K?)", i);
-  for (int i = 0; i < n_hyp; ++i) {
-    if (clouds[i].early) continue;
-    IcpJob j;
-    j.src_first = (int32_t)(all.size() / 3);
-    j.src_count = (int32_t)(clouds[i].pts.size() / 3);
-    all.insert(all.end(), clouds[i].pts.begin(), clouds[i].pts.end());
-    j.tgt_first = j.src_first;  // scene_pcd_down = model_pcd->VoxelDownSample (LL.cpp:109)
-    j.tgt_count = j.src_count;
-    if (scene_cloud) {
-      j.tgt_first = (int32_t)(all.size() / 3);
-      j.tgt_count = (int32_t)(clouds[i].scene.size() / 3);
-      all.insert(all.end(), clouds[i].scene.begin(), clouds[i].scene.end());
-    }
-    memcpy(j.init, clouds[i].init, sizeof(j.init));
-    job_of[i] = (int)jobs.size();
-    jobs.push_back(j);
-    max_count = std::max(max_count, j.tgt_count);
-  }
-  const size_t npts = all.size() / 3;
-  const int64_t words = pso_record_words(h->search);
-  if (!jobs.empty()) {
-    // a pair grows together, its second array allocated last: that one's size is the pair's
-    if (npts * 3 > h->d_nrm.size()) {
-      h->d_pts.reset(); h->d_nrm.reset();
-      const size_t cap = std::max<size_t>(npts * 2, 4096) * 3;
-      CUI(h->d_pts.assign(cap));
-      CUI(h->d_nrm.assign(cap));
-    }
-    if (jobs.size() > h->d_outs.size()) {
-      h->d_jobs.reset(); h->d_outs.reset();
-      const size_t cap = std::max<size_t>(jobs.size() * 2, 16);
-      CUI(h->d_jobs.assign(cap));
-      CUI(h->d_outs.assign(cap));
-    }
-    if (jobs.size() > h->h_outs.size()) CUI(h->h_outs.assign(std::max<size_t>(jobs.size() * 2, 16)));
-    if (h->capture && npts * 2 > h->d_corr.size()) {
-      h->d_knn.reset(); h->d_corr.reset();
-      CUI(h->d_knn.assign(npts * ICP_KNN));
-      CUI(h->d_corr.assign(npts * 2));
-    }
-    int32_t* knn_out = h->capture ? h->d_knn.get() : nullptr;
-    int32_t* corr_out = h->capture ? h->d_corr.get() : nullptr;
-    cudaStream_t st = h->stream.get();
-    if (npts) CUI(cudaMemcpyAsync(h->d_pts.get(), all.data(), npts * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
-    CUI(cudaMemcpyAsync(h->d_jobs.get(), jobs.data(), jobs.size() * sizeof(IcpJob), cudaMemcpyHostToDevice, st));
-    PsoParams q;
-    if (pso) {  // one buffer: the scene, per job its hypothesis (the job number of its draws), then (capture) the records
-      const size_t npix = (size_t)srows * scols, o_hyp = (sizeof(uint16_t) * npix + 15) & ~(size_t)15;
-      const size_t o_rec = o_hyp + sizeof(int64_t) * jobs.size();
-      CUI(h->h_sbuf.reserve(o_rec));
-      uint8_t* hb = h->h_sbuf.get();
-      memcpy(hb, scene_depth, sizeof(uint16_t) * npix);
-      int64_t* hyp = reinterpret_cast<int64_t*>(hb + o_hyp);
-      for (int i = 0; i < n_hyp; ++i)
-        if (job_of[i] >= 0) hyp[(size_t)job_of[i]] = i;
-      CUI(h->d_sbuf.reserve(o_rec + (h->capture ? sizeof(long long) * words * jobs.size() : 0)));
-      uint8_t* b = h->d_sbuf.get();
-      CUI(cudaMemcpyAsync(b, hb, o_rec, cudaMemcpyHostToDevice, st));
-      memset(&q, 0, sizeof(q));
-      q.jobs = h->d_jobs.get(); q.pts = h->d_pts.get(); q.outs = h->d_outs.get(); q.n = (int32_t)jobs.size();
-      q.scene = reinterpret_cast<const uint16_t*>(b); q.srows = srows; q.scols = scols;
-      memcpy(q.sK, sceneK, sizeof(q.sK));
-      q.job = reinterpret_cast<const int64_t*>(b + o_hyp);
-      q.s = h->search;
-      q.record = h->capture ? reinterpret_cast<long long*>(b + o_rec) : nullptr; q.record_words = words;
-    }
-    CUI(cudaEventRecord(h->ev0.get(), st));
-    if (pso) {
-      int rc = launch_pso(q, st);
-      if (rc) return rc;
-    } else {
-      if (max_count > 0 && h->estimation == LM_ICP_POINT_TO_PLANE) {
-        dim3 g((unsigned)((max_count + 127) / 128), (unsigned)jobs.size());
-        k_icp_normals<<<g, 128, 0, st>>>(h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), knn_out);
-        ++h->launches;
-      }
-      launch_icp<false>(h->estimation, (unsigned)jobs.size(), st, h->d_jobs.get(), h->d_pts.get(), h->d_nrm.get(), h->d_outs.get(),
-                        max_iterations, corr_out, PoseShareDev());
-    }
-    ++h->launches;
-    CUI(cudaEventRecord(h->ev1.get(), st));
-    if (pso && h->capture) {
-      h->cap.record.resize((size_t)words * jobs.size());
-      CUI(cudaMemcpyAsync(h->cap.record.data(), q.record, sizeof(long long) * h->cap.record.size(), cudaMemcpyDeviceToHost, st));
-    }
-    CUI(cudaMemcpyAsync(h->h_outs.get(), h->d_outs.get(), jobs.size() * sizeof(IcpOut), cudaMemcpyDeviceToHost, st));
-    CUI(cudaStreamSynchronize(st));
-    CUI(cudaGetLastError());
-    float ms = 0;
-    CUI(cudaEventElapsedTime(&ms, h->ev0.get(), h->ev1.get()));
-    h->last_kernel_us = ms * 1000.f;
-  }
-  if (h->verify) {
-    std::vector<std::vector<double>> raw(jobs.size());
-    for (int i = 0; i < n_hyp; ++i)
-      if (job_of[i] >= 0) raw[(size_t)job_of[i]] = std::move(clouds[i].raw);
-    int rc = icp_verify_host(h, job_of, raw, scene_depth, srows, scols, sceneK);
-    if (rc) return rc;
-  }
-  if (h->capture) {
-    auto& c = h->cap;
-    c.estimation = h->estimation;
-    c.device = false;
-    c.jobs = jobs;
-    c.job_of = job_of;
-    c.outs.assign(h->h_outs.get(), h->h_outs.get() + (jobs.empty() ? 0 : jobs.size()));
-    c.pts = all;
-    c.nrm.assign(npts * 3, 0.0);
-    c.knn.assign(npts * ICP_KNN, -1);
-    c.corr.assign(npts * 2, -1);
-    if (npts) {
-      if (c.estimation == LM_ICP_POINT_TO_PLANE) {
-        CUI(cudaMemcpy(c.nrm.data(), h->d_nrm.get(), npts * 3 * sizeof(double), cudaMemcpyDeviceToHost));
-        CUI(cudaMemcpy(c.knn.data(), h->d_knn.get(), npts * ICP_KNN * sizeof(int32_t), cudaMemcpyDeviceToHost));
-      }
-      if (!pso) CUI(cudaMemcpy(c.corr.data(), h->d_corr.get(), npts * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    }
-    if (!pso || jobs.empty()) c.record.clear();
-    c.record_words = words;
-  }
-  for (int i = 0; i < n_hyp; ++i) {
-    if (job_of[i] < 0) { residual[i] = -1.f; continue; }
-    const IcpOut& o = h->h_outs[job_of[i]];
-    compose(o.T, clouds[i].base, R_out + 9 * i, t_out + 3 * i);
-    residual[i] = (float)o.fitness;
-    h->last_points = jobs[job_of[i]].src_count;
-    h->last_iterations = o.iterations;
-    h->last_rmse = o.rmse;
-  }
-  return LM_OK;
-}
 
 extern "C" int lm_icp_process(lm_icp* h, const uint16_t* scene_depth, int srows, int scols, const uint16_t* model_depth, int mrows,
                               int mcols, const float* sceneK, const float* modelK, const float* R, const float* t, int detectX,
@@ -1136,9 +850,8 @@ extern "C" int lm_icp_process(lm_icp* h, const uint16_t* scene_depth, int srows,
                               t_out, residual);
 }
 
-// [0] points in the down-sampled cloud, [1] ICP iterations, [2] inlier rmse (m), [3] device time of the
-// normals + ICP kernels (point-to-point: the ICP kernel alone) of the last call in microseconds -- all of the LAST
-// hypothesis processed.
+// [0] points in the down-sampled cloud, [1] ICP iterations, [2] inlier rmse (m) -- of the LAST hypothesis with a pose --
+// and [3] device time of the last call in microseconds (include/linemod_b200.h).
 extern "C" int lm_icp_last_stats(lm_icp* h, double* out4) {
   if (!h || !out4) return lm_fail(LM_E_INVALID, "null argument");
   out4[0] = h->last_points; out4[1] = h->last_iterations; out4[2] = h->last_rmse; out4[3] = h->last_kernel_us;
@@ -1207,11 +920,8 @@ extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t c
     return lm_fail(LM_E_STATE, "capture item %d: the particle swarm computes no normals, neighbour lists or correspondences", what);
   if ((what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN) && c.estimation != LM_ICP_POINT_TO_PLANE)
     return lm_fail(LM_E_STATE, "capture item %d: the point-to-point estimation computes no normals or neighbour lists", what);
-  if (what == LM_ICP_CAPTURE_SEARCH && (c.estimation != LM_POSE_PSO || c.device))
-    return lm_fail(LM_E_STATE, "capture item %d: only an LM_POSE_PSO call of lm_icp_process_batch keeps swarm records", what);
-  if (c.device && (what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN || what == LM_ICP_CAPTURE_CORR_FIRST ||
-                   what == LM_ICP_CAPTURE_CORR_LAST))
-    return lm_fail(LM_E_STATE, "capture item %d: lm_icp_process_batch_device keeps no normals, neighbour lists or correspondences", what);
+  if (what == LM_ICP_CAPTURE_SEARCH && c.estimation != LM_POSE_PSO)
+    return lm_fail(LM_E_STATE, "capture item %d: only an LM_POSE_PSO call keeps swarm records", what);
   switch (what) {
     case LM_ICP_CAPTURE_COUNTS:
       tmp = {j.src_count, j.tgt_count};
@@ -1259,12 +969,12 @@ extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t c
 }
 
 // --------------------------------------------------------------------------------------------
-// pose stage on the device (lm_pose.h): build_cloud + voxel_down_sample for the NMS survivors
+// pose stage on the device (lm_pose.h): clouds, initial guesses and the ICP for the NMS survivors or a call's hypotheses
 // --------------------------------------------------------------------------------------------
-// Exactness: every float / double operation that build_cloud and voxel_down_sample do is written with an _rn
-// intrinsic (no FMA contraction), points are compacted with block scans in the host's row-major order, the centroids
-// are summed by one thread each in that order, and the voxel keys are sorted stably, so clouds and initial guesses are
-// bit-identical to the host's.
+// Exactness: every float / double operation of LL.cpp:34-109 is written with an _rn intrinsic (no FMA contraction),
+// points are compacted with block scans in row-major order, the centroids are summed by one thread each in that order,
+// and the voxel keys are sorted stably, so clouds and initial guesses are bit-identical to a sequential float64 build
+// (tests/pose_cloud_model.py).
 #define POSE_THREADS 512
 #define POSE_KEY_BITS 21  // per voxel coordinate: 2^21 voxels of 2.5 mm = 5.2 km of cloud extent
 #define POSE_FIRST_FETCH 16
@@ -1424,7 +1134,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
     __syncthreads();
   }
   if (tid < 6) {
-    // centroids: one thread per sum, in the host's sequential order (LL.cpp:71-104)
+    // centroids: one thread per sum, in the reference's sequential order (LL.cpp:71-104)
     const double* P = tid < 3 ? M : Cs;
     const int n = tid < 3 ? nm : nc;
     double s = 0.0;
@@ -1455,7 +1165,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
   if (tid == 0) {
     for (int k = 0; k < 16; ++k) job->init[k] = (k % 5 == 0) ? 1.0 : 0.0;
     for (int c = 0; c < 3; ++c) {
-      const double cm = __ddiv_rn(s_sum[c], (double)nm), cs = __ddiv_rn(s_sum[3 + c], (double)nc);  // 0/0 -> NaN as the host
+      const double cm = __ddiv_rn(s_sum[c], (double)nm), cs = __ddiv_rn(s_sum[3 + c], (double)nc);  // 0/0 -> NaN as the reference
       job->init[4 * c + 3] = __dsub_rn(cs, cm);
     }
     job->src_first = job->tgt_first = (int32_t)sm;
@@ -1465,7 +1175,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_pose_cloud(PoseParams p) {
   }
 }
 
-// One CTA per cloud slot: mean of every occupied voxel, summed in sorted order (voxel_down_sample).
+// One CTA per cloud slot: mean of every occupied voxel, summed in sorted voxel order (PointCloud::VoxelDownSample).
 __global__ void __launch_bounds__(POSE_THREADS) k_pose_voxel(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ vals,
                                                              const int32_t* __restrict__ seg_begin, const int32_t* __restrict__ seg_end,
                                                              const double* __restrict__ raw, double* __restrict__ pts, IcpJob* jobs,
@@ -1606,60 +1316,6 @@ __global__ void __launch_bounds__(VERIFY_THREADS) k_pose_verify(PoseParams p, co
 }
 
 static bool verify_delta_ok(double inlier_mm) { return std::isfinite(inlier_mm) && inlier_mm >= 0.0; }
-
-// lm_icp_process_batch's verification: job j's raw model cloud raw[j] (uploaded with the scene) moved by the ICP's output
-// h->d_outs[j], one k_pose_verify launch over the jobs; then h->ver per hypothesis (score -1 on the early return).
-static int icp_verify_host(lm_icp* h, const std::vector<int>& job_of, const std::vector<std::vector<double>>& raw,
-                           const uint16_t* scene, int srows, int scols, const float* sK) {
-  const size_t J = raw.size(), npix = (size_t)srows * scols;
-  h->ver.assign(job_of.size(), PoseVerify());
-  for (PoseVerify& v : h->ver) v.score = -1.f;
-  if (J) {
-    // one buffer: scene, segments [4J] (slot j's begin at 2j, its end at 2J + 2j), posed flags [J], points, results [J]
-    size_t npts = 0;
-    for (const auto& r : raw) npts += r.size() / 3;
-    if (npts > 0x7FFFFFFFu) return lm_fail(LM_E_CAPACITY, "%zu model points to verify, at most 2^31 - 1", npts);
-    auto a16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
-    const size_t o_seg = a16(sizeof(uint16_t) * npix), o_posed = a16(o_seg + sizeof(int32_t) * 4 * J);
-    const size_t o_pts = a16(o_posed + J), o_ver = a16(o_pts + sizeof(double) * 3 * npts);
-    std::vector<uint8_t> in(o_ver);
-    memcpy(in.data(), scene, sizeof(uint16_t) * npix);
-    int32_t* seg = reinterpret_cast<int32_t*>(in.data() + o_seg);
-    double* pts = reinterpret_cast<double*>(in.data() + o_pts);
-    size_t at = 0;
-    for (size_t j = 0; j < J; ++j) {
-      seg[2 * j] = (int32_t)at;
-      memcpy(pts + 3 * at, raw[j].data(), sizeof(double) * raw[j].size());
-      at += raw[j].size() / 3;
-      seg[2 * J + 2 * j] = (int32_t)at;
-      in[o_posed + j] = 1;
-    }
-    CUI(h->d_vbuf.reserve(o_ver + sizeof(PoseVerify) * J));
-    cudaStream_t st = h->stream.get();
-    uint8_t* b = h->d_vbuf.get();
-    CUI(cudaMemcpyAsync(b, in.data(), in.size(), cudaMemcpyHostToDevice, st));
-    PoseParams p;
-    memset(&p, 0, sizeof(p));
-    p.scene = reinterpret_cast<const uint16_t*>(b);
-    p.srows = srows; p.scols = scols;
-    memcpy(p.sK, sK, sizeof(p.sK));
-    p.raw = reinterpret_cast<double*>(b + o_pts);
-    p.seg_begin = reinterpret_cast<int32_t*>(b + o_seg); p.seg_end = p.seg_begin + 2 * J;
-    p.posed = b + o_posed;
-    p.rank = 0; p.world = 1;
-    k_pose_verify<false><<<(unsigned)J, VERIFY_THREADS, 0, st>>>(p, h->d_outs.get(), h->verify_mm, reinterpret_cast<PoseVerify*>(b + o_ver),
-                                                                 PoseShareDev());
-    CUI(cudaGetLastError());
-    ++h->launches;
-    std::vector<PoseVerify> out(J);
-    CUI(cudaMemcpyAsync(out.data(), b + o_ver, sizeof(PoseVerify) * J, cudaMemcpyDeviceToHost, st));
-    CUI(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < job_of.size(); ++i)
-      if (job_of[i] >= 0) h->ver[i] = out[(size_t)job_of[i]];
-  }
-  h->verified = true;
-  return LM_OK;
-}
 
 // --------------------------------------------------------------------------------------------
 // LM_POSE_PSO (include/linemod_b200.h): a particle swarm over rotations about the cloud's centroid and translations,
@@ -2366,6 +2022,12 @@ struct PoseChunk {
   PoseVerify* ver;  // o.verify.on: per survivor its verification
   int32_t* status;
   int32_t seq;
+  // capture (unshared chunks; null: none): k_icp_normals' neighbour lists and the ICP kernel's correspondences, indexed
+  // as the stage's points, and k_pose_pso's swarm records, record_words per slot
+  int32_t* knn_out = nullptr;
+  int32_t* corr_out = nullptr;
+  long long* record = nullptr;
+  int64_t record_words = 0;
 };
 
 // k_pose_cloud, the segmented sort, k_pose_voxel, k_icp_normals (point-to-plane only) and the ICP kernel (or k_pose_pso,
@@ -2402,11 +2064,11 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
                                                3 * POSE_KEY_BITS, st));
   k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw.get(), s->d_pts.get(), s->d_jobs.get(),
                                                p.use_scene);
-  // the ICP kernels of lm_icp_process_batch: empty jobs fall through
+  // the ICP kernels: empty jobs fall through
   const bool normals = o.estimation == LM_ICP_POINT_TO_PLANE;
   if (normals) {
     dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
-    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), nullptr);
+    k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.knn_out);
   }
   if (sh) {
     // the results travel to every rank; the collector gathers the chunk in survivor order
@@ -2428,10 +2090,12 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
       memcpy(q.sK, p.sK, sizeof(q.sK));
       q.frame_of = c.frame_of; q.sKs = c.sKs; q.frame_first = c.frame_first; q.first = c.first;
       q.s = o.search;
+      q.record = c.record; q.record_words = c.record_words;
       const int rc = launch_pso(q, st);
       if (rc) return rc;
     } else {
-      launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.outs, o.max_iterations, nullptr, PoseShareDev());
+      launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.outs, o.max_iterations, c.corr_out,
+                        PoseShareDev());
     }
     if (o.verify.on) k_pose_verify<false><<<n, VERIFY_THREADS, 0, st>>>(p, c.outs, o.verify.inlier_mm, c.ver, PoseShareDev());
   }
@@ -2979,7 +2643,7 @@ __global__ void __launch_bounds__(ICP_DEV_PX) k_icp_render_crop(const RenderSrc*
 
 struct IcpDevice {
   lm_pose_stage stage;  // the chunks' cloud buffers (pose_buffers); no registered render
-  Event ev_in, ev_out;  // the caller's stream -> the reads -> the caller's stream
+  PinnedArray<uint16_t> h_planes; DeviceArray<uint16_t> planes;  // lm_icp_process_batch: the scene, then each distinct render
   DeviceArray<uint8_t> in;  // the call's inputs in one copy: renders, K, survivors, chunk sizes, class_begin
   DeviceArray<uint16_t> scene, crops;
   DeviceArray<uint32_t> ext; PinnedArray<uint32_t> h_ext;  // [n][4] extents (k_icp_render_box)
@@ -2988,8 +2652,10 @@ struct IcpDevice {
   DeviceArray<int32_t> status; PinnedArray<int32_t> h_status;  // 4 per chunk (PoseChunk); the host's copy then holds the
                                                                // source count of the last hypothesis with a pose
   DeviceArray<PoseVerify> ver; PinnedArray<PoseVerify> h_ver;  // lm_icp_set_verify: per hypothesis
+  DeviceArray<int32_t> knn, corr; DeviceArray<long long> record;  // lm_icp_set_capture: the chunk's (PoseChunk)
 };
 
+static IcpDevice* icp_device_new() { return new IcpDevice(); }
 static void icp_device_free(IcpDevice* d) { delete d; }
 
 // A device depth plane's format and scale.
@@ -3003,71 +2669,54 @@ static int check_depth_format(const char* what, int format, float scale) {
 
 static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
-extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, int64_t scene_pitch, int scene_format,
-                                           float scene_scale, int srows, int scols, const void* const* model_depths,
-                                           const int64_t* model_pitches, int model_format, float model_scale, int mrows, int mcols,
-                                           const float* sceneK, const float* modelK, const float* R, const float* t,
-                                           const int32_t* detect_xy, int max_iterations, double* R_out, double* t_out, float* residual,
-                                           void* stream) {
-  if (!h || n_hyp < 0 || !scene_depth || !model_depths || !model_pitches || !sceneK || !modelK || !R || !t || !detect_xy || !R_out ||
-      !t_out || !residual)
-    return lm_fail(LM_E_INVALID, "null argument");
-  if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
-  if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
-  int rc = check_depth_format("scene_depth", scene_format, scene_scale);
-  if (!rc) rc = check_depth_format("model_depths", model_format, model_scale);
-  if (rc) return rc;
-  cudaStream_t caller = (cudaStream_t)stream;
-  rc = check_device_stream(h->device, caller);
-  const int sz = scene_format == LM_DEPTH_F32 ? 4 : 2, mz = model_format == LM_DEPTH_F32 ? 4 : 2;
-  if (!rc) rc = check_device_plane(h->device, "scene_depth", scene_depth, scene_pitch, (int64_t)sz * scols, sz);
-  for (int i = 0; i < n_hyp && !rc; ++i) {
-    char what[40];
-    snprintf(what, sizeof(what), "model_depths[%d]", i);
-    rc = check_device_plane(h->device, what, model_depths[i], model_pitches[i], (int64_t)mz * mcols, mz);
-  }
-  if (rc) return rc;
+// A call without hypotheses: no device work; it verified nothing (an empty verification) and captured nothing.
+static int icp_no_hypotheses(lm_icp* h) {
+  h->ver.clear();
+  h->verified = h->verify;
+  h->cap.job_of.clear();
+  return LM_OK;
+}
+
+// lm_icp_process_batch and lm_icp_process_batch_device past their checks: n >= 1 hypotheses, the scene and renders[i] in
+// device memory as lm_icp_process_batch_device takes them, on the handle's stream behind the caller's ev0.  Returns once
+// the outputs are on the host.
+static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pitch, int scene_format, float scene_scale, int srows,
+                     int scols, const RenderSrc* renders, int model_format, float model_scale, int mrows, int mcols,
+                     const float* sceneK, const float* modelK, const float* R, const float* t, const int32_t* detect_xy,
+                     int max_iterations, double* R_out, double* t_out, float* residual) {
   h->verified = false;
-  // capture: what each posed hypothesis's chunk built, copied out behind the chunk; kept only when the call succeeds
+  h->cap.job_of.clear();  // a call that fails keeps no capture
+  IcpDevice& d = *h->dev;
+  cudaStream_t st = h->stream.get();
+  const bool pso = h->estimation == LM_POSE_PSO, normals = h->estimation == LM_ICP_POINT_TO_PLANE;
+  const int64_t words = pso_record_words(h->search);
+  // capture: what each posed hypothesis's chunk built and kept, copied out behind the chunk; kept only when the call succeeds
   std::vector<IcpJob> cjobs;
-  std::vector<int> cjob_of((size_t)n_hyp, -1);
-  std::vector<double> cpts;
+  std::vector<int> cjob_of((size_t)n, -1);
+  std::vector<double> cpts, cnrm;
+  std::vector<int32_t> cknn, ccorr;
+  std::vector<long long> crec;
   auto keep_capture = [&](const IcpOut* outs) {
     auto& c = h->cap;
     c.estimation = h->estimation;
-    c.device = true;
-    c.jobs = cjobs;
-    c.job_of = cjob_of;
+    c.jobs = std::move(cjobs);
+    c.job_of = std::move(cjob_of);
     c.outs.clear();
-    for (int i = 0; i < n_hyp; ++i)
-      if (cjob_of[(size_t)i] >= 0) c.outs.push_back(outs[i]);
-    c.pts = cpts;
-    c.nrm.clear(); c.knn.clear(); c.corr.clear();
+    for (int i = 0; i < n; ++i)
+      if (c.job_of[(size_t)i] >= 0) c.outs.push_back(outs[i]);
+    c.pts = std::move(cpts); c.nrm = std::move(cnrm);
+    c.knn = std::move(cknn); c.corr = std::move(ccorr);
+    c.record = std::move(crec); c.record_words = words;
   };
-  if (h->capture) h->cap.job_of.clear();
-  if (n_hyp == 0) {
-    h->ver.clear();
-    h->verified = h->verify;
-    if (h->capture) keep_capture(nullptr);
-    return LM_OK;
-  }
-  CUI(cudaSetDevice(h->device));
-  if (!h->dev) h->dev = new IcpDevice();
-  IcpDevice& d = *h->dev;
-  if (!d.ev_in.get()) CUI(d.ev_in.create(cudaEventDisableTiming));
-  if (!d.ev_out.get()) CUI(d.ev_out.create(cudaEventDisableTiming));
-  const int n = n_hyp, nc = pose_batch_chunks(n);
+  const int nc = pose_batch_chunks(n);
   // the inputs: survivor i is hypothesis i (class 0, template i) at detect_xy[i]; chunk c holds min(n - 1024 c, 1024)
   const size_t o_K = align16(sizeof(RenderSrc) * n), o_surv = align16(o_K + sizeof(float) * 9 * n);
   const size_t o_cnt = align16(o_surv + sizeof(lm_match) * n), o_cb = align16(o_cnt + sizeof(int32_t) * nc);
   std::vector<uint8_t> in(o_cb + 2 * sizeof(int32_t));
-  RenderSrc* src = reinterpret_cast<RenderSrc*>(in.data());
   lm_match* surv = reinterpret_cast<lm_match*>(in.data() + o_surv);
   int32_t* cnt = reinterpret_cast<int32_t*>(in.data() + o_cnt);
-  for (int i = 0; i < n; ++i) {
-    src[i] = {static_cast<const uint8_t*>(model_depths[i]), model_pitches[i]};
-    surv[i] = {detect_xy[2 * i], detect_xy[2 * i + 1], 0.f, 0, i};
-  }
+  memcpy(in.data(), renders, sizeof(RenderSrc) * n);
+  for (int i = 0; i < n; ++i) surv[i] = {detect_xy[2 * i], detect_xy[2 * i + 1], 0.f, 0, i};
   memcpy(in.data() + o_K, modelK, sizeof(float) * 9 * n);
   for (int c = 0; c < nc; ++c) cnt[c] = std::min(n - c * POSE_CHUNK, POSE_CHUNK);
   const int32_t class_begin[2] = {0, n};
@@ -3083,11 +2732,6 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   const RenderSrc* d_src = reinterpret_cast<const RenderSrc*>(d.in.get());
   const float* d_K = reinterpret_cast<const float*>(d.in.get() + o_K);
   const int f32 = model_format == LM_DEPTH_F32 ? 1 : 0;
-  // the reads of the caller's planes start behind its stream's work
-  cudaStream_t st = h->stream.get();
-  CUI(cudaEventRecord(d.ev_in.get(), caller));
-  CUI(cudaStreamWaitEvent(st, d.ev_in.get(), 0));
-  CUI(cudaEventRecord(h->ev0.get(), st));
   CUI(cudaMemcpyAsync(d.in.get(), in.data(), in.size(), cudaMemcpyHostToDevice, st));
   CUI(cudaMemsetAsync(d.ext.get(), 0xFF, sizeof(uint32_t) * 4 * n, st));
   k_icp_scene<<<dim3((unsigned)((scols + ICP_DEV_PX - 1) / ICP_DEV_PX), (unsigned)srows), ICP_DEV_PX, 0, st>>>(
@@ -3114,18 +2758,6 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     max_bh = std::max(max_bh, b[3]);
     last = i;
   }
-  if (last >= 0) {
-    CUI(d.crops.reserve((size_t)n * stride));
-    rc = pose_buffers(&d.stage, st, std::min(n, POSE_CHUNK), stride);
-    if (rc) return rc;
-    k_icp_render_crop<<<dim3((unsigned)n, (unsigned)((max_bh + RENDER_CROP_ROWS - 1) / RENDER_CROP_ROWS)), ICP_DEV_PX, 0, st>>>(
-        d_src, f32, model_scale, mrows, mcols, d.ext.get(), d_K, stride, d.tpl.get(), d.crops.get());
-    CUI(cudaGetLastError());
-    ++h->launches;
-  }
-  // the crops were the last reads of the caller's planes
-  CUI(cudaEventRecord(d.ev_out.get(), st));
-  CUI(cudaStreamWaitEvent(caller, d.ev_out.get(), 0));
   if (last < 0) {  // every hypothesis takes the early return: no cloud to build
     for (int i = 0; i < n; ++i) residual[i] = -1.f;
     if (h->verify) {
@@ -3136,6 +2768,19 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     if (h->capture) keep_capture(nullptr);
     return LM_OK;
   }
+  CUI(d.crops.reserve((size_t)n * stride));
+  int rc = pose_buffers(&d.stage, st, std::min(n, POSE_CHUNK), stride);
+  if (rc) return rc;
+  if (h->capture) {  // the chunks' capture outputs, indexed as the stage's points and slots
+    const size_t points = 2 * (size_t)pose_slots(&d.stage) * (size_t)pose_area(&d.stage);
+    if (normals) CUI(d.knn.reserve(points * ICP_KNN));
+    if (!pso) CUI(d.corr.reserve(points * 2));
+    if (pso) CUI(d.record.reserve((size_t)pose_slots(&d.stage) * words));
+  }
+  k_icp_render_crop<<<dim3((unsigned)n, (unsigned)((max_bh + RENDER_CROP_ROWS - 1) / RENDER_CROP_ROWS)), ICP_DEV_PX, 0, st>>>(
+      d_src, f32, model_scale, mrows, mcols, d.ext.get(), d_K, stride, d.tpl.get(), d.crops.get());
+  CUI(cudaGetLastError());
+  ++h->launches;
   CUI(cudaMemsetAsync(d.status.get(), 0, sizeof(int32_t) * 4 * nc, st));
   PoseOptions o;
   o.srows = srows; o.scols = scols; o.use_scene_cloud = h->use_scene_cloud ? 1 : 0; o.max_iterations = max_iterations;
@@ -3153,19 +2798,33 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
     k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK; k.frame_first = nullptr;
     k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.ver = h->verify ? d.ver.get() + c0 : nullptr;
     k.status = d.status.get() + 4 * c; k.seq = 0;
+    if (h->capture) {
+      k.knn_out = d.knn.get(); k.corr_out = d.corr.get();
+      k.record = d.record.get(); k.record_words = words;
+    }
     const int l = pose_chunk(&d.stage, o, k);
     if (l < 0) return l;
     h->launches += l;
     if (last >= c0 && last < c0 + cnt[c])  // the chunk's jobs are overwritten by the next chunk's
       CUI(cudaMemcpyAsync(d.h_status.get() + 4 * nc, &d.stage.d_jobs.get()[last - c0].src_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (h->capture) {  // the chunk's jobs and clouds, before the next chunk reuses the buffers
+    if (h->capture) {  // the chunk's jobs, clouds and kernel outputs, before the next chunk reuses the buffers
       CUI(cudaStreamSynchronize(st));
       std::vector<IcpJob> jobs((size_t)cnt[c]);
       CUI(cudaMemcpy(jobs.data(), d.stage.d_jobs.get(), sizeof(IcpJob) * jobs.size(), cudaMemcpyDeviceToHost));
-      auto append = [&](int32_t first, int32_t count) {  // points [first, first + count) of the stage's clouds -> cpts
-        const size_t at = cpts.size();
-        cpts.resize(at + (size_t)count * 3);
-        if (count) CUI(cudaMemcpy(cpts.data() + at, d.stage.d_pts.get() + (size_t)first * 3, sizeof(double) * 3 * count, cudaMemcpyDeviceToHost));
+      // points [first, first + count) of the stage's clouds, with their normals, neighbour lists and correspondences
+      auto append = [&](int32_t first, int32_t count) {
+        const size_t at = cpts.size() / 3, m = (size_t)count;
+        cpts.resize(3 * (at + m));
+        if (normals) { cnrm.resize(3 * (at + m)); cknn.resize(ICP_KNN * (at + m)); }
+        if (!pso) ccorr.resize(2 * (at + m));
+        if (!m) return LM_OK;
+        CUI(cudaMemcpy(cpts.data() + 3 * at, d.stage.d_pts.get() + 3 * (size_t)first, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
+        if (normals) {
+          CUI(cudaMemcpy(cnrm.data() + 3 * at, d.stage.d_nrm.get() + 3 * (size_t)first, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
+          CUI(cudaMemcpy(cknn.data() + ICP_KNN * at, d.knn.get() + ICP_KNN * (size_t)first, sizeof(int32_t) * ICP_KNN * m,
+                         cudaMemcpyDeviceToHost));
+        }
+        if (!pso) CUI(cudaMemcpy(ccorr.data() + 2 * at, d.corr.get() + 2 * (size_t)first, sizeof(int32_t) * 2 * m, cudaMemcpyDeviceToHost));
         return LM_OK;
       };
       for (int i = 0; i < cnt[c]; ++i) {
@@ -3183,6 +2842,11 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
         }
         if (rc) return rc;
         j.src_first = src_at;
+        if (pso) {
+          crec.resize(crec.size() + (size_t)words);
+          CUI(cudaMemcpy(crec.data() + crec.size() - words, d.record.get() + (size_t)i * words, sizeof(long long) * words,
+                         cudaMemcpyDeviceToHost));
+        }
         cjob_of[(size_t)(c0 + i)] = (int)cjobs.size();
         cjobs.push_back(j);
       }
@@ -3217,4 +2881,80 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   h->last_iterations = d.h_outs[(size_t)last].iterations;
   h->last_rmse = d.h_outs[(size_t)last].rmse;
   return LM_OK;
+}
+
+// Batch of hypotheses against one scene depth image.  For hypothesis h: model_depths[h] (mrows x mcols
+// u16), modelK + 9h, R + 9h, t + 3h, detect_xy[2h..2h+1].  Outputs R_out + 9h (row-major f64),
+// t_out + 3h (mm), residual[h] (fitness; -1 on the early return of LL.cpp:52-55, outputs untouched).
+extern "C" int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int srows, int scols,
+                                    const uint16_t* const* model_depths, int mrows, int mcols, const float* sceneK,
+                                    const float* modelK, const float* R, const float* t, const int32_t* detect_xy,
+                                    int max_iterations, double* R_out, double* t_out, float* residual) {
+  if (!h || n_hyp < 0 || !scene_depth || !model_depths || !sceneK || !modelK || !R || !t || !detect_xy || !R_out || !t_out || !residual)
+    return lm_fail(LM_E_INVALID, "null argument");
+  if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
+  if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
+  for (int i = 0; i < n_hyp; ++i)
+    if (!model_depths[i]) return lm_fail(LM_E_INVALID, "model_depths[%d] is null", i);
+  if (n_hyp == 0) return icp_no_hypotheses(h);
+  CUI(cudaSetDevice(h->device));
+  // the scene, then each distinct render once (callers repeat one render for many hypotheses), staged and copied in one
+  const size_t npix = (size_t)srows * scols, mpix = (size_t)mrows * mcols;
+  std::unordered_map<const uint16_t*, size_t> plane_of;
+  std::vector<size_t> at((size_t)n_hyp);
+  for (int i = 0; i < n_hyp; ++i)
+    at[(size_t)i] = plane_of.emplace(model_depths[i], npix + mpix * plane_of.size()).first->second;
+  const size_t total = npix + mpix * plane_of.size();
+  IcpDevice& d = *h->dev;
+  CUI(d.h_planes.reserve(total));
+  CUI(d.planes.reserve(total));
+  memcpy(d.h_planes.get(), scene_depth, sizeof(uint16_t) * npix);
+  for (const auto& p : plane_of) memcpy(d.h_planes.get() + p.second, p.first, sizeof(uint16_t) * mpix);
+  std::vector<RenderSrc> src((size_t)n_hyp);
+  for (int i = 0; i < n_hyp; ++i) src[(size_t)i] = {reinterpret_cast<const uint8_t*>(d.planes.get() + at[(size_t)i]), 2 * (int64_t)mcols};
+  cudaStream_t st = h->stream.get();
+  CUI(cudaEventRecord(h->ev0.get(), st));
+  CUI(cudaMemcpyAsync(d.planes.get(), d.h_planes.get(), sizeof(uint16_t) * total, cudaMemcpyHostToDevice, st));
+  return icp_batch(h, n_hyp, d.planes.get(), 2 * (int64_t)scols, LM_DEPTH_U16_MM, 1.f, srows, scols, src.data(), LM_DEPTH_U16_MM, 1.f,
+                   mrows, mcols, sceneK, modelK, R, t, detect_xy, max_iterations, R_out, t_out, residual);
+}
+
+extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, int64_t scene_pitch, int scene_format,
+                                           float scene_scale, int srows, int scols, const void* const* model_depths,
+                                           const int64_t* model_pitches, int model_format, float model_scale, int mrows, int mcols,
+                                           const float* sceneK, const float* modelK, const float* R, const float* t,
+                                           const int32_t* detect_xy, int max_iterations, double* R_out, double* t_out, float* residual,
+                                           void* stream) {
+  if (!h || n_hyp < 0 || !scene_depth || !model_depths || !model_pitches || !sceneK || !modelK || !R || !t || !detect_xy || !R_out ||
+      !t_out || !residual)
+    return lm_fail(LM_E_INVALID, "null argument");
+  if (srows <= 0 || scols <= 0 || mrows <= 0 || mcols <= 0) return lm_fail(LM_E_INVALID, "empty image");
+  if (max_iterations < 0) return lm_fail(LM_E_INVALID, "max_iterations < 0");
+  int rc = check_depth_format("scene_depth", scene_format, scene_scale);
+  if (!rc) rc = check_depth_format("model_depths", model_format, model_scale);
+  if (rc) return rc;
+  cudaStream_t caller = (cudaStream_t)stream;
+  rc = check_device_stream(h->device, caller);
+  const int sz = scene_format == LM_DEPTH_F32 ? 4 : 2, mz = model_format == LM_DEPTH_F32 ? 4 : 2;
+  if (!rc) rc = check_device_plane(h->device, "scene_depth", scene_depth, scene_pitch, (int64_t)sz * scols, sz);
+  for (int i = 0; i < n_hyp && !rc; ++i) {
+    char what[40];
+    snprintf(what, sizeof(what), "model_depths[%d]", i);
+    rc = check_device_plane(h->device, what, model_depths[i], model_pitches[i], (int64_t)mz * mcols, mz);
+  }
+  if (rc) return rc;
+  if (n_hyp == 0) return icp_no_hypotheses(h);
+  std::vector<RenderSrc> src((size_t)n_hyp);
+  for (int i = 0; i < n_hyp; ++i) src[(size_t)i] = {static_cast<const uint8_t*>(model_depths[i]), model_pitches[i]};
+  CUI(cudaSetDevice(h->device));
+  // the reads of the caller's planes start behind its stream's work, and its later work waits for the call's
+  cudaStream_t st = h->stream.get();
+  CUI(cudaEventRecord(h->ev_in.get(), caller));
+  CUI(cudaStreamWaitEvent(st, h->ev_in.get(), 0));
+  CUI(cudaEventRecord(h->ev0.get(), st));
+  rc = icp_batch(h, n_hyp, scene_depth, scene_pitch, scene_format, scene_scale, srows, scols, src.data(), model_format, model_scale,
+                 mrows, mcols, sceneK, modelK, R, t, detect_xy, max_iterations, R_out, t_out, residual);
+  CUI(cudaEventRecord(h->ev_out.get(), st));
+  CUI(cudaStreamWaitEvent(caller, h->ev_out.get(), 0));
+  return rc;
 }

@@ -6,7 +6,8 @@ the early return of LL.cpp:52-55.
 
 process() and refine_matches() also take depths already in device memory: the scene and the renders as CUDA tensors
 (uint16 mm, or float32 scaled by depth_scale / render_scale), read in order on `stream` (lm_icp_process_batch_device).
-The results are bit for bit those of the same call on the converted uint16 numpy images."""
+Numpy images are copied to the device and run the same kernels (lm_icp_process_batch), so the results are bit for bit
+those of the same call on the converted uint16 numpy images."""
 import numpy as np
 
 from . import _lib

@@ -282,9 +282,8 @@ int lm_match_top(lm_detector* d, const uint8_t* const* quantized, const int* row
  * the device.  Per frame the device builds the clouds (scan-compacted in row-major order), the centroids and the
  * voxel down-sampling (CUB segmented radix sort + voxel means) and runs the ICP kernels; only the survivors and their
  * poses come back.  Clouds, initial guesses, R, t and residual are bit-identical to lm_icp_process_batch on the same
- * survivors and renders, NaN patterns included (lm_debug_pose_clouds shows the clouds), except where a cloud spans more
- * than 2^21 voxels of 2.5 mm along an axis (a tiny, zero or non-finite K): the device then fails the frame with
- * LM_E_INVALID, while lm_icp_process_batch fails only where a voxel index is NaN or beyond int64 (a zero or non-finite K).
+ * survivors and renders, NaN patterns included (lm_debug_pose_clouds shows the clouds); both fail with LM_E_INVALID where
+ * a cloud spans more than 2^21 voxels of 2.5 mm along an axis (a tiny, zero or non-finite K).
  *   lm_set_template_renders  templates [first, first+n) of the bank (bank order, as lm_set_boxes); depths[i] is
  *                            rows x cols u16 mm, K + 9i / R + 9i row-major f32, t + 3i f32 mm.  May be called in
  *                            several ranges.  LM_E_INVALID for a render without a non-zero pixel or a range outside
@@ -701,9 +700,10 @@ int lm_icp_process(lm_icp* h, const uint16_t* scene_depth, int srows, int scols,
                    int mcols, const float* sceneK, const float* modelK, const float* R, const float* t, int detectX,
                    int detectY, int max_iterations, double* R_out, double* t_out, float* residual);
 
-/* The same for n hypotheses against one scene image in one launch (what the callers do for the top
- * matches after NMS, linemod_and_levelup_test.py:351-367): model_depths[i], modelK + 9i, R + 9i,
- * t + 3i, detect_xy[2i..2i+1]; outputs R_out + 9i, t_out + 3i, residual[i]. */
+/* The same for n hypotheses against one scene image (what the callers do for the top matches after NMS,
+ * linemod_and_levelup_test.py:351-367): model_depths[i], modelK + 9i, R + 9i, t + 3i, detect_xy[2i..2i+1]; outputs
+ * R_out + 9i, t_out + 3i, residual[i].  The scene and each distinct model_depths[i] (pointers may repeat) are copied to
+ * the device once, then the call is lm_icp_process_batch_device's on those u16 planes; see there. */
 int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int srows, int scols,
                          const uint16_t* const* model_depths, int mrows, int mcols, const float* sceneK, const float* modelK,
                          const float* R, const float* t, const int32_t* detect_xy, int max_iterations, double* R_out,
@@ -711,7 +711,7 @@ int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int 
 
 /* lm_icp_process_batch for a scene and renders already in device memory (a GPU decoder's depth, a depth network's, a GPU
  * renderer's output): the clouds are built on the device by the pose stage's kernels (k_pose_cloud, a segmented sort,
- * k_pose_voxel), fed by k_icp_scene, k_icp_render_box and k_icp_render_crop, then the same ICP kernels run.
+ * k_pose_voxel), fed by k_icp_scene, k_icp_render_box and k_icp_render_crop, then the ICP kernels run.
  *   Inputs     scene_depth srows x scols, rows scene_pitch BYTES apart; model_depths[i] mrows x mcols, rows
  *              model_pitches[i] bytes apart (pointers may repeat; crop views are fine).  Pixels packed within a row; every
  *              plane is device or managed memory of the handle's device.  scene_format / model_format: LM_DEPTH_U16_MM
@@ -720,21 +720,22 @@ int lm_icp_process_batch(lm_icp* h, int n_hyp, const uint16_t* scene_depth, int 
  *              in lm_icp_process_batch.
  *   Semantics  R_out, t_out and residual are bit for bit lm_icp_process_batch's on the converted u16 images: the early
  *              return of LL.cpp:52-55 (residual -1, R_out / t_out untouched), all-zero renders, a zero anchor and the
- *              NaN patterns they give included.  Where a cloud spans more than 2^21 voxels along an axis the call fails
- *              with LM_E_INVALID instead (lm_set_template_renders' pose stage).  The handle's estimation and
- *              use_scene_cloud apply.
+ *              NaN patterns they give included.  The handle's estimation and use_scene_cloud apply.
  *   Ordering   as lm_bind_images_device: an event recorded on `stream` (a cudaStream_t; NULL = the legacy default stream)
- *              gates the reads, and `stream` waits on a second event behind the last read.  The call returns once the
- *              outputs are on the host; it synchronises the handle's stream only (twice: the render boxes are read back
- *              once to size the crops, lm_pose.h).
- *   Launches   3 (k_icp_scene, k_icp_render_box, k_icp_render_crop) plus, per chunk of 1024 hypotheses, the pose stage's
- *              5 (point-to-plane) or 4 (point-to-point); 2 when every hypothesis takes the early return; none for n_hyp 0.
- * LM_E_INVALID before any device work for a null argument, an empty image, max_iterations < 0, an unknown format, a
- * non-finite or non-positive scale with LM_DEPTH_F32, a stream of another device, a plane that is not device memory of
- * the handle's device or whose pitch is shorter than a row or not aligned to its elements; LM_E_INVALID after the box
- * read-back for a render whose box has 2^21 pixels or more (lm_set_template_renders' limit), and after the chunks for a
- * cloud beyond 2^21 voxels.  With capture on (lm_icp_set_capture) the call also synchronises behind each chunk and
- * copies its clouds out; the outputs do not change.  lm_icp_last_stats and lm_icp_launch_count cover the call. */
+ *              gates the reads, and `stream` waits on a second event behind the call's work.  The call returns once the
+ *              outputs are on the host.
+ * Both calls run on the handle's stream and synchronise it twice: once to read back the render boxes, which size the
+ * crops (lm_pose.h), and once at the end.  Launches: 3 (k_icp_scene, k_icp_render_box, k_icp_render_crop) plus, per
+ * chunk of 1024 hypotheses, the pose stage's 5 (LM_ICP_POINT_TO_PLANE) or 4 (LM_ICP_POINT_TO_POINT, LM_POSE_PSO), plus 1
+ * per chunk when verifying; 2 when every hypothesis takes the early return; none for n_hyp 0.
+ * LM_E_INVALID before any device work for a null argument, an empty image or max_iterations < 0; for
+ * lm_icp_process_batch_device also for an unknown format, a non-finite or non-positive scale with LM_DEPTH_F32, a stream
+ * of another device, a plane that is not device memory of the handle's device or whose pitch is shorter than a row or not
+ * aligned to its elements.  LM_E_INVALID after the box read-back for a render whose box has 2^21 pixels or more
+ * (lm_set_template_renders' limit), and after the chunks for a cloud that spans more than 2^21 voxels of 2.5 mm along an
+ * axis (a tiny, zero or non-finite K); LM_E_CAPACITY when n_hyp (at most 1024 per chunk) renders' crops need 2^31 cloud
+ * points or more.  With capture on (lm_icp_set_capture) the call also synchronises behind each chunk and copies out what
+ * it built and kept; the outputs do not change.  lm_icp_last_stats and lm_icp_launch_count cover the call. */
 int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, int64_t scene_pitch, int scene_format,
                                 float scene_scale, int srows, int scols, const void* const* model_depths,
                                 const int64_t* model_pitches, int model_format, float model_scale, int mrows, int mcols,
@@ -742,52 +743,46 @@ int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* scene_depth, i
                                 const int32_t* detect_xy, int max_iterations, double* R_out, double* t_out, float* residual,
                                 void* stream);
 
-/* Of the last hypothesis processed: [0] points in the down-sampled cloud, [1] ICP iterations run,
- * [2] inlier rmse (m), [3] device time of the last call (us).  After lm_icp_process_batch: the normals and ICP kernels
- * only; a verification (lm_icp_set_verify) runs behind them and is not included.  After lm_icp_process_batch_device: from
- * its input copy to the end of its last chunk's kernels, the box read-back included, and k_pose_verify included when the
- * call verifies. */
+/* Of the last hypothesis with a pose: [0] points in the down-sampled cloud, [1] ICP iterations run, [2] inlier rmse (m);
+ * [3] device time of the last call (us): from lm_icp_process_batch's copy of the planes, or lm_icp_process_batch_device's
+ * gate on `stream`, to the end of its last chunk's kernels, the box read-back included, and k_pose_verify included when
+ * the call verifies. */
 int lm_icp_last_stats(lm_icp* h, double* out4);
 /* NOT the reference's behaviour (default off): register the model cloud against the down-sampled SCENE
  * cloud, which is what LL.cpp:109 evidently meant to do (it down-samples the model cloud twice). */
 int lm_icp_set_use_scene_cloud(lm_icp* h, int on);
-/* LM_ICP_POINT_TO_PLANE (default: k_icp_normals + the ICP kernel, 2 launches per call) or LM_ICP_POINT_TO_POINT (the ICP
- * kernel alone, 1 launch; lm_icp_last_stats [3] then times that kernel alone) for the next lm_icp_process_batch.
- * LM_E_INVALID for any other value. */
+/* LM_ICP_POINT_TO_PLANE (default: k_icp_normals + the ICP kernel), LM_ICP_POINT_TO_POINT (the ICP kernel alone) or
+ * LM_POSE_PSO (k_pose_pso alone, with the settings of lm_icp_set_pose_search) for the next calls.  LM_E_INVALID for any
+ * other value. */
 int lm_icp_set_estimation(lm_icp* h, int estimation);
-/* LM_POSE_PSO's settings for this handle (see lm_set_pose_search); with LM_POSE_PSO lm_icp_process_batch uploads the scene
- * and runs k_pose_pso alone (1 launch, timed by lm_icp_last_stats [3]). */
+/* LM_POSE_PSO's settings for this handle (see lm_set_pose_search); hypothesis i of a call draws as job i. */
 int lm_icp_set_pose_search(lm_icp* h, int particles, int iterations, double dt_mm, double dr_deg, double clamp_mm,
                            uint64_t seed);
 int64_t lm_icp_launch_count(lm_icp* h);
-/* Pose verification (see lm_set_pose_verify) for the next lm_icp_process_batch and lm_icp_process_batch_device: one more
- * launch per call (per chunk of 1024 hypotheses on the device path); the host path also uploads its raw model clouds and
- * the scene.  lm_icp_last_stats [3] includes that launch on the device path only.  lm_icp_verify: score[k], counts6 + 6k of hypothesis k of the last call, *n the hypotheses;
- * LM_E_STATE when that call did not verify.  LM_E_INVALID for a NaN or negative inlier_mm. */
+/* Pose verification (see lm_set_pose_verify) for the next calls: one more launch per chunk of 1024 hypotheses.
+ * lm_icp_verify: score[k], counts6 + 6k of hypothesis k of the last call, *n the hypotheses; LM_E_STATE when that call
+ * did not verify.  LM_E_INVALID for a NaN or negative inlier_mm. */
 int lm_icp_set_verify(lm_icp* h, int on, double inlier_mm);
 int lm_icp_verify(lm_icp* h, float* score, int32_t* counts6, int64_t cap, int64_t* n);
 
 /* ---- introspection of the ICP kernels, used by the stage-by-stage tests ---- */
-/* While capture is on (default off), lm_icp_process_batch and lm_icp_process_batch_device keep, per hypothesis, what
- * their kernels saw and kept in the last call; a call that fails past its argument checks keeps nothing.
- * lm_icp_process_batch_device keeps COUNTS, SOURCE, TARGET, INIT and RESULT (the clouds the pose stage's kernels
- * built); its NORMALS, KNN and CORR_* are LM_E_STATE.  Turning capture on or off drops what was kept.  The outputs do
- * not depend on it. */
+/* While capture is on (default off), both calls keep, per hypothesis, what their kernels saw and kept in the last call;
+ * a call that fails past its argument checks keeps nothing.  Turning capture on or off drops what was kept.  The
+ * outputs do not depend on it. */
 int lm_icp_set_capture(lm_icp* h, int on);
 /* Copies item `what` of hypothesis `hyp` of the last call to `out` (cap bytes):
  *   COUNTS      2 int32: source and target points
- *   SOURCE      source cloud as uploaded, src x 3 f64;  TARGET the target cloud, tgt x 3 f64
+ *   SOURCE      source cloud, src x 3 f64;  TARGET the target cloud, tgt x 3 f64
  *   NORMALS     target normals, tgt x 3 f64
  *   INIT        initial guess, 16 f64 row-major
  *   RESULT      19 f64: the final transformation (16, row-major), fitness, rmse, iterations
  *   KNN         tgt x 30 int32: the neighbours k_icp_normals kept (target indices, kept order, padded with -1)
  *   CORR_FIRST  src int32: the correspondence (target index, -1: none) of every source point on pass 0
  *   CORR_LAST   src int32: the same for the last pass the kernel ran (the pass whose fitness and rmse are returned)
- *   SEARCH      the swarm record of an LM_POSE_PSO call (lm_set_pose_search), lm_icp_process_batch only
- * LM_E_STATE for a hypothesis that took the early return, and for NORMALS / KNN of a call with LM_ICP_POINT_TO_POINT
- * or LM_POSE_PSO (nothing was computed), CORR_* of an LM_POSE_PSO call and SEARCH of any other call or of
- * lm_icp_process_batch_device, LM_E_CAPACITY when cap is too small, LM_E_INVALID for a hypothesis outside the last
- * captured call. */
+ *   SEARCH      the swarm record of an LM_POSE_PSO call (lm_set_pose_search)
+ * LM_E_STATE for a hypothesis that took the early return, and for an item the call's estimation did not compute:
+ * NORMALS / KNN but with LM_ICP_POINT_TO_PLANE, CORR_* with LM_POSE_PSO, SEARCH but with LM_POSE_PSO.  LM_E_CAPACITY when
+ * cap is too small, LM_E_INVALID for a hypothesis outside the last captured call. */
 #define LM_ICP_CAPTURE_COUNTS 0
 #define LM_ICP_CAPTURE_SOURCE 1
 #define LM_ICP_CAPTURE_TARGET 2

@@ -1,5 +1,5 @@
-"""A float64 model of the clouds poseRefine::process builds (LL.cpp:43-109), which the device pose stage's k_pose_cloud,
-segmented sort and k_pose_voxel and lm_icp_process_batch's build_cloud + voxel_down_sample compute.
+"""A float64 model of the clouds poseRefine::process builds (LL.cpp:43-109), which the pose stage's k_pose_cloud,
+segmented sort and k_pose_voxel compute for the detector and for lm_icp_process_batch(_device).
 
 Every arithmetic step is the same IEEE operation as theirs, so the comparison is bit for bit:
   back-projection   f32 (c - cx) / f  (int -> f32, f32 subtract, f32 divide), widened, times the f64 z = d / 1000.0

@@ -310,20 +310,24 @@ def test_pose_refine_surface_takes_tensors(data, estimation, use_scene):
         native.set_use_scene_cloud(False)
 
 
-def test_capture_of_a_device_call(data, icp):
-    """Capture keeps a device call's clouds, initial guess and result, and refuses what that path does not keep."""
+def test_device_call_captures_what_a_host_call_captures(data, icp):
+    """Capture keeps every item of a device call (point-to-plane), each bitwise the host-buffer call's on the same input."""
     g = data["g"]
+    set_mode(icp, MODES[0])
     args = (data["sK"], data["K"][:1], data["R"][:1], data["t"][:1], [[300, 200]])
     icp.set_capture(True)
     try:
+        icp.process_batch(g["depth"], [g["render"]], *args)
+        want = icp.capture(0)
         icp.process_batch_device(lib.DeviceDepths(cuda(g["depth"]), [cuda(g["render"])], 1.0, 1.0, None, 0), *args)
         buf = np.zeros(1 << 20, np.uint8)
         L = lib.load()
-        for what in ("normals", "knn", "corr_first", "corr_last"):
-            rc = L.lm_icp_capture(icp._h, 0, lib.CAPTURE_ITEMS[what], buf.ctypes.data, buf.nbytes)
-            assert rc == lib.LM_E_STATE and "device" in L.lm_last_error().decode(), what
-        for what in ("counts", "source", "target", "init", "result"):
+        for what in ("counts", "source", "target", "normals", "init", "result", "knn", "corr_first", "corr_last"):
             assert L.lm_icp_capture(icp._h, 0, lib.CAPTURE_ITEMS[what], buf.ctypes.data, buf.nbytes) == lib.LM_OK, what
+        got = icp.capture(0)
+        for what in ("source", "target", "normals", "init", "T", "knn", "corr_first", "corr_last"):
+            assert got[what] is not None and got[what].tobytes() == want[what].tobytes(), what
+        assert (got["fitness"], got["rmse"], got["iterations"]) == (want["fitness"], want["rmse"], want["iterations"])
     finally:
         icp.set_capture(False)
 

@@ -219,17 +219,17 @@ def test_batch_equals_single_calls(icp, use_scene):
             assert np.array_equal(np.asarray(v), np.asarray(caps[i][k])), "batch hypothesis %d: %s" % (i, k)
 
 
-def test_switching_launches_and_errors():
+def test_switching_estimation_launches_the_pose_stage_and_errors():
     c = CASES["size_513"]
     args = (c.scene, [c.model, c.model], c.K, np.stack([c.K] * 2), np.stack([c.R] * 2), np.stack([c.t] * 2), [c.xy, c.xy], 30)
     h = lib.NativeIcp()
     h.set_use_scene_cloud(True)
     b0 = h.launch_count()
     p2p = h.process_batch(*args, estimation=P2P)
-    assert h.launch_count() - b0 == 1
+    assert h.launch_count() - b0 == 7
     b0 = h.launch_count()
     plane = h.process_batch(*args, estimation=P2PL)
-    assert h.launch_count() - b0 == 2
+    assert h.launch_count() - b0 == 8
     for est, got in ((P2P, p2p), (P2PL, plane)):
         fresh = lib.NativeIcp()
         fresh.set_use_scene_cloud(True)

@@ -208,14 +208,15 @@ def test_voxel_overflow_fails_the_frame_and_the_next_frame_is_clean(bank):
         fresh.close()
 
 
-def test_unkeyable_intrinsics_are_refused_on_both_icp_paths():
-    """A zero or NaN render K gives clouds without voxel indices: both lm_icp_process_batch and the device path refuse."""
+def test_unkeyable_intrinsics_are_refused_alike_by_both_icp_calls():
+    """A zero or NaN render K gives clouds that span more than 2^21 voxels: lm_icp_process_batch and
+    lm_icp_process_batch_device refuse alike."""
     c = ic.size_case(257)
     icp = lib.NativeIcp()
     try:
         for K in (cases.K(0.0, 100.0, 320.0, 240.0), cases.K(np.nan, 100.0, 320.0, 240.0), cases.K(100.0, 100.0, np.nan, 240.0)):
             args = (c.K, K[None], c.R[None], c.t[None], [c.xy])
-            with pytest.raises(RuntimeError, match="voxel index"):
+            with pytest.raises(RuntimeError, match="spans more than"):
                 icp.process_batch(c.scene, [c.model], *args)
             d = lib.DeviceDepths(cuda(c.scene), [cuda(c.model)], 1.0, 1.0, None, 0)
             with pytest.raises(RuntimeError, match="spans more than"):
@@ -339,7 +340,7 @@ def test_device_icp_capture_equals_the_host_capture():
                                 h.capture(i)
                         continue
                     cg, cw = dev.capture(i), host.capture(i)
-                    for item in ("source", "target", "init", "T"):
+                    for item in ("source", "target", "normals", "init", "T", "knn", "corr_first", "corr_last"):
                         assert same_bits(cg[item], cw[item]), (name, use_scene, i, item, first_difference(cg[item], cw[item]))
                     assert (cg["fitness"], cg["rmse"], cg["iterations"]) == (cw["fitness"], cw["rmse"], cw["iterations"]) or \
                         np.isnan(cg["fitness"]) and np.isnan(cw["fitness"])

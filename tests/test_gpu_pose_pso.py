@@ -171,13 +171,17 @@ def test_frame_chain_equals_process_batch(data, verify):
         # use_scene_cloud has no effect
         again = nat.match_pose(g["rgb"], g["depth"], None, thr, data["sK"], 0.5, top_k, 30, True, PSO)
         ps.same_poses(again, want)
-        # process_batch_device equals process_batch, verification included
-        icp = lib.NativeIcp()
+        # process_batch_device equals process_batch, verification and swarm records included
+        icp, hv = lib.NativeIcp(), lib.NativeIcp()
+        for h in (icp, hv):
+            h.set_capture(True)
         dev = host(data, got[0], icp, verify=10.0 if verify else None, device=True)
         assert [a.tobytes() for a in dev] == [a.tobytes() for a in want]
+        staged = host(data, got[0], hv, verify=10.0 if verify else None)
+        assert [a.tobytes() for a in staged] == [a.tobytes() for a in want]
+        for i in np.flatnonzero(want[2] != -1.0):
+            same_record(icp.capture(int(i))["search"], hv.capture(int(i))["search"])
         if verify:
-            hv = lib.NativeIcp()
-            host(data, got[0], hv, verify=10.0)
             assert [a.tobytes() for a in icp.verify()] == [a.tobytes() for a in hv.verify()]
             assert [a.tobytes() for a in nat.pose_verify()] == [a.tobytes() for a in hv.verify()]
         # the pose NMS on top equals the model on those poses; 4 launches for the pose stage

@@ -1,10 +1,9 @@
-"""refine_matches from numpy depths (host-built clouds, lm_icp_process_batch) against the same call from CUDA tensors
-(clouds built on the device, lm_icp_process_batch_device), on the recorded driver frame (tests/golden/driver_trace.npz)
-and its box-NMS survivors against the allScales bank, with the shifted renders of tests/test_gpu_pose_stage.py.  For the
-first 3, 35 and ~390 survivors the two paths run in alternating blocks within this one process; per path it prints the
-median wall time per call, the median device time lm_icp_last_stats reports (normals + ICP kernels for numpy; input copy
-to the last ICP kernel, box read-back included, for tensors), whether the outputs are identical, and the card's power
-limit and SM clock.
+"""refine_matches from numpy depths (lm_icp_process_batch: the planes copied to the device) against the same call from
+CUDA tensors (lm_icp_process_batch_device), on the recorded driver frame (tests/golden/driver_trace.npz) and its box-NMS
+survivors against the allScales bank, with the shifted renders of tests/test_gpu_pose_stage.py.  For the first 3, 35 and
+~390 survivors the two arms run in alternating blocks within this one process; per arm it prints the median wall time
+per call, the median device time lm_icp_last_stats reports (from the input copy to the last ICP kernel, box read-back
+included), whether the outputs are identical, and the card's power limit and SM clock.
 
     python tools/icp_device_probe.py [--blocks 6] [--calls 20]
 """
