@@ -18,7 +18,10 @@ LIB_PATH = os.environ.get("LINEMOD_B200_LIB") or os.path.join(_HERE, "csrc", "li
 LM_OK, LM_E_INVALID, LM_E_CUDA, LM_E_STATE, LM_E_CAPACITY = 0, -1, -2, -3, -4
 # capture items of lm_icp_capture and lm_debug_pose_clouds (include/linemod_b200.h)
 CAPTURE_ITEMS = dict(counts=0, source=1, target=2, normals=3, init=4, result=5, knn=6, corr_first=7, corr_last=8, slots=9, posed=10,
-                     raw_model=11, raw_scene=12, search=13)
+                     raw_model=11, raw_scene=12, search=13, window=14)
+# lm_track's statuses (LM_TRACK_* of include/linemod_b200.h) by the name poseRefine.getTrackStatus returns
+TRACK_STATUS = ("tracked", "outside", "window", "no_depth")
+TRACK_MAX = 1024  # objects per lm_track call
 SHARD_CONTIGUOUS, SHARD_INTERLEAVED = 0, 1
 
 MATCH_DTYPE = np.dtype([("x", "<i4"), ("y", "<i4"), ("similarity", "<f4"), ("class_index", "<i4"), ("template_id", "<i4")])
@@ -43,6 +46,7 @@ SYMBOLS = [
     "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture", "lm_icp_process_batch_device",
     "lm_set_pose_verify", "lm_pose_verify", "lm_pose_verify_points", "lm_icp_set_verify", "lm_icp_verify",
     "lm_set_pose_search", "lm_icp_set_pose_search", "lm_pose_search_points",
+    "lm_track", "lm_track_device", "lm_pose_transforms",
 ]
 
 # The pose stage's estimation (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT / LM_POSE_PSO of include/linemod_b200.h) by
@@ -461,6 +465,10 @@ def load():
     L.lm_set_pose_search.argtypes = [vp] + search
     L.lm_icp_set_pose_search.argtypes = [vp] + search
     L.lm_pose_search_points.argtypes = [c_int, f64p, c_i64, f64p, u16p, c_int, c_int, f32p] + search + [c_i64, f64p, vp, c_i64]
+    track_out = [f32p, vp, c_int, c_int, c_int, f64p, f64p, f64p, f32p, i32p, i32p]
+    L.lm_track.argtypes = [vp, u16p, c_int, c_int] + track_out
+    L.lm_track_device.argtypes = [vp, vp, c_i64, c_int, c_f, c_int, c_int] + track_out + [vp]
+    L.lm_pose_transforms.argtypes = [vp, f64p, c_i64, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
     L.lm_icp_destroy.restype = None
@@ -1090,12 +1098,16 @@ class NativeDetector:
         """The clouds of the last pose-stage chunk this handle enqueued (lm_debug_pose_clouds): (head, slots).  head is a
         dict of the chunk's slots, rank, world and first (slot i holds survivor first + rank + i * world); slots has one
         dict per slot: posed (bool) and, where posed, counts (src, tgt), source / target [n,3] f64 (down-sampled), init
-        [4,4] f64, raw_model / raw_scene [n,3] f64 (before down-sampling)."""
+        [4,4] f64, raw_model / raw_scene [n,3] f64 (before down-sampling); a track chunk's slots also window (x, y, w, h)
+        and status."""
         head = self._pose_item(-1, "slots", np.zeros(4, np.int32))
         out = []
         for i in range(int(head[0])):
             posed = bool(self._pose_item(i, "posed", np.zeros(1, np.uint8))[0])
             d = dict(posed=posed)
+            w = np.zeros(5, np.int32)
+            if self._L.lm_debug_pose_clouds(self._h, i, CAPTURE_ITEMS["window"], w.ctypes.data_as(ctypes.c_void_p), w.nbytes) == LM_OK:
+                d["window"], d["status"] = w[:4].copy(), int(w[4])  # a track chunk's (lm_track)
             if posed:
                 n, nt = self._pose_item(i, "counts", np.zeros(2, np.int32)).tolist()
                 d.update(counts=(n, nt), source=self._pose_item(i, "source", np.zeros((n, 3))),
@@ -1144,6 +1156,69 @@ class NativeDetector:
         a = (ctypes.c_int64 * 4)()
         check(self._L.lm_pose_stats(self._h, a))
         return [int(v) for v in a]
+
+    def pose_transforms(self):
+        """The 4x4 T of every entry of the last finished pose run (lm_pose_transforms): f64 [n,4,4], NaN without a pose."""
+        n = ctypes.c_int64()
+        f64p = ctypes.POINTER(ctypes.c_double)
+        rc = self._L.lm_pose_transforms(self._h, None, 0, ctypes.byref(n))
+        if rc != LM_E_CAPACITY:
+            check(rc)
+        out = np.empty((int(n.value), 4, 4), np.float64)
+        if out.size:
+            check(self._L.lm_pose_transforms(self._h, out.ctypes.data_as(f64p), out.shape[0], ctypes.byref(n)))
+        return out
+
+    @staticmethod
+    def track_objects(objects):
+        """lm_track_object [n] of (class_index, template_id, T [4,4] f64) triples."""
+        arr = (TrackObject * max(len(objects), 1))()
+        for i, (c, t, T) in enumerate(objects):
+            arr[i].class_index, arr[i].template_id = int(c), int(t)
+            arr[i].T[:] = [float(v) for v in np.asarray(T, np.float64).reshape(16)]
+        return arr
+
+    def track(self, depth, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane"):
+        """lm_track on a u16 HxW numpy depth (mm).  objects: (class_index, template_id, T) triples.  Returns (status [n]
+        int32, T [n,4,4], R [n,3,3], t [n,3] mm, residual [n] f32, box [n,4] int32); an entry not tracked keeps its input
+        T and R / t NaN."""
+        depth = np.ascontiguousarray(depth)
+        if depth.dtype != np.uint16 or depth.ndim != 2:
+            raise TypeError("depth must be a uint16 HxW image (mm)")
+        return self._track(lambda *a: self._L.lm_track(self._h, depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), depth.shape[0],
+                                                       depth.shape[1], *a), sceneK, objects, max_iterations, margin_px, estimation)
+
+    def track_device(self, depth, pitch, depth_format, depth_scale, rows, cols, stream, sceneK, objects, max_iterations=30, margin_px=4,
+                     estimation="point_to_plane"):
+        """lm_track_device on a pitched device plane (u16 mm or f32 scaled by depth_scale) ordered on `stream` (a CUDA stream
+        handle).  Returns what track returns."""
+        return self._track(lambda *a: self._L.lm_track_device(self._h, depth, int(pitch), int(depth_format), ctypes.c_float(depth_scale),
+                                                              int(rows), int(cols), *a, stream), sceneK, objects, max_iterations,
+                           margin_px, estimation)
+
+    def _track(self, fn, sceneK, objects, max_iterations, margin_px, estimation):
+        est = estimation_code(estimation)
+        sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+        n = len(objects)
+        arr = self.track_objects(objects)
+        T = np.stack([np.asarray(o[2], np.float64).reshape(4, 4) for o in objects]) if n else np.zeros((0, 4, 4))
+        T = np.ascontiguousarray(T)
+        Ro = np.full((max(n, 1), 3, 3), np.nan)
+        to = np.full((max(n, 1), 3), np.nan)
+        res = np.zeros(max(n, 1), np.float32)
+        status = np.zeros(max(n, 1), np.int32)
+        box = np.zeros((max(n, 1), 4), np.int32)
+        f32p, f64p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
+        Tout = T if n else np.zeros((1, 4, 4))
+        check(self._L.lm_set_pose_estimation(self._h, est))
+        check(fn(sK.ctypes.data_as(f32p), ctypes.cast(arr, ctypes.c_void_p), n, int(max_iterations), int(margin_px), Tout.ctypes.data_as(f64p), Ro.ctypes.data_as(f64p),
+                 to.ctypes.data_as(f64p), res.ctypes.data_as(f32p), self._i32(status), self._i32(box)))
+        return status[:n].copy(), Tout[:n].copy(), Ro[:n].copy(), to[:n].copy(), res[:n].copy(), box[:n].copy()
+
+
+class TrackObject(ctypes.Structure):
+    """lm_track_object of include/linemod_b200.h."""
+    _fields_ = [("class_index", ctypes.c_int32), ("template_id", ctypes.c_int32), ("T", ctypes.c_double * 16)]
 
 
 class NativeIcp:

@@ -2432,6 +2432,93 @@ extern "C" int lm_debug_pose_clouds(lm_detector* d, int slot, int what, void* ou
   return pose_stage_clouds(d->pose, slot, what, out, cap);
 }
 
+// lm_track and lm_track_device: every refusal before any device work, then the scene (dev null: host depth, copied) and
+// one track run of the pose stage on the detector's stream.
+static int track(lm_detector* d, const void* depth, const DeviceFrame* dev, cudaStream_t caller, int rows, int cols, const float* sceneK,
+                 const lm_track_object* objects, int n, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out,
+                 float* residual, int32_t* status, int32_t* box) {
+  if (!d || !depth || !sceneK || n < 0 || (n > 0 && (!objects || !T_out || !R_out || !t_out || !residual || !status || !box)))
+    return fail(LM_E_INVALID, "null argument or n < 0");
+  if (n > LM_POST_MAX) return fail(LM_E_INVALID, "%d objects, a track run takes at most %d", n, LM_POST_MAX);
+  if (rows <= 0 || cols <= 0) return fail(LM_E_INVALID, "empty depth image %d x %d", rows, cols);
+  if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
+  if (margin_px < 0) return fail(LM_E_INVALID, "margin_px %d < 0", margin_px);
+  if (dev && dev->format != LM_DEPTH_U16_MM && dev->format != LM_DEPTH_F32)
+    return fail(LM_E_INVALID, "unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", dev->format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
+  if (dev && dev->format == LM_DEPTH_F32 && !(std::isfinite(dev->scale) && dev->scale > 0.f))
+    return fail(LM_E_INVALID, "depth_scale %g: float depth needs a finite scale > 0", (double)dev->scale);
+  if (d->pose_estimation == LM_POSE_PSO)
+    return fail(LM_E_STATE, "tracking runs an ICP: LM_POSE_PSO starts from an identity rotation (lm_set_pose_estimation)");
+  if (d->px_rank >= 0) return fail(LM_E_STATE, "tracking does not run with a connected peer exchange");
+  std::vector<TrackObject> obj((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const lm_track_object& o = objects[i];
+    if (o.class_index < 0 || o.class_index >= d->n_classes)
+      return fail(LM_E_INVALID, "object %d: class %d outside the bank's %d classes", i, o.class_index, d->n_classes);
+    const int32_t nt = d->class_begin[o.class_index + 1] - d->class_begin[o.class_index];
+    if (o.template_id < 0 || o.template_id >= nt)
+      return fail(LM_E_INVALID, "object %d: template %d outside class %d's %d templates", i, o.template_id, o.class_index, nt);
+    for (int k = 0; k < 16; ++k)
+      if (!std::isfinite(o.T[k])) return fail(LM_E_INVALID, "object %d: T[%d] is not finite", i, k);
+    obj[(size_t)i].g = d->class_begin[o.class_index] + o.template_id;
+    memcpy(obj[(size_t)i].T, o.T, sizeof(o.T));
+    const int32_t g = (int32_t)obj[(size_t)i].g;
+    if (!d->pose || !pose_stage_covers(d->pose, &g, 1))
+      return fail(LM_E_STATE, "object %d: no template render registered for class %d, template %d (lm_set_template_renders)", i,
+                  o.class_index, o.template_id);
+  }
+  if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
+  if (dev) {
+    int rc = check_device_stream(d->device, caller);
+    const int sz = dev->format == LM_DEPTH_F32 ? 4 : 2;
+    if (!rc) rc = check_device_plane(d->device, "depth", depth, dev->depth_pitch, (int64_t)sz * cols, sz);
+    if (rc) return rc;
+  }
+  if (!d->pose) return fail(LM_E_STATE, "no template renders registered (lm_set_template_renders)");
+  CU(cudaSetDevice(d->device));
+  cudaStream_t st = d->stream.get();
+  d->chain.pose = d->chain.pose_nms = false;  // the stage's buffers now hold the track run: a pending frame's pose stage is abandoned
+  const uint16_t* scene = nullptr;
+  int rc;
+  if (dev) {  // the reads of the caller's plane start behind its stream's work, and its later work waits for the conversion
+    if (!d->ev_in.get()) CU(d->ev_in.create(cudaEventDisableTiming));
+    if (!d->ev_out.get()) CU(d->ev_out.create(cudaEventDisableTiming));
+    CU(cudaEventRecord(d->ev_in.get(), caller));
+    CU(cudaStreamWaitEvent(st, d->ev_in.get(), 0));
+    rc = pose_track_scene(d->pose, st, false, depth, dev->depth_pitch, dev->format, dev->scale, rows, cols, &scene, &d->launches);
+    CU(cudaEventRecord(d->ev_out.get(), st));
+    CU(cudaStreamWaitEvent(caller, d->ev_out.get(), 0));
+  } else {
+    rc = pose_track_scene(d->pose, st, true, depth, 2 * (int64_t)cols, LM_DEPTH_U16_MM, 1.f, rows, cols, &scene, &d->launches);
+  }
+  if (rc) return rc;
+  PoseOptions o = {rows, cols, 1, max_iterations, d->pose_estimation, st, nullptr, d->pose_verify, d->pose_search};
+  return pose_stage_track(d->pose, o, scene, sceneK, obj.data(), n, margin_px, &d->launches, T_out, R_out, t_out, residual, status, box);
+}
+
+extern "C" int lm_track(lm_detector* d, const uint16_t* depth, int rows, int cols, const float* sceneK, const lm_track_object* objects,
+                        int n, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out, float* residual,
+                        int32_t* status, int32_t* box) {
+  return track(d, depth, nullptr, nullptr, rows, cols, sceneK, objects, n, max_iterations, margin_px, T_out, R_out, t_out, residual,
+               status, box);
+}
+
+extern "C" int lm_track_device(lm_detector* d, const void* depth, int64_t depth_pitch, int depth_format, float depth_scale, int rows,
+                               int cols, const float* sceneK, const lm_track_object* objects, int n, int max_iterations, int margin_px,
+                               double* T_out, double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
+  DeviceFrame f = {};
+  f.depth = depth; f.depth_pitch = depth_pitch; f.format = depth_format; f.scale = depth_scale;
+  return track(d, depth, &f, (cudaStream_t)stream, rows, cols, sceneK, objects, n, max_iterations, margin_px, T_out, R_out, t_out,
+               residual, status, box);
+}
+
+extern "C" int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n) {
+  if (!d || !n) return fail(LM_E_INVALID, "null argument");
+  if (!d->pose) return fail(LM_E_STATE, "no pose stage has run");
+  if (d->device >= 0) CU(cudaSetDevice(d->device));
+  return pose_stage_transforms(d->pose, T_out, cap, n);
+}
+
 extern "C" int lm_set_template_depths(lm_detector* d, int64_t first, int64_t n, const float* z_mm) {
   if (!d) return fail(LM_E_INVALID, "null detector");
   if (first < 0 || n < 0 || first + n > d->G)

@@ -25,7 +25,8 @@
 // and a scene (staged from the host, or in the caller's device memory): k_icp_scene, k_icp_render_box and
 // k_icp_render_crop build the per-hypothesis table k_pose_cloud reads (end of this file).  With verification on
 // (lm_set_pose_verify, lm_icp_set_verify) k_pose_verify follows the ICP kernel of an unshared chunk, and k_pose_nms<true>
-// reads it.
+// reads it.  A track chunk (lm_track) builds its clouds with k_track_cloud from given transformations instead of
+// k_pose_cloud from match positions; the rest of the chunk is the same.
 
 #include "linemod_b200.h"
 #include "lm_pose.h"
@@ -34,6 +35,7 @@
 
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -1318,6 +1320,205 @@ __global__ void __launch_bounds__(VERIFY_THREADS) k_pose_verify(PoseParams p, co
 static bool verify_delta_ok(double inlier_mm) { return std::isfinite(inlier_mm) && inlier_mm >= 0.0; }
 
 // --------------------------------------------------------------------------------------------
+// tracking (include/linemod_b200.h, lm_track): a chunk whose clouds come from a given transformation T instead of a
+// match position -- the model cloud of the template, and the scene cloud of the window the model projects to under T
+// --------------------------------------------------------------------------------------------
+struct TrackRec {  // one object's window (x, y, w, h: clipped, with the margin), projected box (unclipped) and status
+  int32_t window[4], box[4];
+  int32_t status, pad;
+};
+
+struct TrackParams {
+  const TrackObject* obj;     // [n] template (bank index) and T
+  const PoseTpl* tpl;
+  const uint16_t* crops;
+  VerifyScene sc;             // the scene depth and intrinsics
+  int32_t margin;
+  int64_t cap;                // most window pixels (LM_TRACK_WINDOW beyond)
+  int64_t stride, M;          // points per object: M model points, then cap scene points
+  double* raw;                // object i's model cloud at i * stride, its scene cloud at i * stride + M
+  unsigned long long* keys;
+  int32_t* vals;
+  int32_t* seg_begin;         // [2n], as PoseParams
+  int32_t* seg_end;
+  IcpJob* jobs;
+  int32_t* err;
+  uint8_t* posed;             // 1: LM_TRACK_TRACKED
+  TrackRec* rec;
+};
+
+// Voxel keys of the n points P (PointCloud::VoxelDownSample(0.0025) about the per-axis minima mn, as k_pose_cloud
+// computes them) into keys / vals from slot on.
+__device__ __forceinline__ void track_voxel_keys(const double* P, int n, const double* mn, size_t slot, unsigned long long* keys,
+                                                 int32_t* vals, int32_t* err) {
+  const unsigned long long F = (1ull << POSE_KEY_BITS) - 1;
+  double o[3];
+  for (int c = 0; c < 3; ++c) o[c] = __dsub_rn(mn[c], 0.00125);
+  for (int j = threadIdx.x; j < n; j += POSE_THREADS) {
+    unsigned long long key = 0;
+    for (int c = 0; c < 3; ++c) {
+      const double v = floor(__ddiv_rn(__dsub_rn(P[3 * j + c], o[c]), 0.0025));
+      unsigned long long a = (unsigned long long)(long long)v;
+      if (!(v >= 0.0 && v <= (double)F)) { atomicExch(err, 1); a = F; }
+      key = (key << POSE_KEY_BITS) | a;
+    }
+    keys[slot + j] = key;
+    vals[slot + j] = j;
+  }
+}
+
+// verify_point's step 3 alone, operation for operation (verify_point itself is left as it is, so that k_pose_verify and
+// k_pose_pso keep their code): true and the pixel (*c, *r) when the point lands in the frame in front of the camera.
+__device__ __forceinline__ bool track_project(const double* T, double px, double py, double pz, const VerifyScene& sc, int* c, int* r) {
+  double q[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    q[k] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4 * k], px), __dmul_rn(T[4 * k + 1], py)), __dmul_rn(T[4 * k + 2], pz)), T[4 * k + 3]);
+  if (!(q[2] > 0.0)) return false;
+  const double u = __dadd_rn(__dmul_rn((double)sc.fx, __ddiv_rn(q[0], q[2])), (double)sc.cx);
+  const double v = __dadd_rn(__dmul_rn((double)sc.fy, __ddiv_rn(q[1], q[2])), (double)sc.cy);
+  if (!isfinite(u) || !isfinite(v)) return false;
+  const double fc = floor(__dadd_rn(u, 0.5)), fr = floor(__dadd_rn(v, 0.5));
+  if (!(fc >= 0.0 && fc < (double)sc.cols && fr >= 0.0 && fr < (double)sc.rows)) return false;
+  *c = (int)fc; *r = (int)fr;
+  return true;
+}
+
+// One CTA per object.  The model cloud is k_pose_cloud's (every crop pixel with render depth > 0, row-major); each of
+// its points is projected under T (track_project) and the in-frame pixels' extent is reduced over the CTA.  The
+// window's pixels with scene depth > 0 are back-projected in row-major order as k_pose_cloud back-projects the scene.
+// Both clouds get their voxel keys; the job starts at T.  An object without the status TRACKED writes an empty job.
+__global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
+  typedef cub::BlockScan<int, POSE_THREADS> Scan;
+  typedef cub::BlockReduce<double, POSE_THREADS> Reduce;
+  __shared__ union {
+    typename Scan::TempStorage scan;
+    typename Reduce::TempStorage reduce;
+  } tmp;
+  __shared__ double s_T[16], s_min[6];
+  __shared__ int s_ext[4], s_win[4], s_status;
+  const int i = blockIdx.x, tid = threadIdx.x;
+  const PoseTpl T = p.tpl[p.obj[i].g];
+  const size_t sm = (size_t)i * p.stride, ss = sm + p.M;
+  double* __restrict__ Mp = p.raw + sm * 3;
+  double* __restrict__ Sp = p.raw + ss * 3;
+  if (tid < 16) s_T[tid] = p.obj[i].T[tid];
+  if (tid == 0) { s_ext[0] = s_ext[1] = INT_MAX; s_ext[2] = s_ext[3] = -1; }
+  __syncthreads();
+  const uint16_t* __restrict__ C = p.crops + T.crop;
+  const int bw = T.bw, npix = T.bw * T.bh;
+  int c0 = INT_MAX, r0 = INT_MAX, c1 = -1, r1 = -1;
+  int base = 0;
+  for (int t0 = 0; t0 < npix; t0 += POSE_THREADS) {
+    const int k = t0 + tid;
+    bool fm = false;
+    double mx = 0, my = 0, mz = 0;
+    if (k < npix && C[k] > 0) {
+      const int r = k / bw, q = k - r * bw;
+      fm = true;
+      mz = __ddiv_rn((double)C[k], 1000.0);
+      mx = pose_backproject(q + T.bx, T.K[2], T.K[0], mz);
+      my = pose_backproject(r + T.by, T.K[5], T.K[4], mz);
+      int pc, pr;
+      if (track_project(s_T, mx, my, mz, p.sc, &pc, &pr)) {
+        c0 = min(c0, pc); c1 = max(c1, pc);
+        r0 = min(r0, pr); r1 = max(r1, pr);
+      }
+    }
+    int excl, agg;
+    Scan(tmp.scan).ExclusiveSum(fm ? 1 : 0, excl, agg);
+    if (fm) { double* o = Mp + 3 * (size_t)(base + excl); o[0] = mx; o[1] = my; o[2] = mz; }
+    base += agg;
+    __syncthreads();
+  }
+  const int nm = base;
+  c0 = __reduce_min_sync(0xffffffffu, c0); r0 = __reduce_min_sync(0xffffffffu, r0);
+  c1 = __reduce_max_sync(0xffffffffu, c1); r1 = __reduce_max_sync(0xffffffffu, r1);
+  if ((tid & 31) == 0) { atomicMin(&s_ext[0], c0); atomicMin(&s_ext[1], r0); atomicMax(&s_ext[2], c1); atomicMax(&s_ext[3], r1); }
+  __syncthreads();
+  if (tid == 0) {
+    TrackRec& rc = p.rec[i];
+    int st = LM_TRACK_TRACKED;
+    for (int k = 0; k < 4; ++k) rc.window[k] = rc.box[k] = s_win[k] = 0;
+    if (s_ext[2] < 0) {
+      st = LM_TRACK_OUTSIDE;
+    } else {
+      const int64_t x0 = s_ext[0], y0 = s_ext[1], x1 = s_ext[2], y1 = s_ext[3], m = p.margin;
+      rc.box[0] = (int)x0; rc.box[1] = (int)y0; rc.box[2] = (int)(x1 - x0 + 1); rc.box[3] = (int)(y1 - y0 + 1);
+      const int64_t wx0 = max(x0 - m, (int64_t)0), wy0 = max(y0 - m, (int64_t)0);
+      const int64_t wx1 = min(x1 + m, (int64_t)p.sc.cols - 1), wy1 = min(y1 + m, (int64_t)p.sc.rows - 1);
+      s_win[0] = (int)wx0; s_win[1] = (int)wy0; s_win[2] = (int)(wx1 - wx0 + 1); s_win[3] = (int)(wy1 - wy0 + 1);
+      for (int k = 0; k < 4; ++k) rc.window[k] = s_win[k];
+      if ((int64_t)s_win[2] * s_win[3] > p.cap) st = LM_TRACK_WINDOW;
+    }
+    s_status = st;
+  }
+  __syncthreads();
+  int ns = 0;
+  if (s_status == LM_TRACK_TRACKED) {  // block-uniform
+    const int wx = s_win[0], wy = s_win[1], ww = s_win[2], wpix = s_win[2] * s_win[3];
+    base = 0;
+    for (int t0 = 0; t0 < wpix; t0 += POSE_THREADS) {
+      const int k = t0 + tid;
+      bool fs = false;
+      double sx = 0, sy = 0, sz = 0;
+      if (k < wpix) {
+        const int r = k / ww, q = k - r * ww;
+        const int sr = wy + r, sc = wx + q;
+        const uint16_t sd = p.sc.depth[(size_t)sr * p.sc.cols + sc];
+        if (sd > 0) {
+          fs = true;
+          sz = __ddiv_rn((double)sd, 1000.0);
+          sx = pose_backproject(sc, p.sc.cx, p.sc.fx, sz);
+          sy = pose_backproject(sr, p.sc.cy, p.sc.fy, sz);
+        }
+      }
+      int excl, agg;
+      Scan(tmp.scan).ExclusiveSum(fs ? 1 : 0, excl, agg);
+      if (fs) { double* o = Sp + 3 * (size_t)(base + excl); o[0] = sx; o[1] = sy; o[2] = sz; }
+      base += agg;
+      __syncthreads();
+    }
+    ns = base;
+    if (ns == 0 && tid == 0) s_status = LM_TRACK_NO_DEPTH;
+    __syncthreads();
+  }
+  IcpJob* job = p.jobs + i;
+  if (s_status != LM_TRACK_TRACKED) {  // block-uniform
+    if (tid == 0) {
+      p.rec[i].status = s_status;
+      p.posed[i] = 0;
+      job->src_first = job->tgt_first = (int32_t)sm;
+      job->src_count = job->tgt_count = 0;
+      for (int k = 0; k < 16; ++k) job->init[k] = s_T[k];
+      p.seg_begin[2 * i] = p.seg_end[2 * i] = (int32_t)sm;
+      p.seg_begin[2 * i + 1] = p.seg_end[2 * i + 1] = (int32_t)ss;
+    }
+    return;
+  }
+  for (int c = 0; c < 6; ++c) {  // per-axis minima of both clouds (exact in any order)
+    const double* P = c < 3 ? Mp : Sp;
+    const int n = c < 3 ? nm : ns;
+    double v = INFINITY;
+    for (int j = tid; j < n; j += POSE_THREADS) v = fmin(v, P[3 * j + c % 3]);
+    v = Reduce(tmp.reduce).Reduce(v, cub::Min());
+    if (tid == 0) s_min[c] = v;
+    __syncthreads();
+  }
+  track_voxel_keys(Mp, nm, s_min, sm, p.keys, p.vals, p.err);
+  track_voxel_keys(Sp, ns, s_min + 3, ss, p.keys, p.vals, p.err);
+  if (tid == 0) {
+    p.rec[i].status = LM_TRACK_TRACKED;
+    p.posed[i] = 1;
+    for (int k = 0; k < 16; ++k) job->init[k] = s_T[k];
+    job->src_first = job->tgt_first = (int32_t)sm;
+    job->src_count = job->tgt_count = 0;  // k_pose_voxel sets the counts
+    p.seg_begin[2 * i] = (int32_t)sm; p.seg_end[2 * i] = (int32_t)sm + nm;
+    p.seg_begin[2 * i + 1] = (int32_t)ss; p.seg_end[2 * i + 1] = (int32_t)ss + ns;
+  }
+}
+
+// --------------------------------------------------------------------------------------------
 // LM_POSE_PSO (include/linemod_b200.h): a particle swarm over rotations about the cloud's centroid and translations,
 // scored against the scene depth with pose verification's projection
 // --------------------------------------------------------------------------------------------
@@ -1859,7 +2060,17 @@ struct lm_pose_stage {
     int slots = 0, rank = 0, world = 1;
     int64_t first = 0;
     const uint8_t* posed = nullptr;
+    bool track = false;  // a track chunk: d_trec holds its windows
   } last;
+  // tracking (pose_stage_track): the scene, the objects and their windows
+  DeviceArray<uint16_t> d_tscene;
+  DeviceArray<TrackObject> d_tobj;
+  DeviceArray<TrackRec> d_trec; PinnedArray<TrackRec> h_trec;
+  // the run last finished, for pose_stage_transforms: finished_ok false once another run is prepared or it failed; its
+  // entries' transformations, or (xf_pending, a run with the pose NMS) its frames' first survivors to find them from
+  bool finished_ok = false, xf_pending = false;
+  std::vector<double> xf;
+  std::vector<int64_t> finished_first;
 };
 
 // The per-chunk buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
@@ -2028,6 +2239,9 @@ struct PoseChunk {
   int32_t* corr_out = nullptr;
   long long* record = nullptr;
   int64_t record_words = 0;
+  // a track chunk (lm_track; null: survivors): k_track_cloud builds the clouds from these objects instead of
+  // k_pose_cloud; the stage's buffers, seg_begin / seg_end, jobs, err and posed are filled in by pose_chunk
+  const TrackParams* track = nullptr;
 };
 
 // k_pose_cloud, the segmented sort, k_pose_voxel, k_icp_normals (point-to-plane only) and the ICP kernel (or k_pose_pso,
@@ -2055,19 +2269,28 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   p.jobs = s->d_jobs.get(); p.err = c.status; p.posed = sh ? s->d_posed.get() : c.posed;
   p.frame_of = c.frame_of; p.sKs = c.sKs;
   p.rank = sh ? sh->rank : 0; p.world = world;
-  k_pose_cloud<<<n, POSE_THREADS, 0, st>>>(p);
+  int64_t items = 2 * n * A, tgt_max = A;  // points of the chunk's cloud slots, and of its largest target cloud
+  if (c.track) {
+    TrackParams q = *c.track;
+    q.raw = p.raw; q.keys = p.keys; q.vals = p.vals; q.seg_begin = p.seg_begin; q.seg_end = p.seg_end;
+    q.jobs = p.jobs; q.err = p.err; q.posed = p.posed;
+    items = n * q.stride; tgt_max = q.cap;
+    k_track_cloud<<<n, POSE_THREADS, 0, st>>>(q);
+  } else {
+    k_pose_cloud<<<n, POSE_THREADS, 0, st>>>(p);
+  }
   // stable (radix) sort of each slot's keys: ties keep the point order, as std::stable_sort
   cub::DoubleBuffer<unsigned long long> dk(s->d_keys[0].get(), s->d_keys[1].get());
   cub::DoubleBuffer<int32_t> dv(s->d_vals[0].get(), s->d_vals[1].get());
   size_t tmp_bytes = s->d_sort_tmp.size();
-  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp.get(), tmp_bytes, dk, dv, (int)(2 * n * A), 2 * n, p.seg_begin, p.seg_end, 0,
+  CUI(cub::DeviceSegmentedRadixSort::SortPairs(s->d_sort_tmp.get(), tmp_bytes, dk, dv, (int)items, 2 * n, p.seg_begin, p.seg_end, 0,
                                                3 * POSE_KEY_BITS, st));
   k_pose_voxel<<<2 * n, POSE_THREADS, 0, st>>>(dk.Current(), dv.Current(), p.seg_begin, p.seg_end, s->d_raw.get(), s->d_pts.get(), s->d_jobs.get(),
                                                p.use_scene);
   // the ICP kernels: empty jobs fall through
   const bool normals = o.estimation == LM_ICP_POINT_TO_PLANE;
   if (normals) {
-    dim3 g((unsigned)((A + 127) / 128), (unsigned)n);
+    dim3 g((unsigned)((tgt_max + 127) / 128), (unsigned)n);
     k_icp_normals<<<g, 128, 0, st>>>(s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), c.knn_out);
   }
   if (sh) {
@@ -2104,6 +2327,7 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   s->last.slots = n; s->last.rank = p.rank; s->last.world = world;
   s->last.first = c.first;
   s->last.posed = p.posed;
+  s->last.track = c.track != nullptr;
   return (sh ? 6 : 5) - (normals ? 0 : 1) + (o.verify.on ? 1 : 0);
 }
 
@@ -2126,9 +2350,20 @@ int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int
     if (slot < 0 || slot >= l.slots) return lm_fail(LM_E_INVALID, "slot %d outside the %d of the last chunk", slot, l.slots);
     if (what != LM_POSE_CAPTURE_POSED && what != LM_ICP_CAPTURE_COUNTS && what != LM_ICP_CAPTURE_SOURCE &&
         what != LM_ICP_CAPTURE_TARGET && what != LM_ICP_CAPTURE_INIT && what != LM_POSE_CAPTURE_RAW_MODEL &&
-        what != LM_POSE_CAPTURE_RAW_SCENE)
+        what != LM_POSE_CAPTURE_RAW_SCENE && what != LM_POSE_CAPTURE_WINDOW)
       return lm_fail(LM_E_INVALID, "unknown pose stage capture item %d", what);
+    if (what == LM_POSE_CAPTURE_WINDOW && !l.track) return lm_fail(LM_E_STATE, "the last chunk was not a track chunk (lm_track): no window");
     CUI(cudaMemcpy(&posed, l.posed + slot, 1, cudaMemcpyDeviceToHost));
+    if (what == LM_POSE_CAPTURE_WINDOW) {
+      TrackRec rec;
+      CUI(cudaMemcpy(&rec, s->d_trec.get() + slot, sizeof(rec), cudaMemcpyDeviceToHost));
+      const int32_t w5[5] = {rec.window[0], rec.window[1], rec.window[2], rec.window[3], rec.status};
+      if (cap < (int64_t)sizeof(w5))
+        return lm_fail(LM_E_CAPACITY, "pose stage capture item %d of slot %d needs %lld bytes, cap is %lld", what, slot, (long long)sizeof(w5),
+                       (long long)cap);
+      memcpy(out, w5, sizeof(w5));
+      return LM_OK;
+    }
     if (what == LM_POSE_CAPTURE_POSED) {
       src = &posed; bytes = 1;
     } else {
@@ -2206,6 +2441,7 @@ static int pose_outputs(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t
 // too).
 static int pose_prepare(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S, bool verify) {
   s->last.valid = false;
+  s->finished_ok = false;
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
@@ -2401,6 +2637,8 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
   const bool verify = r.o.verify.on != 0;
   s->verified = false;
   s->ver.clear();
+  s->finished_ok = s->xf_pending = false;
+  s->xf.clear();
   int64_t published = 0;
   int rc = pose_status(s->h_bstat.get(), batch ? pose_batch_chunks(S) : 1, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0,
                        batch, &published);
@@ -2458,14 +2696,19 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
       at += counts[4 * f];
     }
     s->verified = verify;
+    s->finished_first.assign(first, first + nf + 1);
+    s->finished_ok = s->xf_pending = true;
     return LM_OK;
   }
+  s->xf.assign(16 * (size_t)S, std::numeric_limits<double>::quiet_NaN());
   for (int64_t i = 0; i < S; ++i) {  // every survivor, frame after frame
     if (out) out[i] = surv[i];
     survivor_pose(*survivor_render(s, surv[i]), surv[i], r.o.srows, r.o.scols, s->h_bouts[i], R_out + 9 * i, t_out + 3 * i, residual + i);
+    if (residual[i] != -1.f) memcpy(s->xf.data() + 16 * i, s->h_bouts[i].T, sizeof(s->h_bouts[i].T));
   }
   if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + S);
   s->verified = verify;
+  s->finished_ok = true;
   return LM_OK;
 }
 
@@ -2957,4 +3200,144 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
   CUI(cudaEventRecord(h->ev_out.get(), st));
   CUI(cudaStreamWaitEvent(caller, h->ev_out.get(), 0));
   return rc;
+}
+
+// --------------------------------------------------------------------------------------------
+// tracking on the detector's pose stage (lm_track, lm_track_device) and the transformations of a finished run
+// --------------------------------------------------------------------------------------------
+int pose_track_scene(lm_pose_stage* s, cudaStream_t st, bool host, const void* depth, int64_t pitch, int format, float scale, int rows,
+                     int cols, const uint16_t** d_scene, int64_t* launches) {
+  const size_t npix = (size_t)rows * cols;
+  if (npix > s->d_tscene.size()) {
+    CUI(cudaStreamSynchronize(st));  // an earlier run may still read it
+    CUI(s->d_tscene.reserve(npix));
+  }
+  if (host) {
+    CUI(cudaMemcpyAsync(s->d_tscene.get(), depth, sizeof(uint16_t) * npix, cudaMemcpyHostToDevice, st));
+  } else {
+    k_icp_scene<<<dim3((unsigned)((cols + ICP_DEV_PX - 1) / ICP_DEV_PX), (unsigned)rows), ICP_DEV_PX, 0, st>>>(
+        static_cast<const uint8_t*>(depth), pitch, format == LM_DEPTH_F32 ? 1 : 0, scale, cols, s->d_tscene.get());
+    CUI(cudaGetLastError());
+    ++*launches;
+  }
+  *d_scene = s->d_tscene.get();
+  return LM_OK;
+}
+
+int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_scene, const float* sK, const TrackObject* obj, int n,
+                     int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual, int32_t* status,
+                     int32_t* box) {
+  cudaStream_t st = o.stream;
+  const bool verify = o.verify.on != 0;
+  int rc = pose_prepare(s, st, 1, n, verify);
+  s->verified = false;
+  s->ver.clear();
+  s->xf.clear();
+  s->xf_pending = false;
+  if (rc) return rc;
+  if (n == 0) {
+    s->verified = verify;
+    s->finished_ok = true;
+    return LM_OK;
+  }
+  // object i's clouds: M model points (the largest crop), then a window of up to 4 M scene points
+  const int64_t M = s->area_max, W = 4 * M, stride = M + W;
+  rc = pose_buffers(s, st, (int)((n * stride + 2 * M - 1) / (2 * M)), M);
+  if (rc) return rc;
+  if ((size_t)n > s->h_trec.size()) {
+    CUI(cudaStreamSynchronize(st));
+    s->d_tobj.reset(); s->d_trec.reset(); s->h_trec.reset();
+    CUI(s->d_tobj.assign(n));
+    CUI(s->d_trec.assign(n));
+    CUI(s->h_trec.assign(n));
+  }
+  CUI(cudaMemcpyAsync(s->d_tobj.get(), obj, sizeof(TrackObject) * n, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4, st));
+  TrackParams q;
+  memset(&q, 0, sizeof(q));
+  q.obj = s->d_tobj.get(); q.tpl = s->d_tpl.get(); q.crops = s->d_crops.get();
+  q.sc.depth = d_scene; q.sc.rows = o.srows; q.sc.cols = o.scols;
+  q.sc.fx = sK[0]; q.sc.cx = sK[2]; q.sc.fy = sK[4]; q.sc.cy = sK[5];
+  q.margin = margin; q.cap = W; q.stride = stride; q.M = M;
+  q.rec = s->d_trec.get();
+  PoseChunk k;
+  k.table = {s->d_tpl.get(), s->d_crops.get(), s->d_class_begin.get(), (int32_t)s->class_begin.size() - 1, (int32_t)s->tpl.size()};
+  k.surv = nullptr; k.counts = nullptr; k.slots = n; k.first = 0;
+  k.scene = d_scene; k.frame_of = nullptr; k.sKs = nullptr; k.sK = sK; k.frame_first = nullptr;
+  k.outs = s->d_bouts.get(); k.posed = s->d_bposed.get(); k.ver = s->d_bver.get(); k.status = s->d_bstat.get(); k.seq = 0;
+  k.track = &q;
+  const int l = pose_chunk(s, o, k);
+  if (l < 0) return l;
+  *launches += l;
+  CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_trec.get(), s->d_trec.get(), sizeof(TrackRec) * n, cudaMemcpyDeviceToHost, st));
+  if (verify) CUI(cudaMemcpyAsync(s->h_bver.get(), s->d_bver.get(), sizeof(PoseVerify) * n, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+  CUI(cudaStreamSynchronize(st));
+  CUI(cudaGetLastError());
+  int64_t published = 0;
+  rc = pose_status(s->h_bstat.get(), 1, false, 0, 0, false, &published);
+  if (rc) return rc;
+  s->xf.assign(16 * (size_t)n, std::numeric_limits<double>::quiet_NaN());
+  for (int i = 0; i < n; ++i) {
+    const TrackRec& e = s->h_trec[(size_t)i];
+    status[i] = e.status;
+    memcpy(box + 4 * i, e.box, sizeof(e.box));
+    if (e.status != LM_TRACK_TRACKED) { residual[i] = -1.f; continue; }
+    const IcpOut& q = s->h_bouts[(size_t)i];
+    const TplHost& h = s->tpl[(size_t)obj[i].g];
+    float base[16];
+    init_base(h.R, h.t, base);
+    compose(q.T, base, R_out + 9 * i, t_out + 3 * i);
+    memcpy(T_out + 16 * i, q.T, sizeof(q.T));
+    memcpy(s->xf.data() + 16 * i, q.T, sizeof(q.T));
+    residual[i] = (float)q.fitness;
+  }
+  if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + n);
+  s->verified = verify;
+  s->finished_ok = true;
+  return LM_OK;
+}
+
+int pose_stage_transforms(lm_pose_stage* s, double* T_out, int64_t cap, int64_t* n) {
+  if (!n || (cap > 0 && !T_out)) return lm_fail(LM_E_INVALID, "null argument");
+  if (!s->finished_ok) return lm_fail(LM_E_STATE, "no pose run has finished since the last one was enqueued (or it failed)");
+  if (s->xf_pending) {  // the pose NMS's kept entries: matched to their survivors by their composed pose
+    const PoseRun& r = s->run;
+    const std::vector<int64_t>& first = s->finished_first;
+    s->xf.clear();
+    const int nf = (int)first.size() - 1;
+    const int64_t S = first[(size_t)nf];
+    cudaStream_t st = r.o.stream;
+    std::vector<IcpOut> outs((size_t)S);
+    std::vector<uint8_t> posed((size_t)S);
+    if (S) {
+      CUI(cudaMemcpyAsync(outs.data(), s->d_bouts.get(), sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
+      CUI(cudaMemcpyAsync(posed.data(), s->d_bposed.get(), S, cudaMemcpyDeviceToHost, st));
+      CUI(cudaStreamSynchronize(st));
+    }
+    const PoseNmsHead* heads = nms_heads(s->h_bnms.get());
+    const PoseNmsOut* entries = nms_out(s->h_bnms.get(), nf);
+    for (int f = 0; f < nf; ++f)
+      for (int64_t k = 0; k < heads[f].kept; ++k) {
+        const PoseNmsOut& e = entries[first[(size_t)f] + k];
+        const TplHost* h = survivor_render(s, e.m);
+        int64_t got = -1;
+        for (int64_t i = first[(size_t)f]; h && got < 0 && i < first[(size_t)f + 1]; ++i) {
+          if (!posed[(size_t)i] || (float)outs[(size_t)i].fitness != e.residual) continue;
+          double R[9], t[3];
+          float base[16];
+          init_base(h->R, h->t, base);
+          compose(outs[(size_t)i].T, base, R, t);
+          if (!memcmp(R, e.R, sizeof(R)) && !memcmp(t, e.t, sizeof(t))) got = i;
+        }
+        if (got < 0) return lm_fail(LM_E_STATE, "frame %d, kept pose %lld: no survivor composes to it", f, (long long)k);
+        s->xf.insert(s->xf.end(), outs[(size_t)got].T, outs[(size_t)got].T + 16);
+      }
+    s->xf_pending = false;
+  }
+  *n = (int64_t)s->xf.size() / 16;
+  if (*n > cap) return lm_fail(LM_E_CAPACITY, "%lld entries, capacity %lld", (long long)*n, (long long)cap);
+  if (*n) memcpy(T_out, s->xf.data(), sizeof(double) * s->xf.size());
+  return LM_OK;
 }

@@ -8,7 +8,8 @@
 // of frames, and a single frame is a one-frame run of the same stage: the same chunks, outputs, readbacks and finish.
 // The host composes result = T * init_base after the copy.  The pose NMS (k_pose_nms, one CTA per frame behind the ICP
 // kernel) composes the poses on the device instead, runs the greedy translation NMS of linemod_ros/detect.py over them
-// and compacts the kept ones into one output block.
+// and compacts the kept ones into one output block.  A track run (lm_track) is one chunk whose clouds k_track_cloud builds
+// from each object's transformation and the window its model projects to, in place of k_pose_cloud.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -118,6 +119,29 @@ int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, in
 // Slot `slot`'s item `what` of the last chunk enqueued (lm_debug_pose_clouds), after the caller has synchronised the
 // stream.  Launches nothing.
 int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int64_t cap);
+
+// Tracking (lm_track, include/linemod_b200.h): object i of a track run starts from T at template g of the bank, whose
+// render is registered.
+struct TrackObject {
+  int64_t g;
+  double T[16];
+};
+// The scene of a track run on o.stream: rows x cols u16 mm in the stage's own buffer.  host: depth is a host image,
+// copied; else a caller's device plane (pitch bytes between rows, LM_DEPTH_U16_MM or LM_DEPTH_F32 with scale),
+// converted as lm_bind_images_device converts it.
+int pose_track_scene(lm_pose_stage* s, cudaStream_t st, bool host, const void* depth, int64_t pitch, int format, float scale, int rows,
+                     int cols, const uint16_t** d_scene, int64_t* launches);
+// One track run of n <= 1024 objects against the scene of pose_track_scene, o.estimation an ICP: one chunk, then the
+// outputs of lm_track (an entry without the status TRACKED leaves its T, R, t untouched and gets residual -1).  Returns
+// once they are on the host; the run is then the stage's last finished run (pose_stage_verify, pose_stage_transforms).
+int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_scene, const float* sK, const TrackObject* obj, int n,
+                     int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual, int32_t* status,
+                     int32_t* box);
+// The transformation of every entry of the run last finished (lm_pose_transforms), in entry order, T_out + 16k; NaN for an
+// entry without a pose.  LM_E_STATE once another run has been enqueued or the last one failed; LM_E_CAPACITY (with *n)
+// beyond cap.  The pose NMS's kept entries are matched to their survivors on the host, from one copy of the run's ICP
+// outputs and survivors.
+int pose_stage_transforms(lm_pose_stage* s, double* T_out, int64_t cap, int64_t* n);
 
 // A batch's scene and survivor slots: room for n_frames scene depths of frame_pixels each (frame f at d_scene + f *
 // frame_pixels) and max_surv survivors, which the caller fills on the stream.  It also uploads the renders and grows

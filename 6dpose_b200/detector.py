@@ -69,6 +69,7 @@ class Detector:
         self._peers = None  # (rank, world) once dist.connect_peers has wired the fused exchange
         self._verify = _lib.verify_options(None)  # lm_set_pose_verify's arguments (setPoseVerification)
         self._search = _lib.pose_search_options()  # lm_set_pose_search's arguments (setPoseSearch)
+        self._render_poses = {}  # class_id -> (R [n,3,3], t [n,3]) f32 of its registered renders (track's dict starts)
         self.device = _default_device()
         self.shard = (0, 1)  # (index, count): template shard matched by this process (multi-GPU)
         self.shard_layout = _lib.SHARD_CONTIGUOUS
@@ -295,6 +296,7 @@ class Detector:
                 got += len(chunk)
             if got != n:
                 raise ValueError("class %s: %d renders for %d templates" % (cid, got, n))
+            self._render_poses[cid] = (R.copy(), t.copy())
             first += n
 
     def setPoseVerification(self, inlier_mm=10.0, rank_by="fitness", min_score=None):
@@ -348,7 +350,7 @@ class Detector:
         nat = self._pose_native(class_ids)
         out, R, t, res, _ = nat.match_pose(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold),
                                            int(top_k), int(max_iterations), bool(use_scene_cloud), estimation)
-        return self._pose_pairs(out, R, t, res, self._verification(nat, [len(out)])[0])
+        return self._pose_pairs(out, R, t, res, self._verification(nat, [len(out)])[0], nat.pose_transforms())
 
     def detect(self, sources, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
                max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
@@ -366,7 +368,8 @@ class Detector:
         nat = self._pose_native(class_ids)
         out, R, t, res, _ = nat.detect(sources[0], sources[1], list(masks), float(threshold), sK, float(iou_threshold), int(top_k),
                                        int(max_iterations), bool(use_scene_cloud), float(translation_threshold), estimation)
-        return self._pose_pairs(out, R, t, res, self._verification(nat, [len(out)])[0])  # every kept pose has one: residual >= 0
+        # every kept pose has one: residual >= 0
+        return self._pose_pairs(out, R, t, res, self._verification(nat, [len(out)])[0], nat.pose_transforms())
 
     # ---- a batch of RGB-D frames through one pose stage (lm_detect_batch) ----
     def match_refine_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, top_k=3, max_iterations=30,
@@ -385,7 +388,7 @@ class Detector:
         call, inputs = (nat.detect_batch_device, (inputs,)) if isinstance(inputs, _lib.DeviceBatch) else (nat.detect_batch, inputs)
         got = call(*inputs, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations), bool(use_scene_cloud),
                    pose_nms=False, estimation=estimation)
-        return self._batch_pairs(nat, got)
+        return self._batch_pairs(nat, got, transforms=True)
 
     def detect_batch(self, frames, threshold, class_ids, sceneK, iou_threshold=0.5, translation_threshold=40.0, top_k=0,
                      max_iterations=30, use_scene_cloud=False, masks=[], estimation="point_to_plane", depth_scale=1.0, stream=None):
@@ -398,12 +401,17 @@ class Detector:
         call, inputs = (nat.detect_batch_device, (inputs,)) if isinstance(inputs, _lib.DeviceBatch) else (nat.detect_batch, inputs)
         got = call(*inputs, float(threshold), K, float(iou_threshold), int(top_k), int(max_iterations), bool(use_scene_cloud),
                    pose_nms=True, translation_threshold=float(translation_threshold), estimation=estimation)
-        return self._batch_pairs(nat, got)
+        return self._batch_pairs(nat, got, transforms=True)
 
-    def _batch_pairs(self, nat, got):
-        # one [(Match, poseRefine)] list per frame of a batch call's result
-        ver = self._verification(nat, [len(g[0]) for g in got])
-        return [self._pose_pairs(out, R, t, res, v) for (out, R, t, res, _), v in zip(got, ver)]
+    def _batch_pairs(self, nat, got, transforms=False):
+        # one [(Match, poseRefine)] list per frame of a batch call's result; transforms: with each pose's T
+        # (lm_pose_transforms)
+        sizes = [len(g[0]) for g in got]
+        ver = self._verification(nat, sizes)
+        T = nat.pose_transforms() if transforms else None
+        starts = np.cumsum([0] + sizes)
+        return [self._pose_pairs(out, R, t, res, v, None if T is None else T[a:b])
+                for (out, R, t, res, _), v, a, b in zip(got, ver, starts[:-1], starts[1:])]
 
     def _batch_args(self, frames, class_ids, sceneK, masks, what):
         # the sharded batch calls (dist.py), which take numpy frames: the handle, then (rgb, depth, mask pairs, K)
@@ -463,9 +471,9 @@ class Detector:
                 raise ValueError("%s: %s" % (what, e)) from None
         return (np.stack(rgb), np.stack(depth), pairs), K
 
-    def _pose_pairs(self, out, R, t, res, ver=None):
+    def _pose_pairs(self, out, R, t, res, ver=None, T=None):
         # [(Match, poseRefine)]; a survivor without a pose (residual -1, only without the pose NMS) keeps R / t None.
-        # ver: per entry (score, counts) of the pose verification, or None
+        # ver: per entry (score, counts) of the pose verification, or None; T: per entry its transformation, or None
         from .pose_refine import poseRefine
         pairs = []
         for i, m in enumerate(self._to_matches(out)):
@@ -476,7 +484,92 @@ class Detector:
             if res[i] != -1.0:
                 p._R = R[i].copy()
                 p._t = t[i].reshape(3, 1).copy()
+                if T is not None:
+                    p._T = T[i].copy()
             pairs.append((m, p))
+        return pairs
+
+    # ---- tracking (include/linemod_b200.h, lm_track / lm_track_device) ----
+    def track(self, depth, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane", depth_scale=1.0, stream=None):
+        """Refine each object's last pose against a new depth frame, with no match: the ICP starts from the object's T and
+        registers its template's model cloud against the scene pixels of the window the model projects to (its projected
+        box grown by margin_px).  Not in the reference, whose live loop detects again on every frame (linemod_ros/
+        detect.py:167-168).  depth: a uint16 HxW numpy image (mm), or a CUDA tensor as in match (uint16 mm, or float32
+        scaled by depth_scale, read in order on `stream`).  objects: (Match, poseRefine) pairs of match_refine, detect,
+        the batch calls or track itself, and/or dicts {class_id, template_id, R, t (mm)} converted to T with the
+        template's registered pose (include/linemod_b200.h).  estimation: "point_to_plane" or "point_to_point".
+        Returns [(Match, poseRefine)], one per object in order: Match.x / .y the projected box's top-left, similarity
+        carried over (0.0 for a dict); poseRefine.getTrackStatus() "tracked", "outside", "window" or "no_depth", the
+        last three with residual -1 and the start's R, t and T.  With setPoseVerification, every entry carries its score.
+        TypeError for a pair whose poseRefine has no transformation (refine_matches / process), ValueError for an unknown
+        class or template; both before any device work."""
+        from .pose_refine import poseRefine, pose_to_transform
+        _lib.estimation_code(estimation)
+        objects = list(objects)
+        if len(objects) > _lib.TRACK_MAX:
+            raise ValueError("track: %d objects, at most %d per call" % (len(objects), _lib.TRACK_MAX))
+        order = self.bank.class_ids()
+        index = {c: i for i, c in enumerate(order)}
+        starts = []  # (class_index, template_id, T, Match, R, t)
+        for k, o in enumerate(objects):
+            if isinstance(o, dict):
+                cid, tid = o["class_id"], int(o["template_id"])
+                m, R, t = Match(0, 0, 0.0, cid, tid), np.asarray(o["R"], np.float64).reshape(3, 3), np.asarray(o["t"], np.float64).reshape(3)
+                T = None
+            else:
+                m, p = o
+                cid, tid = m.class_id, int(m.template_id)
+                T = p.getTransformation() if isinstance(p, poseRefine) else None
+                if T is None:
+                    raise TypeError("track: object %d's poseRefine has no transformation (only match_refine, detect, the batch calls "
+                                    "and track return one)" % k)
+                R, t = p.getR(), p.getT()
+            if cid not in index:
+                raise ValueError("track: object %d: class %r is not in the bank" % (k, cid))
+            if not 0 <= tid < self.bank.num_templates(cid):
+                raise ValueError("track: object %d: template %d outside class %r's %d templates" % (k, tid, cid, self.bank.num_templates(cid)))
+            if T is None:
+                if cid not in self._render_poses:
+                    raise ValueError("track: object %d: class %r has no registered renders (setTemplateRenders)" % (k, cid))
+                Rb, tb = self._render_poses[cid]
+                T = pose_to_transform(R, t, Rb[tid], tb[tid])
+            starts.append((index[cid], tid, np.asarray(T, np.float64).reshape(4, 4), m, R, t))
+        sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
+        triples = [(c, t, T) for c, t, T, _, _, _ in starts]
+        if _lib.is_tensor(depth):
+            import torch
+            ptr, pitch, fmt = _lib._depth_plane(depth, "depth", torch)
+            scale = _lib._plane_scale(fmt == _lib.DEPTH_F32, depth_scale, "depth_scale", "depth")
+            if not depth.is_cuda or depth.device.index != int(self.device):
+                raise ValueError("depth is on %s; the detector runs on cuda:%d" % (depth.device, int(self.device)))
+            st = _lib.device_stream(stream, self.device)
+            nat = self._pose_native(())
+            got = nat.track_device(ptr, pitch, fmt, scale, int(depth.shape[0]), int(depth.shape[1]), st.cuda_stream, sK, triples,
+                                   max_iterations, margin_px, estimation)
+        else:
+            _lib.host_frame_options(depth_scale, stream)
+            depth = np.asarray(depth)
+            if depth.dtype != np.uint16 or depth.ndim != 2:
+                raise TypeError("depth must be a uint16 HxW depth image (mm)")
+            nat = self._pose_native(())
+            got = nat.track(depth, sK, triples, max_iterations, margin_px, estimation)
+        status, T, R, t, res, box = got
+        ver = self._verification(nat, [len(starts)])[0]
+        pairs = []
+        for i, (_, tid, T0, m0, R0, t0) in enumerate(starts):
+            p = poseRefine(estimation)
+            p._track_status = _lib.TRACK_STATUS[int(status[i])]
+            p._residual = float(res[i])
+            if ver is not None:
+                p._score, p._verification = ver[i]
+            x, y = (int(box[i, 0]), int(box[i, 1])) if status[i] != 1 else (m0.x, m0.y)
+            if status[i] == 0:
+                p._R, p._t, p._T = R[i].copy(), t[i].reshape(3, 1).copy(), T[i].copy()
+            else:
+                p._R = None if R0 is None else np.asarray(R0, np.float64).reshape(3, 3).copy()
+                p._t = None if t0 is None else np.asarray(t0, np.float64).reshape(3, 1).copy()
+                p._T = T0.copy()
+            pairs.append((Match(x, y, m0.similarity, m0.class_id, tid), p))
         return pairs
 
     def _to_matches(self, out):

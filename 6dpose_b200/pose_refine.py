@@ -37,6 +37,8 @@ class poseRefine:
         self._t = None
         self._score = None         # pose verification (verify_mm, Detector.setPoseVerification): score, counts
         self._verification = None
+        self._T = None             # the ICP's 4x4 transformation (Detector's pose calls and track)
+        self._track_status = None  # Detector.track's status
         self.device = _default_device()
 
     @staticmethod
@@ -107,6 +109,18 @@ class poseRefine:
         -1 without a pose; None when the call did not verify."""
         return self._score
 
+    def getTransformation(self):
+        """The ICP's 4x4 transformation T (f64, row-major), which maps the template's render cloud into the scene camera
+        (include/linemod_b200.h, lm_track): what Detector.track starts the next frame from.  None when the pose did not
+        come from Detector's match_refine, detect, batch calls or track, or has none."""
+        return self._T
+
+    def getTrackStatus(self):
+        """Detector.track's status of this pose: "tracked", "outside" (no model point lands in the frame), "window" (the
+        window exceeds the scene slot) or "no_depth" (no scene depth in the window); None when it did not come from
+        track."""
+        return self._track_status
+
     def getVerification(self):
         """The pose verification's counts, a dict of n_model, outside, missing, inlier, occluded and violation (the last five
         sum to n_model); None when the call did not verify."""
@@ -162,6 +176,24 @@ def refine_matches(sceneDepth, sceneK, matches, modelDepths, modelKs, modelRs, m
             p._R = Ro[i].copy()
             p._t = to[i].reshape(3, 1).copy()
     return out
+
+
+def pose_to_transform(R, t, R_b, t_b):
+    """The transformation T (4x4 f64) of a pose (R [3,3], t [3] mm, as getR / getT return it) of a template whose render
+    was made at (R_b, t_b) (f32, t_b mm), in the order include/linemod_b200.h states (lm_track): T_R = R R_b^T, T_t = t /
+    1000 - T_R b with b = (t_b.x, t_b.y, t_b.z / 1000 in float32).  Every operation is one correctly rounded float64
+    operation."""
+    R = np.asarray(R, np.float64).reshape(3, 3)
+    t = np.asarray(t, np.float64).reshape(3)
+    Rb = np.asarray(R_b, np.float32).reshape(3, 3).astype(np.float64)
+    tb = np.asarray(t_b, np.float32).reshape(3)
+    b = [float(tb[0]), float(tb[1]), float(tb[2] / np.float32(1000.0))]
+    T = np.eye(4)
+    for r in range(3):
+        for c in range(3):
+            T[r, c] = ((float(R[r, 0]) * float(Rb[c, 0])) + float(R[r, 1]) * float(Rb[c, 1])) + float(R[r, 2]) * float(Rb[c, 2])
+        T[r, 3] = float(t[r]) / 1000.0 - (((T[r, 0] * b[0]) + T[r, 1] * b[1]) + T[r, 2] * b[2])
+    return T
 
 
 def nms_translations(ts, scores, thr, device=None):

@@ -471,6 +471,71 @@ int lm_pose_verify(lm_detector* d, float* score, int32_t* counts6, int64_t cap, 
 int lm_pose_verify_points(int device, const double* pts, int64_t n, const double* T, const uint16_t* scene, int rows, int cols,
                           const float* sK, double inlier_mm, int32_t* counts6, float* score);
 
+/* Tracking on the device: detect once, then refine each object's last pose against the next frame's depth, with no match,
+ * box NMS or pose NMS.  A new capability, not a port: the reference's live loop (linemod_ros/detect.py:167-168) runs the
+ * whole detection on every frame.  A tracked object is (class index, template id within the class, T):
+ *   T        the ICP's 4x4 transformation, row-major f64, which maps the template's render cloud (metres, the template's
+ *            camera) into the scene camera: the T of LM_ICP_CAPTURE_RESULT and of verification's step 2, and what
+ *            lm_pose_transforms returns for the entries of lm_complete_pose, lm_complete_detect, the batch calls and
+ *            lm_track.  A caller holding only a pose (R, t mm) as lm_complete_pose returns it converts it with the
+ *            template's registered R_b, t_b (init_base, LL.cpp:34-38: b = (t_b.x, t_b.y, (float)(t_b.z / 1000.0f)), each
+ *            widened to double), every operation correctly rounded, no FMA, in this order:
+ *              T_R[r][c] = ((R[r][0] * R_b[c][0]) + R[r][1] * R_b[c][1]) + R[r][2] * R_b[c][2]      (R R_b^T)
+ *              T_t[r]    = t[r] / 1000 - (((T_R[r][0] * b_0) + T_R[r][1] * b_1) + T_R[r][2] * b_2)
+ *            with row 3 = (0, 0, 0, 1).  T * init_base then gives (R, t) back up to rounding; bit for bit only for a T
+ *            that came from the device.
+ * Each object of a call is one slot of one pose-stage chunk (n <= 1024):
+ *   1. Model cloud: exactly the pose stage's source cloud for that template -- its registered crop back-projected
+ *      (LM_POSE_CAPTURE_RAW_MODEL) and voxel down-sampled -- bit-identical to what a detected survivor of the template gets.
+ *   2. Window: every raw model point projected under T with verification's step 3, operation for operation; the
+ *      min / max column and row of the points that land in the frame in front of the camera are the projected box
+ *      (x, y, w, h), unclipped by the margin.  The window is that box grown by margin_px on each side and clipped to the
+ *      frame.  No point in the frame: LM_TRACK_OUTSIDE.  A window of more than 4 A pixels, A the largest registered crop:
+ *      LM_TRACK_WINDOW (the scene slot holds 4 A points, so an object may roughly double its image size between frames).
+ *   3. Scene cloud: every window pixel with depth > 0, row-major, back-projected with sceneK as the pose stage
+ *      back-projects scene pixels, and voxel down-sampled as the scene cloud is.  No such pixel: LM_TRACK_NO_DEPTH.
+ *      Tracking always registers against the scene (the reference's model-against-itself target would leave T where it
+ *      started), so use_scene_cloud plays no part.
+ *   4. Refinement: the ICP of lm_set_pose_estimation (k_icp_normals + k_icp_point_to_plane, or k_icp_point_to_point)
+ *      from IcpJob::init = T, with max_iterations.
+ *   5. Outputs, entry i for object i: status[i] (LM_TRACK_*); box + 4i the projected box (zeros when OUTSIDE); for
+ *      TRACKED: T_out + 16i the new T, R_out + 9i / t_out + 3i (mm) composed exactly as lm_complete_pose composes them,
+ *      residual[i] the fitness.  Any other status: residual -1, and T, R and t left untouched.
+ *   6. Verification: with lm_set_pose_verify on, k_pose_verify scores every tracked pose, and lm_pose_verify returns the
+ *      scores in entry order (-1 for an entry not tracked).  Nothing is dropped; lm_nms_translations is the caller's.
+ * Refusals, before any device work: LM_E_INVALID for a null argument, n < 0 or n > 1024, an empty image, max_iterations
+ * < 0, margin_px < 0, an unknown depth format or a bad depth_scale, a class or template out of range, a non-finite entry
+ * of T; LM_E_STATE for LM_POSE_PSO (its kernel starts from an identity rotation), a connected peer exchange, or an object
+ * whose template has no registered render (and on a host-only handle); LM_E_CAPACITY as the pose stage's buffers.
+ * A call runs on the detector's stream and returns once the outputs are on the host; it abandons a frame whose pose stage
+ * is pending.  lm_debug_pose_clouds then describes its chunk: slot i is object i, POSED is 1 for TRACKED, INIT is T,
+ * and LM_POSE_CAPTURE_WINDOW gives the window and status.  Launches: 5 (point-to-plane) or 4, plus 1 when verifying, plus
+ * 1 for lm_track_device's conversion.
+ *   lm_track          depth: rows x cols u16 mm on the host, copied.
+ *   lm_track_device   depth: a pitched device plane, LM_DEPTH_U16_MM or LM_DEPTH_F32 with depth_scale, converted as
+ *                     lm_bind_images_device converts it and ordered as it orders the frame: an event on `stream` gates the
+ *                     read, and `stream` waits on a second event once the conversion is done.
+ *   lm_pose_transforms  T_out + 16k: the T of entry k of the pose run last finished (lm_complete_pose, lm_complete_detect
+ *                     (its kept poses), the batch calls, lm_track), in entry order; NaN for an entry without a pose;
+ *                     *n their number.  The pose NMS's outputs are unchanged: its kept poses are matched to their
+ *                     survivors on the host, from one copy of the run's ICP outputs.  LM_E_STATE once another run has
+ *                     started or when the last one failed; LM_E_CAPACITY (with *n) when cap is smaller. */
+#define LM_TRACK_TRACKED 0
+#define LM_TRACK_OUTSIDE 1
+#define LM_TRACK_WINDOW 2
+#define LM_TRACK_NO_DEPTH 3
+typedef struct lm_track_object {
+  int32_t class_index, template_id;
+  double T[16];
+} lm_track_object;
+int lm_track(lm_detector* d, const uint16_t* depth, int rows, int cols, const float* sceneK, const lm_track_object* objects, int n,
+             int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out, float* residual, int32_t* status,
+             int32_t* box);
+int lm_track_device(lm_detector* d, const void* depth, int64_t depth_pitch, int depth_format, float depth_scale, int rows, int cols,
+                    const float* sceneK, const lm_track_object* objects, int n, int max_iterations, int margin_px, double* T_out,
+                    double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box, void* stream);
+int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n);
+
 /* A batch of RGB-D frames in one call: each frame's match and box NMS, then one pose stage and (pose_nms) one pose NMS
  * for the survivors of every frame.  Frame f is rgb + f * rows * cols * 3 and depth + f * rows * cols (all frames one
  * size), masks[2f] / masks[2f + 1] its colour and depth masks (masks NULL: none), sceneK + 9f its intrinsics.  The other
@@ -648,6 +713,8 @@ int lm_debug_coarse(lm_detector* d, uint32_t* mask, int64_t mask_cap, uint16_t* 
  *   LM_ICP_CAPTURE_INIT        initial guess, 16 f64 row-major
  *   LM_POSE_CAPTURE_RAW_MODEL  the model cloud before down-sampling (what k_pose_verify reads), row-major pixel order
  *   LM_POSE_CAPTURE_RAW_SCENE  the scene cloud before down-sampling (empty without use_scene_cloud)
+ *   LM_POSE_CAPTURE_WINDOW     5 int32, a track chunk only (lm_track; LM_E_STATE otherwise): the window x, y, w, h and
+ *                              the status, for every slot
  * LM_E_STATE before any pose stage has run (and after a later one failed before it enqueued a chunk), and for every
  * item but POSED of a slot without a pose; LM_E_CAPACITY when cap is too small; LM_E_INVALID for a slot outside the chunk or an
  * item not listed.  Describes the last chunk only, until the next pose stage is enqueued. */
@@ -655,6 +722,7 @@ int lm_debug_coarse(lm_detector* d, uint32_t* mask, int64_t mask_cap, uint16_t* 
 #define LM_POSE_CAPTURE_POSED 10
 #define LM_POSE_CAPTURE_RAW_MODEL 11
 #define LM_POSE_CAPTURE_RAW_SCENE 12
+#define LM_POSE_CAPTURE_WINDOW 14
 int lm_debug_pose_clouds(lm_detector* d, int slot, int what, void* out, int64_t cap);
 /* Counters of the last lm_run: [0] templates scanned, [1] coarse candidates, [2] algorithmic bytes of
  * the coarse scan (sum over templates, modalities of features x positions; SURVEY 8d),
