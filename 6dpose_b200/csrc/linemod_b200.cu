@@ -315,12 +315,8 @@ extern "C" int lm_create(int device, int n_levels, const int* T, lm_detector** o
     *out = d;
     return LM_OK;
   }
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
-  CU(cudaSetDevice(device));
+  const int rc = open_device(device);
+  if (rc) return rc;
   std::unique_ptr<lm_detector> d(new lm_detector());
   d->device = device;
   d->L = n_levels;
@@ -1278,13 +1274,40 @@ int check_device_stream(int device, cudaStream_t stream) {
   return LM_OK;
 }
 
+// The argument checks the detector, the ICP handle and the standalone entry points share (lm_pose.h).
+int check_depth_format(const char* what, int format, float scale) {
+  if (format != LM_DEPTH_U16_MM && format != LM_DEPTH_F32)
+    return fail(LM_E_INVALID, "%s: unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", what, format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
+  if (format == LM_DEPTH_F32 && !(std::isfinite(scale) && scale > 0.f))
+    return fail(LM_E_INVALID, "%s: scale %g: float depth needs a finite scale > 0", what, (double)scale);
+  return LM_OK;
+}
+
+int check_estimation(int estimation) {
+  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT && estimation != LM_POSE_PSO)
+    return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1, LM_POSE_PSO 3)", estimation);
+  return LM_OK;
+}
+
+int check_inlier_mm(double inlier_mm) {
+  if (!(std::isfinite(inlier_mm) && inlier_mm >= 0.0)) return fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
+  return LM_OK;
+}
+
+int open_device(int device) {
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
+  CU(cudaSetDevice(device));
+  return LM_OK;
+}
+
 static int check_device_frame(lm_detector* d, const DeviceFrame& f, int rows, int cols, cudaStream_t stream, int* lrows, int* lcols) {
   int rc = check_device_stream(d->device, stream);
+  if (!rc) rc = check_depth_format("depth", f.format, f.scale);
   if (rc) return rc;
-  if (f.format != LM_DEPTH_U16_MM && f.format != LM_DEPTH_F32)
-    return fail(LM_E_INVALID, "unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", f.format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
-  if (f.format == LM_DEPTH_F32 && !(std::isfinite(f.scale) && f.scale > 0.f))
-    return fail(LM_E_INVALID, "depth_scale %g: float depth needs a finite scale > 0", (double)f.scale);
   rc = fe_dims(d, rows, cols, lrows, lcols);
   if (rc) return rc;
   const int esize = f.format == LM_DEPTH_F32 ? 4 : 2;
@@ -2393,8 +2416,8 @@ extern "C" int lm_complete_detect(lm_detector* d, lm_match* out, double* R_out, 
 
 extern "C" int lm_set_pose_estimation(lm_detector* d, int estimation) {
   if (!d) return fail(LM_E_INVALID, "null detector");
-  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT && estimation != LM_POSE_PSO)
-    return fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1, LM_POSE_PSO 3)", estimation);
+  const int rc = check_estimation(estimation);
+  if (rc) return rc;
   d->pose_estimation = estimation;
   return LM_OK;
 }
@@ -2407,7 +2430,8 @@ extern "C" int lm_set_pose_search(lm_detector* d, int particles, int iterations,
 
 extern "C" int lm_set_pose_verify(lm_detector* d, int on, double inlier_mm, int rank_by, double min_score) {
   if (!d) return fail(LM_E_INVALID, "null detector");
-  if (!(std::isfinite(inlier_mm) && inlier_mm >= 0.0)) return fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
+  const int rc = check_inlier_mm(inlier_mm);
+  if (rc) return rc;
   if (rank_by != LM_VERIFY_RANK_FITNESS && rank_by != LM_VERIFY_RANK_SCORE)
     return fail(LM_E_INVALID, "unknown rank_by %d (LM_VERIFY_RANK_FITNESS 0, LM_VERIFY_RANK_SCORE 1)", rank_by);
   if (std::isnan(min_score)) return fail(LM_E_INVALID, "min_score is NaN (-INFINITY: no minimum)");
@@ -2443,10 +2467,8 @@ static int track(lm_detector* d, const void* depth, const DeviceFrame* dev, cuda
   if (rows <= 0 || cols <= 0) return fail(LM_E_INVALID, "empty depth image %d x %d", rows, cols);
   if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
   if (margin_px < 0) return fail(LM_E_INVALID, "margin_px %d < 0", margin_px);
-  if (dev && dev->format != LM_DEPTH_U16_MM && dev->format != LM_DEPTH_F32)
-    return fail(LM_E_INVALID, "unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", dev->format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
-  if (dev && dev->format == LM_DEPTH_F32 && !(std::isfinite(dev->scale) && dev->scale > 0.f))
-    return fail(LM_E_INVALID, "depth_scale %g: float depth needs a finite scale > 0", (double)dev->scale);
+  int rc = dev ? check_depth_format("depth", dev->format, dev->scale) : LM_OK;
+  if (rc) return rc;
   if (d->pose_estimation == LM_POSE_PSO)
     return fail(LM_E_STATE, "tracking runs an ICP: LM_POSE_PSO starts from an identity rotation (lm_set_pose_estimation)");
   if (d->px_rank >= 0) return fail(LM_E_STATE, "tracking does not run with a connected peer exchange");
@@ -2469,7 +2491,7 @@ static int track(lm_detector* d, const void* depth, const DeviceFrame* dev, cuda
   }
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (dev) {
-    int rc = check_device_stream(d->device, caller);
+    rc = check_device_stream(d->device, caller);
     const int sz = dev->format == LM_DEPTH_F32 ? 4 : 2;
     if (!rc) rc = check_device_plane(d->device, "depth", depth, dev->depth_pitch, (int64_t)sz * cols, sz);
     if (rc) return rc;
@@ -2479,7 +2501,6 @@ static int track(lm_detector* d, const void* depth, const DeviceFrame* dev, cuda
   cudaStream_t st = d->stream.get();
   d->chain.pose = d->chain.pose_nms = false;  // the stage's buffers now hold the track run: a pending frame's pose stage is abandoned
   const uint16_t* scene = nullptr;
-  int rc;
   if (dev) {  // the reads of the caller's plane start behind its stream's work, and its later work waits for the conversion
     if (!d->ev_in.get()) CU(d->ev_in.create(cudaEventDisableTiming));
     if (!d->ev_out.get()) CU(d->ev_out.create(cudaEventDisableTiming));

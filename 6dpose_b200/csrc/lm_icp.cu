@@ -729,6 +729,18 @@ struct IcpDevice;                    // the calls' buffers (end of this file)
 static IcpDevice* icp_device_new();
 static void icp_device_free(IcpDevice* d);
 
+// lm_icp_set_capture: the kernels' intermediate results of a call, per point in the order of pts
+struct IcpCapture {
+  int estimation = LM_ICP_POINT_TO_PLANE;  // point-to-point computes no normals and no neighbour lists
+  std::vector<IcpJob> jobs;
+  std::vector<int> job_of;  // per hypothesis, -1: early return
+  std::vector<IcpOut> outs;
+  std::vector<double> pts, nrm;
+  std::vector<int32_t> knn, corr;
+  std::vector<long long> record;  // LM_POSE_PSO: the jobs' swarm records, record_words apart
+  int64_t record_words = 0;
+};
+
 struct lm_icp {
   int device = 0;
   Stream stream;  // streams and events first: they outlive the buffers
@@ -741,34 +753,17 @@ struct lm_icp {
   int last_points = 0, last_iterations = 0;
   double last_rmse = 0;
   float last_kernel_us = 0;
-  // lm_icp_set_capture: the kernels' intermediate results of the last call, per point in the order of pts
   bool capture = false;
-  struct {
-    int estimation = LM_ICP_POINT_TO_PLANE;  // point-to-point computes no normals and no neighbour lists
-    std::vector<IcpJob> jobs;
-    std::vector<int> job_of;  // per hypothesis, -1: early return
-    std::vector<IcpOut> outs;
-    std::vector<double> pts, nrm;
-    std::vector<int32_t> knn, corr;
-    std::vector<long long> record;  // LM_POSE_PSO: the jobs' swarm records, record_words apart
-    int64_t record_words = 0;
-  } cap;
-  IcpDevice* dev = nullptr;
-  // lm_icp_set_verify, and the verification of the last call's hypotheses (verified false: that call did not verify)
-  bool verify = false;
+  IcpCapture cap;  // the last call's
+  IcpDevice* dev = nullptr;  // its stage holds the verification of the last call's hypotheses (pose_stage_verify)
+  bool verify = false;  // lm_icp_set_verify
   double verify_mm = 10.0;
-  bool verified = false;
-  std::vector<PoseVerify> ver;
 };
 
 extern "C" int lm_icp_create(int device, lm_icp** out) {
   if (!out) return lm_fail(LM_E_INVALID, "out is null");
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
-  CUI(cudaSetDevice(device));
+  const int rc = open_device(device);
+  if (rc) return rc;
   std::unique_ptr<lm_icp> h(new lm_icp());
   h->device = device;
   CUI(h->stream.create(cudaStreamNonBlocking));
@@ -815,6 +810,14 @@ void compose(const double* T, const float* base, double* R_out, double* t_out) {
     for (int c = 0; c < 3; ++c) R_out[3 * r + c] = res[4 * r + c];
     t_out[r] = res[4 * r + 3] * 1000.0;
   }
+}
+
+// ICP output o against the render made with R, t, as lm_icp_process returns it: T * init_base and the fitness.
+void render_pose(const IcpOut& o, const float* R, const float* t, double* R_out, double* t_out, float* residual) {
+  float base[16];
+  init_base(R, t, base);
+  compose(o.T, base, R_out, t_out);
+  *residual = (float)o.fitness;
 }
 
 }  // namespace
@@ -870,8 +873,8 @@ extern "C" int lm_icp_set_use_scene_cloud(lm_icp* h, int on) {
 
 extern "C" int lm_icp_set_estimation(lm_icp* h, int estimation) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
-  if (estimation != LM_ICP_POINT_TO_PLANE && estimation != LM_ICP_POINT_TO_POINT && estimation != LM_POSE_PSO)
-    return lm_fail(LM_E_INVALID, "unknown ICP estimation %d (LM_ICP_POINT_TO_PLANE 0, LM_ICP_POINT_TO_POINT 1, LM_POSE_PSO 3)", estimation);
+  const int rc = check_estimation(estimation);
+  if (rc) return rc;
   h->estimation = estimation;
   return LM_OK;
 }
@@ -883,90 +886,17 @@ extern "C" int lm_icp_set_pose_search(lm_icp* h, int particles, int iterations, 
 
 extern "C" int lm_icp_set_verify(lm_icp* h, int on, double inlier_mm) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
-  if (!(std::isfinite(inlier_mm) && inlier_mm >= 0.0))
-    return lm_fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
+  const int rc = check_inlier_mm(inlier_mm);
+  if (rc) return rc;
   h->verify = on != 0;
   h->verify_mm = inlier_mm;
   return LM_OK;
-}
-
-static int copy_verify(const PoseVerify* v, int64_t count, float* score, int32_t* counts6, int64_t cap, int64_t* n);
-
-extern "C" int lm_icp_verify(lm_icp* h, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
-  if (!h) return lm_fail(LM_E_INVALID, "null handle");
-  if (!h->verified) return lm_fail(LM_E_STATE, "the last call did not verify (lm_icp_set_verify)");
-  return copy_verify(h->ver.data(), (int64_t)h->ver.size(), score, counts6, cap, n);
 }
 
 extern "C" int lm_icp_set_capture(lm_icp* h, int on) {
   if (!h) return lm_fail(LM_E_INVALID, "null handle");
   h->capture = on != 0;
   h->cap.job_of.clear();
-  return LM_OK;
-}
-
-extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t cap) {
-  if (!h || !out) return lm_fail(LM_E_INVALID, "null argument");
-  const auto& c = h->cap;
-  if (hyp < 0 || hyp >= (int)c.job_of.size())
-    return lm_fail(LM_E_INVALID, "hypothesis %d outside the %d of the last captured call", hyp, (int)c.job_of.size());
-  if (c.job_of[hyp] < 0) return lm_fail(LM_E_STATE, "hypothesis %d took the early return: nothing was captured", hyp);
-  const IcpJob& j = c.jobs[(size_t)c.job_of[hyp]];
-  const IcpOut& o = c.outs[(size_t)c.job_of[hyp]];
-  const void* src = nullptr;
-  int64_t bytes = 0;
-  std::vector<int32_t> tmp;
-  double res[19];
-  if (c.estimation == LM_POSE_PSO && (what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN || what == LM_ICP_CAPTURE_CORR_FIRST ||
-                                       what == LM_ICP_CAPTURE_CORR_LAST))
-    return lm_fail(LM_E_STATE, "capture item %d: the particle swarm computes no normals, neighbour lists or correspondences", what);
-  if ((what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN) && c.estimation != LM_ICP_POINT_TO_PLANE)
-    return lm_fail(LM_E_STATE, "capture item %d: the point-to-point estimation computes no normals or neighbour lists", what);
-  if (what == LM_ICP_CAPTURE_SEARCH && c.estimation != LM_POSE_PSO)
-    return lm_fail(LM_E_STATE, "capture item %d: only an LM_POSE_PSO call keeps swarm records", what);
-  switch (what) {
-    case LM_ICP_CAPTURE_COUNTS:
-      tmp = {j.src_count, j.tgt_count};
-      src = tmp.data(); bytes = 2 * sizeof(int32_t);
-      break;
-    case LM_ICP_CAPTURE_SOURCE:
-      src = c.pts.data() + (size_t)j.src_first * 3; bytes = (int64_t)j.src_count * 3 * sizeof(double);
-      break;
-    case LM_ICP_CAPTURE_TARGET:
-      src = c.pts.data() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double);
-      break;
-    case LM_ICP_CAPTURE_NORMALS:
-      src = c.nrm.data() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double);
-      break;
-    case LM_ICP_CAPTURE_INIT:
-      src = j.init; bytes = sizeof(j.init);
-      break;
-    case LM_ICP_CAPTURE_RESULT:
-      memcpy(res, o.T, sizeof(o.T));
-      res[16] = o.fitness; res[17] = o.rmse; res[18] = o.iterations;
-      src = res; bytes = sizeof(res);
-      break;
-    case LM_ICP_CAPTURE_SEARCH:
-      src = c.record.data() + (size_t)c.job_of[hyp] * c.record_words; bytes = c.record_words * (int64_t)sizeof(long long);
-      break;
-    case LM_ICP_CAPTURE_KNN:
-      src = c.knn.data() + (size_t)j.tgt_first * ICP_KNN; bytes = (int64_t)j.tgt_count * ICP_KNN * sizeof(int32_t);
-      break;
-    case LM_ICP_CAPTURE_CORR_FIRST:
-    case LM_ICP_CAPTURE_CORR_LAST: {
-      // slot 1 holds the last pass after any update; without one, pass 0 was the last pass
-      const int slot = (what == LM_ICP_CAPTURE_CORR_LAST && o.iterations > 0) ? 1 : 0;
-      tmp.resize((size_t)j.src_count);
-      for (int i = 0; i < j.src_count; ++i) tmp[(size_t)i] = c.corr[((size_t)j.src_first + i) * 2 + slot];
-      src = tmp.data(); bytes = (int64_t)j.src_count * sizeof(int32_t);
-      break;
-    }
-    default:
-      return lm_fail(LM_E_INVALID, "unknown capture item %d", what);
-  }
-  if (cap < bytes) return lm_fail(LM_E_CAPACITY, "capture item %d of hypothesis %d needs %lld bytes, cap is %lld", what, hyp,
-                                  (long long)bytes, (long long)cap);
-  if (bytes) memcpy(out, src, (size_t)bytes);
   return LM_OK;
 }
 
@@ -1316,8 +1246,6 @@ __global__ void __launch_bounds__(VERIFY_THREADS) k_pose_verify(PoseParams p, co
     else out[i] = v;
   }
 }
-
-static bool verify_delta_ok(double inlier_mm) { return std::isfinite(inlier_mm) && inlier_mm >= 0.0; }
 
 // --------------------------------------------------------------------------------------------
 // tracking (include/linemod_b200.h, lm_track): a chunk whose clouds come from a given transformation T instead of a
@@ -1782,12 +1710,8 @@ extern "C" int lm_pose_search_points(int device, const double* pts, int64_t n, c
   const int64_t words = pso_record_words(s);
   if (cap > 0 && cap < 8 * words)
     return lm_fail(LM_E_CAPACITY, "the swarm record needs %lld bytes, cap is %lld", (long long)(8 * words), (long long)cap);
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
-  CUI(cudaSetDevice(device));
+  rc = open_device(device);
+  if (rc) return rc;
   // one allocation: pts [n][3], the job, its number, the output, the record, the scene
   IcpJob j;
   memset(&j, 0, sizeof(j));
@@ -2012,7 +1936,7 @@ struct TplHost {
 struct lm_pose_stage {
   std::vector<TplHost> tpl;
   std::vector<int32_t> class_begin;
-  bool dirty = true;           // the device copy of the renders is stale
+  bool dirty = false;          // the device copy of the registered renders is stale (a stage without any has none)
   int64_t area_max = 0;        // largest crop
   DeviceArray<PoseTpl> d_tpl; DeviceArray<uint16_t> d_crops; DeviceArray<int32_t> d_class_begin;
   DeviceArray<PoseRt> d_rt;    // per template: R, t of its render (k_pose_nms composes the poses)
@@ -2224,15 +2148,17 @@ struct PoseChunk {
   int slots;
   int64_t first;    // the run's index of surv[0]
   const uint16_t* scene;
-  const int32_t* frame_of;
-  const float* sKs;
   const float* sK;
-  const int32_t* frame_first;  // a batch's: frame f's first survivor in the run (k_pose_pso's job numbers); else null
   IcpOut* outs;
   uint8_t* posed;
   PoseVerify* ver;  // o.verify.on: per survivor its verification
   int32_t* status;
   int32_t seq;
+  // a batch's survivors' frames and the frames' intrinsics, and frame f's first survivor in the run (k_pose_pso's job
+  // numbers); null: every survivor is of one frame
+  const int32_t* frame_of = nullptr;
+  const float* sKs = nullptr;
+  const int32_t* frame_first = nullptr;
   // capture (unshared chunks; null: none): k_icp_normals' neighbour lists and the ICP kernel's correspondences, indexed
   // as the stage's points, and k_pose_pso's swarm records, record_words per slot
   int32_t* knn_out = nullptr;
@@ -2404,6 +2330,21 @@ int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int
 
 int pose_batch_chunks(int64_t S) { return (int)((S + POSE_CHUNK - 1) / POSE_CHUNK); }
 
+// Chunk c of a run on the stage's registered renders and run outputs: survivors surv + c0 (c0 = c * POSE_CHUNK; counts
+// as PoseChunk), launches for `slots` of them against the one frame scene / sK; its outputs, posed flags and verification
+// from c0 on, status block c and pose exchange share->seq + c.
+static PoseChunk run_chunk(lm_pose_stage* s, const PoseOptions& o, int c, const lm_match* surv, const int32_t* counts, int slots,
+                           const uint16_t* scene, const float* sK) {
+  const int64_t c0 = (int64_t)c * POSE_CHUNK;
+  PoseChunk k;
+  k.table = {s->d_tpl.get(), s->d_crops.get(), s->d_class_begin.get(), (int32_t)s->class_begin.size() - 1, (int32_t)s->tpl.size()};
+  k.surv = surv ? surv + c0 : nullptr; k.counts = counts; k.slots = slots; k.first = c0;
+  k.scene = scene; k.sK = sK;
+  k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.ver = o.verify.on ? s->d_bver.get() + c0 : nullptr;
+  k.status = s->d_bstat.get() + 4 * c; k.seq = o.share ? o.share->seq + c : 0;
+  return k;
+}
+
 // The pose NMS block of a run of n frames: the frames' heads, then the kept poses, frame f's from its first survivor.
 // One copy thus brings back the heads and the first kept poses.
 static PoseNmsHead* nms_heads(uint8_t* block) { return reinterpret_cast<PoseNmsHead*>(block); }
@@ -2511,15 +2452,9 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
   int64_t stage_launches = 0;
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_CHUNK;
-    PoseChunk k;
-    k.table = {s->d_tpl.get(), s->d_crops.get(), s->d_class_begin.get(), (int32_t)s->class_begin.size() - 1, (int32_t)s->tpl.size()};
-    k.surv = run.d_surv + c0;
-    k.counts = batch ? s->d_bstat.get() + 4 * c + 3 : run.d_counts;
-    k.slots = batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound;
-    k.first = c0;
-    k.scene = run.d_scene; k.frame_of = batch ? s->d_bframe.get() + c0 : nullptr;
-    k.sKs = batch ? s->d_bsK.get() : nullptr; k.sK = batch ? nullptr : run.sK; k.frame_first = batch ? s->d_bfirst.get() : nullptr;
-    k.outs = s->d_bouts.get() + c0; k.posed = s->d_bposed.get() + c0; k.ver = s->d_bver.get() + c0; k.status = s->d_bstat.get() + 4 * c; k.seq = sh ? sh->seq + c : 0;
+    PoseChunk k = run_chunk(s, o, c, run.d_surv, batch ? s->d_bstat.get() + 4 * c + 3 : run.d_counts,
+                            batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound, run.d_scene, batch ? nullptr : run.sK);
+    if (batch) { k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get(); k.frame_first = s->d_bfirst.get(); }
     const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
     stage_launches += l;
@@ -2603,15 +2538,11 @@ static bool survivor_fits(const TplHost& h, const lm_match& m, int srows, int sc
   return !(m.x + h.box[2] >= scols || m.y + h.box[3] >= srows);
 }
 
-// Survivor m's pose as lm_complete_pose returns it: T * init_base and the fitness, or residual -1 and R / t untouched
-// where the reference returns early.
-static void survivor_pose(const TplHost& h, const lm_match& m, int srows, int scols, const IcpOut& o, double* R_out, double* t_out,
-                          float* residual) {
-  if (!survivor_fits(h, m, srows, scols)) { *residual = -1.f; return; }
-  float base[16];
-  init_base(h.R, h.t, base);
-  compose(o.T, base, R_out, t_out);
-  *residual = (float)o.fitness;
+// The start of every finish: the run last finished is forgotten, its verification and transformations with it.
+static void pose_forget(lm_pose_stage* s) {
+  s->verified = s->finished_ok = s->xf_pending = false;
+  s->ver.clear();
+  s->xf.clear();
 }
 
 // n kept poses e[] into the caller's arrays (out may be null).
@@ -2635,10 +2566,7 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
   const int64_t S = first[nf];
   if (!batch && n > r.bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, r.bound);
   const bool verify = r.o.verify.on != 0;
-  s->verified = false;
-  s->ver.clear();
-  s->finished_ok = s->xf_pending = false;
-  s->xf.clear();
+  pose_forget(s);
   int64_t published = 0;
   int rc = pose_status(s->h_bstat.get(), batch ? pose_batch_chunks(S) : 1, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0,
                        batch, &published);
@@ -2701,10 +2629,12 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
     return LM_OK;
   }
   s->xf.assign(16 * (size_t)S, std::numeric_limits<double>::quiet_NaN());
-  for (int64_t i = 0; i < S; ++i) {  // every survivor, frame after frame
+  for (int64_t i = 0; i < S; ++i) {  // every survivor, frame after frame; R / t untouched where the reference returns early
     if (out) out[i] = surv[i];
-    survivor_pose(*survivor_render(s, surv[i]), surv[i], r.o.srows, r.o.scols, s->h_bouts[i], R_out + 9 * i, t_out + 3 * i, residual + i);
-    if (residual[i] != -1.f) memcpy(s->xf.data() + 16 * i, s->h_bouts[i].T, sizeof(s->h_bouts[i].T));
+    const TplHost& h = *survivor_render(s, surv[i]);
+    if (!survivor_fits(h, surv[i], r.o.srows, r.o.scols)) { residual[i] = -1.f; continue; }
+    render_pose(s->h_bouts[i], h.R, h.t, R_out + 9 * i, t_out + 3 * i, residual + i);
+    memcpy(s->xf.data() + 16 * i, s->h_bouts[i].T, sizeof(s->h_bouts[i].T));
   }
   if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + S);
   s->verified = verify;
@@ -2725,7 +2655,7 @@ static int copy_verify(const PoseVerify* v, int64_t count, float* score, int32_t
 }
 
 int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
-  if (!s || !s->verified) return lm_fail(LM_E_STATE, "the last completed pose stage did not verify (lm_set_pose_verify)");
+  if (!s || !s->verified) return lm_fail(LM_E_STATE, "the last completed pose stage did not verify (lm_set_pose_verify, lm_icp_set_verify)");
   return copy_verify(s->ver.data(), (int64_t)s->ver.size(), score, counts6, cap, n);
 }
 
@@ -2734,13 +2664,9 @@ extern "C" int lm_pose_verify_points(int device, const double* pts, int64_t n, c
   if (n < 0 || (n > 0 && !pts) || !T || !scene || !sK || !counts6 || !score) return lm_fail(LM_E_INVALID, "null argument or n < 0");
   if (rows <= 0 || cols <= 0) return lm_fail(LM_E_INVALID, "empty scene %d x %d", rows, cols);
   if (n > 0x7FFFFFFFll) return lm_fail(LM_E_CAPACITY, "%lld points, at most 2^31 - 1", (long long)n);
-  if (!verify_delta_ok(inlier_mm)) return lm_fail(LM_E_INVALID, "inlier distance %g mm: must be finite and >= 0", inlier_mm);
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
-  CUI(cudaSetDevice(device));
+  int rc = check_inlier_mm(inlier_mm);
+  if (!rc) rc = open_device(device);
+  if (rc) return rc;
   // k_pose_verify over one slot: one allocation of pts [n][3], the pose (IcpOut), the segments (begin 0 at [0], end n at
   // [2]), the posed flag, the result and the scene [rows][cols]
   IcpOut o;
@@ -2783,12 +2709,8 @@ extern "C" int lm_nms_translations(int device, int64_t n, const double* t, const
   if (!n_keep || n < 0 || (n > 0 && (!t || !score || !keep))) return lm_fail(LM_E_INVALID, "null argument or n < 0");
   if (!(thr >= 0.0)) return lm_fail(LM_E_INVALID, "translation threshold must be >= 0 (NaN given or negative)");
   if (n > NMS_THREADS) return lm_fail(LM_E_CAPACITY, "%lld translations, at most %d", (long long)n, NMS_THREADS);
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return lm_fail(LM_E_CUDA, "no CUDA device available (%s); this library has no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return lm_fail(LM_E_INVALID, "device %d out of range (have %d)", device, ndev);
-  CUI(cudaSetDevice(device));
+  const int rc = open_device(device);
+  if (rc) return rc;
   const size_t m = (size_t)std::max<int64_t>(n, 1);
   // one allocation: t [m][3], score [m], keep [m], n_keep
   DeviceArray<uint8_t> buf;
@@ -2828,6 +2750,12 @@ __global__ void __launch_bounds__(ICP_DEV_PX) k_icp_scene(const uint8_t* __restr
                                                          uint16_t* __restrict__ out) {
   const int y = blockIdx.y, x = blockIdx.x * ICP_DEV_PX + threadIdx.x;
   if (x < cols) out[(size_t)y * cols + x] = lm_depth_at(src + y * pitch, x, f32, scale);
+}
+
+// A caller's rows x cols depth plane (pitch bytes between rows, checked format and scale) into out on st.
+static void launch_scene(const void* depth, int64_t pitch, int format, float scale, int rows, int cols, uint16_t* out, cudaStream_t st) {
+  k_icp_scene<<<dim3((unsigned)((cols + ICP_DEV_PX - 1) / ICP_DEV_PX), (unsigned)rows), ICP_DEV_PX, 0, st>>>(
+      static_cast<const uint8_t*>(depth), pitch, format == LM_DEPTH_F32 ? 1 : 0, scale, cols, out);
 }
 
 // The extent of render blockIdx.x's non-zero pixels (after conversion) over its rows [blockIdx.y * RENDER_BOX_ROWS,
@@ -2885,28 +2813,136 @@ __global__ void __launch_bounds__(ICP_DEV_PX) k_icp_render_crop(const RenderSrc*
 }
 
 struct IcpDevice {
-  lm_pose_stage stage;  // the chunks' cloud buffers (pose_buffers); no registered render
+  lm_pose_stage stage;  // the chunks' buffers and run outputs, and the call's render table and crops in d_tpl / d_crops
   PinnedArray<uint16_t> h_planes; DeviceArray<uint16_t> planes;  // lm_icp_process_batch: the scene, then each distinct render
   DeviceArray<uint8_t> in;  // the call's inputs in one copy: renders, K, survivors, chunk sizes, class_begin
-  DeviceArray<uint16_t> scene, crops;
+  DeviceArray<uint16_t> scene;
   DeviceArray<uint32_t> ext; PinnedArray<uint32_t> h_ext;  // [n][4] extents (k_icp_render_box)
-  DeviceArray<PoseTpl> tpl;
-  DeviceArray<IcpOut> outs; DeviceArray<uint8_t> posed; PinnedArray<IcpOut> h_outs;
-  DeviceArray<int32_t> status; PinnedArray<int32_t> h_status;  // 4 per chunk (PoseChunk); the host's copy then holds the
-                                                               // source count of the last hypothesis with a pose
-  DeviceArray<PoseVerify> ver; PinnedArray<PoseVerify> h_ver;  // lm_icp_set_verify: per hypothesis
   DeviceArray<int32_t> knn, corr; DeviceArray<long long> record;  // lm_icp_set_capture: the chunk's (PoseChunk)
 };
 
 static IcpDevice* icp_device_new() { return new IcpDevice(); }
 static void icp_device_free(IcpDevice* d) { delete d; }
 
-// A device depth plane's format and scale.
-static int check_depth_format(const char* what, int format, float scale) {
-  if (format != LM_DEPTH_U16_MM && format != LM_DEPTH_F32)
-    return lm_fail(LM_E_INVALID, "%s: unknown depth format %d (LM_DEPTH_U16_MM %d, LM_DEPTH_F32 %d)", what, format, LM_DEPTH_U16_MM, LM_DEPTH_F32);
-  if (format == LM_DEPTH_F32 && !(std::isfinite(scale) && scale > 0.f))
-    return lm_fail(LM_E_INVALID, "%s: scale %g: float depth needs a finite scale > 0", what, (double)scale);
+extern "C" int lm_icp_verify(lm_icp* h, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
+  if (!h) return lm_fail(LM_E_INVALID, "null handle");
+  return pose_stage_verify(&h->dev->stage, score, counts6, cap, n);
+}
+
+extern "C" int lm_icp_capture(lm_icp* h, int hyp, int what, void* out, int64_t cap) {
+  if (!h || !out) return lm_fail(LM_E_INVALID, "null argument");
+  const auto& c = h->cap;
+  if (hyp < 0 || hyp >= (int)c.job_of.size())
+    return lm_fail(LM_E_INVALID, "hypothesis %d outside the %d of the last captured call", hyp, (int)c.job_of.size());
+  if (c.job_of[hyp] < 0) return lm_fail(LM_E_STATE, "hypothesis %d took the early return: nothing was captured", hyp);
+  const IcpJob& j = c.jobs[(size_t)c.job_of[hyp]];
+  const IcpOut& o = c.outs[(size_t)c.job_of[hyp]];
+  const void* src = nullptr;
+  int64_t bytes = 0;
+  std::vector<int32_t> tmp;
+  double res[19];
+  if (c.estimation == LM_POSE_PSO && (what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN || what == LM_ICP_CAPTURE_CORR_FIRST ||
+                                       what == LM_ICP_CAPTURE_CORR_LAST))
+    return lm_fail(LM_E_STATE, "capture item %d: the particle swarm computes no normals, neighbour lists or correspondences", what);
+  if ((what == LM_ICP_CAPTURE_NORMALS || what == LM_ICP_CAPTURE_KNN) && c.estimation != LM_ICP_POINT_TO_PLANE)
+    return lm_fail(LM_E_STATE, "capture item %d: the point-to-point estimation computes no normals or neighbour lists", what);
+  if (what == LM_ICP_CAPTURE_SEARCH && c.estimation != LM_POSE_PSO)
+    return lm_fail(LM_E_STATE, "capture item %d: only an LM_POSE_PSO call keeps swarm records", what);
+  switch (what) {
+    case LM_ICP_CAPTURE_COUNTS:
+      tmp = {j.src_count, j.tgt_count};
+      src = tmp.data(); bytes = 2 * sizeof(int32_t);
+      break;
+    case LM_ICP_CAPTURE_SOURCE:
+      src = c.pts.data() + (size_t)j.src_first * 3; bytes = (int64_t)j.src_count * 3 * sizeof(double);
+      break;
+    case LM_ICP_CAPTURE_TARGET:
+      src = c.pts.data() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double);
+      break;
+    case LM_ICP_CAPTURE_NORMALS:
+      src = c.nrm.data() + (size_t)j.tgt_first * 3; bytes = (int64_t)j.tgt_count * 3 * sizeof(double);
+      break;
+    case LM_ICP_CAPTURE_INIT:
+      src = j.init; bytes = sizeof(j.init);
+      break;
+    case LM_ICP_CAPTURE_RESULT:
+      memcpy(res, o.T, sizeof(o.T));
+      res[16] = o.fitness; res[17] = o.rmse; res[18] = o.iterations;
+      src = res; bytes = sizeof(res);
+      break;
+    case LM_ICP_CAPTURE_SEARCH:
+      src = c.record.data() + (size_t)c.job_of[hyp] * c.record_words; bytes = c.record_words * (int64_t)sizeof(long long);
+      break;
+    case LM_ICP_CAPTURE_KNN:
+      src = c.knn.data() + (size_t)j.tgt_first * ICP_KNN; bytes = (int64_t)j.tgt_count * ICP_KNN * sizeof(int32_t);
+      break;
+    case LM_ICP_CAPTURE_CORR_FIRST:
+    case LM_ICP_CAPTURE_CORR_LAST: {
+      // slot 1 holds the last pass after any update; without one, pass 0 was the last pass
+      const int slot = (what == LM_ICP_CAPTURE_CORR_LAST && o.iterations > 0) ? 1 : 0;
+      tmp.resize((size_t)j.src_count);
+      for (int i = 0; i < j.src_count; ++i) tmp[(size_t)i] = c.corr[((size_t)j.src_first + i) * 2 + slot];
+      src = tmp.data(); bytes = (int64_t)j.src_count * sizeof(int32_t);
+      break;
+    }
+    default:
+      return lm_fail(LM_E_INVALID, "unknown capture item %d", what);
+  }
+  if (cap < bytes) return lm_fail(LM_E_CAPACITY, "capture item %d of hypothesis %d needs %lld bytes, cap is %lld", what, hyp,
+                                  (long long)bytes, (long long)cap);
+  if (bytes) memcpy(out, src, (size_t)bytes);
+  return LM_OK;
+}
+
+// The capture of the chunk of hypotheses [c0, c0 + n) behind it, before the next chunk reuses the buffers: each posed
+// hypothesis's job, its clouds with their normals, neighbour lists and correspondences, and its swarm record, appended
+// to cap in the stage's point order.
+static int icp_capture_chunk(const IcpDevice& d, cudaStream_t st, int c0, int n, const uint8_t* posed, IcpCapture& cap) {
+  const lm_pose_stage& s = d.stage;
+  const bool pso = cap.estimation == LM_POSE_PSO, normals = cap.estimation == LM_ICP_POINT_TO_PLANE;
+  const int64_t words = cap.record_words;
+  CUI(cudaStreamSynchronize(st));
+  std::vector<IcpJob> jobs((size_t)n);
+  CUI(cudaMemcpy(jobs.data(), s.d_jobs.get(), sizeof(IcpJob) * jobs.size(), cudaMemcpyDeviceToHost));
+  // points [first, first + count) of the stage's clouds, with their normals, neighbour lists and correspondences
+  auto append = [&](int32_t first, int32_t count) {
+    const size_t at = cap.pts.size() / 3, m = (size_t)count;
+    cap.pts.resize(3 * (at + m));
+    if (normals) { cap.nrm.resize(3 * (at + m)); cap.knn.resize(ICP_KNN * (at + m)); }
+    if (!pso) cap.corr.resize(2 * (at + m));
+    if (!m) return LM_OK;
+    CUI(cudaMemcpy(cap.pts.data() + 3 * at, s.d_pts.get() + 3 * (size_t)first, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
+    if (normals) {
+      CUI(cudaMemcpy(cap.nrm.data() + 3 * at, s.d_nrm.get() + 3 * (size_t)first, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(cap.knn.data() + ICP_KNN * at, d.knn.get() + ICP_KNN * (size_t)first, sizeof(int32_t) * ICP_KNN * m,
+                     cudaMemcpyDeviceToHost));
+    }
+    if (!pso) CUI(cudaMemcpy(cap.corr.data() + 2 * at, d.corr.get() + 2 * (size_t)first, sizeof(int32_t) * 2 * m, cudaMemcpyDeviceToHost));
+    return LM_OK;
+  };
+  for (int i = 0; i < n; ++i) {
+    if (!posed[i]) continue;
+    IcpJob j = jobs[(size_t)i];
+    const bool own_target = j.tgt_first != j.src_first;
+    const int32_t src_at = (int32_t)(cap.pts.size() / 3);
+    int rc = append(j.src_first, j.src_count);
+    if (!rc && own_target) {
+      const int32_t tgt_at = (int32_t)(cap.pts.size() / 3);
+      rc = append(j.tgt_first, j.tgt_count);
+      j.tgt_first = tgt_at;
+    } else {
+      j.tgt_first = src_at;
+    }
+    if (rc) return rc;
+    j.src_first = src_at;
+    if (pso) {
+      cap.record.resize(cap.record.size() + (size_t)words);
+      CUI(cudaMemcpy(cap.record.data() + cap.record.size() - words, d.record.get() + (size_t)i * words, sizeof(long long) * words,
+                     cudaMemcpyDeviceToHost));
+    }
+    cap.job_of[(size_t)(c0 + i)] = (int)cap.jobs.size();
+    cap.jobs.push_back(j);
+  }
   return LM_OK;
 }
 
@@ -2914,43 +2950,28 @@ static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
 // A call without hypotheses: no device work; it verified nothing (an empty verification) and captured nothing.
 static int icp_no_hypotheses(lm_icp* h) {
-  h->ver.clear();
-  h->verified = h->verify;
+  pose_forget(&h->dev->stage);
+  h->dev->stage.verified = h->verify;
   h->cap.job_of.clear();
   return LM_OK;
 }
 
 // lm_icp_process_batch and lm_icp_process_batch_device past their checks: n >= 1 hypotheses, the scene and renders[i] in
-// device memory as lm_icp_process_batch_device takes them, on the handle's stream behind the caller's ev0.  Returns once
-// the outputs are on the host.
+// device memory as lm_icp_process_batch_device takes them, on the handle's stream behind the caller's ev0.  A run of the
+// handle's stage whose table holds the call's renders.  Returns once the outputs are on the host.
 static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pitch, int scene_format, float scene_scale, int srows,
                      int scols, const RenderSrc* renders, int model_format, float model_scale, int mrows, int mcols,
                      const float* sceneK, const float* modelK, const float* R, const float* t, const int32_t* detect_xy,
                      int max_iterations, double* R_out, double* t_out, float* residual) {
-  h->verified = false;
-  h->cap.job_of.clear();  // a call that fails keeps no capture
   IcpDevice& d = *h->dev;
+  lm_pose_stage* s = &d.stage;
+  pose_forget(s);
+  h->cap.job_of.clear();  // a call that fails keeps no capture
   cudaStream_t st = h->stream.get();
-  const bool pso = h->estimation == LM_POSE_PSO, normals = h->estimation == LM_ICP_POINT_TO_PLANE;
-  const int64_t words = pso_record_words(h->search);
-  // capture: what each posed hypothesis's chunk built and kept, copied out behind the chunk; kept only when the call succeeds
-  std::vector<IcpJob> cjobs;
-  std::vector<int> cjob_of((size_t)n, -1);
-  std::vector<double> cpts, cnrm;
-  std::vector<int32_t> cknn, ccorr;
-  std::vector<long long> crec;
-  auto keep_capture = [&](const IcpOut* outs) {
-    auto& c = h->cap;
-    c.estimation = h->estimation;
-    c.jobs = std::move(cjobs);
-    c.job_of = std::move(cjob_of);
-    c.outs.clear();
-    for (int i = 0; i < n; ++i)
-      if (c.job_of[(size_t)i] >= 0) c.outs.push_back(outs[i]);
-    c.pts = std::move(cpts); c.nrm = std::move(cnrm);
-    c.knn = std::move(cknn); c.corr = std::move(ccorr);
-    c.record = std::move(crec); c.record_words = words;
-  };
+  IcpCapture cap;  // kept only when the call succeeds
+  cap.estimation = h->estimation;
+  cap.job_of.assign((size_t)n, -1);
+  cap.record_words = pso_record_words(h->search);
   const int nc = pose_batch_chunks(n);
   // the inputs: survivor i is hypothesis i (class 0, template i) at detect_xy[i]; chunk c holds min(n - 1024 c, 1024)
   const size_t o_K = align16(sizeof(RenderSrc) * n), o_surv = align16(o_K + sizeof(float) * 9 * n);
@@ -2968,17 +2989,13 @@ static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pi
   CUI(d.in.reserve(in.size()));
   CUI(d.scene.reserve((size_t)srows * scols));
   CUI(d.ext.reserve(4 * (size_t)n)); CUI(d.h_ext.reserve(4 * (size_t)n));
-  CUI(d.tpl.reserve(n));
-  CUI(d.outs.reserve(n)); CUI(d.posed.reserve(n)); CUI(d.h_outs.reserve(n));
-  CUI(d.status.reserve(4 * (size_t)nc)); CUI(d.h_status.reserve(4 * (size_t)nc + 1));
-  if (h->verify) { CUI(d.ver.reserve(n)); CUI(d.h_ver.reserve(n)); }
+  CUI(s->d_tpl.reserve(n));
   const RenderSrc* d_src = reinterpret_cast<const RenderSrc*>(d.in.get());
   const float* d_K = reinterpret_cast<const float*>(d.in.get() + o_K);
   const int f32 = model_format == LM_DEPTH_F32 ? 1 : 0;
   CUI(cudaMemcpyAsync(d.in.get(), in.data(), in.size(), cudaMemcpyHostToDevice, st));
   CUI(cudaMemsetAsync(d.ext.get(), 0xFF, sizeof(uint32_t) * 4 * n, st));
-  k_icp_scene<<<dim3((unsigned)((scols + ICP_DEV_PX - 1) / ICP_DEV_PX), (unsigned)srows), ICP_DEV_PX, 0, st>>>(
-      static_cast<const uint8_t*>(scene_depth), scene_pitch, scene_format == LM_DEPTH_F32 ? 1 : 0, scene_scale, scols, d.scene.get());
+  launch_scene(scene_depth, scene_pitch, scene_format, scene_scale, srows, scols, d.scene.get(), st);
   k_icp_render_box<<<dim3((unsigned)n, (unsigned)((mrows + RENDER_BOX_ROWS - 1) / RENDER_BOX_ROWS)), ICP_DEV_PX, 0, st>>>(
       d_src, f32, model_scale, mrows, mcols, d.ext.get());
   CUI(cudaGetLastError());
@@ -3001,128 +3018,82 @@ static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pi
     max_bh = std::max(max_bh, b[3]);
     last = i;
   }
-  if (last < 0) {  // every hypothesis takes the early return: no cloud to build
+  if (last < 0) {  // every hypothesis takes the early return: no cloud to build, and every verification scores -1
     for (int i = 0; i < n; ++i) residual[i] = -1.f;
     if (h->verify) {
-      h->ver.assign((size_t)n, PoseVerify());
-      for (PoseVerify& v : h->ver) v.score = -1.f;
-      h->verified = true;
+      s->ver.assign((size_t)n, PoseVerify());
+      for (PoseVerify& v : s->ver) v.score = -1.f;
+      s->verified = true;
     }
-    if (h->capture) keep_capture(nullptr);
+    if (h->capture) h->cap = std::move(cap);
     return LM_OK;
   }
-  CUI(d.crops.reserve((size_t)n * stride));
-  int rc = pose_buffers(&d.stage, st, std::min(n, POSE_CHUNK), stride);
+  // the run's buffers: clouds of the largest crop, and status blocks for the chunks and one more, whose first word
+  // receives the source count of the last hypothesis with a pose
+  s->area_max = stride;
+  int rc = pose_prepare(s, st, nc + 1, n, h->verify);
   if (rc) return rc;
+  CUI(s->d_crops.reserve((size_t)n * stride));
   if (h->capture) {  // the chunks' capture outputs, indexed as the stage's points and slots
-    const size_t points = 2 * (size_t)pose_slots(&d.stage) * (size_t)pose_area(&d.stage);
-    if (normals) CUI(d.knn.reserve(points * ICP_KNN));
-    if (!pso) CUI(d.corr.reserve(points * 2));
-    if (pso) CUI(d.record.reserve((size_t)pose_slots(&d.stage) * words));
+    const size_t points = 2 * (size_t)pose_slots(s) * (size_t)pose_area(s);
+    if (cap.estimation == LM_ICP_POINT_TO_PLANE) CUI(d.knn.reserve(points * ICP_KNN));
+    if (cap.estimation != LM_POSE_PSO) CUI(d.corr.reserve(points * 2));
+    else CUI(d.record.reserve((size_t)pose_slots(s) * cap.record_words));
   }
   k_icp_render_crop<<<dim3((unsigned)n, (unsigned)((max_bh + RENDER_CROP_ROWS - 1) / RENDER_CROP_ROWS)), ICP_DEV_PX, 0, st>>>(
-      d_src, f32, model_scale, mrows, mcols, d.ext.get(), d_K, stride, d.tpl.get(), d.crops.get());
+      d_src, f32, model_scale, mrows, mcols, d.ext.get(), d_K, stride, s->d_tpl.get(), s->d_crops.get());
   CUI(cudaGetLastError());
   ++h->launches;
-  CUI(cudaMemsetAsync(d.status.get(), 0, sizeof(int32_t) * 4 * nc, st));
-  PoseOptions o;
-  o.srows = srows; o.scols = scols; o.use_scene_cloud = h->use_scene_cloud ? 1 : 0; o.max_iterations = max_iterations;
-  o.estimation = h->estimation; o.stream = st; o.share = nullptr;
-  o.verify = {h->verify ? 1 : 0, LM_VERIFY_RANK_FITNESS, h->verify_mm, -INFINITY};
-  o.search = h->search;
-  const PoseTable table = {d.tpl.get(), d.crops.get(), reinterpret_cast<const int32_t*>(d.in.get() + o_cb), 1, n};
+  CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4 * nc, st));
+  const PoseOptions o = {srows, scols, h->use_scene_cloud ? 1 : 0, max_iterations, h->estimation, st, nullptr,
+                         {h->verify ? 1 : 0, LM_VERIFY_RANK_FITNESS, h->verify_mm, -INFINITY}, h->search};
+  const PoseTable table = {s->d_tpl.get(), s->d_crops.get(), reinterpret_cast<const int32_t*>(d.in.get() + o_cb), 1, n};
   const lm_match* d_surv = reinterpret_cast<const lm_match*>(d.in.get() + o_surv);
   const int32_t* d_cnt = reinterpret_cast<const int32_t*>(d.in.get() + o_cnt);
   for (int c = 0; c < nc; ++c) {
     const int c0 = c * POSE_CHUNK;
-    PoseChunk k;
+    PoseChunk k = run_chunk(s, o, c, d_surv, d_cnt + c, cnt[c], d.scene.get(), sceneK);
     k.table = table;
-    k.surv = d_surv + c0; k.counts = d_cnt + c; k.slots = cnt[c]; k.first = c0;
-    k.scene = d.scene.get(); k.frame_of = nullptr; k.sKs = nullptr; k.sK = sceneK; k.frame_first = nullptr;
-    k.outs = d.outs.get() + c0; k.posed = d.posed.get() + c0; k.ver = h->verify ? d.ver.get() + c0 : nullptr;
-    k.status = d.status.get() + 4 * c; k.seq = 0;
     if (h->capture) {
       k.knn_out = d.knn.get(); k.corr_out = d.corr.get();
-      k.record = d.record.get(); k.record_words = words;
+      k.record = d.record.get(); k.record_words = cap.record_words;
     }
-    const int l = pose_chunk(&d.stage, o, k);
+    const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
     h->launches += l;
     if (last >= c0 && last < c0 + cnt[c])  // the chunk's jobs are overwritten by the next chunk's
-      CUI(cudaMemcpyAsync(d.h_status.get() + 4 * nc, &d.stage.d_jobs.get()[last - c0].src_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    if (h->capture) {  // the chunk's jobs, clouds and kernel outputs, before the next chunk reuses the buffers
-      CUI(cudaStreamSynchronize(st));
-      std::vector<IcpJob> jobs((size_t)cnt[c]);
-      CUI(cudaMemcpy(jobs.data(), d.stage.d_jobs.get(), sizeof(IcpJob) * jobs.size(), cudaMemcpyDeviceToHost));
-      // points [first, first + count) of the stage's clouds, with their normals, neighbour lists and correspondences
-      auto append = [&](int32_t first, int32_t count) {
-        const size_t at = cpts.size() / 3, m = (size_t)count;
-        cpts.resize(3 * (at + m));
-        if (normals) { cnrm.resize(3 * (at + m)); cknn.resize(ICP_KNN * (at + m)); }
-        if (!pso) ccorr.resize(2 * (at + m));
-        if (!m) return LM_OK;
-        CUI(cudaMemcpy(cpts.data() + 3 * at, d.stage.d_pts.get() + 3 * (size_t)first, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
-        if (normals) {
-          CUI(cudaMemcpy(cnrm.data() + 3 * at, d.stage.d_nrm.get() + 3 * (size_t)first, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost));
-          CUI(cudaMemcpy(cknn.data() + ICP_KNN * at, d.knn.get() + ICP_KNN * (size_t)first, sizeof(int32_t) * ICP_KNN * m,
-                         cudaMemcpyDeviceToHost));
-        }
-        if (!pso) CUI(cudaMemcpy(ccorr.data() + 2 * at, d.corr.get() + 2 * (size_t)first, sizeof(int32_t) * 2 * m, cudaMemcpyDeviceToHost));
-        return LM_OK;
-      };
-      for (int i = 0; i < cnt[c]; ++i) {
-        if (!posed[(size_t)(c0 + i)]) continue;
-        IcpJob j = jobs[(size_t)i];
-        const bool own_target = j.tgt_first != j.src_first;
-        const int32_t src_at = (int32_t)(cpts.size() / 3);
-        rc = append(j.src_first, j.src_count);
-        if (!rc && own_target) {
-          const int32_t tgt_at = (int32_t)(cpts.size() / 3);
-          rc = append(j.tgt_first, j.tgt_count);
-          j.tgt_first = tgt_at;
-        } else {
-          j.tgt_first = src_at;
-        }
-        if (rc) return rc;
-        j.src_first = src_at;
-        if (pso) {
-          crec.resize(crec.size() + (size_t)words);
-          CUI(cudaMemcpy(crec.data() + crec.size() - words, d.record.get() + (size_t)i * words, sizeof(long long) * words,
-                         cudaMemcpyDeviceToHost));
-        }
-        cjob_of[(size_t)(c0 + i)] = (int)cjobs.size();
-        cjobs.push_back(j);
-      }
+      CUI(cudaMemcpyAsync(s->h_bstat.get() + 4 * nc, &s->d_jobs.get()[last - c0].src_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    if (h->capture) {
+      rc = icp_capture_chunk(d, st, c0, cnt[c], posed.data() + c0, cap);
+      if (rc) return rc;
     }
   }
   CUI(cudaEventRecord(h->ev1.get(), st));
-  CUI(cudaMemcpyAsync(d.h_outs.get(), d.outs.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
-  CUI(cudaMemcpyAsync(d.h_status.get(), d.status.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
-  if (h->verify) CUI(cudaMemcpyAsync(d.h_ver.get(), d.ver.get(), sizeof(PoseVerify) * n, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  if (h->verify) CUI(cudaMemcpyAsync(s->h_bver.get(), s->d_bver.get(), sizeof(PoseVerify) * n, cudaMemcpyDeviceToHost, st));
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
   float ms = 0;
   CUI(cudaEventElapsedTime(&ms, h->ev0.get(), h->ev1.get()));
   h->last_kernel_us = ms * 1000.f;
-  for (int c = 0; c < nc; ++c)
-    if (d.h_status[4 * (size_t)c])
-      return lm_fail(LM_E_INVALID, "a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
+  int64_t published = 0;
+  rc = pose_status(s->h_bstat.get(), nc, false, 0, 0, false, &published);
+  if (rc) return rc;
   for (int i = 0; i < n; ++i) {
-    if (!posed[(size_t)i]) { residual[i] = -1.f; continue; }
-    const IcpOut& q = d.h_outs[(size_t)i];
-    float base[16];
-    init_base(R + 9 * i, t + 3 * i, base);
-    compose(q.T, base, R_out + 9 * i, t_out + 3 * i);
-    residual[i] = (float)q.fitness;
+    if (posed[(size_t)i]) render_pose(s->h_bouts[(size_t)i], R + 9 * i, t + 3 * i, R_out + 9 * i, t_out + 3 * i, residual + i);
+    else residual[i] = -1.f;
   }
-  if (h->verify) {
-    h->ver.assign(d.h_ver.get(), d.h_ver.get() + n);
-    h->verified = true;
+  if (h->verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + n);
+  s->verified = h->verify;
+  if (h->capture) {
+    for (int i = 0; i < n; ++i)
+      if (cap.job_of[(size_t)i] >= 0) cap.outs.push_back(s->h_bouts[(size_t)i]);
+    h->cap = std::move(cap);
   }
-  if (h->capture) keep_capture(d.h_outs.get());
-  h->last_points = d.h_status[4 * (size_t)nc];
-  h->last_iterations = d.h_outs[(size_t)last].iterations;
-  h->last_rmse = d.h_outs[(size_t)last].rmse;
+  h->last_points = s->h_bstat[4 * (size_t)nc];
+  h->last_iterations = s->h_bouts[(size_t)last].iterations;
+  h->last_rmse = s->h_bouts[(size_t)last].rmse;
   return LM_OK;
 }
 
@@ -3215,8 +3186,7 @@ int pose_track_scene(lm_pose_stage* s, cudaStream_t st, bool host, const void* d
   if (host) {
     CUI(cudaMemcpyAsync(s->d_tscene.get(), depth, sizeof(uint16_t) * npix, cudaMemcpyHostToDevice, st));
   } else {
-    k_icp_scene<<<dim3((unsigned)((cols + ICP_DEV_PX - 1) / ICP_DEV_PX), (unsigned)rows), ICP_DEV_PX, 0, st>>>(
-        static_cast<const uint8_t*>(depth), pitch, format == LM_DEPTH_F32 ? 1 : 0, scale, cols, s->d_tscene.get());
+    launch_scene(depth, pitch, format, scale, rows, cols, s->d_tscene.get(), st);
     CUI(cudaGetLastError());
     ++*launches;
   }
@@ -3229,11 +3199,8 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_s
                      int32_t* box) {
   cudaStream_t st = o.stream;
   const bool verify = o.verify.on != 0;
+  pose_forget(s);
   int rc = pose_prepare(s, st, 1, n, verify);
-  s->verified = false;
-  s->ver.clear();
-  s->xf.clear();
-  s->xf_pending = false;
   if (rc) return rc;
   if (n == 0) {
     s->verified = verify;
@@ -3260,11 +3227,7 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_s
   q.sc.fx = sK[0]; q.sc.cx = sK[2]; q.sc.fy = sK[4]; q.sc.cy = sK[5];
   q.margin = margin; q.cap = W; q.stride = stride; q.M = M;
   q.rec = s->d_trec.get();
-  PoseChunk k;
-  k.table = {s->d_tpl.get(), s->d_crops.get(), s->d_class_begin.get(), (int32_t)s->class_begin.size() - 1, (int32_t)s->tpl.size()};
-  k.surv = nullptr; k.counts = nullptr; k.slots = n; k.first = 0;
-  k.scene = d_scene; k.frame_of = nullptr; k.sKs = nullptr; k.sK = sK; k.frame_first = nullptr;
-  k.outs = s->d_bouts.get(); k.posed = s->d_bposed.get(); k.ver = s->d_bver.get(); k.status = s->d_bstat.get(); k.seq = 0;
+  PoseChunk k = run_chunk(s, o, 0, nullptr, nullptr, n, d_scene, sK);
   k.track = &q;
   const int l = pose_chunk(s, o, k);
   if (l < 0) return l;
@@ -3286,12 +3249,9 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_s
     if (e.status != LM_TRACK_TRACKED) { residual[i] = -1.f; continue; }
     const IcpOut& q = s->h_bouts[(size_t)i];
     const TplHost& h = s->tpl[(size_t)obj[i].g];
-    float base[16];
-    init_base(h.R, h.t, base);
-    compose(q.T, base, R_out + 9 * i, t_out + 3 * i);
+    render_pose(q, h.R, h.t, R_out + 9 * i, t_out + 3 * i, residual + i);
     memcpy(T_out + 16 * i, q.T, sizeof(q.T));
     memcpy(s->xf.data() + 16 * i, q.T, sizeof(q.T));
-    residual[i] = (float)q.fitness;
   }
   if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + n);
   s->verified = verify;
@@ -3324,12 +3284,11 @@ int pose_stage_transforms(lm_pose_stage* s, double* T_out, int64_t cap, int64_t*
         const TplHost* h = survivor_render(s, e.m);
         int64_t got = -1;
         for (int64_t i = first[(size_t)f]; h && got < 0 && i < first[(size_t)f + 1]; ++i) {
-          if (!posed[(size_t)i] || (float)outs[(size_t)i].fitness != e.residual) continue;
+          if (!posed[(size_t)i]) continue;
           double R[9], t[3];
-          float base[16];
-          init_base(h->R, h->t, base);
-          compose(outs[(size_t)i].T, base, R, t);
-          if (!memcmp(R, e.R, sizeof(R)) && !memcmp(t, e.t, sizeof(t))) got = i;
+          float res;
+          render_pose(outs[(size_t)i], h->R, h->t, R, t, &res);
+          if (res == e.residual && !memcmp(R, e.R, sizeof(R)) && !memcmp(t, e.t, sizeof(t))) got = i;
         }
         if (got < 0) return lm_fail(LM_E_STATE, "frame %d, kept pose %lld: no survivor composes to it", f, (long long)k);
         s->xf.insert(s->xf.end(), outs[(size_t)got].T, outs[(size_t)got].T + 16);

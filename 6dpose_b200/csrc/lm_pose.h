@@ -151,8 +151,10 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
 // Chunks of a run with S survivors.
 int pose_batch_chunks(int64_t S);
 
-// lm_icp_process_batch_device feeds the same chunks (pose_chunk in lm_icp.cu) from renders it is handed per call instead
-// of registered ones.  Its table has one entry per hypothesis, written on the device: k_icp_render_box reduces every
+// An lm_icp call (lm_icp_process_batch, lm_icp_process_batch_device) is a run of the ICP handle's own stage: the same
+// chunks (run_chunk, pose_chunk in lm_icp.cu) into the stage's run outputs, the same status check and the stage's
+// verification (lm_icp_verify reads it as pose_stage_verify), but from renders it is handed per call instead of
+// registered ones.  Its table has one entry per hypothesis, written on the device: k_icp_render_box reduces every
 // render's non-zero extent, the host reads the extents back once (n x 16 bytes, one synchronise of the handle's stream),
 // then k_icp_render_crop writes each entry (model_box's box, the anchor, K) and its crop.  The read-back sizes what the
 // host cannot know before: the crop pool (n x the largest crop a posed hypothesis has) and the clouds' slot stride of the
@@ -165,3 +167,11 @@ int pose_batch_chunks(int64_t S);
 // unless stream is a CUDA stream of `device`.
 int check_device_plane(int device, const char* what, const void* p, int64_t pitch, int64_t row, int elem);
 int check_device_stream(int device, cudaStream_t stream);
+
+// Checks shared by the detector, the ICP handle and the standalone entry points, LM_E_INVALID with the message unless a
+// device plane `what` has a known depth format (and a float one a finite scale > 0), an estimation is known, an inlier
+// distance is finite and >= 0.  open_device makes `device` current (LM_E_CUDA without a device, LM_E_INVALID out of range).
+int check_depth_format(const char* what, int format, float scale);
+int check_estimation(int estimation);
+int check_inlier_mm(double inlier_mm);
+int open_device(int device);
