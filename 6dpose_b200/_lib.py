@@ -46,7 +46,7 @@ SYMBOLS = [
     "lm_icp_set_estimation", "lm_icp_set_capture", "lm_icp_capture", "lm_icp_process_batch_device",
     "lm_set_pose_verify", "lm_pose_verify", "lm_pose_verify_points", "lm_icp_set_verify", "lm_icp_verify",
     "lm_set_pose_search", "lm_icp_set_pose_search", "lm_pose_search_points",
-    "lm_track", "lm_track_device", "lm_pose_transforms",
+    "lm_track", "lm_track_device", "lm_track_batch", "lm_track_batch_device", "lm_pose_transforms",
 ]
 
 # The pose stage's estimation (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT / LM_POSE_PSO of include/linemod_b200.h) by
@@ -468,6 +468,9 @@ def load():
     track_out = [f32p, vp, c_int, c_int, c_int, f64p, f64p, f64p, f32p, i32p, i32p]
     L.lm_track.argtypes = [vp, u16p, c_int, c_int] + track_out
     L.lm_track_device.argtypes = [vp, vp, c_i64, c_int, c_f, c_int, c_int] + track_out + [vp]
+    batch_out = track_out[:2] + [i32p] + track_out[3:]  # n_objects [n_frames] in place of n
+    L.lm_track_batch.argtypes = [vp, c_int, u16p, c_int, c_int] + batch_out
+    L.lm_track_batch_device.argtypes = [vp, c_int, ctypes.POINTER(vp), c_i64, c_int, c_f, c_int, c_int] + batch_out + [vp]
     L.lm_pose_transforms.argtypes = [vp, f64p, c_i64, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -1196,9 +1199,35 @@ class NativeDetector:
                                                               int(rows), int(cols), *a, stream), sceneK, objects, max_iterations,
                            margin_px, estimation)
 
-    def _track(self, fn, sceneK, objects, max_iterations, margin_px, estimation):
+    def track_batch(self, depth, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane"):
+        """lm_track_batch on u16 [n,H,W] numpy depths (mm), sceneK [n,3,3].  objects: one list of (class_index, template_id,
+        T) triples per frame.  Returns one tuple per frame, each what track returns for that frame."""
+        depth = np.ascontiguousarray(depth)
+        if depth.dtype != np.uint16 or depth.ndim != 3:
+            raise TypeError("depth must be uint16 [n,H,W] images (mm)")
+        n, rows, cols = depth.shape
+        return self._track(lambda *a: self._L.lm_track_batch(self._h, n, depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows, cols,
+                                                             *a), sceneK, objects, max_iterations, margin_px, estimation, n)
+
+    def track_batch_device(self, planes, pitch, depth_format, depth_scale, rows, cols, stream, sceneK, objects, max_iterations=30,
+                           margin_px=4, estimation="point_to_plane"):
+        """lm_track_batch_device on device planes (data pointers, one pitch, format and depth_scale) ordered on `stream`.
+        Returns what track_batch returns."""
+        n = len(planes)
+        ptrs = (ctypes.c_void_p * max(n, 1))(*planes)
+        return self._track(lambda *a: self._L.lm_track_batch_device(self._h, n, ptrs, int(pitch), int(depth_format), ctypes.c_float(depth_scale),
+                                                                    int(rows), int(cols), *a, stream), sceneK, objects, max_iterations,
+                           margin_px, estimation, n)
+
+    def _track(self, fn, sceneK, objects, max_iterations, margin_px, estimation, n_frames=None):
+        # n_frames None: one frame's objects (lm_track); else one list of objects per frame, and one result tuple per frame
         est = estimation_code(estimation)
-        sK = np.ascontiguousarray(sceneK, np.float32).reshape(9)
+        sK = np.ascontiguousarray(sceneK, np.float32).reshape(-1)
+        counts = None if n_frames is None else np.ascontiguousarray([len(o) for o in objects], np.int32)
+        if counts is not None:
+            if len(counts) != n_frames or sK.size != 9 * n_frames:
+                raise ValueError("%d frames, %d object lists and %d intrinsics" % (n_frames, len(counts), sK.size // 9))
+            objects = [o for frame in objects for o in frame]
         n = len(objects)
         arr = self.track_objects(objects)
         T = np.stack([np.asarray(o[2], np.float64).reshape(4, 4) for o in objects]) if n else np.zeros((0, 4, 4))
@@ -1211,9 +1240,14 @@ class NativeDetector:
         f32p, f64p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
         Tout = T if n else np.zeros((1, 4, 4))
         check(self._L.lm_set_pose_estimation(self._h, est))
-        check(fn(sK.ctypes.data_as(f32p), ctypes.cast(arr, ctypes.c_void_p), n, int(max_iterations), int(margin_px), Tout.ctypes.data_as(f64p), Ro.ctypes.data_as(f64p),
-                 to.ctypes.data_as(f64p), res.ctypes.data_as(f32p), self._i32(status), self._i32(box)))
-        return status[:n].copy(), Tout[:n].copy(), Ro[:n].copy(), to[:n].copy(), res[:n].copy(), box[:n].copy()
+        check(fn(sK.ctypes.data_as(f32p), ctypes.cast(arr, ctypes.c_void_p), n if counts is None else self._i32(counts), int(max_iterations),
+                 int(margin_px), Tout.ctypes.data_as(f64p), Ro.ctypes.data_as(f64p), to.ctypes.data_as(f64p), res.ctypes.data_as(f32p),
+                 self._i32(status), self._i32(box)))
+        got = status[:n].copy(), Tout[:n].copy(), Ro[:n].copy(), to[:n].copy(), res[:n].copy(), box[:n].copy()
+        if counts is None:
+            return got
+        starts = np.cumsum(np.concatenate([[0], counts]))
+        return [tuple(a[s:e] for a in got) for s, e in zip(starts[:-1], starts[1:])]
 
 
 class TrackObject(ctypes.Structure):

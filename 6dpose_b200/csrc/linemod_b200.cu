@@ -2456,44 +2456,70 @@ extern "C" int lm_debug_pose_clouds(lm_detector* d, int slot, int what, void* ou
   return pose_stage_clouds(d->pose, slot, what, out, cap);
 }
 
-// lm_track and lm_track_device: every refusal before any device work, then the scene (dev null: host depth, copied) and
-// one track run of the pose stage on the detector's stream.
-static int track(lm_detector* d, const void* depth, const DeviceFrame* dev, cudaStream_t caller, int rows, int cols, const float* sceneK,
-                 const lm_track_object* objects, int n, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out,
+// Object i of a track call (objects of its frame, or of lm_track) as the pose stage's TrackObject: LM_E_INVALID or
+// LM_E_STATE with the message unless its class, template, T and render are good.
+static int track_object(lm_detector* d, const lm_track_object& o, int i, TrackObject* out) {
+  if (o.class_index < 0 || o.class_index >= d->n_classes)
+    return fail(LM_E_INVALID, "object %d: class %d outside the bank's %d classes", i, o.class_index, d->n_classes);
+  const int32_t nt = d->class_begin[o.class_index + 1] - d->class_begin[o.class_index];
+  if (o.template_id < 0 || o.template_id >= nt)
+    return fail(LM_E_INVALID, "object %d: template %d outside class %d's %d templates", i, o.template_id, o.class_index, nt);
+  for (int k = 0; k < 16; ++k)
+    if (!std::isfinite(o.T[k])) return fail(LM_E_INVALID, "object %d: T[%d] is not finite", i, k);
+  out->g = d->class_begin[o.class_index] + o.template_id;
+  memcpy(out->T, o.T, sizeof(o.T));
+  const int32_t g = (int32_t)out->g;
+  if (!d->pose || !pose_stage_covers(d->pose, &g, 1))
+    return fail(LM_E_STATE, "object %d: no template render registered for class %d, template %d (lm_set_template_renders)", i,
+                o.class_index, o.template_id);
+  return LM_OK;
+}
+
+// lm_track, lm_track_device, lm_track_batch and lm_track_batch_device: every refusal before any device work, then the
+// scenes and one track run of the pose stage on the detector's stream.  planes null: n_frames host images contiguous at
+// depth; else frame f's device plane planes[f] (pitch, format, scale), ordered on `caller`.  Frame f has n_objects[f]
+// objects, in frame order; batch false (lm_track, lm_track_device: one frame): the single call's messages.
+static int track(lm_detector* d, bool batch, int n_frames, const void* depth, const void* const* planes, int64_t pitch, int format,
+                 float scale, cudaStream_t caller, int rows, int cols, const float* sceneK, const lm_track_object* objects,
+                 const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out,
                  float* residual, int32_t* status, int32_t* box) {
+  if (batch) {
+    if (!d || !depth || !sceneK || !n_objects) return fail(LM_E_INVALID, "null argument");
+    if (n_frames < 1) return fail(LM_E_INVALID, "n_frames %d < 1", n_frames);
+    for (int f = 0; f < n_frames; ++f)
+      if (n_objects[f] < 0 || n_objects[f] > LM_POST_MAX)
+        return fail(LM_E_INVALID, "frame %d: %d objects, a track run takes 0 to %d per frame", f, n_objects[f], LM_POST_MAX);
+  }
+  std::vector<int64_t> first((size_t)n_frames + 1, 0);
+  for (int f = 0; f < n_frames; ++f) first[(size_t)f + 1] = first[(size_t)f] + n_objects[f];
+  const int64_t n = first[(size_t)n_frames];
   if (!d || !depth || !sceneK || n < 0 || (n > 0 && (!objects || !T_out || !R_out || !t_out || !residual || !status || !box)))
-    return fail(LM_E_INVALID, "null argument or n < 0");
-  if (n > LM_POST_MAX) return fail(LM_E_INVALID, "%d objects, a track run takes at most %d", n, LM_POST_MAX);
+    return fail(LM_E_INVALID, batch ? "null argument" : "null argument or n < 0");
+  if (n > LM_POST_MAX && !batch) return fail(LM_E_INVALID, "%d objects, a track run takes at most %d", (int)n, LM_POST_MAX);
   if (rows <= 0 || cols <= 0) return fail(LM_E_INVALID, "empty depth image %d x %d", rows, cols);
   if (max_iterations < 0) return fail(LM_E_INVALID, "max_iterations < 0");
   if (margin_px < 0) return fail(LM_E_INVALID, "margin_px %d < 0", margin_px);
-  int rc = dev ? check_depth_format("depth", dev->format, dev->scale) : LM_OK;
+  int rc = planes ? check_depth_format("depth", format, scale) : LM_OK;
   if (rc) return rc;
   if (d->pose_estimation == LM_POSE_PSO)
     return fail(LM_E_STATE, "tracking runs an ICP: LM_POSE_PSO starts from an identity rotation (lm_set_pose_estimation)");
   if (d->px_rank >= 0) return fail(LM_E_STATE, "tracking does not run with a connected peer exchange");
   std::vector<TrackObject> obj((size_t)n);
-  for (int i = 0; i < n; ++i) {
-    const lm_track_object& o = objects[i];
-    if (o.class_index < 0 || o.class_index >= d->n_classes)
-      return fail(LM_E_INVALID, "object %d: class %d outside the bank's %d classes", i, o.class_index, d->n_classes);
-    const int32_t nt = d->class_begin[o.class_index + 1] - d->class_begin[o.class_index];
-    if (o.template_id < 0 || o.template_id >= nt)
-      return fail(LM_E_INVALID, "object %d: template %d outside class %d's %d templates", i, o.template_id, o.class_index, nt);
-    for (int k = 0; k < 16; ++k)
-      if (!std::isfinite(o.T[k])) return fail(LM_E_INVALID, "object %d: T[%d] is not finite", i, k);
-    obj[(size_t)i].g = d->class_begin[o.class_index] + o.template_id;
-    memcpy(obj[(size_t)i].T, o.T, sizeof(o.T));
-    const int32_t g = (int32_t)obj[(size_t)i].g;
-    if (!d->pose || !pose_stage_covers(d->pose, &g, 1))
-      return fail(LM_E_STATE, "object %d: no template render registered for class %d, template %d (lm_set_template_renders)", i,
-                  o.class_index, o.template_id);
-  }
+  for (int f = 0; f < n_frames; ++f)
+    for (int64_t k = first[(size_t)f]; k < first[(size_t)f + 1]; ++k) {
+      rc = track_object(d, objects[k], (int)(k - first[(size_t)f]), &obj[(size_t)k]);
+      if (rc && batch) return fail(rc, "frame %d: %s", f, std::string(g_err).c_str());
+      if (rc) return rc;
+    }
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
-  if (dev) {
+  if (planes) {
     rc = check_device_stream(d->device, caller);
-    const int sz = dev->format == LM_DEPTH_F32 ? 4 : 2;
-    if (!rc) rc = check_device_plane(d->device, "depth", depth, dev->depth_pitch, (int64_t)sz * cols, sz);
+    const int sz = format == LM_DEPTH_F32 ? 4 : 2;
+    for (int f = 0; f < n_frames && !rc; ++f) {
+      char what[40] = "depth";
+      if (batch) snprintf(what, sizeof(what), "depth[%d]", f);
+      rc = check_device_plane(d->device, what, planes[f], pitch, (int64_t)sz * cols, sz);
+    }
     if (rc) return rc;
   }
   if (!d->pose) return fail(LM_E_STATE, "no template renders registered (lm_set_template_renders)");
@@ -2501,36 +2527,51 @@ static int track(lm_detector* d, const void* depth, const DeviceFrame* dev, cuda
   cudaStream_t st = d->stream.get();
   d->chain.pose = d->chain.pose_nms = false;  // the stage's buffers now hold the track run: a pending frame's pose stage is abandoned
   const uint16_t* scene = nullptr;
-  if (dev) {  // the reads of the caller's plane start behind its stream's work, and its later work waits for the conversion
+  if (planes) {  // the reads of the caller's planes start behind its stream's work, and its later work waits for the conversions
     if (!d->ev_in.get()) CU(d->ev_in.create(cudaEventDisableTiming));
     if (!d->ev_out.get()) CU(d->ev_out.create(cudaEventDisableTiming));
     CU(cudaEventRecord(d->ev_in.get(), caller));
     CU(cudaStreamWaitEvent(st, d->ev_in.get(), 0));
-    rc = pose_track_scene(d->pose, st, false, depth, dev->depth_pitch, dev->format, dev->scale, rows, cols, &scene, &d->launches);
+    rc = pose_track_scene(d->pose, st, n_frames, nullptr, planes, pitch, format, scale, rows, cols, &scene, &d->launches);
     CU(cudaEventRecord(d->ev_out.get(), st));
     CU(cudaStreamWaitEvent(caller, d->ev_out.get(), 0));
   } else {
-    rc = pose_track_scene(d->pose, st, true, depth, 2 * (int64_t)cols, LM_DEPTH_U16_MM, 1.f, rows, cols, &scene, &d->launches);
+    rc = pose_track_scene(d->pose, st, n_frames, static_cast<const uint16_t*>(depth), nullptr, 2 * (int64_t)cols, LM_DEPTH_U16_MM, 1.f,
+                          rows, cols, &scene, &d->launches);
   }
   if (rc) return rc;
   PoseOptions o = {rows, cols, 1, max_iterations, d->pose_estimation, st, nullptr, d->pose_verify, d->pose_search};
-  return pose_stage_track(d->pose, o, scene, sceneK, obj.data(), n, margin_px, &d->launches, T_out, R_out, t_out, residual, status, box);
+  return pose_stage_track(d->pose, o, n_frames, scene, sceneK, obj.data(), first.data(), margin_px, &d->launches, T_out, R_out, t_out,
+                          residual, status, box);
 }
 
 extern "C" int lm_track(lm_detector* d, const uint16_t* depth, int rows, int cols, const float* sceneK, const lm_track_object* objects,
                         int n, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out, float* residual,
                         int32_t* status, int32_t* box) {
-  return track(d, depth, nullptr, nullptr, rows, cols, sceneK, objects, n, max_iterations, margin_px, T_out, R_out, t_out, residual,
-               status, box);
+  return track(d, false, 1, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, &n, max_iterations, margin_px,
+               T_out, R_out, t_out, residual, status, box);
 }
 
 extern "C" int lm_track_device(lm_detector* d, const void* depth, int64_t depth_pitch, int depth_format, float depth_scale, int rows,
                                int cols, const float* sceneK, const lm_track_object* objects, int n, int max_iterations, int margin_px,
                                double* T_out, double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
-  DeviceFrame f = {};
-  f.depth = depth; f.depth_pitch = depth_pitch; f.format = depth_format; f.scale = depth_scale;
-  return track(d, depth, &f, (cudaStream_t)stream, rows, cols, sceneK, objects, n, max_iterations, margin_px, T_out, R_out, t_out,
-               residual, status, box);
+  return track(d, false, 1, depth, &depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK, objects, &n,
+               max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
+}
+
+extern "C" int lm_track_batch(lm_detector* d, int n_frames, const uint16_t* depth, int rows, int cols, const float* sceneK,
+                              const lm_track_object* objects, const int32_t* n_objects, int max_iterations, int margin_px, double* T_out,
+                              double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box) {
+  return track(d, true, n_frames, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, n_objects, max_iterations,
+               margin_px, T_out, R_out, t_out, residual, status, box);
+}
+
+extern "C" int lm_track_batch_device(lm_detector* d, int n_frames, const void* const* depth, int64_t depth_pitch, int depth_format,
+                                     float depth_scale, int rows, int cols, const float* sceneK, const lm_track_object* objects,
+                                     const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out,
+                                     double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
+  return track(d, true, n_frames, depth, depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK, objects,
+               n_objects, max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
 }
 
 extern "C" int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n) {

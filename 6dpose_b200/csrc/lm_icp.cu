@@ -1260,7 +1260,11 @@ struct TrackParams {
   const TrackObject* obj;     // [n] template (bank index) and T
   const PoseTpl* tpl;
   const uint16_t* crops;
-  VerifyScene sc;             // the scene depth and intrinsics
+  // object i's frame frame_of[i] (null: frame 0): its depth scene + frame * srows * scols, its intrinsics sKs + 9 * frame
+  const uint16_t* scene;
+  int32_t srows, scols;
+  const int32_t* frame_of;
+  const float* sKs;
   int32_t margin;
   int64_t cap;                // most window pixels (LM_TRACK_WINDOW beyond)
   int64_t stride, M;          // points per object: M model points, then cap scene points
@@ -1316,6 +1320,7 @@ __device__ __forceinline__ bool track_project(const double* T, double px, double
 // its points is projected under T (track_project) and the in-frame pixels' extent is reduced over the CTA.  The
 // window's pixels with scene depth > 0 are back-projected in row-major order as k_pose_cloud back-projects the scene.
 // Both clouds get their voxel keys; the job starts at T.  An object without the status TRACKED writes an empty job.
+// Everything an object's CTA computes depends only on the object and its own frame's depth and intrinsics.
 __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
   typedef cub::BlockScan<int, POSE_THREADS> Scan;
   typedef cub::BlockReduce<double, POSE_THREADS> Reduce;
@@ -1327,11 +1332,19 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
   __shared__ int s_ext[4], s_win[4], s_status;
   const int i = blockIdx.x, tid = threadIdx.x;
   const PoseTpl T = p.tpl[p.obj[i].g];
+  __shared__ VerifyScene sc;  // the object's frame (shared: it stays out of the registers)
   const size_t sm = (size_t)i * p.stride, ss = sm + p.M;
   double* __restrict__ Mp = p.raw + sm * 3;
   double* __restrict__ Sp = p.raw + ss * 3;
   if (tid < 16) s_T[tid] = p.obj[i].T[tid];
-  if (tid == 0) { s_ext[0] = s_ext[1] = INT_MAX; s_ext[2] = s_ext[3] = -1; }
+  if (tid == 0) {
+    s_ext[0] = s_ext[1] = INT_MAX; s_ext[2] = s_ext[3] = -1;
+    const int frame = p.frame_of ? p.frame_of[i] : 0;
+    const float* fK = p.sKs + 9 * frame;
+    sc.depth = p.scene + (size_t)frame * p.srows * p.scols;
+    sc.rows = p.srows; sc.cols = p.scols;
+    sc.fx = fK[0]; sc.cx = fK[2]; sc.fy = fK[4]; sc.cy = fK[5];
+  }
   __syncthreads();
   const uint16_t* __restrict__ C = p.crops + T.crop;
   const int bw = T.bw, npix = T.bw * T.bh;
@@ -1348,7 +1361,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
       mx = pose_backproject(q + T.bx, T.K[2], T.K[0], mz);
       my = pose_backproject(r + T.by, T.K[5], T.K[4], mz);
       int pc, pr;
-      if (track_project(s_T, mx, my, mz, p.sc, &pc, &pr)) {
+      if (track_project(s_T, mx, my, mz, sc, &pc, &pr)) {
         c0 = min(c0, pc); c1 = max(c1, pc);
         r0 = min(r0, pr); r1 = max(r1, pr);
       }
@@ -1374,7 +1387,7 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
       const int64_t x0 = s_ext[0], y0 = s_ext[1], x1 = s_ext[2], y1 = s_ext[3], m = p.margin;
       rc.box[0] = (int)x0; rc.box[1] = (int)y0; rc.box[2] = (int)(x1 - x0 + 1); rc.box[3] = (int)(y1 - y0 + 1);
       const int64_t wx0 = max(x0 - m, (int64_t)0), wy0 = max(y0 - m, (int64_t)0);
-      const int64_t wx1 = min(x1 + m, (int64_t)p.sc.cols - 1), wy1 = min(y1 + m, (int64_t)p.sc.rows - 1);
+      const int64_t wx1 = min(x1 + m, (int64_t)sc.cols - 1), wy1 = min(y1 + m, (int64_t)sc.rows - 1);
       s_win[0] = (int)wx0; s_win[1] = (int)wy0; s_win[2] = (int)(wx1 - wx0 + 1); s_win[3] = (int)(wy1 - wy0 + 1);
       for (int k = 0; k < 4; ++k) rc.window[k] = s_win[k];
       if ((int64_t)s_win[2] * s_win[3] > p.cap) st = LM_TRACK_WINDOW;
@@ -1392,13 +1405,13 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
       double sx = 0, sy = 0, sz = 0;
       if (k < wpix) {
         const int r = k / ww, q = k - r * ww;
-        const int sr = wy + r, sc = wx + q;
-        const uint16_t sd = p.sc.depth[(size_t)sr * p.sc.cols + sc];
+        const int sr = wy + r, scol = wx + q;
+        const uint16_t sd = sc.depth[(size_t)sr * sc.cols + scol];
         if (sd > 0) {
           fs = true;
           sz = __ddiv_rn((double)sd, 1000.0);
-          sx = pose_backproject(sc, p.sc.cx, p.sc.fx, sz);
-          sy = pose_backproject(sr, p.sc.cy, p.sc.fy, sz);
+          sx = pose_backproject(scol, sc.cx, sc.fx, sz);
+          sy = pose_backproject(sr, sc.cy, sc.fy, sz);
         }
       }
       int excl, agg;
@@ -1951,7 +1964,7 @@ struct lm_pose_stage {
   DeviceArray<uint8_t> d_posed;
   // A group of buffers that grows together is freed as a whole, then allocated in order: its last array is empty
   // unless every one was allocated, so its size stands for the group's.
-  // a batch's scene slots and survivors, filled by the caller (pose_batch_reserve)
+  // a batch's scene slots and survivors, filled by the caller (pose_batch_reserve), and a track run's scenes
   DeviceArray<uint16_t> d_bscene;
   DeviceArray<lm_match> d_bsurv;
   // a run's outputs (pose_outputs), a frame's at offset 0: per survivor its frame, ICP output and posed flag
@@ -1984,10 +1997,9 @@ struct lm_pose_stage {
     int slots = 0, rank = 0, world = 1;
     int64_t first = 0;
     const uint8_t* posed = nullptr;
-    bool track = false;  // a track chunk: d_trec holds its windows
+    bool track = false;  // a track chunk: d_trec holds its windows from `first` on
   } last;
-  // tracking (pose_stage_track): the scene, the objects and their windows
-  DeviceArray<uint16_t> d_tscene;
+  // tracking (pose_stage_track; its scenes are in d_bscene): the objects of the run and their windows
   DeviceArray<TrackObject> d_tobj;
   DeviceArray<TrackRec> d_trec; PinnedArray<TrackRec> h_trec;
   // the run last finished, for pose_stage_transforms: finished_ok false once another run is prepared or it failed; its
@@ -2166,7 +2178,8 @@ struct PoseChunk {
   long long* record = nullptr;
   int64_t record_words = 0;
   // a track chunk (lm_track; null: survivors): k_track_cloud builds the clouds from these objects instead of
-  // k_pose_cloud; the stage's buffers, seg_begin / seg_end, jobs, err and posed are filled in by pose_chunk
+  // k_pose_cloud; the stage's buffers, seg_begin / seg_end, jobs, err, posed, the scene and the frame tables are filled
+  // in by pose_chunk
   const TrackParams* track = nullptr;
 };
 
@@ -2200,6 +2213,7 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
     TrackParams q = *c.track;
     q.raw = p.raw; q.keys = p.keys; q.vals = p.vals; q.seg_begin = p.seg_begin; q.seg_end = p.seg_end;
     q.jobs = p.jobs; q.err = p.err; q.posed = p.posed;
+    q.scene = c.scene; q.srows = o.srows; q.scols = o.scols; q.frame_of = c.frame_of; q.sKs = c.sKs;
     items = n * q.stride; tgt_max = q.cap;
     k_track_cloud<<<n, POSE_THREADS, 0, st>>>(q);
   } else {
@@ -2282,7 +2296,7 @@ int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int
     CUI(cudaMemcpy(&posed, l.posed + slot, 1, cudaMemcpyDeviceToHost));
     if (what == LM_POSE_CAPTURE_WINDOW) {
       TrackRec rec;
-      CUI(cudaMemcpy(&rec, s->d_trec.get() + slot, sizeof(rec), cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(&rec, s->d_trec.get() + l.first + slot, sizeof(rec), cudaMemcpyDeviceToHost));
       const int32_t w5[5] = {rec.window[0], rec.window[1], rec.window[2], rec.window[3], rec.status};
       if (cap < (int64_t)sizeof(w5))
         return lm_fail(LM_E_CAPACITY, "pose stage capture item %d of slot %d needs %lld bytes, cap is %lld", what, slot, (long long)sizeof(w5),
@@ -3174,42 +3188,45 @@ extern "C" int lm_icp_process_batch_device(lm_icp* h, int n_hyp, const void* sce
 }
 
 // --------------------------------------------------------------------------------------------
-// tracking on the detector's pose stage (lm_track, lm_track_device) and the transformations of a finished run
+// tracking on the detector's pose stage (lm_track, lm_track_device, lm_track_batch, lm_track_batch_device) and the
+// transformations of a finished run
 // --------------------------------------------------------------------------------------------
-int pose_track_scene(lm_pose_stage* s, cudaStream_t st, bool host, const void* depth, int64_t pitch, int format, float scale, int rows,
-                     int cols, const uint16_t** d_scene, int64_t* launches) {
+int pose_track_scene(lm_pose_stage* s, cudaStream_t st, int n_frames, const uint16_t* host, const void* const* planes, int64_t pitch,
+                     int format, float scale, int rows, int cols, const uint16_t** d_scene, int64_t* launches) {
   const size_t npix = (size_t)rows * cols;
-  if (npix > s->d_tscene.size()) {
+  if ((size_t)n_frames * npix > s->d_bscene.size()) {
     CUI(cudaStreamSynchronize(st));  // an earlier run may still read it
-    CUI(s->d_tscene.reserve(npix));
+    CUI(s->d_bscene.reserve((size_t)n_frames * npix));
   }
   if (host) {
-    CUI(cudaMemcpyAsync(s->d_tscene.get(), depth, sizeof(uint16_t) * npix, cudaMemcpyHostToDevice, st));
+    CUI(cudaMemcpyAsync(s->d_bscene.get(), host, sizeof(uint16_t) * n_frames * npix, cudaMemcpyHostToDevice, st));
   } else {
-    launch_scene(depth, pitch, format, scale, rows, cols, s->d_tscene.get(), st);
+    for (int f = 0; f < n_frames; ++f) launch_scene(planes[f], pitch, format, scale, rows, cols, s->d_bscene.get() + f * npix, st);
     CUI(cudaGetLastError());
-    ++*launches;
+    *launches += n_frames;
   }
-  *d_scene = s->d_tscene.get();
+  *d_scene = s->d_bscene.get();
   return LM_OK;
 }
 
-int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_scene, const float* sK, const TrackObject* obj, int n,
-                     int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual, int32_t* status,
-                     int32_t* box) {
+int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const uint16_t* d_scene, const float* sK, const TrackObject* obj,
+                     const int64_t* first, int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual,
+                     int32_t* status, int32_t* box) {
   cudaStream_t st = o.stream;
   const bool verify = o.verify.on != 0;
+  const int64_t n = first[n_frames];
+  const int nc = pose_batch_chunks(n);
   pose_forget(s);
-  int rc = pose_prepare(s, st, 1, n, verify);
+  int rc = pose_prepare(s, st, n_frames, n, verify);
   if (rc) return rc;
   if (n == 0) {
     s->verified = verify;
     s->finished_ok = true;
     return LM_OK;
   }
-  // object i's clouds: M model points (the largest crop), then a window of up to 4 M scene points
-  const int64_t M = s->area_max, W = 4 * M, stride = M + W;
-  rc = pose_buffers(s, st, (int)((n * stride + 2 * M - 1) / (2 * M)), M);
+  // a chunk's object i: M model points (the largest crop), then a window of up to 4 M scene points
+  const int64_t M = s->area_max, W = 4 * M, stride = M + W, slots = std::min<int64_t>(n, POSE_CHUNK);
+  rc = pose_buffers(s, st, (int)((slots * stride + 2 * M - 1) / (2 * M)), M);
   if (rc) return rc;
   if ((size_t)n > s->h_trec.size()) {
     CUI(cudaStreamSynchronize(st));
@@ -3218,31 +3235,39 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_s
     CUI(s->d_trec.assign(n));
     CUI(s->h_trec.assign(n));
   }
+  // each object's frame and each frame's intrinsics, which k_track_cloud and k_pose_verify read
+  std::vector<int32_t> frame_of((size_t)n);
+  for (int f = 0; f < n_frames; ++f)
+    for (int64_t k = first[f]; k < first[f + 1]; ++k) frame_of[(size_t)k] = f;
   CUI(cudaMemcpyAsync(s->d_tobj.get(), obj, sizeof(TrackObject) * n, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4, st));
-  TrackParams q;
-  memset(&q, 0, sizeof(q));
-  q.obj = s->d_tobj.get(); q.tpl = s->d_tpl.get(); q.crops = s->d_crops.get();
-  q.sc.depth = d_scene; q.sc.rows = o.srows; q.sc.cols = o.scols;
-  q.sc.fx = sK[0]; q.sc.cx = sK[2]; q.sc.fy = sK[4]; q.sc.cy = sK[5];
-  q.margin = margin; q.cap = W; q.stride = stride; q.M = M;
-  q.rec = s->d_trec.get();
-  PoseChunk k = run_chunk(s, o, 0, nullptr, nullptr, n, d_scene, sK);
-  k.track = &q;
-  const int l = pose_chunk(s, o, k);
-  if (l < 0) return l;
-  *launches += l;
+  CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemcpyAsync(s->d_bsK.get(), sK, sizeof(float) * 9 * n_frames, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4 * nc, st));
+  for (int c = 0; c < nc; ++c) {
+    const int64_t c0 = (int64_t)c * POSE_CHUNK;
+    TrackParams q;
+    memset(&q, 0, sizeof(q));
+    q.obj = s->d_tobj.get() + c0; q.tpl = s->d_tpl.get(); q.crops = s->d_crops.get();
+    q.margin = margin; q.cap = W; q.stride = stride; q.M = M;
+    q.rec = s->d_trec.get() + c0;
+    PoseChunk k = run_chunk(s, o, c, nullptr, nullptr, (int)std::min<int64_t>(n - c0, POSE_CHUNK), d_scene, nullptr);
+    k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get();
+    k.track = &q;
+    const int l = pose_chunk(s, o, k);
+    if (l < 0) return l;
+    *launches += l;
+  }
   CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
   CUI(cudaMemcpyAsync(s->h_trec.get(), s->d_trec.get(), sizeof(TrackRec) * n, cudaMemcpyDeviceToHost, st));
   if (verify) CUI(cudaMemcpyAsync(s->h_bver.get(), s->d_bver.get(), sizeof(PoseVerify) * n, cudaMemcpyDeviceToHost, st));
-  CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4, cudaMemcpyDeviceToHost, st));
+  CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
   int64_t published = 0;
-  rc = pose_status(s->h_bstat.get(), 1, false, 0, 0, false, &published);
+  rc = pose_status(s->h_bstat.get(), nc, false, 0, 0, nc > 1, &published);
   if (rc) return rc;
   s->xf.assign(16 * (size_t)n, std::numeric_limits<double>::quiet_NaN());
-  for (int i = 0; i < n; ++i) {
+  for (int64_t i = 0; i < n; ++i) {
     const TrackRec& e = s->h_trec[(size_t)i];
     status[i] = e.status;
     memcpy(box + 4 * i, e.box, sizeof(e.box));

@@ -8,8 +8,9 @@
 // of frames, and a single frame is a one-frame run of the same stage: the same chunks, outputs, readbacks and finish.
 // The host composes result = T * init_base after the copy.  The pose NMS (k_pose_nms, one CTA per frame behind the ICP
 // kernel) composes the poses on the device instead, runs the greedy translation NMS of linemod_ros/detect.py over them
-// and compacts the kept ones into one output block.  A track run (lm_track) is one chunk whose clouds k_track_cloud builds
-// from each object's transformation and the window its model projects to, in place of k_pose_cloud.
+// and compacts the kept ones into one output block.  A track run (lm_track, lm_track_batch) is a run whose clouds
+// k_track_cloud builds from each object's transformation and the window its model projects to in its own frame, in
+// place of k_pose_cloud.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -126,17 +127,20 @@ struct TrackObject {
   int64_t g;
   double T[16];
 };
-// The scene of a track run on o.stream: rows x cols u16 mm in the stage's own buffer.  host: depth is a host image,
-// copied; else a caller's device plane (pitch bytes between rows, LM_DEPTH_U16_MM or LM_DEPTH_F32 with scale),
-// converted as lm_bind_images_device converts it.
-int pose_track_scene(lm_pose_stage* s, cudaStream_t st, bool host, const void* depth, int64_t pitch, int format, float scale, int rows,
-                     int cols, const uint16_t** d_scene, int64_t* launches);
-// One track run of n <= 1024 objects against the scene of pose_track_scene, o.estimation an ICP: one chunk, then the
-// outputs of lm_track (an entry without the status TRACKED leaves its T, R, t untouched and gets residual -1).  Returns
-// once they are on the host; the run is then the stage's last finished run (pose_stage_verify, pose_stage_transforms).
-int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, const uint16_t* d_scene, const float* sK, const TrackObject* obj, int n,
-                     int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual, int32_t* status,
-                     int32_t* box);
+// The scenes of a track run on o.stream: n_frames rows x cols u16 mm frames in the stage's batch scene slots (frame f
+// at *d_scene + f * rows * cols; grown, never shrunk, and shared with pose_batch_reserve).  host: n_frames contiguous
+// host images, copied at once; else the caller's device planes planes[f] (pitch bytes between rows, LM_DEPTH_U16_MM or
+// LM_DEPTH_F32 with scale), converted as lm_bind_images_device converts them, one launch per frame.
+int pose_track_scene(lm_pose_stage* s, cudaStream_t st, int n_frames, const uint16_t* host, const void* const* planes, int64_t pitch,
+                     int format, float scale, int rows, int cols, const uint16_t** d_scene, int64_t* launches);
+// One track run against the scenes of pose_track_scene, o.estimation an ICP: frame f's objects are obj[first[f],
+// first[f + 1]) (at most 1024 per frame), its intrinsics sK + 9f; one chunk per 1024 objects, frames straddling chunk
+// boundaries.  Then the outputs of lm_track in object order (an entry without the status TRACKED leaves its T, R, t
+// untouched and gets residual -1).  Returns once they are on the host; the run is then the stage's last finished run
+// (pose_stage_verify, pose_stage_transforms).  lm_track is the one-frame run.
+int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const uint16_t* d_scene, const float* sK, const TrackObject* obj,
+                     const int64_t* first, int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual,
+                     int32_t* status, int32_t* box);
 // The transformation of every entry of the run last finished (lm_pose_transforms), in entry order, T_out + 16k; NaN for an
 // entry without a pose.  LM_E_STATE once another run has been enqueued or the last one failed; LM_E_CAPACITY (with *n)
 // beyond cap.  The pose NMS's kept entries are matched to their survivors on the host, from one copy of the run's ICP

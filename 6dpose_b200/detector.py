@@ -424,7 +424,6 @@ class Detector:
     def _batch_inputs(self, frames, sceneK, masks, what, depth_scale=1.0, stream=None):
         # every check that needs no device, before the native handle exists.  Returns (inputs, K): inputs is a
         # _lib.DeviceBatch for CUDA tensor frames, else (rgb [n,H,W,3], depth [n,H,W], mask pairs or None)
-        from .pose_refine import poseRefine
         frames = list(frames)
         if not frames:
             raise ValueError("%s: no frames" % what)
@@ -443,13 +442,7 @@ class Detector:
             if any(r.shape != rgb[0].shape or d.shape != rgb[0].shape[:2] for r, d in zip(rgb, depth)):
                 raise ValueError("%s: every frame's colour and depth images must have one size" % what)
         n = len(frames)
-        K = np.asarray(sceneK)
-        if K.size == 9:
-            K = np.repeat(poseRefine._mat(K, np.float32, (3, 3), "sceneK")[None], n, 0)
-        elif K.shape == (n, 3, 3):
-            K = poseRefine._mat(K, np.float32, (n, 3, 3), "sceneK")
-        else:
-            raise ValueError("%s: sceneK must be one 3x3 matrix or %d of them, got shape %s" % (what, n, K.shape))
+        K = self._frame_ks(sceneK, n, what)
         if masks is None:
             raise TypeError("%s: masks must be a list; pass masks=[]" % what)
         masks = list(masks)
@@ -470,6 +463,17 @@ class Detector:
             except ValueError as e:
                 raise ValueError("%s: %s" % (what, e)) from None
         return (np.stack(rgb), np.stack(depth), pairs), K
+
+    @staticmethod
+    def _frame_ks(sceneK, n, what):
+        # one 3x3 f32 intrinsics per frame of a batch call, from one matrix or n of them
+        from .pose_refine import poseRefine
+        K = np.asarray(sceneK)
+        if K.size == 9:
+            return np.repeat(poseRefine._mat(K, np.float32, (3, 3), "sceneK")[None], n, 0)
+        if K.shape == (n, 3, 3):
+            return poseRefine._mat(K, np.float32, (n, 3, 3), "sceneK")
+        raise ValueError("%s: sceneK must be one 3x3 matrix or %d of them, got shape %s" % (what, n, K.shape))
 
     def _pose_pairs(self, out, R, t, res, ver=None, T=None):
         # [(Match, poseRefine)]; a survivor without a pose (residual -1, only without the pose NMS) keeps R / t None.
@@ -503,14 +507,71 @@ class Detector:
         last three with residual -1 and the start's R, t and T.  With setPoseVerification, every entry carries its score.
         TypeError for a pair whose poseRefine has no transformation (refine_matches / process), ValueError for an unknown
         class or template; both before any device work."""
-        from .pose_refine import poseRefine, pose_to_transform
+        from .pose_refine import poseRefine
         _lib.estimation_code(estimation)
+        starts = self._track_starts(objects, "track")
+        sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
+        triples = [(c, t, T) for c, t, T, _, _, _ in starts]
+        if _lib.is_tensor(depth):
+            plane = self._depth_planes([depth], ["depth"], depth_scale, stream)
+            nat = self._pose_native(())
+            got = nat.track_device(plane[0][0], *plane[1:], sK, triples, max_iterations, margin_px, estimation)
+        else:
+            _lib.host_frame_options(depth_scale, stream)
+            depth = np.asarray(depth)
+            if depth.dtype != np.uint16 or depth.ndim != 2:
+                raise TypeError("depth must be a uint16 HxW depth image (mm)")
+            nat = self._pose_native(())
+            got = nat.track(depth, sK, triples, max_iterations, margin_px, estimation)
+        return self._track_pairs(starts, got, self._verification(nat, [len(starts)])[0], estimation)
+
+    def track_batch(self, depths, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane", depth_scale=1.0,
+                    stream=None):
+        """track for many frames in one call (lm_track_batch): several cameras, or several independent sequences at one time
+        step, whose objects then share one pose-stage run and fill the GPU where one frame's few objects cannot.  depths: a
+        sequence of uint16 HxW numpy images of one size, or of CUDA tensors of one size, row pitch and dtype (as track takes
+        them, with depth_scale and stream); sceneK: one 3x3 matrix or one per frame; objects: one list per frame, each entry
+        any kind track takes, at most 1024 per frame.  Returns one [(Match, poseRefine)] list per frame, each equal to track
+        on that frame alone.  TypeError / ValueError before any device work."""
+        _lib.estimation_code(estimation)
+        depths, objects = list(depths), [list(o) for o in objects]
+        n = len(depths)
+        if not n:
+            raise ValueError("track_batch: no frames")
+        if len(objects) != n:
+            raise ValueError("track_batch: %d object lists for %d frames" % (len(objects), n))
+        starts = [self._track_starts(o, "track_batch: frame %d" % f) for f, o in enumerate(objects)]
+        K = self._frame_ks(sceneK, n, "track_batch()")
+        triples = [[(c, t, T) for c, t, T, _, _, _ in s] for s in starts]
+        on_device = [_lib.is_tensor(d) for d in depths]
+        if any(on_device) and not all(on_device):
+            raise TypeError("track_batch: depths mix numpy arrays and torch tensors")
+        if on_device[0]:
+            planes = self._depth_planes(depths, ["depths[%d]" % f for f in range(n)], depth_scale, stream)
+            nat = self._pose_native(())
+            got = nat.track_batch_device(*planes, K, triples, max_iterations, margin_px, estimation)
+        else:
+            _lib.host_frame_options(depth_scale, stream)
+            depths = [np.asarray(d) for d in depths]
+            for f, d in enumerate(depths):
+                if d.dtype != np.uint16 or d.ndim != 2:
+                    raise TypeError("track_batch: depths[%d] must be a uint16 HxW depth image (mm)" % f)
+                if d.shape != depths[0].shape:
+                    raise ValueError("track_batch: depths[%d] is %s, depths[0] %s" % (f, d.shape, depths[0].shape))
+            nat = self._pose_native(())
+            got = nat.track_batch(np.stack(depths), K, triples, max_iterations, margin_px, estimation)
+        ver = self._verification(nat, [len(s) for s in starts])
+        return [self._track_pairs(s, g, v, estimation) for s, g, v in zip(starts, got, ver)]
+
+    def _track_starts(self, objects, what):
+        # track's objects as (class_index, template_id, T, Match, R, t); TypeError / ValueError naming `what`
+        from .pose_refine import poseRefine, pose_to_transform
         objects = list(objects)
         if len(objects) > _lib.TRACK_MAX:
-            raise ValueError("track: %d objects, at most %d per call" % (len(objects), _lib.TRACK_MAX))
+            raise ValueError("%s: %d objects, at most %d per frame" % (what, len(objects), _lib.TRACK_MAX))
         order = self.bank.class_ids()
         index = {c: i for i, c in enumerate(order)}
-        starts = []  # (class_index, template_id, T, Match, R, t)
+        starts = []
         for k, o in enumerate(objects):
             if isinstance(o, dict):
                 cid, tid = o["class_id"], int(o["template_id"])
@@ -521,40 +582,40 @@ class Detector:
                 cid, tid = m.class_id, int(m.template_id)
                 T = p.getTransformation() if isinstance(p, poseRefine) else None
                 if T is None:
-                    raise TypeError("track: object %d's poseRefine has no transformation (only match_refine, detect, the batch calls "
-                                    "and track return one)" % k)
+                    raise TypeError("%s: object %d's poseRefine has no transformation (only match_refine, detect, the batch calls "
+                                    "and track return one)" % (what, k))
                 R, t = p.getR(), p.getT()
             if cid not in index:
-                raise ValueError("track: object %d: class %r is not in the bank" % (k, cid))
+                raise ValueError("%s: object %d: class %r is not in the bank" % (what, k, cid))
             if not 0 <= tid < self.bank.num_templates(cid):
-                raise ValueError("track: object %d: template %d outside class %r's %d templates" % (k, tid, cid, self.bank.num_templates(cid)))
+                raise ValueError("%s: object %d: template %d outside class %r's %d templates" % (what, k, tid, cid, self.bank.num_templates(cid)))
             if T is None:
                 if cid not in self._render_poses:
-                    raise ValueError("track: object %d: class %r has no registered renders (setTemplateRenders)" % (k, cid))
+                    raise ValueError("%s: object %d: class %r has no registered renders (setTemplateRenders)" % (what, k, cid))
                 Rb, tb = self._render_poses[cid]
                 T = pose_to_transform(R, t, Rb[tid], tb[tid])
             starts.append((index[cid], tid, np.asarray(T, np.float64).reshape(4, 4), m, R, t))
-        sK = poseRefine._mat(sceneK, np.float32, (3, 3), "sceneK")
-        triples = [(c, t, T) for c, t, T, _, _, _ in starts]
-        if _lib.is_tensor(depth):
-            import torch
-            ptr, pitch, fmt = _lib._depth_plane(depth, "depth", torch)
-            scale = _lib._plane_scale(fmt == _lib.DEPTH_F32, depth_scale, "depth_scale", "depth")
-            if not depth.is_cuda or depth.device.index != int(self.device):
-                raise ValueError("depth is on %s; the detector runs on cuda:%d" % (depth.device, int(self.device)))
-            st = _lib.device_stream(stream, self.device)
-            nat = self._pose_native(())
-            got = nat.track_device(ptr, pitch, fmt, scale, int(depth.shape[0]), int(depth.shape[1]), st.cuda_stream, sK, triples,
-                                   max_iterations, margin_px, estimation)
-        else:
-            _lib.host_frame_options(depth_scale, stream)
-            depth = np.asarray(depth)
-            if depth.dtype != np.uint16 or depth.ndim != 2:
-                raise TypeError("depth must be a uint16 HxW depth image (mm)")
-            nat = self._pose_native(())
-            got = nat.track(depth, sK, triples, max_iterations, margin_px, estimation)
+        return starts
+
+    def _depth_planes(self, tensors, names, depth_scale, stream):
+        # CUDA depth tensors of one size, row pitch and dtype on the detector's device: (pointers, pitch, format, scale,
+        # rows, cols, stream handle)
+        import torch
+        planes = [_lib._depth_plane(t, name, torch) for t, name in zip(tensors, names)]
+        for t, name, pl in zip(tensors, names, planes):
+            if not t.is_cuda or t.device.index != int(self.device):
+                raise ValueError("%s is on %s; the detector runs on cuda:%d" % (name, t.device, int(self.device)))
+            if tuple(t.shape) != tuple(tensors[0].shape) or pl[1:] != planes[0][1:]:
+                raise ValueError("%s: every depth tensor must have one size, row pitch and dtype" % name)
+        fmt = planes[0][2]
+        scale = _lib._plane_scale(fmt == _lib.DEPTH_F32, depth_scale, "depth_scale", names[0])
+        st = _lib.device_stream(stream, self.device)
+        return ([pl[0] for pl in planes], planes[0][1], fmt, scale, int(tensors[0].shape[0]), int(tensors[0].shape[1]), st.cuda_stream)
+
+    def _track_pairs(self, starts, got, ver, estimation):
+        # [(Match, poseRefine)] of one frame's track results, one per start
+        from .pose_refine import poseRefine
         status, T, R, t, res, box = got
-        ver = self._verification(nat, [len(starts)])[0]
         pairs = []
         for i, (_, tid, T0, m0, R0, t0) in enumerate(starts):
             p = poseRefine(estimation)

@@ -536,6 +536,43 @@ int lm_track_device(lm_detector* d, const void* depth, int64_t depth_pitch, int 
                     double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box, void* stream);
 int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n);
 
+/* Tracking a batch of depth frames in one call: several cameras, or several independent sequences at one time step (a
+ * sequence's next frame starts from this one's results, so a batch never spans time).  Every frame's objects are slots
+ * of one pose-stage run, so a few objects per frame no longer leave most of the GPU idle.
+ *   Frames     frame f's depth is depth + f * rows * cols (lm_track_batch: host, one size for all frames, copied to the
+ *              device in one copy) or the device plane depth[f] (lm_track_batch_device: a common pitch, format and
+ *              scale, converted and ordered on `stream` as lm_track_device orders its plane); its intrinsics are
+ *              sceneK + 9f.
+ *   Objects    frame f's objects are the next n_objects[f] entries of `objects`, in frame order; n_objects[f] lies in
+ *              [0, 1024], lm_track's bound, and a frame without objects may come anywhere.  The outputs (status, box + 4k,
+ *              T_out + 16k, R_out + 9k, t_out + 3k, residual[k]) take the same entry order.
+ *   Bit for bit  frame f's entries are what lm_track (or lm_track_device) returns for that frame and its objects alone:
+ *              status, box, T, R, t and residual, NaN patterns included; lm_pose_transforms and, with verification on,
+ *              lm_pose_verify then return every entry of the batch in entry order.  This holds because everything a slot
+ *              computes -- its window, both clouds, its voxel sort segment, its ICP job and its verification -- depends
+ *              only on its object and its own frame's depth and K, and the window cap 4 A only on the registered renders.
+ *   Chunks     the run is cut into chunks of 1024 slots; a frame may straddle a chunk boundary.  Launches per chunk are a
+ *              track chunk's (5 point-to-plane or 4, plus 1 when verifying), plus one conversion per frame for
+ *              lm_track_batch_device.  lm_debug_pose_clouds then describes the last chunk (slot i is entry 1024 c + i of
+ *              chunk c).
+ * Refusals, before any device work, are lm_track's with its codes and messages, plus the frame (and the object's index
+ * within its frame) where one applies: LM_E_INVALID for a null argument, n_frames < 1, n_objects[f] outside [0, 1024],
+ * an empty image, max_iterations < 0, margin_px < 0, a bad class, template or non-finite T, and (device) an unknown
+ * depth format, a bad depth_scale, a plane of any frame that fails lm_bind_images_device's checks (named depth[f]) or a
+ * stream of another device; LM_E_STATE for an object without a registered render, LM_POSE_PSO, a connected peer exchange
+ * and a host-only handle.  Like lm_track, a call abandons a frame whose pose stage is pending and returns once the
+ * outputs are on the host.
+ * Device memory kept by the handle: n_frames depth slots of rows * cols * 2 bytes, shared with lm_detect_batch's, and
+ * for each of the batch's objects a pose-stage output slot (ICP output, posed flag, frame index, window record and
+ * object, with pinned host copies of the first two); the cloud buffers stay those of one 1024-object chunk. */
+int lm_track_batch(lm_detector* d, int n_frames, const uint16_t* depth, int rows, int cols, const float* sceneK,
+                   const lm_track_object* objects, const int32_t* n_objects, int max_iterations, int margin_px,
+                   double* T_out, double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box);
+int lm_track_batch_device(lm_detector* d, int n_frames, const void* const* depth, int64_t depth_pitch, int depth_format,
+                          float depth_scale, int rows, int cols, const float* sceneK, const lm_track_object* objects,
+                          const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out,
+                          double* t_out, float* residual, int32_t* status, int32_t* box, void* stream);
+
 /* A batch of RGB-D frames in one call: each frame's match and box NMS, then one pose stage and (pose_nms) one pose NMS
  * for the survivors of every frame.  Frame f is rgb + f * rows * cols * 3 and depth + f * rows * cols (all frames one
  * size), masks[2f] / masks[2f + 1] its colour and depth masks (masks NULL: none), sceneK + 9f its intrinsics.  The other
