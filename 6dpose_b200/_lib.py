@@ -47,6 +47,7 @@ SYMBOLS = [
     "lm_set_pose_verify", "lm_pose_verify", "lm_pose_verify_points", "lm_icp_set_verify", "lm_icp_verify",
     "lm_set_pose_search", "lm_icp_set_pose_search", "lm_pose_search_points",
     "lm_track", "lm_track_device", "lm_track_batch", "lm_track_batch_device", "lm_pose_transforms",
+    "lm_peer_track_batch", "lm_peer_track_batch_device",
 ]
 
 # The pose stage's estimation (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT / LM_POSE_PSO of include/linemod_b200.h) by
@@ -471,6 +472,8 @@ def load():
     batch_out = track_out[:2] + [i32p] + track_out[3:]  # n_objects [n_frames] in place of n
     L.lm_track_batch.argtypes = [vp, c_int, u16p, c_int, c_int] + batch_out
     L.lm_track_batch_device.argtypes = [vp, c_int, ctypes.POINTER(vp), c_i64, c_int, c_f, c_int, c_int] + batch_out + [vp]
+    L.lm_peer_track_batch.argtypes = L.lm_track_batch.argtypes
+    L.lm_peer_track_batch_device.argtypes = L.lm_track_batch_device.argtypes
     L.lm_pose_transforms.argtypes = [vp, f64p, c_i64, ctypes.POINTER(c_i64)]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
@@ -1202,22 +1205,42 @@ class NativeDetector:
     def track_batch(self, depth, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane"):
         """lm_track_batch on u16 [n,H,W] numpy depths (mm), sceneK [n,3,3].  objects: one list of (class_index, template_id,
         T) triples per frame.  Returns one tuple per frame, each what track returns for that frame."""
-        depth = np.ascontiguousarray(depth)
-        if depth.dtype != np.uint16 or depth.ndim != 3:
-            raise TypeError("depth must be uint16 [n,H,W] images (mm)")
-        n, rows, cols = depth.shape
-        return self._track(lambda *a: self._L.lm_track_batch(self._h, n, depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows, cols,
-                                                             *a), sceneK, objects, max_iterations, margin_px, estimation, n)
+        return self._track_host(self._L.lm_track_batch, depth, sceneK, objects, max_iterations, margin_px, estimation)
 
     def track_batch_device(self, planes, pitch, depth_format, depth_scale, rows, cols, stream, sceneK, objects, max_iterations=30,
                            margin_px=4, estimation="point_to_plane"):
         """lm_track_batch_device on device planes (data pointers, one pitch, format and depth_scale) ordered on `stream`.
         Returns what track_batch returns."""
+        return self._track_device(self._L.lm_track_batch_device, planes, pitch, depth_format, depth_scale, rows, cols, stream, sceneK,
+                                  objects, max_iterations, margin_px, estimation)
+
+    def peer_track_batch(self, depth, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane"):
+        """track_batch over the ranks of the connected exchange (lm_peer_track_batch): every rank calls it with the same
+        frames, objects and estimation, and every rank returns what track_batch returns on one unconnected handle."""
+        return self._track_host(self._L.lm_peer_track_batch, depth, sceneK, objects, max_iterations, margin_px, estimation)
+
+    def peer_track_batch_device(self, planes, pitch, depth_format, depth_scale, rows, cols, stream, sceneK, objects, max_iterations=30,
+                                margin_px=4, estimation="point_to_plane"):
+        """track_batch_device over the ranks of the connected exchange (lm_peer_track_batch_device), as peer_track_batch."""
+        return self._track_device(self._L.lm_peer_track_batch_device, planes, pitch, depth_format, depth_scale, rows, cols, stream, sceneK,
+                                  objects, max_iterations, margin_px, estimation)
+
+    def _track_host(self, fn, depth, sceneK, objects, max_iterations, margin_px, estimation):
+        # lm_track_batch or lm_peer_track_batch on host depths
+        depth = np.ascontiguousarray(depth)
+        if depth.dtype != np.uint16 or depth.ndim != 3:
+            raise TypeError("depth must be uint16 [n,H,W] images (mm)")
+        n, rows, cols = depth.shape
+        return self._track(lambda *a: fn(self._h, n, depth.ctypes.data_as(ctypes.POINTER(ctypes.c_uint16)), rows, cols, *a), sceneK, objects,
+                           max_iterations, margin_px, estimation, n)
+
+    def _track_device(self, fn, planes, pitch, depth_format, depth_scale, rows, cols, stream, sceneK, objects, max_iterations, margin_px,
+                      estimation):
+        # lm_track_batch_device or lm_peer_track_batch_device on device planes
         n = len(planes)
         ptrs = (ctypes.c_void_p * max(n, 1))(*planes)
-        return self._track(lambda *a: self._L.lm_track_batch_device(self._h, n, ptrs, int(pitch), int(depth_format), ctypes.c_float(depth_scale),
-                                                                    int(rows), int(cols), *a, stream), sceneK, objects, max_iterations,
-                           margin_px, estimation, n)
+        return self._track(lambda *a: fn(self._h, n, ptrs, int(pitch), int(depth_format), ctypes.c_float(depth_scale), int(rows), int(cols), *a,
+                                         stream), sceneK, objects, max_iterations, margin_px, estimation, n)
 
     def _track(self, fn, sceneK, objects, max_iterations, margin_px, estimation, n_frames=None):
         # n_frames None: one frame's objects (lm_track); else one list of objects per frame, and one result tuple per frame

@@ -262,7 +262,7 @@ struct lm_detector {
   int32_t px_seq = 0;
   unsigned long long px_timeout_ns = 1000000000ull;  // collector gives up on a peer after 1 s (LINEMOD_B200_PEER_TIMEOUT_MS)
   bool px_share_pose = false;           // lm_peer_share_pose: the pose stage is divided over the ranks
-  int32_t px_pose_seq = 0;              // pose exchanges so far: one per shared frame, one per chunk of a shared batch
+  int32_t px_pose_seq = 0;              // pose exchanges so far: one per shared frame, one per chunk of a shared batch or track run
   DeviceArray<PeerExchange> d_px;       // device copy of the descriptor (static after connect)
   PeerExchange h_px;
 
@@ -2475,11 +2475,13 @@ static int track_object(lm_detector* d, const lm_track_object& o, int i, TrackOb
   return LM_OK;
 }
 
-// lm_track, lm_track_device, lm_track_batch and lm_track_batch_device: every refusal before any device work, then the
-// scenes and one track run of the pose stage on the detector's stream.  planes null: n_frames host images contiguous at
-// depth; else frame f's device plane planes[f] (pitch, format, scale), ordered on `caller`.  Frame f has n_objects[f]
-// objects, in frame order; batch false (lm_track, lm_track_device: one frame): the single call's messages.
-static int track(lm_detector* d, bool batch, int n_frames, const void* depth, const void* const* planes, int64_t pitch, int format,
+// lm_track, lm_track_device, lm_track_batch, lm_track_batch_device and (peers true: needs a connected exchange, which
+// the others refuse) lm_peer_track_batch, lm_peer_track_batch_device: every refusal before any device work, then the
+// scenes and one track run of the pose stage on the detector's stream, its chunks shared over the ranks with
+// lm_peer_share_pose.  planes null: n_frames host images contiguous at depth; else frame f's device plane planes[f]
+// (pitch, format, scale), ordered on `caller`.  Frame f has n_objects[f] objects, in frame order; batch false (lm_track,
+// lm_track_device: one frame): the single call's messages.
+static int track(lm_detector* d, bool peers, bool batch, int n_frames, const void* depth, const void* const* planes, int64_t pitch, int format,
                  float scale, cudaStream_t caller, int rows, int cols, const float* sceneK, const lm_track_object* objects,
                  const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out,
                  float* residual, int32_t* status, int32_t* box) {
@@ -2503,7 +2505,8 @@ static int track(lm_detector* d, bool batch, int n_frames, const void* depth, co
   if (rc) return rc;
   if (d->pose_estimation == LM_POSE_PSO)
     return fail(LM_E_STATE, "tracking runs an ICP: LM_POSE_PSO starts from an identity rotation (lm_set_pose_estimation)");
-  if (d->px_rank >= 0) return fail(LM_E_STATE, "tracking does not run with a connected peer exchange");
+  if (!peers && d->px_rank >= 0)
+    return fail(LM_E_STATE, "tracking does not run with a connected peer exchange (every rank calls lm_peer_track_batch)");
   std::vector<TrackObject> obj((size_t)n);
   for (int f = 0; f < n_frames; ++f)
     for (int64_t k = first[(size_t)f]; k < first[(size_t)f + 1]; ++k) {
@@ -2511,6 +2514,7 @@ static int track(lm_detector* d, bool batch, int n_frames, const void* depth, co
       if (rc && batch) return fail(rc, "frame %d: %s", f, std::string(g_err).c_str());
       if (rc) return rc;
     }
+  if (peers && d->px_rank < 0) return fail(LM_E_STATE, "lm_peer_track_batch needs a connected peer exchange");
   if (d->device < 0) return fail(LM_E_STATE, "host-only handle (device -1): GPU stages are unavailable");
   if (planes) {
     rc = check_device_stream(d->device, caller);
@@ -2540,29 +2544,36 @@ static int track(lm_detector* d, bool batch, int n_frames, const void* depth, co
                           rows, cols, &scene, &d->launches);
   }
   if (rc) return rc;
-  PoseOptions o = {rows, cols, 1, max_iterations, d->pose_estimation, st, nullptr, d->pose_verify, d->pose_search};
+  PoseShare sh;
+  const bool share = peers && d->px_share_pose;
+  if (share) {  // one pose exchange per chunk, numbered on from the frames' and batches' ones
+    rc = pose_share_of(d, d->px_pose_seq + 1, &sh);
+    if (rc) return rc;
+    d->px_pose_seq += pose_batch_chunks(first[(size_t)n_frames]);
+  }
+  PoseOptions o = {rows, cols, 1, max_iterations, d->pose_estimation, st, share ? &sh : nullptr, d->pose_verify, d->pose_search};
   return pose_stage_track(d->pose, o, n_frames, scene, sceneK, obj.data(), first.data(), margin_px, &d->launches, T_out, R_out, t_out,
-                          residual, status, box);
+                          residual, status, box, peers ? d->pose_stats : nullptr);
 }
 
 extern "C" int lm_track(lm_detector* d, const uint16_t* depth, int rows, int cols, const float* sceneK, const lm_track_object* objects,
                         int n, int max_iterations, int margin_px, double* T_out, double* R_out, double* t_out, float* residual,
                         int32_t* status, int32_t* box) {
-  return track(d, false, 1, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, &n, max_iterations, margin_px,
+  return track(d, false, false, 1, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, &n, max_iterations, margin_px,
                T_out, R_out, t_out, residual, status, box);
 }
 
 extern "C" int lm_track_device(lm_detector* d, const void* depth, int64_t depth_pitch, int depth_format, float depth_scale, int rows,
                                int cols, const float* sceneK, const lm_track_object* objects, int n, int max_iterations, int margin_px,
                                double* T_out, double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
-  return track(d, false, 1, depth, &depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK, objects, &n,
+  return track(d, false, false, 1, depth, &depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK, objects, &n,
                max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
 }
 
 extern "C" int lm_track_batch(lm_detector* d, int n_frames, const uint16_t* depth, int rows, int cols, const float* sceneK,
                               const lm_track_object* objects, const int32_t* n_objects, int max_iterations, int margin_px, double* T_out,
                               double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box) {
-  return track(d, true, n_frames, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, n_objects, max_iterations,
+  return track(d, false, true, n_frames, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, n_objects, max_iterations,
                margin_px, T_out, R_out, t_out, residual, status, box);
 }
 
@@ -2570,8 +2581,23 @@ extern "C" int lm_track_batch_device(lm_detector* d, int n_frames, const void* c
                                      float depth_scale, int rows, int cols, const float* sceneK, const lm_track_object* objects,
                                      const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out,
                                      double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
-  return track(d, true, n_frames, depth, depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK, objects,
+  return track(d, false, true, n_frames, depth, depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK, objects,
                n_objects, max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
+}
+
+extern "C" int lm_peer_track_batch(lm_detector* d, int n_frames, const uint16_t* depth, int rows, int cols, const float* sceneK,
+                                   const lm_track_object* objects, const int32_t* n_objects, int max_iterations, int margin_px,
+                                   double* T_out, double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box) {
+  return track(d, true, true, n_frames, depth, nullptr, 0, LM_DEPTH_U16_MM, 1.f, nullptr, rows, cols, sceneK, objects, n_objects,
+               max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
+}
+
+extern "C" int lm_peer_track_batch_device(lm_detector* d, int n_frames, const void* const* depth, int64_t depth_pitch, int depth_format,
+                                          float depth_scale, int rows, int cols, const float* sceneK, const lm_track_object* objects,
+                                          const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out,
+                                          double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
+  return track(d, true, true, n_frames, depth, depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK,
+               objects, n_objects, max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
 }
 
 extern "C" int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n) {

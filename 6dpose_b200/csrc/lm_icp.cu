@@ -307,8 +307,9 @@ __device__ void solve6(double A[6][6], double b[6], double x[6]) {
 
 // ---- the pose stage shared over the ranks of the peer exchange (lm_pose.h, PoseShare) ----
 // Pose area of every rank's exchange buffer: [2 slots][POSE_SHARE_SLOTS] entries indexed by survivor, then
-// [2][LM_MAX_PEERS] int32 pose flags (slot, publishing rank) and an int32 ticket.  One pose exchange (a shared frame,
-// or one chunk of a shared batch) uses slot seq & 1, seq the exchange's number on the pose counter, which every rank
+// [2][LM_MAX_PEERS] int32 pose flags (slot, publishing rank) and an int32 ticket, then [2 slots][POSE_SHARE_SLOTS]
+// window records that only track chunks use.  One pose exchange (a shared frame, one chunk of a shared batch or of a
+// shared track run) uses slot seq & 1, seq the exchange's number on the pose counter, which every rank
 // advances once per exchange.  Two slots suffice: a rank stores the entries of exchange e only behind its collector of
 // e - 1, which waited for every peer's flag of e - 1, and each peer raised that flag on its stream behind its own
 // collector of e - 2, the last reader of the slot.
@@ -324,24 +325,34 @@ struct PoseShareEntry {  // one survivor: all that pose_stage_finish and k_pose_
 static_assert(sizeof(PoseShareEntry) == 192 && sizeof(PoseShareEntry) % 16 == 0, "pose area entry layout");
 
 #define POSE_SHARE_FLAGS ((size_t)2 * POSE_SHARE_SLOTS * sizeof(PoseShareEntry))  // byte offset of the flags in the area
+// byte offset of a track chunk's window records, [2 slots][POSE_SHARE_SLOTS] TrackRec indexed by object, behind the ticket
+#define POSE_SHARE_TRACK (POSE_SHARE_FLAGS + sizeof(int32_t) * (2 * LM_MAX_PEERS + 4))
 
-size_t pose_share_area_bytes() { return POSE_SHARE_FLAGS + sizeof(int32_t) * (2 * LM_MAX_PEERS + 4); }
+struct TrackRec {  // one tracked object's window (x, y, w, h: clipped, with the margin), projected box (unclipped) and status
+  int32_t window[4], box[4];
+  int32_t status, pad;
+};
+static_assert(sizeof(TrackRec) % 8 == 0 && POSE_SHARE_TRACK % 8 == 0, "pose area track record layout");
+
+size_t pose_share_area_bytes() { return POSE_SHARE_TRACK + (size_t)2 * POSE_SHARE_SLOTS * sizeof(TrackRec); }
 
 struct PoseShareDev {
   uint8_t* area[LM_MAX_PEERS];  // every rank's pose area
   int32_t world, rank, seq;
-  const int32_t* counts;        // [0] survivors written by k_post_nms (a batch chunk: the chunk's size)
+  const int32_t* counts;        // [0] survivors written by k_post_nms (a batch or track chunk: the chunk's size)
   const uint8_t* posed;         // per slot of this rank (k_pose_cloud_share)
   int32_t* status;              // [0] cloud overflow (the OR over the ranks after k_pose_collect), [1] 1: a peer did not
                                 // publish in time, [2] entries this rank published
   unsigned long long timeout_ns;
   int* abort_flag;
+  TrackRec* rec;                // a track chunk's window records by object (k_track_cloud writes this rank's objects',
+                                // k_pose_collect every object's); null for a survivor chunk
 };
 
 // Thread 0 of the CTA of slot blockIdx.x, after its last pass (the ICP kernel's SHARE instantiation, or k_pose_verify's
-// behind the unshared ICP kernel when the stage verifies): the entry of its survivor into the same place of every rank's
-// pose area, then the ticket; the last CTA raises this rank's pose flag everywhere.  The ticket counts CTAs in its low 16
-// bits and published entries above them.
+// behind the unshared ICP kernel when the stage verifies): the entry of its survivor (and a track chunk's window record)
+// into the same place of every rank's pose area, then the ticket; the last CTA raises this rank's pose flag everywhere.
+// The ticket counts CTAs in its low 16 bits and published entries above them.
 __device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const IcpOut& o, const PoseVerify& v) {
   const int i = sh.rank + (int)blockIdx.x * sh.world;  // survivor of this slot
   const bool mine = i < sh.counts[0];
@@ -354,6 +365,11 @@ __device__ __forceinline__ void pose_share_publish(const PoseShareDev& sh, const
     e.ver = v;
     const size_t at = ((size_t)slot * POSE_SHARE_SLOTS + i) * sizeof(PoseShareEntry);
     for (int q = 0; q < sh.world; ++q) *reinterpret_cast<PoseShareEntry*>(sh.area[q] + at) = e;
+    if (sh.rec) {
+      const TrackRec r = sh.rec[i];
+      const size_t rat = POSE_SHARE_TRACK + ((size_t)slot * POSE_SHARE_SLOTS + i) * sizeof(TrackRec);
+      for (int q = 0; q < sh.world; ++q) *reinterpret_cast<TrackRec*>(sh.area[q] + rat) = r;
+    }
   }
   __threadfence_system();  // release: the entries before the ticket
   unsigned* ticket = reinterpret_cast<unsigned*>(sh.area[sh.rank] + POSE_SHARE_FLAGS) + 2 * LM_MAX_PEERS;
@@ -672,7 +688,8 @@ static void launch_icp(int est, unsigned n, cudaStream_t st, const IcpJob* jobs,
 
 // One CTA behind the ICP kernel's SHARE instantiation on each rank's stream: waits (acquire) until every rank's pose flag of the
 // frame has arrived in this rank's pose area, then copies the entries, in survivor order, into the stage's outs / posed.
-// ver (a verifying stage, else null): the entries' verification, in the same order.
+// ver (a verifying stage, else null): the entries' verification, in the same order; a track chunk's window records go
+// to sh.rec in object order.
 __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShareDev sh, IcpOut* __restrict__ outs,
                                                                        uint8_t* __restrict__ posed, PoseVerify* __restrict__ ver) {
   __shared__ int s_late;
@@ -714,6 +731,16 @@ __global__ void __launch_bounds__(POSE_COLLECT_THREADS) k_pose_collect(PoseShare
     posed[i] = (uint8_t)u.e.posed;
     if (ver) ver[i] = u.e.ver;
     err |= u.e.err;
+    if (sh.rec) {
+      union {
+        int2 v[sizeof(TrackRec) / 8];
+        TrackRec r;
+      } t;
+      const int2* rsrc = reinterpret_cast<const int2*>(mine + POSE_SHARE_TRACK + ((size_t)slot * POSE_SHARE_SLOTS + i) * sizeof(TrackRec));
+#pragma unroll
+      for (int k = 0; k < (int)(sizeof(TrackRec) / 8); ++k) t.v[k] = __ldcv(rsrc + k);
+      sh.rec[i] = t.r;
+    }
   }
   err = __syncthreads_or(err);
   if (tid == 0) {
@@ -1251,13 +1278,10 @@ __global__ void __launch_bounds__(VERIFY_THREADS) k_pose_verify(PoseParams p, co
 // tracking (include/linemod_b200.h, lm_track): a chunk whose clouds come from a given transformation T instead of a
 // match position -- the model cloud of the template, and the scene cloud of the window the model projects to under T
 // --------------------------------------------------------------------------------------------
-struct TrackRec {  // one object's window (x, y, w, h: clipped, with the margin), projected box (unclipped) and status
-  int32_t window[4], box[4];
-  int32_t status, pad;
-};
-
 struct TrackParams {
-  const TrackObject* obj;     // [n] template (bank index) and T
+  const TrackObject* obj;     // [counts[0]] template (bank index) and T
+  const int32_t* counts;      // [0] objects of the chunk
+  int32_t rank, world;        // slot j takes object rank + j * world (lm_pose.h)
   const PoseTpl* tpl;
   const uint16_t* crops;
   // object i's frame frame_of[i] (null: frame 0): its depth scene + frame * srows * scols, its intrinsics sKs + 9 * frame
@@ -1268,15 +1292,15 @@ struct TrackParams {
   int32_t margin;
   int64_t cap;                // most window pixels (LM_TRACK_WINDOW beyond)
   int64_t stride, M;          // points per object: M model points, then cap scene points
-  double* raw;                // object i's model cloud at i * stride, its scene cloud at i * stride + M
+  double* raw;                // slot j's model cloud at j * stride, its scene cloud at j * stride + M
   unsigned long long* keys;
   int32_t* vals;
   int32_t* seg_begin;         // [2n], as PoseParams
   int32_t* seg_end;
   IcpJob* jobs;
   int32_t* err;
-  uint8_t* posed;             // 1: LM_TRACK_TRACKED
-  TrackRec* rec;
+  uint8_t* posed;             // per slot, 1: LM_TRACK_TRACKED
+  TrackRec* rec;              // per object
 };
 
 // Voxel keys of the n points P (PointCloud::VoxelDownSample(0.0025) about the per-axis minima mn, as k_pose_cloud
@@ -1316,7 +1340,8 @@ __device__ __forceinline__ bool track_project(const double* T, double px, double
   return true;
 }
 
-// One CTA per object.  The model cloud is k_pose_cloud's (every crop pixel with render depth > 0, row-major); each of
+// One CTA per slot: slot j takes object rank + j * world, and a slot past the chunk's objects writes an empty job (the
+// window record is the object's, the clouds, job and posed flag the slot's).  The model cloud is k_pose_cloud's (every crop pixel with render depth > 0, row-major); each of
 // its points is projected under T (track_project) and the in-frame pixels' extent is reduced over the CTA.  The
 // window's pixels with scene depth > 0 are back-projected in row-major order as k_pose_cloud back-projects the scene.
 // Both clouds get their voxel keys; the job starts at T.  An object without the status TRACKED writes an empty job.
@@ -1330,10 +1355,23 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
   } tmp;
   __shared__ double s_T[16], s_min[6];
   __shared__ int s_ext[4], s_win[4], s_status;
-  const int i = blockIdx.x, tid = threadIdx.x;
+  const int j = blockIdx.x, tid = threadIdx.x;  // slot j
+  const int i = p.rank + j * p.world;            // its object
+  const size_t sm = (size_t)j * p.stride, ss = sm + p.M;
+  IcpJob* job = p.jobs + j;
+  if (i >= p.counts[0]) {  // block-uniform: a slot past the chunk's objects (shared) writes an empty job
+    if (tid == 0) {
+      p.posed[j] = 0;
+      job->src_first = job->tgt_first = (int32_t)sm;
+      job->src_count = job->tgt_count = 0;
+      for (int k = 0; k < 16; ++k) job->init[k] = (k % 5 == 0) ? 1.0 : 0.0;
+      p.seg_begin[2 * j] = p.seg_end[2 * j] = (int32_t)sm;
+      p.seg_begin[2 * j + 1] = p.seg_end[2 * j + 1] = (int32_t)ss;
+    }
+    return;
+  }
   const PoseTpl T = p.tpl[p.obj[i].g];
   __shared__ VerifyScene sc;  // the object's frame (shared: it stays out of the registers)
-  const size_t sm = (size_t)i * p.stride, ss = sm + p.M;
   double* __restrict__ Mp = p.raw + sm * 3;
   double* __restrict__ Sp = p.raw + ss * 3;
   if (tid < 16) s_T[tid] = p.obj[i].T[tid];
@@ -1424,16 +1462,15 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
     if (ns == 0 && tid == 0) s_status = LM_TRACK_NO_DEPTH;
     __syncthreads();
   }
-  IcpJob* job = p.jobs + i;
   if (s_status != LM_TRACK_TRACKED) {  // block-uniform
     if (tid == 0) {
       p.rec[i].status = s_status;
-      p.posed[i] = 0;
+      p.posed[j] = 0;
       job->src_first = job->tgt_first = (int32_t)sm;
       job->src_count = job->tgt_count = 0;
       for (int k = 0; k < 16; ++k) job->init[k] = s_T[k];
-      p.seg_begin[2 * i] = p.seg_end[2 * i] = (int32_t)sm;
-      p.seg_begin[2 * i + 1] = p.seg_end[2 * i + 1] = (int32_t)ss;
+      p.seg_begin[2 * j] = p.seg_end[2 * j] = (int32_t)sm;
+      p.seg_begin[2 * j + 1] = p.seg_end[2 * j + 1] = (int32_t)ss;
     }
     return;
   }
@@ -1450,12 +1487,12 @@ __global__ void __launch_bounds__(POSE_THREADS) k_track_cloud(TrackParams p) {
   track_voxel_keys(Sp, ns, s_min + 3, ss, p.keys, p.vals, p.err);
   if (tid == 0) {
     p.rec[i].status = LM_TRACK_TRACKED;
-    p.posed[i] = 1;
+    p.posed[j] = 1;
     for (int k = 0; k < 16; ++k) job->init[k] = s_T[k];
     job->src_first = job->tgt_first = (int32_t)sm;
     job->src_count = job->tgt_count = 0;  // k_pose_voxel sets the counts
-    p.seg_begin[2 * i] = (int32_t)sm; p.seg_end[2 * i] = (int32_t)sm + nm;
-    p.seg_begin[2 * i + 1] = (int32_t)ss; p.seg_end[2 * i + 1] = (int32_t)ss + ns;
+    p.seg_begin[2 * j] = (int32_t)sm; p.seg_end[2 * j] = (int32_t)sm + nm;
+    p.seg_begin[2 * j + 1] = (int32_t)ss; p.seg_end[2 * j + 1] = (int32_t)ss + ns;
   }
 }
 
@@ -2178,8 +2215,8 @@ struct PoseChunk {
   long long* record = nullptr;
   int64_t record_words = 0;
   // a track chunk (lm_track; null: survivors): k_track_cloud builds the clouds from these objects instead of
-  // k_pose_cloud; the stage's buffers, seg_begin / seg_end, jobs, err, posed, the scene and the frame tables are filled
-  // in by pose_chunk
+  // k_pose_cloud; the stage's buffers, seg_begin / seg_end, jobs, err, posed, counts, rank, world, the scene and the
+  // frame tables are filled in by pose_chunk.  Shared, its window records travel with the entries.
   const TrackParams* track = nullptr;
 };
 
@@ -2213,6 +2250,7 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
     TrackParams q = *c.track;
     q.raw = p.raw; q.keys = p.keys; q.vals = p.vals; q.seg_begin = p.seg_begin; q.seg_end = p.seg_end;
     q.jobs = p.jobs; q.err = p.err; q.posed = p.posed;
+    q.counts = c.counts; q.rank = p.rank; q.world = p.world;
     q.scene = c.scene; q.srows = o.srows; q.scols = o.scols; q.frame_of = c.frame_of; q.sKs = c.sKs;
     items = n * q.stride; tgt_max = q.cap;
     k_track_cloud<<<n, POSE_THREADS, 0, st>>>(q);
@@ -2235,7 +2273,8 @@ static int pose_chunk(lm_pose_stage* s, const PoseOptions& o, const PoseChunk& c
   }
   if (sh) {
     // the results travel to every rank; the collector gathers the chunk in survivor order
-    const PoseShareDev sd = share_dev(*sh, c.seq, c.counts, s->d_posed.get(), c.status);
+    PoseShareDev sd = share_dev(*sh, c.seq, c.counts, s->d_posed.get(), c.status);
+    sd.rec = c.track ? c.track->rec : nullptr;  // a track chunk's window records travel with its entries
     if (o.verify.on) {  // the owner verifies (it holds the cloud), then publishes the pose and its verification
       launch_icp<false>(o.estimation, n, st, s->d_jobs.get(), s->d_pts.get(), s->d_nrm.get(), s->d_souts.get(), o.max_iterations, nullptr,
                         PoseShareDev());
@@ -2296,7 +2335,7 @@ int pose_stage_clouds(const lm_pose_stage* s, int slot, int what, void* out, int
     CUI(cudaMemcpy(&posed, l.posed + slot, 1, cudaMemcpyDeviceToHost));
     if (what == LM_POSE_CAPTURE_WINDOW) {
       TrackRec rec;
-      CUI(cudaMemcpy(&rec, s->d_trec.get() + l.first + slot, sizeof(rec), cudaMemcpyDeviceToHost));
+      CUI(cudaMemcpy(&rec, s->d_trec.get() + l.first + l.rank + (int64_t)slot * l.world, sizeof(rec), cudaMemcpyDeviceToHost));
       const int32_t w5[5] = {rec.window[0], rec.window[1], rec.window[2], rec.window[3], rec.status};
       if (cap < (int64_t)sizeof(w5))
         return lm_fail(LM_E_CAPACITY, "pose stage capture item %d of slot %d needs %lld bytes, cap is %lld", what, slot, (long long)sizeof(w5),
@@ -3211,23 +3250,30 @@ int pose_track_scene(lm_pose_stage* s, cudaStream_t st, int n_frames, const uint
 
 int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const uint16_t* d_scene, const float* sK, const TrackObject* obj,
                      const int64_t* first, int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual,
-                     int32_t* status, int32_t* box) {
+                     int32_t* status, int32_t* box, int64_t* stats4) {
   cudaStream_t st = o.stream;
+  const PoseShare* sh = o.share;
   const bool verify = o.verify.on != 0;
   const int64_t n = first[n_frames];
   const int nc = pose_batch_chunks(n);
   pose_forget(s);
-  int rc = pose_prepare(s, st, n_frames, n, verify);
+  // Every buffer of the run before its first chunk: once chunks run, no device memory is allocated or freed (a free
+  // waits for the whole device, a spinning peer collector of a shared run included).  The cloud buffers come before
+  // pose_prepare, which sizes the slot outputs a verifying shared chunk publishes from by them.
+  // A chunk's slot: M model points (the largest crop), then a window of up to 4 M scene points.
+  const int64_t M = s->area_max, W = 4 * M, stride = M + W, slots = std::min<int64_t>(n, POSE_CHUNK);
+  int rc = n ? pose_buffers(s, st, (int)((slots * stride + 2 * M - 1) / (2 * M)), M) : LM_OK;
+  if (!rc) rc = pose_prepare(s, st, n_frames, n, verify);
   if (rc) return rc;
   if (n == 0) {
+    if (stats4) {
+      stats4[0] = stats4[1] = stats4[2] = 0;
+      stats4[3] = sh ? 1 : 0;
+    }
     s->verified = verify;
     s->finished_ok = true;
     return LM_OK;
   }
-  // a chunk's object i: M model points (the largest crop), then a window of up to 4 M scene points
-  const int64_t M = s->area_max, W = 4 * M, stride = M + W, slots = std::min<int64_t>(n, POSE_CHUNK);
-  rc = pose_buffers(s, st, (int)((slots * stride + 2 * M - 1) / (2 * M)), M);
-  if (rc) return rc;
   if ((size_t)n > s->h_trec.size()) {
     CUI(cudaStreamSynchronize(st));
     s->d_tobj.reset(); s->d_trec.reset(); s->h_trec.reset();
@@ -3235,14 +3281,18 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
     CUI(s->d_trec.assign(n));
     CUI(s->h_trec.assign(n));
   }
-  // each object's frame and each frame's intrinsics, which k_track_cloud and k_pose_verify read
+  // each object's frame and each frame's intrinsics, which k_track_cloud and k_pose_verify read, and each chunk's
+  // status block with its object count in word 3, which k_track_cloud and a shared chunk's publishers read
   std::vector<int32_t> frame_of((size_t)n);
   for (int f = 0; f < n_frames; ++f)
     for (int64_t k = first[f]; k < first[f + 1]; ++k) frame_of[(size_t)k] = f;
+  std::vector<int32_t> stat((size_t)4 * nc, 0);
+  for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(n - (int64_t)c * POSE_CHUNK, POSE_CHUNK);
   CUI(cudaMemcpyAsync(s->d_tobj.get(), obj, sizeof(TrackObject) * n, cudaMemcpyHostToDevice, st));
   CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
   CUI(cudaMemcpyAsync(s->d_bsK.get(), sK, sizeof(float) * 9 * n_frames, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4 * nc, st));
+  CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  int64_t stage_launches = 0;
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_CHUNK;
     TrackParams q;
@@ -3250,11 +3300,12 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
     q.obj = s->d_tobj.get() + c0; q.tpl = s->d_tpl.get(); q.crops = s->d_crops.get();
     q.margin = margin; q.cap = W; q.stride = stride; q.M = M;
     q.rec = s->d_trec.get() + c0;
-    PoseChunk k = run_chunk(s, o, c, nullptr, nullptr, (int)std::min<int64_t>(n - c0, POSE_CHUNK), d_scene, nullptr);
+    PoseChunk k = run_chunk(s, o, c, nullptr, s->d_bstat.get() + 4 * c + 3, stat[(size_t)4 * c + 3], d_scene, nullptr);
     k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get();
     k.track = &q;
     const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
+    stage_launches += l;
     *launches += l;
   }
   CUI(cudaMemcpyAsync(s->h_bouts.get(), s->d_bouts.get(), sizeof(IcpOut) * n, cudaMemcpyDeviceToHost, st));
@@ -3264,8 +3315,14 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
   int64_t published = 0;
-  rc = pose_status(s->h_bstat.get(), nc, false, 0, 0, nc > 1, &published);
+  rc = pose_status(s->h_bstat.get(), nc, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0, nc > 1, &published);
   if (rc) return rc;
+  if (stats4) {
+    stats4[0] = n;
+    stats4[1] = sh ? published : n;
+    stats4[2] = stage_launches;
+    stats4[3] = sh ? 1 : 0;
+  }
   s->xf.assign(16 * (size_t)n, std::numeric_limits<double>::quiet_NaN());
   for (int64_t i = 0; i < n; ++i) {
     const TrackRec& e = s->h_trec[(size_t)i];

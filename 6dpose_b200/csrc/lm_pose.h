@@ -37,8 +37,9 @@ bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel
 // verifies each survivor on the rank that holds its cloud and stores result and verification); k_pose_collect waits for the
 // world flags in this rank's buffer and gathers the results in survivor order into the chunk's outputs, so the host and
 // the pose NMS read what the unshared stage leaves.  The pose area: [2 slots][1024 survivors] entries of 192 bytes,
-// then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket (pose_share_area_bytes in all).  Each pose exchange -- a
-// shared frame, or one chunk of a shared batch -- has its own number on the detector's pose counter.
+// then [2][LM_MAX_PEERS] int32 pose flags and an int32 ticket, then [2][1024] window records of 40 bytes that only track
+// chunks use (pose_share_area_bytes in all).  Each pose exchange -- a shared frame, or one chunk of a shared batch or
+// track run -- has its own number on the detector's pose counter.
 struct PoseShare {
   uint8_t* base[LM_MAX_PEERS];      // every rank's exchange buffer (peer mappings; this rank's own at [rank])
   uint64_t area_offset;             // byte offset of the pose area in every buffer
@@ -137,10 +138,13 @@ int pose_track_scene(lm_pose_stage* s, cudaStream_t st, int n_frames, const uint
 // first[f + 1]) (at most 1024 per frame), its intrinsics sK + 9f; one chunk per 1024 objects, frames straddling chunk
 // boundaries.  Then the outputs of lm_track in object order (an entry without the status TRACKED leaves its T, R, t
 // untouched and gets residual -1).  Returns once they are on the host; the run is then the stage's last finished run
-// (pose_stage_verify, pose_stage_transforms).  lm_track is the one-frame run.
+// (pose_stage_verify, pose_stage_transforms).  lm_track is the one-frame run.  With o.share (lm_peer_track_batch),
+// chunk c is pose exchange o.share->seq + c: object i of a chunk is tracked by rank i % world, and its entry and window
+// record travel to every rank as a shared batch chunk's entries do.  Allocates nothing once its first chunk is enqueued.
+// stats4 (may be null): what lm_pose_stats returns, written once the run succeeded.
 int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const uint16_t* d_scene, const float* sK, const TrackObject* obj,
                      const int64_t* first, int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual,
-                     int32_t* status, int32_t* box);
+                     int32_t* status, int32_t* box, int64_t* stats4);
 // The transformation of every entry of the run last finished (lm_pose_transforms), in entry order, T_out + 16k; NaN for an
 // entry without a pose.  LM_E_STATE once another run has been enqueued or the last one failed; LM_E_CAPACITY (with *n)
 // beyond cap.  The pose NMS's kept entries are matched to their survivors on the host, from one copy of the run's ICP

@@ -533,33 +533,39 @@ class Detector:
         them, with depth_scale and stream); sceneK: one 3x3 matrix or one per frame; objects: one list per frame, each entry
         any kind track takes, at most 1024 per frame.  Returns one [(Match, poseRefine)] list per frame, each equal to track
         on that frame alone.  TypeError / ValueError before any device work."""
+        return self._track_batch(depths, sceneK, objects, max_iterations, margin_px, estimation, depth_scale, stream, False, "track_batch")
+
+    def _track_batch(self, depths, sceneK, objects, max_iterations, margin_px, estimation, depth_scale, stream, peers, what):
+        # track_batch, and (peers) dist.track_batch_sharded on a connected detector; messages name `what`
         _lib.estimation_code(estimation)
         depths, objects = list(depths), [list(o) for o in objects]
         n = len(depths)
         if not n:
-            raise ValueError("track_batch: no frames")
+            raise ValueError("%s: no frames" % what)
         if len(objects) != n:
-            raise ValueError("track_batch: %d object lists for %d frames" % (len(objects), n))
-        starts = [self._track_starts(o, "track_batch: frame %d" % f) for f, o in enumerate(objects)]
-        K = self._frame_ks(sceneK, n, "track_batch()")
+            raise ValueError("%s: %d object lists for %d frames" % (what, len(objects), n))
+        starts = [self._track_starts(o, "%s: frame %d" % (what, f)) for f, o in enumerate(objects)]
+        K = self._frame_ks(sceneK, n, what + "()")
         triples = [[(c, t, T) for c, t, T, _, _, _ in s] for s in starts]
         on_device = [_lib.is_tensor(d) for d in depths]
         if any(on_device) and not all(on_device):
-            raise TypeError("track_batch: depths mix numpy arrays and torch tensors")
+            raise TypeError("%s: depths mix numpy arrays and torch tensors" % what)
         if on_device[0]:
             planes = self._depth_planes(depths, ["depths[%d]" % f for f in range(n)], depth_scale, stream)
             nat = self._pose_native(())
-            got = nat.track_batch_device(*planes, K, triples, max_iterations, margin_px, estimation)
+            run = nat.peer_track_batch_device if peers else nat.track_batch_device
+            got = run(*planes, K, triples, max_iterations, margin_px, estimation)
         else:
             _lib.host_frame_options(depth_scale, stream)
             depths = [np.asarray(d) for d in depths]
             for f, d in enumerate(depths):
                 if d.dtype != np.uint16 or d.ndim != 2:
-                    raise TypeError("track_batch: depths[%d] must be a uint16 HxW depth image (mm)" % f)
+                    raise TypeError("%s: depths[%d] must be a uint16 HxW depth image (mm)" % (what, f))
                 if d.shape != depths[0].shape:
-                    raise ValueError("track_batch: depths[%d] is %s, depths[0] %s" % (f, d.shape, depths[0].shape))
+                    raise ValueError("%s: depths[%d] is %s, depths[0] %s" % (what, f, d.shape, depths[0].shape))
             nat = self._pose_native(())
-            got = nat.track_batch(np.stack(depths), K, triples, max_iterations, margin_px, estimation)
+            run = nat.peer_track_batch if peers else nat.track_batch
+            got = run(np.stack(depths), K, triples, max_iterations, margin_px, estimation)
         ver = self._verification(nat, [len(s) for s in starts])
         return [self._track_pairs(s, g, v, estimation) for s, g, v in zip(starts, got, ver)]
 

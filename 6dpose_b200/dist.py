@@ -50,8 +50,8 @@ def connect_peers(detector, group=None, capacity_records=8192, class_ids=(), sha
     handles travel through the process group (any backend), every rank maps the others' buffers.
 
     share_pose: divide the pose stage of Detector.detect / match_refine and of detect_batch_sharded /
-    match_refine_batch_sharded over the ranks (lm_peer_share_pose).  Only for callers whose every rank runs the pose
-    stage of every frame."""
+    match_refine_batch_sharded / track_batch_sharded over the ranks (lm_peer_share_pose).  Only for callers whose every
+    rank runs the pose stage of every frame."""
     import torch.distributed as dist
     if not isinstance(share_pose, (bool, int, np.bool_, np.integer)):
         raise TypeError("connect_peers(share_pose=...): a bool, got %s" % type(share_pose).__name__)
@@ -79,12 +79,17 @@ def disconnect_peers(detector, group=None):
     dist.barrier(group=group)
 
 
-def _connected_batch(detector, frames, class_ids, sceneK, masks, group, what):
-    # the native handle and its arguments for lm_peer_detect_batch; nothing touches a device before the checks
+def _check_connected(detector, group, what):
+    # RuntimeError unless the detector is connected to the peer exchange of this rank and world
     import torch.distributed as dist
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     if getattr(detector, "_peers", None) != (rank, world):
         raise RuntimeError("%s needs a detector connected to the peer exchange of rank %d of %d (dist.connect_peers)" % (what, rank, world))
+
+
+def _connected_batch(detector, frames, class_ids, sceneK, masks, group, what):
+    # the native handle and its arguments for lm_peer_detect_batch; nothing touches a device before the checks
+    _check_connected(detector, group, what)
     return detector._batch_args(frames, class_ids, sceneK, masks, what)
 
 
@@ -112,6 +117,19 @@ def detect_batch_sharded(detector, frames, threshold, class_ids, sceneK, iou_thr
                                 bool(use_scene_cloud), pose_nms=True, translation_threshold=float(translation_threshold),
                                 estimation=estimation)
     return detector._batch_pairs(nat, got)
+
+
+def track_batch_sharded(detector, depths, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane", depth_scale=1.0,
+                        stream=None, group=None):
+    """Detector.track_batch over the connected peer exchange (lm_peer_track_batch); with connect_peers(share_pose=True)
+    each rank tracks its share of every chunk's objects and the results travel to every rank.  Every rank calls it with
+    the same depths, objects and arguments (estimation included), in the same order as its other pose exchanges, and
+    returns the whole result, equal to track_batch on one unconnected detector.  A single frame is a one-frame batch.
+    RuntimeError when the detector is not connected for this rank and world, and track_batch's TypeError / ValueError,
+    all before any device work."""
+    _check_connected(detector, group, "track_batch_sharded()")
+    return detector._track_batch(depths, sceneK, objects, max_iterations, margin_px, estimation, depth_scale, stream, True,
+                                 "track_batch_sharded")
 
 
 def match_quantized_sharded(detector, quantized, threshold, class_ids=(), group=None):

@@ -234,9 +234,10 @@ int lm_peer_disconnect(lm_detector* d);
  *                       peer's pose collector included -- so run such a frame unshared first.
  * A peer whose poses do not arrive within LINEMOD_B200_PEER_TIMEOUT_MS fails the frame with LM_E_STATE (the message names
  * the pose exchange) and raises the device's abort flag of the exchange, as the record collector does.
- * Each pose exchange -- a shared frame, or one chunk of a shared lm_peer_detect_batch -- takes the next number of the
- * handle's pose counter (reset by lm_peer_export), and consecutive exchanges alternate between the two slots of the pose
- * area.  lm_detect_batch still refuses a connected exchange; lm_peer_detect_batch is its connected form. */
+ * Each pose exchange -- a shared frame, or one chunk of a shared lm_peer_detect_batch or lm_peer_track_batch -- takes
+ * the next number of the handle's pose counter (reset by lm_peer_export), and consecutive exchanges alternate between
+ * the two slots of the pose area.  lm_detect_batch and the track calls still refuse a connected exchange;
+ * lm_peer_detect_batch and lm_peer_track_batch are their connected forms. */
 int lm_peer_share_pose(lm_detector* d, int on);
 
 /* Copy the kept records of the last completed run to the host, sorted by (work, seq). */
@@ -505,7 +506,8 @@ int lm_pose_verify_points(int device, const double* pts, int64_t n, const double
  *      scores in entry order (-1 for an entry not tracked).  Nothing is dropped; lm_nms_translations is the caller's.
  * Refusals, before any device work: LM_E_INVALID for a null argument, n < 0 or n > 1024, an empty image, max_iterations
  * < 0, margin_px < 0, an unknown depth format or a bad depth_scale, a class or template out of range, a non-finite entry
- * of T; LM_E_STATE for LM_POSE_PSO (its kernel starts from an identity rotation), a connected peer exchange, or an object
+ * of T; LM_E_STATE for LM_POSE_PSO (its kernel starts from an identity rotation), a connected peer exchange (use
+ * lm_peer_track_batch there), or an object
  * whose template has no registered render (and on a host-only handle); LM_E_CAPACITY as the pose stage's buffers.
  * A call runs on the detector's stream and returns once the outputs are on the host; it abandons a frame whose pose stage
  * is pending.  lm_debug_pose_clouds then describes its chunk: slot i is object i, POSED is 1 for TRACKED, INIT is T,
@@ -572,6 +574,41 @@ int lm_track_batch_device(lm_detector* d, int n_frames, const void* const* depth
                           float depth_scale, int rows, int cols, const float* sceneK, const lm_track_object* objects,
                           const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out,
                           double* t_out, float* residual, int32_t* status, int32_t* box, void* stream);
+
+/* lm_track_batch and lm_track_batch_device over the ranks of a connected peer exchange, with the same arguments and
+ * outputs.  Every rank returns what one unconnected handle holding the same renders returns from lm_track_batch on the
+ * same frames and objects, bit for bit: status, box, T, R, t and residual, NaN patterns included; lm_pose_transforms and,
+ * with verification on, lm_pose_verify then return the same entries.  Calling it is the caller's promise that every rank
+ * calls it with the same frames, objects, estimation and verification settings, in the same order as its other pose
+ * exchanges (shared frames, lm_peer_detect_batch).
+ *   Pose       sharing off: every rank tracks every object itself, and the exchange is not touched (5 launches per chunk
+ *              point-to-plane, 4 point-to-point).  Sharing on (lm_peer_share_pose): the run is cut into chunks of 1024
+ *              objects as lm_track_batch cuts it; within a chunk of C objects, object i is tracked by rank i % world in
+ *              ceil(C / world) slots.  The owner builds its window and clouds, refines it and (verification on) verifies
+ *              it, then stores its ICP output, posed flag, overflow flag, verification and window record (window,
+ *              projected box, status) into the pose area of every rank; a collector gathers them in object order, as for
+ *              a shared batch chunk (6 launches per chunk point-to-plane, 5 point-to-point; a rank without an object in
+ *              the chunk still publishes).  Each chunk is one pose exchange and takes the next number of the pose
+ *              counter, so shared frames, lm_peer_detect_batch and lm_peer_track_batch interleave in any order.  Add 1
+ *              launch per chunk when verifying, and one conversion per frame for lm_peer_track_batch_device.  A run
+ *              without objects launches nothing and exchanges nothing.
+ * Refusals, before any device work: LM_E_STATE without a connected exchange, for LM_POSE_PSO and on a host-only handle;
+ * otherwise every refusal of lm_track_batch / lm_track_batch_device with its code and "frame f: object k" message.
+ * lm_track, lm_track_device, lm_track_batch and lm_track_batch_device still refuse a connected exchange.  A peer whose
+ * poses do not arrive in time fails the call with LM_E_STATE (the message names the pose exchange).
+ * No device memory is allocated or freed once the run's first chunk is enqueued: the scenes, the pose stage's outputs and
+ * cloud buffers and the per-object records are grown before it.  Ranks that are handles of ONE process on ONE device call
+ * from their own host threads, and each first runs the largest shape (frames, frame size, objects) it will run shared
+ * with sharing off: that call grows the buffers while no collector spins, since a free waits for the whole device -- a
+ * peer's collector included.  lm_pose_stats afterwards: the objects, the objects this rank tracked over all chunks, the
+ * pose stage's launches (the conversions not counted) and 1 if shared. */
+int lm_peer_track_batch(lm_detector* d, int n_frames, const uint16_t* depth, int rows, int cols, const float* sceneK,
+                        const lm_track_object* objects, const int32_t* n_objects, int max_iterations, int margin_px,
+                        double* T_out, double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box);
+int lm_peer_track_batch_device(lm_detector* d, int n_frames, const void* const* depth, int64_t depth_pitch, int depth_format,
+                               float depth_scale, int rows, int cols, const float* sceneK, const lm_track_object* objects,
+                               const int32_t* n_objects, int max_iterations, int margin_px, double* T_out, double* R_out,
+                               double* t_out, float* residual, int32_t* status, int32_t* box, void* stream);
 
 /* A batch of RGB-D frames in one call: each frame's match and box NMS, then one pose stage and (pose_nms) one pose NMS
  * for the survivors of every frame.  Frame f is rgb + f * rows * cols * 3 and depth + f * rows * cols (all frames one
@@ -751,7 +788,7 @@ int lm_debug_coarse(lm_detector* d, uint32_t* mask, int64_t mask_cap, uint16_t* 
  *   LM_POSE_CAPTURE_RAW_MODEL  the model cloud before down-sampling (what k_pose_verify reads), row-major pixel order
  *   LM_POSE_CAPTURE_RAW_SCENE  the scene cloud before down-sampling (empty without use_scene_cloud)
  *   LM_POSE_CAPTURE_WINDOW     5 int32, a track chunk only (lm_track; LM_E_STATE otherwise): the window x, y, w, h and
- *                              the status, for every slot
+ *                              the status of the slot's object, for every slot
  * LM_E_STATE before any pose stage has run (and after a later one failed before it enqueued a chunk), and for every
  * item but POSED of a slot without a pose; LM_E_CAPACITY when cap is too small; LM_E_INVALID for a slot outside the chunk or an
  * item not listed.  Describes the last chunk only, until the next pose stage is enqueued. */
@@ -783,8 +820,8 @@ void* lm_stream(lm_detector* d);
  * a frame's pose stage is 5, whatever its survivor count; 6 when shared over the exchange; one fewer each with
  * LM_ICP_POINT_TO_POINT). */
 int64_t lm_launch_count(lm_detector* d);
-/* About the last pose stage this handle completed (lm_complete_pose / lm_complete_detect; lm_peer_detect_batch: see there,
- * lm_detect_batch leaves it as it was): [0] box-NMS survivors,
+/* About the last pose stage this handle completed (lm_complete_pose / lm_complete_detect; lm_peer_detect_batch and
+ * lm_peer_track_batch: see there; lm_detect_batch and lm_track_batch leave it as it was): [0] box-NMS survivors,
  * [1] hypotheses this rank refined (all survivors unshared; its share with lm_peer_share_pose, as counted by the ICP
  * kernel), [2] launches of the stage, [3] 1 if it was shared.  Zeros before the first.  `out4` has 4 entries. */
 int lm_pose_stats(lm_detector* d, int64_t* out4);
