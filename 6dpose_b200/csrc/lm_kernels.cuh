@@ -1248,16 +1248,19 @@ __global__ void __launch_bounds__(256) k_refine_prep(PrepParams p) {
 // refinement (k_refine_bits, or k_refine), which computes them exactly -- the filter never changes a result, it only
 // removes work.
 //
-// One warp owns one candidate.  Lane k of each half-warp owns patch column k: the 16 columns of one row block are 16
-// consecutive words of the column-major H-plane (k_refine_prep), so every load of a half-warp reads ONE 64-byte window
-// and a warp-wide load touches two windows (one per half-warp).  Of every 32 consecutive features half-warp h adds
-// features 16h .. 16h+15, two per register: the 16 rows of the first feature of a pair in the low half-word, of the
-// second in the high half-word (one PRMT), so the 9-bit vertical counters (carry-save adders, 8 features per step) count
-// the same 16 cells twice, in two halves.  A candidate is a chain of nf / 32 steps.  Lane L decodes descriptor L of the
-// step once (byte offset and shift packed in one register) and stores it to shared memory; every lane picks up four
-// descriptors of its half-warp with one 128-bit broadcast load.  Control flow is warp-uniform.  Every LM_FILTER_CHECK
-// features, once `need` exceeds the features still to come, the partial counters meet (vc_fold) and a candidate none of
-// whose cells can still reach `need` is found with a bit-sliced compare and dropped; the last check is at the end.
+// One warp counts two candidates at a time.  Lane k of each half-warp owns patch column k: the 16 columns of one row
+// block are 16 consecutive words of the column-major H-plane (k_refine_prep), so every load of a half-warp reads ONE
+// 64-byte window and a warp-wide load touches two windows (one per half-warp).  Of every 32 consecutive features
+// half-warp h adds features 16h .. 16h+15, two per register: the 16 rows of the first feature of a pair in the low
+// half-word, of the second in the high half-word (one PRMT), so the 9-bit vertical counters (carry-save adders, 8
+// features per step) count the same 16 cells twice, in two halves.  A candidate is a chain of nf / 32 steps; the two
+// chains of a warp run side by side, so a step has 32 independent loads per lane instead of 16.  Lane L decodes
+// descriptor L of the step once per candidate (byte offset and shift packed in one register) and stores it to shared
+// memory; every lane picks up four descriptors of its half-warp with one 128-bit broadcast load.  Control flow is
+// warp-uniform.  Every LM_FILTER_CHECK features, once `need` exceeds the features still to come, the partial counters
+// meet (vc_fold) and a candidate none of whose cells can still reach `need` is found with a bit-sliced compare and
+// dropped; the last check is at the end.  Each candidate is checked against its own `need` and dies on its own; the
+// other one then goes on alone.
 // --------------------------------------------------------------------------------------------
 struct FilterParams {
   const uint32_t* rp;      // H-planes of the filtered level
@@ -1348,128 +1351,201 @@ __device__ __forceinline__ uint32_t lm_plane_rows(const char* col, uint32_t v) {
 }
 
 #ifndef LM_FILTER_MIN_CTAS
-#define LM_FILTER_MIN_CTAS 4  // 64 registers: more of a step's 16 loads in flight per warp (5 CTAs at 48: slower, DESIGN.md §9)
-#endif
-#ifndef LM_FILTER_CHUNK
-#define LM_FILTER_CHUNK 1  // consecutive candidates a warp takes from the queue at a time (2..16 measured: tail imbalance costs more than the L1 reuse buys)
+// 64 registers, no spill.  Two candidates per warp: 4 CTAs per SM measured 11 800-11 920 frames/s and a 57-58 us filter
+// stage, 3 CTAs at 80 registers 11 100 and 62 us (H100 80GB HBM3, 700 W; DESIGN.md §9).  One candidate per warp: 5 CTAs
+// at 48 registers was slower than 4.
+#define LM_FILTER_MIN_CTAS 4
 #endif
 #ifndef LM_FILTER_CHECK
 #define LM_FILTER_CHECK 64  // features between two bound checks, a multiple of 32 (32 measured: the extra merges cost more than the words they save, DESIGN.md §9)
 #endif
+
+// One candidate's place in the filter's step loop: its column, row block and descriptors, the lane's descriptor of the
+// next step, and the partial counters.
+struct FilterCand {
+  const char* col;     // this lane's column of the H-plane
+  const uint32_t* fd;  // the template's descriptors of the filtered level
+  int cy, nf, nfp, need;
+  uint32_t d_next;
+  uint32_t ch[LM_FILTER_BITS];
+  bool lane_alive;
+};
+
+// what the filter does with a candidate before counting: 0 = pass it on uncounted (a template the filter does not take,
+// or need <= 0), 1 = drop it (need > nf: LL.cpp:1935-1937 would drop whatever the patch holds), 2 = count it
+__device__ __forceinline__ int filter_triage(int4 fi) {
+  if (!(fi.w & 2)) return 0;
+  const int need = (int)((unsigned)fi.w >> 8);
+  if (need > fi.y) return 1;
+  return need > 0 ? 2 : 0;
+}
+
+__device__ __forceinline__ void filter_setup(FilterCand& k, const FilterParams& p, uint2 e, int4 fi, int lane) {
+  const int T = p.ref.T, border = 8 * T, j = (int)e.y;
+  // patch origin of the candidate at the filtered level (LL.cpp:1871-1880, 1380-1381)
+  int x = (j % p.low.Wd) * p.low.T + p.low.off;
+  int y = (j / p.low.Wd) * p.low.T + p.low.off;
+  x = x * 2 + 1;
+  y = y * 2 + 1;
+  x = max(x, border); y = max(y, border);
+  x = min(x, p.ref.cols - (fi.z & 0xFFFF) - border);
+  y = min(y, p.ref.rows - (int)((unsigned)fi.z >> 16) - border);
+  k.col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + (lane & 15)));
+  k.cy = y / T - 8;
+  k.fd = p.rdesc + fi.x;
+  k.nf = fi.y;
+  k.nfp = (fi.y + 31) & ~31;  // descriptors are padded with zero-plane entries
+  k.need = (int)((unsigned)fi.w >> 8);
+  k.d_next = __ldg(k.fd + lane);
+#pragma unroll
+  for (int b = 0; b < LM_FILTER_BITS; ++b) k.ch[b] = 0u;
+  k.lane_alive = true;
+}
+
+// lane L's descriptor of step i (feature i + L) in shared-memory form: plane BYTE offset (incl. the candidate's row
+// block) : 27 | shift : 5; the next step's descriptor is loaded one step ahead
+__device__ __forceinline__ uint32_t filter_step_desc(FilterCand& k, int i, int lane, int Wd) {
+  const uint32_t d = k.d_next;
+  if (i + 32 < k.nfp) k.d_next = __ldg(k.fd + i + 32 + lane);
+  const int py0 = k.cy + (int)(d >> 23);
+  return (((d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd)) << 7) | ((uint32_t)py0 & 15u);
+}
+
+// the 16 plane words of a lane's half of a step, two features per register (features 16 hw + 4m .. + 3 in sd[m])
+__device__ __forceinline__ void filter_rows(const uint4* sd, const char* col, uint32_t (&xh)[8]) {
+#pragma unroll
+  for (int m = 0; m < 4; ++m) {
+    const uint4 v = sd[m];
+    xh[2 * m] = __byte_perm(lm_plane_rows(col, v.x), lm_plane_rows(col, v.y), 0x5410);
+    xh[2 * m + 1] = __byte_perm(lm_plane_rows(col, v.z), lm_plane_rows(col, v.w), 0x5410);
+  }
+}
+
+// after `done` features: cells that can still reach `need` have CH >= need - (features not yet added); true when no cell
+// of the candidate can (warp-uniform)
+__device__ __forceinline__ bool filter_dead(FilterCand& k, int done, int hw) {
+  const int thr = k.need - max(k.nf - done, 0);
+  if (thr > 0 && (done >= k.nf || done % LM_FILTER_CHECK == 0)) {
+    vc_fold(k.ch);
+    k.lane_alive = (vc_ge(k.ch, thr) & 0xFFFFu) != 0u;
+    if (!__any_sync(0xffffffffu, k.lane_alive)) return true;
+    // the totals live on in the low half-words of half-warp 0; the rest starts its partial counts again
+    const uint32_t keep = hw ? 0u : 0xFFFFu;
+#pragma unroll
+    for (int b = 0; b < LM_FILTER_BITS; ++b) k.ch[b] &= keep;
+  }
+  return false;
+}
+
 // Layout contract with the host (prepare_bank / prepare_work): every template's descriptors are padded to a multiple of
 // 32 with descriptors that point into an all-zero tail of the plane buffer (so the loop needs no bounds predicate), and
 // finfo[w] = {first descriptor, features of the level, width | height << 16, flags | need << 8} with `need` computed on
 // the host for the call's threshold with the same two IEEE float operations (lm_min_kept_raw).
 __global__ void __launch_bounds__(256, LM_FILTER_MIN_CTAS) k_refine_filter_w(FilterParams p) {
   lm_pdl_wait();
-  // per warp: the 32 decoded descriptors of a step, two buffers (consecutive steps alternate, so one __syncwarp per step
-  // orders a buffer's reads before its next write)
-  __shared__ uint4 s_desc[8][2][8];
-  const int lane = threadIdx.x & 31, hw = lane >> 4, ck = lane & 15;
-  uint4 (*const sd)[8] = s_desc[threadIdx.x >> 5];
+  // per warp: the decoded descriptors of a step for each of the two candidates, two buffers (consecutive steps
+  // alternate, so one __syncwarp per step orders a buffer's reads before its next write)
+  __shared__ uint4 s_desc[8][2][2][8];
+  const int lane = threadIdx.x & 31, hw = lane >> 4;
+  uint4 (*const sd)[2][8] = s_desc[threadIdx.x >> 5];
   int sb = 0;
   const int total = min(p.off[p.n_work], p.cand_cap);
-  const int T = p.ref.T, border = 8 * T;
   const int Wd = p.Wd;
   unsigned words_read = 0, dropped_feats = 0;
-  // A warp takes LM_FILTER_CHUNK consecutive candidates at a time: the list is ordered by template, then cell, so they
-  // mostly share the template (descriptors) and their patches overlap (neighbouring cells) -- what the first one pulled
-  // into L1 serves the others.  The NEXT candidate's cell and per-template record are fetched while the current one is
+  // A warp takes two consecutive candidates A, B at a time: the list is ordered by template, then cell, so they mostly
+  // share the template (descriptors).  The NEXT pair's cells and per-template records are fetched while this pair is
   // being counted.
-  int c_base = 0, k_in = 0;
-  if (lane == 0) c_base = atomicAdd(p.queue, LM_FILTER_CHUNK);
-  c_base = __shfl_sync(0xffffffffu, c_base, 0);
-  int c_next = c_base;
-  uint2 e_next = make_uint2(0u, 0u);
-  int4 fi_next = make_int4(0, 0, 0, 0);
+  int c_next = 0;
+  if (lane == 0) c_next = atomicAdd(p.queue, 2);
+  c_next = __shfl_sync(0xffffffffu, c_next, 0);
+  uint2 ea_next = make_uint2(0u, 0u), eb_next = ea_next;
+  int4 fa_next = make_int4(0, 0, 0, 0), fb_next = fa_next;
   if (c_next < total) {
-    e_next = __ldcg(p.cand + c_next);
-    fi_next = __ldg(p.finfo + e_next.x);
+    ea_next = __ldcg(p.cand + c_next);
+    fa_next = __ldg(p.finfo + ea_next.x);
+    if (c_next + 1 < total) {
+      eb_next = __ldcg(p.cand + c_next + 1);
+      fb_next = __ldg(p.finfo + eb_next.x);
+    }
   }
   for (;;) {
     const int c = c_next;
     if (c >= total) break;
-    const uint2 e = e_next;
-    const int4 fi = fi_next;
-    if (++k_in == LM_FILTER_CHUNK) {
-      k_in = 0;
-      if (lane == 0) c_base = atomicAdd(p.queue, LM_FILTER_CHUNK);
-      c_base = __shfl_sync(0xffffffffu, c_base, 0);
-    }
-    c_next = c_base + k_in;
+    const bool has_b = c + 1 < total;
+    const uint2 ea = ea_next, eb = eb_next;
+    const int4 fa = fa_next, fb = fb_next;
+    if (lane == 0) c_next = atomicAdd(p.queue, 2);
+    c_next = __shfl_sync(0xffffffffu, c_next, 0);
     if (c_next < total) {
-      e_next = __ldcg(p.cand + c_next);
-      fi_next = __ldg(p.finfo + e_next.x);
-    }
-    const int j = (int)e.y;
-    bool pass = true;
-    if (fi.w & 2) {
-      const int nf = fi.y;
-      const int need = (int)((unsigned)fi.w >> 8);
-      if (need > nf) {  // nothing can be kept (LL.cpp:1935-1937 would drop whatever the patch holds)
-        if (lane == 0) dropped_feats += (unsigned)nf;
-        pass = false;
-      } else if (need > 0) {
-        // patch origin of the candidate at the filtered level (LL.cpp:1871-1880, 1380-1381)
-        int x = (j % p.low.Wd) * p.low.T + p.low.off;
-        int y = (j / p.low.Wd) * p.low.T + p.low.off;
-        x = x * 2 + 1;
-        y = y * 2 + 1;
-        x = max(x, border); y = max(y, border);
-        x = min(x, p.ref.cols - (fi.z & 0xFFFF) - border);
-        y = min(y, p.ref.rows - (int)((unsigned)fi.z >> 16) - border);
-        const char* __restrict__ col = reinterpret_cast<const char*>(p.rp + (x / T - 8 + ck));  // this lane's column
-        const int cy = y / T - 8;
-        const uint32_t* __restrict__ fd = p.rdesc + fi.x;
-        const int nfp = (nf + 31) & ~31;  // descriptors are padded with zero-plane entries
-        uint32_t ch[LM_FILTER_BITS];
-#pragma unroll
-        for (int b = 0; b < LM_FILTER_BITS; ++b) ch[b] = 0u;
-        bool lane_alive = true, dead = false;
-        uint32_t d_next = __ldg(fd + lane);
-        for (int i = 0; i < nfp; i += 32) {
-          // lane L decodes feature i + L: plane BYTE offset (incl. the row block of this candidate) : 27 | shift : 5
-          const uint32_t d = d_next;
-          if (i + 32 < nfp) d_next = __ldg(fd + i + 32 + lane);  // one step ahead
-          const int py0 = cy + (int)(d >> 23);
-          reinterpret_cast<uint32_t*>(sd[sb])[lane] = (((d & 0x7FFFFFu) + (uint32_t)((py0 >> 4) * Wd)) << 7) | ((uint32_t)py0 & 15u);
-          __syncwarp();
-          // Every lane loads, dead ones too: a dead column keeps adding its true counts, and a column once below the
-          // running bound stays below it (each step adds at most 32 features to a cell and raises the bound by 32), so
-          // the decision is the same as with zeros.  The loads carry no lane-dependent branch, which lets the compiler
-          // issue all 16 of a step before the first one is used; the half-warp reads the same 64-byte window either way.
-          uint32_t xh[8];
-#pragma unroll
-          for (int m = 0; m < 4; ++m) {
-            const uint4 v = sd[sb][hw * 4 + m];  // features i + 16 hw + 4m .. + 3
-            xh[2 * m] = __byte_perm(lm_plane_rows(col, v.x), lm_plane_rows(col, v.y), 0x5410);
-            xh[2 * m + 1] = __byte_perm(lm_plane_rows(col, v.z), lm_plane_rows(col, v.w), 0x5410);
-          }
-          sb ^= 1;
-          if (lane_alive) words_read += 16;
-          vc_add8n<LM_FILTER_BITS>(ch, xh);
-          // cells that can still reach `need`: CH >= need - (features not yet added); warp-uniform
-          const int done = i + 32;
-          const int thr = need - max(nf - done, 0);
-          if (thr > 0 && (done >= nf || done % LM_FILTER_CHECK == 0)) {
-            vc_fold(ch);
-            lane_alive = (vc_ge(ch, thr) & 0xFFFFu) != 0u;
-            if (!__any_sync(0xffffffffu, lane_alive)) { dead = true; break; }
-            // the totals live on in the low half-words of half-warp 0; the rest starts its partial counts again
-            const uint32_t keep = hw ? 0u : 0xFFFFu;
-#pragma unroll
-            for (int b = 0; b < LM_FILTER_BITS; ++b) ch[b] &= keep;
-          }
-        }
-        if (dead) {
-          if (lane == 0) dropped_feats += (unsigned)nf;  // the reference's work for it (algorithmic bytes / 256)
-          pass = false;
-        }
+      ea_next = __ldcg(p.cand + c_next);
+      fa_next = __ldg(p.finfo + ea_next.x);
+      if (c_next + 1 < total) {
+        eb_next = __ldcg(p.cand + c_next + 1);
+        fb_next = __ldg(p.finfo + eb_next.x);
       }
     }
-    if (pass && lane == 0) {
-      if (p.surv2 && !(fi.w & 2)) p.surv2[atomicAdd(p.queue + 2, 1)] = (uint32_t)c;  // byte-wise refinement (k_refine)
+    int sa = filter_triage(fa), sbt = has_b ? filter_triage(fb) : 0;
+    // While both are counted, one step is two independent chains: every lane issues A's 16 loads and B's 16 with no
+    // lane-dependent branch, so B's loads are in flight while A's words are added.  Once one is dead or finished, the
+    // other goes on alone from where it is.
+    FilterCand k;
+    int i = 0;
+    if (sa == 2 && sbt == 2) {
+      FilterCand kb;
+      filter_setup(k, p, ea, fa, lane);
+      filter_setup(kb, p, eb, fb, lane);
+      const int nfp2 = min(k.nfp, kb.nfp);
+      bool dead_a, dead_b;
+      do {
+        reinterpret_cast<uint32_t*>(sd[sb][0])[lane] = filter_step_desc(k, i, lane, Wd);
+        reinterpret_cast<uint32_t*>(sd[sb][1])[lane] = filter_step_desc(kb, i, lane, Wd);
+        __syncwarp();
+        uint32_t xa[8], xb[8];
+        filter_rows(sd[sb][0] + 4 * hw, k.col, xa);
+        filter_rows(sd[sb][1] + 4 * hw, kb.col, xb);
+        sb ^= 1;
+        words_read += 16u * ((unsigned)k.lane_alive + (unsigned)kb.lane_alive);
+        vc_add8n<LM_FILTER_BITS>(k.ch, xa);
+        vc_add8n<LM_FILTER_BITS>(kb.ch, xb);
+        i += 32;
+        dead_a = filter_dead(k, i, hw);
+        dead_b = filter_dead(kb, i, hw);
+      } while (i < nfp2 && !dead_a && !dead_b);
+      sa = dead_a ? 1 : (i < k.nfp ? 2 : 0);
+      sbt = dead_b ? 1 : (i < kb.nfp ? 2 : 0);
+      if (sbt == 2) k = kb;
+    } else if (sa == 2) {
+      filter_setup(k, p, ea, fa, lane);
+    } else if (sbt == 2) {
+      filter_setup(k, p, eb, fb, lane);
+    }
+    if (sa == 2 || sbt == 2) {
+      // One warp, one candidate: a chain of nfp / 32 steps.
+      bool dead = false;
+      for (; i < k.nfp;) {
+        reinterpret_cast<uint32_t*>(sd[sb][0])[lane] = filter_step_desc(k, i, lane, Wd);
+        __syncwarp();
+        uint32_t xh[8];
+        filter_rows(sd[sb][0] + 4 * hw, k.col, xh);
+        sb ^= 1;
+        if (k.lane_alive) words_read += 16;
+        vc_add8n<LM_FILTER_BITS>(k.ch, xh);
+        i += 32;
+        if (filter_dead(k, i, hw)) { dead = true; break; }
+      }
+      if (sa == 2) sa = dead ? 1 : 0;
+      else sbt = dead ? 1 : 0;
+    }
+    if (lane == 0) {
+      // dropped: the reference's work for it (algorithmic bytes / 256); kept: on to the exact pass
+      if (sa == 1) dropped_feats += (unsigned)fa.y;
+      else if (p.surv2 && !(fa.w & 2)) p.surv2[atomicAdd(p.queue + 2, 1)] = (uint32_t)c;  // byte-wise refinement (k_refine)
       else p.surv[atomicAdd(p.queue + 1, 1)] = (uint32_t)c;
+      if (has_b) {
+        if (sbt == 1) dropped_feats += (unsigned)fb.y;
+        else if (p.surv2 && !(fb.w & 2)) p.surv2[atomicAdd(p.queue + 2, 1)] = (uint32_t)(c + 1);
+        else p.surv[atomicAdd(p.queue + 1, 1)] = (uint32_t)(c + 1);
+      }
     }
   }
   words_read = __reduce_add_sync(0xffffffffu, words_read);
