@@ -1798,7 +1798,14 @@ static int complete_frame(lm_detector* d, bool post, bool survivors) {
                     (long long)d->px_cap);
     }
     const int64_t kept = post ? d->h_post_counts[1] : hres(d)->count;
-    const int64_t cands = post ? d->h_post_counts[3] : hres(d)->coarse_candidates;
+    int64_t cands = post ? d->h_post_counts[3] : hres(d)->coarse_candidates;
+    if (!post && d->px_rank >= 0 && cands > cand_cap(d)) {
+      // behind the exchange the header counts every rank's candidates; this rank's list holds only its own (off[n_work])
+      int own = 0;
+      CU(cudaMemcpyAsync(&own, d->d_off.get() + d->shard_count, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      cands = own;
+    }
     if (kept <= d->res_cap && cands <= cand_cap(d)) return LM_OK;
     if (pass == LM_COMPLETE_PASSES)
       return fail(LM_E_CAPACITY, "%lld records kept of %lld candidates after %d passes: the result block holds %lld, the candidate "
@@ -2887,8 +2894,11 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   if (!d->chain.completed) return fail(LM_E_STATE, "lm_run has not been called");
   if (cap < LM_PLAN_ENTRIES) return fail(LM_E_CAPACITY, "need %d entries", LM_PLAN_ENTRIES);
   CU(cudaSetDevice(d->device));
-  int queue[4];
+  int queue[4], listed = 0;
   CU(cudaMemcpyAsync(queue, d->d_queue.get(), sizeof(queue), cudaMemcpyDeviceToHost, d->stream.get()));
+  // the shard's own list length (off[n_work]): behind the exchange the header counts every rank's candidates
+  if (d->shard_count > 0 && (size_t)d->shard_count < d->d_off.size())
+    CU(cudaMemcpyAsync(&listed, d->d_off.get() + d->shard_count, sizeof(int), cudaMemcpyDeviceToHost, d->stream.get()));
   CU(cudaStreamSynchronize(d->stream.get()));
   const FramePlan& pl = d->chain.plan;
   const LevelHost& low = d->lv[d->L - 1];
@@ -2912,7 +2922,7 @@ extern "C" int lm_debug_plan(lm_detector* d, int32_t* out, int64_t cap) {
   out[14] = (int32_t)std::count_if(d->h_finfo.begin(), d->h_finfo.end(), [](const int4& f) { return (f.w & 2) != 0; });
   out[15] = pl.gated ? 1 : 0;
   // work items of the refinement kernels that ran (-1: it did not run)
-  const int total = (int)std::min<int64_t>(hres(d)->coarse_candidates, cand_cap(d));
+  const int total = (int)std::min<int64_t>(listed, cand_cap(d));  // what the refinement kernels take (k_refine_filter_w)
   if (pl.filter) out[16] = total;
   if (pl.bits) {
     out[17] = std::min(queue[1], total);
@@ -2962,7 +2972,7 @@ extern "C" int lm_counters(lm_detector* d, int64_t* out8) {
   out8[4] = hres(d)->count;
   out8[5] = (int64_t)d->h_counters[1] * 16;
   out8[6] = (int64_t)d->h_counters[4] * 256;  // ... of which: candidates the filter dropped
-  out8[7] = (int64_t)d->h_counters[5] * 4;    // bytes of H-planes the filter read
+  out8[7] = (int64_t)d->h_counters[5] * 4;    // plane bytes the filter and k_refine_bits read (one shared counter)
   return LM_OK;
 }
 

@@ -754,7 +754,8 @@ int lm_debug_time_k1(lm_detector* d, int level, int reps, float* us);
  * k_coarse_packed, [7] templates on k_coarse_bytes, [8] k_coarse_packed stages the bit-planes in shared memory (1/0),
  * [9] its team split S, [10] bit-plane bytes, [11] its tasks ([8]..[11]: -1 without packed templates),
  * [12] the refinement filter is available for the frame size (1/0), [13] bit-sliced refinement (two levels, 1/0),
- * [14] templates of the shard the filter takes, [15] the frame ran depth-gated (1/0), then the work items of
+ * [14] templates of the shard the filter takes, [15] the frame ran depth-gated (1/0), then the work items (this
+ * handle's shard only, also behind the peer exchange) of
  * [16] k_refine_filter_w, [17] k_refine_bits, [18] k_refine<true>, [19] k_refine<false> (-1: it did not run), [20] the
  * CTAs k_refine_bits runs with (the ones resident at once; -1: it did not run), [21] what K1 builds of the lowest level:
  * bit 0 its spread bit-planes, bit 1 its byte linear memories (built only when k_coarse_bytes has templates).

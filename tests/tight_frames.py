@@ -176,6 +176,7 @@ class Model:
         self.rows, self.cols, self.Tr = rows, cols, Tr
         self.Wd, self.Hd = cols // Tr, rows // Tr
         resp = [oracle.response_maps(oracle.spread(q[lr][m], Tr)) for m in range(self.M)]
+        self.resp = resp  # [modality] -> u8 [8, rows, cols] responses of the filtered level
         Tl = self.T[-1]
         low = q[-1]
         self.low_Wd = low[0].shape[1] // Tl
