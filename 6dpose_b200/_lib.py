@@ -47,7 +47,7 @@ SYMBOLS = [
     "lm_set_pose_verify", "lm_pose_verify", "lm_pose_verify_points", "lm_icp_set_verify", "lm_icp_verify",
     "lm_set_pose_search", "lm_icp_set_pose_search", "lm_pose_search_points",
     "lm_track", "lm_track_device", "lm_track_batch", "lm_track_batch_device", "lm_pose_transforms",
-    "lm_peer_track_batch", "lm_peer_track_batch_device",
+    "lm_peer_track_batch", "lm_peer_track_batch_device", "lm_set_track_views", "lm_track_templates", "lm_track_views_points",
 ]
 
 # The pose stage's estimation (LM_ICP_POINT_TO_PLANE / LM_ICP_POINT_TO_POINT / LM_POSE_PSO of include/linemod_b200.h) by
@@ -98,6 +98,17 @@ def verify_options(inlier, rank_by="fitness", min_score=None):
             raise ValueError("rank_by=\"score\" and min_score need pose verification on (inlier_mm not None)")
         return 0, 10.0, 0, -math.inf
     return 1, inlier_mm(inlier), VERIFY_RANKS[rank_by], lo
+
+
+def track_views_option(turn_deg):
+    """lm_set_track_views's (on, turn_deg) for Detector.setTrackViews: None turns view following off; otherwise a number
+    in [0, 180) degrees.  TypeError / ValueError before any device work."""
+    if turn_deg is None:
+        return 0, 0.0
+    d = _real(turn_deg, "turn_deg")
+    if not 0.0 <= d < 180.0:
+        raise ValueError("turn_deg must lie in [0, 180) degrees, got %r" % turn_deg)
+    return 1, d
 
 
 # The particle swarm of estimation="pso" (lm_set_pose_search): its settings by name, with their defaults and limits
@@ -475,6 +486,9 @@ def load():
     L.lm_peer_track_batch.argtypes = L.lm_track_batch.argtypes
     L.lm_peer_track_batch_device.argtypes = L.lm_track_batch_device.argtypes
     L.lm_pose_transforms.argtypes = [vp, f64p, c_i64, ctypes.POINTER(c_i64)]
+    L.lm_set_track_views.argtypes = [vp, c_int, ctypes.c_double]
+    L.lm_track_templates.argtypes = [vp, i32p, c_i64, ctypes.POINTER(c_i64)]
+    L.lm_track_views_points.argtypes = [c_int, c_i64, f32p, f32p, c_i64, f64p, ctypes.c_double, ctypes.POINTER(c_i64), f64p]
     L.lm_icp_create.argtypes = [c_int, ctypes.POINTER(vp)]
     L.lm_icp_destroy.argtypes = [vp]
     L.lm_icp_destroy.restype = None
@@ -1175,6 +1189,23 @@ class NativeDetector:
             check(self._L.lm_pose_transforms(self._h, out.ctypes.data_as(f64p), out.shape[0], ctypes.byref(n)))
         return out
 
+    def set_track_views(self, on, turn_deg=0.0):
+        """lm_set_track_views for the next track calls: view following on or off, and the turn (degrees) from the
+        template's view beyond which an object re-chooses its template."""
+        check(self._L.lm_set_track_views(self._h, 1 if on else 0, float(turn_deg)))
+
+    def track_templates(self):
+        """The template (within its class) of every entry of the last finished track run (lm_track_templates): int32 [n]."""
+        n = ctypes.c_int64()
+        i32p = ctypes.POINTER(ctypes.c_int32)
+        rc = self._L.lm_track_templates(self._h, None, 0, ctypes.byref(n))
+        if rc != LM_E_CAPACITY:
+            check(rc)
+        out = np.zeros(int(n.value), np.int32)
+        if out.size:
+            check(self._L.lm_track_templates(self._h, out.ctypes.data_as(i32p), out.size, ctypes.byref(n)))
+        return out
+
     @staticmethod
     def track_objects(objects):
         """lm_track_object [n] of (class_index, template_id, T [4,4] f64) triples."""
@@ -1496,3 +1527,20 @@ def pose_verify_points(pts, T, scene, sceneK, inlier_mm=10.0, device=0):
                                   sK.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), float(inlier_mm),
                                   counts.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), ctypes.byref(score)))
     return float(score.value), counts
+
+
+def track_views_points(R_b, t_b, k, T, turn_deg, device=0):
+    """View following on caller arrays (lm_track_views_points): one object at template k with T [4,4] f64 among the
+    templates R_b [n,3,3], t_b [n,3] f32 of one class.  Returns (chosen template, T [4,4] f64)."""
+    L = load()
+    Rb = np.ascontiguousarray(R_b, np.float32).reshape(-1, 9)
+    tb = np.ascontiguousarray(t_b, np.float32).reshape(-1, 3)
+    if Rb.shape[0] != tb.shape[0]:
+        raise ValueError("%d rotations and %d translations" % (Rb.shape[0], tb.shape[0]))
+    T = np.ascontiguousarray(T, np.float64).reshape(16)
+    out = np.zeros(16, np.float64)
+    chosen = ctypes.c_int64()
+    f32p, f64p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)
+    check(L.lm_track_views_points(int(device), Rb.shape[0], Rb.ctypes.data_as(f32p), tb.ctypes.data_as(f32p), int(k), T.ctypes.data_as(f64p),
+                                  float(turn_deg), ctypes.byref(chosen), out.ctypes.data_as(f64p)))
+    return int(chosen.value), out.reshape(4, 4)

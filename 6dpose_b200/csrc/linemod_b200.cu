@@ -251,6 +251,7 @@ struct lm_detector {
   int pose_estimation = LM_ICP_POINT_TO_PLANE;  // lm_set_pose_estimation: for the next pose stage
   PoseVerifyOptions pose_verify = {0, LM_VERIFY_RANK_FITNESS, 10.0, -INFINITY};  // lm_set_pose_verify: likewise
   PoseSearch pose_search = pose_search_default();  // lm_set_pose_search: likewise
+  int track_views = 0; double track_view_tau = 0.0;  // lm_set_track_views: for the next track calls
   int64_t pose_stats[4] = {0, 0, 0, 0};  // lm_pose_stats of the last completed pose stage
 
   // multi-GPU exchange fused into k_refine (lm_peer_*)
@@ -2558,7 +2559,8 @@ static int track(lm_detector* d, bool peers, bool batch, int n_frames, const voi
     if (rc) return rc;
     d->px_pose_seq += pose_batch_chunks(first[(size_t)n_frames]);
   }
-  PoseOptions o = {rows, cols, 1, max_iterations, d->pose_estimation, st, share ? &sh : nullptr, d->pose_verify, d->pose_search};
+  PoseOptions o = {rows, cols, 1, max_iterations, d->pose_estimation, st, share ? &sh : nullptr, d->pose_verify, d->pose_search,
+                   d->track_views, d->track_view_tau};
   return pose_stage_track(d->pose, o, n_frames, scene, sceneK, obj.data(), first.data(), margin_px, &d->launches, T_out, R_out, t_out,
                           residual, status, box, peers ? d->pose_stats : nullptr);
 }
@@ -2605,6 +2607,22 @@ extern "C" int lm_peer_track_batch_device(lm_detector* d, int n_frames, const vo
                                           double* t_out, float* residual, int32_t* status, int32_t* box, void* stream) {
   return track(d, true, true, n_frames, depth, depth, depth_pitch, depth_format, depth_scale, (cudaStream_t)stream, rows, cols, sceneK,
                objects, n_objects, max_iterations, margin_px, T_out, R_out, t_out, residual, status, box);
+}
+
+extern "C" int lm_set_track_views(lm_detector* d, int on, double turn_deg) {
+  if (!d) return fail(LM_E_INVALID, "null detector");
+  double tau = 0.0;
+  const int rc = track_view_tau(on, turn_deg, &tau);
+  if (rc) return rc;
+  d->track_views = on ? 1 : 0;
+  d->track_view_tau = tau;
+  return LM_OK;
+}
+
+extern "C" int lm_track_templates(lm_detector* d, int32_t* template_id, int64_t cap, int64_t* n) {
+  if (!d || !n) return fail(LM_E_INVALID, "null argument");
+  if (!d->pose) return fail(LM_E_STATE, "no pose stage has run");
+  return pose_stage_track_templates(d->pose, template_id, cap, n);
 }
 
 extern "C" int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n) {

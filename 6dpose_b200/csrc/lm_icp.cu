@@ -1975,6 +1975,112 @@ __global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
   }
 }
 
+// --------------------------------------------------------------------------------------------
+// view following (lm_set_track_views, include/linemod_b200.h): each tracked object re-chooses its template from its
+// pose before k_track_cloud reads it
+// --------------------------------------------------------------------------------------------
+#define VIEW_THREADS 256
+
+struct TrackViewParams {
+  TrackObject* obj;           // [counts[0]]: template and T, overwritten with the chosen template and T'
+  const int32_t* counts;      // [0] objects
+  const PoseRt* rt;           // per template of the bank: R_b, t_b of its render
+  const uint8_t* has;         // per template of the bank: 1 when its render is registered
+  const int32_t* class_begin; // [n_classes + 1]
+  int32_t n_classes;
+  double tau;                 // 1 + 2 cos(turn_deg)
+};
+
+// ((a0 * b0) + a1 * b1) + a2 * b2, every operation correctly rounded
+__device__ __forceinline__ double view_dot3(double a0, double b0, double a1, double b1, double a2, double b2) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a0, b0), __dmul_rn(a1, b1)), __dmul_rn(a2, b2));
+}
+
+// trace(Ro^T R): s = s + Ro[r][c] * R[r][c] from 0.0, r outer, c inner
+__device__ __forceinline__ double view_score(const double* Ro, const float* R) {
+  double s = 0.0;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) s = __dadd_rn(s, __dmul_rn(Ro[k], (double)R[k]));
+  return s;
+}
+
+// One CTA per object.  Its class is the one whose templates hold its template k; every thread scans a stride of the
+// class's templates with a render, a block arg-max (nms_argmax_warp: lowest index on ties, a NaN score never a
+// candidate) gives j*, and thread 0 decides and re-expresses T (include/linemod_b200.h, lm_set_track_views).
+__global__ void __launch_bounds__(VIEW_THREADS) k_track_views(TrackViewParams p) {
+  __shared__ double s_Ro[9];
+  __shared__ int32_t s_range[2];
+  __shared__ unsigned long long s_key[VIEW_THREADS / 32];
+  __shared__ int s_idx[VIEW_THREADS / 32];
+  const int i = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  if (i >= p.counts[0]) return;  // block-uniform
+  TrackObject* o = p.obj + i;
+  const int64_t k = o->g;
+  if (tid < 9) {
+    const int r = tid / 3, c = tid - 3 * (tid / 3);
+    const float* Rk = p.rt[k].R;
+    s_Ro[tid] = view_dot3(o->T[4 * r], (double)Rk[c], o->T[4 * r + 1], (double)Rk[3 + c], o->T[4 * r + 2], (double)Rk[6 + c]);
+  }
+  if (tid == 0) {  // the last class beginning at or before k (an empty class shares its begin with the next)
+    int lo = 0, hi = p.n_classes;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (p.class_begin[mid] <= k) lo = mid;
+      else hi = mid;
+    }
+    s_range[0] = p.class_begin[lo]; s_range[1] = p.class_begin[lo + 1];
+  }
+  __syncthreads();
+  double Ro[9];
+#pragma unroll
+  for (int q = 0; q < 9; ++q) Ro[q] = s_Ro[q];
+  unsigned long long bk = 0ull;
+  int bi = -1;
+  for (int j = s_range[0] + tid; j < s_range[1]; j += VIEW_THREADS) {
+    if (!p.has[j]) continue;
+    const double s = view_score(Ro, p.rt[j].R);
+    if (s != s) continue;
+    const unsigned long long key = nms_score_key(s);
+    if (bi < 0 || key > bk) { bk = key; bi = j; }  // ascending j: the first of equal keys stays
+  }
+  nms_argmax_warp(bk, bi);
+  if (lane == 0) { s_key[wid] = bk; s_idx[wid] = bi; }
+  __syncthreads();
+  if (wid != 0) return;
+  bk = lane < VIEW_THREADS / 32 ? s_key[lane] : 0ull;
+  bi = lane < VIEW_THREADS / 32 ? s_idx[lane] : -1;
+  nms_argmax_warp(bk, bi);
+  if (lane != 0) return;
+  const double sk = view_score(Ro, p.rt[k].R);
+  if (!(sk < p.tau) || bi < 0 || bi == k) return;
+  const float* Rj = p.rt[bi].R;
+  if (!(view_score(Ro, Rj) > sk)) return;
+  const float* Rk = p.rt[k].R;
+  double bk3[3], bj3[3], QR[9], Qt[3], T[16];
+  for (int r = 0; r < 3; ++r) {
+    bk3[r] = __ddiv_rn((double)p.rt[k].t[r], 1000.0);
+    bj3[r] = __ddiv_rn((double)p.rt[bi].t[r], 1000.0);
+  }
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c)
+      QR[3 * r + c] = view_dot3(Rk[3 * r], Rj[3 * c], Rk[3 * r + 1], Rj[3 * c + 1], Rk[3 * r + 2], Rj[3 * c + 2]);
+  for (int r = 0; r < 3; ++r) Qt[r] = __dsub_rn(bk3[r], view_dot3(QR[3 * r], bj3[0], QR[3 * r + 1], bj3[1], QR[3 * r + 2], bj3[2]));
+  for (int q = 0; q < 16; ++q) T[q] = o->T[q];
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) o->T[4 * r + c] = view_dot3(T[4 * r], QR[c], T[4 * r + 1], QR[3 + c], T[4 * r + 2], QR[6 + c]);
+    o->T[4 * r + 3] = __dadd_rn(view_dot3(T[4 * r], Qt[0], T[4 * r + 1], Qt[1], T[4 * r + 2], Qt[2]), T[4 * r + 3]);
+  }
+  o->T[12] = o->T[13] = o->T[14] = 0.0; o->T[15] = 1.0;
+  o->g = bi;
+}
+
+int track_view_tau(int on, double turn_deg, double* tau) {
+  if (on && !(turn_deg >= 0.0 && turn_deg < 180.0))
+    return lm_fail(LM_E_INVALID, "turn_deg must lie in [0, 180), got %g", turn_deg);
+  *tau = on ? 1.0 + 2.0 * cos(turn_deg * 0.017453292519943295) : 0.0;
+  return LM_OK;
+}
+
 struct TplHost {
   bool set = false;
   int box[4] = {0, 0, 0, 0};
@@ -1990,6 +2096,7 @@ struct lm_pose_stage {
   int64_t area_max = 0;        // largest crop
   DeviceArray<PoseTpl> d_tpl; DeviceArray<uint16_t> d_crops; DeviceArray<int32_t> d_class_begin;
   DeviceArray<PoseRt> d_rt;    // per template: R, t of its render (k_pose_nms composes the poses)
+  DeviceArray<uint8_t> d_has;  // per template: 1 when its render is registered (k_track_views)
   // per-chunk buffers for pose_slots() survivors of pose_area() points per crop (pose_buffers); d_posed: a shared
   // chunk's posed flags per slot, which k_pose_collect gathers into the run's
   DeviceArray<double> d_raw, d_cpts, d_pts, d_nrm;
@@ -2043,6 +2150,10 @@ struct lm_pose_stage {
   // entries' transformations, or (xf_pending, a run with the pose NMS) its frames' first survivors to find them from
   bool finished_ok = false, xf_pending = false;
   std::vector<double> xf;
+  // a finished track run's template per entry within its class (pose_stage_track_templates); tracked false: the run
+  // last finished was no track run
+  bool tracked = false;
+  std::vector<int32_t> track_tpl;
   std::vector<int64_t> finished_first;
 };
 
@@ -2108,6 +2219,7 @@ bool pose_stage_covers(const lm_pose_stage* s, const int32_t* sel, int64_t n_sel
 static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
   std::vector<PoseTpl> tp(s->tpl.size());
   std::vector<PoseRt> rt(s->tpl.size());
+  std::vector<uint8_t> has(s->tpl.size());
   int64_t pool = 0;
   for (size_t g = 0; g < s->tpl.size(); ++g) {
     const TplHost& h = s->tpl[g];
@@ -2118,15 +2230,17 @@ static int pose_upload(lm_pose_stage* s, cudaStream_t st) {
     for (int k = 0; k < 9; ++k) d.K[k] = h.set ? h.K[k] : 0.f;
     for (int k = 0; k < 9; ++k) rt[g].R[k] = h.set ? h.R[k] : 0.f;
     for (int k = 0; k < 3; ++k) rt[g].t[k] = h.set ? h.t[k] : 0.f;
+    has[g] = h.set ? 1 : 0;
     pool += (int64_t)h.crop.size();
   }
   std::vector<uint16_t> crops((size_t)std::max<int64_t>(pool, 1));
   for (size_t g = 0; g < s->tpl.size(); ++g)
     if (!s->tpl[g].crop.empty()) memcpy(crops.data() + tp[g].crop, s->tpl[g].crop.data(), s->tpl[g].crop.size() * sizeof(uint16_t));
   CUI(cudaStreamSynchronize(st));  // an earlier frame may still read the old copy
-  s->d_tpl.reset(); s->d_crops.reset(); s->d_class_begin.reset(); s->d_rt.reset();
+  s->d_tpl.reset(); s->d_crops.reset(); s->d_class_begin.reset(); s->d_rt.reset(); s->d_has.reset();
   CUI(upload(s->d_tpl, tp, st));
   CUI(upload(s->d_rt, rt, st));
+  CUI(upload(s->d_has, has, st));
   CUI(upload(s->d_crops, crops, st));
   CUI(upload(s->d_class_begin, s->class_begin, st));
   CUI(cudaStreamSynchronize(st));  // host vectors go out of scope
@@ -2593,9 +2707,10 @@ static bool survivor_fits(const TplHost& h, const lm_match& m, int srows, int sc
 
 // The start of every finish: the run last finished is forgotten, its verification and transformations with it.
 static void pose_forget(lm_pose_stage* s) {
-  s->verified = s->finished_ok = s->xf_pending = false;
+  s->verified = s->finished_ok = s->xf_pending = s->tracked = false;
   s->ver.clear();
   s->xf.clear();
+  s->track_tpl.clear();
 }
 
 // n kept poses e[] into the caller's arrays (out may be null).
@@ -2753,6 +2868,45 @@ extern "C" int lm_pose_verify_points(int device, const double* pts, int64_t n, c
   CUI(cudaMemcpy(&v, d_out, sizeof(v), cudaMemcpyDeviceToHost));
   memcpy(counts6, v.counts, sizeof(v.counts));
   *score = v.score;
+  return LM_OK;
+}
+
+// View following on caller arrays (lm_track_views_points): k_track_views over one object of a one-class bank of n
+// templates, every one with a render.
+extern "C" int lm_track_views_points(int device, int64_t n, const float* R_b, const float* t_b, int64_t k, const double* T, double turn_deg,
+                                     int64_t* chosen, double* T_out) {
+  if (!R_b || !t_b || !T || !chosen || !T_out) return lm_fail(LM_E_INVALID, "null argument");
+  if (n < 1 || n > 0x7FFFFFFFll) return lm_fail(LM_E_INVALID, "%lld templates, 1 to 2^31 - 1", (long long)n);
+  if (k < 0 || k >= n) return lm_fail(LM_E_INVALID, "template %lld outside the %lld", (long long)k, (long long)n);
+  for (int q = 0; q < 16; ++q)
+    if (!std::isfinite(T[q])) return lm_fail(LM_E_INVALID, "T[%d] is not finite", q);
+  double tau = 0.0;
+  int rc = track_view_tau(1, turn_deg, &tau);
+  if (!rc) rc = open_device(device);
+  if (rc) return rc;
+  std::vector<PoseRt> rt((size_t)n);
+  for (int64_t j = 0; j < n; ++j) {
+    memcpy(rt[(size_t)j].R, R_b + 9 * j, sizeof(rt[0].R));
+    memcpy(rt[(size_t)j].t, t_b + 3 * j, sizeof(rt[0].t));
+  }
+  const std::vector<uint8_t> has((size_t)n, 1);
+  const std::vector<int32_t> cb = {0, (int32_t)n, 1};  // class_begin, then the object count
+  std::vector<TrackObject> obj(1);
+  obj[0].g = k;
+  memcpy(obj[0].T, T, sizeof(obj[0].T));
+  DeviceArray<PoseRt> d_rt; DeviceArray<uint8_t> d_has; DeviceArray<int32_t> d_cb; DeviceArray<TrackObject> d_obj;
+  CUI(upload(d_rt, rt, 0));
+  CUI(upload(d_has, has, 0));
+  CUI(upload(d_cb, cb, 0));
+  CUI(upload(d_obj, obj, 0));
+  TrackViewParams v;
+  v.obj = d_obj.get(); v.counts = d_cb.get() + 2; v.rt = d_rt.get(); v.has = d_has.get(); v.class_begin = d_cb.get();
+  v.n_classes = 1; v.tau = tau;
+  k_track_views<<<1, VIEW_THREADS>>>(v);
+  CUI(cudaGetLastError());
+  CUI(cudaMemcpy(obj.data(), d_obj.get(), sizeof(TrackObject), cudaMemcpyDeviceToHost));
+  *chosen = obj[0].g;
+  memcpy(T_out, obj[0].T, sizeof(obj[0].T));
   return LM_OK;
 }
 
@@ -3271,7 +3425,7 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
       stats4[3] = sh ? 1 : 0;
     }
     s->verified = verify;
-    s->finished_ok = true;
+    s->finished_ok = s->tracked = true;
     return LM_OK;
   }
   if ((size_t)n > s->h_trec.size()) {
@@ -3295,6 +3449,15 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
   int64_t stage_launches = 0;
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_CHUNK;
+    if (o.views) {  // every rank re-chooses every object of the chunk, so all ranks hold the same objects
+      TrackViewParams v;
+      v.obj = s->d_tobj.get() + c0; v.counts = s->d_bstat.get() + 4 * c + 3;
+      v.rt = s->d_rt.get(); v.has = s->d_has.get(); v.class_begin = s->d_class_begin.get();
+      v.n_classes = (int32_t)s->class_begin.size() - 1; v.tau = o.view_tau;
+      k_track_views<<<stat[(size_t)4 * c + 3], VIEW_THREADS, 0, st>>>(v);
+      ++stage_launches;
+      ++*launches;
+    }
     TrackParams q;
     memset(&q, 0, sizeof(q));
     q.obj = s->d_tobj.get() + c0; q.tpl = s->d_tpl.get(); q.crops = s->d_crops.get();
@@ -3312,6 +3475,11 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
   CUI(cudaMemcpyAsync(s->h_trec.get(), s->d_trec.get(), sizeof(TrackRec) * n, cudaMemcpyDeviceToHost, st));
   if (verify) CUI(cudaMemcpyAsync(s->h_bver.get(), s->d_bver.get(), sizeof(PoseVerify) * n, cudaMemcpyDeviceToHost, st));
   CUI(cudaMemcpyAsync(s->h_bstat.get(), s->d_bstat.get(), sizeof(int32_t) * 4 * nc, cudaMemcpyDeviceToHost, st));
+  std::vector<TrackObject> chosen;  // view following: the objects as k_track_views left them
+  if (o.views) {
+    chosen.resize((size_t)n);
+    CUI(cudaMemcpyAsync(chosen.data(), s->d_tobj.get(), sizeof(TrackObject) * n, cudaMemcpyDeviceToHost, st));
+  }
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
   int64_t published = 0;
@@ -3324,20 +3492,35 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
     stats4[3] = sh ? 1 : 0;
   }
   s->xf.assign(16 * (size_t)n, std::numeric_limits<double>::quiet_NaN());
+  s->track_tpl.resize((size_t)n);
   for (int64_t i = 0; i < n; ++i) {
     const TrackRec& e = s->h_trec[(size_t)i];
     status[i] = e.status;
     memcpy(box + 4 * i, e.box, sizeof(e.box));
+    // an entry not tracked keeps its start, template included
+    const int64_t g = e.status == LM_TRACK_TRACKED && o.views ? chosen[(size_t)i].g : obj[i].g;
+    const int64_t cls = std::upper_bound(s->class_begin.begin(), s->class_begin.end(), (int32_t)obj[i].g) - s->class_begin.begin() - 1;
+    s->track_tpl[(size_t)i] = (int32_t)(g - s->class_begin[(size_t)cls]);
     if (e.status != LM_TRACK_TRACKED) { residual[i] = -1.f; continue; }
     const IcpOut& q = s->h_bouts[(size_t)i];
-    const TplHost& h = s->tpl[(size_t)obj[i].g];
+    const TplHost& h = s->tpl[(size_t)g];
     render_pose(q, h.R, h.t, R_out + 9 * i, t_out + 3 * i, residual + i);
     memcpy(T_out + 16 * i, q.T, sizeof(q.T));
     memcpy(s->xf.data() + 16 * i, q.T, sizeof(q.T));
   }
   if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + n);
   s->verified = verify;
-  s->finished_ok = true;
+  s->finished_ok = s->tracked = true;
+  return LM_OK;
+}
+
+int pose_stage_track_templates(const lm_pose_stage* s, int32_t* template_id, int64_t cap, int64_t* n) {
+  if (!n || (cap > 0 && !template_id)) return lm_fail(LM_E_INVALID, "null argument");
+  if (!s || !s->finished_ok || !s->tracked)
+    return lm_fail(LM_E_STATE, "the pose run last finished was no track run (lm_track, lm_track_batch, lm_peer_track_batch), or it failed");
+  *n = (int64_t)s->track_tpl.size();
+  if (*n > cap) return lm_fail(LM_E_CAPACITY, "%lld entries, capacity %lld", (long long)*n, (long long)cap);
+  if (*n) memcpy(template_id, s->track_tpl.data(), sizeof(int32_t) * (size_t)*n);
   return LM_OK;
 }
 

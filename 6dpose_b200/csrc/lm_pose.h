@@ -10,7 +10,8 @@
 // kernel) composes the poses on the device instead, runs the greedy translation NMS of linemod_ros/detect.py over them
 // and compacts the kept ones into one output block.  A track run (lm_track, lm_track_batch) is a run whose clouds
 // k_track_cloud builds from each object's transformation and the window its model projects to in its own frame, in
-// place of k_pose_cloud.
+// place of k_pose_cloud; with view following on (lm_set_track_views), k_track_views re-chooses each object's template
+// and T ahead of it.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -79,6 +80,8 @@ struct PoseOptions {
   const PoseShare* share;     // null: this rank refines every survivor (LM_POSE_PSO: always)
   PoseVerifyOptions verify;  // zero: off
   PoseSearch search;          // LM_POSE_PSO only
+  int views;                  // track runs: view following on (lm_set_track_views), k_track_views ahead of each chunk
+  double view_tau;            // its threshold 1 + 2 cos(turn_deg)
 };
 
 // One run of the pose stage: a batch of frames (lm_detect_batch, lm_peer_detect_batch), or a frame as a one-frame run
@@ -145,6 +148,12 @@ int pose_track_scene(lm_pose_stage* s, cudaStream_t st, int n_frames, const uint
 int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const uint16_t* d_scene, const float* sK, const TrackObject* obj,
                      const int64_t* first, int margin, int64_t* launches, double* T_out, double* R_out, double* t_out, float* residual,
                      int32_t* status, int32_t* box, int64_t* stats4);
+// LM_E_INVALID unless turn_deg lies in [0, 180) (on only); else *tau = 1 + 2 cos(turn_deg) (libm cos), 0 when off.
+int track_view_tau(int on, double turn_deg, double* tau);
+// The template of every entry of the run last finished (lm_track_templates), within its class, in entry order: the one
+// view following chose for a TRACKED entry, the start's for any other.  LM_E_STATE unless that run was a track run that
+// succeeded; LM_E_CAPACITY (with *n) beyond cap.
+int pose_stage_track_templates(const lm_pose_stage* s, int32_t* template_id, int64_t cap, int64_t* n);
 // The transformation of every entry of the run last finished (lm_pose_transforms), in entry order, T_out + 16k; NaN for an
 // entry without a pose.  LM_E_STATE once another run has been enqueued or the last one failed; LM_E_CAPACITY (with *n)
 // beyond cap.  The pose NMS's kept entries are matched to their survivors on the host, from one copy of the run's ICP

@@ -68,6 +68,7 @@ class Detector:
         self._template_depths = None  # training distances registered with the native handle (setTemplateDepths)
         self._peers = None  # (rank, world) once dist.connect_peers has wired the fused exchange
         self._verify = _lib.verify_options(None)  # lm_set_pose_verify's arguments (setPoseVerification)
+        self._views = _lib.track_views_option(None)  # lm_set_track_views's arguments (setTrackViews)
         self._search = _lib.pose_search_options()  # lm_set_pose_search's arguments (setPoseSearch)
         self._render_poses = {}  # class_id -> (R [n,3,3], t [n,3]) f32 of its registered renders (track's dict starts)
         self.device = _default_device()
@@ -308,6 +309,15 @@ class Detector:
         survivors scoring below it are dropped before the pose NMS.  A pose stage shared over the ranks verifies too."""
         self._verify = _lib.verify_options(inlier_mm, rank_by, min_score)
 
+    def setTrackViews(self, turn_deg=None):
+        """View following for track, track_batch and dist.track_batch_sharded (include/linemod_b200.h,
+        lm_set_track_views): once an object has turned more than turn_deg degrees from its template's training view,
+        it switches to the template of its class whose view is closest to its current orientation before its clouds are
+        built, so the ICP keeps registering the surface the camera now sees.  The returned Match.template_id is the
+        template chosen, and the poseRefine's R, t and transformation belong to it, so feeding the pairs back continues
+        from it.  None turns view following off (the default).  Checked here, before any device work."""
+        self._views = _lib.track_views_option(turn_deg)
+
     def setPoseSearch(self, particles=64, iterations=40, dt_mm=40.0, dr_deg=30.0, clamp_mm=20.0, seed=0):
         """The particle swarm of estimation="pso" (include/linemod_b200.h, LM_POSE_PSO / lm_set_pose_search) for
         match_refine, detect, the batch calls and dist's unshared sharded calls: particles, iterations, the bounds of the
@@ -320,6 +330,7 @@ class Detector:
         nat = self._select(list(class_ids))
         nat.set_pose_verify(*self._verify)
         nat.set_pose_search(*self._search)
+        nat.set_track_views(*self._views)
         return nat
 
     def _verification(self, nat, sizes):
@@ -523,7 +534,7 @@ class Detector:
                 raise TypeError("depth must be a uint16 HxW depth image (mm)")
             nat = self._pose_native(())
             got = nat.track(depth, sK, triples, max_iterations, margin_px, estimation)
-        return self._track_pairs(starts, got, self._verification(nat, [len(starts)])[0], estimation)
+        return self._track_pairs(starts, got, self._verification(nat, [len(starts)])[0], nat.track_templates(), estimation)
 
     def track_batch(self, depths, sceneK, objects, max_iterations=30, margin_px=4, estimation="point_to_plane", depth_scale=1.0,
                     stream=None):
@@ -567,7 +578,9 @@ class Detector:
             run = nat.peer_track_batch if peers else nat.track_batch
             got = run(np.stack(depths), K, triples, max_iterations, margin_px, estimation)
         ver = self._verification(nat, [len(s) for s in starts])
-        return [self._track_pairs(s, g, v, estimation) for s, g, v in zip(starts, got, ver)]
+        tpl = nat.track_templates()
+        at = np.cumsum([0] + [len(s) for s in starts])
+        return [self._track_pairs(s, g, v, tpl[a:b], estimation) for s, g, v, a, b in zip(starts, got, ver, at[:-1], at[1:])]
 
     def _track_starts(self, objects, what):
         # track's objects as (class_index, template_id, T, Match, R, t); TypeError / ValueError naming `what`
@@ -618,12 +631,12 @@ class Detector:
         st = _lib.device_stream(stream, self.device)
         return ([pl[0] for pl in planes], planes[0][1], fmt, scale, int(tensors[0].shape[0]), int(tensors[0].shape[1]), st.cuda_stream)
 
-    def _track_pairs(self, starts, got, ver, estimation):
-        # [(Match, poseRefine)] of one frame's track results, one per start
+    def _track_pairs(self, starts, got, ver, templates, estimation):
+        # [(Match, poseRefine)] of one frame's track results, one per start; templates: each entry's (lm_track_templates)
         from .pose_refine import poseRefine
         status, T, R, t, res, box = got
         pairs = []
-        for i, (_, tid, T0, m0, R0, t0) in enumerate(starts):
+        for i, (_, _, T0, m0, R0, t0) in enumerate(starts):
             p = poseRefine(estimation)
             p._track_status = _lib.TRACK_STATUS[int(status[i])]
             p._residual = float(res[i])
@@ -636,7 +649,7 @@ class Detector:
                 p._R = None if R0 is None else np.asarray(R0, np.float64).reshape(3, 3).copy()
                 p._t = None if t0 is None else np.asarray(t0, np.float64).reshape(3, 1).copy()
                 p._T = T0.copy()
-            pairs.append((Match(x, y, m0.similarity, m0.class_id, tid), p))
+            pairs.append((Match(x, y, m0.similarity, m0.class_id, int(templates[i])), p))
         return pairs
 
     def _to_matches(self, out):

@@ -486,6 +486,9 @@ int lm_pose_verify_points(int device, const double* pts, int64_t n, const double
  *            with row 3 = (0, 0, 0, 1).  T * init_base then gives (R, t) back up to rounding; bit for bit only for a T
  *            that came from the device.
  * Each object of a call is one slot of one pose-stage chunk (n <= 1024):
+ *   0. View following (lm_set_track_views, off by default): the object may first switch to the template of its class
+ *      whose training view lies closest to its current orientation, with T re-expressed for it; every later step then
+ *      uses that template.  Off, the object keeps its template.
  *   1. Model cloud: exactly the pose stage's source cloud for that template -- its registered crop back-projected
  *      (LM_POSE_CAPTURE_RAW_MODEL) and voxel down-sampled -- bit-identical to what a detected survivor of the template gets.
  *   2. Window: every raw model point projected under T with verification's step 3, operation for operation; the
@@ -512,7 +515,7 @@ int lm_pose_verify_points(int device, const double* pts, int64_t n, const double
  * A call runs on the detector's stream and returns once the outputs are on the host; it abandons a frame whose pose stage
  * is pending.  lm_debug_pose_clouds then describes its chunk: slot i is object i, POSED is 1 for TRACKED, INIT is T,
  * and LM_POSE_CAPTURE_WINDOW gives the window and status.  Launches: 5 (point-to-plane) or 4, plus 1 when verifying, plus
- * 1 for lm_track_device's conversion.
+ * 1 with view following (per chunk, in every track call), plus 1 for lm_track_device's conversion.
  *   lm_track          depth: rows x cols u16 mm on the host, copied.
  *   lm_track_device   depth: a pitched device plane, LM_DEPTH_U16_MM or LM_DEPTH_F32 with depth_scale, converted as
  *                     lm_bind_images_device converts it and ordered as it orders the frame: an event on `stream` gates the
@@ -538,6 +541,48 @@ int lm_track_device(lm_detector* d, const void* depth, int64_t depth_pitch, int 
                     double* R_out, double* t_out, float* residual, int32_t* status, int32_t* box, void* stream);
 int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n);
 
+/* View following for the track calls.  A tracked object's model cloud is the surface its template's render saw from one
+ * viewpoint; once the object has turned far from that view, the scene shows faces the cloud lacks and the ICP drifts.
+ * With view following on, k_track_views (one CTA per object, one launch per chunk, ahead of k_track_cloud) re-chooses
+ * each object's template among the registered renders of its class from its rotation alone, and rewrites the object's
+ * template and T on the device, so the window, both clouds, IcpJob::init, verification and LM_POSE_CAPTURE_* all see the
+ * chosen template.  The rule, in double, every operation correctly rounded in the order written and no FMA; R_b, t_b
+ * are the registered f32 values widened; the object has template k of class c and T (4x4, row-major):
+ *   1. tau = 1.0 + 2.0 * cos(turn_deg * 0.017453292519943295) (libm cos, on the host).
+ *   2. Ro[r][c] = ((T[r][0] * Rk[0][c]) + T[r][1] * Rk[1][c]) + T[r][2] * Rk[2][c], Rk = R_b of template k.
+ *   3. s_j = trace(Ro^T R_j) for every template j of class c with a registered render (k included), summed from 0.0 as
+ *      s = s + Ro[r][c] * R_j[r][c], r outer, c inner.  A NaN s_j is no candidate.
+ *   4. !(s_k < tau): keep k (the object is within turn_deg of its template's view).  Otherwise j* = arg-max s_j, the
+ *      lowest j on ties; switch only when j* != k and s_j* > s_k.  Kept: T stays the input's bits.
+ *   5. Switching: P_j = [R_j | b_j], b_j[r] = t_bj[r] / 1000.0 (metres on every axis, since the render cloud is metric;
+ *      unlike init_base, which converts t.z only), and
+ *        Q_R[r][c] = ((Rk[r][0] * Rj[c][0]) + Rk[r][1] * Rj[c][1]) + Rk[r][2] * Rj[c][2]            (Rk Rj^T)
+ *        Q_t[r]    = b_k[r] - (((Q_R[r][0] * b_j[0]) + Q_R[r][1] * b_j[1]) + Q_R[r][2] * b_j[2])
+ *        T'[r][c]  = ((T[r][0] * Q_R[0][c]) + T[r][1] * Q_R[1][c]) + T[r][2] * Q_R[2][c]
+ *        T'[r][3]  = (((T[r][0] * Q_t[0]) + T[r][1] * Q_t[1]) + T[r][2] * Q_t[2]) + T[r][3],   row 3 = (0, 0, 0, 1)
+ *      so the physical object stays where T put it.
+ * A call with view following on therefore returns, bit for bit, what the same call with it off returns for the objects
+ * (class, j*, T') -- status, box, T, R, t, residual, lm_pose_transforms and lm_pose_verify -- and its R_out / t_out are
+ * composed with the chosen template's render pose.  Shared over the ranks, every rank re-chooses every object of each
+ * chunk, so the exchange's layout is unchanged.
+ *   lm_set_track_views  for the detector's next lm_track, lm_track_device, lm_track_batch, lm_track_batch_device,
+ *                       lm_peer_track_batch and lm_peer_track_batch_device.  on 0 ignores turn_deg.  LM_E_INVALID when
+ *                       on and turn_deg is NaN, negative or >= 180.  No device work (a host-only handle takes it);
+ *                       loading another bank keeps it.
+ *   lm_track_templates  template_id[k]: the template within its class of entry k of the track run last finished, in
+ *                       entry order -- the chosen one for a TRACKED entry, the start's for any other (whose T, R and t
+ *                       stay untouched).  With view following off, every entry's start template.  *n their number.
+ *                       LM_E_STATE when the run last finished was no track run or failed; LM_E_CAPACITY (with *n) when
+ *                       cap is smaller.
+ *   lm_track_views_points  k_track_views on caller arrays: one object at template k (T [16] f64) of one class of n
+ *                       templates, R_b [n][9] and t_b [n][3] f32, all with a render; *chosen = the template it keeps or
+ *                       switches to, T_out [16] its T.  LM_E_INVALID for a null argument, n < 1, k outside [0, n), a
+ *                       non-finite T or a turn_deg lm_set_track_views refuses. */
+int lm_set_track_views(lm_detector* d, int on, double turn_deg);
+int lm_track_templates(lm_detector* d, int32_t* template_id, int64_t cap, int64_t* n);
+int lm_track_views_points(int device, int64_t n, const float* R_b, const float* t_b, int64_t k, const double* T, double turn_deg,
+                          int64_t* chosen, double* T_out);
+
 /* Tracking a batch of depth frames in one call: several cameras, or several independent sequences at one time step (a
  * sequence's next frame starts from this one's results, so a batch never spans time).  Every frame's objects are slots
  * of one pose-stage run, so a few objects per frame no longer leave most of the GPU idle.
@@ -554,7 +599,7 @@ int lm_pose_transforms(lm_detector* d, double* T_out, int64_t cap, int64_t* n);
  *              computes -- its window, both clouds, its voxel sort segment, its ICP job and its verification -- depends
  *              only on its object and its own frame's depth and K, and the window cap 4 A only on the registered renders.
  *   Chunks     the run is cut into chunks of 1024 slots; a frame may straddle a chunk boundary.  Launches per chunk are a
- *              track chunk's (5 point-to-plane or 4, plus 1 when verifying), plus one conversion per frame for
+ *              track chunk's (5 point-to-plane or 4, plus 1 when verifying, plus 1 with view following), plus one conversion per frame for
  *              lm_track_batch_device.  lm_debug_pose_clouds then describes the last chunk (slot i is entry 1024 c + i of
  *              chunk c).
  * Refusals, before any device work, are lm_track's with its codes and messages, plus the frame (and the object's index
@@ -590,7 +635,8 @@ int lm_track_batch_device(lm_detector* d, int n_frames, const void* const* depth
  *              a shared batch chunk (6 launches per chunk point-to-plane, 5 point-to-point; a rank without an object in
  *              the chunk still publishes).  Each chunk is one pose exchange and takes the next number of the pose
  *              counter, so shared frames, lm_peer_detect_batch and lm_peer_track_batch interleave in any order.  Add 1
- *              launch per chunk when verifying, and one conversion per frame for lm_peer_track_batch_device.  A run
+ *              launch per chunk when verifying, 1 per chunk with view following (every rank re-chooses every object
+ *              of the chunk), and one conversion per frame for lm_peer_track_batch_device.  A run
  *              without objects launches nothing and exchanges nothing.
  * Refusals, before any device work: LM_E_STATE without a connected exchange, for LM_POSE_PSO and on a host-only handle;
  * otherwise every refusal of lm_track_batch / lm_track_batch_device with its code and "frame f: object k" message.
