@@ -11,6 +11,10 @@ The model restates what k_icp_normals and k_icp_point_to_plane compute, by brute
   normal_model            the smallest eigenvector of E[x x^T] - E[x] E[x]^T, summed in a given neighbour order
   corr_check              nearest target within the strict radius d^2 < 1e-4
   gn_step                 one Gauss-Newton step from given correspondences and normals
+and checks one pass of the ICP loop from any pose T_k the kernel had (T_{k+1} = U T_k):
+  check_plane_step        U against gn_step, relative to cond * eps * |x| plus the residuals' rounding (step_floor)
+  check_point_step        U against a float64 Umeyama of the pass's pairs, relative to kappa * eps plus the points' rounding
+  stop_pass               the pass the stop rule ends on, from the fitness and rmse of every pass
 The kernels' squared distances and sums may be FMA-contracted, so where a decision compares two of them the model
 accepts either answer inside a band of a few ulps (BAND).
 """
@@ -327,23 +331,159 @@ def corr_check(Ps, Q, corr, chunk=1024):
     return ok, d2
 
 
-def gn_step(Ps, Q, Nq, corr):
+def gn_step(Ps, Q, Nq, corr, full=False):
     """One Gauss-Newton step of point-to-plane ICP from given correspondences (float64).  Returns (x or None when J^T J
-    is exactly singular, cond(J^T J))."""
+    is exactly singular, cond(J^T J)), and with full=True also the step's rounding floor (step_floor) and whether J^T J
+    has an exactly zero row (no pair, or a column of J zero in every pair: singular in any elimination order)."""
     si = np.nonzero(corr >= 0)[0]
     vs, vt, nt = Ps[si], Q[corr[si]], Nq[corr[si]]
     r = ((vs - vt) * nt).sum(1)
     J = np.concatenate([np.cross(vs, nt), nt], 1)
     JTJ, JTr = J.T @ J, J.T @ r
+    zero_row = bool((JTJ == 0).all(1).any())
     try:
         x = np.linalg.solve(JTJ, -JTr)
     except np.linalg.LinAlgError:
-        return None, np.inf
-    return x, float(np.linalg.cond(JTJ))
+        return (None, np.inf, np.inf, zero_row) if full else (None, np.inf)
+    cond = float(np.linalg.cond(JTJ))
+    if not full:
+        return x, cond
+    return x, cond, step_floor(JTJ, J, vs, vt), zero_row
 
 
-def step_from_T(T1, init):
-    """The 6-vector x with T1 = TransformVector6dToMatrix4d(x) @ init, for init = [I | c]."""
-    U = T1[:3, :3]
-    t = T1[:3, 3] - U @ init[:3, 3]
+def step_floor(JTJ, J, vs, vt):
+    """||(J^T J)^-1||_2 * sum_i ||J_i|| * eps * (|p_i|_inf + |q_i|_inf): how far the rounding of the residuals
+    r_i = (p_i - q_i) . n_i alone moves the solution.  A step relative to |x| cannot bound a converged pass, where |x|
+    is down to the residuals' own rounding; this term does."""
+    inv = 1.0 / float(np.linalg.svd(JTJ, compute_uv=False)[-1])
+    mag = np.abs(vs).max(1) + np.abs(vt).max(1)
+    return inv * float((np.linalg.norm(J, axis=1) * EPS * mag).sum())
+
+
+def update_of(T1, T0):
+    """The update U with T1 = U @ T0, for rigid T0 (its rotation block transposed, not inverted)."""
+    U = np.eye(4)
+    U[:3, :3] = T1[:3, :3] @ T0[:3, :3].T
+    U[:3, 3] = T1[:3, 3] - U[:3, :3] @ T0[:3, 3]
+    return U
+
+
+def principal_angles(x):
+    """x with the angles step_from_T recovers from TransformVector6dToMatrix4d(x): x1 in [-pi/2, pi/2], x0 and x2 in
+    [-pi, pi].  A diverging step (an ill-conditioned J^T J) can leave that branch; (x0 + pi, pi - x1, x2 + pi) is the
+    same rotation.  x is returned unchanged, without rounding, when it is inside."""
+    a = np.array(x[:3], np.float64)
+    if np.all(np.abs(a) <= [np.pi, np.pi / 2, np.pi]):
+        return np.asarray(x, np.float64)
+    wrap = lambda v: (v + np.pi) % (2 * np.pi) - np.pi
+    a = wrap(a)
+    if abs(a[1]) > np.pi / 2:
+        a = wrap(np.array([a[0] + np.pi, np.pi - a[1], a[2] + np.pi]))
+    return np.concatenate([a, np.asarray(x[3:], np.float64)])
+
+
+def step_from_T(T1, T0):
+    """The 6-vector x with T1 = TransformVector6dToMatrix4d(x) @ T0, for any rigid T0 (for T0 = [I | c] the rotation
+    is T1's own, exactly)."""
+    U = update_of(T1, T0)
+    t = U[:3, 3]
     return np.array([np.arctan2(U[2, 1], U[2, 2]), np.arcsin(-U[2, 0]), np.arctan2(U[1, 0], U[0, 0]), t[0], t[1], t[2]])
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the update of pass k: T_{k+1} = U T_k from the pairs of pass k
+# ------------------------------------------------------------------------------------------------------------------
+STEP_COND_MAX = 1e10  # point-to-plane steps of a J^T J above this condition number are not compared
+STOP_TOL = 1e-6      # the stop rule's thresholds (ICPConvergenceCriteria's relative_fitness and relative_rmse)
+
+
+def proper_rotation(R, tol=1e-12):
+    return bool(np.all(np.isfinite(R)) and abs(np.linalg.det(R) - 1) <= tol and np.abs(R @ R.T - np.eye(3)).max() <= tol)
+
+
+def check_plane_step(key, src, tgt, normals, T0, T1, corr, K, floor=True):
+    """The point-to-plane update of one pass, T1 = U T0, against gn_step from the pass's pairs corr at T0.  Returns
+    (outcome, ratio, cond): "singular" (J^T J has an exactly zero row: T1 == T0 bit for bit), "cond" (singular to
+    rounding, or cond(J^T J) above STEP_COND_MAX: U need only be a proper rotation) or "compared", where
+        |x_kernel - x_model|_inf <= K (cond eps |x|_inf + floor) + recover
+    (floor: step_floor, or none with floor=False; recover: the rounding of step_from_T) and ratio is the error over the
+    bracket."""
+    x_m, cond, fl, zero_row = gn_step(transform(T0, src), tgt, normals, corr, full=True)
+    if zero_row:
+        assert np.array_equal(T1, T0), "step %s: singular J^T J must give the identity update" % key
+        return "singular", None, cond
+    U = update_of(T1, T0)
+    assert np.all(np.isfinite(U)) and proper_rotation(U[:3, :3]), "step %s: the update is not a proper rotation" % key
+    if x_m is None or cond > STEP_COND_MAX:  # singular to rounding only: the kernel's elimination may not see it
+        return "cond", None, cond
+    x_k, x_m = step_from_T(T1, T0), principal_angles(x_m)
+    err = float(np.abs(x_k - x_m).max())
+    scale = cond * EPS * float(np.abs(x_m).max()) + (fl if floor else 0.0)
+    recover = 16 * EPS * (1 + float(np.abs(T0).max()))
+    ratio = err / max(scale, 1e-300)
+    assert err <= K * scale + recover, "step %s: %r, model %r (cond %.3g, ratio %.3g)" % (key, x_k, x_m, cond, ratio)
+    return "compared", ratio, cond
+
+
+def umeyama_model(p, q):
+    """Two-pass float64 Umeyama: (R, t, singular values d, s = det U det V sign, pbar)."""
+    pb, qb = p.mean(0), q.mean(0)
+    sig = (q - qb).T @ (p - pb) / p.shape[0]
+    U, d, Vt = np.linalg.svd(sig)
+    s = -1.0 if np.linalg.det(U) * np.linalg.det(Vt) < 0 else 1.0
+    R = (U * [1.0, 1.0, s]) @ Vt
+    return R, qb - R @ pb, d, s, pb
+
+
+def p2p_cost(R, t, p, q):
+    return float(((p @ R.T + t - q) ** 2).sum())
+
+
+def check_point_step(key, src, tgt, T0, T1, corr, K, floor=True):
+    """The point-to-point update of one pass, T1 = U T0, against umeyama_model of the pass's pairs at T0.  Returns
+    (outcome, ratio, kappa): "empty" (no pair: T1 == T0 bit for bit), "degenerate" (one or two pairs, or collinear ones:
+    any proper rotation at the model's minimum cost; one pair keeps R exactly) or "compared", where with
+    kappa = d1 / (d2 + s d3) of the pairs' covariance
+        |R_kernel - R_model|_inf <= K (kappa eps + floor),   |t_kernel - t_model|_inf <= K (1 + |pbar|_inf)(kappa eps + floor)
+    floor = eps sum_i (|p_i - pbar| + |q_i - qbar|)(|p_i|_inf + |q_i|_inf) / (n (d2 + s d3)): the rounding of the points
+    themselves through the covariance (none with floor=False), and ratio is the larger error over its bracket."""
+    si = np.nonzero(corr >= 0)[0]
+    if si.size == 0:
+        assert np.array_equal(T1, T0), "step %s: no pair must give the identity update" % key
+        return "empty", None, None
+    p, q = transform(T0, src)[si], tgt[corr[si]]
+    upd = update_of(T1, T0)
+    Rk, tk = upd[:3, :3], upd[:3, 3]
+    assert np.all(np.isfinite(upd)), "step %s: %r" % (key, upd)
+    Rm, tm, d, s, pb = umeyama_model(p, q)
+    if si.size == 1:
+        assert np.array_equal(T1[:3, :3], T0[:3, :3]), "step %s: one pair must give R = I exactly" % key
+    gap = d[1] + s * d[2]
+    if si.size < 3 or not gap > 1e-9 * d[0]:
+        assert proper_rotation(Rk), "step %s: %r is not a proper rotation" % (key, Rk)
+        cm, ck = p2p_cost(Rm, tm, p, q), p2p_cost(Rk, tk, p, q)
+        scale = float(((p - p.mean(0)) ** 2).sum() + ((q - q.mean(0)) ** 2).sum())
+        assert ck <= cm + 1e-12 * scale + 1e-24, "step %s: cost %r, minimum %r" % (key, ck, cm)
+        return "degenerate", None, None
+    kappa = d[0] / gap
+    fl = 0.0
+    if floor:
+        spread = np.linalg.norm(p - pb, axis=1) + np.linalg.norm(q - q.mean(0), axis=1)
+        fl = EPS * float((spread * (np.abs(p).max(1) + np.abs(q).max(1))).sum()) / (p.shape[0] * gap)
+    bracket = kappa * EPS + fl
+    eR = float(np.abs(Rk - Rm).max()) / bracket
+    et = float(np.abs(tk - tm).max()) / ((1 + float(np.abs(pb).max())) * bracket)
+    assert eR <= K and et <= K, "step %s: R ratio %.3g, t ratio %.3g (kappa %.3g)" % (key, eR, et, kappa)
+    return "compared", max(eR, et), kappa
+
+
+def stop_pass(fits, rmses, max_iter):
+    """The pass RegistrationICP stops at, from the fitness and rmse of passes 0, 1, ...: the first k >= 1 with
+    |f_{k-1} - f_k| < 1e-6 and |r_{k-1} - r_k| < 1e-6 (strict, float64), capped at max_iter.  None when the passes
+    given end before either."""
+    for k in range(0, len(fits)):
+        if k >= 1 and abs(fits[k - 1] - fits[k]) < STOP_TOL and abs(rmses[k - 1] - rmses[k]) < STOP_TOL:
+            return k
+        if k >= max_iter:
+            return k
+    return None
