@@ -1918,6 +1918,7 @@ struct PoseNmsParams {
   PoseNmsOut* out;          // kept poses in keep order, frame f's from out + frame_first[f]
   // null: one frame, survivors [0, counts[0]).  Else frame f's survivors are [frame_first[f], frame_first[f + 1]).
   const int32_t* frame_first;
+  int32_t* src;             // per kept pose its survivor's index in the run (at out's index): its T is in outs
   // VERIFY only: per survivor its verification (k_pose_verify), per kept pose its copy (at out's index), and the
   // ranking and minimum score of lm_set_pose_verify
   const PoseVerify* ver;
@@ -1927,8 +1928,8 @@ struct PoseNmsParams {
 };
 
 // Behind the ICP kernel: candidates are the survivors with a pose, score -(double)residual.  One frame per CTA.
-// VERIFY (behind k_pose_verify): a survivor scoring below min_score is no candidate, rank_by may put the score first, and
-// every kept pose's verification goes to vout.
+// Every kept pose's survivor goes to src.  VERIFY (behind k_pose_verify): a survivor scoring below min_score is no
+// candidate, rank_by may put the score first, and every kept pose's verification goes to vout.
 template <bool VERIFY>
 __global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
   const int i = threadIdx.x;
@@ -1967,6 +1968,7 @@ __global__ void __launch_bounds__(NMS_THREADS) k_pose_nms(PoseNmsParams p) {
     o.m = surv[i];
     o.residual = res;
     p.out[first + rank] = o;
+    p.src[first + rank] = first + i;
   }
   if (i == 0) {
     PoseNmsHead h;
@@ -2089,6 +2091,47 @@ struct TplHost {
   std::vector<uint16_t> crop;
 };
 
+// What filled the finished-run record: a frame or batch without the pose NMS, one with it, a track run, an lm_icp call.
+enum class PoseRunKind { none, poses, kept, track, icp };
+
+// The run last finished: all that pose_stage_verify, pose_stage_transforms and pose_stage_track_templates read (lm_pose.h
+// gives their rules).  Each finish resets it before anything can fail, and fills it once the run has succeeded.
+struct PoseFinished {
+  PoseRunKind kind = PoseRunKind::none;
+  bool stale = false;             // a run has been prepared since: T, kept and tpl no longer answer; ver still does
+  bool verified = false;          // the run verified: ver holds its entries' verification
+  std::vector<PoseVerify> ver;
+  std::vector<double> T;          // poses, track: [entry][16], NaN for an entry without a pose
+  // kept: per frame, the index of its first kept pose in d_bksrc and d_bouts and its number of kept poses; the run's
+  // survivors and stream
+  std::vector<std::pair<int64_t, int64_t>> kept;
+  int64_t survivors = 0;
+  cudaStream_t stream = nullptr;
+  std::vector<int32_t> tpl;       // track: per entry its template within its class
+
+  void reset() {
+    kind = PoseRunKind::none;
+    stale = verified = false;
+    ver.clear(); T.clear(); kept.clear(); tpl.clear();
+    survivors = 0;
+    stream = nullptr;
+  }
+  // A run of kind k succeeded; v (verify: its n entries') is the verification.
+  void fill(PoseRunKind k, bool verify, const PoseVerify* v, int64_t n) {
+    kind = k;
+    stale = false;
+    verified = verify;
+    if (verify) ver.assign(v, v + n);
+  }
+  // n entries, none with a pose until compose() gives it one.
+  void entries(int64_t n) { T.assign(16 * (size_t)n, std::numeric_limits<double>::quiet_NaN()); }
+  // Entry i from ICP output o against the render made with R, t: its R, t and residual out (render_pose), its T here.
+  void compose(int64_t i, const IcpOut& o, const float* R, const float* t, double* R_out, double* t_out, float* residual) {
+    render_pose(o, R, t, R_out + 9 * i, t_out + 3 * i, residual + i);
+    memcpy(T.data() + 16 * i, o.T, sizeof(o.T));
+  }
+};
+
 struct lm_pose_stage {
   std::vector<TplHost> tpl;
   std::vector<int32_t> class_begin;
@@ -2111,13 +2154,15 @@ struct lm_pose_stage {
   // a batch's scene slots and survivors, filled by the caller (pose_batch_reserve), and a track run's scenes
   DeviceArray<uint16_t> d_bscene;
   DeviceArray<lm_match> d_bsurv;
-  // a run's outputs (pose_outputs), a frame's at offset 0: per survivor its frame, ICP output and posed flag
+  // a run's outputs (pose_outputs), a frame's at offset 0: per survivor its frame, ICP output and posed flag, and per
+  // kept pose of the pose NMS its survivor
   DeviceArray<int32_t> d_bframe;
   // only once a run verifies: per survivor its verification and per kept pose its copy, the host's copy of either
   // (h_bver last: survivors), and per chunk slot the ICP output a verifying shared stage publishes from
   DeviceArray<PoseVerify> d_bver, d_bvkept; PinnedArray<PoseVerify> h_bver;
   DeviceArray<IcpOut> d_souts;
-  DeviceArray<IcpOut> d_bouts; DeviceArray<uint8_t> d_bposed; PinnedArray<IcpOut> h_bouts;  // h_bouts last: survivors
+  DeviceArray<IcpOut> d_bouts; DeviceArray<uint8_t> d_bposed; DeviceArray<int32_t> d_bksrc;
+  PinnedArray<IcpOut> h_bouts;  // h_bouts last: survivors
   // per frame its first survivor and intrinsics, per chunk (at most one per frame) a status block (PoseChunk; [3] a
   // batch chunk's size)
   DeviceArray<int32_t> d_bfirst; DeviceArray<float> d_bsK;  // [frames + 1], [frames][9]
@@ -2130,9 +2175,7 @@ struct lm_pose_stage {
   PoseShare share = {};
   std::vector<int64_t> first;
   int64_t launches = 0, fetched = 0;
-  // the verification of the entries of the run last finished (pose_stage_verify); verified false: it did not verify
-  bool verified = false;
-  std::vector<PoseVerify> ver;
+  PoseFinished done;
   // the last chunk pose_chunk enqueued (pose_stage_clouds): its slots, rank and world, its first survivor in the run and
   // its posed flags per slot.  valid false before the first chunk and from the next pose_prepare on, which may move the
   // buffers.
@@ -2146,15 +2189,6 @@ struct lm_pose_stage {
   // tracking (pose_stage_track; its scenes are in d_bscene): the objects of the run and their windows
   DeviceArray<TrackObject> d_tobj;
   DeviceArray<TrackRec> d_trec; PinnedArray<TrackRec> h_trec;
-  // the run last finished, for pose_stage_transforms: finished_ok false once another run is prepared or it failed; its
-  // entries' transformations, or (xf_pending, a run with the pose NMS) its frames' first survivors to find them from
-  bool finished_ok = false, xf_pending = false;
-  std::vector<double> xf;
-  // a finished track run's template per entry within its class (pose_stage_track_templates); tracked false: the run
-  // last finished was no track run
-  bool tracked = false;
-  std::vector<int32_t> track_tpl;
-  std::vector<int64_t> finished_first;
 };
 
 // The per-chunk buffers: slots of 2 clouds of pose_area() points for each of pose_slots() survivors.  d_sort_tmp is
@@ -2531,10 +2565,11 @@ static int pose_outputs(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t
     CUI(s->h_bstat.assign(4 * (size_t)n_frames));
   }
   if (surv) {
-    s->d_bframe.reset(); s->d_bouts.reset(); s->d_bposed.reset(); s->h_bouts.reset();
+    s->d_bframe.reset(); s->d_bouts.reset(); s->d_bposed.reset(); s->d_bksrc.reset(); s->h_bouts.reset();
     CUI(s->d_bframe.assign(S));
     CUI(s->d_bouts.assign(S));
     CUI(s->d_bposed.assign(S));
+    CUI(s->d_bksrc.assign(S));
     CUI(s->h_bouts.assign(S));
   }
   if (block) {
@@ -2549,7 +2584,7 @@ static int pose_outputs(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t
 // too).
 static int pose_prepare(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t S, bool verify) {
   s->last.valid = false;
-  s->finished_ok = false;
+  s->done.stale = true;
   if (s->dirty) {
     int rc = pose_upload(s, st);
     if (rc) return rc;
@@ -2590,6 +2625,25 @@ int pose_batch_reserve(lm_pose_stage* s, cudaStream_t st, int n_frames, int64_t 
   return LM_OK;
 }
 
+// Entries of chunk c of a run of S entries.
+static int chunk_size(int64_t S, int c) { return (int)std::min<int64_t>(S - (int64_t)c * POSE_CHUNK, POSE_CHUNK); }
+
+// The tables a batch or track run's chunks read, on st: each entry's frame (entries of frame f: [first[f], first[f + 1])),
+// each frame's intrinsics (sK + 9f), and each chunk's status block with its size in word 3.
+static int run_tables(lm_pose_stage* s, cudaStream_t st, int nf, const int64_t* first, const float* sK) {
+  const int64_t S = first[nf];
+  const int nc = pose_batch_chunks(S);
+  std::vector<int32_t> frame_of((size_t)S);
+  for (int f = 0; f < nf; ++f)
+    for (int64_t k = first[f]; k < first[f + 1]; ++k) frame_of[(size_t)k] = f;
+  std::vector<int32_t> stat((size_t)4 * nc, 0);
+  for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = chunk_size(S, c);
+  if (S) CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
+  CUI(cudaMemcpyAsync(s->d_bsK.get(), sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
+  if (nc) CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  return LM_OK;
+}
+
 int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) {
   const PoseOptions& o = run.o;
   cudaStream_t st = o.stream;
@@ -2602,17 +2656,11 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
     return lm_fail(LM_E_STATE, "the pose stage shared over the ranks does not run LM_POSE_PSO: turn lm_peer_share_pose off");
   int rc = pose_prepare(s, st, nf, S, o.verify.on != 0);
   if (rc) return rc;
-  if (batch) {  // each survivor's frame, each frame's first survivor and intrinsics, each chunk's status block and size
-    std::vector<int32_t> frame_of((size_t)S);
-    for (int f = 0; f < nf; ++f)
-      for (int64_t k = run.first[f]; k < run.first[f + 1]; ++k) frame_of[(size_t)k] = f;
-    std::vector<int32_t> first32(run.first, run.first + nf + 1);
-    std::vector<int32_t> stat((size_t)4 * nc, 0);
-    for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(S - (int64_t)c * POSE_CHUNK, POSE_CHUNK);
-    if (S) CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * S, cudaMemcpyHostToDevice, st));
+  if (batch) {
+    rc = run_tables(s, st, nf, run.first, run.sK);
+    if (rc) return rc;
+    std::vector<int32_t> first32(run.first, run.first + nf + 1);  // each frame's first survivor (k_pose_nms, k_pose_pso)
     CUI(cudaMemcpyAsync(s->d_bfirst.get(), first32.data(), sizeof(int32_t) * (nf + 1), cudaMemcpyHostToDevice, st));
-    CUI(cudaMemcpyAsync(s->d_bsK.get(), run.sK, sizeof(float) * 9 * nf, cudaMemcpyHostToDevice, st));
-    if (nc) CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
   } else {  // a frame's survivor count is the box NMS's
     CUI(cudaMemsetAsync(s->d_bstat.get(), 0, sizeof(int32_t) * 4, st));
   }
@@ -2620,7 +2668,7 @@ int pose_stage_enqueue(lm_pose_stage* s, const PoseRun& run, int64_t* launches) 
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_CHUNK;
     PoseChunk k = run_chunk(s, o, c, run.d_surv, batch ? s->d_bstat.get() + 4 * c + 3 : run.d_counts,
-                            batch ? (int)std::min<int64_t>(S - c0, POSE_CHUNK) : run.bound, run.d_scene, batch ? nullptr : run.sK);
+                            batch ? chunk_size(S, c) : run.bound, run.d_scene, batch ? nullptr : run.sK);
     if (batch) { k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get(); k.frame_first = s->d_bfirst.get(); }
     const int l = pose_chunk(s, o, k);
     if (l < 0) return l;
@@ -2652,7 +2700,7 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches) {
   p.surv = r.d_surv; p.counts = batch ? nullptr : r.d_counts; p.posed = s->d_bposed.get(); p.outs = s->d_bouts.get();
   p.rt = s->d_rt.get(); p.class_begin = s->d_class_begin.get();
   p.thr = thr;
-  p.head = nms_heads(s->d_bnms.get()); p.out = nms_out(s->d_bnms.get(), nf);
+  p.head = nms_heads(s->d_bnms.get()); p.out = nms_out(s->d_bnms.get(), nf); p.src = s->d_bksrc.get();
   p.frame_first = batch ? s->d_bfirst.get() : nullptr;
   const PoseVerifyOptions& v = r.o.verify;
   p.ver = s->d_bver.get(); p.vout = s->d_bvkept.get(); p.rank_by = v.rank_by; p.min_score = v.min_score;
@@ -2668,28 +2716,34 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches) {
   return LM_OK;
 }
 
-// After the stream has been synchronised: the error of nb status blocks of 4 int32 (PoseChunk), block c that of pose
-// exchange seq + c when shared; a batch's message names the chunk.  *published: the entries summed.
-static int pose_status(const int32_t* h, int nb, bool shared, int32_t seq, unsigned long long timeout_ns, bool batch,
-                       int64_t* published) {
+// After the stream has been synchronised: the error of a run of n entries from its nb status blocks of 4 int32
+// (PoseChunk), block c that of pose exchange sh->seq + c when shared (sh); a batch's message names the chunk.  Once they
+// are clean, stats4 (may be null) gets what lm_pose_stats returns: n, the entries this rank published (unshared: n),
+// the run's launches and 1 when shared.
+static int pose_status(const int32_t* h, int nb, const PoseShare* sh, bool batch, int64_t n, int64_t launches, int64_t* stats4) {
   int32_t overflow = 0;
-  int64_t sum = 0;
+  int64_t published = 0;
   for (int c = 0; c < nb; ++c) {
     const int32_t* b = h + 4 * c;
-    if (shared && b[1]) {
+    if (sh && b[1]) {
       if (batch)
         return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d (chunk %d of the batch) within %llu ms "
                        "(or an earlier collector on this device already gave up); every rank must run every batch while sharing is on",
-                       seq + c, c, timeout_ns / 1000000ull);
+                       sh->seq + c, c, sh->timeout_ns / 1000000ull);
       return lm_fail(LM_E_STATE, "pose exchange: a rank did not publish its poses of exchange %d within %llu ms (or an earlier collector "
                      "on this device already gave up); every rank must run the pose stage of every frame while sharing is on",
-                     seq + c, timeout_ns / 1000000ull);
+                     sh->seq + c, sh->timeout_ns / 1000000ull);
     }
     overflow |= b[0];
-    if (shared) sum += b[2];
+    if (sh) published += b[2];
   }
   if (overflow) return lm_fail(LM_E_INVALID, "pose stage: a cloud spans more than 2^%d voxels of 2.5 mm along an axis", POSE_KEY_BITS);
-  *published = sum;
+  if (stats4) {
+    stats4[0] = n;
+    stats4[1] = sh ? published : n;
+    stats4[2] = launches;
+    stats4[3] = sh ? 1 : 0;
+  }
   return LM_OK;
 }
 
@@ -2703,14 +2757,6 @@ static const TplHost* survivor_render(const lm_pose_stage* s, const lm_match& m)
 // LL.cpp:52-55: the reference returns early where the render's box, placed at the match, leaves the frame.
 static bool survivor_fits(const TplHost& h, const lm_match& m, int srows, int scols) {
   return !(m.x + h.box[2] >= scols || m.y + h.box[3] >= srows);
-}
-
-// The start of every finish: the run last finished is forgotten, its verification and transformations with it.
-static void pose_forget(lm_pose_stage* s) {
-  s->verified = s->finished_ok = s->xf_pending = s->tracked = false;
-  s->ver.clear();
-  s->xf.clear();
-  s->track_tpl.clear();
 }
 
 // n kept poses e[] into the caller's arrays (out may be null).
@@ -2734,17 +2780,10 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
   const int64_t S = first[nf];
   if (!batch && n > r.bound) return lm_fail(LM_E_STATE, "%lld survivors for a pose stage launched for %d", (long long)n, r.bound);
   const bool verify = r.o.verify.on != 0;
-  pose_forget(s);
-  int64_t published = 0;
-  int rc = pose_status(s->h_bstat.get(), batch ? pose_batch_chunks(S) : 1, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0,
-                       batch, &published);
+  PoseFinished& d = s->done;
+  d.reset();
+  int rc = pose_status(s->h_bstat.get(), batch ? pose_batch_chunks(S) : 1, sh, batch, S, s->launches, stats4);
   if (rc) return rc;
-  if (stats4) {
-    stats4[0] = S;
-    stats4[1] = sh ? published : S;
-    stats4[2] = s->launches;
-    stats4[3] = sh ? 1 : 0;
-  }
   const PoseNmsHead* heads = nms_heads(s->h_bnms.get());
   PoseNmsOut* entries = nms_out(s->h_bnms.get(), nf);
   int64_t total = 0, end = 0;  // entries, and the end of the host copy they need
@@ -2784,29 +2823,27 @@ int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_matc
                           cudaMemcpyDeviceToHost, st));
     CUI(cudaStreamSynchronize(st));
   }
-  if (r.pose_nms) {
+  if (r.pose_nms) {  // the kept poses' transformations stay on the device until pose_stage_transforms
+    d.fill(PoseRunKind::kept, verify, s->h_bver.get(), 0);
+    d.survivors = S;
+    d.stream = r.o.stream;
     int64_t at = 0;
     for (int f = 0; f < nf; ++f) {
       copy_kept(entries + first[f], counts[4 * f], out ? out + at : nullptr, R_out + 9 * at, t_out + 3 * at, residual + at);
-      if (verify) s->ver.insert(s->ver.end(), s->h_bver.get() + first[f], s->h_bver.get() + first[f] + counts[4 * f]);
+      if (verify) d.ver.insert(d.ver.end(), s->h_bver.get() + first[f], s->h_bver.get() + first[f] + counts[4 * f]);
+      d.kept.emplace_back(first[f], counts[4 * f]);
       at += counts[4 * f];
     }
-    s->verified = verify;
-    s->finished_first.assign(first, first + nf + 1);
-    s->finished_ok = s->xf_pending = true;
     return LM_OK;
   }
-  s->xf.assign(16 * (size_t)S, std::numeric_limits<double>::quiet_NaN());
+  d.fill(PoseRunKind::poses, verify, s->h_bver.get(), S);
+  d.entries(S);
   for (int64_t i = 0; i < S; ++i) {  // every survivor, frame after frame; R / t untouched where the reference returns early
     if (out) out[i] = surv[i];
     const TplHost& h = *survivor_render(s, surv[i]);
     if (!survivor_fits(h, surv[i], r.o.srows, r.o.scols)) { residual[i] = -1.f; continue; }
-    render_pose(s->h_bouts[i], h.R, h.t, R_out + 9 * i, t_out + 3 * i, residual + i);
-    memcpy(s->xf.data() + 16 * i, s->h_bouts[i].T, sizeof(s->h_bouts[i].T));
+    d.compose(i, s->h_bouts[i], h.R, h.t, R_out, t_out, residual);
   }
-  if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + S);
-  s->verified = verify;
-  s->finished_ok = true;
   return LM_OK;
 }
 
@@ -2823,8 +2860,8 @@ static int copy_verify(const PoseVerify* v, int64_t count, float* score, int32_t
 }
 
 int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, int64_t cap, int64_t* n) {
-  if (!s || !s->verified) return lm_fail(LM_E_STATE, "the last completed pose stage did not verify (lm_set_pose_verify, lm_icp_set_verify)");
-  return copy_verify(s->ver.data(), (int64_t)s->ver.size(), score, counts6, cap, n);
+  if (!s || !s->done.verified) return lm_fail(LM_E_STATE, "the last completed pose stage did not verify (lm_set_pose_verify, lm_icp_set_verify)");
+  return copy_verify(s->done.ver.data(), (int64_t)s->done.ver.size(), score, counts6, cap, n);
 }
 
 extern "C" int lm_pose_verify_points(int device, const double* pts, int64_t n, const double* T, const uint16_t* scene, int rows,
@@ -3157,8 +3194,8 @@ static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
 // A call without hypotheses: no device work; it verified nothing (an empty verification) and captured nothing.
 static int icp_no_hypotheses(lm_icp* h) {
-  pose_forget(&h->dev->stage);
-  h->dev->stage.verified = h->verify;
+  h->dev->stage.done.reset();
+  h->dev->stage.done.fill(PoseRunKind::icp, h->verify, nullptr, 0);
   h->cap.job_of.clear();
   return LM_OK;
 }
@@ -3172,7 +3209,7 @@ static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pi
                      int max_iterations, double* R_out, double* t_out, float* residual) {
   IcpDevice& d = *h->dev;
   lm_pose_stage* s = &d.stage;
-  pose_forget(s);
+  s->done.reset();
   h->cap.job_of.clear();  // a call that fails keeps no capture
   cudaStream_t st = h->stream.get();
   IcpCapture cap;  // kept only when the call succeeds
@@ -3227,11 +3264,9 @@ static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pi
   }
   if (last < 0) {  // every hypothesis takes the early return: no cloud to build, and every verification scores -1
     for (int i = 0; i < n; ++i) residual[i] = -1.f;
-    if (h->verify) {
-      s->ver.assign((size_t)n, PoseVerify());
-      for (PoseVerify& v : s->ver) v.score = -1.f;
-      s->verified = true;
-    }
+    std::vector<PoseVerify> none(h->verify ? (size_t)n : 0, PoseVerify());
+    for (PoseVerify& v : none) v.score = -1.f;
+    s->done.fill(PoseRunKind::icp, h->verify, none.data(), n);
     if (h->capture) h->cap = std::move(cap);
     return LM_OK;
   }
@@ -3284,15 +3319,13 @@ static int icp_batch(lm_icp* h, int n, const void* scene_depth, int64_t scene_pi
   float ms = 0;
   CUI(cudaEventElapsedTime(&ms, h->ev0.get(), h->ev1.get()));
   h->last_kernel_us = ms * 1000.f;
-  int64_t published = 0;
-  rc = pose_status(s->h_bstat.get(), nc, false, 0, 0, false, &published);
+  rc = pose_status(s->h_bstat.get(), nc, nullptr, false, n, 0, nullptr);
   if (rc) return rc;
+  s->done.fill(PoseRunKind::icp, h->verify, s->h_bver.get(), n);
   for (int i = 0; i < n; ++i) {
     if (posed[(size_t)i]) render_pose(s->h_bouts[(size_t)i], R + 9 * i, t + 3 * i, R_out + 9 * i, t_out + 3 * i, residual + i);
     else residual[i] = -1.f;
   }
-  if (h->verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + n);
-  s->verified = h->verify;
   if (h->capture) {
     for (int i = 0; i < n; ++i)
       if (cap.job_of[(size_t)i] >= 0) cap.outs.push_back(s->h_bouts[(size_t)i]);
@@ -3410,7 +3443,8 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
   const bool verify = o.verify.on != 0;
   const int64_t n = first[n_frames];
   const int nc = pose_batch_chunks(n);
-  pose_forget(s);
+  PoseFinished& d = s->done;
+  d.reset();
   // Every buffer of the run before its first chunk: once chunks run, no device memory is allocated or freed (a free
   // waits for the whole device, a spinning peer collector of a shared run included).  The cloud buffers come before
   // pose_prepare, which sizes the slot outputs a verifying shared chunk publishes from by them.
@@ -3419,14 +3453,9 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
   int rc = n ? pose_buffers(s, st, (int)((slots * stride + 2 * M - 1) / (2 * M)), M) : LM_OK;
   if (!rc) rc = pose_prepare(s, st, n_frames, n, verify);
   if (rc) return rc;
-  if (n == 0) {
-    if (stats4) {
-      stats4[0] = stats4[1] = stats4[2] = 0;
-      stats4[3] = sh ? 1 : 0;
-    }
-    s->verified = verify;
-    s->finished_ok = s->tracked = true;
-    return LM_OK;
+  if (n == 0) {  // no chunk, so no status block to check
+    d.fill(PoseRunKind::track, verify, nullptr, 0);
+    return pose_status(s->h_bstat.get(), 0, sh, false, 0, 0, stats4);
   }
   if ((size_t)n > s->h_trec.size()) {
     CUI(cudaStreamSynchronize(st));
@@ -3435,26 +3464,20 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
     CUI(s->d_trec.assign(n));
     CUI(s->h_trec.assign(n));
   }
-  // each object's frame and each frame's intrinsics, which k_track_cloud and k_pose_verify read, and each chunk's
-  // status block with its object count in word 3, which k_track_cloud and a shared chunk's publishers read
-  std::vector<int32_t> frame_of((size_t)n);
-  for (int f = 0; f < n_frames; ++f)
-    for (int64_t k = first[f]; k < first[f + 1]; ++k) frame_of[(size_t)k] = f;
-  std::vector<int32_t> stat((size_t)4 * nc, 0);
-  for (int c = 0; c < nc; ++c) stat[(size_t)4 * c + 3] = (int32_t)std::min<int64_t>(n - (int64_t)c * POSE_CHUNK, POSE_CHUNK);
+  // the objects, and the tables that k_track_cloud, k_pose_verify and a shared chunk's publishers read
   CUI(cudaMemcpyAsync(s->d_tobj.get(), obj, sizeof(TrackObject) * n, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bframe.get(), frame_of.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bsK.get(), sK, sizeof(float) * 9 * n_frames, cudaMemcpyHostToDevice, st));
-  CUI(cudaMemcpyAsync(s->d_bstat.get(), stat.data(), sizeof(int32_t) * stat.size(), cudaMemcpyHostToDevice, st));
+  rc = run_tables(s, st, n_frames, first, sK);
+  if (rc) return rc;
   int64_t stage_launches = 0;
   for (int c = 0; c < nc; ++c) {
     const int64_t c0 = (int64_t)c * POSE_CHUNK;
+    const int m = chunk_size(n, c);
     if (o.views) {  // every rank re-chooses every object of the chunk, so all ranks hold the same objects
       TrackViewParams v;
       v.obj = s->d_tobj.get() + c0; v.counts = s->d_bstat.get() + 4 * c + 3;
       v.rt = s->d_rt.get(); v.has = s->d_has.get(); v.class_begin = s->d_class_begin.get();
       v.n_classes = (int32_t)s->class_begin.size() - 1; v.tau = o.view_tau;
-      k_track_views<<<stat[(size_t)4 * c + 3], VIEW_THREADS, 0, st>>>(v);
+      k_track_views<<<m, VIEW_THREADS, 0, st>>>(v);
       ++stage_launches;
       ++*launches;
     }
@@ -3463,7 +3486,7 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
     q.obj = s->d_tobj.get() + c0; q.tpl = s->d_tpl.get(); q.crops = s->d_crops.get();
     q.margin = margin; q.cap = W; q.stride = stride; q.M = M;
     q.rec = s->d_trec.get() + c0;
-    PoseChunk k = run_chunk(s, o, c, nullptr, s->d_bstat.get() + 4 * c + 3, stat[(size_t)4 * c + 3], d_scene, nullptr);
+    PoseChunk k = run_chunk(s, o, c, nullptr, s->d_bstat.get() + 4 * c + 3, m, d_scene, nullptr);
     k.frame_of = s->d_bframe.get() + c0; k.sKs = s->d_bsK.get();
     k.track = &q;
     const int l = pose_chunk(s, o, k);
@@ -3482,17 +3505,11 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
   }
   CUI(cudaStreamSynchronize(st));
   CUI(cudaGetLastError());
-  int64_t published = 0;
-  rc = pose_status(s->h_bstat.get(), nc, sh != nullptr, sh ? sh->seq : 0, sh ? sh->timeout_ns : 0, nc > 1, &published);
+  rc = pose_status(s->h_bstat.get(), nc, sh, nc > 1, n, stage_launches, stats4);
   if (rc) return rc;
-  if (stats4) {
-    stats4[0] = n;
-    stats4[1] = sh ? published : n;
-    stats4[2] = stage_launches;
-    stats4[3] = sh ? 1 : 0;
-  }
-  s->xf.assign(16 * (size_t)n, std::numeric_limits<double>::quiet_NaN());
-  s->track_tpl.resize((size_t)n);
+  d.fill(PoseRunKind::track, verify, s->h_bver.get(), n);
+  d.entries(n);
+  d.tpl.resize((size_t)n);
   for (int64_t i = 0; i < n; ++i) {
     const TrackRec& e = s->h_trec[(size_t)i];
     status[i] = e.status;
@@ -3500,68 +3517,45 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
     // an entry not tracked keeps its start, template included
     const int64_t g = e.status == LM_TRACK_TRACKED && o.views ? chosen[(size_t)i].g : obj[i].g;
     const int64_t cls = std::upper_bound(s->class_begin.begin(), s->class_begin.end(), (int32_t)obj[i].g) - s->class_begin.begin() - 1;
-    s->track_tpl[(size_t)i] = (int32_t)(g - s->class_begin[(size_t)cls]);
+    d.tpl[(size_t)i] = (int32_t)(g - s->class_begin[(size_t)cls]);
     if (e.status != LM_TRACK_TRACKED) { residual[i] = -1.f; continue; }
     const IcpOut& q = s->h_bouts[(size_t)i];
     const TplHost& h = s->tpl[(size_t)g];
-    render_pose(q, h.R, h.t, R_out + 9 * i, t_out + 3 * i, residual + i);
+    d.compose(i, q, h.R, h.t, R_out, t_out, residual);
     memcpy(T_out + 16 * i, q.T, sizeof(q.T));
-    memcpy(s->xf.data() + 16 * i, q.T, sizeof(q.T));
   }
-  if (verify) s->ver.assign(s->h_bver.get(), s->h_bver.get() + n);
-  s->verified = verify;
-  s->finished_ok = s->tracked = true;
   return LM_OK;
 }
 
 int pose_stage_track_templates(const lm_pose_stage* s, int32_t* template_id, int64_t cap, int64_t* n) {
   if (!n || (cap > 0 && !template_id)) return lm_fail(LM_E_INVALID, "null argument");
-  if (!s || !s->finished_ok || !s->tracked)
+  if (!s || s->done.kind != PoseRunKind::track || s->done.stale)
     return lm_fail(LM_E_STATE, "the pose run last finished was no track run (lm_track, lm_track_batch, lm_peer_track_batch), or it failed");
-  *n = (int64_t)s->track_tpl.size();
+  const std::vector<int32_t>& tpl = s->done.tpl;
+  *n = (int64_t)tpl.size();
   if (*n > cap) return lm_fail(LM_E_CAPACITY, "%lld entries, capacity %lld", (long long)*n, (long long)cap);
-  if (*n) memcpy(template_id, s->track_tpl.data(), sizeof(int32_t) * (size_t)*n);
+  if (*n) memcpy(template_id, tpl.data(), sizeof(int32_t) * (size_t)*n);
   return LM_OK;
 }
 
-int pose_stage_transforms(lm_pose_stage* s, double* T_out, int64_t cap, int64_t* n) {
+int pose_stage_transforms(const lm_pose_stage* s, double* T_out, int64_t cap, int64_t* n) {
   if (!n || (cap > 0 && !T_out)) return lm_fail(LM_E_INVALID, "null argument");
-  if (!s->finished_ok) return lm_fail(LM_E_STATE, "no pose run has finished since the last one was enqueued (or it failed)");
-  if (s->xf_pending) {  // the pose NMS's kept entries: matched to their survivors by their composed pose
-    const PoseRun& r = s->run;
-    const std::vector<int64_t>& first = s->finished_first;
-    s->xf.clear();
-    const int nf = (int)first.size() - 1;
-    const int64_t S = first[(size_t)nf];
-    cudaStream_t st = r.o.stream;
-    std::vector<IcpOut> outs((size_t)S);
-    std::vector<uint8_t> posed((size_t)S);
-    if (S) {
-      CUI(cudaMemcpyAsync(outs.data(), s->d_bouts.get(), sizeof(IcpOut) * S, cudaMemcpyDeviceToHost, st));
-      CUI(cudaMemcpyAsync(posed.data(), s->d_bposed.get(), S, cudaMemcpyDeviceToHost, st));
-      CUI(cudaStreamSynchronize(st));
-    }
-    const PoseNmsHead* heads = nms_heads(s->h_bnms.get());
-    const PoseNmsOut* entries = nms_out(s->h_bnms.get(), nf);
-    for (int f = 0; f < nf; ++f)
-      for (int64_t k = 0; k < heads[f].kept; ++k) {
-        const PoseNmsOut& e = entries[first[(size_t)f] + k];
-        const TplHost* h = survivor_render(s, e.m);
-        int64_t got = -1;
-        for (int64_t i = first[(size_t)f]; h && got < 0 && i < first[(size_t)f + 1]; ++i) {
-          if (!posed[(size_t)i]) continue;
-          double R[9], t[3];
-          float res;
-          render_pose(outs[(size_t)i], h->R, h->t, R, t, &res);
-          if (res == e.residual && !memcmp(R, e.R, sizeof(R)) && !memcmp(t, e.t, sizeof(t))) got = i;
-        }
-        if (got < 0) return lm_fail(LM_E_STATE, "frame %d, kept pose %lld: no survivor composes to it", f, (long long)k);
-        s->xf.insert(s->xf.end(), outs[(size_t)got].T, outs[(size_t)got].T + 16);
-      }
-    s->xf_pending = false;
-  }
-  *n = (int64_t)s->xf.size() / 16;
+  const PoseFinished& d = s->done;
+  const bool poses = d.kind == PoseRunKind::poses || d.kind == PoseRunKind::kept || d.kind == PoseRunKind::track;
+  if (!poses || d.stale) return lm_fail(LM_E_STATE, "no pose run has finished since the last one was enqueued (or it failed)");
+  *n = (int64_t)d.T.size() / 16;
+  for (const auto& k : d.kept) *n += k.second;
   if (*n > cap) return lm_fail(LM_E_CAPACITY, "%lld entries, capacity %lld", (long long)*n, (long long)cap);
-  if (*n) memcpy(T_out, s->xf.data(), sizeof(double) * s->xf.size());
+  if (!d.T.empty()) memcpy(T_out, d.T.data(), sizeof(double) * d.T.size());
+  if (d.kept.empty() || !*n) return LM_OK;
+  // the pose NMS's kept poses: each names its survivor, whose ICP output holds its T.  Only a later run, which makes d
+  // stale, writes d_bksrc and d_bouts again.
+  std::vector<int32_t> src((size_t)d.survivors);
+  std::vector<IcpOut> outs((size_t)d.survivors);
+  CUI(cudaMemcpyAsync(src.data(), s->d_bksrc.get(), sizeof(int32_t) * src.size(), cudaMemcpyDeviceToHost, d.stream));
+  CUI(cudaMemcpyAsync(outs.data(), s->d_bouts.get(), sizeof(IcpOut) * outs.size(), cudaMemcpyDeviceToHost, d.stream));
+  CUI(cudaStreamSynchronize(d.stream));
+  for (const auto& k : d.kept)
+    for (int64_t j = 0; j < k.second; ++j, T_out += 16) memcpy(T_out, outs[(size_t)src[(size_t)(k.first + j)]].T, sizeof(double) * 16);
   return LM_OK;
 }

@@ -117,8 +117,28 @@ int pose_stage_enqueue_nms(lm_pose_stage* s, double thr, int64_t* launches);
 int pose_stage_finish(lm_pose_stage* s, const lm_match* surv, int64_t n, lm_match* out, double* R_out, double* t_out, float* residual,
                       int64_t cap, int64_t* n_out, int64_t* counts, int64_t* stats4);
 
-// The verification of the entries of the run last finished, in their order (lm_pose_verify): LM_E_STATE when it did not
-// verify, LM_E_CAPACITY (with *n) beyond cap.
+// The run last finished.  The stage keeps one record of it, which three getters read:
+//   pose_stage_verify (lm_pose_verify, lm_icp_verify): its entries' verification, in entry order.
+//   pose_stage_transforms (lm_pose_transforms): its entries' transformations, T_out + 16k, NaN for an entry without a pose.
+//   pose_stage_track_templates (lm_track_templates): its entries' templates within their class.
+// What each returns, by what last happened on the stage:
+//   - a frame or batch without the pose NMS (pose_stage_finish): verify, every survivor's when the run verified, else
+//     LM_E_STATE; transforms, every survivor's (NaN where the reference returns early); templates, LM_E_STATE.
+//   - a frame or batch with the pose NMS: the same for the kept poses, frame after frame in keep order.  k_pose_nms
+//     stores each kept pose's survivor on the device; transforms copies the survivors' ICP outputs on the run's stream.
+//   - a track run (pose_stage_track, 0 objects included): verify as above; transforms, every object's (NaN for an entry
+//     not TRACKED); templates, every object's (see pose_stage_track_templates).
+//   - an lm_icp call, on the ICP handle's own stage (n hypotheses; none: n = 0): verify, when lm_icp_set_verify is on,
+//     every hypothesis's (score -1 and zero counts where it returns early), else LM_E_STATE.  Nothing reads its other
+//     entries.
+//   - a run whose finish failed: LM_E_STATE from all three.  A finish resets the record before it checks the run's
+//     status blocks, so every failure past that point (a cloud overflow, a peer that did not publish, a survivor
+//     without a render, LM_E_CAPACITY for too small outputs, a CUDA error) leaves it empty.  pose_stage_finish's check of
+//     the survivor count against the launch comes before the reset, and a call that fails before it reaches the stage
+//     leaves the record as it was.
+//   - a run enqueued (pose_stage_enqueue, pose_batch_reserve) and not yet finished: verify still returns the last
+//     finished run's verification; transforms and templates return LM_E_STATE.
+// LM_E_CAPACITY (with *n) beyond cap.
 int pose_stage_verify(const lm_pose_stage* s, float* score, int32_t* counts6, int64_t cap, int64_t* n);
 
 // Slot `slot`'s item `what` of the last chunk enqueued (lm_debug_pose_clouds), after the caller has synchronised the
@@ -151,14 +171,10 @@ int pose_stage_track(lm_pose_stage* s, const PoseOptions& o, int n_frames, const
 // LM_E_INVALID unless turn_deg lies in [0, 180) (on only); else *tau = 1 + 2 cos(turn_deg) (libm cos), 0 when off.
 int track_view_tau(int on, double turn_deg, double* tau);
 // The template of every entry of the run last finished (lm_track_templates), within its class, in entry order: the one
-// view following chose for a TRACKED entry, the start's for any other.  LM_E_STATE unless that run was a track run that
-// succeeded; LM_E_CAPACITY (with *n) beyond cap.
+// view following chose for a TRACKED entry, the start's for any other.  When it answers: pose_stage_verify.
 int pose_stage_track_templates(const lm_pose_stage* s, int32_t* template_id, int64_t cap, int64_t* n);
-// The transformation of every entry of the run last finished (lm_pose_transforms), in entry order, T_out + 16k; NaN for an
-// entry without a pose.  LM_E_STATE once another run has been enqueued or the last one failed; LM_E_CAPACITY (with *n)
-// beyond cap.  The pose NMS's kept entries are matched to their survivors on the host, from one copy of the run's ICP
-// outputs and survivors.
-int pose_stage_transforms(lm_pose_stage* s, double* T_out, int64_t cap, int64_t* n);
+// The transformation of every entry of the run last finished (lm_pose_transforms).  When it answers: pose_stage_verify.
+int pose_stage_transforms(const lm_pose_stage* s, double* T_out, int64_t cap, int64_t* n);
 
 // A batch's scene and survivor slots: room for n_frames scene depths of frame_pixels each (frame f at d_scene + f *
 // frame_pixels) and max_surv survivors, which the caller fills on the stream.  It also uploads the renders and grows

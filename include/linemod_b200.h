@@ -522,9 +522,9 @@ int lm_pose_verify_points(int device, const double* pts, int64_t n, const double
  *                     read, and `stream` waits on a second event once the conversion is done.
  *   lm_pose_transforms  T_out + 16k: the T of entry k of the pose run last finished (lm_complete_pose, lm_complete_detect
  *                     (its kept poses), the batch calls, lm_track), in entry order; NaN for an entry without a pose;
- *                     *n their number.  The pose NMS's outputs are unchanged: its kept poses are matched to their
- *                     survivors on the host, from one copy of the run's ICP outputs.  LM_E_STATE once another run has
- *                     started or when the last one failed; LM_E_CAPACITY (with *n) when cap is smaller. */
+ *                     *n their number.  The pose NMS records each kept pose's survivor on the device; the T of
+ *                     that survivor's ICP output is copied here, only when asked.  LM_E_STATE once another run has started or when the last one
+ *                     failed; LM_E_CAPACITY (with *n) when cap is smaller. */
 #define LM_TRACK_TRACKED 0
 #define LM_TRACK_OUTSIDE 1
 #define LM_TRACK_WINDOW 2
